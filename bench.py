@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Headline benchmark: cuda_allreduce_ring_chunked, float32, on N B200s of one node.
+"""Headline benchmark: cuda_allreduce_ring_chunked, float32, on N H100s of one node.
 
     python bench.py --gpus 1 --steps 20 --warmup 5
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
@@ -7,16 +7,19 @@
     ... bench.py --impl reference ...   # unmodified pytorch/gloo benchmark_cuda from baseline/_ref
 
 A *step* is one `CudaAllreduceRingChunked.run()` on a 1e8-element float32 buffer per
-GPU (400 MB, larger than the 126 MB L2, so back-to-back steps cannot hit in cache).
+GPU (400 MB, larger than the 50 MB L2, so back-to-back steps cannot hit in cache).
 Timing: CUDA events on the launching stream around exactly K steps, barrier +
 synchronize on both sides, max over ranks. `value` is the allreduce bus bandwidth
 (algbw * 2(N-1)/N, GB/s per GPU — the figure BASELINE.json asks for, against the
-900 GB/s/direction NVLink roofline). With N=1 a one-buffer allreduce is the
+450 GB/s/direction NVLink 4 roofline of an H100 SXM). With N=1 a one-buffer allreduce is the
 identity, so the N=1 run uses two local buffers per rank (`--inputs 2`, which the
 reference's benchmark supports too) and reports algorithm bandwidth instead.
 The JSON also carries a latency sweep (p50/p99, L2 flushed between iterations),
 an end-to-end number (pinned-host H2D of the input and D2H of the result every
 step) and the clocks seen while timing.
+
+--dump-outputs DIR writes the buffers the last timed step produced (a fixed sample of
+each, float32 .npy) so that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -43,6 +46,48 @@ METRIC = ("cuda_allreduce_ring_chunked float32 aggregate bus bandwidth (GB/s sum
 PUBLISHED_BUSBW_GBS = 2.8  # BASELINE.md: 20 MB allreduce_ring_chunked, 4 machines, 40 GbE (derived busbw)
 HEADLINE_ELEMENTS = 100_000_000
 SWEEP = [1, 10, 100, 1_000, 10_000, 100_000, 1_000_000, 10_000_000]
+NVLINK_GBS_PER_DIR = 450   # H100 SXM data sheet: NVLink 4, 18 links, 900 GB/s both directions together
+HBM_GBS = 3350             # H100 SXM data sheet: HBM3
+DUMP_BYTES = 32 << 20      # what --dump-outputs writes in all, over every rank and buffer
+
+
+def dump_growth_fits(elements, total, runs):
+    """The headline step is an in-place sum over `total` buffers and its inputs are filled once, so
+    after the first run every buffer holds S = the sum of the inputs and each further run multiplies
+    it by `total`. True when total**runs * max|S| stays below the float32 maximum."""
+    import math
+
+    import numpy as np
+
+    largest = (total * (total - 1) / 2) + (elements - 1) * total * total  # max of S, see fill_inputs
+    return math.log(largest) + runs * math.log(total) < math.log(float(np.finfo(np.float32).max))
+
+
+def dump_outputs(out_dir, tensors, rank, world):
+    """Writes each buffer the allreduce left on this rank as <out_dir>/allreduce_rank<r>_buf<i>.npy (float32).
+    With W warmup and K timed steps the values are total**(W + K) times the element-wise sum of the
+    inputs (total = GPUs x buffers per GPU; see dump_growth_fits). A buffer larger than its share of
+    DUMP_BYTES is reduced to a stratified sample: one element from each of `per` equal strides, at an
+    offset drawn from a generator seeded with the buffer's index, so every run with the same arguments
+    samples the same elements. Nothing is written when a sampled value is not finite."""
+    import numpy as np
+    import torch
+
+    per = DUMP_BYTES // 4 // (world * len(tensors))
+    arrays = []
+    for i, t in enumerate(tensors):
+        flat = t.reshape(-1)
+        n = flat.numel()
+        if n > per:
+            stride = n // per
+            idx = np.arange(per, dtype=np.int64) * stride + np.random.default_rng(i).integers(0, stride, per)
+            flat = flat[torch.from_numpy(idx).to(flat.device)]
+        arrays.append(flat.float().cpu().numpy())
+    if not all(np.isfinite(a).all() for a in arrays):
+        raise SystemExit(f"--dump-outputs: the buffers on rank {rank} hold non-finite values; nothing written")
+    os.makedirs(out_dir, exist_ok=True)
+    for i, a in enumerate(arrays):
+        np.save(os.path.join(out_dir, f"allreduce_rank{rank}_buf{i}.npy"), a)
 
 
 def env_int(name, dflt):
@@ -313,6 +358,9 @@ def run_ours(args):
 
     total = world * inputs
     tri_all = total * (total - 1) / 2
+    if args.dump_outputs and not dump_growth_fits(args.elements, total, args.warmup + args.steps):
+        raise SystemExit(f"--dump-outputs: with {total} buffers the summed values grow {total}x per step and "
+                         f"would overflow float32 within --warmup {args.warmup} + --steps {args.steps}; use fewer steps")
 
     def fill_inputs(ts):
         for i, t in enumerate(ts):
@@ -348,6 +396,8 @@ def run_ours(args):
     launches = cu.launch_count() - launches0
     total_ms = float(host_max([ev0.elapsed_time(ev1)])[0])
     ms_per_step = total_ms / args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, ts, rank, world)
     with torch.cuda.stream(stream):
         fill_inputs(ts)
         algo.run()
@@ -591,21 +641,19 @@ def run_ours(args):
         if world > 1 and resolved == "hybrid":  # per-mille `tile` of the vector goes peer to peer, the rest through the switch
             pm = (plan.get("tile") or 175) / 1000.0
             wire_factor = (1 - pm) * (1 + 1 / world) + pm * 2 * (world - 1) / world
-        roofline = {"nvlink_gbs_per_dir_nominal": 900,
-                    "nvlink_gbs_per_dir_measured_guide": 770,
+        roofline = {"nvlink_gbs_per_dir_nominal": NVLINK_GBS_PER_DIR,
                     "nvlink_gbs_per_dir_measured_here": link,
-                    "how": "measured_here = 256 MB one-directional put (our peerCopyKernel) to the next rank, device timed; "
-                           "guide = /opt/skills/guides/B200_PROFILING.md (driver-measured peer copy)"}
+                    "how": "nominal = H100 SXM data sheet; measured_here = 256 MB one-directional put (our peerCopyKernel) "
+                           "to the next rank, device timed"}
         if wire_factor:
             wire = size_bytes * wire_factor / (ms_per_step * 1e-3) / 1e9
             roofline.update({"variant": resolved, "wire_bytes_per_gpu_per_dir": int(size_bytes * wire_factor),
-                             "wire_gbs_per_dir": round(wire, 1), "frac_of_nominal": round(wire / 900, 3),
-                             "frac_of_measured_guide": round(wire / 770, 3),
+                             "wire_gbs_per_dir": round(wire, 1), "frac_of_nominal": round(wire / NVLINK_GBS_PER_DIR, 3),
                              "frac_of_measured_here": round(wire / link, 3) if link else None})
         else:
-            roofline.update({"variant": resolved, "hbm_gbs_measured": 6588.7,
+            roofline.update({"variant": resolved, "hbm_gbs_datasheet": HBM_GBS,
                              "hbm_bytes_per_step": size_bytes * inputs * 2,
-                             "frac_of_measured_hbm": round(size_bytes * inputs * 2 / (ms_per_step * 1e-3) / 1e9 / 6588.7, 3)})
+                             "frac_of_datasheet_hbm": round(size_bytes * inputs * 2 / (ms_per_step * 1e-3) / 1e9 / HBM_GBS, 3)})
         out = {
             "metric": METRIC,
             "value": round(value, 3), "unit": "GB/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
@@ -620,7 +668,7 @@ def run_ours(args):
                        "parallelism": f"allreduce x{world}", "cpu_affinity_cpus": len(cpus), "kernel_variant": resolved,
                        "launch_shape": plan, "tuning_table": cu.tuning_source(),
                        "buffers": "library symmetric allocator (peer-mapped; NVLS multicast-bound when >2 GPUs)",
-                       "l2": "inputs larger than L2 (400 MB > 126 MB) for the headline; 256 MB flush between sweep iterations",
+                       "l2": "inputs larger than L2 (400 MB > 50 MB) for the headline; 256 MB flush between sweep iterations",
                        "timing": "CUDA events on the launching stream, max over ranks",
                        "verification": "whole buffer on every rank, device-side closed form, before and after the timed loop"},
             "algbw_gbs": round(algbw, 3), "busbw_gbs": round(busbw, 3) if busbw else None,
@@ -815,7 +863,14 @@ def main():
     ap.add_argument("--quick", action="store_true", help="headline + e2e + latency sweep only (skip BASELINE configs 3-5)")
     ap.add_argument("--no-verify-matrix", action="store_true", help="skip the multi-GPU correctness matrix before timing")
     ap.add_argument("--e2e-chunks", type=int, default=16, help="pieces of the host<->device pipeline in the e2e run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="--impl ours only: write the buffers of the last timed step (float32 .npy, a fixed sample "
+                         "of at most 32 MB in all)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs covers --impl ours only")
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""In-tree native build for gloo_b200 (C++17 + CUDA sm_100a).
+"""In-tree native build for gloo_b200 (C++17 + CUDA sm_90a).
 
 Generates build/build.ninja and runs ninja. Produces:
   gloo_b200/_C.<abi>.so          python extension: whole library + pybind11 bindings
@@ -7,7 +7,7 @@ Generates build/build.ninja and runs ninja. Produces:
   gloo_b200/bin/glb_benchmark    C++ benchmark CLI (host + CUDA collectives)
   gloo_b200/bin/glb_selftest     C++ self-test binary (threads-as-ranks)
 
-Everything CUDA is compiled with  -gencode arch=compute_100a,code=sm_100a -lineinfo.
+Everything CUDA is compiled with  -gencode arch=compute_90a,code=sm_90a -lineinfo.
 cudart is linked statically and the driver API / NCCL are resolved at run time
 (cudaGetDriverEntryPoint / dlopen), so the extension imports on a CPU-only box.
 
@@ -38,7 +38,7 @@ NVCC = os.path.join(CUDA_HOME, "bin", "nvcc")
 # system compiler unless GLB_CXX overrides it.
 CXX = os.environ.get("GLB_CXX") or ("/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++")
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def ext_suffix() -> str:

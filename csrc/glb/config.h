@@ -27,4 +27,4 @@
 #define GLB_HAVE_TRANSPORT_NVLINK GLB_USE_CUDA  // cuda::PeerContext peer-memory data plane
 
 // The only GPU architecture this library is written for.
-#define GLB_CUDA_ARCH "sm_100a"
+#define GLB_CUDA_ARCH "sm_90a"

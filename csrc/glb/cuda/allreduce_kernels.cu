@@ -1,4 +1,4 @@
-// Fused allreduce kernels over NVLink peer memory (sm_100a).
+// Fused allreduce kernels over NVLink peer memory (sm_90a).
 //
 //   barrierKernel        flag barrier only.
 //   llAllreduce          smallest messages. Flag-in-data ("LL") protocol: every rank stores
@@ -627,9 +627,8 @@ nvlsAllreduceKernel(CommArgs a, char* mcBase, PeerPtrs bufs, size_t count, float
 }
 
 // ---- NVLS + peer-to-peer hybrid ---------------------------------------------------------------
-// Measured on 8 x B200: the in-switch reduction saturates at ~0.75 of the link rate and gets
-// SLOWER with more CTAs in flight (tune_P8: 32 CTAs x unroll 2 beats 296 x 8 by 9-30 %), i.e.
-// the bound is the switch's reduction path, not NVLink. The links therefore have headroom that
+// When the in-switch reduction saturates below the link rate (more CTAs in flight do not help),
+// the bound is the switch's reduction path, not NVLink. The links then have headroom that
 // a plain peer-to-peer two-shot can use at the same time: the vector is cut in two, CTAs
 // [0, nvlsBlocks) run the multimem path on the first part, the remaining CTAs run the two-shot
 // exchange on the second part, under the same two barriers.

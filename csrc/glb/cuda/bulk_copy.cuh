@@ -1,7 +1,7 @@
 // TMA bulk copies (cp.async.bulk, SASS: UBLKCP) for the pure data-movement kernels.
 //
 // A copy kernel built from LDG/STG needs hundreds of resident threads per SM just to keep
-// enough 16-byte accesses in flight over a ~2 us NVLink round trip. The Blackwell copy
+// enough 16-byte accesses in flight over a ~2 us NVLink round trip. The Hopper copy
 // engine inside each SM (TMA) moves whole chunks asynchronously instead: ONE thread per CTA
 // issues  global -> shared  (completion signalled on an mbarrier) and  shared -> global
 // (bulk async-groups); the data never touches registers and the SM's warps stay free.

@@ -1,4 +1,4 @@
-// Data-movement collectives over NVLink peer memory (sm_100a): broadcast,
+// Data-movement collectives over NVLink peer memory (sm_90a): broadcast,
 // allgather(v), alltoall(v), reduce_scatter, reduce, gather(v), scatter. All are
 // single kernels bracketed by device-side flag barriers; payload moves with
 // 128-bit peer loads/stores (or multimem.st through the NVSwitch where a multicast
@@ -154,8 +154,7 @@ __device__ __forceinline__ void gridCopy(char* dst, const char* src, size_t byte
 //         forwards its slice to the other P-2 ranks while the root is already sending the
 //         next chunk. Root egress = S, every other GPU's ingress = S and egress
 //         S(P-2)/(P-1): all links run at once, nothing is sent twice over the same port
-//         (measured on 8 x B200: a single multimem.st source tops out at ~390 GB/s, NCCL's
-//         ring broadcast at ~650).
+//         (a single multimem.st source is bound by the root's one egress stream).
 __global__ void __launch_bounds__(kThreads, 2)
 broadcastKernel(CommArgs a, PeerPtrs bufs, char* mc, size_t bytes, int root, int mode, bool vec, int tile) {
   const uint32_t e = loadEpoch(a);

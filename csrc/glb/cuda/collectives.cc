@@ -304,7 +304,7 @@ void allreduce(PeerContext& pc, const PeerBuffer& buf, size_t byteOffset, size_t
       GLB_ENFORCE(hasMc && nvlsSupports(dt, op) && hybridKernelFor(dt, pc.size) != nullptr && ep.extra.n == 0,
                   "hybrid allreduce: sum of f32/f16/bf16 on a multicast-bound buffer, 4 or 8 ranks, one pointer");
       // cfg.blocks = all CTAs, cfg.unroll = CTAs of the NVLS part, tile = per-mille of the vector done peer to peer
-      int blocks = plan.cfg.blocks > 0 ? plan.cfg.blocks : 148;
+      int blocks = plan.cfg.blocks > 0 ? plan.cfg.blocks : 132;
       blocks = std::max(2, std::min(blocks, pc.coResidentBlocks(hybridKernelFor(dt, pc.size))));
       const int nvlsBlocks = std::max(1, std::min(plan.cfg.unroll > 0 ? plan.cfg.unroll : 32, blocks - 1));
       const int permille = std::max(0, std::min((ep.tile > 0 ? ep.tile : plan.tile > 0 ? plan.tile : 175), 900));
@@ -624,7 +624,7 @@ void allgatherv(PeerContext& pc, const void* in, const PeerBuffer& out, size_t o
   }
   // No multicast here: an allgather's bottleneck is what every GPU RECEIVES ((P-1)/P of the
   // output either way); multimem.st would only relieve the uplink and additionally deliver
-  // each block back to its sender (measured at P=2: 312 GB/s with, 540 GB/s without).
+  // each block back to its sender.
   gatherCommon(pc, in, out.ptrsAt(outOffset), nullptr, out.vectorOk && outOffset % 16 == 0, bytesPerRank, -1, stream);
 }
 

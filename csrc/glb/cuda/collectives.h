@@ -43,19 +43,19 @@ const char* allreduceAlgoName(AllreduceAlgo a);
 AllreduceAlgo allreduceAlgoFromName(const std::string& name);
 
 // Process-wide knobs (initialised from GLB_CUDA_* env vars). Per-size decisions come from
-// the measured tuning table (tuning.h); these are the fallbacks and global caps.
+// the tuning table (tuning.h); these are the fallbacks and global caps.
 struct Tuning {
   size_t llMaxBytes = 16 * 1024;        // flag-in-data one-shot while bytes <= this
   size_t oneShotMaxBytes = 256 * 1024;  // barrier one-shot while bytes <= this / P; above: two-shot / NVLS
   size_t nvlsMinBytes = 32 * 1024;      // >= : NVLS when the buffer has a multicast alias (and P > 2)
   int maxBlocks = 128;                  // CTAs for the bandwidth kernels (clamped to the co-residency cap)
   int oneShotBlocks = 8;
-  bool nvlsReduceScatter = false;       // multimem.ld_reduce in reduce_scatter / reduce: measured slower than the
-                                        // P2P pull at P=4 (403 vs 343 us @256 MB) and equal at P=8, so off by default
-  int copyBlocks = 296;                 // CTAs for the store-only kernels (40 regs: 2-3 CTAs per SM)
+  bool nvlsReduceScatter = false;       // multimem.ld_reduce in reduce_scatter / reduce instead of the P2P pull
+                                        // (GLB_CUDA_NVLS_REDUCE_SCATTER); off by default
+  int copyBlocks = 264;                 // CTAs for the store-only kernels (40 regs: 2-3 CTAs per SM; 2 x 132 SMs)
   int alltoallvBlocks = 64;             // fixed grid of the v-variant (sizes are rank-local, the grid must not be)
   size_t bcastDirectMaxBytes = 256 * 1024;  // <= : root pushes everything itself
-  size_t bcastRelayMinBytes = 64u << 20;    // >= : chunk-pipelined relay broadcast (P > 2; measured cross-over 32-256 MB)
+  size_t bcastRelayMinBytes = 64u << 20;    // >= : chunk-pipelined relay broadcast (P > 2)
   int pipeTile = 1024;                  // 16-byte groups per tile of the pipelined kernel (power of two)
   int pipeExchangeThreads = 256;        // threads of each CTA that drive NVLink in the pipelined kernel
   bool tmaCopies = false;               // put / get / large allgather through cp.async.bulk (TMA) instead of LDG/STG

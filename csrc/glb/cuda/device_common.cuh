@@ -1,4 +1,4 @@
-// Device-side building blocks shared by every collective kernel (sm_100a):
+// Device-side building blocks shared by every collective kernel (sm_90a):
 //
 //  * CommArgs / SignalPad — per-rank signal page mapped into every peer. A kernel
 //    synchronises with its peers by storing a monotonically increasing epoch into

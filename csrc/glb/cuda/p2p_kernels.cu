@@ -1,4 +1,4 @@
-// Point-to-point transfers between two GPUs over NVLink peer memory (sm_100a).
+// Point-to-point transfers between two GPUs over NVLink peer memory (sm_90a).
 //
 // The reference moves GPU buffers between two ranks only through a transport::Pair
 // (ibverbs + GPUDirect: transport/ibverbs/pair.cc:328-384, buffer.cc:24-59) — there is no
@@ -119,7 +119,7 @@ p2pKernel(CommArgs a, const char* sendPtr, size_t sendBytes, int dst, char* recv
 
 // ---- zero-copy neighbour exchange ----------------------------------------------------------------
 // sendrecv() above costs two passes (sender -> mailbox, mailbox -> user buffer) and a flag
-// round trip per 32 KB stripe: 73-100 GB/s measured on B200 against a ~690 GB/s link. When
+// round trip per 32 KB stripe, far below what the link carries. When
 // the RECEIVE buffer is peer-mapped (a registered / symmetric buffer that every rank uses at
 // the same offset - the double-buffered K/V block of ring attention, a pipeline stage's
 // activation slot) the sender can write straight into it. What is left of the protocol is

@@ -1,4 +1,4 @@
-// Pipelined allreduce for ARBITRARY device pointers (sm_100a).
+// Pipelined allreduce for ARBITRARY device pointers (sm_90a).
 //
 // The reference API takes plain `T*` (cuda_allreduce_ring_chunked.h:30-36); a pointer that
 // is neither registered nor symmetric cannot be read by the peers (and cannot be bound to an

@@ -161,8 +161,10 @@ __global__ void spinKernel(long long cycles) {
   }
 }
 
-// Measured on B200, 2 x 400 MB fp32 (scripts/bench_local.py, profiles/r2/local_shapes.json):
-// 4 CTAs/SM x 1 pack 0.269 ms (5.96 TB/s), x 2 packs 0.279, 8 CTAs/SM 0.295, 2 CTAs/SM 0.353.
+// Measured on an H100 80GB HBM3 (SXM, power limit 700 W), 2 x 400 MB fp32 (scripts/bench_local.py,
+// p50 of 20): 4 CTAs/SM x 1 pack 0.578 ms (2.77 TB/s), x 2 packs 0.579, 6 CTAs/SM 0.588,
+// 8 CTAs/SM 0.601, 2 CTAs/SM 0.681; the tiled variant is within 0.5 % of the grid-stride one.
+// bench.py's N=1 step on the same card and in the same session: 0.578-0.584 ms.
 struct LocalShape {
   int ctasPerSm = 4;
   int unroll = 1;
@@ -187,7 +189,7 @@ LocalShape& localShape() {
 }
 
 int gridFor(size_t items, int threads, int ctasPerSm = 4) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   size_t want = (items + threads - 1) / threads;
@@ -244,7 +246,7 @@ void launchLocalAllreduceMany(void* const* bufs, int n, size_t count, DataType d
   }
   dispatchType(dt, [&](auto tag) {
     using T = decltype(tag);
-    // Launch shape: measured on B200 (scripts/bench_local.py); GLB_LOCAL_SHAPE = "<ctas per SM>,<unroll>,<tiled>".
+    // Launch shape: measured on H100 (scripts/bench_local.py); GLB_LOCAL_SHAPE = "<ctas per SM>,<unroll>,<tiled>".
     const LocalShape shape = localShape();
     const int grid = gridFor(count / PackTraits<T>::kElems / shape.unroll + 1, kLocalThreads, shape.ctasPerSm);
     const DevOp dop = static_cast<DevOp>(op);

@@ -166,8 +166,8 @@ void ensureTuningLoaded() {
     if (const char* f = std::getenv("GLB_TUNE_FILE")) candidates.push_back(f);
     const std::string dir = libraryDir();
     if (!dir.empty()) {
-      candidates.push_back(dir + "/tuning/b200.tune");     // next to _C.so (python package)
-      candidates.push_back(dir + "/../tuning/b200.tune");  // next to lib/libglb.so
+      candidates.push_back(dir + "/tuning/h100.tune");     // next to _C.so (python package)
+      candidates.push_back(dir + "/../tuning/h100.tune");  // next to lib/libglb.so
     }
     for (const auto& c : candidates) {
       std::string err;

@@ -6,7 +6,7 @@
 // time: `python -m gloo_b200.tune` (scripts/glb_tune.py) measures every variant and launch
 // shape on the box and writes a table; the library loads it at start-up
 // (GLB_TUNE_FILE, else <package>/tuning/<device>.tune) and `choose*` consult it. Without
-// a table the built-in defaults apply (derived from the committed B200 table).
+// a table the built-in defaults of collectives.h apply.
 //
 // File format, one entry per line ('#' starts a comment):
 //   <collective> P=<ranks> buf=<sym|reg|user> maxbytes=<N|inf> algo=<name> blocks=<n> [unroll=<n>] [tile=<n>]

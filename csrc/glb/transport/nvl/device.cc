@@ -344,7 +344,7 @@ class Dev : public Device {
   }
   std::string str() const override { return strcat_all("nvl(cuda:", cudaDevice_, " ", pci_, ") over ", control_->str()); }
   const std::string& getPCIBusID() const override { return pci_; }
-  int getInterfaceSpeed() const override { return 900 * 8 * 1000; }  // Mb/s: 900 GB/s per direction (NVLink 5)
+  int getInterfaceSpeed() const override { return 450 * 8 * 1000; }  // Mb/s: 450 GB/s per direction (H100 SXM, NVLink 4)
   bool hasGPUDirect() const override { return true; }
   std::shared_ptr<Context> createContext(int rank, int size) override {
     return std::make_shared<Ctx>(control_->createContext(rank, size), cudaDevice_);

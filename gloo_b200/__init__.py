@@ -1,8 +1,8 @@
-"""gloo_b200 — a Blackwell-native collective-communications library with the
+"""gloo_b200 — a Hopper-native (H100, sm_90a) collective-communications library with the
 capabilities and API surface of pytorch/gloo.
 
 Layers (see DESIGN.md):
-  _C                  native core (C++17 + CUDA sm_100a), built in-tree by build.py
+  _C                  native core (C++17 + CUDA sm_90a), built in-tree by build.py
   gloo_b200.ops       collectives API for numpy arrays / torch tensors (host + CUDA)
   gloo_b200.parallel  consumers: DDP gradient sync, ZeRO/FSDP shard ops, TP, MoE
                       dispatch/combine, Ulysses / ring sequence parallel helpers

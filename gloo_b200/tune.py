@@ -13,7 +13,7 @@ with every launch shape of a small grid (CTAs x unroll, tile for the pipelined k
 device-timed with CUDA events, max over ranks, median of the iterations, L2 flushed between
 iterations. The fastest candidate per size becomes a table entry; adjacent sizes with the
 same choice are merged. ``<out>.tune`` is the table (`GLB_TUNE_FILE`, or copy it to
-``gloo_b200/tuning/b200.tune``), ``<out>.json`` keeps every measurement, including the NCCL
+``gloo_b200/tuning/h100.tune``), ``<out>.json`` keeps every measurement, including the NCCL
 comparator at the same sizes, so the table can be audited: AUTO must never be more than a
 few percent off the best pinned variant.
 """
@@ -35,7 +35,7 @@ def geometric_sizes(lo: int, hi: int, per_octave: int = 1):
     return sorted(set(max(4, s) for s in out))
 
 
-def compress(results, P, dtype_name="float32", device_name="NVIDIA B200", cores=148):
+def compress(results, P, dtype_name="float32", device_name="NVIDIA H100 80GB HBM3", cores=132):
     """Measurements -> table lines (see the module docstring)."""
     # ---- compress into a table ---------------------------------------------------------------------------
     # Raw "fastest candidate per size" is noisy: shapes within a few percent of each other trade
@@ -216,9 +216,9 @@ def main(argv=None):
     sizes = geometric_sizes(args.min_bytes, args.max_bytes, 1)
     if args.quick:
         sizes = sizes[::2] + ([sizes[-1]] if (len(sizes) - 1) % 2 else [])
-    cores = 148
-    blocks_bw = [32, 64, 96, 128, 148] if not args.quick else [64, 128, 148]
-    blocks_light = [64, 148, 222, 296] if not args.quick else [148, 296]
+    cores = torch.cuda.get_device_properties(local).multi_processor_count
+    blocks_bw = [32, 64, 96, 128, cores] if not args.quick else [64, 128, cores]
+    blocks_light = [64, cores, cores * 3 // 2, cores * 2] if not args.quick else [cores, cores * 2]
     collectives = [c for c in args.collectives.split(",") if c]
     kinds = [k for k in args.kinds.split(",") if k]
     results = []   # every measurement
@@ -278,21 +278,21 @@ def main(argv=None):
                             cands.append(attempt("two_shot", lambda: cc.allreduce(t, algo="two_shot", stream=stream, blocks=b, unroll=u), nb,
                                                  blocks=b, unroll=u))
                 if kind == "sym" and cc.nvls_available() and nb >= 4096:
-                    nvls_blocks = [4, 8, 16, 24, 32, 48, 64, 96] if args.focus == "nvls" else blocks_bw + [222, 296]
+                    nvls_blocks = [4, 8, 16, 24, 32, 48, 64, 96] if args.focus == "nvls" else blocks_bw + [cores * 3 // 2, cores * 2]
                     for b in nvls_blocks:
                         for u in ((2, 4) if args.focus == "nvls" else (2, 4, 8)):
                             cands.append(attempt("nvls", lambda: cc.allreduce(t, algo="nvls", stream=stream, blocks=b, unroll=u), nb,
                                                  blocks=b, unroll=u))
                 if kind == "sym" and cc.nvls_available() and nb >= (1 << 20) and P in (2, 4, 8) and args.focus == "nvls":
                     # blocks = all CTAs, unroll = CTAs of the multicast part, tile = per-mille done peer to peer
-                    for b in (64, 96, 128, 148):
+                    for b in (64, 96, 128, cores):
                         for nb_mc in (8, 16, 24, 32):
                             for pm in (100, 175, 250, 350, 500):
                                 cands.append(attempt("hybrid", lambda: cc.allreduce(t, algo="hybrid", stream=stream, blocks=b,
                                                                                     unroll=nb_mc, tile=pm), nb,
                                                      blocks=b, unroll=nb_mc, tile=pm))
                 if kind == "user" and nb >= 32768 and args.focus != "nvls":
-                    for b in ([64, 128, 148] if not args.quick else [148]):
+                    for b in ([64, 128, cores] if not args.quick else [cores]):
                         for tile in (256, 1024, 4096):
                             for xw in (4, 8, 12):  # exchange warps of the 16 per CTA
                                 cands.append(attempt("pipelined", lambda: cc.allreduce(t, algo="pipelined", stream=stream, blocks=b,
@@ -359,19 +359,19 @@ def main(argv=None):
                         continue
                     if name == "nvls" and not cc.nvls_available():
                         continue
-                    for b in ([64, 148] if args.quick else [32, 64, 148]):
+                    for b in ([64, cores] if args.quick else [32, 64, cores]):
                         cu.tuning_clear()
                         cu.tuning_load_string(f"broadcast P={P} buf=reg maxbytes=inf algo={name} blocks={b}\n")
                         cu.set_tuning({"copy_blocks": 512, "max_blocks": b})
                         cands.append(attempt(name, call, total, blocks=b))
             if coll == "allgather" and per >= (256 << 10):
-                for b in (37, 74, 148):  # TMA variant: cp.async.bulk through shared memory, 1 CTA per SM
+                for b in (cores // 4, cores // 2, cores):  # TMA variant: cp.async.bulk through shared memory, 1 CTA per SM
                     cu.tuning_clear()
                     cu.tuning_load_string(f"allgather P={P} buf=reg maxbytes=inf algo=tma blocks={b}\n")
-                    cu.set_tuning({"copy_blocks": 512, "max_blocks": 148})
+                    cu.set_tuning({"copy_blocks": 512, "max_blocks": cores})
                     cands.append(attempt("tma", call, total, blocks=b))
             cu.tuning_clear()
-            cu.set_tuning({"ll_max_bytes": 16384, "copy_blocks": 296, "max_blocks": 128})
+            cu.set_tuning({"ll_max_bytes": 16384, "copy_blocks": cores * 2, "max_blocks": 128})
             best = record(coll, "reg", per if coll != "broadcast" else total, cands)
             if best:
                 bw = total / (best["us"] * 1e-6) / 1e9 * ((P - 1) / P if coll != "broadcast" else 1.0)

@@ -2,7 +2,7 @@
 """NVLink traffic of the hot allreduce kernels on the REAL multi-GPU path, from the driver's
 per-link byte counters (``nvidia-smi nvlink -gt d``): bytes that crossed the links per step,
 next to the algorithmic bytes of the variant (Nsight Compute cannot profile kernels of
-different ranks that wait for each other, see profiles/README.md). One rank per GPU
+different ranks that wait for each other). One rank per GPU
 (torchrun). Writes one JSON document.
 """
 import argparse

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Regenerate profiles/sass_*.txt and profiles/sass_summary.md from the built library
-(cuobjdump -sass, sm_100a). One listing per hot kernel + a table of the opcodes that prove what
+(cuobjdump -sass, sm_90a). One listing per hot kernel + a table of the opcodes that prove what
 the kernel does: 128-bit peer loads / stores, sys-scope flag traffic, multimem (LDGMC / STG..MC),
 TMA bulk copies (UBLKCP), mbarrier traffic (SYNCS)."""
 import os
@@ -72,7 +72,7 @@ def main():
         ops = [re.sub(r"^\s*/\*[0-9a-f]+\*/\s*", "", ln).split(";")[0] for ln in body if re.match(r"\s*/\*[0-9a-f]{4}\*/", ln)]
         ops = [re.sub(r"^@!?U?P\d+\s+", "", o).split()[0] for o in ops if o.strip()]
         with open(os.path.join(OUT, f"sass_{tag}.txt"), "w") as f:
-            f.write(f"// {dem[mangled.index(hit[0])]}\n// cuobjdump -sass gloo_b200/lib/libglb.so (sm_100a)\n")
+            f.write(f"// {dem[mangled.index(hit[0])]}\n// cuobjdump -sass gloo_b200/lib/libglb.so (sm_90a)\n")
             f.write("\n".join(body) + "\n")
 
         def count(rx):
@@ -81,7 +81,7 @@ def main():
         rows.append((tag, len(ops), count(r"^LDG\.E.*128"), count(r"^STG\.E.*128"), count(r"^LDG.*STRONG\.SYS"),
                      count(r"^STG.*STRONG\.SYS"), count(r"UBLKCP"), ", ".join(notable[:10])))
     with open(os.path.join(OUT, "sass_summary.md"), "w") as f:
-        f.write("# SASS evidence (`python scripts/sass_report.py`: cuobjdump -sass gloo_b200/lib/libglb.so, sm_100a)\n\n"
+        f.write("# SASS evidence (`python scripts/sass_report.py`: cuobjdump -sass gloo_b200/lib/libglb.so, sm_90a)\n\n"
                 "Peer traffic is plain `LDG.E.128` / `STG.E.128` on NVLink-mapped addresses in the same kernel as the\n"
                 "reduction; flag barriers and flag-in-data lines are `ST/LD.E.STRONG.SYS`; the NVLS kernels show the multimem\n"
                 "instructions (`LDGMC.E.ADD…`, stores to the multicast alias); the TMA copy kernels show `UBLKCP.S.G` /\n"

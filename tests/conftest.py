@@ -11,7 +11,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "multigpu: needs at least 2 CUDA devices")
     config.addinivalue_line("markers", "slow: long-running sweep")
 

@@ -578,8 +578,6 @@ def test_local_op_classes():
 
 # ---- consumers: gradients living in symmetric buckets (kept last in the file) ----------------------------------
 
-@pytest.mark.xfail(strict=False, reason="written after the round's GPU minutes were spent: construction, hooks and views ran on a B200, "
-                   "the deferred launch path has only been exercised on CPU tensors")
 @pytest.mark.parametrize("size", [2, 3])
 def test_gradient_bucketer_cuda(size):
     """GradientBucketer on CUDA: p.grad is a view into a symmetric bucket, buckets are averaged by the fused

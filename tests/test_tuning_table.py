@@ -41,7 +41,7 @@ def test_parse_lookup_and_dump():
 def test_packaged_table_parses():
     import os
 
-    path = os.path.join(os.path.dirname(gb.__file__), "tuning", "b200.tune")
+    path = os.path.join(os.path.dirname(gb.__file__), "tuning", "h100.tune")
     if not os.path.exists(path):
         return
     cu.tuning_clear()
@@ -56,7 +56,7 @@ def test_packaged_table_is_complete_and_sane():
     sorted and ends with maxbytes=inf, and the algorithm names are ones the selector knows."""
     import os
 
-    path = os.path.join(os.path.dirname(gb.__file__), "tuning", "b200.tune")
+    path = os.path.join(os.path.dirname(gb.__file__), "tuning", "h100.tune")
     lines = [ln.split("#")[0].strip() for ln in open(path)]
     lines = [ln for ln in lines if ln]
     cu.tuning_clear()
