@@ -446,6 +446,8 @@ GLB_INSTANTIATE(float)
 GLB_INSTANTIATE(double)
 GLB_INSTANTIATE(float16)
 GLB_INSTANTIATE(bfloat16)
+GLB_INSTANTIATE(float8_e4m3)
+GLB_INSTANTIATE(float8_e5m2)
 #undef GLB_INSTANTIATE
 
 }  // namespace glb

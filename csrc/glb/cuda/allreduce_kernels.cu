@@ -22,7 +22,8 @@
 //                        NVSwitch: multimem.ld_reduce pulls the switch-reduced
 //                        chunk, multimem.st broadcasts it; ~S(1+1/P) per direction.
 //   castAllreduce        two-shot / NVLS with an output dtype different from the input dtype
-//                        (fp32 accumulate -> bf16/fp16 store, or 16-bit in -> fp32 out).
+//                        (fp32 accumulate -> bf16/fp16/fp8 store, or 16-bit / fp8 in -> fp32
+//                        or bf16 out).
 //
 // Every variant applies the epilogue `scale` (AVG = 1/P, loss scaling, ...) to the fp32
 // accumulator before the single final rounding, and — when a rank passes several local
@@ -115,6 +116,14 @@ template <>
 struct AccType<__nv_bfloat16> {
   using type = float;
 };
+template <>
+struct AccType<__nv_fp8_e4m3> {
+  using type = float;
+};
+template <>
+struct AccType<__nv_fp8_e5m2> {
+  using type = float;
+};
 
 template <typename T>
 __device__ __forceinline__ typename AccType<T>::type toAcc(T x) {
@@ -128,6 +137,14 @@ template <>
 __device__ __forceinline__ float toAcc<__nv_bfloat16>(__nv_bfloat16 x) {
   return __bfloat162float(x);
 }
+template <>
+__device__ __forceinline__ float toAcc<__nv_fp8_e4m3>(__nv_fp8_e4m3 x) {
+  return fp8ToFloat(x);
+}
+template <>
+__device__ __forceinline__ float toAcc<__nv_fp8_e5m2>(__nv_fp8_e5m2 x) {
+  return fp8ToFloat(x);
+}
 template <typename TO, typename A>
 __device__ __forceinline__ TO fromAcc(A x) {
   return static_cast<TO>(x);
@@ -139,6 +156,14 @@ __device__ __forceinline__ __half fromAcc<__half, float>(float x) {
 template <>
 __device__ __forceinline__ __nv_bfloat16 fromAcc<__nv_bfloat16, float>(float x) {
   return __float2bfloat16_rn(x);
+}
+template <>
+__device__ __forceinline__ __nv_fp8_e4m3 fromAcc<__nv_fp8_e4m3, float>(float x) {
+  return floatToFp8<__nv_fp8_e4m3>(x);
+}
+template <>
+__device__ __forceinline__ __nv_fp8_e5m2 fromAcc<__nv_fp8_e5m2, float>(float x) {
+  return floatToFp8<__nv_fp8_e5m2>(x);
 }
 
 // `ll.p[r]` is the LL region of rank r's pool: [parity][source rank][line]. A launch uses
@@ -551,11 +576,13 @@ twoShotAllreduceKernel(CommArgs a, PeerPtrs bufs, size_t count, DevOp op, float 
     const size_t tailStart = nvec * PT::kElems;
     size_t tb, te;
     shareOf(count - tailStart, P, a.rank, tb, te);
+    using TA = TailAcc<T>;
     for (size_t i = tailStart + tb + tid; i < tailStart + te; i += nthreads) {
-      T acc = static_cast<const T*>(bufs.p[0])[i];
-      for (int r = 1; r < P; r++) acc = PT::combineOne(acc, static_cast<const T*>(bufs.p[r])[i], op);
-      if (scale != 1.0f) acc = PT::scaleOne(acc, scale);
-      for (int r = 0; r < P; r++) static_cast<T*>(bufs.p[r])[i] = acc;
+      typename TA::type acc = TA::load(static_cast<const T*>(bufs.p[0])[i]);
+      for (int r = 1; r < P; r++) acc = TA::combine(acc, TA::load(static_cast<const T*>(bufs.p[r])[i]), op);
+      if (scale != 1.0f) acc = TA::scale(acc, scale);
+      const T res = TA::store(acc);
+      for (int r = 0; r < P; r++) static_cast<T*>(bufs.p[r])[i] = res;
     }
   }
 
@@ -720,7 +747,7 @@ hybridAllreduceKernel(CommArgs a, char* mcBase, PeerPtrs bufs, size_t count, flo
 // ---- cast epilogue: out-of-place, output dtype != input dtype --------------------------------
 // Rank r reduces items [share r) of every rank's input (peer loads, or multimem.ld_reduce
 // when `mcIn` is set), scales, rounds ONCE to TO and stores into every rank's output.
-// An item is 8 elements: 32 B of float, 16 B of half / bf16.
+// An item is 8 elements: 32 B of float, 16 B of half / bf16, 8 B of fp8.
 template <typename TI, typename TO>
 __global__ void __launch_bounds__(kThreads)
 castAllreduceKernel(CommArgs a, PeerPtrs ins, char* mcIn, PeerPtrs outs, size_t count, DevOp op, float scale,
@@ -740,7 +767,8 @@ castAllreduceKernel(CommArgs a, PeerPtrs ins, char* mcIn, PeerPtrs outs, size_t 
   shareOf(nitems, P, a.rank, ib, ie);
   for (size_t it = ib + tid; it < ie; it += nthreads) {
     float acc[8];
-    if (mcIn != nullptr) {
+    // FP8 has no multimem form: its instantiations compile only the peer-load path, whatever mcIn is.
+    if (hasMultimem<TI>() && mcIn != nullptr) {
       if constexpr (std::is_same<TI, float>::value) {
         const Pack16 x = Multimem<float>::ldReduceAdd(mcIn + it * 32), y = Multimem<float>::ldReduceAdd(mcIn + it * 32 + 16);
 #pragma unroll
@@ -748,7 +776,7 @@ castAllreduceKernel(CommArgs a, PeerPtrs ins, char* mcIn, PeerPtrs outs, size_t 
           acc[k] = __uint_as_float(x.w[k]);
           acc[4 + k] = __uint_as_float(y.w[k]);
         }
-      } else {
+      } else if constexpr (hasMultimem<TI>()) {
         const auto w = PackTraits<TI>::widen(Multimem<TI>::ldReduceAdd(mcIn + it * 16));
 #pragma unroll
         for (int k = 0; k < 8; k++) acc[k] = w.v[k];
@@ -801,13 +829,25 @@ void dispatchType(DataType dt, F&& f) {
     case DataType::FLOAT64: f(double{}); break;
     case DataType::FLOAT16: f(__half{}); break;
     case DataType::BFLOAT16: f(__nv_bfloat16{}); break;
+    case DataType::FLOAT8_E4M3: f(__nv_fp8_e4m3{}); break;
+    case DataType::FLOAT8_E5M2: f(__nv_fp8_e5m2{}); break;
   }
 }
 
-template <typename T>
-constexpr bool isHotType() {
-  return std::is_same<T, float>::value || std::is_same<T, __half>::value || std::is_same<T, __nv_bfloat16>::value;
-}
+// (input, output) dtype pairs of the cast epilogue: X(input tag, input type, output tag, output type).
+#define GLB_CAST_PAIRS(X)                                      \
+  X(FLOAT32, float, FLOAT16, __half)                           \
+  X(FLOAT32, float, BFLOAT16, __nv_bfloat16)                   \
+  X(FLOAT16, __half, FLOAT32, float)                           \
+  X(BFLOAT16, __nv_bfloat16, FLOAT32, float)                   \
+  X(FLOAT8_E4M3, __nv_fp8_e4m3, FLOAT32, float)                \
+  X(FLOAT8_E5M2, __nv_fp8_e5m2, FLOAT32, float)                \
+  X(FLOAT8_E4M3, __nv_fp8_e4m3, BFLOAT16, __nv_bfloat16)       \
+  X(FLOAT8_E5M2, __nv_fp8_e5m2, BFLOAT16, __nv_bfloat16)       \
+  X(FLOAT32, float, FLOAT8_E4M3, __nv_fp8_e4m3)                \
+  X(FLOAT32, float, FLOAT8_E5M2, __nv_fp8_e5m2)                \
+  X(BFLOAT16, __nv_bfloat16, FLOAT8_E4M3, __nv_fp8_e4m3)       \
+  X(BFLOAT16, __nv_bfloat16, FLOAT8_E5M2, __nv_fp8_e5m2)
 
 template <typename K>
 const void* fn(K kernel) {
@@ -817,7 +857,16 @@ const void* fn(K kernel) {
 // The instantiation of the two-shot kernel for (T, P, unroll); unroll 0 = default for P.
 template <typename T>
 const void* twoShotFn(int P, int unroll) {
-  if constexpr (isHotType<T>()) {
+  if constexpr (PackTraits<T>::kElems > 8) {
+    // 16-lane (FP8) packs: one instantiation per P, the ones -Xptxas -v shows free of spills
+    // (their 16 fp32 lanes per pack leave no room for <4,2>, <4,4>, <8,1> or <2,8>).
+    switch (P) {
+      case 2: return unroll == 1 || unroll == 2 ? fn(twoShotAllreduceKernel<T, 2, 2>) : fn(twoShotAllreduceKernel<T, 2, 4>);
+      case 4: return fn(twoShotAllreduceKernel<T, 4, 1>);
+      case 8: return fn(twoShotAllreduceKernel<T, 8, 2>);
+      default: return fn(twoShotAllreduceKernel<T, 0, 1>);
+    }
+  } else if constexpr (isHotType<T>()) {
     switch (P) {
       case 2:
         if (unroll == 2) return fn(twoShotAllreduceKernel<T, 2, 2>);
@@ -863,7 +912,8 @@ void touch(const void* kernel) {
 void preloadAllreduceKernels() {
   touch(fn(barrierKernel));
   for (DataType dt : {DataType::INT8, DataType::UINT8, DataType::INT16, DataType::INT32, DataType::UINT32, DataType::INT64,
-                      DataType::UINT64, DataType::FLOAT32, DataType::FLOAT64, DataType::FLOAT16, DataType::BFLOAT16}) {
+                      DataType::UINT64, DataType::FLOAT32, DataType::FLOAT64, DataType::FLOAT16, DataType::BFLOAT16,
+                      DataType::FLOAT8_E4M3, DataType::FLOAT8_E5M2}) {
     dispatchType(dt, [&](auto tag) {
       using T = decltype(tag);
       touch(fn(llAllreduceKernel<T, T>));
@@ -875,6 +925,8 @@ void preloadAllreduceKernels() {
         for (int P : {2, 4, 8}) {
           for (int u : {1, 2, 4, 8}) touch(twoShotFn<T>(P, u));
         }
+      }
+      if constexpr (hasMultimem<T>()) {
         for (int u : {2, 4, 8}) touch(nvlsFn<T>(u));
       }
     });
@@ -882,14 +934,11 @@ void preloadAllreduceKernels() {
   for (DataType dt : {DataType::FLOAT32, DataType::FLOAT16, DataType::BFLOAT16}) {
     for (int P : {2, 4, 8}) touch(hybridKernelFor(dt, P));
   }
-  touch(fn(llAllreduceKernel<float, __half>));
-  touch(fn(llAllreduceKernel<float, __nv_bfloat16>));
-  touch(fn(llAllreduceKernel<__half, float>));
-  touch(fn(llAllreduceKernel<__nv_bfloat16, float>));
-  touch(fn(castAllreduceKernel<float, __half>));
-  touch(fn(castAllreduceKernel<float, __nv_bfloat16>));
-  touch(fn(castAllreduceKernel<__half, float>));
-  touch(fn(castAllreduceKernel<__nv_bfloat16, float>));
+#define GLB_TOUCH_CAST(EI, TI, EO, TO)           \
+  touch(fn(llAllreduceKernel<TI, TO>)); \
+  touch(fn(castAllreduceKernel<TI, TO>));
+  GLB_CAST_PAIRS(GLB_TOUCH_CAST)
+#undef GLB_TOUCH_CAST
   cudaGetLastError();
 }
 
@@ -906,9 +955,11 @@ void launchBarrier(const CommArgs& a, cudaStream_t stream) {
 
 bool castSupported(DataType in, DataType out) {
   if (in == out) return true;
-  const bool in16 = in == DataType::FLOAT16 || in == DataType::BFLOAT16;
-  const bool out16 = out == DataType::FLOAT16 || out == DataType::BFLOAT16;
-  return (in == DataType::FLOAT32 && out16) || (in16 && out == DataType::FLOAT32);
+#define GLB_IS_CAST(EI, TI, EO, TO) \
+  if (in == DataType::EI && out == DataType::EO) return true;
+  GLB_CAST_PAIRS(GLB_IS_CAST)
+#undef GLB_IS_CAST
+  return false;
 }
 
 void launchLLAllreduce(const CommArgs& a, const void* in, void* out, size_t count, DataType dt, DataType outDt,
@@ -920,10 +971,13 @@ void launchLLAllreduce(const CommArgs& a, const void* in, void* out, size_t coun
                                                            count, dop, scale, ll, static_cast<char*>(ll.p[a.rank]), \
                                                            srcStride, parityStride, extra)
   if (dt != outDt) {
-    if (dt == DataType::FLOAT32 && outDt == DataType::FLOAT16) GLB_LL(float, __half);
-    else if (dt == DataType::FLOAT32 && outDt == DataType::BFLOAT16) GLB_LL(float, __nv_bfloat16);
-    else if (dt == DataType::FLOAT16 && outDt == DataType::FLOAT32) GLB_LL(__half, float);
-    else if (dt == DataType::BFLOAT16 && outDt == DataType::FLOAT32) GLB_LL(__nv_bfloat16, float);
+#define GLB_LL_CAST(EI, TI, EO, TO)                    \
+  if (dt == DataType::EI && outDt == DataType::EO) { \
+    GLB_LL(TI, TO);                                  \
+    return;                                          \
+  }
+    GLB_CAST_PAIRS(GLB_LL_CAST)
+#undef GLB_LL_CAST
     return;
   }
   dispatchType(dt, [&](auto tag) {
@@ -991,6 +1045,7 @@ void launchTwoShotAllreduce(const CommArgs& a, const PeerPtrs& bufs, size_t coun
   launch(twoShotKernelFor(dt, a.nranks, cfg.unroll), cfg.blocks, kThreads, args, stream);
 }
 
+// multimem.ld_reduce has no e4m3 / e5m2 form on sm_90a: FP8 never takes the NVLS paths.
 bool nvlsSupports(DataType dt, ReduceOp op) {
   return op == ReduceOp::SUM && (dt == DataType::FLOAT32 || dt == DataType::FLOAT16 || dt == DataType::BFLOAT16);
 }
@@ -1040,10 +1095,10 @@ void launchHybridAllreduce(const CommArgs& a, void* mcPtr, const PeerPtrs& bufs,
 }
 
 const void* castKernelFor(DataType in, DataType out) {
-  if (in == DataType::FLOAT32 && out == DataType::FLOAT16) return fn(castAllreduceKernel<float, __half>);
-  if (in == DataType::FLOAT32 && out == DataType::BFLOAT16) return fn(castAllreduceKernel<float, __nv_bfloat16>);
-  if (in == DataType::FLOAT16 && out == DataType::FLOAT32) return fn(castAllreduceKernel<__half, float>);
-  if (in == DataType::BFLOAT16 && out == DataType::FLOAT32) return fn(castAllreduceKernel<__nv_bfloat16, float>);
+#define GLB_CAST_FN(EI, TI, EO, TO) \
+  if (in == DataType::EI && out == DataType::EO) return fn(castAllreduceKernel<TI, TO>);
+  GLB_CAST_PAIRS(GLB_CAST_FN)
+#undef GLB_CAST_FN
   return nullptr;
 }
 

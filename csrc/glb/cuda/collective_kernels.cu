@@ -560,8 +560,7 @@ reducePullKernel(CommArgs a, PeerPtrs ins, char* mcIn, T* __restrict__ out, EArg
   const size_t nvec = v16 ? len / PT::kElems : 0;
   const size_t byteOff = off * sizeof(T);
   if (useMc && v16) {
-    if constexpr (std::is_same<T, float>::value || std::is_same<T, __half>::value ||
-                  std::is_same<T, __nv_bfloat16>::value) {
+    if constexpr (hasMultimem<T>()) {
       constexpr int U = 4;
       for (size_t v0 = tid; v0 < nvec; v0 += nthreads * U) {
         Pack16 r[U];
@@ -618,11 +617,12 @@ reducePullKernel(CommArgs a, PeerPtrs ins, char* mcIn, T* __restrict__ out, EArg
       }
     }
   }
+  using TA = TailAcc<T>;
   for (size_t i = nvec * PT::kElems + tid; i < len; i += nthreads) {
-    T acc = static_cast<const T*>(ins.p[0])[off + i];
-    for (int r = 1; r < P; r++) acc = PT::combineOne(acc, static_cast<const T*>(ins.p[r])[off + i], op);
-    if (scale != 1.0f) acc = PT::scaleOne(acc, scale);
-    out[i] = acc;
+    typename TA::type acc = TA::load(static_cast<const T*>(ins.p[0])[off + i]);
+    for (int r = 1; r < P; r++) acc = TA::combine(acc, TA::load(static_cast<const T*>(ins.p[r])[off + i]), op);
+    if (scale != 1.0f) acc = TA::scale(acc, scale);
+    out[i] = TA::store(acc);
   }
   blockBarrier(a, e + 2);
   retire(a, 2, 0);
@@ -632,9 +632,7 @@ namespace {
 template <typename T>
 void launchReducePullT(const CommArgs& a, const PeerPtrs& ins, char* mc, void* out, const EArgs& ea, DevOp dop,
                        float scale, bool vec, bool useMc, int blocks, cudaStream_t stream) {
-  constexpr bool hot = std::is_same<T, float>::value || std::is_same<T, __half>::value ||
-                       std::is_same<T, __nv_bfloat16>::value;
-  if constexpr (hot) {
+  if constexpr (isHotType<T>()) {
     switch (a.nranks) {
       case 2: reducePullKernel<T, 2, 4><<<blocks, kThreads, 0, stream>>>(a, ins, mc, static_cast<T*>(out), ea, dop, scale, vec, useMc); return;
       case 4: reducePullKernel<T, 4, 2><<<blocks, kThreads, 0, stream>>>(a, ins, mc, static_cast<T*>(out), ea, dop, scale, vec, useMc); return;
@@ -672,6 +670,8 @@ void launchReducePull(const CommArgs& a, const PeerPtrs& ins, void* mcIn, void* 
     GLB_CASE(FLOAT64, double)
     GLB_CASE(FLOAT16, __half)
     GLB_CASE(BFLOAT16, __nv_bfloat16)
+    GLB_CASE(FLOAT8_E4M3, __nv_fp8_e4m3)
+    GLB_CASE(FLOAT8_E5M2, __nv_fp8_e5m2)
   }
 #undef GLB_CASE
 }
@@ -760,9 +760,7 @@ const void* alltoallPushKernelPtr() { return reinterpret_cast<const void*>(allto
 const void* reducePullKernelPtr(DataType dt, int nranks) {
 #define GLB_RP(E, T)                                                                                   \
   case DataType::E: {                                                                                  \
-    constexpr bool hot = std::is_same<T, float>::value || std::is_same<T, __half>::value ||            \
-                         std::is_same<T, __nv_bfloat16>::value;                                        \
-    if constexpr (hot) {                                                                               \
+    if constexpr (isHotType<T>()) {                                                                    \
       if (nranks == 2) return reinterpret_cast<const void*>(reducePullKernel<T, 2, 4>);                \
       if (nranks == 4) return reinterpret_cast<const void*>(reducePullKernel<T, 4, 2>);                \
       if (nranks == 8) return reinterpret_cast<const void*>(reducePullKernel<T, 8, 2>);                \
@@ -781,6 +779,8 @@ const void* reducePullKernelPtr(DataType dt, int nranks) {
     GLB_RP(FLOAT64, double)
     GLB_RP(FLOAT16, __half)
     GLB_RP(BFLOAT16, __nv_bfloat16)
+    GLB_RP(FLOAT8_E4M3, __nv_fp8_e4m3)
+    GLB_RP(FLOAT8_E5M2, __nv_fp8_e5m2)
   }
 #undef GLB_RP
   return nullptr;
@@ -801,13 +801,14 @@ void preloadCollectiveKernels() {
 #define GLB_TOUCH_RP(T) touch(reinterpret_cast<const void*>(reducePullKernel<T, 0, 1>));
   GLB_TOUCH_RP(int8_t) GLB_TOUCH_RP(uint8_t) GLB_TOUCH_RP(int16_t) GLB_TOUCH_RP(int32_t) GLB_TOUCH_RP(uint32_t)
   GLB_TOUCH_RP(long long) GLB_TOUCH_RP(unsigned long long) GLB_TOUCH_RP(float) GLB_TOUCH_RP(double)
-  GLB_TOUCH_RP(__half) GLB_TOUCH_RP(__nv_bfloat16)
+  GLB_TOUCH_RP(__half) GLB_TOUCH_RP(__nv_bfloat16) GLB_TOUCH_RP(__nv_fp8_e4m3) GLB_TOUCH_RP(__nv_fp8_e5m2)
 #undef GLB_TOUCH_RP
 #define GLB_TOUCH_HOT(T)                                                   \
   touch(reinterpret_cast<const void*>(reducePullKernel<T, 2, 4>));         \
   touch(reinterpret_cast<const void*>(reducePullKernel<T, 4, 2>));         \
   touch(reinterpret_cast<const void*>(reducePullKernel<T, 8, 2>));
   GLB_TOUCH_HOT(float) GLB_TOUCH_HOT(__half) GLB_TOUCH_HOT(__nv_bfloat16)
+  GLB_TOUCH_HOT(__nv_fp8_e4m3) GLB_TOUCH_HOT(__nv_fp8_e5m2)
 #undef GLB_TOUCH_HOT
   cudaGetLastError();
 }

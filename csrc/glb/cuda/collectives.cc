@@ -108,7 +108,8 @@ void finish(PeerContext& pc, cudaStream_t stream, const char* what) {
 
 float scaleOf(const Epilogue& ep, DataType dt) {
   if (ep.scale == 1.0) return 1.0f;
-  GLB_ENFORCE(dt == DataType::FLOAT32 || dt == DataType::FLOAT64 || dt == DataType::FLOAT16 || dt == DataType::BFLOAT16,
+  GLB_ENFORCE(dt == DataType::FLOAT32 || dt == DataType::FLOAT64 || dt == DataType::FLOAT16 || dt == DataType::BFLOAT16 ||
+                  isFp8(dt),
               "a scale epilogue needs a floating-point buffer");
   return static_cast<float>(ep.scale);
 }
@@ -119,6 +120,15 @@ int clampBlocks(PeerContext& pc, const void* kernel, int wanted, size_t vecsPerR
   const size_t need = ceilDiv(std::max<size_t>(vecsPerRank, 1), static_cast<size_t>(kThreads) * std::max(unroll, 1));
   int b = static_cast<int>(std::min<size_t>(need, static_cast<size_t>(std::max(wanted, 1))));
   return std::max(1, std::min(b, pc.coResidentBlocks(kernel)));
+}
+
+// multimem.ld_reduce has no FP8 form on sm_90a: an explicit request for a multicast variant
+// on an FP8 buffer is an error rather than a silent change of algorithm.
+void rejectFp8Multicast(AllreduceAlgo algo, DataType dt) {
+  if (isFp8(dt) && (algo == AllreduceAlgo::NVLS || algo == AllreduceAlgo::HYBRID)) {
+    GLB_THROW_INVALID_OPERATION_EXCEPTION("allreduce: ", allreduceAlgoName(algo), " has no ", dataTypeName(dt),
+                                          " reduction (multimem.ld_reduce on sm_90a reduces f32 / f16 / bf16 only)");
+  }
 }
 
 int defaultUnroll(AllreduceAlgo a, int P) {
@@ -253,6 +263,7 @@ void allreduce(PeerContext& pc, const PeerBuffer& buf, size_t byteOffset, size_t
   GLB_ENFORCE_LE(byteOffset + bytes, buf.bytes, "allreduce range exceeds the registered buffer");
   GLB_ENFORCE(op != ReduceOp::CUSTOM, "custom reductions run on the host path only");
   GLB_ENFORCE(!ep.castOutput || ep.outDtype == dt, "in-place allreduce cannot change the dtype; use allreduceCast");
+  rejectFp8Multicast(algo, dt);
   const float scale = scaleOf(ep, dt);
   DeviceGuard g(pc.device);
   char* local = static_cast<char*>(buf.local) + byteOffset;
@@ -338,6 +349,7 @@ void allreduce(PeerContext& pc, const void* in, void* out, size_t count, DataTyp
   pc.checkHealth();
   if (count == 0) return;
   GLB_ENFORCE(op != ReduceOp::CUSTOM, "custom reductions run on the host path only");
+  rejectFp8Multicast(algo, dt);
   DeviceGuard g(pc.device);
   const size_t es = elementSize(dt);
   const size_t bytes = count * es;
@@ -397,7 +409,7 @@ void allreduceCast(PeerContext& pc, const PeerBuffer& in, size_t inOffset, const
                    size_t count, DataType dt, DataType outDt, ReduceOp op, cudaStream_t stream, const Epilogue& ep) {
   GLB_TRACE_RANGE("glb::cuda::allreduceCast");
   if (count == 0) return;
-  GLB_ENFORCE(dt != outDt && castSupported(dt, outDt), "allreduceCast: supported conversions are f32 <-> f16 / bf16");
+  GLB_ENFORCE(dt != outDt && castSupported(dt, outDt), "allreduceCast: supported conversions are f32 <-> f16 / bf16, fp8 -> f32 / bf16 and f32 / bf16 -> fp8");
   GLB_ENFORCE(op != ReduceOp::CUSTOM, "custom reductions run on the host path only");
   GLB_ENFORCE_LE(inOffset + count * elementSize(dt), in.bytes, "allreduceCast input range exceeds the buffer");
   GLB_ENFORCE_LE(outOffset + count * elementSize(outDt), out.bytes, "allreduceCast output range exceeds the buffer");

@@ -5,13 +5,14 @@
 //    the peers' pads (st.release.sys) and spinning on its own pad
 //    (ld.acquire.sys): this replaces the host-side stream.wait() + notification
 //    Buffers of the reference (cuda_allreduce_ring_chunked.cc:177-208).
-//  * 16-byte vector packs with fp32 accumulation for 16-bit types and a runtime
-//    reduction op (uniform branch; these kernels are link/HBM bound).
+//  * 16-byte vector packs with fp32 accumulation for 16-bit and 8-bit float types and a
+//    runtime reduction op (uniform branch; these kernels are link/HBM bound).
 //  * multimem.* wrappers for the NVLS (NVSwitch multicast) path.
 #pragma once
 
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 
 #include <cstdint>
@@ -354,6 +355,130 @@ struct PackTraits<__nv_bfloat16> {
   }
 };
 
+// FP8 (e4m3 / e5m2): 16 lanes per pack, fp32 accumulator. Widening is exact (fp8 -> f16x2 ->
+// f32x2); narrowing rounds to nearest even and saturates to +-max finite
+// (cvt.rn.satfinite.{e4m3,e5m2}x2.f32, the only fp32 -> fp8 conversion on sm_90a).
+template <typename T>
+struct Fp8Format;
+template <>
+struct Fp8Format<__nv_fp8_e4m3> {
+  static constexpr __nv_fp8_interpretation_t value = __NV_E4M3;
+};
+template <>
+struct Fp8Format<__nv_fp8_e5m2> {
+  static constexpr __nv_fp8_interpretation_t value = __NV_E5M2;
+};
+
+template <typename T>
+__device__ __forceinline__ float2 fp8x2ToFloat2(uint32_t x2) {
+  const __half2 h = __half2(__nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(x2), Fp8Format<T>::value));
+  return __half22float2(h);
+}
+template <typename T>
+__device__ __forceinline__ uint32_t float2ToFp8x2(float a, float b) {
+  return __nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, Fp8Format<T>::value);
+}
+template <typename T>
+__device__ __forceinline__ float fp8ToFloat(T x) {
+  return __half2float(__half(__nv_cvt_fp8_to_halfraw(x.__x, Fp8Format<T>::value)));
+}
+template <typename T>
+__device__ __forceinline__ T floatToFp8(float x) {
+  T r;
+  r.__x = __nv_cvt_float_to_fp8(x, __NV_SATFINITE, Fp8Format<T>::value);
+  return r;
+}
+
+template <typename T>
+struct Fp8PackTraits {
+  static constexpr int kElems = 16;
+  struct AccPack {
+    float v[16];
+  };
+  __device__ static AccPack widen(const Pack16& p) {
+    AccPack a;
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      const float2 lo = fp8x2ToFloat2<T>(p.w[i] & 0xffffu), hi = fp8x2ToFloat2<T>(p.w[i] >> 16);
+      a.v[4 * i] = lo.x;
+      a.v[4 * i + 1] = lo.y;
+      a.v[4 * i + 2] = hi.x;
+      a.v[4 * i + 3] = hi.y;
+    }
+    return a;
+  }
+  __device__ static void combine(AccPack& a, const Pack16& p, DevOp op) {
+    // two lanes at a time: widening the whole pack first keeps 16 more registers live
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+      const float2 f = fp8x2ToFloat2<T>((p.w[i / 2] >> (16 * (i % 2))) & 0xffffu);
+      a.v[2 * i] = applyOp<float>(a.v[2 * i], f.x, op);
+      a.v[2 * i + 1] = applyOp<float>(a.v[2 * i + 1], f.y, op);
+    }
+  }
+  __device__ static Pack16 narrow(const AccPack& a) {
+    Pack16 p;
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      p.w[i] = float2ToFp8x2<T>(a.v[4 * i], a.v[4 * i + 1]) | (float2ToFp8x2<T>(a.v[4 * i + 2], a.v[4 * i + 3]) << 16);
+    }
+    return p;
+  }
+  __device__ static T combineOne(T a, T b, DevOp op) {
+    return floatToFp8<T>(applyOp<float>(fp8ToFloat(a), fp8ToFloat(b), op));
+  }
+  __device__ static void scale(AccPack& a, float s) {
+#pragma unroll
+    for (int i = 0; i < 16; i++) a.v[i] *= s;
+  }
+  __device__ static T scaleOne(T a, float s) { return floatToFp8<T>(fp8ToFloat(a) * s); }
+};
+template <>
+struct PackTraits<__nv_fp8_e4m3> : Fp8PackTraits<__nv_fp8_e4m3> {};
+template <>
+struct PackTraits<__nv_fp8_e5m2> : Fp8PackTraits<__nv_fp8_e5m2> {};
+
+template <typename T>
+constexpr bool isFp8Type() {
+  return std::is_same<T, __nv_fp8_e4m3>::value || std::is_same<T, __nv_fp8_e5m2>::value;
+}
+
+// Scalar tails (elements after the last whole pack). FP8 accumulates them in fp32 and rounds
+// once, like its packs; every other type keeps its element-typed accumulator (16-bit tails
+// round after each combine, as they always have).
+template <typename T>
+struct TailAcc {
+  using type = T;
+  __device__ static T load(T x) { return x; }
+  __device__ static T store(T x) { return x; }
+  __device__ static T combine(T a, T b, DevOp op) { return PackTraits<T>::combineOne(a, b, op); }
+  __device__ static T scale(T a, float s) { return PackTraits<T>::scaleOne(a, s); }
+};
+template <typename T>
+struct Fp8TailAcc {
+  using type = float;
+  __device__ static float load(T x) { return fp8ToFloat(x); }
+  __device__ static T store(float x) { return floatToFp8<T>(x); }
+  __device__ static float combine(float a, float b, DevOp op) { return applyOp<float>(a, b, op); }
+  __device__ static float scale(float a, float s) { return a * s; }
+};
+template <>
+struct TailAcc<__nv_fp8_e4m3> : Fp8TailAcc<__nv_fp8_e4m3> {};
+template <>
+struct TailAcc<__nv_fp8_e5m2> : Fp8TailAcc<__nv_fp8_e5m2> {};
+// Element types that get the P-specialised (two-shot, pipelined, reduce-pull) instantiations.
+template <typename T>
+constexpr bool isHotType() {
+  return std::is_same<T, float>::value || std::is_same<T, __half>::value || std::is_same<T, __nv_bfloat16>::value ||
+         isFp8Type<T>();
+}
+// Element types multimem.ld_reduce can add on sm_90a (NVLS, hybrid, multicast pipelines).
+// It has no e4m3 / e5m2 form on this target, so FP8 never takes those paths.
+template <typename T>
+constexpr bool hasMultimem() {
+  return std::is_same<T, float>::value || std::is_same<T, __half>::value || std::is_same<T, __nv_bfloat16>::value;
+}
+
 // ---- mixed-precision items (cast epilogue) --------------------------------------------
 // Eight consecutive elements of T as fp32 lanes: 2 x 16 B for float, 1 x 16 B for the
 // 16-bit types. Used by the kernels whose output dtype differs from the input dtype
@@ -419,12 +544,42 @@ struct Item8<__nv_bfloat16> {
   __device__ static __nv_bfloat16 fromFloat(float x) { return __float2bfloat16_rn(x); }
 };
 
+// FP8: 8 elements are 8 bytes (one 64-bit access).
+template <typename T>
+struct Fp8Item8 {
+  static constexpr int kBytes = 8;
+  __device__ static void load(const void* p, float (&v)[8]) {
+    const uint2 x = *static_cast<const uint2*>(p);
+    const uint32_t w[2] = {x.x, x.y};
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+      const float2 lo = fp8x2ToFloat2<T>(w[i] & 0xffffu), hi = fp8x2ToFloat2<T>(w[i] >> 16);
+      v[4 * i] = lo.x;
+      v[4 * i + 1] = lo.y;
+      v[4 * i + 2] = hi.x;
+      v[4 * i + 3] = hi.y;
+    }
+  }
+  __device__ static void store(void* p, const float (&v)[8]) {
+    uint2 x;
+    x.x = float2ToFp8x2<T>(v[0], v[1]) | (float2ToFp8x2<T>(v[2], v[3]) << 16);
+    x.y = float2ToFp8x2<T>(v[4], v[5]) | (float2ToFp8x2<T>(v[6], v[7]) << 16);
+    *static_cast<uint2*>(p) = x;
+  }
+  __device__ static float toFloat(T x) { return fp8ToFloat(x); }
+  __device__ static T fromFloat(float x) { return floatToFp8<T>(x); }
+};
+template <>
+struct Item8<__nv_fp8_e4m3> : Fp8Item8<__nv_fp8_e4m3> {};
+template <>
+struct Item8<__nv_fp8_e5m2> : Fp8Item8<__nv_fp8_e5m2> {};
+
 // ---- NVLS (multimem) --------------------------------------------------------------
 // ld_reduce returns the reduction of the same address across every GPU bound to
 // the multicast object (performed inside the NVSwitch); st broadcasts to all.
 
 template <typename T>
-struct Multimem;  // only add for float / half / bf16; min/max for half/bf16
+struct Multimem;  // only add for float / half / bf16 (see hasMultimem)
 
 template <>
 struct Multimem<float> {
@@ -480,6 +635,8 @@ template <> struct DevType<DataType::FLOAT32> { using type = float; };
 template <> struct DevType<DataType::FLOAT64> { using type = double; };
 template <> struct DevType<DataType::FLOAT16> { using type = __half; };
 template <> struct DevType<DataType::BFLOAT16> { using type = __nv_bfloat16; };
+template <> struct DevType<DataType::FLOAT8_E4M3> { using type = __nv_fp8_e4m3; };
+template <> struct DevType<DataType::FLOAT8_E5M2> { using type = __nv_fp8_e5m2; };
 
 }  // namespace cuda
 }  // namespace glb

@@ -116,38 +116,71 @@ pipelinedAllreduceKernel(CommArgs a, const T* in, T* out, size_t count, DevOp op
           // Peer exchange inside the pool, like the two-shot kernel: kSlots x U independent
           // 128-bit loads in flight per thread (an NVLink round trip is ~2 us).
           constexpr int kSlots = NR > 0 ? NR : kMaxRanks;
-          constexpr int U = NR == 2 ? 8 : (NR == 4 ? 4 : (NR == 8 ? 2 : 1));
+          // 16-lane (FP8) packs widen to twice the fp32 registers of 8-lane ones: half the packs in
+          // flight keeps the exchange free of spills (-Xptxas -v).
+          constexpr int kWide = PT::kElems > 8 ? 2 : 1;
+          constexpr int U0 = NR == 2 ? 8 : (NR == 4 ? 4 : (NR == 8 ? 2 : 1));
+          constexpr int U = U0 / kWide > 0 ? U0 / kWide : 1;
           char* peer[kSlots];
 #pragma unroll
           for (int q = 0; q < kSlots; q++) {
             peer[q] = q < P ? static_cast<char*>(stage.p[(a.rank + q) % P]) + slot + w0 * 16 : nullptr;
           }
-          for (size_t o0 = xt; o0 < T_; o0 += static_cast<size_t>(xn) * U) {
-            Pack16 v[U][kSlots];
+          if constexpr (kWide > 1 && kSlots > 8) {
+            // Any P with 16-lane packs: the peers' packs come in two batches of 8 (same order).
+            for (size_t o = xt; o < T_; o += static_cast<size_t>(xn)) {
+              typename PT::AccPack acc;
 #pragma unroll
-            for (int u = 0; u < U; u++) {
-              const size_t o = o0 + static_cast<size_t>(u) * xn;
-              if (o < T_) {
+              for (int b0 = 0; b0 < kSlots; b0 += 8) {
+                Pack16 v[8];
 #pragma unroll
-                for (int q = 0; q < kSlots; q++) {
-                  if (q < P) v[u][q] = ld128_stream(peer[q] + o * 16);
+                for (int q = 0; q < 8; q++) {
+                  if (b0 + q < P) v[q] = ld128_stream(peer[b0 + q] + o * 16);
+                }
+#pragma unroll
+                for (int q = 0; q < 8; q++) {
+                  if (b0 + q == 0) {
+                    acc = PT::widen(v[q]);
+                  } else if (b0 + q < P) {
+                    PT::combine(acc, v[q], op);
+                  }
                 }
               }
+              if (scale != 1.0f) PT::scale(acc, scale);
+              const Pack16 res = PT::narrow(acc);
+#pragma unroll
+              for (int q = 0; q < kSlots; q++) {
+                if (q < P) st128_stream(peer[q] + o * 16, res);
+              }
             }
+          } else {
+            for (size_t o0 = xt; o0 < T_; o0 += static_cast<size_t>(xn) * U) {
+              Pack16 v[U][kSlots];
 #pragma unroll
-            for (int u = 0; u < U; u++) {
-              const size_t o = o0 + static_cast<size_t>(u) * xn;
-              if (o < T_) {
-                typename PT::AccPack acc = PT::widen(v[u][0]);
+              for (int u = 0; u < U; u++) {
+                const size_t o = o0 + static_cast<size_t>(u) * xn;
+                if (o < T_) {
 #pragma unroll
-                for (int q = 1; q < kSlots; q++) {
-                  if (q < P) PT::combine(acc, v[u][q], op);
+                  for (int q = 0; q < kSlots; q++) {
+                    if (q < P) v[u][q] = ld128_stream(peer[q] + o * 16);
+                  }
                 }
-                if (scale != 1.0f) PT::scale(acc, scale);
-                const Pack16 res = PT::narrow(acc);
+              }
 #pragma unroll
-                for (int q = 0; q < kSlots; q++) {
-                  if (q < P) st128_stream(peer[q] + o * 16, res);
+              for (int u = 0; u < U; u++) {
+                const size_t o = o0 + static_cast<size_t>(u) * xn;
+                if (o < T_) {
+                  typename PT::AccPack acc = PT::widen(v[u][0]);
+#pragma unroll
+                  for (int q = 1; q < kSlots; q++) {
+                    if (q < P) PT::combine(acc, v[u][q], op);
+                  }
+                  if (scale != 1.0f) PT::scale(acc, scale);
+                  const Pack16 res = PT::narrow(acc);
+#pragma unroll
+                  for (int q = 0; q < kSlots; q++) {
+                    if (q < P) st128_stream(peer[q] + o * 16, res);
+                  }
                 }
               }
             }
@@ -155,7 +188,8 @@ pipelinedAllreduceKernel(CommArgs a, const T* in, T* out, size_t count, DevOp op
         }
       }
     } else {
-      constexpr int CU = 4;  // independent 128-bit accesses in flight per copy thread
+      // independent 128-bit accesses in flight per copy thread (half for 16-lane packs, as above)
+      constexpr int CU = PT::kElems > 8 ? 2 : 4;
       const size_t PT_ = static_cast<size_t>(P) * T_;
       // ---- C(i-2): pool -> user output ----------------------------------------------------
       if (i >= 2) {
@@ -222,9 +256,10 @@ pipelinedAllreduceKernel(CommArgs a, const T* in, T* out, size_t count, DevOp op
 namespace {
 template <typename T>
 const void* pipeFn(bool mc, int nranks) {
-  constexpr bool hot = std::is_same<T, float>::value || std::is_same<T, __half>::value || std::is_same<T, __nv_bfloat16>::value;
-  if constexpr (hot) {
+  if constexpr (hasMultimem<T>()) {
     if (mc) return reinterpret_cast<const void*>(pipelinedAllreduceKernel<T, true, 0>);
+  }
+  if constexpr (isHotType<T>()) {
     if (nranks == 2) return reinterpret_cast<const void*>(pipelinedAllreduceKernel<T, false, 2>);
     if (nranks == 4) return reinterpret_cast<const void*>(pipelinedAllreduceKernel<T, false, 4>);
     if (nranks == 8) return reinterpret_cast<const void*>(pipelinedAllreduceKernel<T, false, 8>);
@@ -245,6 +280,8 @@ const void* pipeKernelForImpl(DataType dt, bool mc, int nranks) {
     case DataType::FLOAT64: return pipeFn<double>(false, nranks);
     case DataType::FLOAT16: return pipeFn<__half>(mc, nranks);
     case DataType::BFLOAT16: return pipeFn<__nv_bfloat16>(mc, nranks);
+    case DataType::FLOAT8_E4M3: return pipeFn<__nv_fp8_e4m3>(false, nranks);
+    case DataType::FLOAT8_E5M2: return pipeFn<__nv_fp8_e5m2>(false, nranks);
   }
   return nullptr;
 }
@@ -254,7 +291,8 @@ const void* pipelinedKernelFor(DataType dt, bool mc, int nranks) { return pipeKe
 
 void preloadPipelineKernels() {
   for (DataType dt : {DataType::INT8, DataType::UINT8, DataType::INT16, DataType::INT32, DataType::UINT32, DataType::INT64,
-                      DataType::UINT64, DataType::FLOAT32, DataType::FLOAT64, DataType::FLOAT16, DataType::BFLOAT16}) {
+                      DataType::UINT64, DataType::FLOAT32, DataType::FLOAT64, DataType::FLOAT16, DataType::BFLOAT16,
+                      DataType::FLOAT8_E4M3, DataType::FLOAT8_E5M2}) {
     for (bool mc : {false, true}) {
       for (int nr : {0, 2, 4, 8}) {
         cudaFuncAttributes attr;

@@ -52,10 +52,11 @@ localReduceManyKernel(T* __restrict__ dst, SrcPtrs srcs, int nsrc, size_t count,
     for (int s = 1; s < nsrc; s++) PT::combine(acc, ld128_stream(static_cast<const char*>(srcs.p[s]) + v * 16), op);
     st128(reinterpret_cast<char*>(dst) + v * 16, PT::narrow(acc));
   }
+  using TA = TailAcc<T>;
   for (size_t i = nvec * PT::kElems + tid; i < count; i += nthreads) {
-    T acc = static_cast<const T*>(srcs.p[0])[i];
-    for (int s = 1; s < nsrc; s++) acc = PT::combineOne(acc, static_cast<const T*>(srcs.p[s])[i], op);
-    dst[i] = acc;
+    typename TA::type acc = TA::load(static_cast<const T*>(srcs.p[0])[i]);
+    for (int s = 1; s < nsrc; s++) acc = TA::combine(acc, TA::load(static_cast<const T*>(srcs.p[s])[i]), op);
+    dst[i] = TA::store(acc);
   }
 }
 
@@ -63,12 +64,13 @@ localReduceManyKernel(T* __restrict__ dst, SrcPtrs srcs, int nsrc, size_t count,
 template <typename T>
 __device__ __forceinline__ void localAllreduceScalar(const DstPtrs& bufs, int n, size_t first, size_t count, DevOp op,
                                                      float scale, size_t tid, size_t nthreads) {
-  using PT = PackTraits<T>;
+  using TA = TailAcc<T>;
   for (size_t i = first + tid; i < count; i += nthreads) {
-    T acc = static_cast<const T*>(bufs.p[0])[i];
-    for (int s = 1; s < n; s++) acc = PT::combineOne(acc, static_cast<const T*>(bufs.p[s])[i], op);
-    if (scale != 1.0f) acc = PT::scaleOne(acc, scale);
-    for (int s = 0; s < n; s++) static_cast<T*>(bufs.p[s])[i] = acc;
+    typename TA::type acc = TA::load(static_cast<const T*>(bufs.p[0])[i]);
+    for (int s = 1; s < n; s++) acc = TA::combine(acc, TA::load(static_cast<const T*>(bufs.p[s])[i]), op);
+    if (scale != 1.0f) acc = TA::scale(acc, scale);
+    const T res = TA::store(acc);
+    for (int s = 0; s < n; s++) static_cast<T*>(bufs.p[s])[i] = res;
   }
 }
 
@@ -199,6 +201,8 @@ __global__ void verifyKernel(const T* buf, size_t count, double start, double st
       got = static_cast<double>(__half2float(buf[i]));
     } else if constexpr (std::is_same<T, __nv_bfloat16>::value) {
       got = static_cast<double>(__bfloat162float(buf[i]));
+    } else if constexpr (isFp8Type<T>()) {
+      got = static_cast<double>(fp8ToFloat(buf[i]));
     } else {
       got = static_cast<double>(buf[i]);
     }
@@ -236,6 +240,8 @@ __global__ void fillKernel(T* dst, size_t count, double start, double stride) {
       dst[i] = __float2half_rn(static_cast<float>(v));
     } else if constexpr (std::is_same<T, __nv_bfloat16>::value) {
       dst[i] = __float2bfloat16_rn(static_cast<float>(v));
+    } else if constexpr (isFp8Type<T>()) {
+      dst[i] = floatToFp8<T>(static_cast<float>(v));
     } else {
       dst[i] = static_cast<T>(v);
     }
@@ -317,6 +323,8 @@ void dispatchType(DataType dt, F&& f) {
     case DataType::FLOAT64: f(double{}); break;
     case DataType::FLOAT16: f(__half{}); break;
     case DataType::BFLOAT16: f(__nv_bfloat16{}); break;
+    case DataType::FLOAT8_E4M3: f(__nv_fp8_e4m3{}); break;
+    case DataType::FLOAT8_E5M2: f(__nv_fp8_e5m2{}); break;
   }
 }
 
@@ -446,7 +454,8 @@ void preloadLocalKernels() {
     cudaFuncGetAttributes(&attr, k);
   };
   for (DataType dt : {DataType::INT8, DataType::UINT8, DataType::INT16, DataType::INT32, DataType::UINT32, DataType::INT64,
-                      DataType::UINT64, DataType::FLOAT32, DataType::FLOAT64, DataType::FLOAT16, DataType::BFLOAT16}) {
+                      DataType::UINT64, DataType::FLOAT32, DataType::FLOAT64, DataType::FLOAT16, DataType::BFLOAT16,
+                      DataType::FLOAT8_E4M3, DataType::FLOAT8_E5M2}) {
     dispatchType(dt, [&](auto tag) {
       using T = decltype(tag);
       touch(reinterpret_cast<const void*>(localReduceManyKernel<T>));

@@ -144,6 +144,8 @@ void launchSchedule(const CommArgs& a, const PeerPtrs& bufs, const PeerPtrs& sta
     GLB_CASE(FLOAT64, double)
     GLB_CASE(FLOAT16, __half)
     GLB_CASE(BFLOAT16, __nv_bfloat16)
+    GLB_CASE(FLOAT8_E4M3, __nv_fp8_e4m3)
+    GLB_CASE(FLOAT8_E5M2, __nv_fp8_e5m2)
   }
 #undef GLB_CASE
 }
@@ -165,6 +167,8 @@ void preloadScheduleKernels() {
   touch(reinterpret_cast<const void*>(scheduleKernel<double>));
   touch(reinterpret_cast<const void*>(scheduleKernel<__half>));
   touch(reinterpret_cast<const void*>(scheduleKernel<__nv_bfloat16>));
+  touch(reinterpret_cast<const void*>(scheduleKernel<__nv_fp8_e4m3>));
+  touch(reinterpret_cast<const void*>(scheduleKernel<__nv_fp8_e5m2>));
   cudaGetLastError();
 }
 

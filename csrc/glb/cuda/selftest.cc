@@ -140,6 +140,32 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
       });
     }
 
+    // ---- two-shot on e4m3 (16 lanes per pack, fp32 accumulate, one saturating rounding) ------
+    if (P == 4) {
+      R.run("twoShotAllreduceKernel<e4m3,4>", [&]() -> std::string {
+        for (int r = 0; r < P; r++) launchFill(pp.p[r], n, DataType::FLOAT8_E4M3, r + 1, 0.0, stream);
+        LaunchCfg cfg;
+        cfg.blocks = std::min(pc.coResidentBlocks(twoShotKernelFor(DataType::FLOAT8_E4M3, P, 2)), 32);
+        cfg.unroll = 2;
+        launchTwoShotAllreduce(ca, pp, n, DataType::FLOAT8_E4M3, ReduceOp::SUM, 0.5f, true, LocalPtrs(), cfg, stream);
+        noteLaunch();
+        std::vector<uint8_t> h(n);
+        GLB_CUDA_CHECK(cudaMemcpyAsync(h.data(), pp.p[P - 1], n, cudaMemcpyDeviceToHost, stream));
+        GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+        const size_t nv8 = n / 16;
+        size_t b8, e8, t8b, t8e;
+        shareOfHost(nv8, P, 0, b8, e8);
+        shareOfHost(n - nv8 * 16, P, 0, t8b, t8e);
+        for (size_t i = 0; i < n; i++) {
+          const bool mine = (i / 16 >= b8 && i / 16 < e8 && i < nv8 * 16) || (i >= nv8 * 16 + t8b && i < nv8 * 16 + t8e);
+          const float want = mine ? 5.0f : static_cast<float>(P);  // 0.5 * (1 + 2 + 3 + 4), else rank P-1's input
+          const float got = float8_e4m3::toFloat(h[i]);
+          if (got != want) return strcat_all("element ", i, ": got ", got, " want ", want);
+        }
+        return "";
+      });
+    }
+
     // ---- reduce-scatter / reduce pull -----------------------------------------------------
     R.run(strcat_all("reducePullKernel<float,", P, ">"), [&]() -> std::string {
       fillAll();
@@ -322,6 +348,21 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
       GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
       for (size_t i = 0; i < m; i++) {
         if (bf16ToFloat(h[i]) != 3.0f) return strcat_all("element ", i, ": got ", bf16ToFloat(h[i]));
+      }
+      return "";
+    });
+    R.run("llAllreduceKernel<e4m3,e4m3>", [&]() -> std::string {
+      const size_t m = 1001;
+      DevBuf in(m), out(m);
+      launchFill(in.p, m, DataType::FLOAT8_E4M3, 1.5, 0.0, stream);
+      launchLLAllreduce(one, in.p, out.p, m, DataType::FLOAT8_E4M3, DataType::FLOAT8_E4M3, ReduceOp::SUM, 0.25f,
+                        pc.llPtrs(), pc.llSrcStride(), pc.llParityStride(), LocalPtrs(), 1, 256, stream);
+      noteLaunch();
+      std::vector<uint8_t> h(m);
+      GLB_CUDA_CHECK(cudaMemcpyAsync(h.data(), out.p, m, cudaMemcpyDeviceToHost, stream));
+      GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+      for (size_t i = 0; i < m; i++) {
+        if (float8_e4m3::toFloat(h[i]) != 0.375f) return strcat_all("element ", i, ": got ", float8_e4m3::toFloat(h[i]));
       }
       return "";
     });

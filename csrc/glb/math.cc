@@ -154,6 +154,8 @@ ReduceFn getReduceFn(DataType dtype, ReduceOp op) {
     case DataType::FLOAT64: return pick<double>(op);
     case DataType::FLOAT16: return pick<float16>(op);
     case DataType::BFLOAT16: return pick<bfloat16>(op);
+    case DataType::FLOAT8_E4M3: return pick<float8_e4m3>(op);
+    case DataType::FLOAT8_E5M2: return pick<float8_e5m2>(op);
   }
   GLB_THROW_INVALID_OPERATION_EXCEPTION("unknown dtype");
 }

@@ -5,7 +5,8 @@
 //
 // float16 / bfloat16 go through fp32; when the CPU has AVX2+F16C the 16-bit paths
 // run 8 lanes at a time (runtime-dispatched, so the binary still runs on CPUs
-// without them). Parity: gloo/math.h:15-95, math.cc:17-98.
+// without them). float8_e4m3 / float8_e5m2 use the generic scalar templates below: every
+// element is widened to fp32, combined, and rounded back (RNE, saturating). Parity: gloo/math.h:15-95, math.cc:17-98.
 #pragma once
 
 #include <cstddef>

@@ -152,6 +152,21 @@ PYBIND11_MODULE(_C, m) {
   m.def("float_to_half_bits", [](float f) { return float16::fromFloat(f); });
   m.def("half_bits_to_float", [](uint16_t b) { return float16::toFloat(b); });
   m.def("float_to_bfloat_bits", [](float f) { return bfloat16::fromFloat(f); });
+  // FP8 encode / decode of the host types (dtype: DataType.FLOAT8_E4M3 or FLOAT8_E5M2).
+  m.def("float_to_fp8_bits", [](float f, int dt) -> uint8_t {
+    switch (static_cast<DataType>(dt)) {
+      case DataType::FLOAT8_E4M3: return float8_e4m3::fromFloat(f);
+      case DataType::FLOAT8_E5M2: return float8_e5m2::fromFloat(f);
+      default: GLB_THROW_INVALID_OPERATION_EXCEPTION("float_to_fp8_bits: not an FP8 dtype: ", dt);
+    }
+  }, py::arg("f"), py::arg("dtype"));
+  m.def("fp8_bits_to_float", [](uint8_t b, int dt) -> float {
+    switch (static_cast<DataType>(dt)) {
+      case DataType::FLOAT8_E4M3: return float8_e4m3::toFloat(b);
+      case DataType::FLOAT8_E5M2: return float8_e5m2::toFloat(b);
+      default: GLB_THROW_INVALID_OPERATION_EXCEPTION("fp8_bits_to_float: not an FP8 dtype: ", dt);
+    }
+  }, py::arg("b"), py::arg("dtype"));
   m.def("factorize", &detail::factorize);
 
   // ---- stores -------------------------------------------------------------------

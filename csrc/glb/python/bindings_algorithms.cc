@@ -80,6 +80,8 @@ void registerOldStyle(py::module_& m) {
       GLB_CASE(FLOAT64, double)
       GLB_CASE(FLOAT16, float16)
       GLB_CASE(BFLOAT16, bfloat16)
+      GLB_CASE(FLOAT8_E4M3, float8_e4m3)
+      GLB_CASE(FLOAT8_E5M2, float8_e5m2)
 #undef GLB_CASE
       default: break;
     }

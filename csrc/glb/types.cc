@@ -19,11 +19,15 @@ Slot Slot::add(uint64_t i) const {
 
 std::ostream& operator<<(std::ostream& os, const float16& v) { return os << static_cast<float>(v); }
 std::ostream& operator<<(std::ostream& os, const bfloat16& v) { return os << static_cast<float>(v); }
+std::ostream& operator<<(std::ostream& os, const float8_e4m3& v) { return os << static_cast<float>(v); }
+std::ostream& operator<<(std::ostream& os, const float8_e5m2& v) { return os << static_cast<float>(v); }
 
 size_t elementSize(DataType t) {
   switch (t) {
     case DataType::INT8:
-    case DataType::UINT8: return 1;
+    case DataType::UINT8:
+    case DataType::FLOAT8_E4M3:
+    case DataType::FLOAT8_E5M2: return 1;
     case DataType::FLOAT16:
     case DataType::BFLOAT16:
     case DataType::INT16: return 2;
@@ -50,6 +54,8 @@ const char* dataTypeName(DataType t) {
     case DataType::FLOAT64: return "float64";
     case DataType::FLOAT16: return "float16";
     case DataType::BFLOAT16: return "bfloat16";
+    case DataType::FLOAT8_E4M3: return "float8_e4m3";
+    case DataType::FLOAT8_E5M2: return "float8_e5m2";
   }
   return "?";
 }

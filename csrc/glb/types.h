@@ -1,6 +1,6 @@
-// Fundamental value types: Slot (64-bit message tag algebra), float16 / bfloat16
-// (host-side storage types with software conversion), DataType / ReduceOp enums
-// shared by the host and CUDA paths.
+// Fundamental value types: Slot (64-bit message tag algebra), float16 / bfloat16 /
+// float8_e4m3 / float8_e5m2 (host-side storage types with software conversion),
+// DataType / ReduceOp enums shared by the host and CUDA paths.
 // Parity: gloo/types.h:40-335, types.cc:16-32.
 #pragma once
 
@@ -198,6 +198,84 @@ struct alignas(2) bfloat16 {
   GLB_HOST_DEVICE bfloat16& operator/=(const bfloat16& o) { return *this = bfloat16(float(*this) / float(o)); }
 };
 
+// ---- 8-bit float storage types ------------------------------------------------------
+// OCP FP8. E4M3 ("fn"): bias 7, no infinities, S.1111.111 is NaN, max finite 448.
+// E5M2: bias 15, IEEE-style infinities and NaNs, max finite 57344.
+// Decoding is exact. Encoding rounds to nearest even and SATURATES to +-max finite, which is
+// what the only fp32 -> fp8 conversion on sm_90a does (cvt.rn.satfinite); torch's CPU .to()
+// instead turns an overflow into NaN (e4m3fn) or inf (e5m2). NaN stays NaN.
+namespace detail {
+template <int kExpBits, int kManBits, uint8_t kMaxCode>
+struct Fp8Codec {
+  static constexpr int kBias = (1 << (kExpBits - 1)) - 1;
+
+  GLB_HOST_DEVICE static uint8_t encode(float f) {
+    const uint32_t u = f2u(f);
+    const uint32_t sign = (u >> 24) & 0x80u;
+    const uint32_t mag = u & 0x7fffffffu;
+    if (mag > 0x7f800000u) return static_cast<uint8_t>(sign | 0x7fu);  // NaN
+    // At most half the smallest subnormal 2^(1 - bias - man): rounds to (signed) zero.
+    if (mag <= (static_cast<uint32_t>(127 - kBias - kManBits) << 23)) return static_cast<uint8_t>(sign);
+    const int32_t exp = static_cast<int32_t>(mag >> 23) - 127;
+    const uint32_t man = (mag & 0x7fffffu) | 0x800000u;
+    uint32_t shift = 23 - kManBits;
+    uint32_t hexp = 0;
+    if (exp < 1 - kBias) {
+      shift += static_cast<uint32_t>(1 - kBias - exp);  // subnormal result
+    } else {
+      hexp = static_cast<uint32_t>(exp + kBias);
+    }
+    uint32_t q = man >> shift;
+    const uint32_t rem = man & ((1u << shift) - 1), mid = 1u << (shift - 1);
+    if (rem > mid || (rem == mid && (q & 1u))) q++;
+    // As in float16::fromFloat: the implicit bit of q folds into the exponent field.
+    uint32_t code = hexp == 0 ? q : ((hexp - 1) << kManBits) + q;
+    if (code > kMaxCode) code = kMaxCode;  // saturate (also the inf / NaN codes of the format)
+    return static_cast<uint8_t>(sign | code);
+  }
+
+  GLB_HOST_DEVICE static float decode(uint8_t b) {
+    const uint32_t sign = (static_cast<uint32_t>(b) & 0x80u) << 24;
+    const uint32_t exp = (b >> kManBits) & ((1u << kExpBits) - 1);
+    const uint32_t man = b & ((1u << kManBits) - 1);
+    if (kExpBits == 4 && exp == 15 && man == 7) return u2f(sign | 0x7fc00000u);
+    if (kExpBits == 5 && exp == 31) return u2f(sign | 0x7f800000u | (man != 0 ? 0x400000u : 0u));
+    if (exp == 0) {  // subnormal: man * 2^(1 - bias - man bits), exact in fp32
+      const float v = static_cast<float>(man) * u2f(static_cast<uint32_t>(127 + 1 - kBias - kManBits) << 23);
+      return u2f(sign | f2u(v));
+    }
+    return u2f(sign | ((exp - kBias + 127) << 23) | (man << (23 - kManBits)));
+  }
+};
+}  // namespace detail
+
+#define GLB_DEFINE_FP8(NAME, EXP, MAN, MAXCODE)                                                    \
+  struct alignas(1) NAME {                                                                         \
+    using Codec = detail::Fp8Codec<EXP, MAN, MAXCODE>;                                             \
+    uint8_t x = 0;                                                                                 \
+    NAME() = default;                                                                              \
+    GLB_HOST_DEVICE NAME(float f) : x(Codec::encode(f)) {}                                         \
+    GLB_HOST_DEVICE explicit NAME(double d) : x(Codec::encode(static_cast<float>(d))) {}           \
+    GLB_HOST_DEVICE NAME(int v) : x(Codec::encode(static_cast<float>(v))) {}                       \
+    GLB_HOST_DEVICE explicit NAME(long v) : x(Codec::encode(static_cast<float>(v))) {}             \
+    GLB_HOST_DEVICE explicit NAME(unsigned long v) : x(Codec::encode(static_cast<float>(v))) {}    \
+    GLB_HOST_DEVICE static NAME fromBits(uint8_t b) {                                              \
+      NAME h;                                                                                      \
+      h.x = b;                                                                                     \
+      return h;                                                                                    \
+    }                                                                                              \
+    GLB_HOST_DEVICE static uint8_t fromFloat(float f) { return Codec::encode(f); }                 \
+    GLB_HOST_DEVICE static float toFloat(uint8_t b) { return Codec::decode(b); }                   \
+    GLB_HOST_DEVICE operator float() const { return Codec::decode(x); }                            \
+    GLB_HOST_DEVICE NAME& operator+=(const NAME& o) { return *this = NAME(float(*this) + float(o)); } \
+    GLB_HOST_DEVICE NAME& operator-=(const NAME& o) { return *this = NAME(float(*this) - float(o)); } \
+    GLB_HOST_DEVICE NAME& operator*=(const NAME& o) { return *this = NAME(float(*this) * float(o)); } \
+    GLB_HOST_DEVICE NAME& operator/=(const NAME& o) { return *this = NAME(float(*this) / float(o)); } \
+  };
+GLB_DEFINE_FP8(float8_e4m3, 4, 3, 0x7e)  // 0x7e = 448
+GLB_DEFINE_FP8(float8_e5m2, 5, 2, 0x7b)  // 0x7b = 57344
+#undef GLB_DEFINE_FP8
+
 #define GLB_DEFINE_HALF_BINOPS(T)                                                                   \
   GLB_HOST_DEVICE inline T operator+(const T& a, const T& b) { return T(float(a) + float(b)); }     \
   GLB_HOST_DEVICE inline T operator-(const T& a, const T& b) { return T(float(a) - float(b)); }     \
@@ -211,10 +289,14 @@ struct alignas(2) bfloat16 {
   GLB_HOST_DEVICE inline bool operator!=(const T& a, const T& b) { return float(a) != float(b); }
 GLB_DEFINE_HALF_BINOPS(float16)
 GLB_DEFINE_HALF_BINOPS(bfloat16)
+GLB_DEFINE_HALF_BINOPS(float8_e4m3)
+GLB_DEFINE_HALF_BINOPS(float8_e5m2)
 #undef GLB_DEFINE_HALF_BINOPS
 
 std::ostream& operator<<(std::ostream& os, const float16& v);
 std::ostream& operator<<(std::ostream& os, const bfloat16& v);
+std::ostream& operator<<(std::ostream& os, const float8_e4m3& v);
+std::ostream& operator<<(std::ostream& os, const float8_e5m2& v);
 
 // ---- runtime type / op tags --------------------------------------------------
 enum class DataType : int {
@@ -229,9 +311,13 @@ enum class DataType : int {
   BFLOAT16 = 8,
   UINT32 = 9,
   INT16 = 10,
+  FLOAT8_E4M3 = 11,
+  FLOAT8_E5M2 = 12,
 };
 
 enum class ReduceOp : int { SUM = 1, PRODUCT = 2, MAX = 3, MIN = 4, CUSTOM = 1000 };
+
+inline bool isFp8(DataType t) { return t == DataType::FLOAT8_E4M3 || t == DataType::FLOAT8_E5M2; }
 
 size_t elementSize(DataType t);
 const char* dataTypeName(DataType t);
@@ -258,6 +344,8 @@ GLB_DTYPE(float, FLOAT32)
 GLB_DTYPE(double, FLOAT64)
 GLB_DTYPE(float16, FLOAT16)
 GLB_DTYPE(bfloat16, BFLOAT16)
+GLB_DTYPE(float8_e4m3, FLOAT8_E4M3)
+GLB_DTYPE(float8_e5m2, FLOAT8_E5M2)
 #undef GLB_DTYPE
 
 }  // namespace glb

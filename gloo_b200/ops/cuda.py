@@ -28,7 +28,8 @@ def _torch_dtype_to_glb(dtype) -> DataType:
     import torch
 
     return {torch.float32: DataType.FLOAT32, torch.float16: DataType.FLOAT16, torch.bfloat16: DataType.BFLOAT16,
-            torch.float64: DataType.FLOAT64}[dtype]
+            torch.float64: DataType.FLOAT64, torch.float8_e4m3fn: DataType.FLOAT8_E4M3,
+            torch.float8_e5m2: DataType.FLOAT8_E5M2}[dtype]
 
 
 def _stream(stream) -> int:
@@ -152,8 +153,10 @@ class CudaContext:
 
         ``scale`` / ``average`` (= 1/size) are applied to the fp32 accumulator inside the
         collective kernel, before the single rounding to the output dtype. ``out`` may have a
-        different dtype (float32 <-> float16 / bfloat16): registered tensors of any size, plain
-        tensors up to the LL limit. ``extra``: more local tensors of the same shape that are
+        different dtype (float32 <-> float16 / bfloat16, FP8 -> float32 / bfloat16 and
+        float32 / bfloat16 -> FP8): registered tensors of any size, plain tensors up to the LL
+        limit. FP8 results round to nearest even and saturate to the format's largest finite
+        value. ``extra``: more local tensors of the same shape that are
         folded into the reduction and overwritten with the result (multi-pointer semantics).
         ``blocks`` / ``unroll`` / ``tile`` pin the launch shape (tuner)."""
         ptr, n, dt, _ = describe(tensor)

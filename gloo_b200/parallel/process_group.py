@@ -182,6 +182,18 @@ def _is_avg(reduce_op) -> bool:
     return reduce_op == dist.ReduceOp.AVG
 
 
+_FP8 = (torch.float8_e4m3fn, torch.float8_e5m2)
+
+
+def _divide_(t, n: int):
+    """t /= n in place. torch has no division kernel for FP8 tensors, so those take a float32
+    round trip (one rounding, like the fused scale of the CUDA kernels)."""
+    if t.dtype in _FP8:
+        t.copy_(t.float().div_(n))
+    else:
+        t.div_(n)
+
+
 class GlbProcessGroup(dist.ProcessGroup):
     def __init__(self, store, rank: int, world_size: int, timeout: timedelta):
         super().__init__(rank, world_size)
@@ -241,11 +253,11 @@ class GlbProcessGroup(dist.ProcessGroup):
                 fused = _is_avg(opts.reduceOp) and w.is_floating_point()
                 self._cc(w).allreduce(w, op=op, average=fused)
                 if _is_avg(opts.reduceOp) and not fused:
-                    w.div_(self._world)
+                    _divide_(w, self._world)
             else:
                 H.allreduce(self.ctx, w, op=op)
                 if _is_avg(opts.reduceOp):
-                    w.div_(self._world)
+                    _divide_(w, self._world)
             if w is not t:
                 t.copy_(w)
         return _done(tensors)
@@ -296,11 +308,11 @@ class GlbProcessGroup(dist.ProcessGroup):
             fused = _is_avg(opts.reduceOp) and out.is_floating_point()
             self._cc(out).reduce_scatter(out.view(-1), inp.view(-1), op=op, scale=1.0 / self._world if fused else 1.0)
             if _is_avg(opts.reduceOp) and not fused:
-                out.div_(self._world)
+                _divide_(out, self._world)
         else:
             H.reduce_scatter(self.ctx, out.view(-1), inp.view(-1), op=op)
             if _is_avg(opts.reduceOp):
-                out.div_(self._world)
+                _divide_(out, self._world)
         if out is not output_tensor:
             output_tensor.copy_(out)
         return _done(output_tensor)
@@ -365,7 +377,7 @@ class GlbProcessGroup(dist.ProcessGroup):
             else:
                 H.reduce(self.ctx, w, root=opts.rootRank, op=op)
             if _is_avg(opts.reduceOp) and self._rank == opts.rootRank:
-                w.div_(self._world)
+                _divide_(w, self._world)
             if w is not t:
                 t.copy_(w)
         return _done(tensors)

@@ -19,6 +19,8 @@ class DataType(enum.IntEnum):
     BFLOAT16 = 8
     UINT32 = 9
     INT16 = 10
+    FLOAT8_E4M3 = 11
+    FLOAT8_E5M2 = 12
 
 
 class ReduceOp(enum.IntEnum):
@@ -51,7 +53,7 @@ _NP = {
 _SIZES = {
     DataType.INT8: 1, DataType.UINT8: 1, DataType.INT16: 2, DataType.FLOAT16: 2, DataType.BFLOAT16: 2,
     DataType.INT32: 4, DataType.UINT32: 4, DataType.FLOAT32: 4, DataType.INT64: 8, DataType.UINT64: 8,
-    DataType.FLOAT64: 8,
+    DataType.FLOAT64: 8, DataType.FLOAT8_E4M3: 1, DataType.FLOAT8_E5M2: 1,
 }
 
 
@@ -63,6 +65,8 @@ def _torch_map():
         torch.int32: DataType.INT32, torch.int64: DataType.INT64, torch.float32: DataType.FLOAT32,
         torch.float64: DataType.FLOAT64, torch.float16: DataType.FLOAT16, torch.bfloat16: DataType.BFLOAT16,
         torch.bool: DataType.UINT8,
+        # numpy has no FP8 dtype: these two formats are reachable through torch tensors only.
+        torch.float8_e4m3fn: DataType.FLOAT8_E4M3, torch.float8_e5m2: DataType.FLOAT8_E5M2,
     }
 
 
@@ -79,7 +83,10 @@ def describe(x: Any) -> Tuple[int, int, DataType, bool]:
     if is_torch(x):
         if not x.is_contiguous():
             raise ValueError("tensor must be contiguous")
-        return x.data_ptr(), x.numel(), _torch_map()[x.dtype], x.is_cuda
+        dt = _torch_map().get(x.dtype)
+        if dt is None:
+            raise TypeError(f"unsupported dtype {x.dtype}")
+        return x.data_ptr(), x.numel(), dt, x.is_cuda
     if isinstance(x, np.ndarray):
         if not x.flags["C_CONTIGUOUS"]:
             raise ValueError("array must be C-contiguous")

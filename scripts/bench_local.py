@@ -19,11 +19,16 @@ the rate is bytes moved / p50. Prints the card name, power limit and max SM cloc
 process, one JSON line per variant and round, and a summary with each variant's median over
 the rounds and the bulk step as a fraction of each ceiling. An argument writes the summary there.
 
+--dtype (float32, bfloat16 or float8_e4m3fn; default float32) picks the element type of the step.
+The buffers stay 2 x 400 MB whatever the dtype, so every rate compares directly with memcpy_d2d;
+read_only and write_only run on a float32 view of the same bytes.
+
 On an H100 80GB HBM3 (SXM, power limit 700 W, max SM clock 1980 MHz), medians of 3 rounds:
 fused_ldg_stg 0.570 ms (2.81 TB/s), fused_bulk 0.548 ms (2.92 TB/s), copy_ldg_stg 0.581 ms,
 copy_bulk 0.565 ms, memcpy_d2d 0.536 ms (2.98 TB/s), read_only 2.86 TB/s, write_only 3.22 TB/s.
 The bulk step runs at 0.98 of the device-to-device copy and 1.04 of the LDG/STG step.
 """
+import argparse
 import json
 import os
 import subprocess
@@ -36,8 +41,9 @@ import torch  # noqa: E402
 import gloo_b200 as gb  # noqa: E402
 
 cu = gb._C.cuda
-N = 100_000_000
-F32 = int(gb.DataType.FLOAT32)
+NBYTES = 400_000_000  # per buffer
+DTYPES = {"float32": (torch.float32, gb.DataType.FLOAT32), "bfloat16": (torch.bfloat16, gb.DataType.BFLOAT16),
+          "float8_e4m3fn": (torch.float8_e4m3fn, gb.DataType.FLOAT8_E4M3)}
 ROUNDS = 3
 TIMED = 20
 
@@ -53,17 +59,27 @@ def card():
 
 
 def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("summary", nargs="?", help="write the summary JSON here")
+    ap.add_argument("--dtype", choices=sorted(DTYPES), default="float32")
+    args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_local.py measures on a GPU"
-    a, b = torch.ones(N, device="cuda"), torch.ones(N, device="cuda")
-    c, d = torch.empty(N, device="cuda"), torch.empty(N, device="cuda")
+    dtype, glb_dt = DTYPES[args.dtype][0], int(DTYPES[args.dtype][1])
+    es = torch.empty((), dtype=dtype).element_size()
+    N = NBYTES // es
+    a, b = torch.ones(N, device="cuda", dtype=dtype), torch.ones(N, device="cuda", dtype=dtype)
+    c, d = torch.empty(N, device="cuda", dtype=dtype), torch.empty(N, device="cuda", dtype=dtype)
+    # float32 views of the same bytes for the read / write ceilings (torch reduces no FP8 tensor)
+    a32, b32 = a.view(torch.float32), b.view(torch.float32)
+    ones32 = torch.ones(4 // es, dtype=dtype).view(torch.float32).item()  # a float32 word of dtype ones
     stream = torch.cuda.current_stream().cuda_stream
-    nbytes = N * 4
+    nbytes = N * es
 
     def step(ptrs, pinned):
         # pinned: the LDG/STG kernel whatever the size; otherwise the library's own choice
         cu.set_local_shape(4, 1, False) if pinned else cu.set_local_shape(0, 0, False)
         for p in ptrs:
-            cu.local_allreduce_many(p, N, F32, 1, 0.5 if len(p) > 1 else 1.0, stream)
+            cu.local_allreduce_many(p, N, glb_dt, 1, 0.5 if len(p) > 1 else 1.0, stream)
 
     both, each = [[a.data_ptr(), b.data_ptr()]], [[a.data_ptr()], [b.data_ptr()]]
     variants = {
@@ -72,11 +88,11 @@ def main():
         "copy_ldg_stg": (lambda: step(each, True), 4 * nbytes),
         "copy_bulk": (lambda: step(each, False), 4 * nbytes),
         "memcpy_d2d": (lambda: (c.copy_(a), d.copy_(b)), 4 * nbytes),
-        "read_only": (lambda: (a.sum(), b.sum()), 2 * nbytes),
-        "write_only": (lambda: (a.fill_(1.0), b.fill_(1.0)), 2 * nbytes),
+        "read_only": (lambda: (a32.sum(), b32.sum()), 2 * nbytes),
+        "write_only": (lambda: (a32.fill_(ones32), b32.fill_(ones32)), 2 * nbytes),
     }
     info = card()
-    print(json.dumps({"card": info}), flush=True)
+    print(json.dumps({"card": info, "dtype": args.dtype}), flush=True)
     per = {k: [] for k in variants}
     try:
         for rnd in range(ROUNDS):
@@ -91,7 +107,7 @@ def main():
                 torch.cuda.synchronize()
                 ms = sorted(x.elapsed_time(y) for x, y in evs)[TIMED // 2]
                 # the inputs are all ones and the fused step scales by 0.5: every variant keeps them so
-                ok = all(float(t[i]) == 1.0 for t in (a, b) for i in (0, N // 3, N - 1))
+                ok = all(t[i].float().item() == 1.0 for t in (a, b) for i in (0, N // 3, N - 1))
                 assert ok, f"{name} changed the buffers"
                 per[name].append(ms)
                 print(json.dumps({"round": rnd, "variant": name, "ms": round(ms, 4),
@@ -100,13 +116,13 @@ def main():
         cu.set_local_shape(0, 0, False)
     med = {k: sorted(v)[len(v) // 2] for k, v in per.items()}
     rate = {k: variants[k][1] / (med[k] * 1e-3) / 1e9 for k in variants}
-    summary = {"card": info, "rounds": ROUNDS, "launches_per_round": TIMED,
+    summary = {"card": info, "dtype": args.dtype, "rounds": ROUNDS, "launches_per_round": TIMED,
                "ms": {k: round(v, 4) for k, v in med.items()},
                "gbs": {k: round(v, 1) for k, v in rate.items()},
                "fused_bulk_over": {k: round(rate["fused_bulk"] / rate[k], 3) for k in variants if k != "fused_bulk"}}
     print("summary:", json.dumps(summary), flush=True)
-    if len(sys.argv) > 1:
-        with open(sys.argv[1], "w") as f:
+    if args.summary:
+        with open(args.summary, "w") as f:
             json.dump(summary, f, indent=1)
 
 
