@@ -5,6 +5,8 @@
 //   ├── IoException                 transport failure; the context is poisoned and
 //   │   └── TimeoutException        must be re-created (same contract as the
 //   │                               reference, docs/errors.md:5-13)
+//   ├── InputException              bad data found on the device (a collective's
+//   │                               device-side counts); the context stays usable
 //   └── EnforceNotMet               failed GLB_ENFORCE (logging.h)
 //
 // Parity: gloo/common/error.h:21-48.
@@ -29,6 +31,10 @@ struct Exception : public std::runtime_error {
 
 struct InvalidOperationException : public Exception {
   explicit InvalidOperationException(const std::string& msg) : Exception(msg) {}
+};
+
+struct InputException : public Exception {
+  explicit InputException(const std::string& msg) : Exception(msg) {}
 };
 
 struct IoException : public Exception {

@@ -533,6 +533,367 @@ void launchAlltoallPush(const CommArgs& a, const void* in, const PeerPtrs& outs,
                                                       recvOffTable != nullptr, onlySrc, vec);
 }
 
+// ---- device-split all-to-all-v (expert-parallel dispatch / combine) ----------------------------
+// Splits are device arrays of row counts; nothing about them passes through the host. P ranks,
+// E local experts per rank, K = P·E chunks per rank. Count matrix M[s][k] = entry k of rank s's
+// in_splits, read after the first barrier from column s of the a2aCount table of my own pad.
+//   forward: k = j·E + e = rows of rank s for expert e of rank j; input packed in k order; on
+//            rank j expert e's segment starts at a multiple of `align` rows and holds the rows of
+//            sources 0..P-1 one after the other.
+//   inverse: k = e·P + s = rows of my expert e that go back to rank s, read at in_offsets[k]; on
+//            rank s they land packed in (holder j, e) order: where s's forward input rows were.
+// A destination whose rows exceed the capacity it published receives nothing; invalid input
+// anywhere (negative or oversized split, offsets out of range, headers that differ) moves
+// nothing anywhere. Both are reported to the host of every rank through InputStatus.
+namespace {
+
+constexpr uint32_t kA2aBad = 0xffffffffu;  // a count that is not a valid row count
+
+// Spin until the grid-barrier generation moves past `g`, bounded like every other device-side
+// wait: 0 when it moved, kAbortTimeout / kAbortPeer when the wait was abandoned.
+static __device__ __noinline__ uint32_t waitGenSlow(const volatile uint32_t* gen, uint32_t g, uint32_t* abortWord,
+                                                    unsigned long long timeoutNs) {
+  const unsigned long long t0 = globalTimerNs();
+  uint32_t polls = 0;
+  while (*gen == g) {
+    if ((++polls & 127u) == 0u) {
+      if (ld_relaxed_sys(abortWord) != 0u) return kAbortPeer;
+      if (timeoutNs != 0ull && globalTimerNs() - t0 > timeoutNs) {
+        atomicCAS(abortWord, 0u, static_cast<uint32_t>(kAbortTimeout));
+        return kAbortTimeout;
+      }
+    }
+  }
+  return 0u;
+}
+
+// Grid barrier among the CTAs of THIS launch on this rank. It relies on every CTA being resident
+// (the grid is capped by coResidentBlocks); should that fail, e.g. because another process holds
+// SMs, the wait gives up after the context timeout like a barrier does, raises the abort word and
+// returns false. Every CTA still counts its arrival, so the last one to arrive resets the counter
+// and the next launch starts clean. Everything a CTA wrote before, at system scope, is visible to
+// every CTA after it, and is covered by their later release stores.
+__device__ __forceinline__ bool localGridSync(const CommArgs& a) {
+  SignalPad* me = a.self;
+  __syncthreads();
+  int ok = 1;
+  if (threadIdx.x == 0) {
+    volatile uint32_t* gen = &me->a2aGen;
+    const uint32_t g = *gen;
+    __threadfence_system();
+    if (atomicAdd(&me->a2aArrive, 1u) == gridDim.x - 1) {
+      atomicExch(&me->a2aArrive, 0u);
+      __threadfence();
+      atomicAdd(&me->a2aGen, 1u);
+    } else if (*gen == g) {
+      const uint32_t rc = waitGenSlow(gen, g, &me->abort, a.timeoutNs);
+      if (rc != 0u) {
+        reportAbort(a, rc, a.rank);
+        ok = 0;
+      }
+    }
+    __threadfence();
+  }
+  return __syncthreads_and(ok) != 0;
+}
+
+// Exclusive prefix sum over the CTA (one value per thread); `total` gets the sum.
+__device__ __forceinline__ unsigned long long blockExclusiveScan(unsigned long long v, unsigned long long* warpSums,
+                                                                 unsigned long long& total) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  unsigned long long x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) warpSums[w] = x;
+  __syncthreads();
+  if (w == 0) {
+    unsigned long long s = lane < nw ? warpSums[lane] : 0ull;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long y = __shfl_up_sync(0xffffffffu, s, o);
+      if (lane >= o) s += y;
+    }
+    if (lane < nw) warpSums[lane] = s;
+  }
+  __syncthreads();
+  total = warpSums[nw - 1];
+  const unsigned long long r = x - v + (w > 0 ? warpSums[w - 1] : 0ull);
+  __syncthreads();
+  return r;
+}
+
+__device__ __forceinline__ uint32_t ldPad(const uint32_t* p) { return *reinterpret_cast<const volatile uint32_t*>(p); }
+
+}  // namespace
+
+struct A2aDevArgs {
+  const char* in;
+  unsigned long long inRows;
+  unsigned long long rowBytes;
+  const long long* inSplits;
+  const long long* inOffsets;  // inverse only
+  long long* outSplits;        // forward only, may be null
+  long long* outOffsets;
+  char* stagedOut;             // plain output: copied from my staging after barrier 2; null = zero copy
+  uint32_t capRows;
+  int experts;
+  int align;
+  int inverse;
+  InputStatus* status;  // host-mapped
+};
+
+__global__ void __launch_bounds__(kThreads)
+alltoallvDevKernel(CommArgs a, PeerPtrs outs, A2aDevArgs d) {
+  constexpr int kMaxK = kMaxRanks * kMaxA2aExperts;
+  __shared__ unsigned long long sSrc[kMaxK];  // my chunk k: first input row
+  __shared__ unsigned long long sDst[kMaxK];  //             first row in its destination's output
+  __shared__ unsigned long long sAux[kMaxK];  // forward: column sums, then expert bases; inverse: R[j][s]
+  __shared__ unsigned long long sRcv[kMaxK];  // forward: first row of my receive segment e·P+s
+  __shared__ uint32_t sRcvCnt[kMaxK];         //          and its rows
+  __shared__ uint32_t sCnt[kMaxK];            // my chunk k: rows
+  __shared__ unsigned long long sNeed[kMaxRanks], sCap[kMaxRanks], sBytes[kMaxRanks];
+  __shared__ unsigned long long sBlkOff[kMaxRanks], sBlkLen[kMaxRanks];
+  __shared__ unsigned long long sWarp[32];
+  const uint32_t ep = loadEpoch(a);
+  const int P = a.nranks, E = d.experts, K = P * E, me = a.rank, t = threadIdx.x;
+  const unsigned long long rb = d.rowBytes;
+
+  // ---- my own splits: validate, and where each chunk starts in my input ----
+  long long v = 0, o = 0;
+  bool bad = false;
+  if (t < K) {
+    v = d.inSplits[t];
+    bad = v < 0 || v > 0x7fffffffll;
+    if (d.inverse) {
+      o = d.inOffsets[t];
+      bad = bad || o < 0 || static_cast<unsigned long long>(o) > d.inRows ||
+            (!bad && static_cast<unsigned long long>(v) > d.inRows - static_cast<unsigned long long>(o));
+    }
+  }
+  const unsigned long long c = bad ? 0ull : static_cast<unsigned long long>(v);
+  unsigned long long inTotal;
+  const unsigned long long prefix = blockExclusiveScan(t < K ? c : 0ull, sWarp, inTotal);
+  if (t < K) {
+    sCnt[t] = static_cast<uint32_t>(c);
+    sSrc[t] = d.inverse ? static_cast<unsigned long long>(o) : prefix;
+  }
+  const bool localBad = __syncthreads_or(bad || (!d.inverse && inTotal > d.inRows)) != 0;
+
+  // ---- publish: header + counts into column `me` of every rank's tables, spread over the grid ----
+  {
+    const size_t gtid = static_cast<size_t>(blockIdx.x) * blockDim.x + t;
+    const size_t gthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
+    for (size_t i = gtid; i < static_cast<size_t>(P) * K; i += gthreads) {
+      const int peer = static_cast<int>(i / K), k = static_cast<int>(i % K);
+      const long long x = d.inSplits[k];
+      a.sig[peer]->a2aCount[k][me] = (x < 0 || x > 0x7fffffffll) ? kA2aBad : static_cast<uint32_t>(x);
+    }
+    if (blockIdx.x == 0 && t < P) {
+      uint32_t* h = &a.sig[t]->a2aHdr[0][me];
+      const uint32_t hdr[kA2aHdrWords] = {static_cast<uint32_t>(rb), static_cast<uint32_t>(E), static_cast<uint32_t>(d.align),
+                                          static_cast<uint32_t>(d.inverse), d.capRows, localBad ? 1u : 0u};
+#pragma unroll
+      for (int w = 0; w < kA2aHdrWords; w++) h[w * kMaxRanks] = hdr[w];
+    }
+  }
+  // CTA b's release at the barrier must cover what the other CTAs published.
+  const bool ok1 = localGridSync(a) && blockBarrier(a, ep + 1);
+
+  // ---- the count matrix: validity, capacities, every offset ----
+  const SignalPad* pad = a.self;
+  bool invalid = false;
+  if (ok1) {
+    bool b = false;
+    if (t < P) {
+      const uint32_t want[4] = {static_cast<uint32_t>(rb), static_cast<uint32_t>(E), static_cast<uint32_t>(d.align),
+                                static_cast<uint32_t>(d.inverse)};
+#pragma unroll
+      for (int w = 0; w < 4; w++) b = b || ldPad(&pad->a2aHdr[w][t]) != want[w];
+      b = b || ldPad(&pad->a2aHdr[5][t]) != 0u;
+      sCap[t] = ldPad(&pad->a2aHdr[4][t]);
+    }
+    for (int i = t; i < P * K; i += blockDim.x) b = b || ldPad(&pad->a2aCount[i % K][i / K]) == kA2aBad;
+    invalid = __syncthreads_or(b) != 0;
+  }
+  if (ok1 && !invalid) {
+    if (!d.inverse) {
+      // Column k = j·E + e: rows of sources before me, and of all sources.
+      if (t < K) {
+        unsigned long long before = 0, all = 0;
+        for (int s = 0; s < P; s++) {
+          const unsigned long long m = ldPad(&pad->a2aCount[t][s]);
+          before += s < me ? m : 0ull;
+          all += m;
+        }
+        sDst[t] = before;
+        sAux[t] = all;
+      }
+      __syncthreads();
+      // Destination j: expert segments start at multiples of `align`; it needs up to the end of the last.
+      if (t < P) {
+        unsigned long long base = 0;
+        for (int e = 0; e < E; e++) {
+          const unsigned long long n = sAux[t * E + e];
+          sAux[t * E + e] = base;
+          base += n;
+          if (e + 1 < E) base = (base + d.align - 1) / d.align * d.align;
+        }
+        sNeed[t] = base;
+      }
+      __syncthreads();
+      if (t < K) {
+        sDst[t] += sAux[t];
+        // My receive segment (e, s), t = e·P + s.
+        const int e = t / P, s = t % P;
+        unsigned long long off = sAux[me * E + e];
+        for (int s2 = 0; s2 < s; s2++) off += ldPad(&pad->a2aCount[me * E + e][s2]);
+        sRcv[t] = off;
+        sRcvCnt[t] = ldPad(&pad->a2aCount[me * E + e][s]);
+      }
+    } else {
+      // R[j][s] = rows holder j returns to rank s.
+      for (int i = t; i < P * P; i += blockDim.x) {
+        const int j = i / P, s = i % P;
+        unsigned long long r = 0;
+        for (int e = 0; e < E; e++) r += ldPad(&pad->a2aCount[e * P + s][j]);
+        sAux[i] = r;
+      }
+      __syncthreads();
+      if (t < P) {
+        unsigned long long need = 0, base = 0;
+        for (int j = 0; j < P; j++) {
+          need += sAux[j * P + t];
+          base += j < me ? sAux[j * P + t] : 0ull;
+        }
+        sNeed[t] = need;
+        for (int e = 0; e < E; e++) {
+          sDst[e * P + t] = base;
+          base += sCnt[e * P + t];
+        }
+      }
+    }
+    __syncthreads();
+    if (t < P) {
+      unsigned long long rows = 0;
+      for (int i = 0; i < E; i++) rows += sCnt[d.inverse ? i * P + t : t * E + i];
+      sBytes[t] = sNeed[t] > sCap[t] ? 0ull : rows * rb;  // an overflowing destination gets nothing
+    }
+    __syncthreads();
+    if (t == 0) {
+      // CTAs dealt to destinations in proportion to their bytes, at least one each (as launchAlltoallPush).
+      // The share is computed in double (spare x bytes may not fit 64 bits) and the running total
+      // is clamped, so rounding can never deal out more CTAs than the grid has.
+      unsigned long long total = 0, used = 0, extraUsed = 0;
+      for (int j = 0; j < P; j++) total += sBytes[j];
+      const unsigned long long spare = gridDim.x > static_cast<unsigned>(P) ? gridDim.x - P : 0u;
+      for (int j = 0; j < P; j++) {
+        unsigned long long extra =
+            total > 0 ? static_cast<unsigned long long>(static_cast<double>(spare) * static_cast<double>(sBytes[j]) /
+                                                        static_cast<double>(total))
+                      : 0ull;
+        extra = extra < spare - extraUsed ? extra : spare - extraUsed;
+        extraUsed += extra;
+        sBlkOff[j] = used;
+        sBlkLen[j] = 1 + extra;
+        used += sBlkLen[j];
+      }
+    }
+    __syncthreads();
+  }
+
+  // ---- report, receive metadata, payload ----
+  if (ok1 && blockIdx.x == 0) {
+    if (t == 0) {
+      int over = -1;
+      if (!invalid) {
+        for (int j = P - 1; j >= 0; j--) over = sNeed[j] > sCap[j] ? j : over;
+      }
+      volatile InputStatus* st = d.status;
+      if (st != nullptr && (invalid || over >= 0) && st->code == kInputOk) {
+        st->rank = over >= 0 ? static_cast<uint32_t>(over) : 0u;
+        st->need = over >= 0 ? sNeed[over] : 0ull;
+        st->avail = over >= 0 ? sCap[over] : 0ull;
+        __threadfence_system();
+        st->code = invalid ? kInputInvalid : kInputOverflow;
+      }
+    }
+    if (!invalid && !d.inverse && d.outSplits != nullptr && t < K) {
+      d.outSplits[t] = sRcvCnt[t];
+      d.outOffsets[t] = static_cast<long long>(sRcv[t]);
+    }
+  }
+  if (ok1 && !invalid) {
+    const bool partitioned = gridDim.x >= static_cast<unsigned>(P);
+    for (int i = 0; i < P; i++) {
+      const int dst = (me + i) % P;
+      if (sBytes[dst] == 0) continue;
+      size_t tid, nthreads;
+      if (partitioned) {
+        const size_t b0 = sBlkOff[dst], nb = sBlkLen[dst];
+        if (blockIdx.x < b0 || blockIdx.x >= b0 + nb) continue;
+        tid = (blockIdx.x - b0) * blockDim.x + t;
+        nthreads = nb * blockDim.x;
+      } else {
+        tid = static_cast<size_t>(blockIdx.x) * blockDim.x + t;
+        nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
+      }
+      for (int x = 0; x < E; x++) {
+        const int k = d.inverse ? x * P + dst : dst * E + x;
+        if (sCnt[k] == 0) continue;
+        gridCopy(static_cast<char*>(outs.p[dst]) + sDst[k] * rb, d.in + sSrc[k] * rb, sCnt[k] * rb, true, tid, nthreads);
+      }
+    }
+  }
+  blockBarrier(a, ep + 2);
+  // NO pad table reads from here on. Once every CTA of every rank has arrived at barrier 2 a peer
+  // may finish and start its next launch, which rewrites its column of my tables before its own
+  // barrier 1 without waiting for anything. Everything below comes from shared memory.
+
+  // ---- plain output: my staging -> out, once every CTA of every peer has pushed ----
+  if (d.stagedOut != nullptr) {
+    const bool synced = localGridSync(a);
+    if (synced && ok1 && !invalid && sNeed[me] <= sCap[me] && ld_relaxed_sys(&a.self->abort) == 0u) {
+      const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + t;
+      const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
+      const char* stage = static_cast<const char*>(outs.p[me]);
+      if (d.inverse) {
+        gridCopy(d.stagedOut, stage, sNeed[me] * rb, true, tid, nthreads);
+      } else {
+        // Segment by segment: alignment gaps of `out` stay untouched.
+        for (int k = 0; k < K; k++) {
+          const unsigned long long n = sRcvCnt[k];
+          if (n > 0) gridCopy(d.stagedOut + sRcv[k] * rb, stage + sRcv[k] * rb, n * rb, true, tid, nthreads);
+        }
+      }
+    }
+  }
+  retire(a, 2, 0);
+}
+
+void launchAlltoallvDev(const CommArgs& a, const PeerPtrs& outs, const void* in, size_t inRows, size_t rowBytes,
+                        const long long* inSplits, const long long* inOffsets, long long* outSplits,
+                        long long* outOffsets, void* stagedOut, uint32_t capRows, int experts, int align, bool inverse,
+                        InputStatus* status, int blocks, cudaStream_t stream) {
+  A2aDevArgs d;
+  d.in = static_cast<const char*>(in);
+  d.inRows = inRows;
+  d.rowBytes = rowBytes;
+  d.inSplits = inSplits;
+  d.inOffsets = inOffsets;
+  d.outSplits = outSplits;
+  d.outOffsets = outOffsets;
+  d.stagedOut = static_cast<char*>(stagedOut);
+  d.capRows = capRows;
+  d.experts = experts;
+  d.align = align;
+  d.inverse = inverse ? 1 : 0;
+  d.status = status;
+  alltoallvDevKernel<<<blocks, kThreads, 0, stream>>>(a, outs, d);
+}
+
 // ---- reduce_scatter / reduce: pull my slice from every peer's input, reduce, store -----------
 // Inputs are peer-mapped. Rank r reduces elements [elemOff[r], elemOff[r]+elemLen[r])
 // and writes them to `out` (local pointer; for reduce() it is the root's peer-mapped
@@ -757,6 +1118,7 @@ const void* broadcastKernelPtr() { return reinterpret_cast<const void*>(broadcas
 const void* gatherPushKernelPtr() { return reinterpret_cast<const void*>(gatherPushKernel); }
 const void* gatherBulkKernelPtr() { return reinterpret_cast<const void*>(gatherBulkKernel); }
 const void* alltoallPushKernelPtr() { return reinterpret_cast<const void*>(alltoallPushKernel); }
+const void* alltoallvDevKernelPtr() { return reinterpret_cast<const void*>(alltoallvDevKernel); }
 const void* reducePullKernelPtr(DataType dt, int nranks) {
 #define GLB_RP(E, T)                                                                                   \
   case DataType::E: {                                                                                  \
@@ -797,6 +1159,7 @@ void preloadCollectiveKernels() {
                        static_cast<int>(kBulkSmemBytes));
   touch(reinterpret_cast<const void*>(gatherBulkKernel));
   touch(reinterpret_cast<const void*>(alltoallPushKernel));
+  touch(reinterpret_cast<const void*>(alltoallvDevKernel));
   touch(reinterpret_cast<const void*>(llExchangeKernel));
 #define GLB_TOUCH_RP(T) touch(reinterpret_cast<const void*>(reducePullKernel<T, 0, 1>));
   GLB_TOUCH_RP(int8_t) GLB_TOUCH_RP(uint8_t) GLB_TOUCH_RP(int16_t) GLB_TOUCH_RP(int32_t) GLB_TOUCH_RP(uint32_t)

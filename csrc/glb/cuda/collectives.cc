@@ -767,6 +767,58 @@ void alltoallv(PeerContext& pc, const void* in, const std::vector<size_t>& sendB
   if (roff.back() > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(out, st.mine, roff.back(), cudaMemcpyDeviceToDevice, stream));
 }
 
+namespace {
+// Like the host-count v-variant the grid is fixed (the sizes are only known on the device, the
+// grid must be the same on every rank), and P = 1 runs the same kernel: the expert-major layout
+// still applies.
+void alltoallvDevCommon(PeerContext& pc, const void* in, size_t inRows, size_t rowBytes, const int64_t* inSplits,
+                        const int64_t* inOffsets, const PeerPtrs& outs, void* stagedOut, size_t capacityRows,
+                        int64_t* outSplits, int64_t* outOffsets, int experts, int align, bool inverse,
+                        cudaStream_t stream) {
+  GLB_TRACE_RANGE("glb::cuda::alltoallv_dev");
+  GLB_ENFORCE(experts >= 1 && experts <= kMaxA2aExperts, "alltoallv_dev: experts per rank must be in 1..",
+              kMaxA2aExperts, ", got ", experts);
+  GLB_ENFORCE(align >= 1, "alltoallv_dev: align must be at least 1, got ", align);
+  GLB_ENFORCE(rowBytes > 0 && rowBytes <= 0xffffffffull, "alltoallv_dev: row size must be 1 byte .. 4 GB, got ",
+              rowBytes);
+  GLB_ENFORCE(inSplits != nullptr, "alltoallv_dev: no input splits");
+  GLB_ENFORCE(!inverse || inOffsets != nullptr, "alltoallv_dev: the inverse exchange needs the input offsets");
+  GLB_ENFORCE(inverse || (outSplits != nullptr && outOffsets != nullptr),
+              "alltoallv_dev: the forward exchange needs output splits and offsets");
+  const uint32_t cap = static_cast<uint32_t>(std::min<size_t>(capacityRows, 0xfffffffeull));
+  const int blocks =
+      std::max(1, std::min({tuning().alltoallvBlocks, pc.coResidentBlocks(alltoallvDevKernelPtr()), kMaxBlocks}));
+  prologue(pc, stream);
+  launchAlltoallvDev(pc.comm(), outs, in, inRows, rowBytes, reinterpret_cast<const long long*>(inSplits),
+                     reinterpret_cast<const long long*>(inOffsets), reinterpret_cast<long long*>(outSplits),
+                     reinterpret_cast<long long*>(outOffsets), stagedOut, cap, experts, align, inverse,
+                     pc.inputStatusDevice(), blocks, stream);
+  finish(pc, stream, "alltoallv_dev");
+}
+}  // namespace
+
+void alltoallvDev(PeerContext& pc, const void* in, size_t inRows, size_t rowBytes, const int64_t* inSplits,
+                  const int64_t* inOffsets, const PeerBuffer& out, size_t outOffset, size_t capacityRows,
+                  int64_t* outSplits, int64_t* outOffsets, int experts, int align, bool inverse, cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  GLB_ENFORCE(rowBytes > 0, "alltoallv_dev: row size must be positive");
+  GLB_ENFORCE_LE(outOffset + capacityRows * rowBytes, out.bytes, "alltoallv_dev output exceeds the registered buffer");
+  alltoallvDevCommon(pc, in, inRows, rowBytes, inSplits, inOffsets, out.ptrsAt(outOffset), nullptr, capacityRows,
+                     outSplits, outOffsets, experts, align, inverse, stream);
+}
+
+void alltoallvDev(PeerContext& pc, const void* in, size_t inRows, size_t rowBytes, const int64_t* inSplits,
+                  const int64_t* inOffsets, void* out, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets,
+                  int experts, int align, bool inverse, cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  GLB_ENFORCE(rowBytes > 0, "alltoallv_dev: row size must be positive");
+  // Peers push into my staging area; I copy my rows out of it inside the same kernel.
+  const auto l = layoutOf(pc);
+  alltoallvDevCommon(pc, in, inRows, rowBytes, inSplits, inOffsets, pc.stagePtrs(l.bulkOff), out,
+                     std::min(capacityRows, l.bulkBytes / rowBytes), outSplits, outOffsets, experts, align, inverse,
+                     stream);
+}
+
 void scatter(PeerContext& pc, const void* in, const PeerBuffer& out, size_t outOffset, size_t bytes, int root,
              cudaStream_t stream) {
   DeviceGuard g(pc.device);

@@ -135,6 +135,27 @@ void alltoallv(PeerContext& pc, const void* in, const std::vector<size_t>& sendB
                size_t outOffset, const std::vector<size_t>& recvBytes, cudaStream_t stream);
 void alltoallv(PeerContext& pc, const void* in, const std::vector<size_t>& sendBytes, void* out,
                const std::vector<size_t>& recvBytes, cudaStream_t stream);
+
+// All-to-all-v whose row counts live on the device (expert-parallel dispatch / combine): one
+// kernel, no host value depends on the device data, so it needs no synchronisation and can be
+// captured in a CUDA graph. A row is `rowBytes` on every rank; `in` holds `inRows` rows.
+// `inSplits` has P·E int64 entries.
+//   forward (inverse = false): entry j·E + e = my rows for expert e of rank j, packed in that
+//     order in `in`. Each rank receives expert-major: expert e's segment starts at a multiple of
+//     `align` rows and holds the rows of sources 0..P-1 in order; it writes outSplits[e·P + s] /
+//     outOffsets[e·P + s] (int64, rows) for its segment from source s.
+//   inverse: `inSplits` / `inOffsets` (entry e·P + s) describe the forward output layout; the
+//     rows go back to where they came from, packed in (holder, expert) order.
+// An output that would need more than its capacity (`capacityRows`, and for a plain pointer also
+// what fits the staging pool) receives nothing; invalid splits or offsets move nothing. Either
+// is raised as InputException by the next checkHealth() on every rank that runs after the kernel
+// has (synchronize() is the dependable place: earlier calls may not see it yet).
+void alltoallvDev(PeerContext& pc, const void* in, size_t inRows, size_t rowBytes, const int64_t* inSplits,
+                  const int64_t* inOffsets, const PeerBuffer& out, size_t outOffset, size_t capacityRows,
+                  int64_t* outSplits, int64_t* outOffsets, int experts, int align, bool inverse, cudaStream_t stream);
+void alltoallvDev(PeerContext& pc, const void* in, size_t inRows, size_t rowBytes, const int64_t* inSplits,
+                  const int64_t* inOffsets, void* out, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets,
+                  int experts, int align, bool inverse, cudaStream_t stream);
 // Fixed-size alltoall: every chunk is `bytes` long on every rank (this is known to all
 // ranks, so the small-message LL kernel and size-dependent grids are safe here).
 void alltoall(PeerContext& pc, const void* in, const PeerBuffer& out, size_t outOffset, size_t bytes,

@@ -12,12 +12,29 @@ constexpr int kMaxRanks = 16;
 constexpr int kMaxBlocks = 512;   // upper bound on CTAs of one collective kernel
 constexpr int kThreads = 512;     // threads per CTA of the data-moving kernels
 constexpr int kP2pLanes = 64;     // max CTAs per direction of a point-to-point transfer
+constexpr int kMaxA2aExperts = 32;  // local experts per rank of the device-split all-to-all-v
+constexpr int kA2aHdrWords = 6;     // its per-rank header: rowBytes, E, align, inverse, capacity, bad input
 
 // Why a kernel gave up (SignalPad::abort / the host status word).
 enum AbortCode : uint32_t {
   kAbortNone = 0,
   kAbortTimeout = 1,   // a peer did not reach the barrier within the timeout
   kAbortPeer = 2,      // a peer (or another CTA) aborted first and told us
+};
+
+// Data error found on the device by the device-split all-to-all-v. It is reported through a
+// host-mapped word of its own (not the abort word): the context stays usable, and the next host
+// call raises it as an input error.
+enum InputCode : uint32_t {
+  kInputOk = 0,
+  kInputOverflow = 1,  // a destination needs more output rows than it has
+  kInputInvalid = 2,   // a negative or oversized split, an offset out of range, or headers that differ
+};
+struct InputStatus {
+  uint32_t code;             // InputCode; written last, cleared by the host when it raises
+  uint32_t rank;             // the overflowing destination
+  unsigned long long need;   // rows it needs
+  unsigned long long avail;  // rows it has
 };
 
 // One per rank, at the start of its symmetric pool. `flag[b][s]` is written by
@@ -42,6 +59,17 @@ struct alignas(128) SignalPad {
   uint32_t p2pTail[kP2pLanes][kMaxRanks];
   uint32_t p2pSent[kP2pLanes][kMaxRanks];
   uint32_t p2pRecvd[kP2pLanes][kMaxRanks];
+  // Device-split all-to-all-v (alltoallvDevKernel). Before its first barrier rank s writes its
+  // header and its P·E row counts into column s of these tables in EVERY rank's pad (the layout
+  // of `flag`), so after the barrier each rank reads the whole count matrix from its own pad.
+  // Rank s writes them again only in its next launch, after all of its CTAs have passed the
+  // second barrier of this one, i.e. after every reader has finished. That holds because no rank
+  // reads the tables after its own second barrier.
+  uint32_t a2aHdr[kA2aHdrWords][kMaxRanks];
+  uint32_t a2aCount[kMaxRanks * kMaxA2aExperts][kMaxRanks];
+  // Grid barrier among this rank's own CTAs of one launch: arrivals, generation.
+  uint32_t a2aArrive;
+  uint32_t a2aGen;
 };
 
 struct CommArgs {

@@ -70,7 +70,16 @@ void launchAlltoallPush(const CommArgs& a, const void* in, const PeerPtrs& outs,
 void launchReducePull(const CommArgs& a, const PeerPtrs& ins, void* mcIn, void* out, const size_t* elemOff,
                       const size_t* elemLen, DataType dt, ReduceOp op, float scale, bool vec, bool useMc, int blocks,
                       cudaStream_t stream);
+// Device-split all-to-all-v: row counts come from device arrays (int64, P·E entries) and are
+// exchanged inside the kernel. `outs.p[r]` is rank r's output (zero copy) or staging area; with
+// `stagedOut` set, each rank copies its rows from its staging area to stagedOut after the second
+// barrier. See collective_kernels.cu for the two layouts.
+void launchAlltoallvDev(const CommArgs& a, const PeerPtrs& outs, const void* in, size_t inRows, size_t rowBytes,
+                        const long long* inSplits, const long long* inOffsets, long long* outSplits,
+                        long long* outOffsets, void* stagedOut, uint32_t capRows, int experts, int align, bool inverse,
+                        InputStatus* status, int blocks, cudaStream_t stream);
 // Entry points, for occupancy queries (every CTA of a collective kernel must be resident).
+const void* alltoallvDevKernelPtr();
 const void* broadcastKernelPtr();
 const void* gatherPushKernelPtr();
 const void* gatherBulkKernelPtr();

@@ -215,9 +215,12 @@ PeerContext::PeerContext(std::shared_ptr<Context> context, int dev, PeerOptions 
   comm_.self = comm_.sig[rank];
   // Status word the kernels raise when a device-side wait gives up.
   GLB_CUDA_CHECK(cudaHostAlloc(reinterpret_cast<void**>(&hostStatus_), 64, cudaHostAllocMapped | cudaHostAllocPortable));
-  *hostStatus_ = 0;
+  std::memset(hostStatus_, 0, 64);
   GLB_CUDA_CHECK(cudaHostGetDevicePointer(reinterpret_cast<void**>(&hostStatusDev_), hostStatus_, 0));
   comm_.hostStatus = hostStatusDev_;
+  static_assert(16 + sizeof(InputStatus) <= 64, "the input status must fit the pinned status block");
+  inputStatus_ = reinterpret_cast<InputStatus*>(reinterpret_cast<char*>(hostStatus_) + 16);
+  inputStatusDev_ = reinterpret_cast<InputStatus*>(reinterpret_cast<char*>(hostStatusDev_) + 16);
   setTimeout(std::chrono::duration_cast<std::chrono::milliseconds>(context->getTimeout()));
   GLB_CUDA_CHECK(cudaEventCreateWithFlags(&orderEvent_, cudaEventDisableTiming));
   hostBarrier();
@@ -413,7 +416,21 @@ void PeerContext::setTimeout(std::chrono::milliseconds t) {
 void PeerContext::checkHealth() {
   if (!poisoned_) {
     const uint32_t st = *static_cast<volatile uint32_t*>(hostStatus_);
-    if (st == 0) return;
+    if (st == 0) {
+      volatile InputStatus* in = inputStatus_;
+      const uint32_t code = in->code;
+      if (code == kInputOk) return;
+      const uint32_t who = in->rank;
+      const unsigned long long need = in->need, avail = in->avail;
+      in->code = kInputOk;  // raised once; the next call starts clean
+      if (code == kInputOverflow) {
+        GLB_THROW(InputException, "alltoallv_dev: rank ", who, " needs ", need, " output rows but has room for ", avail,
+                  "; no rows were sent to it");
+      }
+      GLB_THROW(InputException,
+                "alltoallv_dev: invalid splits (a negative or > 2^31-1 count, an offset outside the input, splits "
+                "summing to more rows than the input has, or arguments that differ between ranks); nothing was sent");
+    }
     poisoned_ = true;
     const uint32_t code = st & 0xffu, who = st >> 8;
     poisonReason_ = code == kAbortTimeout

@@ -126,8 +126,12 @@ class PeerContext : public std::enable_shared_from_this<PeerContext> {
   // (gloo/transport/tcp/unbound_buffer.cc:52-94). Rebuild the context to continue.
   void setTimeout(std::chrono::milliseconds t);
   std::chrono::milliseconds timeout() const { return timeout_; }
+  // Also raises InputException (once, then clears it) when a kernel found invalid device-side
+  // input, e.g. the splits of alltoallvDev(); that does not poison the context.
   void checkHealth();
   bool poisoned() const { return poisoned_; }
+  // Device alias of the host-mapped word such kernels report input errors through.
+  InputStatus* inputStatusDevice() const { return inputStatusDev_; }
   // cudaStreamSynchronize + checkHealth: the place where a dead peer surfaces.
   void synchronize(cudaStream_t stream);
 
@@ -220,6 +224,8 @@ class PeerContext : public std::enable_shared_from_this<PeerContext> {
   CommArgs comm_;
   uint32_t* hostStatus_ = nullptr;     // pinned + mapped: written by kernels that give up
   uint32_t* hostStatusDev_ = nullptr;  // device alias of hostStatus_
+  InputStatus* inputStatus_ = nullptr;     // in the same pinned block, after the abort word
+  InputStatus* inputStatusDev_ = nullptr;
   std::chrono::milliseconds timeout_{0};
   bool poisoned_ = false;
   std::string poisonReason_;

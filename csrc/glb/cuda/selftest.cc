@@ -302,6 +302,76 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
       }
       return "";
     });
+    // Device-split all-to-all-v. Rank 0 writes its counts into column j of the tables for virtual
+    // peer j, which is column j of its own pad: every virtual rank holds rank 0's splits. Rank 0's
+    // segments then have a closed form: on rank j, expert e's segment starts at
+    // base_e = sum over e' < e of roundUp(P * split(j, e'), align), and rank 0's rows come first.
+    R.run(strcat_all("alltoallvDevKernel (dispatch + combine, E=3, align=8, 12-byte rows) P=", P), [&]() -> std::string {
+      const int E = 3, A = 8, K = P * E;
+      const size_t rb = 12, cap = n * 4 / rb;
+      std::vector<int64_t> sp(K), pre(K + 1, 0);
+      for (int k = 0; k < K; k++) {
+        sp[k] = (k * 7 + 3) % 11;
+        pre[k + 1] = pre[k] + sp[k];
+      }
+      auto base = [&](int j, int e) {
+        int64_t b = 0;
+        for (int x = 0; x < e; x++) b = (b + P * sp[j * E + x] + A - 1) / A * A;
+        return b;
+      };
+      DevBuf in(pre[K] * rb), splits(K * 8), outSplits(K * 8), outOffsets(K * 8);
+      launchFill(in.p, pre[K] * 3, DataType::FLOAT32, 0.0, 1.0, stream);  // row r = {3r, 3r+1, 3r+2}
+      GLB_CUDA_CHECK(cudaMemcpyAsync(splits.p, sp.data(), K * 8, cudaMemcpyHostToDevice, stream));
+      for (int r = 0; r < P; r++) GLB_CUDA_CHECK(cudaMemsetAsync(pp.p[r], 0xff, n * 4, stream));
+      const int blocks = std::min(pc.coResidentBlocks(alltoallvDevKernelPtr()), 16);
+      launchAlltoallvDev(ca, pp, in.p, pre[K], rb, static_cast<const long long*>(splits.p), nullptr,
+                         static_cast<long long*>(outSplits.p), static_cast<long long*>(outOffsets.p), nullptr,
+                         static_cast<uint32_t>(cap), E, A, false, pc.inputStatusDevice(), blocks, stream);
+      noteLaunch();
+      std::vector<int64_t> os(K), oo(K);
+      GLB_CUDA_CHECK(cudaMemcpyAsync(os.data(), outSplits.p, K * 8, cudaMemcpyDeviceToHost, stream));
+      GLB_CUDA_CHECK(cudaMemcpyAsync(oo.data(), outOffsets.p, K * 8, cudaMemcpyDeviceToHost, stream));
+      for (int j = 0; j < P; j++) {
+        auto h = download(pp.p[j], n, stream);
+        for (int e = 0; e < E; e++) {
+          const int k = j * E + e;
+          const int64_t at = base(j, e);
+          for (int64_t r = 0; r < sp[k]; r++) {
+            for (int c = 0; c < 3; c++) {
+              const float got = h[(at + r) * 3 + c];
+              if (!close(got, 3.0 * (pre[k] + r) + c)) return strcat_all("dispatch dst ", j, " expert ", e, " row ", r, ": got ", got);
+            }
+          }
+          // Virtual rank 1's rows follow (never written). An empty segment has no such row: the
+          // next expert's segment starts at the same place.
+          if (sp[k] > 0 && !std::isnan(h[(at + sp[k]) * 3])) {
+            return strcat_all("dispatch dst ", j, ": wrote past rank 0's segment");
+          }
+        }
+      }
+      for (int e = 0; e < E; e++) {
+        for (int s = 0; s < P; s++) {
+          if (os[e * P + s] != sp[e] || oo[e * P + s] != base(0, e) + s * sp[e]) {
+            return strcat_all("out_splits/out_offsets[", e * P + s, "] = ", os[e * P + s], "/", oo[e * P + s]);
+          }
+        }
+      }
+      // Combine from rank 0's dispatch output: its own rows come back to where they were.
+      DevBuf back(n * 4);
+      PeerPtrs bp = pp;
+      bp.p[0] = back.p;
+      GLB_CUDA_CHECK(cudaMemsetAsync(back.p, 0, n * 4, stream));
+      launchAlltoallvDev(ca, bp, pp.p[0], cap, rb, static_cast<const long long*>(outSplits.p),
+                         static_cast<const long long*>(outOffsets.p), nullptr, nullptr, nullptr,
+                         static_cast<uint32_t>(cap), E, 1, true, pc.inputStatusDevice(), blocks, stream);
+      noteLaunch();
+      auto h = download(back.p, n, stream);
+      for (int64_t i = 0; i < pre[E] * 3; i++) {
+        if (!close(h[i], static_cast<double>(i))) return strcat_all("combine element ", i, ": got ", h[i]);
+      }
+      if (h[pre[E] * 3] != 0.0f) return "combine wrote past its rows";
+      return "";
+    });
 
     // ---- literal schedule executor (halving-doubling, plain and pipelined) -------------------
     R.run(strcat_all("scheduleKernel<float>(halving_doubling) P=", P), [&]() -> std::string {

@@ -113,9 +113,13 @@ PYBIND11_MODULE(_C, m) {
   static py::exception<TimeoutException> toExc(m, "TimeoutError", ioExc.ptr());
   static py::exception<InvalidOperationException> invExc(m, "InvalidOperationError", m.attr("GlbError").ptr());
   static py::exception<EnforceNotMet> enfExc(m, "EnforceError", m.attr("GlbError").ptr());
+  // Invalid data found on the device: a ValueError, like the host-side argument checks.
+  static py::exception<InputException> inExc(m, "InputError", PyExc_ValueError);
   py::register_exception_translator([](std::exception_ptr p) {
     try {
       if (p) std::rethrow_exception(p);
+    } catch (const InputException& e) {
+      py::set_error(inExc, e.what());
     } catch (const TimeoutException& e) {
       py::set_error(toExc, e.what());
     } catch (const IoException& e) {

@@ -175,6 +175,27 @@ void registerCudaAlgorithms(py::module_& m) {
     py::gil_scoped_release nogil;
     alltoallv(pc, P(in), sendBytes, P(out), recvBytes, S(st));
   });
+  // Device-split all-to-all-v. Splits / offsets are addresses of int64 device arrays (0 = none);
+  // `buf` is the registered output (None: `out` is a plain device pointer, staged).
+  m.def("alltoallv_dev", [](PeerContext& pc, uintptr_t in, size_t inRows, size_t rowBytes, uintptr_t inSplits,
+                            uintptr_t inOffsets, py::object buf, size_t off, uintptr_t out, size_t capacityRows,
+                            uintptr_t outSplits, uintptr_t outOffsets, int experts, int align, bool inverse,
+                            uintptr_t st) {
+    const PeerBuffer* reg = buf.is_none() ? nullptr : buf.cast<const PeerBuffer*>();
+    auto* is = reinterpret_cast<const int64_t*>(inSplits);
+    auto* io = reinterpret_cast<const int64_t*>(inOffsets);
+    auto* os = reinterpret_cast<int64_t*>(outSplits);
+    auto* oo = reinterpret_cast<int64_t*>(outOffsets);
+    py::gil_scoped_release nogil;
+    if (reg != nullptr) {
+      alltoallvDev(pc, P(in), inRows, rowBytes, is, io, *reg, off, capacityRows, os, oo, experts, align, inverse, S(st));
+    } else {
+      alltoallvDev(pc, P(in), inRows, rowBytes, is, io, P(out), capacityRows, os, oo, experts, align, inverse, S(st));
+    }
+  }, py::arg("pc"), py::arg("input"), py::arg("in_rows"), py::arg("row_bytes"), py::arg("in_splits"),
+     py::arg("in_offsets"), py::arg("buf"), py::arg("buf_offset"), py::arg("out"), py::arg("capacity_rows"),
+     py::arg("out_splits"), py::arg("out_offsets"), py::arg("experts"), py::arg("align"), py::arg("inverse"),
+     py::arg("stream"));
   m.def("alltoall_reg", [](PeerContext& pc, uintptr_t in, const PeerBuffer& out, size_t off, size_t bytes, uintptr_t st) {
     py::gil_scoped_release nogil;
     alltoall(pc, P(in), out, off, bytes, S(st));

@@ -198,6 +198,9 @@ class CudaContext:
         self.pc.set_timeout(int(ms))
 
     def check_health(self):
+        """Raise ``IoError`` if a device-side wait timed out (the context is then unusable), or
+        ``ValueError`` (``InputError``) once if a kernel found invalid device-side input, such as
+        the splits of :meth:`alltoallv_dev`."""
         self.pc.check_health()
 
     def synchronize(self, stream=None):
@@ -305,6 +308,71 @@ class CudaContext:
         else:
             _cu.alltoallv(self.pc, input.data_ptr(), send, output.data_ptr(), recv, _stream(stream))
         return output
+
+    def _dev_rows(self, out, inp) -> int:
+        """Bytes of one row (everything but dim 0); ``out`` and ``inp`` must agree on it."""
+        _, _, dt, icuda = describe(inp)
+        _, _, odt, ocuda = describe(out)
+        if not (icuda and ocuda):
+            raise ValueError("alltoallv_dev needs CUDA tensors")
+        if odt != dt or tuple(out.shape[1:]) != tuple(inp.shape[1:]) or inp.dim() == 0:
+            raise ValueError(f"alltoallv_dev: rows of out {tuple(out.shape)} {out.dtype} and input "
+                             f"{tuple(inp.shape)} {inp.dtype} differ")
+        row = 1
+        for d in inp.shape[1:]:
+            row *= int(d)
+        if row == 0:
+            raise ValueError("alltoallv_dev: rows must not be empty")
+        return row * element_size(dt)
+
+    def _dev_index(self, t, name: str, n: int) -> int:
+        import torch
+
+        if (not isinstance(t, torch.Tensor) or t.dtype != torch.int64 or not t.is_cuda
+                or t.device.index != self.device or not t.is_contiguous() or t.numel() != n):
+            raise ValueError(f"alltoallv_dev: {name} must be a contiguous int64 tensor of {n} entries on "
+                             f"cuda:{self.device}")
+        return t.data_ptr()
+
+    def alltoallv_dev(self, out, inp, in_splits, out_splits, out_offsets, experts: int = 1, align: int = 1,
+                      stream=None):
+        """All-to-all-v whose row counts stay on the device: no host synchronisation, graph-capturable.
+
+        ``in_splits`` (int64 CUDA tensor of ``size * experts`` entries): entry ``j * experts + e`` is
+        how many rows of ``inp`` (packed in that order) go to local expert ``e`` of rank ``j``. Each
+        rank receives expert-major into ``out``: the segment of expert ``e`` starts at a multiple of
+        ``align`` rows and holds the rows of ranks 0, 1, ... in order; ``out_splits[e * size + s]`` and
+        ``out_offsets[e * size + s]`` receive the row count and first row of the part from rank ``s``.
+        ``out.shape[0]`` is the capacity: a rank that would need more rows receives none. That, or
+        invalid splits, is raised as ``ValueError`` on every rank by the first host call on this
+        context made after the stream has passed the failed call. Check with ``synchronize()`` (or
+        ``check_health()`` after a stream sync) at a point every rank reaches: a rank whose stream
+        has not run the call yet does not know about it, and a collective that raises on one rank
+        only would leave its peers waiting.
+        Registered / symmetric ``out``: zero copy; any other tensor goes through the staging pool."""
+        rb = self._dev_rows(out, inp)
+        k = self.size * int(experts)
+        si = self._dev_index(in_splits, "in_splits", k)
+        so = self._dev_index(out_splits, "out_splits", k)
+        oo = self._dev_index(out_offsets, "out_offsets", k)
+        buf, off = self.lookup(out)
+        _cu.alltoallv_dev(self.pc, inp.data_ptr(), int(inp.shape[0]), rb, si, 0, buf, off, out.data_ptr(),
+                          int(out.shape[0]), so, oo, int(experts), int(align), False, _stream(stream))
+        return out
+
+    def alltoallv_dev_combine(self, out, inp, in_splits, in_offsets, experts: int = 1, stream=None):
+        """Inverse of :meth:`alltoallv_dev`: ``inp`` is laid out as a dispatch output, described by
+        ``in_splits`` / ``in_offsets`` (that call's ``out_splits`` / ``out_offsets``; gaps allowed).
+        Every row goes back to its source, which receives them packed in (rank, expert) order:
+        exactly where its dispatch input rows were."""
+        rb = self._dev_rows(out, inp)
+        k = self.size * int(experts)
+        si = self._dev_index(in_splits, "in_splits", k)
+        io = self._dev_index(in_offsets, "in_offsets", k)
+        buf, off = self.lookup(out)
+        _cu.alltoallv_dev(self.pc, inp.data_ptr(), int(inp.shape[0]), rb, si, io, buf, off, out.data_ptr(),
+                          int(out.shape[0]), 0, 0, int(experts), 1, True, _stream(stream))
+        return out
 
     def scatter(self, output, input=None, root: int = 0, stream=None):
         nbytes = output.numel() * output.element_size()

@@ -495,6 +495,26 @@ class MoEDispatcher(_Base):
         # inverse of dispatch: what I received goes back to where it came from
         return self.dispatch(expert_out, recv_counts, out, send_counts)[0]
 
+    def dispatch_dev(self, tokens, splits, out, experts: int = 1, align: int = 1):
+        """dispatch() with the counts on the device: no ``.tolist()``, no host count exchange, one
+        kernel (CUDA graph capturable). ``splits``: int64 CUDA tensor, entry ``j * experts + e`` =
+        rows of ``tokens`` (packed in that order) for local expert ``e`` of rank ``j``. ``out``
+        receives expert-major (see ``CudaContext.alltoallv_dev``). Returns
+        ``(out, out_splits, out_offsets)``, entry ``e * size + s`` = rows from rank ``s`` for my
+        expert ``e`` and where they start. Overflow or invalid splits surface as ``ValueError`` at
+        the next ``cc.synchronize()`` (see ``CudaContext.alltoallv_dev``)."""
+        import torch
+
+        out_splits = torch.empty(self.size * experts, dtype=torch.int64, device=tokens.device)
+        out_offsets = torch.empty_like(out_splits)
+        self.cc.alltoallv_dev(out, tokens, splits, out_splits, out_offsets, experts=experts, align=align)
+        return out, out_splits, out_offsets
+
+    def combine_dev(self, expert_out, out_splits, out_offsets, out, experts: int = 1):
+        """Inverse of dispatch_dev(): the rows of ``expert_out`` (dispatch_dev's layout) go back to
+        their sources; ``out`` gets them where the dispatched ``tokens`` rows were."""
+        return self.cc.alltoallv_dev_combine(out, expert_out, out_splits, out_offsets, experts=experts)
+
 
 class UlyssesAttention(_Base):
     """DeepSpeed-Ulysses: [S/P, H, D] <-> [S, H/P, D] with one alltoall each way."""

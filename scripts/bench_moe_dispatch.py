@@ -1,0 +1,133 @@
+"""MoE dispatch + combine: host-count alltoallv against the device-split alltoallv_dev.
+
+One rank per visible GPU. With a single GPU the ranks are threads sharing it (--ranks, default 2):
+those figures show what removing the ``.tolist()`` sync and the TCP count exchange saves, not
+what NVLink bandwidth looks like, and are labelled as such.
+
+Per dispatch + combine pair it times:
+  host   splits.tolist() + TCP alltoall of the counts + cc.alltoallv, and the inverse alltoallv
+  dev    MoEDispatcher.dispatch_dev + combine_dev (no host sync)
+  graph  the same two calls captured once in a CUDA graph and replayed
+
+Rows: --tokens x top-k routed to --experts local experts per rank, rows of --hidden elements, in
+bf16 and FP8 e4m3. Outputs are symmetric (zero copy) for every path.
+
+    python scripts/bench_moe_dispatch.py [--ranks 2] [--iters 20]
+"""
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+import time
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+import torch  # noqa: E402
+
+import gloo_b200 as gb  # noqa: E402
+from gloo_b200.ops import cuda as gcu  # noqa: E402
+from gloo_b200.parallel.strategies import MoEDispatcher  # noqa: E402
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+        return q[0] if q else torch.cuda.get_device_name(0)
+    except (OSError, subprocess.SubprocessError):
+        return torch.cuda.get_device_name(0) + ", power limit unknown"
+
+
+def run_rank(ctx, args, dtype, shared):
+    if shared:  # spawn_threads already gave this rank cuda:0 and a stream of its own
+        return measure(ctx, args, dtype, 0)
+    torch.cuda.set_device(ctx.rank)
+    with torch.cuda.stream(gcu.new_stream(ctx.rank)):
+        return measure(ctx, args, dtype, ctx.rank)
+
+
+def measure(ctx, args, dtype, dev):
+    cc = gcu.CudaContext(ctx, dev, stage_bytes=16 << 20)
+    moe = MoEDispatcher(ctx, cc)
+    P, E, H = ctx.size, args.experts, args.hidden
+    G = P * E
+    k = min(args.topk, G)
+    rows = args.tokens * k
+    g = torch.Generator(device="cuda").manual_seed(1234 + ctx.rank)
+    logits = torch.randn(args.tokens, G, device="cuda", generator=g)
+    flat = torch.topk(logits, k, dim=-1).indices.reshape(-1)
+    splits = torch.zeros(G, dtype=torch.int64, device="cuda").index_add_(0, flat, torch.ones_like(flat))
+    tokens = torch.randn(rows, H, device="cuda", generator=g).to(dtype)
+    cap = P * rows
+    out = cc.empty((cap, H), dtype)
+    back = cc.empty((rows, H), dtype)
+    stream = torch.cuda.current_stream()
+
+    def host_pair():
+        sp = splits.tolist()
+        per = moe.exchange_counts(sp)
+        send = [sum(sp[j * E:(j + 1) * E]) * H for j in range(P)]
+        recv = [sum(per[s * E:(s + 1) * E]) * H for s in range(P)]
+        cc.alltoallv(out, recv, tokens, send)
+        cc.alltoallv(back, send, out, recv)
+
+    def dev_pair():
+        _, osp, ooff = moe.dispatch_dev(tokens, splits, out, experts=E)
+        moe.combine_dev(out, osp, ooff, back, experts=E)
+
+    graph = torch.cuda.CUDAGraph()
+
+    def timed(fn):
+        fn()
+        cc.synchronize()
+        times = []
+        for _ in range(args.iters):
+            cc.pc.host_barrier()
+            t0 = time.perf_counter()
+            fn()
+            cc.synchronize()
+            times.append((time.perf_counter() - t0) * 1e3)
+        return statistics.median(times)
+
+    res = {"host": timed(host_pair), "dev": timed(dev_pair)}
+    cc.pc.host_barrier()
+    with torch.cuda.graph(graph, stream=stream, capture_error_mode="thread_local"):
+        dev_pair()
+    cc.pc.host_barrier()
+    res["graph"] = timed(graph.replay)
+    res["bytes_per_rank"] = 2 * rows * H * tokens.element_size()
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("--ranks", type=int, default=2, help="threads sharing the GPU when only one is visible")
+    ap.add_argument("--tokens", type=int, default=4096)
+    ap.add_argument("--topk", type=int, default=8)
+    ap.add_argument("--hidden", type=int, default=7168)
+    ap.add_argument("--experts", type=int, default=8, help="local experts per rank")
+    ap.add_argument("--iters", type=int, default=20)
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), "needs a GPU"
+    ngpu = torch.cuda.device_count()
+    shared = ngpu == 1
+    P = args.ranks if shared else ngpu
+    label = f"{P} threads as ranks sharing one GPU" if shared else f"{P} GPUs, one rank each"
+    print(f"# card: {card()}", flush=True)
+    print(f"# ranks: {label}; {args.tokens} tokens x top-{args.topk}, hidden {args.hidden}, "
+          f"{args.experts} experts per rank; median of {args.iters} dispatch + combine pairs (rank 0)", flush=True)
+    print(f"{'dtype':>14} {'host ms':>9} {'dev ms':>9} {'graph ms':>9} {'host/dev':>9} {'MB/rank':>9}")
+    for dtype in (torch.bfloat16, torch.float8_e4m3fn):
+        if shared:
+            r = gb.spawn_threads(P, run_rank, args, dtype, True, cuda_device=0, timeout_ms=300000)[0]
+        else:
+            r = gb.spawn_threads(P, run_rank, args, dtype, False, timeout_ms=300000)[0]
+        print(f"{str(dtype).replace('torch.', ''):>14} {r['host']:9.3f} {r['dev']:9.3f} {r['graph']:9.3f} "
+              f"{r['host'] / r['dev']:9.2f} {r['bytes_per_rank'] / 1e6:9.1f}", flush=True)
+        print(json.dumps({"dtype": str(dtype), "ranks": P, "shared_gpu": shared, **r}), flush=True)
+
+
+if __name__ == "__main__":
+    main()
