@@ -104,68 +104,6 @@ __device__ __forceinline__ void storeLocalGroup(T* out, const LocalPtrs& extra, 
 
 // ---- LL (flag in data) -------------------------------------------------------------------
 
-template <typename T>
-struct AccType {
-  using type = T;
-};
-template <>
-struct AccType<__half> {
-  using type = float;
-};
-template <>
-struct AccType<__nv_bfloat16> {
-  using type = float;
-};
-template <>
-struct AccType<__nv_fp8_e4m3> {
-  using type = float;
-};
-template <>
-struct AccType<__nv_fp8_e5m2> {
-  using type = float;
-};
-
-template <typename T>
-__device__ __forceinline__ typename AccType<T>::type toAcc(T x) {
-  return x;
-}
-template <>
-__device__ __forceinline__ float toAcc<__half>(__half x) {
-  return __half2float(x);
-}
-template <>
-__device__ __forceinline__ float toAcc<__nv_bfloat16>(__nv_bfloat16 x) {
-  return __bfloat162float(x);
-}
-template <>
-__device__ __forceinline__ float toAcc<__nv_fp8_e4m3>(__nv_fp8_e4m3 x) {
-  return fp8ToFloat(x);
-}
-template <>
-__device__ __forceinline__ float toAcc<__nv_fp8_e5m2>(__nv_fp8_e5m2 x) {
-  return fp8ToFloat(x);
-}
-template <typename TO, typename A>
-__device__ __forceinline__ TO fromAcc(A x) {
-  return static_cast<TO>(x);
-}
-template <>
-__device__ __forceinline__ __half fromAcc<__half, float>(float x) {
-  return __float2half_rn(x);
-}
-template <>
-__device__ __forceinline__ __nv_bfloat16 fromAcc<__nv_bfloat16, float>(float x) {
-  return __float2bfloat16_rn(x);
-}
-template <>
-__device__ __forceinline__ __nv_fp8_e4m3 fromAcc<__nv_fp8_e4m3, float>(float x) {
-  return floatToFp8<__nv_fp8_e4m3>(x);
-}
-template <>
-__device__ __forceinline__ __nv_fp8_e5m2 fromAcc<__nv_fp8_e5m2, float>(float x) {
-  return floatToFp8<__nv_fp8_e5m2>(x);
-}
-
 // `ll.p[r]` is the LL region of rank r's pool: [parity][source rank][line]. A launch uses
 // parity = seq & 1; two halves suffice because a rank can run at most one launch ahead of
 // its slowest peer (it needs that peer's lines of launch s+1 to finish launch s+1).
@@ -177,7 +115,7 @@ __global__ void __launch_bounds__(kThreads)
 llAllreduceKernel(CommArgs a, const T* in, TO* out, size_t count, DevOp op, float scale, PeerPtrs ll, char* myLL,
                   size_t srcStride, size_t parityStride, LocalPtrs extra) {
   constexpr int K = 8 / sizeof(T);
-  using A = typename AccType<T>::type;
+  using A = typename Scalar<T>::Acc;
   const uint32_t seq = ld_relaxed_sys(&a.self->llSeq) + 1u;
   const size_t base = (seq & 1u) * parityStride;
   const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -240,10 +178,10 @@ llAllreduceKernel(CommArgs a, const T* in, TO* out, size_t count, DevOp op, floa
           const T* x = reinterpret_cast<const T*>(d);
           if (r == 0) {
 #pragma unroll
-            for (int k = 0; k < K; k++) acc[k] = toAcc<T>(x[k]);
+            for (int k = 0; k < K; k++) acc[k] = Scalar<T>::toAcc(x[k]);
           } else {
 #pragma unroll
-            for (int k = 0; k < K; k++) acc[k] = applyOp<A>(acc[k], toAcc<T>(x[k]), op);
+            for (int k = 0; k < K; k++) acc[k] = applyOp<A>(acc[k], Scalar<T>::toAcc(x[k]), op);
           }
         }
       }
@@ -258,7 +196,7 @@ llAllreduceKernel(CommArgs a, const T* in, TO* out, size_t count, DevOp op, floa
 #pragma unroll
     for (int k = 0; k < K; k++) {
       if (i0 + k < count) {
-        const TO o = fromAcc<TO, A>(acc[k]);
+        const TO o = Scalar<TO>::fromAcc(acc[k]);
         out[i0 + k] = o;
         if constexpr (std::is_same<T, TO>::value) {
           if (extra.n > 0) {
@@ -288,7 +226,7 @@ __global__ void __launch_bounds__(kThreads)
 llReduceScatterKernel(CommArgs a, const T* in, T* out, size_t per, DevOp op, float scale, PeerPtrs ll, char* myLL,
                       size_t srcStride, size_t parityStride) {
   constexpr int K = 8 / sizeof(T);
-  using A = typename AccType<T>::type;
+  using A = typename Scalar<T>::Acc;
   const uint32_t seq = ld_relaxed_sys(&a.self->llSeq) + 1u;
   const size_t base = (seq & 1u) * parityStride;
   const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -331,7 +269,7 @@ llReduceScatterKernel(CommArgs a, const T* in, T* out, size_t per, DevOp op, flo
       }
       const T* x = reinterpret_cast<const T*>(d);
 #pragma unroll
-      for (int k = 0; k < K; k++) acc[k] = r == 0 ? toAcc<T>(x[k]) : applyOp<A>(acc[k], toAcc<T>(x[k]), op);
+      for (int k = 0; k < K; k++) acc[k] = r == 0 ? Scalar<T>::toAcc(x[k]) : applyOp<A>(acc[k], Scalar<T>::toAcc(x[k]), op);
     }
     if (!alive) break;
 #pragma unroll
@@ -341,7 +279,7 @@ llReduceScatterKernel(CommArgs a, const T* in, T* out, size_t per, DevOp op, flo
         if constexpr (std::is_floating_point<A>::value) {
           if (scale != 1.0f) v = static_cast<A>(v * scale);
         }
-        out[u * K + k] = fromAcc<T, A>(v);
+        out[u * K + k] = Scalar<T>::fromAcc(v);
       }
     }
   }
@@ -801,38 +739,23 @@ castAllreduceKernel(CommArgs a, PeerPtrs ins, char* mcIn, PeerPtrs outs, size_t 
     size_t tb, te;
     shareOf(count - tailStart, P, a.rank, tb, te);
     for (size_t i = tailStart + tb + tid; i < tailStart + te; i += nthreads) {
-      float acc = II::toFloat(static_cast<const TI*>(ins.p[0])[i]);
-      for (int r = 1; r < P; r++) acc = applyOp<float>(acc, II::toFloat(static_cast<const TI*>(ins.p[r])[i]), op);
+      float acc = Scalar<TI>::toAcc(static_cast<const TI*>(ins.p[0])[i]);
+      for (int r = 1; r < P; r++) acc = applyOp<float>(acc, Scalar<TI>::toAcc(static_cast<const TI*>(ins.p[r])[i]), op);
       acc *= scale;
-      for (int r = 0; r < P; r++) static_cast<TO*>(outs.p[r])[i] = OI::fromFloat(acc);
+      for (int r = 0; r < P; r++) static_cast<TO*>(outs.p[r])[i] = Scalar<TO>::fromAcc(acc);
     }
   }
   blockBarrier(a, e + 2);
   retire(a, 2, 0);
 }
 
-// ---- host-side launchers ----------------------------------------------------------------
+// ---- kernel selectors -----------------------------------------------------------------------
+// Each selector returns the instantiation that runs for its arguments. The launcher launches it,
+// the ...KernelFor() occupancy queries return it and preloadAllreduceKernels() touches it over
+// the whole argument domain, so all three always name the same kernel. Capability tests are
+// `if constexpr`, so an instantiation that cannot run is never named.
 
 namespace {
-
-template <typename F>
-void dispatchType(DataType dt, F&& f) {
-  switch (dt) {
-    case DataType::INT8: f(int8_t{}); break;
-    case DataType::UINT8: f(uint8_t{}); break;
-    case DataType::INT16: f(int16_t{}); break;
-    case DataType::INT32: f(int32_t{}); break;
-    case DataType::UINT32: f(uint32_t{}); break;
-    case DataType::INT64: f((long long){}); break;
-    case DataType::UINT64: f((unsigned long long){}); break;
-    case DataType::FLOAT32: f(float{}); break;
-    case DataType::FLOAT64: f(double{}); break;
-    case DataType::FLOAT16: f(__half{}); break;
-    case DataType::BFLOAT16: f(__nv_bfloat16{}); break;
-    case DataType::FLOAT8_E4M3: f(__nv_fp8_e4m3{}); break;
-    case DataType::FLOAT8_E5M2: f(__nv_fp8_e5m2{}); break;
-  }
-}
 
 // (input, output) dtype pairs of the cast epilogue: X(input tag, input type, output tag, output type).
 #define GLB_CAST_PAIRS(X)                                      \
@@ -849,6 +772,19 @@ void dispatchType(DataType dt, F&& f) {
   X(BFLOAT16, __nv_bfloat16, FLOAT8_E4M3, __nv_fp8_e4m3)       \
   X(BFLOAT16, __nv_bfloat16, FLOAT8_E5M2, __nv_fp8_e5m2)
 
+// Calls f(TI{}, TO{}) when (in, out) is a cast pair; returns whether it is one.
+template <typename F>
+bool dispatchCast(DataType in, DataType out, F&& f) {
+#define GLB_CAST_CASE(EI, TI, EO, TO)                \
+  if (in == DataType::EI && out == DataType::EO) { \
+    f(TI{}, TO{});                                 \
+    return true;                                   \
+  }
+  GLB_CAST_PAIRS(GLB_CAST_CASE)
+#undef GLB_CAST_CASE
+  return false;
+}
+
 template <typename K>
 const void* fn(K kernel) {
   return reinterpret_cast<const void*>(kernel);
@@ -856,89 +792,85 @@ const void* fn(K kernel) {
 
 // The instantiation of the two-shot kernel for (T, P, unroll); unroll 0 = default for P.
 template <typename T>
-const void* twoShotFn(int P, int unroll) {
+auto twoShotFn(int P, int unroll) {
   if constexpr (PackTraits<T>::kElems > 8) {
     // 16-lane (FP8) packs: one instantiation per P, the ones -Xptxas -v shows free of spills
     // (their 16 fp32 lanes per pack leave no room for <4,2>, <4,4>, <8,1> or <2,8>).
     switch (P) {
-      case 2: return unroll == 1 || unroll == 2 ? fn(twoShotAllreduceKernel<T, 2, 2>) : fn(twoShotAllreduceKernel<T, 2, 4>);
-      case 4: return fn(twoShotAllreduceKernel<T, 4, 1>);
-      case 8: return fn(twoShotAllreduceKernel<T, 8, 2>);
-      default: return fn(twoShotAllreduceKernel<T, 0, 1>);
+      case 2: return unroll == 1 || unroll == 2 ? twoShotAllreduceKernel<T, 2, 2> : twoShotAllreduceKernel<T, 2, 4>;
+      case 4: return twoShotAllreduceKernel<T, 4, 1>;
+      case 8: return twoShotAllreduceKernel<T, 8, 2>;
+      default: return twoShotAllreduceKernel<T, 0, 1>;
     }
   } else if constexpr (isHotType<T>()) {
     switch (P) {
       case 2:
-        if (unroll == 2) return fn(twoShotAllreduceKernel<T, 2, 2>);
-        if (unroll == 8) return fn(twoShotAllreduceKernel<T, 2, 8>);
-        return fn(twoShotAllreduceKernel<T, 2, 4>);
+        if (unroll == 2) return twoShotAllreduceKernel<T, 2, 2>;
+        if (unroll == 8) return twoShotAllreduceKernel<T, 2, 8>;
+        return twoShotAllreduceKernel<T, 2, 4>;
       case 4:
-        if (unroll == 1) return fn(twoShotAllreduceKernel<T, 4, 1>);
-        if (unroll == 4) return fn(twoShotAllreduceKernel<T, 4, 4>);
-        return fn(twoShotAllreduceKernel<T, 4, 2>);
+        if (unroll == 1) return twoShotAllreduceKernel<T, 4, 1>;
+        if (unroll == 4) return twoShotAllreduceKernel<T, 4, 4>;
+        return twoShotAllreduceKernel<T, 4, 2>;
       case 8:
-        if (unroll == 1) return fn(twoShotAllreduceKernel<T, 8, 1>);
-        return fn(twoShotAllreduceKernel<T, 8, 2>);
+        if (unroll == 1) return twoShotAllreduceKernel<T, 8, 1>;
+        return twoShotAllreduceKernel<T, 8, 2>;
       default: break;
     }
   }
-  return fn(twoShotAllreduceKernel<T, 0, 1>);
+  return twoShotAllreduceKernel<T, 0, 1>;
 }
 
+// nullptr where multimem.ld_reduce cannot add T. The NVLS and hybrid kernels' signatures do not
+// depend on T, so the float instantiation can name the return type without instantiating more.
 template <typename T>
-const void* nvlsFn(int unroll) {
-  if (unroll == 2) return fn(nvlsAllreduceKernel<T, 2>);
-  if (unroll == 8) return fn(nvlsAllreduceKernel<T, 8>);
-  return fn(nvlsAllreduceKernel<T, 4>);
+auto nvlsFn(int unroll) -> decltype(&nvlsAllreduceKernel<float, 4>) {
+  if constexpr (hasMultimem<T>()) {
+    if (unroll == 2) return nvlsAllreduceKernel<T, 2>;
+    if (unroll == 8) return nvlsAllreduceKernel<T, 8>;
+    return nvlsAllreduceKernel<T, 4>;
+  }
+  return nullptr;
 }
 
-void launch(const void* kernel, int blocks, int threads, void** args, cudaStream_t stream) {
-  cudaLaunchKernel(kernel, dim3(static_cast<unsigned>(blocks)), dim3(static_cast<unsigned>(threads)), args, 0, stream);
+// nullptr where multimem.ld_reduce cannot add T, or for P outside {2, 4, 8}.
+template <typename T>
+auto hybridFn(int P) -> decltype(&hybridAllreduceKernel<float, 2>) {
+  if constexpr (hasMultimem<T>()) {
+    switch (P) {
+      case 2: return hybridAllreduceKernel<T, 2>;
+      case 4: return hybridAllreduceKernel<T, 4>;
+      case 8: return hybridAllreduceKernel<T, 8>;
+      default: break;
+    }
+  }
+  return nullptr;
 }
 
-}  // namespace
-
-// Force-load every kernel of this file. With CUDA's lazy module loading the first
-// launch of a kernel may have to synchronise the context; if a peer rank on the same
-// device is already spinning inside its collective kernel that launch never happens
-// (documented lazy-loading deadlock for kernels that assume concurrency).
-namespace {
-void touch(const void* kernel) {
-  cudaFuncAttributes attr;
-  cudaFuncGetAttributes(&attr, kernel);
-}
 }  // namespace
 
 void preloadAllreduceKernels() {
-  touch(fn(barrierKernel));
-  for (DataType dt : {DataType::INT8, DataType::UINT8, DataType::INT16, DataType::INT32, DataType::UINT32, DataType::INT64,
-                      DataType::UINT64, DataType::FLOAT32, DataType::FLOAT64, DataType::FLOAT16, DataType::BFLOAT16,
-                      DataType::FLOAT8_E4M3, DataType::FLOAT8_E5M2}) {
+  touchKernel(barrierKernel);
+  for (DataType dt : kAllDataTypes) {
     dispatchType(dt, [&](auto tag) {
       using T = decltype(tag);
-      touch(fn(llAllreduceKernel<T, T>));
-      touch(fn(llReduceScatterKernel<T>));
-      touch(fn(oneShotAllreduceKernel<T>));
-      touch(fn(oneShotPushAllreduceKernel<T>));
-      touch(twoShotFn<T>(0, 0));
-      if constexpr (isHotType<T>()) {
-        for (int P : {2, 4, 8}) {
-          for (int u : {1, 2, 4, 8}) touch(twoShotFn<T>(P, u));
-        }
+      touchKernel(llAllreduceKernel<T, T>);
+      touchKernel(llReduceScatterKernel<T>);
+      touchKernel(oneShotAllreduceKernel<T>);
+      touchKernel(oneShotPushAllreduceKernel<T>);
+      for (int P : {0, 2, 4, 8}) {
+        for (int u : {0, 1, 2, 4, 8}) touchKernel(twoShotFn<T>(P, u));
+        touchKernel(hybridFn<T>(P));
       }
-      if constexpr (hasMultimem<T>()) {
-        for (int u : {2, 4, 8}) touch(nvlsFn<T>(u));
-      }
+      for (int u : {0, 2, 4, 8}) touchKernel(nvlsFn<T>(u));
     });
+    for (DataType out : kAllDataTypes) {
+      dispatchCast(dt, out, [&](auto ti, auto to) {
+        touchKernel(llAllreduceKernel<decltype(ti), decltype(to)>);
+        touchKernel(castAllreduceKernel<decltype(ti), decltype(to)>);
+      });
+    }
   }
-  for (DataType dt : {DataType::FLOAT32, DataType::FLOAT16, DataType::BFLOAT16}) {
-    for (int P : {2, 4, 8}) touch(hybridKernelFor(dt, P));
-  }
-#define GLB_TOUCH_CAST(EI, TI, EO, TO)           \
-  touch(fn(llAllreduceKernel<TI, TO>)); \
-  touch(fn(castAllreduceKernel<TI, TO>));
-  GLB_CAST_PAIRS(GLB_TOUCH_CAST)
-#undef GLB_TOUCH_CAST
   cudaGetLastError();
 }
 
@@ -954,37 +886,25 @@ void launchBarrier(const CommArgs& a, cudaStream_t stream) {
 }
 
 bool castSupported(DataType in, DataType out) {
-  if (in == out) return true;
-#define GLB_IS_CAST(EI, TI, EO, TO) \
-  if (in == DataType::EI && out == DataType::EO) return true;
-  GLB_CAST_PAIRS(GLB_IS_CAST)
-#undef GLB_IS_CAST
-  return false;
+  return in == out || dispatchCast(in, out, [](auto, auto) {});
 }
 
 void launchLLAllreduce(const CommArgs& a, const void* in, void* out, size_t count, DataType dt, DataType outDt,
                        ReduceOp op, float scale, const PeerPtrs& ll, size_t srcStride, size_t parityStride,
                        const LocalPtrs& extra, int blocks, int threads, cudaStream_t stream) {
-  const DevOp dop = static_cast<DevOp>(op);
-#define GLB_LL(TI, TO)                                                                                              \
-  llAllreduceKernel<TI, TO><<<blocks, threads, 0, stream>>>(a, static_cast<const TI*>(in), static_cast<TO*>(out), \
-                                                           count, dop, scale, ll, static_cast<char*>(ll.p[a.rank]), \
-                                                           srcStride, parityStride, extra)
+  auto go = [&](auto ti, auto to) {
+    using TI = decltype(ti);
+    using TO = decltype(to);
+    llAllreduceKernel<TI, TO><<<blocks, threads, 0, stream>>>(a, static_cast<const TI*>(in), static_cast<TO*>(out),
+                                                             count, static_cast<DevOp>(op), scale, ll,
+                                                             static_cast<char*>(ll.p[a.rank]), srcStride, parityStride,
+                                                             extra);
+  };
   if (dt != outDt) {
-#define GLB_LL_CAST(EI, TI, EO, TO)                    \
-  if (dt == DataType::EI && outDt == DataType::EO) { \
-    GLB_LL(TI, TO);                                  \
-    return;                                          \
+    dispatchCast(dt, outDt, go);
+  } else {
+    dispatchType(dt, [&](auto tag) { go(tag, tag); });
   }
-    GLB_CAST_PAIRS(GLB_LL_CAST)
-#undef GLB_LL_CAST
-    return;
-  }
-  dispatchType(dt, [&](auto tag) {
-    using T = decltype(tag);
-    GLB_LL(T, T);
-  });
-#undef GLB_LL
 }
 
 void launchLLReduceScatter(const CommArgs& a, const void* in, void* out, size_t perRank, DataType dt, ReduceOp op,
@@ -1021,98 +941,69 @@ void launchOneShotAllreduce(const CommArgs& a, const void* in, void* out, size_t
 
 const void* twoShotKernelFor(DataType dt, int nranks, int unroll) {
   const void* k = nullptr;
-  dispatchType(dt, [&](auto tag) { k = twoShotFn<decltype(tag)>(nranks, unroll); });
+  dispatchType(dt, [&](auto tag) { k = fn(twoShotFn<decltype(tag)>(nranks, unroll)); });
   return k;
 }
 
 const void* nvlsKernelFor(DataType dt, int unroll) {
-  switch (dt) {
-    case DataType::FLOAT32: return nvlsFn<float>(unroll);
-    case DataType::FLOAT16: return nvlsFn<__half>(unroll);
-    case DataType::BFLOAT16: return nvlsFn<__nv_bfloat16>(unroll);
-    default: return nullptr;
-  }
+  const void* k = nullptr;
+  dispatchType(dt, [&](auto tag) { k = fn(nvlsFn<decltype(tag)>(unroll)); });
+  return k;
+}
+
+const void* hybridKernelFor(DataType dt, int nranks) {
+  const void* k = nullptr;
+  dispatchType(dt, [&](auto tag) { k = fn(hybridFn<decltype(tag)>(nranks)); });
+  return k;
+}
+
+const void* castKernelFor(DataType in, DataType out) {
+  const void* k = nullptr;
+  dispatchCast(in, out, [&](auto ti, auto to) { k = fn(castAllreduceKernel<decltype(ti), decltype(to)>); });
+  return k;
 }
 
 void launchTwoShotAllreduce(const CommArgs& a, const PeerPtrs& bufs, size_t count, DataType dt, ReduceOp op,
                             float scale, bool vectorOk, const LocalPtrs& extra, const LaunchCfg& cfg,
                             cudaStream_t stream) {
-  DevOp dop = static_cast<DevOp>(op);
-  CommArgs ca = a;
-  PeerPtrs pb = bufs;
-  LocalPtrs ex = extra;
-  void* args[] = {&ca, &pb, &count, &dop, &scale, &vectorOk, &ex};
-  launch(twoShotKernelFor(dt, a.nranks, cfg.unroll), cfg.blocks, kThreads, args, stream);
+  dispatchType(dt, [&](auto tag) {
+    twoShotFn<decltype(tag)>(a.nranks, cfg.unroll)<<<cfg.blocks, kThreads, 0, stream>>>(
+        a, bufs, count, static_cast<DevOp>(op), scale, vectorOk, extra);
+  });
 }
 
 // multimem.ld_reduce has no e4m3 / e5m2 form on sm_90a: FP8 never takes the NVLS paths.
 bool nvlsSupports(DataType dt, ReduceOp op) {
-  return op == ReduceOp::SUM && (dt == DataType::FLOAT32 || dt == DataType::FLOAT16 || dt == DataType::BFLOAT16);
+  bool ok = false;
+  dispatchType(dt, [&](auto tag) { ok = hasMultimem<decltype(tag)>(); });
+  return op == ReduceOp::SUM && ok;
 }
 
 void launchNvlsAllreduce(const CommArgs& a, void* mcPtr, const PeerPtrs& bufs, size_t count, DataType dt, float scale,
                          const LocalPtrs& extra, const LaunchCfg& cfg, cudaStream_t stream) {
-  const void* k = nvlsKernelFor(dt, cfg.unroll);
-  if (k == nullptr) return;
-  CommArgs ca = a;
-  char* mc = static_cast<char*>(mcPtr);
-  PeerPtrs pb = bufs;
-  LocalPtrs ex = extra;
-  void* args[] = {&ca, &mc, &pb, &count, &scale, &ex};
-  launch(k, cfg.blocks, kThreads, args, stream);
-}
-
-namespace {
-template <typename T>
-const void* hybridFn(int P) {
-  switch (P) {
-    case 2: return fn(hybridAllreduceKernel<T, 2>);
-    case 4: return fn(hybridAllreduceKernel<T, 4>);
-    case 8: return fn(hybridAllreduceKernel<T, 8>);
-    default: return nullptr;
-  }
-}
-}  // namespace
-
-const void* hybridKernelFor(DataType dt, int nranks) {
-  switch (dt) {
-    case DataType::FLOAT32: return hybridFn<float>(nranks);
-    case DataType::FLOAT16: return hybridFn<__half>(nranks);
-    case DataType::BFLOAT16: return hybridFn<__nv_bfloat16>(nranks);
-    default: return nullptr;
-  }
+  dispatchType(dt, [&](auto tag) {
+    if (auto k = nvlsFn<decltype(tag)>(cfg.unroll)) {
+      k<<<cfg.blocks, kThreads, 0, stream>>>(a, static_cast<char*>(mcPtr), bufs, count, scale, extra);
+    }
+  });
 }
 
 void launchHybridAllreduce(const CommArgs& a, void* mcPtr, const PeerPtrs& bufs, size_t count, DataType dt, float scale,
                            int blocks, int nvlsBlocks, unsigned p2pPermille, cudaStream_t stream) {
-  const void* k = hybridKernelFor(dt, a.nranks);
-  if (k == nullptr) return;
-  CommArgs ca = a;
-  char* mc = static_cast<char*>(mcPtr);
-  PeerPtrs pb = bufs;
-  void* args[] = {&ca, &mc, &pb, &count, &scale, &nvlsBlocks, &p2pPermille};
-  launch(k, blocks, kThreads, args, stream);
-}
-
-const void* castKernelFor(DataType in, DataType out) {
-#define GLB_CAST_FN(EI, TI, EO, TO) \
-  if (in == DataType::EI && out == DataType::EO) return fn(castAllreduceKernel<TI, TO>);
-  GLB_CAST_PAIRS(GLB_CAST_FN)
-#undef GLB_CAST_FN
-  return nullptr;
+  dispatchType(dt, [&](auto tag) {
+    if (auto k = hybridFn<decltype(tag)>(a.nranks)) {
+      k<<<blocks, kThreads, 0, stream>>>(a, static_cast<char*>(mcPtr), bufs, count, scale, nvlsBlocks, p2pPermille);
+    }
+  });
 }
 
 void launchCastAllreduce(const CommArgs& a, const PeerPtrs& ins, void* mcIn, const PeerPtrs& outs, size_t count,
                          DataType dt, DataType outDt, ReduceOp op, float scale, bool vectorOk, int blocks,
                          cudaStream_t stream) {
-  const void* k = castKernelFor(dt, outDt);
-  if (k == nullptr) return;
-  CommArgs ca = a;
-  PeerPtrs pi = ins, po = outs;
-  char* mc = static_cast<char*>(mcIn);
-  DevOp dop = static_cast<DevOp>(op);
-  void* args[] = {&ca, &pi, &mc, &po, &count, &dop, &scale, &vectorOk};
-  launch(k, blocks, kThreads, args, stream);
+  dispatchCast(dt, outDt, [&](auto ti, auto to) {
+    castAllreduceKernel<decltype(ti), decltype(to)><<<blocks, kThreads, 0, stream>>>(
+        a, ins, static_cast<char*>(mcIn), outs, count, static_cast<DevOp>(op), scale, vectorOk);
+  });
 }
 
 }  // namespace cuda

@@ -3,7 +3,6 @@
 // single kernels bracketed by device-side flag barriers; payload moves with
 // 128-bit peer loads/stores (or multimem.st through the NVSwitch where a multicast
 // alias exists). None of these has a CUDA variant in the reference (SURVEY §0.6).
-#include "glb/cuda/bulk_copy.cuh"
 #include "glb/cuda/device_common.cuh"
 #include "glb/cuda/kernels.h"
 
@@ -398,61 +397,12 @@ gatherPushKernel(CommArgs a, const char* __restrict__ in, PeerPtrs outs, char* m
   retire(a, 2, 0);
 }
 
-// Same protocol (two barriers, same CTA count) with the payload moved by the TMA: every CTA loads
-// its slice of my block into shared memory ONCE (cp.async.bulk) and stores it to every peer from
-// there; one thread per CTA issues, no data passes through registers.
-__global__ void __launch_bounds__(128)
-gatherBulkKernel(CommArgs a, const char* __restrict__ in, PeerPtrs outs, VArgs va, int onlyDst) {
-  extern __shared__ __align__(128) char smem[];
-  __shared__ BulkRing ring;
-  bulkRingInit(ring);
-  const uint32_t e = loadEpoch(a);
-  const int P = a.nranks;
-  if (!blockBarrier<false>(a, e + 1)) {
-    retire(a, 2, 0);
-    return;
-  }
-  const size_t off = va.off[a.rank], len = va.len[a.rank];
-  const size_t units = len / 16;
-  const size_t per = (units + gridDim.x - 1) / gridDim.x;
-  const size_t lo = static_cast<size_t>(blockIdx.x) * per, hi = lo + per < units ? lo + per : units;
-  char* dst[kMaxRanks];
-  int ndst = 0;
-#pragma unroll
-  for (int i = 0; i < kMaxRanks; i++) {
-    dst[i] = nullptr;
-    if (onlyDst < 0 && i < P) dst[ndst++] = static_cast<char*>(outs.p[(a.rank + i) % P]) + off + lo * 16;
-  }
-  if (onlyDst >= 0) dst[ndst++] = static_cast<char*>(outs.p[onlyDst]) + off + lo * 16;
-  if (lo < hi) ctaBulkCopy<kMaxRanks>(ring, smem, in + lo * 16, dst, ndst, (hi - lo) * 16);
-  if (blockIdx.x == 0) {  // sub-16-byte tail
-    for (size_t i = units * 16 + threadIdx.x; i < len; i += blockDim.x) {
-      const char c = in[i];
-      if (onlyDst >= 0) {
-        (static_cast<char*>(outs.p[onlyDst]) + off)[i] = c;
-      } else {
-        for (int r = 0; r < P; r++) (static_cast<char*>(outs.p[r]) + off)[i] = c;
-      }
-    }
-  }
-  blockBarrier(a, e + 2);
-  retire(a, 2, 0);
-}
-
 void launchGatherPush(const CommArgs& a, const void* in, const PeerPtrs& outs, void* mcOut, const size_t* offs,
-                      const size_t* lens, int onlyDst, bool vec, int blocks, cudaStream_t stream, bool tma) {
+                      const size_t* lens, int onlyDst, bool vec, int blocks, cudaStream_t stream) {
   VArgs va;
   for (int i = 0; i < kMaxRanks; i++) {
     va.off[i] = i < a.nranks ? offs[i] : 0;
     va.len[i] = i < a.nranks ? lens[i] : 0;
-  }
-  // The TMA variant needs 16-byte aligned source, offset and destinations; a rank whose
-  // pointers do not qualify runs the LDG/STG kernel with the SAME grid and barrier protocol.
-  bool aligned = vec && reinterpret_cast<uintptr_t>(in) % 16 == 0 && va.off[a.rank] % 16 == 0 && mcOut == nullptr;
-  for (int i = 0; i < a.nranks; i++) aligned = aligned && reinterpret_cast<uintptr_t>(outs.p[i]) % 16 == 0;
-  if (tma && aligned) {
-    gatherBulkKernel<<<blocks, 128, kBulkSmemBytes, stream>>>(a, static_cast<const char*>(in), outs, va, onlyDst);
-    return;
   }
   gatherPushKernel<<<blocks, kThreads, 0, stream>>>(a, static_cast<const char*>(in), outs, static_cast<char*>(mcOut),
                                                     va, onlyDst, vec);
@@ -990,18 +940,15 @@ reducePullKernel(CommArgs a, PeerPtrs ins, char* mcIn, T* __restrict__ out, EArg
 }
 
 namespace {
+// The reduce-pull instantiation for (T, P).
 template <typename T>
-void launchReducePullT(const CommArgs& a, const PeerPtrs& ins, char* mc, void* out, const EArgs& ea, DevOp dop,
-                       float scale, bool vec, bool useMc, int blocks, cudaStream_t stream) {
+auto reducePullFn(int nranks) {
   if constexpr (isHotType<T>()) {
-    switch (a.nranks) {
-      case 2: reducePullKernel<T, 2, 4><<<blocks, kThreads, 0, stream>>>(a, ins, mc, static_cast<T*>(out), ea, dop, scale, vec, useMc); return;
-      case 4: reducePullKernel<T, 4, 2><<<blocks, kThreads, 0, stream>>>(a, ins, mc, static_cast<T*>(out), ea, dop, scale, vec, useMc); return;
-      case 8: reducePullKernel<T, 8, 2><<<blocks, kThreads, 0, stream>>>(a, ins, mc, static_cast<T*>(out), ea, dop, scale, vec, useMc); return;
-      default: break;
-    }
+    if (nranks == 2) return reducePullKernel<T, 2, 4>;
+    if (nranks == 4) return reducePullKernel<T, 4, 2>;
+    if (nranks == 8) return reducePullKernel<T, 8, 2>;
   }
-  reducePullKernel<T, 0, 1><<<blocks, kThreads, 0, stream>>>(a, ins, mc, static_cast<T*>(out), ea, dop, scale, vec, useMc);
+  return reducePullKernel<T, 0, 1>;
 }
 }  // namespace
 
@@ -1013,30 +960,12 @@ void launchReducePull(const CommArgs& a, const PeerPtrs& ins, void* mcIn, void* 
     ea.off[i] = i < a.nranks ? elemOff[i] : 0;
     ea.len[i] = i < a.nranks ? elemLen[i] : 0;
   }
-  const DevOp dop = static_cast<DevOp>(op);
-  char* mc = static_cast<char*>(mcIn);
-#define GLB_CASE(E, T)                                                              \
-  case DataType::E:                                                                 \
-    launchReducePullT<T>(a, ins, mc, out, ea, dop, scale, vec, useMc, blocks, stream);     \
-    break;
-  switch (dt) {
-    GLB_CASE(INT8, int8_t)
-    GLB_CASE(UINT8, uint8_t)
-    GLB_CASE(INT16, int16_t)
-    GLB_CASE(INT32, int32_t)
-    GLB_CASE(UINT32, uint32_t)
-    GLB_CASE(INT64, long long)
-    GLB_CASE(UINT64, unsigned long long)
-    GLB_CASE(FLOAT32, float)
-    GLB_CASE(FLOAT64, double)
-    GLB_CASE(FLOAT16, __half)
-    GLB_CASE(BFLOAT16, __nv_bfloat16)
-    GLB_CASE(FLOAT8_E4M3, __nv_fp8_e4m3)
-    GLB_CASE(FLOAT8_E5M2, __nv_fp8_e5m2)
-  }
-#undef GLB_CASE
+  dispatchType(dt, [&](auto tag) {
+    using T = decltype(tag);
+    reducePullFn<T>(a.nranks)<<<blocks, kThreads, 0, stream>>>(a, ins, static_cast<char*>(mcIn), static_cast<T*>(out),
+                                                               ea, static_cast<DevOp>(op), scale, vec, useMc);
+  });
 }
-
 
 // ---- small allgather / alltoall without a barrier: flag-in-data lines -------------------------
 // Same protocol and pool region as llAllreduceKernel (every rank hears from every peer in a
@@ -1116,63 +1045,25 @@ void launchLLExchange(const CommArgs& a, const void* in, void* out, size_t bytes
 
 const void* broadcastKernelPtr() { return reinterpret_cast<const void*>(broadcastKernel); }
 const void* gatherPushKernelPtr() { return reinterpret_cast<const void*>(gatherPushKernel); }
-const void* gatherBulkKernelPtr() { return reinterpret_cast<const void*>(gatherBulkKernel); }
 const void* alltoallPushKernelPtr() { return reinterpret_cast<const void*>(alltoallPushKernel); }
 const void* alltoallvDevKernelPtr() { return reinterpret_cast<const void*>(alltoallvDevKernel); }
 const void* reducePullKernelPtr(DataType dt, int nranks) {
-#define GLB_RP(E, T)                                                                                   \
-  case DataType::E: {                                                                                  \
-    if constexpr (isHotType<T>()) {                                                                    \
-      if (nranks == 2) return reinterpret_cast<const void*>(reducePullKernel<T, 2, 4>);                \
-      if (nranks == 4) return reinterpret_cast<const void*>(reducePullKernel<T, 4, 2>);                \
-      if (nranks == 8) return reinterpret_cast<const void*>(reducePullKernel<T, 8, 2>);                \
-    }                                                                                                  \
-    return reinterpret_cast<const void*>(reducePullKernel<T, 0, 1>);                                   \
-  }
-  switch (dt) {
-    GLB_RP(INT8, int8_t)
-    GLB_RP(UINT8, uint8_t)
-    GLB_RP(INT16, int16_t)
-    GLB_RP(INT32, int32_t)
-    GLB_RP(UINT32, uint32_t)
-    GLB_RP(INT64, long long)
-    GLB_RP(UINT64, unsigned long long)
-    GLB_RP(FLOAT32, float)
-    GLB_RP(FLOAT64, double)
-    GLB_RP(FLOAT16, __half)
-    GLB_RP(BFLOAT16, __nv_bfloat16)
-    GLB_RP(FLOAT8_E4M3, __nv_fp8_e4m3)
-    GLB_RP(FLOAT8_E5M2, __nv_fp8_e5m2)
-  }
-#undef GLB_RP
-  return nullptr;
+  const void* k = nullptr;
+  dispatchType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(reducePullFn<decltype(tag)>(nranks)); });
+  return k;
 }
 
 void preloadCollectiveKernels() {
-  auto touch = [](const void* k) {
-    cudaFuncAttributes attr;
-    cudaFuncGetAttributes(&attr, k);
-  };
-  touch(reinterpret_cast<const void*>(broadcastKernel));
-  touch(reinterpret_cast<const void*>(gatherPushKernel));
-  cudaFuncSetAttribute(reinterpret_cast<const void*>(gatherBulkKernel), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       static_cast<int>(kBulkSmemBytes));
-  touch(reinterpret_cast<const void*>(gatherBulkKernel));
-  touch(reinterpret_cast<const void*>(alltoallPushKernel));
-  touch(reinterpret_cast<const void*>(alltoallvDevKernel));
-  touch(reinterpret_cast<const void*>(llExchangeKernel));
-#define GLB_TOUCH_RP(T) touch(reinterpret_cast<const void*>(reducePullKernel<T, 0, 1>));
-  GLB_TOUCH_RP(int8_t) GLB_TOUCH_RP(uint8_t) GLB_TOUCH_RP(int16_t) GLB_TOUCH_RP(int32_t) GLB_TOUCH_RP(uint32_t)
-  GLB_TOUCH_RP(long long) GLB_TOUCH_RP(unsigned long long) GLB_TOUCH_RP(float) GLB_TOUCH_RP(double)
-  GLB_TOUCH_RP(__half) GLB_TOUCH_RP(__nv_bfloat16) GLB_TOUCH_RP(__nv_fp8_e4m3) GLB_TOUCH_RP(__nv_fp8_e5m2)
-#undef GLB_TOUCH_RP
-#define GLB_TOUCH_HOT(T)                                                   \
-  touch(reinterpret_cast<const void*>(reducePullKernel<T, 2, 4>));         \
-  touch(reinterpret_cast<const void*>(reducePullKernel<T, 4, 2>));         \
-  touch(reinterpret_cast<const void*>(reducePullKernel<T, 8, 2>));
-  GLB_TOUCH_HOT(float) GLB_TOUCH_HOT(__half) GLB_TOUCH_HOT(__nv_bfloat16)
-  GLB_TOUCH_HOT(__nv_fp8_e4m3) GLB_TOUCH_HOT(__nv_fp8_e5m2)
-#undef GLB_TOUCH_HOT
+  touchKernel(broadcastKernel);
+  touchKernel(gatherPushKernel);
+  touchKernel(alltoallPushKernel);
+  touchKernel(alltoallvDevKernel);
+  touchKernel(llExchangeKernel);
+  for (DataType dt : kAllDataTypes) {
+    dispatchType(dt, [&](auto tag) {
+      for (int P : {0, 2, 4, 8}) touchKernel(reducePullFn<decltype(tag)>(P));
+    });
+  }
   cudaGetLastError();
 }
 

@@ -58,7 +58,7 @@ struct Tuning {
   size_t bcastRelayMinBytes = 64u << 20;    // >= : chunk-pipelined relay broadcast (P > 2)
   int pipeTile = 1024;                  // 16-byte groups per tile of the pipelined kernel (power of two)
   int pipeExchangeThreads = 256;        // threads of each CTA that drive NVLink in the pipelined kernel
-  bool tmaCopies = false;               // put / get / large allgather through cp.async.bulk (TMA) instead of LDG/STG
+  bool tmaCopies = false;               // put / get / exchange through cp.async.bulk (TMA) instead of LDG/STG
                                         // when no table entry decides (GLB_CUDA_TMA)
 };
 Tuning& tuning();

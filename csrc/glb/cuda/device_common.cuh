@@ -389,6 +389,37 @@ __device__ __forceinline__ T floatToFp8(float x) {
   return r;
 }
 
+// One element of T as its fp32 value (16-bit and FP8 types) or as itself (every other type),
+// and back: widening is exact, narrowing rounds to nearest even (FP8 also saturates).
+template <typename T>
+struct Scalar {
+  using Acc = T;
+  __device__ static T toAcc(T x) { return x; }
+  __device__ static T fromAcc(T x) { return x; }
+};
+template <>
+struct Scalar<__half> {
+  using Acc = float;
+  __device__ static float toAcc(__half x) { return __half2float(x); }
+  __device__ static __half fromAcc(float x) { return __float2half_rn(x); }
+};
+template <>
+struct Scalar<__nv_bfloat16> {
+  using Acc = float;
+  __device__ static float toAcc(__nv_bfloat16 x) { return __bfloat162float(x); }
+  __device__ static __nv_bfloat16 fromAcc(float x) { return __float2bfloat16_rn(x); }
+};
+template <typename T>
+struct Fp8Scalar {
+  using Acc = float;
+  __device__ static float toAcc(T x) { return fp8ToFloat(x); }
+  __device__ static T fromAcc(float x) { return floatToFp8<T>(x); }
+};
+template <>
+struct Scalar<__nv_fp8_e4m3> : Fp8Scalar<__nv_fp8_e4m3> {};
+template <>
+struct Scalar<__nv_fp8_e5m2> : Fp8Scalar<__nv_fp8_e5m2> {};
+
 template <typename T>
 struct Fp8PackTraits {
   static constexpr int kElems = 16;
@@ -457,8 +488,8 @@ struct TailAcc {
 template <typename T>
 struct Fp8TailAcc {
   using type = float;
-  __device__ static float load(T x) { return fp8ToFloat(x); }
-  __device__ static T store(float x) { return floatToFp8<T>(x); }
+  __device__ static float load(T x) { return Scalar<T>::toAcc(x); }
+  __device__ static T store(float x) { return Scalar<T>::fromAcc(x); }
   __device__ static float combine(float a, float b, DevOp op) { return applyOp<float>(a, b, op); }
   __device__ static float scale(float a, float s) { return a * s; }
 };
@@ -506,8 +537,6 @@ struct Item8<float> {
     st128_stream(p, a);
     st128_stream(static_cast<char*>(p) + 16, b);
   }
-  __device__ static float toFloat(float x) { return x; }
-  __device__ static float fromFloat(float x) { return x; }
 };
 template <>
 struct Item8<__half> {
@@ -523,8 +552,6 @@ struct Item8<__half> {
     for (int i = 0; i < 8; i++) a.v[i] = v[i];
     st128_stream(p, PackTraits<__half>::narrow(a));
   }
-  __device__ static float toFloat(__half x) { return __half2float(x); }
-  __device__ static __half fromFloat(float x) { return __float2half_rn(x); }
 };
 template <>
 struct Item8<__nv_bfloat16> {
@@ -540,8 +567,6 @@ struct Item8<__nv_bfloat16> {
     for (int i = 0; i < 8; i++) a.v[i] = v[i];
     st128_stream(p, PackTraits<__nv_bfloat16>::narrow(a));
   }
-  __device__ static float toFloat(__nv_bfloat16 x) { return __bfloat162float(x); }
-  __device__ static __nv_bfloat16 fromFloat(float x) { return __float2bfloat16_rn(x); }
 };
 
 // FP8: 8 elements are 8 bytes (one 64-bit access).
@@ -566,8 +591,6 @@ struct Fp8Item8 {
     x.y = float2ToFp8x2<T>(v[4], v[5]) | (float2ToFp8x2<T>(v[6], v[7]) << 16);
     *static_cast<uint2*>(p) = x;
   }
-  __device__ static float toFloat(T x) { return fp8ToFloat(x); }
-  __device__ static T fromFloat(float x) { return floatToFp8<T>(x); }
 };
 template <>
 struct Item8<__nv_fp8_e4m3> : Fp8Item8<__nv_fp8_e4m3> {};
@@ -621,22 +644,47 @@ __device__ __forceinline__ void multimemSt128(void* mc, const Pack16& v) {
                : "memory");
 }
 
-// Map the public dtype tags to device element types.
-template <DataType D>
-struct DevType;
-template <> struct DevType<DataType::INT8> { using type = int8_t; };
-template <> struct DevType<DataType::UINT8> { using type = uint8_t; };
-template <> struct DevType<DataType::INT16> { using type = int16_t; };
-template <> struct DevType<DataType::INT32> { using type = int32_t; };
-template <> struct DevType<DataType::UINT32> { using type = uint32_t; };
-template <> struct DevType<DataType::INT64> { using type = long long; };
-template <> struct DevType<DataType::UINT64> { using type = unsigned long long; };
-template <> struct DevType<DataType::FLOAT32> { using type = float; };
-template <> struct DevType<DataType::FLOAT64> { using type = double; };
-template <> struct DevType<DataType::FLOAT16> { using type = __half; };
-template <> struct DevType<DataType::BFLOAT16> { using type = __nv_bfloat16; };
-template <> struct DevType<DataType::FLOAT8_E4M3> { using type = __nv_fp8_e4m3; };
-template <> struct DevType<DataType::FLOAT8_E5M2> { using type = __nv_fp8_e5m2; };
+// ---- host side: dtype dispatch and kernel preloading ----------------------------------
+
+// Calls f(T{}) with the device element type T of dt. Each kernel family picks its
+// instantiation from T in one selector, which the launcher, the occupancy query and the
+// preload all call.
+template <typename F>
+void dispatchType(DataType dt, F&& f) {
+  switch (dt) {
+    case DataType::INT8: f(int8_t{}); break;
+    case DataType::UINT8: f(uint8_t{}); break;
+    case DataType::INT16: f(int16_t{}); break;
+    case DataType::INT32: f(int32_t{}); break;
+    case DataType::UINT32: f(uint32_t{}); break;
+    case DataType::INT64: f(0LL); break;
+    case DataType::UINT64: f(0ULL); break;
+    case DataType::FLOAT32: f(float{}); break;
+    case DataType::FLOAT64: f(double{}); break;
+    case DataType::FLOAT16: f(__half{}); break;
+    case DataType::BFLOAT16: f(__nv_bfloat16{}); break;
+    case DataType::FLOAT8_E4M3: f(__nv_fp8_e4m3{}); break;
+    case DataType::FLOAT8_E5M2: f(__nv_fp8_e5m2{}); break;
+  }
+}
+
+constexpr DataType kAllDataTypes[] = {DataType::INT8,    DataType::UINT8,       DataType::INT16,      DataType::INT32,
+                                      DataType::UINT32,  DataType::INT64,       DataType::UINT64,     DataType::FLOAT32,
+                                      DataType::FLOAT64, DataType::FLOAT16,     DataType::BFLOAT16,   DataType::FLOAT8_E4M3,
+                                      DataType::FLOAT8_E5M2};
+
+// Force-load one kernel. With CUDA's lazy module loading the first launch of a kernel may
+// have to synchronise the context; if a peer rank on the same device is already spinning
+// inside its collective kernel, that launch never happens (DESIGN.md, "Running ranks that
+// share one GPU"). So the preload*Kernels() functions touch every kernel a launcher can start,
+// by calling each selector over its whole domain (a selector returns nullptr for arguments
+// that have no kernel).
+template <typename K>
+void touchKernel(K kernel) {
+  if (kernel == nullptr) return;
+  cudaFuncAttributes attr;
+  cudaFuncGetAttributes(&attr, reinterpret_cast<const void*>(kernel));
+}
 
 }  // namespace cuda
 }  // namespace glb

@@ -63,7 +63,7 @@ void launchPipelinedAllreduce(const CommArgs& a, const void* in, void* out, size
 void launchBroadcast(const CommArgs& a, const PeerPtrs& bufs, void* mc, size_t bytes, int root, int mode, bool vec,
                      int blocks, int tile, cudaStream_t stream);
 void launchGatherPush(const CommArgs& a, const void* in, const PeerPtrs& outs, void* mcOut, const size_t* offs,
-                      const size_t* lens, int onlyDst, bool vec, int blocks, cudaStream_t stream, bool tma = false);
+                      const size_t* lens, int onlyDst, bool vec, int blocks, cudaStream_t stream);
 void launchAlltoallPush(const CommArgs& a, const void* in, const PeerPtrs& outs, const size_t* sendOff,
                         const size_t* sendLen, const size_t* dstOff, const size_t* recvOffTable, int onlySrc,
                         bool vec, int blocks, cudaStream_t stream);
@@ -82,7 +82,6 @@ void launchAlltoallvDev(const CommArgs& a, const PeerPtrs& outs, const void* in,
 const void* alltoallvDevKernelPtr();
 const void* broadcastKernelPtr();
 const void* gatherPushKernelPtr();
-const void* gatherBulkKernelPtr();
 const void* alltoallPushKernelPtr();
 const void* reducePullKernelPtr(DataType dt, int nranks);
 // Flag-in-data exchange for small messages (no barrier): mode 0 = allgather (my block to

@@ -254,51 +254,34 @@ pipelinedAllreduceKernel(CommArgs a, const T* in, T* out, size_t count, DevOp op
 }
 
 namespace {
+// The pipelined instantiation for (T, multicast stage, P).
 template <typename T>
-const void* pipeFn(bool mc, int nranks) {
+auto pipeFn(bool mc, int nranks) {
   if constexpr (hasMultimem<T>()) {
-    if (mc) return reinterpret_cast<const void*>(pipelinedAllreduceKernel<T, true, 0>);
+    if (mc) return pipelinedAllreduceKernel<T, true, 0>;
   }
   if constexpr (isHotType<T>()) {
-    if (nranks == 2) return reinterpret_cast<const void*>(pipelinedAllreduceKernel<T, false, 2>);
-    if (nranks == 4) return reinterpret_cast<const void*>(pipelinedAllreduceKernel<T, false, 4>);
-    if (nranks == 8) return reinterpret_cast<const void*>(pipelinedAllreduceKernel<T, false, 8>);
+    if (nranks == 2) return pipelinedAllreduceKernel<T, false, 2>;
+    if (nranks == 4) return pipelinedAllreduceKernel<T, false, 4>;
+    if (nranks == 8) return pipelinedAllreduceKernel<T, false, 8>;
   }
-  return reinterpret_cast<const void*>(pipelinedAllreduceKernel<T, false, 0>);
-}
-
-const void* pipeKernelForImpl(DataType dt, bool mc, int nranks) {
-  switch (dt) {
-    case DataType::INT8: return pipeFn<int8_t>(false, nranks);
-    case DataType::UINT8: return pipeFn<uint8_t>(false, nranks);
-    case DataType::INT16: return pipeFn<int16_t>(false, nranks);
-    case DataType::INT32: return pipeFn<int32_t>(false, nranks);
-    case DataType::UINT32: return pipeFn<uint32_t>(false, nranks);
-    case DataType::INT64: return pipeFn<long long>(false, nranks);
-    case DataType::UINT64: return pipeFn<unsigned long long>(false, nranks);
-    case DataType::FLOAT32: return pipeFn<float>(mc, nranks);
-    case DataType::FLOAT64: return pipeFn<double>(false, nranks);
-    case DataType::FLOAT16: return pipeFn<__half>(mc, nranks);
-    case DataType::BFLOAT16: return pipeFn<__nv_bfloat16>(mc, nranks);
-    case DataType::FLOAT8_E4M3: return pipeFn<__nv_fp8_e4m3>(false, nranks);
-    case DataType::FLOAT8_E5M2: return pipeFn<__nv_fp8_e5m2>(false, nranks);
-  }
-  return nullptr;
+  return pipelinedAllreduceKernel<T, false, 0>;
 }
 }  // namespace
 
-const void* pipelinedKernelFor(DataType dt, bool mc, int nranks) { return pipeKernelForImpl(dt, mc, nranks); }
+const void* pipelinedKernelFor(DataType dt, bool mc, int nranks) {
+  const void* k = nullptr;
+  dispatchType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(pipeFn<decltype(tag)>(mc, nranks)); });
+  return k;
+}
 
 void preloadPipelineKernels() {
-  for (DataType dt : {DataType::INT8, DataType::UINT8, DataType::INT16, DataType::INT32, DataType::UINT32, DataType::INT64,
-                      DataType::UINT64, DataType::FLOAT32, DataType::FLOAT64, DataType::FLOAT16, DataType::BFLOAT16,
-                      DataType::FLOAT8_E4M3, DataType::FLOAT8_E5M2}) {
-    for (bool mc : {false, true}) {
-      for (int nr : {0, 2, 4, 8}) {
-        cudaFuncAttributes attr;
-        cudaFuncGetAttributes(&attr, pipeKernelForImpl(dt, mc, nr));
+  for (DataType dt : kAllDataTypes) {
+    dispatchType(dt, [](auto tag) {
+      for (bool mc : {false, true}) {
+        for (int nr : {0, 2, 4, 8}) touchKernel(pipeFn<decltype(tag)>(mc, nr));
       }
-    }
+    });
   }
   cudaGetLastError();
 }
@@ -307,14 +290,13 @@ void launchPipelinedAllreduce(const CommArgs& a, const void* in, void* out, size
                               float scale, const PeerPtrs& stage, void* mcStage, int tileVecs, int exchangeThreads,
                               const LocalPtrs& extra, int blocks, cudaStream_t stream) {
   const bool mc = mcStage != nullptr && nvlsSupports(dt, op);
-  const void* k = pipeKernelForImpl(dt, mc, a.nranks);
-  CommArgs ca = a;
-  PeerPtrs st = stage;
-  LocalPtrs ex = extra;
-  char* mcp = mc ? static_cast<char*>(mcStage) : nullptr;
-  DevOp dop = static_cast<DevOp>(op);
-  void* args[] = {&ca, &in, &out, &count, &dop, &scale, &st, &mcp, &tileVecs, &exchangeThreads, &ex};
-  cudaLaunchKernel(k, dim3(static_cast<unsigned>(blocks)), dim3(kThreads), args, 0, stream);
+  dispatchType(dt, [&](auto tag) {
+    using T = decltype(tag);
+    pipeFn<T>(mc, a.nranks)<<<blocks, kThreads, 0, stream>>>(a, static_cast<const T*>(in), static_cast<T*>(out), count,
+                                                             static_cast<DevOp>(op), scale, stage,
+                                                             mc ? static_cast<char*>(mcStage) : nullptr, tileVecs,
+                                                             exchangeThreads, extra);
+  });
 }
 
 }  // namespace cuda

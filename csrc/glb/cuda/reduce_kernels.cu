@@ -196,16 +196,7 @@ __global__ void verifyKernel(const T* buf, size_t count, double start, double st
   unsigned long long bad = 0;
   for (size_t i = tid; i < count; i += nthreads) {
     const double want = start + stride * static_cast<double>(i);
-    double got;
-    if constexpr (std::is_same<T, __half>::value) {
-      got = static_cast<double>(__half2float(buf[i]));
-    } else if constexpr (std::is_same<T, __nv_bfloat16>::value) {
-      got = static_cast<double>(__bfloat162float(buf[i]));
-    } else if constexpr (isFp8Type<T>()) {
-      got = static_cast<double>(fp8ToFloat(buf[i]));
-    } else {
-      got = static_cast<double>(buf[i]);
-    }
+    const double got = static_cast<double>(Scalar<T>::toAcc(buf[i]));
     const double err = fabs(got - want);
     if (!(err <= atol + rtol * fabs(want))) {
       bad++;
@@ -236,15 +227,7 @@ __global__ void fillKernel(T* dst, size_t count, double start, double stride) {
   const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
   for (size_t i = tid; i < count; i += nthreads) {
     const double v = start + stride * static_cast<double>(i);
-    if constexpr (std::is_same<T, __half>::value) {
-      dst[i] = __float2half_rn(static_cast<float>(v));
-    } else if constexpr (std::is_same<T, __nv_bfloat16>::value) {
-      dst[i] = __float2bfloat16_rn(static_cast<float>(v));
-    } else if constexpr (isFp8Type<T>()) {
-      dst[i] = floatToFp8<T>(static_cast<float>(v));
-    } else {
-      dst[i] = static_cast<T>(v);
-    }
+    dst[i] = Scalar<T>::fromAcc(static_cast<typename Scalar<T>::Acc>(v));
   }
 }
 
@@ -309,23 +292,17 @@ int gridFor(size_t items, int threads, int ctasPerSm = 4) {
   return static_cast<int>(want < 1 ? 1 : (want > cap ? cap : want));
 }
 
-template <typename F>
-void dispatchType(DataType dt, F&& f) {
-  switch (dt) {
-    case DataType::INT8: f(int8_t{}); break;
-    case DataType::UINT8: f(uint8_t{}); break;
-    case DataType::INT16: f(int16_t{}); break;
-    case DataType::INT32: f(int32_t{}); break;
-    case DataType::UINT32: f(uint32_t{}); break;
-    case DataType::INT64: f((long long){}); break;
-    case DataType::UINT64: f((unsigned long long){}); break;
-    case DataType::FLOAT32: f(float{}); break;
-    case DataType::FLOAT64: f(double{}); break;
-    case DataType::FLOAT16: f(__half{}); break;
-    case DataType::BFLOAT16: f(__nv_bfloat16{}); break;
-    case DataType::FLOAT8_E4M3: f(__nv_fp8_e4m3{}); break;
-    case DataType::FLOAT8_E5M2: f(__nv_fp8_e5m2{}); break;
+// The LDG/STG fused-step instantiation for a launch shape (unroll 1, 2 or 4).
+template <typename T>
+auto localAllreduceFn(int unroll, bool tiled) {
+  if (tiled) {
+    if (unroll == 4) return localAllreduceManyKernel<T, 4, true>;
+    if (unroll == 1) return localAllreduceManyKernel<T, 1, true>;
+    return localAllreduceManyKernel<T, 2, true>;
   }
+  if (unroll == 4) return localAllreduceManyKernel<T, 4, false>;
+  if (unroll == 1) return localAllreduceManyKernel<T, 1, false>;
+  return localAllreduceManyKernel<T, 2, false>;
 }
 
 bool aligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; }
@@ -385,17 +362,9 @@ void launchLocalAllreduceMany(void* const* bufs, int n, size_t count, DataType d
     using T = decltype(tag);
     // Launch shape: measured on H100 (scripts/bench_local.py); GLB_LOCAL_SHAPE = "<ctas per SM>,<unroll>,<tiled>".
     const int grid = gridFor(count / PackTraits<T>::kElems / shape.unroll + 1, kLocalThreads, shape.ctasPerSm);
-    const DevOp dop = static_cast<DevOp>(op);
-    auto go = [&](auto kernel) { kernel<<<grid, kLocalThreads, 0, stream>>>(bp, n, count, dop, scale, vectorOk); };
-    if (shape.tiled) {
-      if (shape.unroll == 4) go(localAllreduceManyKernel<T, 4, true>);
-      else if (shape.unroll == 1) go(localAllreduceManyKernel<T, 1, true>);
-      else go(localAllreduceManyKernel<T, 2, true>);
-    } else {
-      if (shape.unroll == 4) go(localAllreduceManyKernel<T, 4, false>);
-      else if (shape.unroll == 1) go(localAllreduceManyKernel<T, 1, false>);
-      else go(localAllreduceManyKernel<T, 2, false>);
-    }
+    localAllreduceFn<T>(shape.unroll, shape.tiled)<<<grid, kLocalThreads, 0, stream>>>(bp, n, count,
+                                                                                     static_cast<DevOp>(op), scale,
+                                                                                     vectorOk);
   });
 }
 
@@ -449,29 +418,20 @@ void setLocalAllreduceShape(int ctasPerSm, int unroll, bool tiled) {
 }
 
 void preloadLocalKernels() {
-  auto touch = [](const void* k) {
-    cudaFuncAttributes attr;
-    cudaFuncGetAttributes(&attr, k);
-  };
-  for (DataType dt : {DataType::INT8, DataType::UINT8, DataType::INT16, DataType::INT32, DataType::UINT32, DataType::INT64,
-                      DataType::UINT64, DataType::FLOAT32, DataType::FLOAT64, DataType::FLOAT16, DataType::BFLOAT16,
-                      DataType::FLOAT8_E4M3, DataType::FLOAT8_E5M2}) {
-    dispatchType(dt, [&](auto tag) {
+  for (DataType dt : kAllDataTypes) {
+    dispatchType(dt, [](auto tag) {
       using T = decltype(tag);
-      touch(reinterpret_cast<const void*>(localReduceManyKernel<T>));
-      touch(reinterpret_cast<const void*>(localAllreduceManyKernel<T, 1, false>));
-      touch(reinterpret_cast<const void*>(localAllreduceManyKernel<T, 2, false>));
-      touch(reinterpret_cast<const void*>(localAllreduceManyKernel<T, 4, false>));
-      touch(reinterpret_cast<const void*>(localAllreduceManyKernel<T, 1, true>));
-      touch(reinterpret_cast<const void*>(localAllreduceManyKernel<T, 2, true>));
-      touch(reinterpret_cast<const void*>(localAllreduceManyKernel<T, 4, true>));
-      touch(reinterpret_cast<const void*>(localAllreduceManyBulkKernel<T>));
-      touch(reinterpret_cast<const void*>(verifyKernel<T>));
-      touch(reinterpret_cast<const void*>(fillKernel<T>));
+      touchKernel(localReduceManyKernel<T>);
+      for (bool tiled : {false, true}) {
+        for (int u : {1, 2, 4}) touchKernel(localAllreduceFn<T>(u, tiled));
+      }
+      touchKernel(localAllreduceManyBulkKernel<T>);
+      touchKernel(verifyKernel<T>);
+      touchKernel(fillKernel<T>);
     });
   }
-  touch(reinterpret_cast<const void*>(localBroadcastKernel));
-  touch(reinterpret_cast<const void*>(spinKernel));
+  touchKernel(localBroadcastKernel);
+  touchKernel(spinKernel);
   cudaGetLastError();
 }
 

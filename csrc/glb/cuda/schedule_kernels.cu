@@ -127,48 +127,14 @@ scheduleKernel(CommArgs a, PeerPtrs bufs, PeerPtrs stage, const SchedStep* __res
 void launchSchedule(const CommArgs& a, const PeerPtrs& bufs, const PeerPtrs& stage, const SchedStep* table,
                     int nsteps, int nbarriers, DataType dt, ReduceOp op, float scale, size_t count, bool vectorOk,
                     int blocks, cudaStream_t stream) {
-  const DevOp dop = static_cast<DevOp>(op);
-#define GLB_CASE(E, T)                                                                                          \
-  case DataType::E:                                                                                             \
-    scheduleKernel<T><<<blocks, kThreads, 0, stream>>>(a, bufs, stage, table, nsteps, nbarriers, dop, scale, count, vectorOk); \
-    break;
-  switch (dt) {
-    GLB_CASE(INT8, int8_t)
-    GLB_CASE(UINT8, uint8_t)
-    GLB_CASE(INT16, int16_t)
-    GLB_CASE(INT32, int32_t)
-    GLB_CASE(UINT32, uint32_t)
-    GLB_CASE(INT64, long long)
-    GLB_CASE(UINT64, unsigned long long)
-    GLB_CASE(FLOAT32, float)
-    GLB_CASE(FLOAT64, double)
-    GLB_CASE(FLOAT16, __half)
-    GLB_CASE(BFLOAT16, __nv_bfloat16)
-    GLB_CASE(FLOAT8_E4M3, __nv_fp8_e4m3)
-    GLB_CASE(FLOAT8_E5M2, __nv_fp8_e5m2)
-  }
-#undef GLB_CASE
+  dispatchType(dt, [&](auto tag) {
+    scheduleKernel<decltype(tag)><<<blocks, kThreads, 0, stream>>>(a, bufs, stage, table, nsteps, nbarriers,
+                                                                  static_cast<DevOp>(op), scale, count, vectorOk);
+  });
 }
 
-
 void preloadScheduleKernels() {
-  auto touch = [](const void* k) {
-    cudaFuncAttributes attr;
-    cudaFuncGetAttributes(&attr, k);
-  };
-  touch(reinterpret_cast<const void*>(scheduleKernel<int8_t>));
-  touch(reinterpret_cast<const void*>(scheduleKernel<uint8_t>));
-  touch(reinterpret_cast<const void*>(scheduleKernel<int16_t>));
-  touch(reinterpret_cast<const void*>(scheduleKernel<int32_t>));
-  touch(reinterpret_cast<const void*>(scheduleKernel<uint32_t>));
-  touch(reinterpret_cast<const void*>(scheduleKernel<long long>));
-  touch(reinterpret_cast<const void*>(scheduleKernel<unsigned long long>));
-  touch(reinterpret_cast<const void*>(scheduleKernel<float>));
-  touch(reinterpret_cast<const void*>(scheduleKernel<double>));
-  touch(reinterpret_cast<const void*>(scheduleKernel<__half>));
-  touch(reinterpret_cast<const void*>(scheduleKernel<__nv_bfloat16>));
-  touch(reinterpret_cast<const void*>(scheduleKernel<__nv_fp8_e4m3>));
-  touch(reinterpret_cast<const void*>(scheduleKernel<__nv_fp8_e5m2>));
+  for (DataType dt : kAllDataTypes) dispatchType(dt, [](auto tag) { touchKernel(scheduleKernel<decltype(tag)>); });
   cudaGetLastError();
 }
 

@@ -267,25 +267,6 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
       }
       return h[per] == 0.0f ? "" : "wrote outside my block";
     });
-    R.run(strcat_all("gatherBulkKernel(allgather, TMA) P=", P), [&]() -> std::string {
-      const size_t per = n / P / 4 * 4;  // 16-byte granular blocks
-      std::vector<size_t> off(P), len(P, per * 4);
-      for (int r = 0; r < P; r++) off[r] = r * per * 4;
-      DevBuf in(per * 4);
-      launchFill(in.p, per, DataType::FLOAT32, 3.0, 1.0, stream);
-      for (int r = 0; r < P; r++) GLB_CUDA_CHECK(cudaMemsetAsync(pp.p[r], 0, n * 4, stream));
-      launchGatherPush(ca, in.p, pp, nullptr, off.data(), len.data(), -1, true,
-                       std::min(pc.coResidentBlocks(gatherBulkKernelPtr(), 128), 16), stream, /*tma=*/true);
-      noteLaunch();
-      for (int r : {0, P - 1}) {
-        auto h = download(pp.p[r], n, stream);
-        for (size_t i = 0; i < per; i++) {
-          if (!close(h[i], 3.0 + i)) return strcat_all("dst ", r, " element ", i, ": got ", h[i]);
-        }
-        if (h[per] != 0.0f) return "wrote outside my block";
-      }
-      return "";
-    });
     R.run(strcat_all("alltoallPushKernel P=", P), [&]() -> std::string {
       const size_t per = n / P / 4 * 4;
       std::vector<size_t> soff(P), slen(P, per * 4), doff(P, 0);

@@ -3,7 +3,7 @@
 400 MB buffers and the virtual-rank loopback of the collective kernels on 64 MB buffers, so
 that `ncu --set full -k regex:...` captures the hot kernels at a realistic size.
 
-  ncu --set full --clock-control none --import-source on -k regex:'localAllreduceMany|twoShotAllreduce|pipelinedAllreduce|gatherBulk|peerBulkCopy' \
+  ncu --set full --clock-control none --import-source on -k regex:'localAllreduceMany|twoShotAllreduce|pipelinedAllreduce|peerBulkCopy' \
       -c 8 -o gpurun_out/prof_r2 python scripts/ncu_target.py
 """
 import os

@@ -33,7 +33,6 @@ KERNELS = [
     ("reduce_pull_f32_P8", r"reducePullKernel<float, 8, 2>"),
     ("broadcast", r"broadcastKernel"),
     ("gather_push", r"gatherPushKernel"),
-    ("gather_bulk_tma", r"gatherBulkKernel"),
     ("alltoall_push", r"alltoallPushKernel"),
     ("p2p_sendrecv", r"p2pKernel"),
     ("exchange_zero_copy", r"exchangeKernel<false>"),
