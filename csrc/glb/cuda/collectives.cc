@@ -225,30 +225,49 @@ void runOneShot(PeerContext& pc, const void* in, void* out, size_t count, DataTy
   launchOneShotAllreduce(pc.comm(), in, out, count, dt, op, scale, pc.stagePtrs(0), l.half, extra, blocks, stream);
 }
 
+// Launch shape of a kernel that pipelines plain pointers through `slots` pool slots, each of
+// `shares` x blocks x tile 16-byte groups. `payloadBytes` is the largest payload in the same
+// units as one slot (the whole vector for the allreduce, P x the largest share for
+// reduce_scatter, the largest block for allgather). A zero hint takes the tuning default.
+struct PipeShape {
+  int blocks = 1;
+  int tile = 16;
+  int xthreads = 32;
+};
+
+PipeShape pipeShape(PeerContext& pc, const void* kernel, int slots, int shares, size_t payloadBytes, int blocksHint,
+                    int tileHint, int xthreadsHint, const char* what) {
+  const auto l = layoutOf(pc);
+  PipeShape sh;
+  sh.blocks = std::max(1, std::min(blocksHint > 0 ? blocksHint : tuning().maxBlocks, pc.coResidentBlocks(kernel)));
+  // Tile: a power of two, small enough for every slot in the bulk region and for a few
+  // steps of pipelining on mid-sized messages.
+  const int tile = tileHint > 0 ? tileHint : tuning().pipeTile;
+  auto slotBytes = [&](int tl, int bl) { return static_cast<size_t>(shares) * bl * tl * 16; };
+  while (sh.tile * 2 <= tile) sh.tile *= 2;
+  while (sh.tile > 16 && (slots * slotBytes(sh.tile, sh.blocks) > l.bulkBytes ||
+                          payloadBytes < 4 * slotBytes(sh.tile, sh.blocks))) {
+    sh.tile /= 2;
+  }
+  while (sh.blocks > 1 && payloadBytes < slotBytes(sh.tile, sh.blocks)) sh.blocks = (sh.blocks + 1) / 2;  // tiny messages: fewer CTAs
+  GLB_ENFORCE_LE(slots * slotBytes(sh.tile, sh.blocks), l.bulkBytes, "staging pool too small for the pipelined ", what,
+                 "; raise GLB_CUDA_STAGE_MB (CudaContext stage_bytes)");
+  const int x = xthreadsHint > 0 ? xthreadsHint : tuning().pipeExchangeThreads;
+  sh.xthreads = std::max(32, std::min(kThreads - 32, x / 32 * 32));
+  return sh;
+}
+
 void runPipelined(PeerContext& pc, const void* in, void* out, size_t count, DataType dt, ReduceOp op, float scale,
                   const LocalPtrs& extra, const AllreducePlan& plan, cudaStream_t stream) {
   const auto l = layoutOf(pc);
   const size_t es = elementSize(dt);
   const size_t groups = ceilDiv(count * es, size_t(16));
   const bool mc = pc.nvlsAvailable() && pc.size > 2 && nvlsSupports(dt, op);
-  const void* kernel = pipelinedKernelFor(dt, mc, pc.size);
-  int blocks = plan.cfg.blocks > 0 ? plan.cfg.blocks : tuning().maxBlocks;
-  blocks = std::max(1, std::min(blocks, pc.coResidentBlocks(kernel)));
-  // Tile: a power of two, small enough for three slots in the bulk region and for a few
-  // steps of pipelining on mid-sized messages.
-  int tile = plan.tile > 0 ? plan.tile : tuning().pipeTile;
-  auto chunkBytes = [&](int tl, int bl) { return static_cast<size_t>(pc.size) * bl * tl * 16; };
-  int t2 = 16;
-  while (t2 * 2 <= tile) t2 *= 2;
-  tile = t2;
-  while (tile > 16 && (3 * chunkBytes(tile, blocks) > l.bulkBytes || groups * 16 < 4 * chunkBytes(tile, blocks))) tile /= 2;
-  while (blocks > 1 && groups * 16 < chunkBytes(tile, blocks)) blocks = (blocks + 1) / 2;  // tiny messages: fewer CTAs
-  GLB_ENFORCE_LE(3 * chunkBytes(tile, blocks), l.bulkBytes, "staging pool too small for the pipelined allreduce; raise GLB_CUDA_STAGE_MB");
   // cfg.unroll doubles as "exchange warps" for this kernel (0 = the pipeExchangeThreads knob).
-  int xthreads = plan.cfg.unroll > 0 ? plan.cfg.unroll * 32 : tuning().pipeExchangeThreads;
-  xthreads = std::max(32, std::min(kThreads - 32, xthreads / 32 * 32));
+  const PipeShape sh = pipeShape(pc, pipelinedKernelFor(dt, mc, pc.size), 3, pc.size, groups * 16, plan.cfg.blocks,
+                                 plan.tile, plan.cfg.unroll * 32, "allreduce");
   launchPipelinedAllreduce(pc.comm(), in, out, count, dt, op, scale, pc.stagePtrs(l.bulkOff),
-                           mc ? pc.stageMc(l.bulkOff) : nullptr, tile, xthreads, extra, blocks, stream);
+                           mc ? pc.stageMc(l.bulkOff) : nullptr, sh.tile, sh.xthreads, extra, sh.blocks, stream);
 }
 
 }  // namespace
@@ -591,6 +610,24 @@ void gatherCommon(PeerContext& pc, const void* in, const PeerPtrs& outs, void* m
   finish(pc, stream, "allgather/gather");
 }
 
+// Plain pointers whose payload is larger than the pool's bulk region: one kernel pipelines
+// copy-in and pull through two pool slots (pipeline_kernels.cu). Every rank holds the whole
+// size vector and the same pool size, so all ranks pick this path together.
+bool exceedsBulk(const PeerContext& pc, size_t bytes) { return bytes > layoutOf(pc).bulkBytes; }
+
+void runPipelinedGather(PeerContext& pc, const void* in, void* out, const std::vector<size_t>& bytesPerRank, int onlyDst,
+                        cudaStream_t stream) {
+  GLB_TRACE_RANGE("glb::cuda::allgather/gather(pipelined)");
+  GLB_ENFORCE_EQ(static_cast<int>(bytesPerRank.size()), pc.size, "need one byte count per rank");
+  auto off = prefix(bytesPerRank);
+  const size_t largest = *std::max_element(bytesPerRank.begin(), bytesPerRank.end());
+  const PipeShape sh = pipeShape(pc, pipelinedAllgatherKernelPtr(), 2, 1, largest, 0, 0, 0, "allgather / gather");
+  prologue(pc, stream);
+  launchPipelinedAllgather(pc.comm(), in, out, off.data(), bytesPerRank.data(), onlyDst,
+                           pc.stagePtrs(layoutOf(pc).bulkOff), sh.tile, sh.xthreads, sh.blocks, stream);
+  finish(pc, stream, "allgather/gather(pipelined)");
+}
+
 bool allEqual(const std::vector<size_t>& v) {
   for (size_t x : v) {
     if (x != v[0]) return false;
@@ -649,6 +686,10 @@ void allgatherv(PeerContext& pc, const void* in, void* out, const std::vector<si
     return;
   }
   if (allEqual(bytesPerRank) && tryLLExchange(pc, in, out, bytesPerRank[0], 0, stream)) return;
+  if (exceedsBulk(pc, off.back())) {
+    runPipelinedGather(pc, in, out, bytesPerRank, -1, stream);
+    return;
+  }
   auto st = stagedBulk(pc, off.back(), "allgather");
   gatherCommon(pc, in, st.ptrs, nullptr, true, bytesPerRank, -1, stream);
   if (off.back() > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(out, st.mine, off.back(), cudaMemcpyDeviceToDevice, stream));
@@ -672,6 +713,11 @@ void gatherv(PeerContext& pc, const void* in, void* out, const std::vector<size_
   auto off = prefix(bytesPerRank);
   if (pc.size == 1) {
     if (out != in && off.back() > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(out, in, off.back(), cudaMemcpyDeviceToDevice, stream));
+    return;
+  }
+  GLB_ENFORCE(root >= 0 && root < pc.size, "gather: invalid root ", root);
+  if (exceedsBulk(pc, off.back())) {
+    runPipelinedGather(pc, in, out, bytesPerRank, root, stream);
     return;
   }
   auto st = stagedBulk(pc, off.back(), "gather");
@@ -939,6 +985,21 @@ void reduce_scatter(PeerContext& pc, const void* in, void* out, const std::vecto
   }
   GLB_ENFORCE(op != ReduceOp::CUSTOM, "custom reductions run on the host path only");
   if (tryLLReduceScatter(pc, in, out, counts, dt, op, scale, stream)) return;
+  if (exceedsBulk(pc, off.back() * es)) {
+    GLB_TRACE_RANGE("glb::cuda::reduce_scatter(pipelined)");
+    GLB_ENFORCE_EQ(static_cast<int>(counts.size()), pc.size, "need one element count per rank");
+    Epilogue ep;
+    ep.scale = scale;
+    const float s = scaleOf(ep, dt);
+    const size_t largest = *std::max_element(counts.begin(), counts.end());
+    const PipeShape sh = pipeShape(pc, pipelinedReduceScatterKernelFor(dt, pc.size), 2, pc.size,
+                                   largest * es * pc.size, 0, 0, 0, "reduce_scatter");
+    prologue(pc, stream);
+    launchPipelinedReduceScatter(pc.comm(), in, out, off.data(), counts.data(), dt, op, s,
+                                 pc.stagePtrs(layoutOf(pc).bulkOff), sh.tile, sh.xthreads, sh.blocks, stream);
+    finish(pc, stream, "reduce_scatter(pipelined)");
+    return;
+  }
   auto st = stagedBulk(pc, off.back() * es, "reduce_scatter");
   if (off.back() > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(st.mine, in, off.back() * es, cudaMemcpyDeviceToDevice, stream));
   reducePullCommon(pc, st.ptrs, st.mc, true, out, counts, dt, op, scale, stream);

@@ -53,11 +53,25 @@ const void* twoShotKernelFor(DataType dt, int nranks, int unroll);
 const void* nvlsKernelFor(DataType dt, int unroll);
 const void* castKernelFor(DataType in, DataType out);
 
-// pipeline_kernels.cu — arbitrary pointers through the pool, 3-stage in-kernel pipeline.
+// pipeline_kernels.cu — arbitrary pointers through the pool, in-kernel pipelines (allreduce:
+// 3 stages).
 const void* pipelinedKernelFor(DataType dt, bool mc, int nranks);
 void launchPipelinedAllreduce(const CommArgs& a, const void* in, void* out, size_t count, DataType dt, ReduceOp op,
                               float scale, const PeerPtrs& stage, void* mcStage, int tileVecs, int exchangeThreads,
                               const LocalPtrs& extra, int blocks, cudaStream_t stream);
+// allgather(v) / gather(v) of plain pointers of any size, two-stage pipeline through two pool
+// slots of G x tileVecs 16-byte groups. Rank r's block (lens[r] bytes) lands at offs[r] of the
+// output of every rank, or of rank onlyDst only (>= 0: gather; nothing else writes its out).
+const void* pipelinedAllgatherKernelPtr();
+void launchPipelinedAllgather(const CommArgs& a, const void* in, void* out, const size_t* offs, const size_t* lens,
+                              int onlyDst, const PeerPtrs& stage, int tileVecs, int exchangeThreads, int blocks,
+                              cudaStream_t stream);
+// reduce_scatter of plain pointers of any size: rank r's share is elemLen[r] elements at
+// elemOff[r] of `in`; `out` receives my share, reduced over all ranks and scaled.
+const void* pipelinedReduceScatterKernelFor(DataType dt, int nranks);
+void launchPipelinedReduceScatter(const CommArgs& a, const void* in, void* out, const size_t* elemOff,
+                                  const size_t* elemLen, DataType dt, ReduceOp op, float scale, const PeerPtrs& stage,
+                                  int tileVecs, int exchangeThreads, int blocks, cudaStream_t stream);
 
 // collective_kernels.cu -----------------------------------------------------------------------
 void launchBroadcast(const CommArgs& a, const PeerPtrs& bufs, void* mc, size_t bytes, int root, int mode, bool vec,

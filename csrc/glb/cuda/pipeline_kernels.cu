@@ -18,7 +18,35 @@
 // Ownership: a chunk is P shares x G tiles x T 16-byte groups; CTA b owns tile b of every
 // share in every stage, so the CTA-to-CTA flag barrier is all the synchronisation needed
 // (the CTA that reads a peer's tile is barrier-paired with the CTA that wrote it).
+//
+// allgather(v) / gather(v) and reduce_scatter of plain pointers use the same framework with
+// two stages, and both PULL:
+//
+//     step i:   A(i)    copy chunk i of my data     user input -> my pool slot i % 2   (local HBM)
+//               B(i-1)  load chunk i-1 from slot (i-1) % 2 of every peer, (reduce,) store to
+//                       the user output                                                 (NVLink)
+//
+// Chunk i covers bytes [i*C, (i+1)*C) of EVERY rank's block (allgather) or share
+// (reduce_scatter), C = G*T*16. The chunk count comes from the largest block, so the grid and
+// the number of steps (chunks + 1, one barrier each) are the same on every rank.
+//
+// Two slots are enough: nothing is written back into the pool to be read again later. The slot
+// a rank fills in step i+1 is the slot its peers read in step i; the rank starts step i+1 only
+// after barrier i, and it passes barrier i only when CTA b of every peer has finished step i.
+//
+// Pool rules, which every kernel that uses the bulk region keeps, so that consecutive calls
+// need no other synchronisation:
+//  * Before its first barrier, a kernel writes only its own pool. A peer may still be reading
+//    its own bulk region at that point: the staged paths copy out of the pool with a
+//    cudaMemcpyAsync after their kernel's final barrier. Pulling keeps this rule without an
+//    entry barrier (gatherPushKernel, which pushes, pays one before its first remote store).
+//  * A kernel reads a peer's pool for the last time before its own final barrier.
+//
+// Why pull: a pushed chunk lands in the receiver's pool and has to be read again to reach the
+// output, an extra (P-1)·s pass over the receiver's HBM; pulling costs one extra s (my own
+// block into my pool).
 #include "glb/cuda/device_common.cuh"
+#include "glb/cuda/grid_copy.cuh"
 #include "glb/cuda/kernels.h"
 
 namespace glb {
@@ -275,17 +303,6 @@ const void* pipelinedKernelFor(DataType dt, bool mc, int nranks) {
   return k;
 }
 
-void preloadPipelineKernels() {
-  for (DataType dt : kAllDataTypes) {
-    dispatchType(dt, [](auto tag) {
-      for (bool mc : {false, true}) {
-        for (int nr : {0, 2, 4, 8}) touchKernel(pipeFn<decltype(tag)>(mc, nr));
-      }
-    });
-  }
-  cudaGetLastError();
-}
-
 void launchPipelinedAllreduce(const CommArgs& a, const void* in, void* out, size_t count, DataType dt, ReduceOp op,
                               float scale, const PeerPtrs& stage, void* mcStage, int tileVecs, int exchangeThreads,
                               const LocalPtrs& extra, int blocks, cudaStream_t stream) {
@@ -297,6 +314,268 @@ void launchPipelinedAllreduce(const CommArgs& a, const void* in, void* out, size
                                                              mc ? static_cast<char*>(mcStage) : nullptr, tileVecs,
                                                              exchangeThreads, extra);
   });
+}
+
+// Per-rank blocks (allgather: bytes) or shares (reduce_scatter: elements).
+struct PipeBlocks {
+  size_t off[kMaxRanks];
+  size_t len[kMaxRanks];
+};
+
+namespace {
+// Part of a block of `len` units that falls into tile b of chunk c (units per tile: tileUnits).
+__device__ __forceinline__ size_t tilePart(size_t len, size_t c, size_t chunkUnits, size_t tileUnits) {
+  const size_t s = c * chunkUnits + blockIdx.x * tileUnits;
+  return len > s ? (len - s < tileUnits ? len - s : tileUnits) : 0;
+}
+
+__device__ __forceinline__ size_t largestOf(const PipeBlocks& pb, int P) {
+  size_t m = 0;
+  for (int q = 0; q < P; q++) m = pb.len[q] > m ? pb.len[q] : m;
+  return m;
+}
+}  // namespace
+
+// Slot: C bytes, my chunk. A(i): my chunk i -> my slot, and to out + off[me] unless `in` already
+// is that address (in place) or I receive nothing (gather, not the root). B(i-1): chunk i-1 of
+// every peer's slot -> out + off[q] (only the root for gather: a non-root never writes its out).
+__global__ void __launch_bounds__(kThreads)
+pipelinedAllgatherKernel(CommArgs a, const char* in, char* out, PipeBlocks pb, int onlyDst, PeerPtrs stage,
+                         int tileVecs, int exchangeThreads) {
+  const int P = a.nranks, me = a.rank;
+  const size_t tileBytes = static_cast<size_t>(tileVecs) * 16;
+  const size_t C = gridDim.x * tileBytes;
+  const size_t nchunks = (largestOf(pb, P) + C - 1) / C;
+  const size_t tileOff = blockIdx.x * tileBytes;
+  const uint32_t e = loadEpoch(a);
+  char* myStage = static_cast<char*>(stage.p[me]);
+  const bool receiver = onlyDst < 0 || onlyDst == me;
+  const bool copyOwn = receiver && out + pb.off[me] != in;
+  const bool exchanger = static_cast<int>(threadIdx.x) < exchangeThreads;
+  const int xt = threadIdx.x, xn = exchangeThreads;
+  const int ct = threadIdx.x - exchangeThreads, cn = blockDim.x - exchangeThreads;
+
+  for (size_t i = 0; i < nchunks + 1; i++) {
+    if (exchanger) {
+      // ---- B(i-1): pull every peer's chunk i-1 into my output ----
+      if (i >= 1 && receiver) {
+        const size_t c = i - 1;
+        for (int k = 1; k < P; k++) {
+          const int q = (me + k) % P;
+          const size_t n = tilePart(pb.len[q], c, C, tileBytes);
+          if (n > 0) {
+            gridCopy(out + pb.off[q] + c * C + tileOff,
+                     static_cast<const char*>(stage.p[q]) + (c % 2) * C + tileOff, n, true, xt, xn);
+          }
+        }
+      }
+    } else if (i < nchunks) {
+      // ---- A(i): my chunk i -> my slot (and my own block of the output) ----
+      const size_t n = tilePart(pb.len[me], i, C, tileBytes);
+      if (n > 0) {
+        const char* src = in + i * C + tileOff;
+        gridCopy(myStage + (i % 2) * C + tileOff, src, n, true, ct, cn);
+        if (copyOwn) gridCopy(out + pb.off[me] + i * C + tileOff, src, n, true, ct, cn);
+      }
+    }
+    if (!blockBarrier(a, e + static_cast<uint32_t>(i) + 1)) break;
+  }
+  retire(a, static_cast<uint32_t>(nchunks + 1), 0);
+}
+
+// Slot: P sub-slots of C bytes, sub-slot q = chunk i of share q. A(i): chunk i of every share of
+// `in` -> my slot i % 2. B(i-1): sub-slot `me` of slot (i-1) % 2 from all P pools, reduced in the
+// accumulator type of PackTraits (fp32 for the 16-bit and FP8 types), scaled, rounded once and
+// stored to out + (i-1)·C. Counts are in elements: a share of `in`, and `out`, may start at an
+// address that is not 16-byte aligned (element-wise loads / stores at their groups).
+template <typename T, int NR>
+__global__ void __launch_bounds__(kThreads)
+pipelinedReduceScatterKernel(CommArgs a, const T* in, T* out, PipeBlocks pb, DevOp op, float scale, PeerPtrs stage,
+                             int tileVecs, int exchangeThreads) {
+  using PT = PackTraits<T>;
+  const int P = NR > 0 ? NR : a.nranks;
+  const int me = a.rank;
+  const size_t T_ = static_cast<size_t>(tileVecs);
+  const size_t tileElems = T_ * PT::kElems;
+  const size_t chunkElems = gridDim.x * tileElems;
+  const size_t C = chunkElems * sizeof(T);  // = G*T*16 bytes
+  const size_t slotBytes = static_cast<size_t>(P) * C;
+  const size_t nchunks = (largestOf(pb, P) + chunkElems - 1) / chunkElems;
+  const size_t tileOff = blockIdx.x * T_ * 16;
+  const uint32_t e = loadEpoch(a);
+  char* myStage = static_cast<char*>(stage.p[me]);
+  const bool outAligned = reinterpret_cast<uintptr_t>(out) % 16 == 0;
+  const bool exchanger = static_cast<int>(threadIdx.x) < exchangeThreads;
+  const int xt = threadIdx.x, xn = exchangeThreads;
+  const int ct = threadIdx.x - exchangeThreads, cn = blockDim.x - exchangeThreads;
+
+  for (size_t i = 0; i < nchunks + 1; i++) {
+    if (exchanger) {
+      // ---- B(i-1): reduce my share's tile of chunk i-1 from every pool ----
+      const size_t c = i - 1;
+      const size_t n = i >= 1 ? tilePart(pb.len[me], c, chunkElems, tileElems) : 0;
+      if (n > 0) {
+        const size_t ng = (n + PT::kElems - 1) / PT::kElems;
+        T* dst = out + c * chunkElems + blockIdx.x * tileElems;
+        // Like the peer path of the allreduce pipeline: rank-rotated order, kSlots x U
+        // independent 128-bit loads in flight per thread (half the packs for 16-lane FP8). U is 6
+        // rather than 8 at P = 2, and any P loads in batches (of 4 for 8-byte lanes): the
+        // element-wise output path needs the registers, and this keeps every instantiation free
+        // of spills (-Xptxas -v).
+        constexpr int kSlots = NR > 0 ? NR : kMaxRanks;
+        constexpr int kWide = PT::kElems > 8 ? 2 : 1;
+        constexpr int U0 = NR == 2 ? 6 : (NR == 4 ? 4 : (NR == 8 ? 2 : 1));
+        constexpr int U = U0 / kWide > 0 ? U0 / kWide : 1;
+        constexpr int kBatch = sizeof(T) == 8 ? 4 : 8;
+        const char* peer[kSlots];
+#pragma unroll
+        for (int q = 0; q < kSlots; q++) {
+          peer[q] = q < P ? static_cast<const char*>(stage.p[(me + q) % P]) + (c % 2) * slotBytes + me * C + tileOff
+                          : nullptr;
+        }
+        if constexpr (kSlots > 8) {
+          // Any P: the peers' packs come in batches (same order).
+          for (size_t o = xt; o < ng; o += static_cast<size_t>(xn)) {
+            typename PT::AccPack acc;
+#pragma unroll
+            for (int b0 = 0; b0 < kSlots; b0 += kBatch) {
+              Pack16 v[kBatch];
+#pragma unroll
+              for (int q = 0; q < kBatch; q++) {
+                if (b0 + q < P) v[q] = ld128_stream(peer[b0 + q] + o * 16);
+              }
+#pragma unroll
+              for (int q = 0; q < kBatch; q++) {
+                if (b0 + q == 0) {
+                  acc = PT::widen(v[q]);
+                } else if (b0 + q < P) {
+                  PT::combine(acc, v[q], op);
+                }
+              }
+            }
+            if (scale != 1.0f) PT::scale(acc, scale);
+            storeGroupP(dst, o, n, outAligned, PT::narrow(acc));
+          }
+        } else {
+          for (size_t o0 = xt; o0 < ng; o0 += static_cast<size_t>(xn) * U) {
+            Pack16 v[U][kSlots];
+#pragma unroll
+            for (int u = 0; u < U; u++) {
+              const size_t o = o0 + static_cast<size_t>(u) * xn;
+              if (o < ng) {
+#pragma unroll
+                for (int q = 0; q < kSlots; q++) {
+                  if (q < P) v[u][q] = ld128_stream(peer[q] + o * 16);
+                }
+              }
+            }
+#pragma unroll
+            for (int u = 0; u < U; u++) {
+              const size_t o = o0 + static_cast<size_t>(u) * xn;
+              if (o < ng) {
+                typename PT::AccPack acc = PT::widen(v[u][0]);
+#pragma unroll
+                for (int q = 1; q < kSlots; q++) {
+                  if (q < P) PT::combine(acc, v[u][q], op);
+                }
+                if (scale != 1.0f) PT::scale(acc, scale);
+                storeGroupP(dst, o, n, outAligned, PT::narrow(acc));
+              }
+            }
+          }
+        }
+      }
+    } else if (i < nchunks) {
+      // ---- A(i): chunk i of every share -> my slot (zero past a share's end) ----
+      constexpr int CU = PT::kElems > 8 ? 2 : 4;
+      char* slot = myStage + (i % 2) * slotBytes + tileOff;
+      for (int q = 0; q < P; q++) {
+        const size_t n = tilePart(pb.len[q], i, chunkElems, tileElems);
+        if (n == 0) continue;
+        const size_t ng = (n + PT::kElems - 1) / PT::kElems;
+        const T* src = in + pb.off[q] + i * chunkElems + blockIdx.x * tileElems;
+        const bool aligned = reinterpret_cast<uintptr_t>(src) % 16 == 0;
+        for (size_t j0 = ct; j0 < ng; j0 += static_cast<size_t>(cn) * CU) {
+          Pack16 p[CU];
+#pragma unroll
+          for (int u = 0; u < CU; u++) {
+            const size_t j = j0 + static_cast<size_t>(u) * cn;
+            if (j < ng) p[u] = loadGroupP(src, j, n, aligned);
+          }
+#pragma unroll
+          for (int u = 0; u < CU; u++) {
+            const size_t j = j0 + static_cast<size_t>(u) * cn;
+            if (j < ng) st128(slot + q * C + j * 16, p[u]);
+          }
+        }
+      }
+    }
+    if (!blockBarrier(a, e + static_cast<uint32_t>(i) + 1)) break;
+  }
+  retire(a, static_cast<uint32_t>(nchunks + 1), 0);
+}
+
+namespace {
+// The pipelined reduce_scatter instantiation for (T, P).
+template <typename T>
+auto pipeRsFn(int nranks) {
+  if constexpr (isHotType<T>()) {
+    if (nranks == 2) return pipelinedReduceScatterKernel<T, 2>;
+    if (nranks == 4) return pipelinedReduceScatterKernel<T, 4>;
+    if (nranks == 8) return pipelinedReduceScatterKernel<T, 8>;
+  }
+  return pipelinedReduceScatterKernel<T, 0>;
+}
+
+PipeBlocks pipeBlocks(int nranks, const size_t* offs, const size_t* lens) {
+  PipeBlocks pb;
+  for (int i = 0; i < kMaxRanks; i++) {
+    pb.off[i] = i < nranks ? offs[i] : 0;
+    pb.len[i] = i < nranks ? lens[i] : 0;
+  }
+  return pb;
+}
+}  // namespace
+
+const void* pipelinedAllgatherKernelPtr() { return reinterpret_cast<const void*>(pipelinedAllgatherKernel); }
+
+const void* pipelinedReduceScatterKernelFor(DataType dt, int nranks) {
+  const void* k = nullptr;
+  dispatchType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(pipeRsFn<decltype(tag)>(nranks)); });
+  return k;
+}
+
+void launchPipelinedAllgather(const CommArgs& a, const void* in, void* out, const size_t* offs, const size_t* lens,
+                              int onlyDst, const PeerPtrs& stage, int tileVecs, int exchangeThreads, int blocks,
+                              cudaStream_t stream) {
+  pipelinedAllgatherKernel<<<blocks, kThreads, 0, stream>>>(a, static_cast<const char*>(in), static_cast<char*>(out),
+                                                            pipeBlocks(a.nranks, offs, lens), onlyDst, stage, tileVecs,
+                                                            exchangeThreads);
+}
+
+void launchPipelinedReduceScatter(const CommArgs& a, const void* in, void* out, const size_t* elemOff,
+                                  const size_t* elemLen, DataType dt, ReduceOp op, float scale, const PeerPtrs& stage,
+                                  int tileVecs, int exchangeThreads, int blocks, cudaStream_t stream) {
+  dispatchType(dt, [&](auto tag) {
+    using T = decltype(tag);
+    pipeRsFn<T>(a.nranks)<<<blocks, kThreads, 0, stream>>>(a, static_cast<const T*>(in), static_cast<T*>(out),
+                                                           pipeBlocks(a.nranks, elemOff, elemLen),
+                                                           static_cast<DevOp>(op), scale, stage, tileVecs,
+                                                           exchangeThreads);
+  });
+}
+
+void preloadPipelineKernels() {
+  for (DataType dt : kAllDataTypes) {
+    dispatchType(dt, [](auto tag) {
+      for (bool mc : {false, true}) {
+        for (int nr : {0, 2, 4, 8}) touchKernel(pipeFn<decltype(tag)>(mc, nr));
+      }
+      for (int nr : {0, 2, 4, 8}) touchKernel(pipeRsFn<decltype(tag)>(nr));
+    });
+  }
+  touchKernel(pipelinedAllgatherKernel);
+  cudaGetLastError();
 }
 
 }  // namespace cuda

@@ -463,6 +463,71 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
     });
   }
 
+  // ---- pipelined allgather / reduce_scatter for plain pointers (same aliasing) -----------------
+  // Every virtual rank's slot is my slot, so every block rank 0 pulls is its own input, and the
+  // share it reduces is P copies of share 0 of its input.
+  auto aliasedBulk = [&](int P) {
+    PeerPtrs st;
+    std::memset(&st, 0, sizeof(st));
+    for (int r = 0; r < P; r++) st.p[r] = myStage + 2 * half;
+    return st;
+  };
+  for (int P : {2, 8}) {
+    for (size_t shift : {size_t(0), size_t(1)}) {
+      R.run(strcat_all("pipelinedAllgatherKernel P=", P, shift ? " (out 1 byte off)" : ""), [&]() -> std::string {
+        const CommArgs ca = pc.loopbackComm(P);
+        const int blocks = std::min(pc.coResidentBlocks(pipelinedAllgatherKernelPtr()), 8), tile = 64;
+        const size_t C = static_cast<size_t>(blocks) * tile * 16;
+        GLB_ENFORCE_LE(2 * C, pc.stageBytes() - 2 * half, "pool too small for the pipelined self-test");
+        const size_t bytes = 5 * C + 36;  // five whole chunks and a part that is not a whole 16-byte group
+        std::vector<size_t> offs(P), lens(P, bytes);
+        for (int r = 0; r < P; r++) offs[r] = r * bytes;
+        DevBuf in(bytes), out(P * bytes + shift);
+        launchFill(in.p, bytes / 4, DataType::FLOAT32, 1.0, 1.0, stream);
+        GLB_CUDA_CHECK(cudaMemsetAsync(out.p, 0, out.bytes, stream));
+        launchPipelinedAllgather(ca, in.p, static_cast<char*>(out.p) + shift, offs.data(), lens.data(), -1, aliasedBulk(P),
+                                 tile, 256, blocks, stream);
+        noteLaunch();
+        std::vector<char> hin(bytes), hout(out.bytes);
+        GLB_CUDA_CHECK(cudaMemcpyAsync(hin.data(), in.p, bytes, cudaMemcpyDeviceToHost, stream));
+        GLB_CUDA_CHECK(cudaMemcpyAsync(hout.data(), out.p, out.bytes, cudaMemcpyDeviceToHost, stream));
+        GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+        for (int r = 0; r < P; r++) {
+          if (std::memcmp(hout.data() + shift + offs[r], hin.data(), bytes) != 0) return strcat_all("block ", r, " differs");
+        }
+        return "";
+      });
+    }
+  }
+  // P = 3 runs the generic-P instantiation; P = 8 has uneven shares and an output one element off.
+  for (int P : {2, 8, 3}) {
+    R.run(strcat_all("pipelinedReduceScatterKernel<float,", P == 3 ? 0 : P, "> P=", P), [&]() -> std::string {
+      const CommArgs ca = pc.loopbackComm(P);
+      const void* k = pipelinedReduceScatterKernelFor(DataType::FLOAT32, P);
+      const int blocks = std::min(pc.coResidentBlocks(k), 8), tile = 32;
+      const size_t chunkElems = static_cast<size_t>(blocks) * tile * 4;
+      GLB_ENFORCE_LE(2 * P * chunkElems * 4, pc.stageBytes() - 2 * half, "pool too small for the pipelined self-test");
+      std::vector<size_t> counts(P), off(P + 1, 0);
+      for (int r = 0; r < P; r++) {
+        counts[r] = 3 * chunkElems + (P == 2 ? 0 : 7 + 5 * r);
+        off[r + 1] = off[r] + counts[r];
+      }
+      const size_t shift = P == 8 ? 1 : 0;
+      DevBuf in(off[P] * 4), out((counts[0] + shift) * 4);
+      launchFill(in.p, off[P], DataType::FLOAT32, 0.0, 1.0, stream);  // share 0 = 0, 1, 2, ...
+      GLB_CUDA_CHECK(cudaMemsetAsync(out.p, 0, out.bytes, stream));
+      launchPipelinedReduceScatter(ca, in.p, static_cast<float*>(out.p) + shift, off.data(), counts.data(),
+                                   DataType::FLOAT32, ReduceOp::SUM, 0.5f, aliasedBulk(P), tile, 256, blocks, stream);
+      noteLaunch();
+      auto h = download(out.p, counts[0] + shift, stream);
+      for (size_t i = 0; i < counts[0]; i++) {
+        const double want = 0.5 * P * static_cast<double>(i);
+        if (!close(h[i + shift], want)) return strcat_all("element ", i, ": got ", h[i + shift], " want ", want);
+      }
+      return "";
+    });
+  }
+
   // ---- point to point: fused send + recv through my own mailbox --------------------------------
   R.run("p2pKernel(sendrecv)", [&]() -> std::string {
     const CommArgs ca = pc.loopbackComm(2);

@@ -5,7 +5,10 @@ and offers the collective suite for torch CUDA tensors. A tensor is either
 
 * *registered* (``ctx.register(t)`` or allocated with ``ctx.empty(...)``): kernels
   read/write the peers' copies directly (zero-copy, NVLS-capable when symmetric);
-* anything else: staged through the pool inside the same call.
+* anything else: staged through the per-rank pool (``stage_bytes``) inside the same call.
+  allreduce, broadcast, allgather(v), gather(v) and reduce_scatter take any size: beyond the
+  pool they stream through it in one pipelined kernel. alltoall(v), scatter and reduce still
+  need the payload to fit the pool's bulk region (the pool minus two one-shot halves).
 
 Every method is asynchronous on the current torch stream unless ``stream`` is given,
 and must be called in the same order on every rank.
@@ -261,9 +264,13 @@ class CudaContext:
         return tensor
 
     def allgather(self, output, input, stream=None):
+        """Every rank's ``input`` (same size on all ranks), concatenated in rank order. Any size:
+        a plain ``output`` larger than the staging pool streams through it in one kernel; ``input``
+        may be this rank's slice of ``output`` (in place)."""
         return self.allgatherv(output, input, [input.numel()] * self.size, stream)
 
     def allgatherv(self, output, input, counts: Sequence[int], stream=None):
+        """Like :meth:`allgather` with ``counts[r]`` elements from rank r (zero allowed); any size."""
         es = output.element_size()
         sizes = [int(c) * es for c in counts]
         buf, off = self.lookup(output)
@@ -275,9 +282,12 @@ class CudaContext:
         return output
 
     def gather(self, output, input, root: int = 0, stream=None):
+        """Every rank's ``input`` into the root's ``output``, in rank order; any size. Other ranks
+        may pass ``output=None``; their output is never written."""
         return self.gatherv(output, input, [input.numel()] * self.size, root, stream)
 
     def gatherv(self, output, input, counts: Sequence[int], root: int = 0, stream=None):
+        """Like :meth:`gather` with ``counts[r]`` elements from rank r; any size."""
         es = input.element_size()
         sizes = [int(c) * es for c in counts]
         optr = output.data_ptr() if output is not None else 0
@@ -386,6 +396,10 @@ class CudaContext:
 
     def reduce_scatter(self, output, input, counts: Optional[Sequence[int]] = None, op: ReduceOp = ReduceOp.SUM,
                        stream=None, scale: float = 1.0):
+        """``output`` := share ``rank`` of the reduction of every rank's ``input`` (``counts[r]``
+        elements for rank r, an even split by default), times ``scale`` (floating types), with one
+        rounding. Any size: a plain ``input`` larger than the staging pool streams through it in one
+        kernel; ``output`` may be this rank's share of ``input`` (in place)."""
         ptr, n, dt, _ = describe(input)
         if counts is None:
             base, rem = divmod(n, self.size)

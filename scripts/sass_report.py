@@ -30,6 +30,8 @@ KERNELS = [
     ("cast_f32_to_bf16", r"castAllreduceKernel<float, __nv_bfloat16>"),
     ("pipelined_f32_nvls", r"pipelinedAllreduceKernel<float, true, 0>"),
     ("pipelined_f32_P2", r"pipelinedAllreduceKernel<float, false, 2>"),
+    ("pipelined_allgather", r"pipelinedAllgatherKernel"),
+    ("pipelined_reduce_scatter_bf16_P8", r"pipelinedReduceScatterKernel<__nv_bfloat16, 8>"),
     ("reduce_pull_f32_P8", r"reducePullKernel<float, 8, 2>"),
     ("broadcast", r"broadcastKernel"),
     ("gather_push", r"gatherPushKernel"),

@@ -2,7 +2,15 @@
 """Bandwidth sweep of the data-movement collectives (configs 4 and 5 of BASELINE.json):
 allgather, alltoall, alltoall_v, broadcast, reduce_scatter — 1 KB .. 1 GB per-rank payload,
 device-timed, max over ranks, against the NCCL comparator. torchrun, one rank per GPU.
-Also the named fp16 schedules (config 3) with --schedules."""
+Also the named fp16 schedules (config 3) with --schedules.
+
+--plain (or --threads P) sweeps allgather and reduce_scatter of PLAIN tensors, 1 MB .. 1 GB of
+allgather output / reduce_scatter input, in four arms: "staged" (payload copied through the
+staging pool, where it fits), "pipelined" (the pipelined kernel: the default pool where the
+payload does not fit it, and a second context whose pool is smaller than the payload but holds
+two full-size slots where it does), "registered" (symmetric buffers, zero copy: the ceiling) and
+NCCL (more than one GPU). --threads P runs P ranks as threads on ONE GPU, each on its own
+gcu.new_stream(): the ranks share that GPU's HBM, so those figures are not NVLink figures."""
 import argparse
 import json
 import os
@@ -17,6 +25,135 @@ import gloo_b200 as gb  # noqa: E402
 from gloo_b200.ops import cuda as gcu  # noqa: E402
 
 
+def _timer(ctx, world, stream, flush):
+    def timed(fn, iters):
+        evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(iters)]
+        with torch.cuda.stream(stream):
+            for _ in range(3):
+                fn()
+            for a, b in evs:
+                flush.fill_(0)
+                a.record(stream)
+                fn()
+                b.record(stream)
+        stream.synchronize()
+        per = np.asarray([a.elapsed_time(b) * 1e3 for a, b in evs], dtype=np.float64)
+        if world > 1:
+            gb.allreduce(ctx, per, op=gb.ReduceOp.MAX)
+        per.sort()
+        return float(per[len(per) // 2])
+    return timed
+
+
+# Launch shape of the pipelined kernels at the defaults (GLB_CUDA_BLOCKS, GLB_CUDA_PIPE_TILE): one
+# full-size slot is shares x 128 CTAs x 1024 x 16 bytes.
+FULL_SLOT = 128 * 1024 * 16
+HALVES = 2 * (256 << 10)      # the pool's two one-shot halves (GLB_CUDA_ONESHOT_MAX)
+
+
+def plain_rows(ctx, cc, ctx_small, P, rank, stream, iters, max_bytes, nccl):
+    """Rows of the plain-tensor arms. `ctx_small(stage_bytes)` returns a CudaContext with that
+    pool on a context of its own (a context has one pool per device)."""
+    bulk = cc.pc.stage_bytes() - HALVES
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
+    timed = _timer(ctx, P, stream, flush)
+    F32 = int(gb.DataType.FLOAT32)
+    sizes = [m << 20 for m in (1, 4, 16, 64, 256, 1024) if (m << 20) <= max_bytes]
+    small = {}
+    rows = []
+    for op in ("allgather", "reduce_scatter"):
+        shares = 1 if op == "allgather" else P
+        slots = 2 * shares * FULL_SLOT
+        for total in sizes:
+            n = total // 4 // P * P
+            per = n // P
+            it = iters if total < (64 << 20) else max(5, iters // 4)
+            row = {"op": op + "_plain", "bytes": n * 4}
+            big_in = torch.ones(n if op == "reduce_scatter" else per, device="cuda")
+            big_out = torch.empty(per if op == "reduce_scatter" else n, device="cuda")
+
+            def call(c, o, i):
+                if op == "allgather":
+                    return lambda: c.allgather(o, i, stream=stream)
+                return lambda: c.reduce_scatter(o, i, [per] * P, stream=stream)
+
+            try:
+                if n * 4 <= bulk:
+                    row["staged_us"] = round(timed(call(cc, big_out, big_in), it), 2)
+                    if n * 4 > slots:  # a pool that holds two full-size slots but not the payload
+                        if slots not in small:
+                            small[slots] = ctx_small(slots + HALVES)
+                        row["pipelined_pool_mb"] = round(small[slots].pc.stage_bytes() / 2**20, 1)
+                        row["pipelined_us"] = round(timed(call(small[slots], big_out, big_in), it), 2)
+                else:
+                    row["pipelined_us"] = round(timed(call(cc, big_out, big_in), it), 2)
+                sym_in = cc.empty(big_in.numel(), torch.float32)
+                sym_in.fill_(1)
+                sym_out = cc.empty(big_out.numel(), torch.float32)
+                if op == "allgather":
+                    row["registered_us"] = round(timed(call(cc, sym_out, big_in), it), 2)
+                else:
+                    row["registered_us"] = round(timed(call(cc, big_out, sym_in), it), 2)
+                del sym_in, sym_out
+                if nccl is not None:
+                    if op == "allgather":
+                        fn = lambda: nccl.allgather(big_in.data_ptr(), big_out.data_ptr(), per, F32, stream.cuda_stream)  # noqa: E731
+                    else:
+                        fn = lambda: nccl.reduce_scatter(big_in.data_ptr(), big_out.data_ptr(), per, F32, 1, stream.cuda_stream)  # noqa: E731
+                    row["nccl_us"] = round(timed(fn, it), 2)
+                for k in [k for k in row if k.endswith("_us")]:
+                    row[k[:-3] + "_gbs"] = round(n * 4 / (row[k] * 1e-6) / 1e9, 1)
+            except Exception as e:  # noqa: BLE001
+                row["error"] = f"{type(e).__name__}: {str(e)[:160]}"
+            rows.append(row)
+            if rank == 0:
+                print(json.dumps(row), flush=True)
+            del big_in, big_out
+            torch.cuda.synchronize()
+            gb.barrier(ctx)
+    return rows
+
+
+def card_line():
+    """Name and power limit of the card, read in the same run as the numbers."""
+    import subprocess
+
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
+    except Exception:  # noqa: BLE001
+        return torch.cuda.get_device_name()
+
+
+def threads_main(args):
+    P = args.threads
+    print(f"card: {card_line()}; {P} ranks as threads on cuda:0 sharing its HBM (not NVLink figures)", flush=True)
+
+    def fn(ctx):
+        stream = gcu.new_stream(0)
+        made = []
+
+        def ctx_small(stage):
+            # A second context over the same threads (a context has one pool per device).
+            c2 = gb.init_context(ctx.rank, P, store=store, prefix=f"small{len(made)}", timeout_ms=120000)
+            made.append(c2)
+            return gcu.CudaContext(c2, 0, stage_bytes=stage)
+
+        cc = gcu.CudaContext(ctx, 0, stage_bytes=128 << 20)
+        rows = plain_rows(ctx, cc, ctx_small, P, ctx.rank, stream, args.iters, args.max_bytes, None)
+        torch.cuda.synchronize()
+        for c2 in made:
+            gb.barrier(c2)
+        return rows
+
+    store = gb._C.HashStore()
+    rows = gb.spawn_threads(P, fn, cuda_device=0, timeout_ms=120000)[0]
+    if args.out:
+        with open(args.out, "w") as f:
+            json.dump({"threads": P, "card": card_line(), "rows": rows}, f, indent=1)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default="")
@@ -24,7 +161,12 @@ def main():
     ap.add_argument("--max-bytes", type=int, default=1 << 30)
     ap.add_argument("--ops", default="allgather,alltoall,alltoall_v,broadcast,reduce_scatter")
     ap.add_argument("--schedules", action="store_true")
+    ap.add_argument("--plain", action="store_true", help="also the plain-tensor allgather / reduce_scatter arms")
+    ap.add_argument("--threads", type=int, default=0, help="P ranks as threads on one GPU (plain arms only)")
     args = ap.parse_args()
+    if args.threads:
+        threads_main(args)
+        return
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local = int(os.environ.get("LOCAL_RANK", 0))
     torch.cuda.set_device(local)
@@ -42,23 +184,7 @@ def main():
     stream = torch.cuda.Stream()
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     F32 = int(gb.DataType.FLOAT32)
-
-    def timed(fn, iters):
-        evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(iters)]
-        with torch.cuda.stream(stream):
-            for _ in range(3):
-                fn()
-            for a, b in evs:
-                flush.fill_(0)
-                a.record(stream)
-                fn()
-                b.record(stream)
-        stream.synchronize()
-        per = np.asarray([a.elapsed_time(b) * 1e3 for a, b in evs], dtype=np.float64)
-        if world > 1:
-            gb.allreduce(ctx, per, op=gb.ReduceOp.MAX)
-        per.sort()
-        return float(per[len(per) // 2])
+    timed = _timer(ctx, world, stream, flush)
 
     rows = []
     sizes = []
@@ -176,6 +302,18 @@ def main():
                     print(json.dumps(row), flush=True)
                 torch.cuda.synchronize()
                 gb.barrier(ctx)
+    if args.plain:
+        if rank == 0:
+            print(f"card: {card_line()}", flush=True)
+        smalls = []
+
+        def ctx_small(stage):
+            c2 = gb.init_context(rank, world, path=f"/tmp/glb_swc_small{len(smalls)}_{os.environ.get('MASTER_PORT', '0')}_"
+                                 f"{os.getppid()}", timeout_ms=120000)
+            smalls.append(c2)
+            return gcu.CudaContext(c2, local, stage_bytes=stage)
+
+        rows += plain_rows(ctx, cc, ctx_small, world, rank, stream, args.iters, args.max_bytes, nccl)
     if rank == 0 and args.out:
         with open(args.out, "w") as f:
             json.dump({"world": world, "describe": cc.describe(), "rows": rows}, f, indent=1)
