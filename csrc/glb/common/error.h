@@ -5,8 +5,10 @@
 //   ├── IoException                 transport failure; the context is poisoned and
 //   │   └── TimeoutException        must be re-created (same contract as the
 //   │                               reference, docs/errors.md:5-13)
-//   ├── InputException              bad data found on the device (a collective's
-//   │                               device-side counts); the context stays usable
+//   ├── InputException              bad input: data found on the device (a collective's
+//   │                               device-side counts) or buffers a collective cannot
+//   │                               take (overlapping input and output); the context
+//   │                               stays usable
 //   └── EnforceNotMet               failed GLB_ENFORCE (logging.h)
 //
 // Parity: gloo/common/error.h:21-48.

@@ -228,7 +228,9 @@ void runOneShot(PeerContext& pc, const void* in, void* out, size_t count, DataTy
 // Launch shape of a kernel that pipelines plain pointers through `slots` pool slots, each of
 // `shares` x blocks x tile 16-byte groups. `payloadBytes` is the largest payload in the same
 // units as one slot (the whole vector for the allreduce, P x the largest share for
-// reduce_scatter, the largest block for allgather). A zero hint takes the tuning default.
+// reduce_scatter and reduce, the largest block for allgather, P x the block for alltoall and
+// scatter, and the bulk region for alltoallv, whose byte counts are rank-local). A zero hint takes
+// the tuning default.
 struct PipeShape {
   int blocks = 1;
   int tile = 16;
@@ -757,6 +759,34 @@ void alltoallCommon(PeerContext& pc, const void* in, const std::vector<size_t>& 
                      -1, vec, blocks, stream);
   finish(pc, stream, "alltoall");
 }
+
+// Plain pointers beyond the staged path: one kernel streams the blocks through two pool slots
+// (pipeline_kernels.cu). `shapeBytes` sizes the launch and must be the same on every rank: the grid
+// and the tile feed the step count and the barrier pairing.
+void runPipelinedAlltoall(PeerContext& pc, const void* in, void* out, const std::vector<size_t>& sendBytes,
+                          const std::vector<size_t>& recvBytes, size_t shapeBytes, const char* what,
+                          cudaStream_t stream) {
+  GLB_TRACE_RANGE("glb::cuda::alltoall/scatter(pipelined)");
+  GLB_ENFORCE_EQ(static_cast<int>(sendBytes.size()), pc.size, what, ": need one send size per rank");
+  GLB_ENFORCE_EQ(static_cast<int>(recvBytes.size()), pc.size, what, ": need one recv size per rank");
+  auto soff = prefix(sendBytes);
+  auto roff = prefix(recvBytes);
+  const PipeShape sh = pipeShape(pc, pipelinedAlltoallKernelPtr(), 2, pc.size, shapeBytes, 0, 0, 0, what);
+  prologue(pc, stream);
+  launchPipelinedAlltoall(pc.comm(), in, out, soff.data(), sendBytes.data(), roff.data(), recvBytes.data(),
+                          pc.stagePtrs(layoutOf(pc).bulkOff), sh.tile, sh.xthreads, sh.blocks, stream);
+  finish(pc, stream, what);
+}
+
+// The pipelined exchange writes the output while later chunks of the input are still to be read,
+// so, as in NCCL, the two buffers must not overlap. The check sees this rank's pointers only: a
+// rank that raises here does not launch, and peers that did launch wait for it until the timeout.
+void rejectOverlap(const void* in, size_t inBytes, const void* out, size_t outBytes, const char* what) {
+  const uintptr_t i = reinterpret_cast<uintptr_t>(in), o = reinterpret_cast<uintptr_t>(out);
+  if (inBytes > 0 && outBytes > 0 && i < o + outBytes && o < i + inBytes) {
+    GLB_THROW(InputException, what, ": the input and output buffers overlap, which is not supported");
+  }
+}
 }  // namespace
 
 void alltoall(PeerContext& pc, const void* in, const PeerBuffer& out, size_t outOffset, size_t bytes,
@@ -780,6 +810,12 @@ void alltoall(PeerContext& pc, const void* in, void* out, size_t bytes, cudaStre
     return;
   }
   if (tryLLExchange(pc, in, out, bytes, 1, stream)) return;
+  if (exceedsBulk(pc, bytes * pc.size)) {
+    rejectOverlap(in, bytes * pc.size, out, bytes * pc.size, "alltoall");
+    std::vector<size_t> sizes(pc.size, bytes);
+    runPipelinedAlltoall(pc, in, out, sizes, sizes, bytes * pc.size, "alltoall(pipelined)", stream);
+    return;
+  }
   auto st = stagedBulk(pc, bytes * pc.size, "alltoall");
   std::vector<size_t> sizes(pc.size, bytes);
   alltoallCommon(pc, in, sizes, st.ptrs, true, sizes, true, stream);
@@ -802,15 +838,15 @@ void alltoallv(PeerContext& pc, const void* in, const std::vector<size_t>& sendB
 void alltoallv(PeerContext& pc, const void* in, const std::vector<size_t>& sendBytes, void* out,
                const std::vector<size_t>& recvBytes, cudaStream_t stream) {
   DeviceGuard g(pc.device);
-  auto roff = prefix(recvBytes);
   if (pc.size == 1) {
     if (out != in && sendBytes[0] > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(out, in, sendBytes[0], cudaMemcpyDeviceToDevice, stream));
     return;
   }
-  // Every rank stages the same span so the (data-dependent) fit check cannot diverge.
-  auto st = stagedBulk(pc, roff.back(), "alltoall");
-  alltoallCommon(pc, in, sendBytes, st.ptrs, true, recvBytes, false, stream);
-  if (roff.back() > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(out, st.mine, roff.back(), cudaMemcpyDeviceToDevice, stream));
+  rejectOverlap(in, prefix(sendBytes).back(), out, prefix(recvBytes).back(), "alltoallv");
+  // Always the pipelined kernel: the byte counts are rank-local, so no rule that every rank
+  // evaluates alike could choose between it and a staged launch. The kernel agrees on its step
+  // count on the device, and its launch shape comes from the pool size alone.
+  runPipelinedAlltoall(pc, in, out, sendBytes, recvBytes, layoutOf(pc).bulkBytes, "alltoallv(pipelined)", stream);
 }
 
 namespace {
@@ -888,6 +924,14 @@ void scatter(PeerContext& pc, const void* in, void* out, size_t bytes, int root,
   DeviceGuard g(pc.device);
   if (pc.size == 1) {
     if (out != in && bytes > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(out, in, bytes, cudaMemcpyDeviceToDevice, stream));
+    return;
+  }
+  GLB_ENFORCE(root >= 0 && root < pc.size, "scatter: invalid root ", root);
+  if (exceedsBulk(pc, bytes)) {
+    // Only the root sends; every rank receives its block from the root.
+    std::vector<size_t> send(pc.size, pc.rank == root ? bytes : 0), recv(pc.size, 0);
+    recv[root] = bytes;
+    runPipelinedAlltoall(pc, in, out, send, recv, bytes * pc.size, "scatter(pipelined)", stream);
     return;
   }
   auto st = stagedBulk(pc, bytes, "scatter");
@@ -1035,17 +1079,31 @@ void reduce(PeerContext& pc, const void* in, void* out, size_t count, DataType d
     if (in != out && count > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(out, in, count * es, cudaMemcpyDeviceToDevice, stream));
     return;
   }
-  // Stage inputs in the first half of the bulk region, collect results in the second.
+  GLB_ENFORCE(root >= 0 && root < pc.size, "reduce: invalid root ", root);
+  std::vector<size_t> counts(pc.size);
+  for (int r = 0; r < pc.size; r++) counts[r] = count / pc.size + (static_cast<size_t>(r) < count % pc.size ? 1 : 0);
+  auto off = prefix(counts);
   const auto l = layoutOf(pc);
   const size_t half = l.bulkBytes / 2 / 16 * 16;
-  GLB_ENFORCE_LE(count * es, half, "reduce: payload does not fit the staging pool; register the buffers");
+  if (count * es > half) {
+    // Larger than the staged path takes: one kernel streams the shares through the pool and the
+    // root pulls the reduced shares (pipeline_kernels.cu). count and the pool size are the same on
+    // every rank, so every rank takes this path together.
+    GLB_TRACE_RANGE("glb::cuda::reduce(pipelined)");
+    GLB_ENFORCE(op != ReduceOp::CUSTOM, "custom reductions run on the host path only");
+    const PipeShape sh = pipeShape(pc, pipelinedReduceKernelFor(dt, pc.size), 2, pc.size + 1, counts[0] * es * pc.size,
+                                   0, 0, 0, "reduce");
+    prologue(pc, stream);
+    launchPipelinedReduce(pc.comm(), in, out, off.data(), counts.data(), root, dt, op, pc.stagePtrs(l.bulkOff), sh.tile,
+                          sh.xthreads, sh.blocks, stream);
+    finish(pc, stream, "reduce(pipelined)");
+    return;
+  }
+  // Stage inputs in the first half of the bulk region, collect results in the second.
   PeerPtrs ins = pc.stagePtrs(l.bulkOff);
   PeerPtrs outs = pc.stagePtrs(l.bulkOff + half);
   char* mine = static_cast<char*>(ins.p[pc.rank]);
   if (count > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(mine, in, count * es, cudaMemcpyDeviceToDevice, stream));
-  std::vector<size_t> counts(pc.size);
-  for (int r = 0; r < pc.size; r++) counts[r] = count / pc.size + (static_cast<size_t>(r) < count % pc.size ? 1 : 0);
-  auto off = prefix(counts);
   char* dst = static_cast<char*>(outs.p[root]) + off[pc.rank] * es;
   reducePullCommon(pc, ins, pc.stageMc(l.bulkOff), true, dst, counts, dt, op, 1.0, stream);
   if (pc.rank == root && count > 0) {

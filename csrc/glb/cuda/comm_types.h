@@ -70,6 +70,15 @@ struct alignas(128) SignalPad {
   // Grid barrier among this rank's own CTAs of one launch: arrivals, generation.
   uint32_t a2aArrive;
   uint32_t a2aGen;
+  // Pipelined all-to-all (pipelinedAlltoallKernel): before its first barrier rank s writes the
+  // number of chunks it needs into column s of this table in EVERY rank's pad (the layout of
+  // `flag`), so after the barrier each rank takes the maximum over its own row. Rank s rewrites its
+  // column only in a later launch, after all its CTAs have passed this launch's final barrier, and
+  // CTA b of every reader arrives there only after it has read (it reads right after barrier 1).
+  // That needs the final barrier to be a later one than barrier 1: the kernel runs at least two
+  // steps, even when every block is empty. 32-bit entries: in the loopback self-test peer pads are
+  // this pad shifted by one column, which keeps them aligned.
+  uint32_t pipeChunks[kMaxRanks];
 };
 
 struct CommArgs {

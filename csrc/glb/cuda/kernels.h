@@ -72,6 +72,20 @@ const void* pipelinedReduceScatterKernelFor(DataType dt, int nranks);
 void launchPipelinedReduceScatter(const CommArgs& a, const void* in, void* out, const size_t* elemOff,
                                   const size_t* elemLen, DataType dt, ReduceOp op, float scale, const PeerPtrs& stage,
                                   int tileVecs, int exchangeThreads, int blocks, cudaStream_t stream);
+// reduce to `root` of plain pointers of any size: `count` elements cut into the shares of
+// reduce_scatter (elemOff / elemLen); only the root writes `out` (null elsewhere is fine).
+const void* pipelinedReduceKernelFor(DataType dt, int nranks);
+void launchPipelinedReduce(const CommArgs& a, const void* in, void* out, const size_t* elemOff, const size_t* elemLen,
+                           int root, DataType dt, ReduceOp op, const PeerPtrs& stage, int tileVecs, int exchangeThreads,
+                           int blocks, cudaStream_t stream);
+// alltoall(v) / scatter of plain pointers of any size: my block for rank j is sendLen[j] bytes at
+// sendOff[j] of `in`; the block from rank q lands at recvOff[q] of `out` (recvLen[q] bytes). The
+// lengths may differ between ranks: the kernel agrees on the step count on the device. Scatter:
+// only the root sends, and every rank receives from the root only.
+const void* pipelinedAlltoallKernelPtr();
+void launchPipelinedAlltoall(const CommArgs& a, const void* in, void* out, const size_t* sendOff, const size_t* sendLen,
+                             const size_t* recvOff, const size_t* recvLen, const PeerPtrs& stage, int tileVecs,
+                             int exchangeThreads, int blocks, cudaStream_t stream);
 
 // collective_kernels.cu -----------------------------------------------------------------------
 void launchBroadcast(const CommArgs& a, const PeerPtrs& bufs, void* mc, size_t bytes, int root, int mode, bool vec,

@@ -34,6 +34,21 @@
 // a rank fills in step i+1 is the slot its peers read in step i; the rank starts step i+1 only
 // after barrier i, and it passes barrier i only when CTA b of every peer has finished step i.
 //
+// alltoall(v) / scatter and reduce use the same framework and also pull:
+//  * pipelinedAlltoallKernel: two slots of P sub-slots of C bytes. A(i) copies chunk i of my block
+//    for rank j into sub-slot j of my slot i % 2 (my own block straight to the output); B(i-1)
+//    pulls sub-slot `me` of slot (i-1) % 2 of every peer into the output. Two slots are enough for
+//    the reason above. The v-variant's lengths are rank-local, so the ranks agree on the chunk
+//    count on the device: each publishes its need before barrier 1 (SignalPad::pipeChunks) and
+//    all run max(maximum, 1) + 1 steps. Even when every block is empty there are two barriers,
+//    so the table is read before the final barrier (see SignalPad::pipeChunks).
+//  * pipelinedReduceKernel: the input slots of reduce_scatter plus two result slots of C bytes,
+//    three stages and chunks + 2 steps. B(i-1) reduces my share of chunk i-1; the root stores it
+//    to the output, every other rank to its own result slot (i-1) % 2. C(i-2), root only, pulls
+//    share q of chunk i-2 from peer q's result slot (i-2) % 2. Two result slots are enough: a rank
+//    rewrites result slot k in step k+2, after barrier k+1, which it passes only when the root's
+//    CTA b has finished step k+1, the step in which the root reads that slot.
+//
 // Pool rules, which every kernel that uses the bulk region keeps, so that consecutive calls
 // need no other synchronisation:
 //  * Before its first barrier, a kernel writes only its own pool. A peer may still be reading
@@ -515,6 +530,257 @@ pipelinedReduceScatterKernel(CommArgs a, const T* in, T* out, PipeBlocks pb, Dev
   retire(a, static_cast<uint32_t>(nchunks + 1), 0);
 }
 
+// The two data stages of the pipelined reduce below. They do what the A and B stages of the
+// reduce_scatter kernel above do; that kernel keeps its own copy, whose code generation (registers,
+// no spills) was tuned on its own.
+//
+// B stage: n elements (one tile) at byte `srcOff` of every rank's pool, reduced in the accumulator
+// type of PackTraits, scaled, rounded once and stored to dst. dst may start at an address that is
+// not 16-byte aligned (element-wise stores at its groups).
+template <typename T, int NR>
+__device__ __forceinline__ void reducePoolTile(const PeerPtrs& stage, int P, int me, size_t srcOff, T* dst, size_t n,
+                                               DevOp op, float scale, bool outAligned, int xt, int xn) {
+  using PT = PackTraits<T>;
+  const size_t ng = (n + PT::kElems - 1) / PT::kElems;
+  // Rank-rotated order, kSlots x U independent 128-bit loads in flight per thread (half the packs
+  // for 16-lane FP8), any P in batches. Half of reduce_scatter's depth: the kernel also carries the
+  // root's pull stage. Any P takes each peer's address from `stage` at its load instead of holding
+  // 16 pointers in registers. Both keep every instantiation free of spills (-Xptxas -v).
+  constexpr int kSlots = NR > 0 ? NR : kMaxRanks;
+  constexpr int kWide = PT::kElems > 8 ? 2 : 1;
+  constexpr int U0 = NR == 2 ? 4 : (NR == 4 ? 2 : 1);
+  constexpr int U = U0 / kWide > 0 ? U0 / kWide : 1;
+  constexpr int kBatch = sizeof(T) == 8 || PT::kElems > 8 ? 2 : 4;
+  if constexpr (kSlots > 8) {
+    // Any P: the peers' packs come in batches (same order).
+    for (size_t o = xt; o < ng; o += static_cast<size_t>(xn)) {
+      typename PT::AccPack acc;
+#pragma unroll
+      for (int b0 = 0; b0 < kSlots; b0 += kBatch) {
+        Pack16 v[kBatch];
+#pragma unroll
+        for (int q = 0; q < kBatch; q++) {
+          if (b0 + q < P) {
+            const int r = me + b0 + q < P ? me + b0 + q : me + b0 + q - P;
+            v[q] = ld128_stream(static_cast<const char*>(stage.p[r]) + srcOff + o * 16);
+          }
+        }
+#pragma unroll
+        for (int q = 0; q < kBatch; q++) {
+          if (b0 + q == 0) {
+            acc = PT::widen(v[q]);
+          } else if (b0 + q < P) {
+            PT::combine(acc, v[q], op);
+          }
+        }
+      }
+      if (scale != 1.0f) PT::scale(acc, scale);
+      storeGroupP(dst, o, n, outAligned, PT::narrow(acc));
+    }
+  } else {
+    const char* peer[kSlots];
+#pragma unroll
+    for (int q = 0; q < kSlots; q++) {
+      peer[q] = q < P ? static_cast<const char*>(stage.p[(me + q) % P]) + srcOff : nullptr;
+    }
+    for (size_t o0 = xt; o0 < ng; o0 += static_cast<size_t>(xn) * U) {
+      Pack16 v[U][kSlots];
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        const size_t o = o0 + static_cast<size_t>(u) * xn;
+        if (o < ng) {
+#pragma unroll
+          for (int q = 0; q < kSlots; q++) {
+            if (q < P) v[u][q] = ld128_stream(peer[q] + o * 16);
+          }
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        const size_t o = o0 + static_cast<size_t>(u) * xn;
+        if (o < ng) {
+          typename PT::AccPack acc = PT::widen(v[u][0]);
+#pragma unroll
+          for (int q = 1; q < kSlots; q++) {
+            if (q < P) PT::combine(acc, v[u][q], op);
+          }
+          if (scale != 1.0f) PT::scale(acc, scale);
+          storeGroupP(dst, o, n, outAligned, PT::narrow(acc));
+        }
+      }
+    }
+  }
+}
+
+// A stage: chunk i of every share of `in` -> sub-slot q
+// of `slot` (tile b of it; `slot` already points at the tile).
+template <typename T>
+__device__ __forceinline__ void stageShares(const T* in, const PipeBlocks& pb, int P, size_t i, size_t chunkElems,
+                                            size_t tileElems, size_t C, char* slot, int ct, int cn) {
+  using PT = PackTraits<T>;
+  constexpr int CU = PT::kElems > 8 ? 2 : 4;
+  for (int q = 0; q < P; q++) {
+    const size_t n = tilePart(pb.len[q], i, chunkElems, tileElems);
+    if (n == 0) continue;
+    const size_t ng = (n + PT::kElems - 1) / PT::kElems;
+    const T* src = in + pb.off[q] + i * chunkElems + blockIdx.x * tileElems;
+    const bool aligned = reinterpret_cast<uintptr_t>(src) % 16 == 0;
+    for (size_t j0 = ct; j0 < ng; j0 += static_cast<size_t>(cn) * CU) {
+      Pack16 p[CU];
+#pragma unroll
+      for (int u = 0; u < CU; u++) {
+        const size_t j = j0 + static_cast<size_t>(u) * cn;
+        if (j < ng) p[u] = loadGroupP(src, j, n, aligned);
+      }
+#pragma unroll
+      for (int u = 0; u < CU; u++) {
+        const size_t j = j0 + static_cast<size_t>(u) * cn;
+        if (j < ng) st128(slot + q * C + j * 16, p[u]);
+      }
+    }
+  }
+}
+
+// reduce to `root`: the shares are those of reduce_scatter, with three stages and two more pool
+// slots of C bytes (the result slots) after the two input slots.
+//   A(i)    chunk i of every share of `in` -> my input slot i % 2                     (local HBM)
+//   B(i-1)  sub-slot `me` of input slot (i-1) % 2 from all P pools, reduced; the root stores
+//           its share to `out`, every other rank to its OWN result slot (i-1) % 2       (NVLink)
+//   C(i-2)  root only: share q of chunk i-2 from result slot (i-2) % 2 of peer q -> out (NVLink)
+// chunks + 2 steps, one barrier each. A non-root never touches `out` (it may be null).
+template <typename T, int NR>
+__global__ void __launch_bounds__(kThreads)
+pipelinedReduceKernel(CommArgs a, const T* in, T* out, PipeBlocks pb, int root, DevOp op, PeerPtrs stage, int tileVecs,
+                      int exchangeThreads) {
+  using PT = PackTraits<T>;
+  const int P = NR > 0 ? NR : a.nranks;
+  const int me = a.rank;
+  const bool isRoot = me == root;
+  const size_t T_ = static_cast<size_t>(tileVecs);
+  const size_t tileElems = T_ * PT::kElems;
+  const size_t chunkElems = gridDim.x * tileElems;
+  const size_t C = chunkElems * sizeof(T);
+  const size_t slotBytes = static_cast<size_t>(P) * C;
+  const size_t resultOff = 2 * slotBytes;
+  const size_t nchunks = (largestOf(pb, P) + chunkElems - 1) / chunkElems;
+  const size_t tileOff = blockIdx.x * T_ * 16;
+  const uint32_t e = loadEpoch(a);
+  char* myStage = static_cast<char*>(stage.p[me]);
+  const bool outAligned = !isRoot || reinterpret_cast<uintptr_t>(out + pb.off[me]) % 16 == 0;
+  const bool exchanger = static_cast<int>(threadIdx.x) < exchangeThreads;
+  const int xt = threadIdx.x, xn = exchangeThreads;
+  const int ct = threadIdx.x - exchangeThreads, cn = blockDim.x - exchangeThreads;
+
+  for (size_t i = 0; i < nchunks + 2; i++) {
+    if (exchanger) {
+      // ---- B(i-1): reduce my share's tile of chunk i-1 from every pool ----
+      const size_t c = i - 1;
+      const size_t n = i >= 1 && c < nchunks ? tilePart(pb.len[me], c, chunkElems, tileElems) : 0;
+      if (n > 0) {
+        T* dst = isRoot ? out + pb.off[me] + c * chunkElems + blockIdx.x * tileElems
+                        : reinterpret_cast<T*>(myStage + resultOff + (c % 2) * C + tileOff);
+        reducePoolTile<T, NR>(stage, P, me, (c % 2) * slotBytes + me * C + tileOff, dst, n, op, 1.0f, outAligned, xt,
+                              xn);
+      }
+    } else {
+      // ---- C(i-2): the root pulls every peer's reduced share of chunk i-2 ----
+      if (isRoot && i >= 2) {
+        const size_t c = i - 2;
+        for (int k = 1; k < P; k++) {
+          const int q = (me + k) % P;
+          const size_t n = tilePart(pb.len[q], c, chunkElems, tileElems);
+          if (n > 0) {
+            gridCopy(reinterpret_cast<char*>(out + pb.off[q] + c * chunkElems + blockIdx.x * tileElems),
+                     static_cast<const char*>(stage.p[q]) + resultOff + (c % 2) * C + tileOff, n * sizeof(T), true, ct,
+                     cn);
+          }
+        }
+      }
+      // ---- A(i): chunk i of every share -> my input slot ----
+      if (i < nchunks) {
+        stageShares(in, pb, P, i, chunkElems, tileElems, C, myStage + (i % 2) * slotBytes + tileOff, ct, cn);
+      }
+    }
+    if (!blockBarrier(a, e + static_cast<uint32_t>(i) + 1)) break;
+  }
+  retire(a, static_cast<uint32_t>(nchunks + 2), 0);
+}
+
+// alltoall(v) and scatter. Slot: P sub-slots of C bytes, sub-slot j = chunk i of my block for
+// destination j. Block j of `in` is send.len[j] bytes at send.off[j]; the block from source q lands
+// at out + recv.off[q] (recv.len[q] bytes).
+//   A(i)    chunk i of my block for every destination j != me -> sub-slot j of my slot i % 2; my
+//           own block straight from `in` to out + recv.off[me]                         (local HBM)
+//   B(i-1)  sub-slot `me` of slot (i-1) % 2 of every peer q -> out + recv.off[q] + (i-1)·C (NVLink)
+// Scatter is the form in which only the root has blocks to send and every rank receives from the
+// root only: a non-root never reads `in`.
+// The step count: the lengths are rank-local (alltoallv), so each rank publishes the chunks it
+// needs in the pipeChunks table before barrier 1 and every rank runs max(max, 1) + 1 steps. A(0)
+// depends only on my own lengths, so it runs before that maximum is known. At least one chunk, so
+// at least two barriers, even when every block is empty: the table is read between barrier 1 and
+// the final barrier, and a peer rewrites its column in its next launch only after passing that
+// final barrier, i.e. after every reader has read. With a single barrier, a peer could pass it,
+// start its next launch and rewrite its column before a slow CTA here has read this launch's value.
+__global__ void __launch_bounds__(kThreads)
+pipelinedAlltoallKernel(CommArgs a, const char* in, char* out, PipeBlocks send, PipeBlocks recv, PeerPtrs stage,
+                        int tileVecs, int exchangeThreads) {
+  const int P = a.nranks, me = a.rank;
+  const size_t tileBytes = static_cast<size_t>(tileVecs) * 16;
+  const size_t C = gridDim.x * tileBytes;
+  const size_t slotBytes = static_cast<size_t>(P) * C;
+  const size_t tileOff = blockIdx.x * tileBytes;
+  const uint32_t e = loadEpoch(a);
+  char* myStage = static_cast<char*>(stage.p[me]);
+  const size_t ownLen = send.len[me] < recv.len[me] ? send.len[me] : recv.len[me];
+  const bool exchanger = static_cast<int>(threadIdx.x) < exchangeThreads;
+  const int xt = threadIdx.x, xn = exchangeThreads;
+  const int ct = threadIdx.x - exchangeThreads, cn = blockDim.x - exchangeThreads;
+  // Every CTA writes the same value: the barrier pairs CTA b with CTA b only, so the column a CTA
+  // reads must have been written by its own twin. The thread that writes peer q's pad is the one
+  // that releases the barrier flag to q.
+  if (threadIdx.x < P) {
+    const size_t largest = largestOf(send, P) > largestOf(recv, P) ? largestOf(send, P) : largestOf(recv, P);
+    st_relaxed_sys(&a.sig[threadIdx.x]->pipeChunks[me], static_cast<uint32_t>((largest + C - 1) / C));
+  }
+
+  size_t nchunks = 0;  // known after barrier 1
+  for (size_t i = 0; i < nchunks + 1; i++) {
+    if (exchanger) {
+      // ---- B(i-1): pull my sub-slot of chunk i-1 from every peer ----
+      if (i >= 1) {
+        const size_t c = i - 1;
+        for (int k = 1; k < P; k++) {
+          const int q = (me + k) % P;
+          const size_t n = tilePart(recv.len[q], c, C, tileBytes);
+          if (n > 0) {
+            gridCopy(out + recv.off[q] + c * C + tileOff,
+                     static_cast<const char*>(stage.p[q]) + (c % 2) * slotBytes + me * C + tileOff, n, true, xt, xn);
+          }
+        }
+      }
+    } else {
+      // ---- A(i): chunk i of every block -> my slot (my own block -> out) ----
+      for (int k = 0; k < P; k++) {
+        const int j = (me + k) % P;
+        const size_t n = tilePart(j == me ? ownLen : send.len[j], i, C, tileBytes);
+        if (n > 0) {
+          char* dst = j == me ? out + recv.off[me] + i * C + tileOff : myStage + (i % 2) * slotBytes + j * C + tileOff;
+          gridCopy(dst, in + send.off[j] + i * C + tileOff, n, true, ct, cn);
+        }
+      }
+    }
+    if (!blockBarrier(a, e + static_cast<uint32_t>(i) + 1)) break;
+    if (i == 0) {
+      nchunks = 1;  // at least two barriers: the read below must come before the final one
+      for (int q = 0; q < P; q++) {
+        const size_t need = ld_relaxed_sys(&a.self->pipeChunks[q]);
+        nchunks = need > nchunks ? need : nchunks;
+      }
+    }
+  }
+  retire(a, static_cast<uint32_t>(nchunks + 1), 0);
+}
+
 namespace {
 // The pipelined reduce_scatter instantiation for (T, P).
 template <typename T>
@@ -525,6 +791,17 @@ auto pipeRsFn(int nranks) {
     if (nranks == 8) return pipelinedReduceScatterKernel<T, 8>;
   }
   return pipelinedReduceScatterKernel<T, 0>;
+}
+
+// The pipelined reduce instantiation for (T, P).
+template <typename T>
+auto pipeReduceFn(int nranks) {
+  if constexpr (isHotType<T>()) {
+    if (nranks == 2) return pipelinedReduceKernel<T, 2>;
+    if (nranks == 4) return pipelinedReduceKernel<T, 4>;
+    if (nranks == 8) return pipelinedReduceKernel<T, 8>;
+  }
+  return pipelinedReduceKernel<T, 0>;
 }
 
 PipeBlocks pipeBlocks(int nranks, const size_t* offs, const size_t* lens) {
@@ -538,10 +815,17 @@ PipeBlocks pipeBlocks(int nranks, const size_t* offs, const size_t* lens) {
 }  // namespace
 
 const void* pipelinedAllgatherKernelPtr() { return reinterpret_cast<const void*>(pipelinedAllgatherKernel); }
+const void* pipelinedAlltoallKernelPtr() { return reinterpret_cast<const void*>(pipelinedAlltoallKernel); }
 
 const void* pipelinedReduceScatterKernelFor(DataType dt, int nranks) {
   const void* k = nullptr;
   dispatchType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(pipeRsFn<decltype(tag)>(nranks)); });
+  return k;
+}
+
+const void* pipelinedReduceKernelFor(DataType dt, int nranks) {
+  const void* k = nullptr;
+  dispatchType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(pipeReduceFn<decltype(tag)>(nranks)); });
   return k;
 }
 
@@ -565,16 +849,40 @@ void launchPipelinedReduceScatter(const CommArgs& a, const void* in, void* out, 
   });
 }
 
+void launchPipelinedReduce(const CommArgs& a, const void* in, void* out, const size_t* elemOff, const size_t* elemLen,
+                           int root, DataType dt, ReduceOp op, const PeerPtrs& stage, int tileVecs, int exchangeThreads,
+                           int blocks, cudaStream_t stream) {
+  dispatchType(dt, [&](auto tag) {
+    using T = decltype(tag);
+    pipeReduceFn<T>(a.nranks)<<<blocks, kThreads, 0, stream>>>(a, static_cast<const T*>(in), static_cast<T*>(out),
+                                                               pipeBlocks(a.nranks, elemOff, elemLen), root,
+                                                               static_cast<DevOp>(op), stage, tileVecs, exchangeThreads);
+  });
+}
+
+void launchPipelinedAlltoall(const CommArgs& a, const void* in, void* out, const size_t* sendOff, const size_t* sendLen,
+                             const size_t* recvOff, const size_t* recvLen, const PeerPtrs& stage, int tileVecs,
+                             int exchangeThreads, int blocks, cudaStream_t stream) {
+  pipelinedAlltoallKernel<<<blocks, kThreads, 0, stream>>>(a, static_cast<const char*>(in), static_cast<char*>(out),
+                                                           pipeBlocks(a.nranks, sendOff, sendLen),
+                                                           pipeBlocks(a.nranks, recvOff, recvLen), stage, tileVecs,
+                                                           exchangeThreads);
+}
+
 void preloadPipelineKernels() {
   for (DataType dt : kAllDataTypes) {
     dispatchType(dt, [](auto tag) {
       for (bool mc : {false, true}) {
         for (int nr : {0, 2, 4, 8}) touchKernel(pipeFn<decltype(tag)>(mc, nr));
       }
-      for (int nr : {0, 2, 4, 8}) touchKernel(pipeRsFn<decltype(tag)>(nr));
+      for (int nr : {0, 2, 4, 8}) {
+        touchKernel(pipeRsFn<decltype(tag)>(nr));
+        touchKernel(pipeReduceFn<decltype(tag)>(nr));
+      }
     });
   }
   touchKernel(pipelinedAllgatherKernel);
+  touchKernel(pipelinedAlltoallKernel);
   cudaGetLastError();
 }
 

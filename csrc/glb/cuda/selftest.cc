@@ -527,6 +527,98 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
       return "";
     });
   }
+  // reduce to root 0 with every virtual rank's slots aliasing mine: rank 0 stores P copies of share 0
+  // of its input as its own share, and pulls every other share from "peer q's" result slot, which is
+  // its own, which a root never writes: zero, as cleared here. The output starts filled with NaN.
+  // P = 2 has even shares; P = 8 uneven ones and an output one element off; P = 3 is generic.
+  for (int P : {2, 8, 3}) {
+    R.run(strcat_all("pipelinedReduceKernel<float,", P == 3 ? 0 : P, "> P=", P), [&]() -> std::string {
+      const CommArgs ca = pc.loopbackComm(P);
+      const int blocks = std::min(pc.coResidentBlocks(pipelinedReduceKernelFor(DataType::FLOAT32, P)), 8), tile = 32;
+      const size_t chunkElems = static_cast<size_t>(blocks) * tile * 4, C = chunkElems * 4;
+      GLB_ENFORCE_LE((2 * P + 2) * C, pc.stageBytes() - 2 * half, "pool too small for the pipelined self-test");
+      const size_t count = P * 3 * chunkElems + (P == 2 ? 0 : 5);
+      std::vector<size_t> counts(P), off(P + 1, 0);
+      for (int r = 0; r < P; r++) {
+        counts[r] = count / P + (static_cast<size_t>(r) < count % P ? 1 : 0);
+        off[r + 1] = off[r] + counts[r];
+      }
+      const size_t shift = P == 8 ? 1 : 0;
+      DevBuf in(count * 4), out((count + shift) * 4);
+      launchFill(in.p, count, DataType::FLOAT32, 0.0, 1.0, stream);
+      GLB_CUDA_CHECK(cudaMemsetAsync(out.p, 0xff, out.bytes, stream));
+      GLB_CUDA_CHECK(cudaMemsetAsync(myStage + 2 * half + 2 * P * C, 0, 2 * C, stream));
+      launchPipelinedReduce(ca, in.p, static_cast<float*>(out.p) + shift, off.data(), counts.data(), 0, DataType::FLOAT32,
+                            ReduceOp::SUM, aliasedBulk(P), tile, 256, blocks, stream);
+      noteLaunch();
+      auto h = download(out.p, count + shift, stream);
+      for (size_t i = 0; i < count; i++) {
+        const double want = i < counts[0] ? static_cast<double>(P) * i : 0.0;
+        if (!close(h[i + shift], want)) return strcat_all("element ", i, ": got ", h[i + shift], " want ", want);
+      }
+      return "";
+    });
+  }
+  // alltoall(v): virtual peer q's pool is my pool shifted by q sub-slots, so sub-slot 0 of its slot
+  // is sub-slot q of mine and rank 0 pulls back its own block for destination q. Blocks are uneven
+  // (some empty, some several chunks), received in the reverse order, into an output one byte off.
+  for (int P : {2, 8}) {
+    R.run(strcat_all("pipelinedAlltoallKernel P=", P, " (uneven blocks, out 1 byte off)"), [&]() -> std::string {
+      const CommArgs ca = pc.loopbackComm(P);
+      const int blocks = std::min(pc.coResidentBlocks(pipelinedAlltoallKernelPtr()), 8), tile = 64;
+      const size_t C = static_cast<size_t>(blocks) * tile * 16;
+      GLB_ENFORCE_LE(2 * P * C, pc.stageBytes() - 2 * half, "pool too small for the pipelined self-test");
+      std::vector<size_t> len(P), soff(P, 0), roff(P, 0);
+      for (int j = 0; j < P; j++) len[j] = j % 3 == 2 ? 0 : (j % 4 + 1) * C + 13 * j + 3;
+      for (int j = 1; j < P; j++) soff[j] = soff[j - 1] + len[j - 1];
+      for (int j = P - 2; j >= 0; j--) roff[j] = roff[j + 1] + len[j + 1];
+      const size_t total = soff[P - 1] + len[P - 1];
+      PeerPtrs st;
+      std::memset(&st, 0, sizeof(st));
+      for (int q = 0; q < P; q++) st.p[q] = myStage + 2 * half + q * C;
+      DevBuf in(total), out(total + 1);
+      launchFill(in.p, total / 4, DataType::FLOAT32, 1.0, 1.0, stream);
+      GLB_CUDA_CHECK(cudaMemsetAsync(out.p, 0, out.bytes, stream));
+      launchPipelinedAlltoall(ca, in.p, static_cast<char*>(out.p) + 1, soff.data(), len.data(), roff.data(), len.data(),
+                              st, tile, 256, blocks, stream);
+      noteLaunch();
+      std::vector<char> hin(total), hout(out.bytes);
+      GLB_CUDA_CHECK(cudaMemcpyAsync(hin.data(), in.p, total, cudaMemcpyDeviceToHost, stream));
+      GLB_CUDA_CHECK(cudaMemcpyAsync(hout.data(), out.p, out.bytes, cudaMemcpyDeviceToHost, stream));
+      GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+      for (int j = 0; j < P; j++) {
+        if (std::memcmp(hout.data() + 1 + roff[j], hin.data() + soff[j], len[j]) != 0) return strcat_all("block ", j, " differs");
+      }
+      return hout[0] == 0 ? "" : "wrote before the output";
+    });
+  }
+  // The scatter form at root 0, the root's path: it stages the blocks for the other ranks and copies
+  // its own block straight to its output; it receives from nobody else.
+  R.run("pipelinedAlltoallKernel (scatter, root 0) P=4", [&]() -> std::string {
+    const int P = 4;
+    const CommArgs ca = pc.loopbackComm(P);
+    const int blocks = std::min(pc.coResidentBlocks(pipelinedAlltoallKernelPtr()), 8), tile = 64;
+    const size_t C = static_cast<size_t>(blocks) * tile * 16, bytes = 3 * C + 20;
+    GLB_ENFORCE_LE(2 * P * C, pc.stageBytes() - 2 * half, "pool too small for the pipelined self-test");
+    std::vector<size_t> slen(P, bytes), soff(P), rlen(P, 0), roff(P, 0);
+    for (int j = 0; j < P; j++) soff[j] = j * bytes;
+    rlen[0] = bytes;
+    DevBuf in(P * bytes), out(bytes + 16);
+    launchFill(in.p, P * bytes / 4, DataType::FLOAT32, 0.0, 1.0, stream);
+    GLB_CUDA_CHECK(cudaMemsetAsync(out.p, 0, out.bytes, stream));
+    launchPipelinedAlltoall(ca, in.p, out.p, soff.data(), slen.data(), roff.data(), rlen.data(), aliasedBulk(P), tile, 256,
+                            blocks, stream);
+    noteLaunch();
+    std::vector<char> hin(bytes), hout(out.bytes);
+    GLB_CUDA_CHECK(cudaMemcpyAsync(hin.data(), in.p, bytes, cudaMemcpyDeviceToHost, stream));
+    GLB_CUDA_CHECK(cudaMemcpyAsync(hout.data(), out.p, out.bytes, cudaMemcpyDeviceToHost, stream));
+    GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+    if (std::memcmp(hout.data(), hin.data(), bytes) != 0) return "block 0 differs";
+    for (size_t i = bytes; i < out.bytes; i++) {
+      if (hout[i] != 0) return "wrote past the output";
+    }
+    return "";
+  });
 
   // ---- point to point: fused send + recv through my own mailbox --------------------------------
   R.run("p2pKernel(sendrecv)", [&]() -> std::string {

@@ -6,9 +6,8 @@ and offers the collective suite for torch CUDA tensors. A tensor is either
 * *registered* (``ctx.register(t)`` or allocated with ``ctx.empty(...)``): kernels
   read/write the peers' copies directly (zero-copy, NVLS-capable when symmetric);
 * anything else: staged through the per-rank pool (``stage_bytes``) inside the same call.
-  allreduce, broadcast, allgather(v), gather(v) and reduce_scatter take any size: beyond the
-  pool they stream through it in one pipelined kernel. alltoall(v), scatter and reduce still
-  need the payload to fit the pool's bulk region (the pool minus two one-shot halves).
+  every collective takes any size: beyond the pool's bulk region (the pool minus two one-shot
+  halves) the payload streams through it in one pipelined kernel.
 
 Every method is asynchronous on the current torch stream unless ``stream`` is given,
 and must be called in the same order on every rank.
@@ -299,7 +298,8 @@ class CudaContext:
         return output
 
     def alltoall(self, output, input, stream=None):
-        """Fixed-size exchange: chunk j of ``input`` goes to rank j (one size for all ranks)."""
+        """Fixed-size exchange: chunk j of ``input`` goes to rank j (one size for all ranks). Any size;
+        a plain ``input`` and ``output`` must not overlap (ValueError beyond the staged path)."""
         per = input.numel() // self.size * input.element_size()
         buf, off = self.lookup(output)
         if buf is not None:
@@ -309,6 +309,12 @@ class CudaContext:
         return output
 
     def alltoallv(self, output, out_counts: Sequence[int], input, in_counts: Sequence[int], stream=None):
+        """Block j of ``input`` (``in_counts[j]`` elements) goes to rank j; the block from rank q lands
+        in ``output`` after the blocks of ranks < q (``out_counts[q]`` elements). Any size. A plain
+        ``input`` and ``output`` must not overlap, at any size (``gloo_b200._C.InputError``, a
+        ValueError): the plain alltoallv always runs the pipelined kernel, which writes the output
+        while it still reads the input. Earlier versions staged a call that fit the pool, so a small
+        in-place call used to work; it now raises."""
         es = input.element_size()
         send = [int(c) * es for c in in_counts]
         recv = [int(c) * es for c in out_counts]
@@ -385,6 +391,8 @@ class CudaContext:
         return out
 
     def scatter(self, output, input=None, root: int = 0, stream=None):
+        """Block ``rank`` of the root's ``input`` -> ``output``. Any size; ``input`` is read on the
+        root only (None elsewhere)."""
         nbytes = output.numel() * output.element_size()
         iptr = input.data_ptr() if input is not None else 0
         buf, off = self.lookup(output)
@@ -412,6 +420,8 @@ class CudaContext:
         return output
 
     def reduce(self, output, input, root: int = 0, op: ReduceOp = ReduceOp.SUM, stream=None):
+        """``output`` on ``root`` := the reduction of every rank's ``input``. Any size; a non-root's
+        ``output`` is never written and may be None."""
         ptr, n, dt, _ = describe(input)
         ibuf, ioff = self.lookup(input)
         obuf, ooff = (self.lookup(output) if output is not None else (None, 0))

@@ -230,10 +230,8 @@ class GlbProcessGroup(dist.ProcessGroup):
         idx = tensor.device.index if tensor.device.index is not None else torch.cuda.current_device()
         if idx not in self._cuda:
             # torch tensors are not registered with the peer context, so they travel through
-            # its staging pool (GLB_PG_STAGE_MB, default 128). all_reduce, broadcast,
-            # all_gather(_into_tensor), gather and reduce_scatter(_tensor) take any size: they
-            # stream through the pool. all_to_all, scatter and reduce still need the whole
-            # payload to fit; raise GLB_PG_STAGE_MB for larger ones.
+            # its staging pool (GLB_PG_STAGE_MB, default 128). Every collective takes any size:
+            # a payload larger than the pool streams through it.
             stage = int(os.environ.get("GLB_PG_STAGE_MB", "128")) << 20
             with torch.cuda.device(idx):
                 self._cuda[idx] = gcu.CudaContext(self.ctx, idx, stage_bytes=stage)

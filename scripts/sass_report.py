@@ -32,6 +32,8 @@ KERNELS = [
     ("pipelined_f32_P2", r"pipelinedAllreduceKernel<float, false, 2>"),
     ("pipelined_allgather", r"pipelinedAllgatherKernel"),
     ("pipelined_reduce_scatter_bf16_P8", r"pipelinedReduceScatterKernel<__nv_bfloat16, 8>"),
+    ("pipelined_alltoall", r"pipelinedAlltoallKernel"),
+    ("pipelined_reduce_bf16_P8", r"pipelinedReduceKernel<__nv_bfloat16, 8>"),
     ("reduce_pull_f32_P8", r"reducePullKernel<float, 8, 2>"),
     ("broadcast", r"broadcastKernel"),
     ("gather_push", r"gatherPushKernel"),

@@ -4,12 +4,14 @@ allgather, alltoall, alltoall_v, broadcast, reduce_scatter — 1 KB .. 1 GB per-
 device-timed, max over ranks, against the NCCL comparator. torchrun, one rank per GPU.
 Also the named fp16 schedules (config 3) with --schedules.
 
---plain (or --threads P) sweeps allgather and reduce_scatter of PLAIN tensors, 1 MB .. 1 GB of
-allgather output / reduce_scatter input, in four arms: "staged" (payload copied through the
-staging pool, where it fits), "pipelined" (the pipelined kernel: the default pool where the
-payload does not fit it, and a second context whose pool is smaller than the payload but holds
-two full-size slots where it does), "registered" (symmetric buffers, zero copy: the ceiling) and
-NCCL (more than one GPU). --threads P runs P ranks as threads on ONE GPU, each on its own
+--plain (or --threads P) sweeps allgather, reduce_scatter, alltoall, alltoall_v, scatter and
+reduce of PLAIN tensors (--plain-ops picks some), 1 MB .. 1 GB of what each rank sends or holds
+(allgather output, reduce_scatter / alltoall / scatter root / reduce input), in four arms:
+"staged" (payload copied through the staging pool, where it fits), "pipelined" (the pipelined
+kernel: the default pool where the payload does not fit it, and a second context whose pool is
+smaller than the payload but holds the pipelined slots where it does; alltoall_v always runs it),
+"registered" (symmetric buffers, zero copy: the ceiling) and NCCL (more than one GPU, allgather /
+reduce_scatter / alltoall). --threads P runs P ranks as threads on ONE GPU, each on its own
 gcu.new_stream(): the ranks share that GPU's HBM, so those figures are not NVLink figures."""
 import argparse
 import json
@@ -49,9 +51,28 @@ def _timer(ctx, world, stream, flush):
 # full-size slot is shares x 128 CTAs x 1024 x 16 bytes.
 FULL_SLOT = 128 * 1024 * 16
 HALVES = 2 * (256 << 10)      # the pool's two one-shot halves (GLB_CUDA_ONESHOT_MAX)
+PLAIN_OPS = ("allgather", "reduce_scatter", "alltoall", "alltoall_v", "scatter", "reduce")
 
 
-def plain_rows(ctx, cc, ctx_small, P, rank, stream, iters, max_bytes, nccl):
+def _plain_shape(op, n, P):
+    """(input elements, output elements, pool slots in full-size slot bytes, bytes the staged path
+    compares with the bulk region, or None when it has no staged path) of one plain-tensor op, with
+    `n` = the elements each rank sends / holds."""
+    per = n // P
+    if op == "allgather":
+        return per, n, 2 * FULL_SLOT, n * 4
+    if op == "reduce_scatter":
+        return n, per, 2 * P * FULL_SLOT, n * 4
+    if op == "alltoall":
+        return n, n, 2 * P * FULL_SLOT, n * 4
+    if op == "alltoall_v":
+        return n, n, 2 * P * FULL_SLOT, None  # always pipelined
+    if op == "scatter":
+        return n, per, 2 * P * FULL_SLOT, per * 4
+    return n, n, 2 * (P + 1) * FULL_SLOT, 2 * n * 4  # reduce: the staged path takes half the bulk region
+
+
+def plain_rows(ctx, cc, ctx_small, P, rank, stream, iters, max_bytes, nccl, ops=PLAIN_OPS):
     """Rows of the plain-tensor arms. `ctx_small(stage_bytes)` returns a CudaContext with that
     pool on a context of its own (a context has one pool per device)."""
     bulk = cc.pc.stage_bytes() - HALVES
@@ -61,26 +82,39 @@ def plain_rows(ctx, cc, ctx_small, P, rank, stream, iters, max_bytes, nccl):
     sizes = [m << 20 for m in (1, 4, 16, 64, 256, 1024) if (m << 20) <= max_bytes]
     small = {}
     rows = []
-    for op in ("allgather", "reduce_scatter"):
-        shares = 1 if op == "allgather" else P
-        slots = 2 * shares * FULL_SLOT
+    for op in ops:
         for total in sizes:
             n = total // 4 // P * P
             per = n // P
+            n_in, n_out, slots, staged_bytes = _plain_shape(op, n, P)
+            # alltoall_v: uneven but balanced split, rank r sends weight w[(j - r) % P] to rank j
+            w = [k + 1 for k in range(P)]
+            unit = [n * x // sum(w) for x in w]
+            unit[-1] += n - sum(unit)
+            send = [unit[(j - rank) % P] for j in range(P)]
+            recv = [unit[(rank - i) % P] for i in range(P)]
             it = iters if total < (64 << 20) else max(5, iters // 4)
             row = {"op": op + "_plain", "bytes": n * 4}
-            big_in = torch.ones(n if op == "reduce_scatter" else per, device="cuda")
-            big_out = torch.empty(per if op == "reduce_scatter" else n, device="cuda")
+            big_in = torch.ones(n_in, device="cuda")
+            big_out = torch.empty(n_out, device="cuda")
 
             def call(c, o, i):
                 if op == "allgather":
                     return lambda: c.allgather(o, i, stream=stream)
-                return lambda: c.reduce_scatter(o, i, [per] * P, stream=stream)
+                if op == "reduce_scatter":
+                    return lambda: c.reduce_scatter(o, i, [per] * P, stream=stream)
+                if op == "alltoall":
+                    return lambda: c.alltoall(o, i, stream=stream)
+                if op == "alltoall_v":
+                    return lambda: c.alltoallv(o, recv, i, send, stream=stream)
+                if op == "scatter":
+                    return lambda: c.scatter(o, i, root=0, stream=stream)
+                return lambda: c.reduce(o, i, root=0, stream=stream)
 
             try:
-                if n * 4 <= bulk:
+                if staged_bytes is not None and staged_bytes <= bulk:
                     row["staged_us"] = round(timed(call(cc, big_out, big_in), it), 2)
-                    if n * 4 > slots:  # a pool that holds two full-size slots but not the payload
+                    if staged_bytes > slots:  # a pool that holds the pipelined slots but not the payload
                         if slots not in small:
                             small[slots] = ctx_small(slots + HALVES)
                         row["pipelined_pool_mb"] = round(small[slots].pc.stage_bytes() / 2**20, 1)
@@ -90,16 +124,20 @@ def plain_rows(ctx, cc, ctx_small, P, rank, stream, iters, max_bytes, nccl):
                 sym_in = cc.empty(big_in.numel(), torch.float32)
                 sym_in.fill_(1)
                 sym_out = cc.empty(big_out.numel(), torch.float32)
-                if op == "allgather":
+                if op in ("allgather", "alltoall", "alltoall_v", "scatter"):
                     row["registered_us"] = round(timed(call(cc, sym_out, big_in), it), 2)
-                else:
+                elif op == "reduce_scatter":
                     row["registered_us"] = round(timed(call(cc, big_out, sym_in), it), 2)
+                else:  # reduce: the registered path needs both buffers registered
+                    row["registered_us"] = round(timed(call(cc, sym_out, sym_in), it), 2)
                 del sym_in, sym_out
-                if nccl is not None:
+                if nccl is not None and op in ("allgather", "reduce_scatter", "alltoall"):
                     if op == "allgather":
                         fn = lambda: nccl.allgather(big_in.data_ptr(), big_out.data_ptr(), per, F32, stream.cuda_stream)  # noqa: E731
-                    else:
+                    elif op == "reduce_scatter":
                         fn = lambda: nccl.reduce_scatter(big_in.data_ptr(), big_out.data_ptr(), per, F32, 1, stream.cuda_stream)  # noqa: E731
+                    else:
+                        fn = lambda: nccl.alltoall(big_in.data_ptr(), big_out.data_ptr(), per, F32, stream.cuda_stream)  # noqa: E731
                     row["nccl_us"] = round(timed(fn, it), 2)
                 for k in [k for k in row if k.endswith("_us")]:
                     row[k[:-3] + "_gbs"] = round(n * 4 / (row[k] * 1e-6) / 1e9, 1)
@@ -141,7 +179,7 @@ def threads_main(args):
             return gcu.CudaContext(c2, 0, stage_bytes=stage)
 
         cc = gcu.CudaContext(ctx, 0, stage_bytes=128 << 20)
-        rows = plain_rows(ctx, cc, ctx_small, P, ctx.rank, stream, args.iters, args.max_bytes, None)
+        rows = plain_rows(ctx, cc, ctx_small, P, ctx.rank, stream, args.iters, args.max_bytes, None, args.plain_ops)
         torch.cuda.synchronize()
         for c2 in made:
             gb.barrier(c2)
@@ -161,7 +199,9 @@ def main():
     ap.add_argument("--max-bytes", type=int, default=1 << 30)
     ap.add_argument("--ops", default="allgather,alltoall,alltoall_v,broadcast,reduce_scatter")
     ap.add_argument("--schedules", action="store_true")
-    ap.add_argument("--plain", action="store_true", help="also the plain-tensor allgather / reduce_scatter arms")
+    ap.add_argument("--plain", action="store_true", help="also the plain-tensor arms")
+    ap.add_argument("--plain-ops", type=lambda v: tuple(o for o in v.split(",") if o), default=PLAIN_OPS,
+                    help="plain-tensor ops to sweep (default: " + ",".join(PLAIN_OPS) + ")")
     ap.add_argument("--threads", type=int, default=0, help="P ranks as threads on one GPU (plain arms only)")
     args = ap.parse_args()
     if args.threads:
@@ -313,7 +353,7 @@ def main():
             smalls.append(c2)
             return gcu.CudaContext(c2, local, stage_bytes=stage)
 
-        rows += plain_rows(ctx, cc, ctx_small, world, rank, stream, args.iters, args.max_bytes, nccl)
+        rows += plain_rows(ctx, cc, ctx_small, world, rank, stream, args.iters, args.max_bytes, nccl, args.plain_ops)
     if rank == 0 and args.out:
         with open(args.out, "w") as f:
             json.dump({"world": world, "describe": cc.describe(), "rows": rows}, f, indent=1)
