@@ -472,8 +472,81 @@ struct A2aDevArgs {
   InputStatus* status;  // host-mapped
 };
 
+// The quantising dispatch (kQuant): bf16 rows of H elements in, e4m3 codes (rowBytes = H) and
+// one fp32 scale per 128-element block out. The scales of rank j go to `scales.p[j]`, row-major
+// (rows, H / 128), or, staged, into j's staging area right after its `capRows` rows of codes.
+// Its own type, so that the copying form keeps its parameter block.
+template <bool kQuant>
+struct A2aDevKernelArgs : A2aDevArgs {};
+template <>
+struct A2aDevKernelArgs<true> : A2aDevArgs {
+  PeerPtrs scales;     // zero copy: every rank's out_scales
+  float* stagedScales; // plain output: copied from my staging after barrier 2; null = zero copy
+};
+
+constexpr int kQuantUnroll = 4;      // blocks in flight per half-warp
+constexpr float kE4m3Max = 448.0f;
+constexpr float kQuantMinAmax = 1e-4f;
+
+// Header word 3: bit 0 = inverse, bit 1 = quantising. Ranks that disagree on either read the
+// call as invalid, like differing row sizes.
+template <bool kQuant>
+__device__ __forceinline__ uint32_t a2aDirection(int inverse) {
+  return static_cast<uint32_t>(inverse) | (kQuant ? 2u : 0u);
+}
+
+// Chunk of `nblk` blocks: bf16 at `in`, codes to `codes`, scales to `scales`. A half-warp owns a
+// block: each lane loads 8 elements (16 bytes), the block amax takes 4 shuffles within the 16
+// lanes, each lane stores 8 codes (8 bytes), lane 0 of the half stores the scale. The loop is
+// warp-uniform so the shuffles run with a full mask; lanes past the end take part with zeros.
+// `tid` / `nthreads` are multiples of 32 apart from the lane, like every caller of gridCopy.
+// Numerics: amax = max(max |x|, 1e-4f); code = e4m3(x * (448 * (1 / amax))); scale = amax / 448,
+// each step a correctly rounded fp32 operation (no contraction, no approximate division). The
+// multiplier is a rounded reciprocal times 448, not a rounded 448 / amax: that is what torch
+// evaluates for `448.0 / amax` (a scalar over a tensor), so torch code reproduces every byte.
+__device__ __forceinline__ void quantCopy(char* codes, float* scales, const char* in, unsigned long long nblk,
+                                          size_t tid, size_t nthreads) {
+  const int lane = static_cast<int>(tid & 31), half = lane >> 4, hl = lane & 15;
+  const unsigned long long nwarps = nthreads / 32, warp = tid / 32;
+  for (unsigned long long base = warp * (2 * kQuantUnroll); base < nblk; base += nwarps * (2 * kQuantUnroll)) {
+    uint4 v[kQuantUnroll];
+#pragma unroll
+    for (int u = 0; u < kQuantUnroll; u++) {
+      const unsigned long long blk = base + 2 * u + half;
+      v[u] = blk < nblk ? *reinterpret_cast<const uint4*>(in + blk * (2 * kFp8Block) + hl * 16)
+                        : make_uint4(0u, 0u, 0u, 0u);
+    }
+#pragma unroll
+    for (int u = 0; u < kQuantUnroll; u++) {
+      const unsigned long long blk = base + 2 * u + half;
+      const uint32_t w[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
+      float f[8];
+#pragma unroll
+      for (int i = 0; i < 4; i++) {
+        f[2 * i] = __uint_as_float(w[i] << 16);
+        f[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u);
+      }
+      float amax = 0.0f;
+#pragma unroll
+      for (int i = 0; i < 8; i++) amax = fmaxf(amax, fabsf(f[i]));
+#pragma unroll
+      for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+      amax = fmaxf(amax, kQuantMinAmax);
+      const float s = __fmul_rn(__frcp_rn(amax), kE4m3Max);
+      uint32_t c[4];
+#pragma unroll
+      for (int i = 0; i < 4; i++) c[i] = float2ToFp8x2<__nv_fp8_e4m3>(__fmul_rn(f[2 * i], s), __fmul_rn(f[2 * i + 1], s));
+      if (blk < nblk) {
+        *reinterpret_cast<uint2*>(codes + blk * kFp8Block + hl * 8) = make_uint2(c[0] | (c[1] << 16), c[2] | (c[3] << 16));
+        if (hl == 0) scales[blk] = __fdiv_rn(amax, kE4m3Max);
+      }
+    }
+  }
+}
+
+template <bool kQuant>
 __global__ void __launch_bounds__(kThreads)
-alltoallvDevKernel(CommArgs a, PeerPtrs outs, A2aDevArgs d) {
+alltoallvDevKernel(CommArgs a, PeerPtrs outs, A2aDevKernelArgs<kQuant> d) {
   constexpr int kMaxK = kMaxRanks * kMaxA2aExperts;
   __shared__ unsigned long long sSrc[kMaxK];  // my chunk k: first input row
   __shared__ unsigned long long sDst[kMaxK];  //             first row in its destination's output
@@ -521,7 +594,7 @@ alltoallvDevKernel(CommArgs a, PeerPtrs outs, A2aDevArgs d) {
     if (blockIdx.x == 0 && t < P) {
       uint32_t* h = &a.sig[t]->a2aHdr[0][me];
       const uint32_t hdr[kA2aHdrWords] = {static_cast<uint32_t>(rb), static_cast<uint32_t>(E), static_cast<uint32_t>(d.align),
-                                          static_cast<uint32_t>(d.inverse), d.capRows, localBad ? 1u : 0u};
+                                          a2aDirection<kQuant>(d.inverse), d.capRows, localBad ? 1u : 0u};
 #pragma unroll
       for (int w = 0; w < kA2aHdrWords; w++) h[w * kMaxRanks] = hdr[w];
     }
@@ -536,7 +609,7 @@ alltoallvDevKernel(CommArgs a, PeerPtrs outs, A2aDevArgs d) {
     bool b = false;
     if (t < P) {
       const uint32_t want[4] = {static_cast<uint32_t>(rb), static_cast<uint32_t>(E), static_cast<uint32_t>(d.align),
-                                static_cast<uint32_t>(d.inverse)};
+                                a2aDirection<kQuant>(d.inverse)};
 #pragma unroll
       for (int w = 0; w < 4; w++) b = b || ldPad(&pad->a2aHdr[w][t]) != want[w];
       b = b || ldPad(&pad->a2aHdr[5][t]) != 0u;
@@ -670,7 +743,16 @@ alltoallvDevKernel(CommArgs a, PeerPtrs outs, A2aDevArgs d) {
       for (int x = 0; x < E; x++) {
         const int k = d.inverse ? x * P + dst : dst * E + x;
         if (sCnt[k] == 0) continue;
-        gridCopy(static_cast<char*>(outs.p[dst]) + sDst[k] * rb, d.in + sSrc[k] * rb, sCnt[k] * rb, true, tid, nthreads);
+        if constexpr (kQuant) {
+          // Input rows are 2·rb bytes (bf16); a row is rb / 128 blocks.
+          const unsigned long long bpr = rb / kFp8Block;
+          char* codes = static_cast<char*>(outs.p[dst]);
+          float* scales = d.stagedScales != nullptr ? reinterpret_cast<float*>(codes + sCap[dst] * rb)
+                                                    : static_cast<float*>(d.scales.p[dst]);
+          quantCopy(codes + sDst[k] * rb, scales + sDst[k] * bpr, d.in + sSrc[k] * rb * 2, sCnt[k] * bpr, tid, nthreads);
+        } else {
+          gridCopy(static_cast<char*>(outs.p[dst]) + sDst[k] * rb, d.in + sSrc[k] * rb, sCnt[k] * rb, true, tid, nthreads);
+        }
       }
     }
   }
@@ -693,6 +775,14 @@ alltoallvDevKernel(CommArgs a, PeerPtrs outs, A2aDevArgs d) {
         for (int k = 0; k < K; k++) {
           const unsigned long long n = sRcvCnt[k];
           if (n > 0) gridCopy(d.stagedOut + sRcv[k] * rb, stage + sRcv[k] * rb, n * rb, true, tid, nthreads);
+          if constexpr (kQuant) {
+            // The scales follow my capRows rows of codes in my staging area.
+            const unsigned long long sb = rb / kFp8Block * sizeof(float);  // scale bytes per row
+            if (n > 0) {
+              gridCopy(reinterpret_cast<char*>(d.stagedScales) + sRcv[k] * sb, stage + sCap[me] * rb + sRcv[k] * sb,
+                       n * sb, true, tid, nthreads);
+            }
+          }
         }
       }
     }
@@ -704,7 +794,7 @@ void launchAlltoallvDev(const CommArgs& a, const PeerPtrs& outs, const void* in,
                         const long long* inSplits, const long long* inOffsets, long long* outSplits,
                         long long* outOffsets, void* stagedOut, uint32_t capRows, int experts, int align, bool inverse,
                         InputStatus* status, int blocks, cudaStream_t stream) {
-  A2aDevArgs d;
+  A2aDevKernelArgs<false> d;
   d.in = static_cast<const char*>(in);
   d.inRows = inRows;
   d.rowBytes = rowBytes;
@@ -718,7 +808,30 @@ void launchAlltoallvDev(const CommArgs& a, const PeerPtrs& outs, const void* in,
   d.align = align;
   d.inverse = inverse ? 1 : 0;
   d.status = status;
-  alltoallvDevKernel<<<blocks, kThreads, 0, stream>>>(a, outs, d);
+  alltoallvDevKernel<false><<<blocks, kThreads, 0, stream>>>(a, outs, d);
+}
+
+void launchAlltoallvDevFp8(const CommArgs& a, const PeerPtrs& outs, const PeerPtrs& scales, const void* in,
+                           size_t inRows, size_t hidden, const long long* inSplits, long long* outSplits,
+                           long long* outOffsets, void* stagedOut, float* stagedScales, uint32_t capRows, int experts,
+                           int align, InputStatus* status, int blocks, cudaStream_t stream) {
+  A2aDevKernelArgs<true> d;
+  d.in = static_cast<const char*>(in);
+  d.inRows = inRows;
+  d.rowBytes = hidden;  // e4m3 codes: one byte per element
+  d.inSplits = inSplits;
+  d.inOffsets = nullptr;
+  d.outSplits = outSplits;
+  d.outOffsets = outOffsets;
+  d.stagedOut = static_cast<char*>(stagedOut);
+  d.capRows = capRows;
+  d.experts = experts;
+  d.align = align;
+  d.inverse = 0;
+  d.status = status;
+  d.scales = scales;
+  d.stagedScales = stagedScales;
+  alltoallvDevKernel<true><<<blocks, kThreads, 0, stream>>>(a, outs, d);
 }
 
 // ---- reduce_scatter / reduce: pull my slice from every peer's input, reduce, store -----------
@@ -923,7 +1036,10 @@ void launchLLExchange(const CommArgs& a, const void* in, void* out, size_t bytes
 const void* broadcastKernelPtr() { return reinterpret_cast<const void*>(broadcastKernel); }
 const void* gatherPushKernelPtr() { return reinterpret_cast<const void*>(gatherPushKernel); }
 const void* alltoallPushKernelPtr() { return reinterpret_cast<const void*>(alltoallPushKernel); }
-const void* alltoallvDevKernelPtr() { return reinterpret_cast<const void*>(alltoallvDevKernel); }
+const void* alltoallvDevKernelPtr(bool fp8) {
+  return fp8 ? reinterpret_cast<const void*>(alltoallvDevKernel<true>)
+             : reinterpret_cast<const void*>(alltoallvDevKernel<false>);
+}
 const void* reducePullKernelPtr(DataType dt, int nranks) {
   const void* k = nullptr;
   dispatchType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(reducePullFn<decltype(tag)>(nranks)); });
@@ -934,7 +1050,8 @@ void preloadCollectiveKernels() {
   touchKernel(broadcastKernel);
   touchKernel(gatherPushKernel);
   touchKernel(alltoallPushKernel);
-  touchKernel(alltoallvDevKernel);
+  touchKernel(alltoallvDevKernel<false>);
+  touchKernel(alltoallvDevKernel<true>);
   touchKernel(llExchangeKernel);
   for (DataType dt : kAllDataTypes) {
     dispatchType(dt, [&](auto tag) {

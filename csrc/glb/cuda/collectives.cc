@@ -853,10 +853,12 @@ namespace {
 // Like the host-count v-variant the grid is fixed (the sizes are only known on the device, the
 // grid must be the same on every rank), and P = 1 runs the same kernel: the expert-major layout
 // still applies.
+// `scales` non-null: the quantising form (rowBytes = hidden, bf16 input); `stagedScales` goes
+// with `stagedOut`.
 void alltoallvDevCommon(PeerContext& pc, const void* in, size_t inRows, size_t rowBytes, const int64_t* inSplits,
                         const int64_t* inOffsets, const PeerPtrs& outs, void* stagedOut, size_t capacityRows,
                         int64_t* outSplits, int64_t* outOffsets, int experts, int align, bool inverse,
-                        cudaStream_t stream) {
+                        cudaStream_t stream, const PeerPtrs* scales = nullptr, float* stagedScales = nullptr) {
   GLB_TRACE_RANGE("glb::cuda::alltoallv_dev");
   GLB_ENFORCE(experts >= 1 && experts <= kMaxA2aExperts, "alltoallv_dev: experts per rank must be in 1..",
               kMaxA2aExperts, ", got ", experts);
@@ -868,14 +870,28 @@ void alltoallvDevCommon(PeerContext& pc, const void* in, size_t inRows, size_t r
   GLB_ENFORCE(inverse || (outSplits != nullptr && outOffsets != nullptr),
               "alltoallv_dev: the forward exchange needs output splits and offsets");
   const uint32_t cap = static_cast<uint32_t>(std::min<size_t>(capacityRows, 0xfffffffeull));
+  const bool fp8 = scales != nullptr;
   const int blocks =
-      std::max(1, std::min({tuning().alltoallvBlocks, pc.coResidentBlocks(alltoallvDevKernelPtr()), kMaxBlocks}));
+      std::max(1, std::min({tuning().alltoallvBlocks, pc.coResidentBlocks(alltoallvDevKernelPtr(fp8)), kMaxBlocks}));
   prologue(pc, stream);
-  launchAlltoallvDev(pc.comm(), outs, in, inRows, rowBytes, reinterpret_cast<const long long*>(inSplits),
-                     reinterpret_cast<const long long*>(inOffsets), reinterpret_cast<long long*>(outSplits),
-                     reinterpret_cast<long long*>(outOffsets), stagedOut, cap, experts, align, inverse,
-                     pc.inputStatusDevice(), blocks, stream);
+  if (fp8) {
+    launchAlltoallvDevFp8(pc.comm(), outs, *scales, in, inRows, rowBytes, reinterpret_cast<const long long*>(inSplits),
+                          reinterpret_cast<long long*>(outSplits), reinterpret_cast<long long*>(outOffsets), stagedOut,
+                          stagedScales, cap, experts, align, pc.inputStatusDevice(), blocks, stream);
+  } else {
+    launchAlltoallvDev(pc.comm(), outs, in, inRows, rowBytes, reinterpret_cast<const long long*>(inSplits),
+                       reinterpret_cast<const long long*>(inOffsets), reinterpret_cast<long long*>(outSplits),
+                       reinterpret_cast<long long*>(outOffsets), stagedOut, cap, experts, align, inverse,
+                       pc.inputStatusDevice(), blocks, stream);
+  }
   finish(pc, stream, "alltoallv_dev");
+}
+
+void checkFp8Dispatch(const void* in, const void* out, size_t hidden) {
+  GLB_ENFORCE(hidden > 0 && hidden % kFp8Block == 0, "alltoallv_dev (bf16 -> e4m3): the row length must be a "
+              "positive multiple of ", kFp8Block, ", got ", hidden);
+  GLB_ENFORCE(reinterpret_cast<uintptr_t>(in) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0,
+              "alltoallv_dev (bf16 -> e4m3): input and output must be 16-byte aligned");
 }
 }  // namespace
 
@@ -899,6 +915,38 @@ void alltoallvDev(PeerContext& pc, const void* in, size_t inRows, size_t rowByte
   alltoallvDevCommon(pc, in, inRows, rowBytes, inSplits, inOffsets, pc.stagePtrs(l.bulkOff), out,
                      std::min(capacityRows, l.bulkBytes / rowBytes), outSplits, outOffsets, experts, align, inverse,
                      stream);
+}
+
+void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidden, const int64_t* inSplits,
+                     const PeerBuffer& out, size_t outOffset, const PeerBuffer& outScales, size_t scalesOffset,
+                     size_t capacityRows, int64_t* outSplits, int64_t* outOffsets, int experts, int align,
+                     cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  checkFp8Dispatch(in, static_cast<const char*>(out.local) + outOffset, hidden);
+  GLB_ENFORCE_LE(outOffset + capacityRows * hidden, out.bytes, "alltoallv_dev output exceeds the registered buffer");
+  GLB_ENFORCE_LE(scalesOffset + capacityRows * (hidden / kFp8Block) * sizeof(float), outScales.bytes,
+                 "alltoallv_dev output scales exceed the registered buffer");
+  GLB_ENFORCE(scalesOffset % sizeof(float) == 0, "alltoallv_dev: output scales must be 4-byte aligned");
+  const PeerPtrs scales = outScales.ptrsAt(scalesOffset);
+  alltoallvDevCommon(pc, in, inRows, hidden, inSplits, nullptr, out.ptrsAt(outOffset), nullptr, capacityRows, outSplits,
+                     outOffsets, experts, align, false, stream, &scales, nullptr);
+}
+
+void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidden, const int64_t* inSplits,
+                     void* out, float* outScales, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets,
+                     int experts, int align, cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  checkFp8Dispatch(in, out, hidden);
+  GLB_ENFORCE(reinterpret_cast<uintptr_t>(outScales) % sizeof(float) == 0,
+              "alltoallv_dev: output scales must be 4-byte aligned");
+  // Peers push codes into my staging area and the scales after my capacity's worth of codes; a
+  // row takes hidden + hidden / 32 bytes there (hidden is a multiple of 128, so the scales start
+  // 16-byte aligned).
+  const auto l = layoutOf(pc);
+  const PeerPtrs none{};
+  alltoallvDevCommon(pc, in, inRows, hidden, inSplits, nullptr, pc.stagePtrs(l.bulkOff), out,
+                     std::min(capacityRows, l.bulkBytes / (hidden + hidden / kFp8Block * sizeof(float))), outSplits,
+                     outOffsets, experts, align, false, stream, &none, outScales);
 }
 
 void scatter(PeerContext& pc, const void* in, const PeerBuffer& out, size_t outOffset, size_t bytes, int root,

@@ -156,6 +156,21 @@ void alltoallvDev(PeerContext& pc, const void* in, size_t inRows, size_t rowByte
 void alltoallvDev(PeerContext& pc, const void* in, size_t inRows, size_t rowBytes, const int64_t* inSplits,
                   const int64_t* inOffsets, void* out, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets,
                   int experts, int align, bool inverse, cudaStream_t stream);
+// The quantising form of the forward alltoallvDev (FP8 expert dispatch): `in` holds `inRows` bf16
+// rows of `hidden` elements (a multiple of kFp8Block); each row arrives as `hidden` e4m3 codes in
+// `out` and hidden / kFp8Block fp32 scales in `outScales` (row-major, capacityRows rows), at the
+// same row index, so x ~= code * scale. Per block of kFp8Block elements: amax = max(max|x|, 1e-4),
+// code = e4m3(x * (448 * (1 / amax))) (round to nearest even, saturating), scale = amax / 448,
+// each a correctly rounded fp32 operation. Splits, layout, capacity and error reporting are those of
+// alltoallvDev. `in` and `out` must be 16-byte aligned. For plain pointers the capacity is also
+// capped by what fits the staging pool at hidden + hidden / 32 bytes a row.
+void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidden, const int64_t* inSplits,
+                     const PeerBuffer& out, size_t outOffset, const PeerBuffer& outScales, size_t scalesOffset,
+                     size_t capacityRows, int64_t* outSplits, int64_t* outOffsets, int experts, int align,
+                     cudaStream_t stream);
+void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidden, const int64_t* inSplits,
+                     void* out, float* outScales, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets,
+                     int experts, int align, cudaStream_t stream);
 // Fixed-size alltoall: every chunk is `bytes` long on every rank (this is known to all
 // ranks, so the small-message LL kernel and size-dependent grids are safe here).
 void alltoall(PeerContext& pc, const void* in, const PeerBuffer& out, size_t outOffset, size_t bytes,

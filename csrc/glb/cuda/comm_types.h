@@ -13,7 +13,8 @@ constexpr int kMaxBlocks = 512;   // upper bound on CTAs of one collective kerne
 constexpr int kThreads = 512;     // threads per CTA of the data-moving kernels
 constexpr int kP2pLanes = 64;     // max CTAs per direction of a point-to-point transfer
 constexpr int kMaxA2aExperts = 32;  // local experts per rank of the device-split all-to-all-v
-constexpr int kA2aHdrWords = 6;     // its per-rank header: rowBytes, E, align, inverse, capacity, bad input
+constexpr int kA2aHdrWords = 6;     // its per-rank header: rowBytes, E, align, direction, capacity, bad input
+constexpr int kFp8Block = 128;      // elements per fp32 scale of its quantising (bf16 -> e4m3) form
 
 // Why a kernel gave up (SignalPad::abort / the host status word).
 enum AbortCode : uint32_t {

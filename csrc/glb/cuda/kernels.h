@@ -106,8 +106,16 @@ void launchAlltoallvDev(const CommArgs& a, const PeerPtrs& outs, const void* in,
                         const long long* inSplits, const long long* inOffsets, long long* outSplits,
                         long long* outOffsets, void* stagedOut, uint32_t capRows, int experts, int align, bool inverse,
                         InputStatus* status, int blocks, cudaStream_t stream);
+// Its quantising forward form: `in` holds bf16 rows of `hidden` elements (a multiple of 128);
+// each destination receives e4m3 codes in `outs.p[r]` and one fp32 scale per 128-element block
+// in `scales.p[r]` (rows x hidden / 128). With `stagedOut` / `stagedScales` set, `outs.p[r]` is
+// rank r's staging area and holds its codes, followed by its scales after capRows rows.
+void launchAlltoallvDevFp8(const CommArgs& a, const PeerPtrs& outs, const PeerPtrs& scales, const void* in,
+                           size_t inRows, size_t hidden, const long long* inSplits, long long* outSplits,
+                           long long* outOffsets, void* stagedOut, float* stagedScales, uint32_t capRows, int experts,
+                           int align, InputStatus* status, int blocks, cudaStream_t stream);
 // Entry points, for occupancy queries (every CTA of a collective kernel must be resident).
-const void* alltoallvDevKernelPtr();
+const void* alltoallvDevKernelPtr(bool fp8 = false);
 const void* broadcastKernelPtr();
 const void* gatherPushKernelPtr();
 const void* alltoallPushKernelPtr();

@@ -353,6 +353,96 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
       if (h[pre[E] * 3] != 0.0f) return "combine wrote past its rows";
       return "";
     });
+    // Its quantising form (bf16 -> e4m3 codes + one fp32 scale per 128 elements). Every block holds
+    // small integers and one element of magnitude 448, so its scale is exactly 1 and its codes are
+    // the e4m3 encodings of the inputs. The layout has the closed form of the case above.
+    if (P == 2 || P == 8) {
+      R.run(strcat_all("alltoallvDevKernel<fp8> (dispatch, E=2, align=4, H=256) P=", P), [&]() -> std::string {
+        const int E = 2, A = 4, K = P * E, H = 256, nb = H / kFp8Block;
+        const size_t cap = 512;
+        std::vector<int64_t> sp(K), pre(K + 1, 0);
+        for (int k = 0; k < K; k++) {
+          sp[k] = (k * 5 + 1) % 4;
+          pre[k + 1] = pre[k] + sp[k];
+        }
+        auto base = [&](int j, int e) {
+          int64_t b = 0;
+          for (int x = 0; x < e; x++) b = (b + P * sp[j * E + x] + A - 1) / A * A;
+          return b;
+        };
+        auto value = [&](int64_t r, int i) -> float {
+          const int b = i / kFp8Block, pos = i % kFp8Block;
+          if (pos == (r * 3 + b * 5) % kFp8Block) return (r + b) % 2 ? -448.0f : 448.0f;
+          return static_cast<float>((r * 7 + i * 3) % 33 - 16);
+        };
+        std::vector<uint16_t> rows(pre[K] * H);
+        for (int64_t r = 0; r < pre[K]; r++) {
+          for (int i = 0; i < H; i++) {
+            const float f = value(r, i);
+            uint32_t w;
+            std::memcpy(&w, &f, 4);
+            rows[r * H + i] = static_cast<uint16_t>(w >> 16);  // exact: small integers and 448
+          }
+        }
+        DevBuf in(rows.size() * 2), splits(K * 8), outSplits(K * 8), outOffsets(K * 8);
+        std::vector<std::unique_ptr<DevBuf>> scaleBufs;
+        PeerPtrs sc;
+        std::memset(&sc, 0, sizeof(sc));
+        for (int r = 0; r < P; r++) {
+          scaleBufs.emplace_back(new DevBuf(cap * nb * 4));
+          sc.p[r] = scaleBufs[r]->p;
+          GLB_CUDA_CHECK(cudaMemsetAsync(sc.p[r], 0xff, cap * nb * 4, stream));
+          GLB_CUDA_CHECK(cudaMemsetAsync(pp.p[r], 0xff, cap * H, stream));
+        }
+        GLB_CUDA_CHECK(cudaMemcpyAsync(in.p, rows.data(), rows.size() * 2, cudaMemcpyHostToDevice, stream));
+        GLB_CUDA_CHECK(cudaMemcpyAsync(splits.p, sp.data(), K * 8, cudaMemcpyHostToDevice, stream));
+        const int blocks = std::min(pc.coResidentBlocks(alltoallvDevKernelPtr(true)), 16);
+        launchAlltoallvDevFp8(ca, pp, sc, in.p, pre[K], H, static_cast<const long long*>(splits.p),
+                              static_cast<long long*>(outSplits.p), static_cast<long long*>(outOffsets.p), nullptr,
+                              nullptr, static_cast<uint32_t>(cap), E, A, pc.inputStatusDevice(), blocks, stream);
+        noteLaunch();
+        std::vector<int64_t> os(K), oo(K);
+        GLB_CUDA_CHECK(cudaMemcpyAsync(os.data(), outSplits.p, K * 8, cudaMemcpyDeviceToHost, stream));
+        GLB_CUDA_CHECK(cudaMemcpyAsync(oo.data(), outOffsets.p, K * 8, cudaMemcpyDeviceToHost, stream));
+        for (int j = 0; j < P; j++) {
+          std::vector<uint8_t> codes(cap * H);
+          std::vector<float> scales(cap * nb);
+          GLB_CUDA_CHECK(cudaMemcpyAsync(codes.data(), pp.p[j], codes.size(), cudaMemcpyDeviceToHost, stream));
+          GLB_CUDA_CHECK(cudaMemcpyAsync(scales.data(), sc.p[j], scales.size() * 4, cudaMemcpyDeviceToHost, stream));
+          GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+          for (int e = 0; e < E; e++) {
+            const int k = j * E + e;
+            const int64_t at = base(j, e);
+            for (int64_t r = 0; r < sp[k]; r++) {
+              for (int i = 0; i < H; i++) {
+                const uint8_t want = float8_e4m3::fromFloat(value(pre[k] + r, i));
+                if (codes[(at + r) * H + i] != want) {
+                  return strcat_all("dst ", j, " expert ", e, " row ", r, " element ", i, ": code ",
+                                    static_cast<int>(codes[(at + r) * H + i]), ", want ", static_cast<int>(want));
+                }
+              }
+              for (int b = 0; b < nb; b++) {
+                if (scales[(at + r) * nb + b] != 1.0f) {
+                  return strcat_all("dst ", j, " expert ", e, " row ", r, " scale ", b, ": ", scales[(at + r) * nb + b]);
+                }
+              }
+            }
+            // Virtual rank 1's rows follow and are never written, in either tensor.
+            if (sp[k] > 0 && (codes[(at + sp[k]) * H] != 0xff || !std::isnan(scales[(at + sp[k]) * nb]))) {
+              return strcat_all("dispatch dst ", j, ": wrote past rank 0's segment");
+            }
+          }
+        }
+        for (int e = 0; e < E; e++) {
+          for (int s = 0; s < P; s++) {
+            if (os[e * P + s] != sp[e] || oo[e * P + s] != base(0, e) + s * sp[e]) {
+              return strcat_all("out_splits/out_offsets[", e * P + s, "] = ", os[e * P + s], "/", oo[e * P + s]);
+            }
+          }
+        }
+        return "";
+      });
+    }
 
     // ---- literal schedule executor (halving-doubling, plain and pipelined) -------------------
     R.run(strcat_all("scheduleKernel<float>(halving_doubling) P=", P), [&]() -> std::string {

@@ -196,7 +196,33 @@ void registerCudaAlgorithms(py::module_& m) {
      py::arg("in_offsets"), py::arg("buf"), py::arg("buf_offset"), py::arg("out"), py::arg("capacity_rows"),
      py::arg("out_splits"), py::arg("out_offsets"), py::arg("experts"), py::arg("align"), py::arg("inverse"),
      py::arg("stream"));
-  m.def("alltoall_reg", [](PeerContext& pc, uintptr_t in, const PeerBuffer& out, size_t off, size_t bytes, uintptr_t st) {
+  // Its quantising forward form (bf16 rows of `hidden` elements -> e4m3 codes + fp32 block scales).
+  // `buf` / `scales_buf` are the registered outputs (both None: `out` / `out_scales` are plain
+  // device pointers, staged).
+  m.def("alltoallv_dev_fp8", [](PeerContext& pc, uintptr_t in, size_t inRows, size_t hidden, uintptr_t inSplits,
+                                py::object buf, size_t off, uintptr_t out, py::object scalesBuf, size_t scalesOff,
+                                uintptr_t outScales, size_t capacityRows, uintptr_t outSplits, uintptr_t outOffsets,
+                                int experts, int align, uintptr_t st) {
+    GLB_ENFORCE(buf.is_none() == scalesBuf.is_none(),
+                "alltoallv_dev: out and out_scales must both be registered or both be plain");
+    const PeerBuffer* reg = buf.is_none() ? nullptr : buf.cast<const PeerBuffer*>();
+    const PeerBuffer* sreg = scalesBuf.is_none() ? nullptr : scalesBuf.cast<const PeerBuffer*>();
+    auto* is = reinterpret_cast<const int64_t*>(inSplits);
+    auto* os = reinterpret_cast<int64_t*>(outSplits);
+    auto* oo = reinterpret_cast<int64_t*>(outOffsets);
+    py::gil_scoped_release nogil;
+    if (reg != nullptr) {
+      alltoallvDevFp8(pc, P(in), inRows, hidden, is, *reg, off, *sreg, scalesOff, capacityRows, os, oo, experts, align,
+                      S(st));
+    } else {
+      alltoallvDevFp8(pc, P(in), inRows, hidden, is, P(out), reinterpret_cast<float*>(outScales), capacityRows, os, oo,
+                      experts, align, S(st));
+    }
+  }, py::arg("pc"), py::arg("input"), py::arg("in_rows"), py::arg("hidden"), py::arg("in_splits"), py::arg("buf"),
+     py::arg("buf_offset"), py::arg("out"), py::arg("scales_buf"), py::arg("scales_offset"), py::arg("out_scales"),
+     py::arg("capacity_rows"), py::arg("out_splits"), py::arg("out_offsets"), py::arg("experts"), py::arg("align"),
+     py::arg("stream"));
+  m.def("alltoall_reg",[](PeerContext& pc, uintptr_t in, const PeerBuffer& out, size_t off, size_t bytes, uintptr_t st) {
     py::gil_scoped_release nogil;
     alltoall(pc, P(in), out, off, bytes, S(st));
   });

@@ -351,7 +351,7 @@ class CudaContext:
         return t.data_ptr()
 
     def alltoallv_dev(self, out, inp, in_splits, out_splits, out_offsets, experts: int = 1, align: int = 1,
-                      stream=None):
+                      out_scales=None, stream=None):
         """All-to-all-v whose row counts stay on the device: no host synchronisation, graph-capturable.
 
         ``in_splits`` (int64 CUDA tensor of ``size * experts`` entries): entry ``j * experts + e`` is
@@ -365,7 +365,23 @@ class CudaContext:
         ``check_health()`` after a stream sync) at a point every rank reaches: a rank whose stream
         has not run the call yet does not know about it, and a collective that raises on one rank
         only would leave its peers waiting.
-        Registered / symmetric ``out``: zero copy; any other tensor goes through the staging pool."""
+        Registered / symmetric ``out``: zero copy; any other tensor goes through the staging pool.
+
+        Quantising form (FP8 expert dispatch, the 1x128 per-token-group recipe): ``inp`` bf16
+        ``(rows, H)`` with H a multiple of 128, ``out`` float8_e4m3fn ``(cap, H)`` and ``out_scales``
+        a contiguous float32 ``(cap, H // 128)`` CUDA tensor. The sender quantises while it sends, so
+        the link carries FP8. Each row lands at the same index in ``out`` and ``out_scales``, and
+        ``x ~= float(code) * scale``. Per block of 128 elements, in fp32 with correct rounding:
+        ``amax = max(max |x|, 1e-4)``, ``code = e4m3(x * (448 * (1 / amax)))`` (round to nearest
+        even, saturating), ``scale = amax / 448``: what torch computes for
+        ``(x.float() * (448.0 / amax)).to(torch.float8_e4m3fn)`` and ``amax / 448.0``, byte for byte.
+        NaN and infinite inputs are not supported. ``inp`` and
+        ``out`` must be 16-byte aligned, and ``out`` and ``out_scales`` both registered / symmetric
+        (zero copy) or both plain (staged; the capacity is then also capped by what fits the pool at
+        H + H / 32 bytes a row). Other dtype pairs (other inputs, e5m2) raise ``ValueError``."""
+        if out_scales is not None or self._is_fp8_dispatch(out, inp):
+            return self._alltoallv_dev_fp8(out, inp, in_splits, out_splits, out_offsets, experts, align, out_scales,
+                                           stream)
         rb = self._dev_rows(out, inp)
         k = self.size * int(experts)
         si = self._dev_index(in_splits, "in_splits", k)
@@ -374,6 +390,52 @@ class CudaContext:
         buf, off = self.lookup(out)
         _cu.alltoallv_dev(self.pc, inp.data_ptr(), int(inp.shape[0]), rb, si, 0, buf, off, out.data_ptr(),
                           int(out.shape[0]), so, oo, int(experts), int(align), False, _stream(stream))
+        return out
+
+    @staticmethod
+    def _is_fp8_dispatch(out, inp) -> bool:
+        """A dtype pair that only the quantising form could serve: an FP8 out fed another dtype."""
+        import torch
+
+        return (out.dtype in (torch.float8_e4m3fn, torch.float8_e5m2) and inp.dtype != out.dtype)
+
+    def _alltoallv_dev_fp8(self, out, inp, in_splits, out_splits, out_offsets, experts, align, out_scales, stream):
+        import torch
+
+        form = ("the quantising alltoallv_dev takes bfloat16 input (rows, H) with H a multiple of 128, "
+                "float8_e4m3fn out (cap, H) and float32 out_scales (cap, H // 128)")
+        if out_scales is None:
+            raise ValueError(f"alltoallv_dev: out_scales missing; {form}")
+        if inp.dtype != torch.bfloat16 or out.dtype != torch.float8_e4m3fn:
+            raise ValueError(f"alltoallv_dev: got {inp.dtype} input and {out.dtype} out; {form}")
+        if not isinstance(out_scales, torch.Tensor) or out_scales.dtype != torch.float32:
+            raise ValueError(f"alltoallv_dev: out_scales must be a float32 tensor; {form}")
+        tensors = (inp, out, out_scales)
+        if not all(t.is_cuda and t.device.index == self.device for t in tensors):
+            raise ValueError(f"alltoallv_dev: input, out and out_scales must be CUDA tensors on cuda:{self.device}")
+        if inp.dim() != 2 or out.dim() != 2 or out_scales.dim() != 2:
+            raise ValueError(f"alltoallv_dev: input {tuple(inp.shape)}, out {tuple(out.shape)} and out_scales "
+                             f"{tuple(out_scales.shape)} must be 2-D; {form}")
+        H, cap = int(inp.shape[1]), int(out.shape[0])
+        if H == 0 or H % 128 != 0:
+            raise ValueError(f"alltoallv_dev: row length {H} is not a positive multiple of 128; {form}")
+        if int(out.shape[1]) != H or tuple(out_scales.shape) != (cap, H // 128):
+            raise ValueError(f"alltoallv_dev: out {tuple(out.shape)} and out_scales {tuple(out_scales.shape)} do not "
+                             f"match input rows of {H}; {form}")
+        if not all(t.is_contiguous() for t in tensors):
+            raise ValueError("alltoallv_dev: input, out and out_scales must be contiguous")
+        if inp.data_ptr() % 16 != 0 or out.data_ptr() % 16 != 0:
+            raise ValueError("alltoallv_dev: input and out must be 16-byte aligned for the quantising form")
+        buf, off = self.lookup(out)
+        sbuf, soff = self.lookup(out_scales)
+        if (buf is None) != (sbuf is None):
+            raise ValueError("alltoallv_dev: out and out_scales must both be registered / symmetric or both plain")
+        k = self.size * int(experts)
+        si = self._dev_index(in_splits, "in_splits", k)
+        so = self._dev_index(out_splits, "out_splits", k)
+        oo = self._dev_index(out_offsets, "out_offsets", k)
+        _cu.alltoallv_dev_fp8(self.pc, inp.data_ptr(), int(inp.shape[0]), H, si, buf, off, out.data_ptr(), sbuf, soff,
+                              out_scales.data_ptr(), cap, so, oo, int(experts), int(align), _stream(stream))
         return out
 
     def alltoallv_dev_combine(self, out, inp, in_splits, in_offsets, experts: int = 1, stream=None):

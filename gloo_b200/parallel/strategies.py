@@ -510,6 +510,23 @@ class MoEDispatcher(_Base):
         self.cc.alltoallv_dev(out, tokens, splits, out_splits, out_offsets, experts=experts, align=align)
         return out, out_splits, out_offsets
 
+    def dispatch_dev_fp8(self, tokens, splits, out, out_scales, experts: int = 1, align: int = 1):
+        """dispatch_dev() that quantises on the way: ``tokens`` bf16 ``(rows, H)``, H a multiple of
+        128; ``out`` float8_e4m3fn ``(cap, H)`` receives the codes and ``out_scales`` float32
+        ``(cap, H // 128)`` one scale per 1x128 block, row for row (see
+        ``CudaContext.alltoallv_dev``). One kernel, no host sync, half the bytes of a bf16 dispatch
+        on the link. Returns ``(out, out_scales, out_splits, out_offsets)``. The experts' bf16
+        outputs go back with combine_dev(): the row layout is the same."""
+        import torch
+
+        out_splits = torch.empty(self.size * experts, dtype=torch.int64, device=tokens.device)
+        out_offsets = torch.empty_like(out_splits)
+        self.cc.alltoallv_dev(out, tokens, splits, out_splits, out_offsets, experts=experts, align=align,
+                              out_scales=out_scales)
+        return out, out_scales, out_splits, out_offsets
+
+    dispatch_fp8 = dispatch_dev_fp8
+
     def combine_dev(self, expert_out, out_splits, out_offsets, out, experts: int = 1):
         """Inverse of dispatch_dev(): the rows of ``expert_out`` (dispatch_dev's layout) go back to
         their sources; ``out`` gets them where the dispatched ``tokens`` rows were."""

@@ -12,6 +12,12 @@ Per dispatch + combine pair it times:
 Rows: --tokens x top-k routed to --experts local experts per rank, rows of --hidden elements, in
 bf16 and FP8 e4m3. Outputs are symmetric (zero copy) for every path.
 
+A second table times the FP8 dispatch of bf16 rows (dispatch only, median per call, rank 0):
+  bf16      MoEDispatcher.dispatch_dev of the bf16 rows
+  composed  torch 1x128 quantisation, then alltoallv_dev of the codes and of the scale rows
+  fused     MoEDispatcher.dispatch_dev_fp8 (quantises inside the dispatch kernel)
+The three outputs are checked against each other before timing.
+
     python scripts/bench_moe_dispatch.py [--ranks 2] [--iters 20]
 """
 import argparse
@@ -23,6 +29,9 @@ import sys
 import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+# Ranks may be threads sharing one GPU: a rank loading a torch kernel for the first time must not
+# block behind another rank's collective kernel that waits for it.
+os.environ.setdefault("CUDA_MODULE_LOADING", "EAGER")
 
 import torch  # noqa: E402
 
@@ -101,6 +110,88 @@ def measure(ctx, args, dtype, dev):
     return res
 
 
+def quantise(x):
+    """The 1x128 per-token-group recipe with torch ops (what the fused kernel computes). The scale
+    divides by a tensor: torch's CUDA division by a Python scalar multiplies by its reciprocal."""
+    n, H = x.shape
+    xf = x.float().view(n, H // 128, 128)
+    amax = xf.abs().amax(-1).clamp(min=1e-4)
+    codes = (xf * (448.0 / amax)[..., None]).to(torch.float8_e4m3fn).view(n, H)
+    return codes, amax / torch.full_like(amax, 448.0)
+
+
+def run_rank_fp8(ctx, args, shared):
+    if shared:
+        return measure_fp8(ctx, args, 0)
+    torch.cuda.set_device(ctx.rank)
+    with torch.cuda.stream(gcu.new_stream(ctx.rank)):
+        return measure_fp8(ctx, args, ctx.rank)
+
+
+def measure_fp8(ctx, args, dev):
+    cc = gcu.CudaContext(ctx, dev, stage_bytes=16 << 20)
+    moe = MoEDispatcher(ctx, cc)
+    P, E, H = ctx.size, args.experts, args.hidden
+    G = P * E
+    k = min(args.topk, G)
+    rows = args.tokens * k
+    g = torch.Generator(device="cuda").manual_seed(4321 + ctx.rank)
+    flat = torch.topk(torch.randn(args.tokens, G, device="cuda", generator=g), k, dim=-1).indices.reshape(-1)
+    splits = torch.zeros(G, dtype=torch.int64, device="cuda").index_add_(0, flat, torch.ones_like(flat))
+    tokens = torch.randn(rows, H, device="cuda", generator=g).to(torch.bfloat16)
+    cap = P * rows
+    out_bf16 = cc.empty((cap, H), torch.bfloat16)
+    codes = [cc.empty((cap, H), torch.float8_e4m3fn) for _ in range(2)]
+    scales = [cc.empty((cap, H // 128), torch.float32) for _ in range(2)]
+    osp = torch.empty(G, dtype=torch.int64, device="cuda")
+    ooff, osp2, ooff2 = torch.empty_like(osp), torch.empty_like(osp), torch.empty_like(osp)
+
+    def bf16():
+        moe.dispatch_dev(tokens, splits, out_bf16, experts=E)
+
+    def composed():
+        c, s = quantise(tokens)
+        cc.alltoallv_dev(codes[0], c, splits, osp, ooff, experts=E)
+        cc.alltoallv_dev(scales[0], s, splits, osp2, ooff2, experts=E)
+
+    def fused():
+        moe.dispatch_dev_fp8(tokens, splits, codes[1], scales[1], experts=E)
+
+    quantise(tokens)  # this rank's torch kernels and allocations, before any peer waits on it
+    cc.synchronize()
+    cc.pc.host_barrier()
+    for fn in (bf16, composed, fused):
+        fn()
+    cc.synchronize()
+    # Every received row: fused == composed byte for byte, and both dequantise to the bf16 rows.
+    n = int(osp.sum())
+    lo = int(ooff.min()) if n else 0
+    assert torch.equal(codes[0].view(torch.uint8)[lo:lo + n], codes[1].view(torch.uint8)[lo:lo + n])
+    assert torch.equal(scales[0].view(torch.int32)[lo:lo + n], scales[1].view(torch.int32)[lo:lo + n])
+    deq = (codes[1][lo:lo + n].float().view(n, H // 128, 128) * scales[1][lo:lo + n, :, None]).view(n, H)
+    ref = out_bf16[lo:lo + n].float()
+    assert bool(((deq - ref).abs() <= ref.abs().view(n, H // 128, 128).amax(-1).repeat_interleave(128, -1)
+                 / 16 + 1e-30).all()), "fp8 dispatch is not within e4m3 rounding of the bf16 dispatch"
+
+    def timed(fn):
+        fn()
+        cc.synchronize()
+        times = []
+        for _ in range(args.iters):
+            cc.pc.host_barrier()
+            t0 = time.perf_counter()
+            fn()
+            cc.synchronize()
+            times.append((time.perf_counter() - t0) * 1e3)
+        return statistics.median(times)
+
+    res = {"bf16": timed(bf16), "composed": timed(composed), "fused": timed(fused)}
+    # Bytes this rank sends (its own rows included): bf16 rows, or e4m3 codes + fp32 scales.
+    res["bytes_bf16"] = rows * H * 2
+    res["bytes_fp8"] = rows * (H + H // 128 * 4)
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--ranks", type=int, default=2, help="threads sharing the GPU when only one is visible")
@@ -127,6 +218,16 @@ def main():
         print(f"{str(dtype).replace('torch.', ''):>14} {r['host']:9.3f} {r['dev']:9.3f} {r['graph']:9.3f} "
               f"{r['host'] / r['dev']:9.2f} {r['bytes_per_rank'] / 1e6:9.1f}", flush=True)
         print(json.dumps({"dtype": str(dtype), "ranks": P, "shared_gpu": shared, **r}), flush=True)
+
+    print(f"# FP8 dispatch of bf16 rows ({label}); median of {args.iters} dispatch calls (rank 0)", flush=True)
+    if shared:
+        r = gb.spawn_threads(P, run_rank_fp8, args, True, cuda_device=0, timeout_ms=300000)[0]
+    else:
+        r = gb.spawn_threads(P, run_rank_fp8, args, False, timeout_ms=300000)[0]
+    print(f"{'arm':>10} {'ms':>9} {'MB/rank':>9}")
+    for arm, nbytes in (("bf16", r["bytes_bf16"]), ("composed", r["bytes_fp8"]), ("fused", r["bytes_fp8"])):
+        print(f"{arm:>10} {r[arm]:9.3f} {nbytes / 1e6:9.1f}", flush=True)
+    print(json.dumps({"table": "fp8_dispatch", "ranks": P, "shared_gpu": shared, **r}), flush=True)
 
 
 if __name__ == "__main__":

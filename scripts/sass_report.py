@@ -38,6 +38,8 @@ KERNELS = [
     ("broadcast", r"broadcastKernel"),
     ("gather_push", r"gatherPushKernel"),
     ("alltoall_push", r"alltoallPushKernel"),
+    ("alltoallv_dev", r"alltoallvDevKernel<false>"),
+    ("alltoallv_dev_fp8", r"alltoallvDevKernel<true>"),
     ("p2p_sendrecv", r"p2pKernel"),
     ("exchange_zero_copy", r"exchangeKernel<false>"),
     ("exchange_zero_copy_tma", r"exchangeKernel<true>"),
