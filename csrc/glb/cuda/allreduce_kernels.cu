@@ -34,6 +34,7 @@
 // memory + TCP (cuda_allreduce_ring_chunked.cc:129-273) and reduces on the CPU.
 #include "glb/cuda/device_common.cuh"
 #include "glb/cuda/kernels.h"
+#include "glb/cuda/peer_reduce.cuh"
 
 namespace glb {
 namespace cuda {
@@ -476,37 +477,13 @@ twoShotAllreduceKernel(CommArgs a, PeerPtrs bufs, size_t count, DevOp op, float 
   char* peer[kSlots];
 #pragma unroll
   for (int i = 0; i < kSlots; i++) peer[i] = i < P ? static_cast<char*>(bufs.p[(a.rank + i) % P]) : nullptr;
-
-  for (size_t v0 = vb + tid; v0 < ve; v0 += nthreads * UNROLL) {
-    Pack16 p[UNROLL][kSlots];
+  auto toEveryPeer = [&](size_t v, const Pack16& res) {
 #pragma unroll
-    for (int u = 0; u < UNROLL; u++) {
-      const size_t v = v0 + static_cast<size_t>(u) * nthreads;
-      if (v < ve) {
-#pragma unroll
-        for (int i = 0; i < kSlots; i++) {
-          if (i < P) p[u][i] = ld128_stream(peer[i] + v * 16);
-        }
-      }
+    for (int i = 0; i < kSlots; i++) {
+      if (i < P) st128_stream(peer[i] + v * 16, res);
     }
-#pragma unroll
-    for (int u = 0; u < UNROLL; u++) {
-      const size_t v = v0 + static_cast<size_t>(u) * nthreads;
-      if (v < ve) {
-        typename PT::AccPack acc = PT::widen(p[u][0]);
-#pragma unroll
-        for (int i = 1; i < kSlots; i++) {
-          if (i < P) PT::combine(acc, p[u][i], op);
-        }
-        if (scale != 1.0f) PT::scale(acc, scale);
-        const Pack16 res = PT::narrow(acc);
-#pragma unroll
-        for (int i = 0; i < kSlots; i++) {
-          if (i < P) st128_stream(peer[i] + v * 16, res);
-        }
-      }
-    }
-  }
+  };
+  reducePeers<T, kSlots, UNROLL, 0>(P, vb + tid, ve, nthreads, op, scale, [&](int i) { return peer[i]; }, toEveryPeer);
 
   // Scalar tail (count not a multiple of the pack width, or unaligned buffers):
   // split across ranks the same way.
@@ -531,14 +508,6 @@ twoShotAllreduceKernel(CommArgs a, PeerPtrs bufs, size_t count, DevOp op, float 
 
 // ---- NVLS -----------------------------------------------------------------------------
 
-template <typename T>
-__device__ __forceinline__ Pack16 scalePack(const Pack16& p, float s) {
-  using PT = PackTraits<T>;
-  typename PT::AccPack acc = PT::widen(p);
-  PT::scale(acc, s);
-  return PT::narrow(acc);
-}
-
 template <typename T, int UNROLL>
 __global__ void __launch_bounds__(kThreads)
 nvlsAllreduceKernel(CommArgs a, char* mcBase, PeerPtrs bufs, size_t count, float scale, LocalPtrs extra) {
@@ -562,6 +531,7 @@ nvlsAllreduceKernel(CommArgs a, char* mcBase, PeerPtrs bufs, size_t count, float
   }
   size_t vb, ve;
   shareOf(nvec, P, a.rank, vb, ve);
+  // Not reduceMultimem: through it some UNROLL = 8 instantiations schedule differently and spill.
   for (size_t v0 = vb + tid; v0 < ve; v0 += nthreads * UNROLL) {
     Pack16 r[UNROLL];
 #pragma unroll
@@ -619,20 +589,8 @@ hybridAllreduceKernel(CommArgs a, char* mcBase, PeerPtrs bufs, size_t count, flo
     const size_t nthreads = static_cast<size_t>(nvlsBlocks) * blockDim.x;
     size_t vb, ve;
     shareOf(nvlsVec, P, a.rank, vb, ve);
-    constexpr int U = 2;
-    for (size_t v0 = vb + tid; v0 < ve; v0 += nthreads * U) {
-      Pack16 r[U];
-#pragma unroll
-      for (int u = 0; u < U; u++) {
-        const size_t v = v0 + static_cast<size_t>(u) * nthreads;
-        if (v < ve) r[u] = Multimem<T>::ldReduceAdd(mcBase + v * 16);
-      }
-#pragma unroll
-      for (int u = 0; u < U; u++) {
-        const size_t v = v0 + static_cast<size_t>(u) * nthreads;
-        if (v < ve) multimemSt128(mcBase + v * 16, scale != 1.0f ? scalePack<T>(r[u], scale) : r[u]);
-      }
-    }
+    reduceMultimem<T, 2>(mcBase, vb + tid, ve, nthreads, scale,
+                         [&](size_t v, const Pack16& r) { multimemSt128(mcBase + v * 16, r); });
   } else {
     const size_t tid = static_cast<size_t>(blockIdx.x - nvlsBlocks) * blockDim.x + threadIdx.x;
     const size_t nthreads = static_cast<size_t>(gridDim.x - nvlsBlocks) * blockDim.x;
@@ -643,30 +601,11 @@ hybridAllreduceKernel(CommArgs a, char* mcBase, PeerPtrs bufs, size_t count, flo
     char* peer[P];
 #pragma unroll
     for (int i = 0; i < P; i++) peer[i] = static_cast<char*>(bufs.p[(a.rank + i) % P]);
-    for (size_t v0 = vb + tid; v0 < ve; v0 += nthreads * UP) {
-      Pack16 p[UP][P];
+    auto toEveryPeer = [&](size_t v, const Pack16& res) {
 #pragma unroll
-      for (int u = 0; u < UP; u++) {
-        const size_t v = v0 + static_cast<size_t>(u) * nthreads;
-        if (v < ve) {
-#pragma unroll
-          for (int i = 0; i < P; i++) p[u][i] = ld128_stream(peer[i] + v * 16);
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < UP; u++) {
-        const size_t v = v0 + static_cast<size_t>(u) * nthreads;
-        if (v < ve) {
-          typename PT::AccPack acc = PT::widen(p[u][0]);
-#pragma unroll
-          for (int i = 1; i < P; i++) PT::combine(acc, p[u][i], DevOp::SUM);
-          if (scale != 1.0f) PT::scale(acc, scale);
-          const Pack16 res = PT::narrow(acc);
-#pragma unroll
-          for (int i = 0; i < P; i++) st128_stream(peer[i] + v * 16, res);
-        }
-      }
-    }
+      for (int i = 0; i < P; i++) st128_stream(peer[i] + v * 16, res);
+    };
+    reducePeers<T, P, UP, 0>(P, vb + tid, ve, nthreads, DevOp::SUM, scale, [&](int i) { return peer[i]; }, toEveryPeer);
     // sub-pack tail: peer-to-peer group, split like the two-shot tail
     const size_t tailStart = nvec * PT::kElems;
     size_t tb, te;

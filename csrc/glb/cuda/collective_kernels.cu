@@ -6,6 +6,7 @@
 #include "glb/cuda/device_common.cuh"
 #include "glb/cuda/grid_copy.cuh"
 #include "glb/cuda/kernels.h"
+#include "glb/cuda/peer_reduce.cuh"
 
 namespace glb {
 namespace cuda {
@@ -860,30 +861,9 @@ reducePullKernel(CommArgs a, PeerPtrs ins, char* mcIn, T* __restrict__ out, EArg
   const bool v16 = vec && (off * sizeof(T)) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0;
   const size_t nvec = v16 ? len / PT::kElems : 0;
   const size_t byteOff = off * sizeof(T);
+  auto store = [&](size_t v, const Pack16& r) { st128(reinterpret_cast<char*>(out) + v * 16, r); };
   if (useMc && v16) {
-    if constexpr (hasMultimem<T>()) {
-      constexpr int U = 4;
-      for (size_t v0 = tid; v0 < nvec; v0 += nthreads * U) {
-        Pack16 r[U];
-#pragma unroll
-        for (int u = 0; u < U; u++) {
-          const size_t v = v0 + u * nthreads;
-          if (v < nvec) r[u] = Multimem<T>::ldReduceAdd(mcIn + byteOff + v * 16);
-        }
-#pragma unroll
-        for (int u = 0; u < U; u++) {
-          const size_t v = v0 + u * nthreads;
-          if (v < nvec) {
-            if (scale != 1.0f) {
-              typename PT::AccPack acc = PT::widen(r[u]);
-              PT::scale(acc, scale);
-              r[u] = PT::narrow(acc);
-            }
-            st128(reinterpret_cast<char*>(out) + v * 16, r[u]);
-          }
-        }
-      }
-    }
+    if constexpr (hasMultimem<T>()) reduceMultimem<T, 4>(mcIn + byteOff, tid, nvec, nthreads, scale, store);
   } else {
     constexpr int kSlots = NR > 0 ? NR : kMaxRanks;
     const char* peer[kSlots];
@@ -891,32 +871,7 @@ reducePullKernel(CommArgs a, PeerPtrs ins, char* mcIn, T* __restrict__ out, EArg
     for (int i = 0; i < kSlots; i++) {
       peer[i] = i < P ? static_cast<const char*>(ins.p[(a.rank + i) % P]) + byteOff : nullptr;
     }
-    for (size_t v0 = tid; v0 < nvec; v0 += nthreads * UNROLL) {
-      Pack16 p[UNROLL][kSlots];
-#pragma unroll
-      for (int u = 0; u < UNROLL; u++) {
-        const size_t v = v0 + static_cast<size_t>(u) * nthreads;
-        if (v < nvec) {
-#pragma unroll
-          for (int i = 0; i < kSlots; i++) {
-            if (i < P) p[u][i] = ld128_stream(peer[i] + v * 16);
-          }
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < UNROLL; u++) {
-        const size_t v = v0 + static_cast<size_t>(u) * nthreads;
-        if (v < nvec) {
-          typename PT::AccPack acc = PT::widen(p[u][0]);
-#pragma unroll
-          for (int i = 1; i < kSlots; i++) {
-            if (i < P) PT::combine(acc, p[u][i], op);
-          }
-          if (scale != 1.0f) PT::scale(acc, scale);
-          st128(reinterpret_cast<char*>(out) + v * 16, PT::narrow(acc));
-        }
-      }
-    }
+    reducePeers<T, kSlots, UNROLL, 0>(P, tid, nvec, nthreads, op, scale, [&](int i) { return peer[i]; }, store);
   }
   using TA = TailAcc<T>;
   for (size_t i = nvec * PT::kElems + tid; i < len; i += nthreads) {

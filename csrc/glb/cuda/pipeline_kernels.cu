@@ -63,6 +63,7 @@
 #include "glb/cuda/device_common.cuh"
 #include "glb/cuda/grid_copy.cuh"
 #include "glb/cuda/kernels.h"
+#include "glb/cuda/peer_reduce.cuh"
 
 namespace glb {
 namespace cuda {
@@ -132,6 +133,8 @@ pipelinedAllreduceKernel(CommArgs a, const T* in, T* out, size_t count, DevOp op
       if (i >= 1 && i - 1 < nchunks) {
         const size_t slot = ((i - 1) % 3) * slotBytes;
         const size_t w0 = (static_cast<size_t>(a.rank) * G + b) * T_;
+        // Not reduceMultimem / reducePeers: through them this kernel's registers are allocated
+        // differently, and the instantiations that already spill spill other amounts.
         if constexpr (MC) {
           char* mc = mcStage + slot + w0 * 16;
           constexpr int U = 4;
@@ -398,6 +401,35 @@ pipelinedAllgatherKernel(CommArgs a, const char* in, char* out, PipeBlocks pb, i
   retire(a, static_cast<uint32_t>(nchunks + 1), 0);
 }
 
+// A stage of reduce_scatter and reduce: chunk i of every share of `in` -> sub-slot q of `slot`
+// (tile b of it; `slot` already points at the tile).
+template <typename T>
+__device__ __forceinline__ void stageShares(const T* in, const PipeBlocks& pb, int P, size_t i, size_t chunkElems,
+                                            size_t tileElems, size_t C, char* slot, int ct, int cn) {
+  using PT = PackTraits<T>;
+  constexpr int CU = PT::kElems > 8 ? 2 : 4;
+  for (int q = 0; q < P; q++) {
+    const size_t n = tilePart(pb.len[q], i, chunkElems, tileElems);
+    if (n == 0) continue;
+    const size_t ng = (n + PT::kElems - 1) / PT::kElems;
+    const T* src = in + pb.off[q] + i * chunkElems + blockIdx.x * tileElems;
+    const bool aligned = reinterpret_cast<uintptr_t>(src) % 16 == 0;
+    for (size_t j0 = ct; j0 < ng; j0 += static_cast<size_t>(cn) * CU) {
+      Pack16 p[CU];
+#pragma unroll
+      for (int u = 0; u < CU; u++) {
+        const size_t j = j0 + static_cast<size_t>(u) * cn;
+        if (j < ng) p[u] = loadGroupP(src, j, n, aligned);
+      }
+#pragma unroll
+      for (int u = 0; u < CU; u++) {
+        const size_t j = j0 + static_cast<size_t>(u) * cn;
+        if (j < ng) st128(slot + q * C + j * 16, p[u]);
+      }
+    }
+  }
+}
+
 // Slot: P sub-slots of C bytes, sub-slot q = chunk i of share q. A(i): chunk i of every share of
 // `in` -> my slot i % 2. B(i-1): sub-slot `me` of slot (i-1) % 2 from all P pools, reduced in the
 // accumulator type of PackTraits (fp32 for the 16-bit and FP8 types), scaled, rounded once and
@@ -432,213 +464,30 @@ pipelinedReduceScatterKernel(CommArgs a, const T* in, T* out, PipeBlocks pb, Dev
       if (n > 0) {
         const size_t ng = (n + PT::kElems - 1) / PT::kElems;
         T* dst = out + c * chunkElems + blockIdx.x * tileElems;
-        // Like the peer path of the allreduce pipeline: rank-rotated order, kSlots x U
-        // independent 128-bit loads in flight per thread (half the packs for 16-lane FP8). U is 6
-        // rather than 8 at P = 2, and any P loads in batches (of 4 for 8-byte lanes): the
-        // element-wise output path needs the registers, and this keeps every instantiation free
-        // of spills (-Xptxas -v).
+        // Half the packs for 16-lane FP8, as in the allreduce pipeline. U is 6 rather than 8 at
+        // P = 2, and any P loads in batches (of 4 for 8-byte lanes): the element-wise output path
+        // needs the registers, and this keeps every instantiation free of spills (-Xptxas -v).
         constexpr int kSlots = NR > 0 ? NR : kMaxRanks;
         constexpr int kWide = PT::kElems > 8 ? 2 : 1;
         constexpr int U0 = NR == 2 ? 6 : (NR == 4 ? 4 : (NR == 8 ? 2 : 1));
         constexpr int U = U0 / kWide > 0 ? U0 / kWide : 1;
-        constexpr int kBatch = sizeof(T) == 8 ? 4 : 8;
+        constexpr int kBatch = kSlots <= 8 ? 0 : (sizeof(T) == 8 ? 4 : 8);
         const char* peer[kSlots];
 #pragma unroll
         for (int q = 0; q < kSlots; q++) {
           peer[q] = q < P ? static_cast<const char*>(stage.p[(me + q) % P]) + (c % 2) * slotBytes + me * C + tileOff
                           : nullptr;
         }
-        if constexpr (kSlots > 8) {
-          // Any P: the peers' packs come in batches (same order).
-          for (size_t o = xt; o < ng; o += static_cast<size_t>(xn)) {
-            typename PT::AccPack acc;
-#pragma unroll
-            for (int b0 = 0; b0 < kSlots; b0 += kBatch) {
-              Pack16 v[kBatch];
-#pragma unroll
-              for (int q = 0; q < kBatch; q++) {
-                if (b0 + q < P) v[q] = ld128_stream(peer[b0 + q] + o * 16);
-              }
-#pragma unroll
-              for (int q = 0; q < kBatch; q++) {
-                if (b0 + q == 0) {
-                  acc = PT::widen(v[q]);
-                } else if (b0 + q < P) {
-                  PT::combine(acc, v[q], op);
-                }
-              }
-            }
-            if (scale != 1.0f) PT::scale(acc, scale);
-            storeGroupP(dst, o, n, outAligned, PT::narrow(acc));
-          }
-        } else {
-          for (size_t o0 = xt; o0 < ng; o0 += static_cast<size_t>(xn) * U) {
-            Pack16 v[U][kSlots];
-#pragma unroll
-            for (int u = 0; u < U; u++) {
-              const size_t o = o0 + static_cast<size_t>(u) * xn;
-              if (o < ng) {
-#pragma unroll
-                for (int q = 0; q < kSlots; q++) {
-                  if (q < P) v[u][q] = ld128_stream(peer[q] + o * 16);
-                }
-              }
-            }
-#pragma unroll
-            for (int u = 0; u < U; u++) {
-              const size_t o = o0 + static_cast<size_t>(u) * xn;
-              if (o < ng) {
-                typename PT::AccPack acc = PT::widen(v[u][0]);
-#pragma unroll
-                for (int q = 1; q < kSlots; q++) {
-                  if (q < P) PT::combine(acc, v[u][q], op);
-                }
-                if (scale != 1.0f) PT::scale(acc, scale);
-                storeGroupP(dst, o, n, outAligned, PT::narrow(acc));
-              }
-            }
-          }
-        }
+        reducePeers<T, kSlots, U, kBatch>(P, xt, ng, xn, op, scale, [&](int q) { return peer[q]; },
+                                          [&](size_t o, const Pack16& r) { storeGroupP(dst, o, n, outAligned, r); });
       }
     } else if (i < nchunks) {
       // ---- A(i): chunk i of every share -> my slot (zero past a share's end) ----
-      constexpr int CU = PT::kElems > 8 ? 2 : 4;
-      char* slot = myStage + (i % 2) * slotBytes + tileOff;
-      for (int q = 0; q < P; q++) {
-        const size_t n = tilePart(pb.len[q], i, chunkElems, tileElems);
-        if (n == 0) continue;
-        const size_t ng = (n + PT::kElems - 1) / PT::kElems;
-        const T* src = in + pb.off[q] + i * chunkElems + blockIdx.x * tileElems;
-        const bool aligned = reinterpret_cast<uintptr_t>(src) % 16 == 0;
-        for (size_t j0 = ct; j0 < ng; j0 += static_cast<size_t>(cn) * CU) {
-          Pack16 p[CU];
-#pragma unroll
-          for (int u = 0; u < CU; u++) {
-            const size_t j = j0 + static_cast<size_t>(u) * cn;
-            if (j < ng) p[u] = loadGroupP(src, j, n, aligned);
-          }
-#pragma unroll
-          for (int u = 0; u < CU; u++) {
-            const size_t j = j0 + static_cast<size_t>(u) * cn;
-            if (j < ng) st128(slot + q * C + j * 16, p[u]);
-          }
-        }
-      }
+      stageShares(in, pb, P, i, chunkElems, tileElems, C, myStage + (i % 2) * slotBytes + tileOff, ct, cn);
     }
     if (!blockBarrier(a, e + static_cast<uint32_t>(i) + 1)) break;
   }
   retire(a, static_cast<uint32_t>(nchunks + 1), 0);
-}
-
-// The two data stages of the pipelined reduce below. They do what the A and B stages of the
-// reduce_scatter kernel above do; that kernel keeps its own copy, whose code generation (registers,
-// no spills) was tuned on its own.
-//
-// B stage: n elements (one tile) at byte `srcOff` of every rank's pool, reduced in the accumulator
-// type of PackTraits, scaled, rounded once and stored to dst. dst may start at an address that is
-// not 16-byte aligned (element-wise stores at its groups).
-template <typename T, int NR>
-__device__ __forceinline__ void reducePoolTile(const PeerPtrs& stage, int P, int me, size_t srcOff, T* dst, size_t n,
-                                               DevOp op, float scale, bool outAligned, int xt, int xn) {
-  using PT = PackTraits<T>;
-  const size_t ng = (n + PT::kElems - 1) / PT::kElems;
-  // Rank-rotated order, kSlots x U independent 128-bit loads in flight per thread (half the packs
-  // for 16-lane FP8), any P in batches. Half of reduce_scatter's depth: the kernel also carries the
-  // root's pull stage. Any P takes each peer's address from `stage` at its load instead of holding
-  // 16 pointers in registers. Both keep every instantiation free of spills (-Xptxas -v).
-  constexpr int kSlots = NR > 0 ? NR : kMaxRanks;
-  constexpr int kWide = PT::kElems > 8 ? 2 : 1;
-  constexpr int U0 = NR == 2 ? 4 : (NR == 4 ? 2 : 1);
-  constexpr int U = U0 / kWide > 0 ? U0 / kWide : 1;
-  constexpr int kBatch = sizeof(T) == 8 || PT::kElems > 8 ? 2 : 4;
-  if constexpr (kSlots > 8) {
-    // Any P: the peers' packs come in batches (same order).
-    for (size_t o = xt; o < ng; o += static_cast<size_t>(xn)) {
-      typename PT::AccPack acc;
-#pragma unroll
-      for (int b0 = 0; b0 < kSlots; b0 += kBatch) {
-        Pack16 v[kBatch];
-#pragma unroll
-        for (int q = 0; q < kBatch; q++) {
-          if (b0 + q < P) {
-            const int r = me + b0 + q < P ? me + b0 + q : me + b0 + q - P;
-            v[q] = ld128_stream(static_cast<const char*>(stage.p[r]) + srcOff + o * 16);
-          }
-        }
-#pragma unroll
-        for (int q = 0; q < kBatch; q++) {
-          if (b0 + q == 0) {
-            acc = PT::widen(v[q]);
-          } else if (b0 + q < P) {
-            PT::combine(acc, v[q], op);
-          }
-        }
-      }
-      if (scale != 1.0f) PT::scale(acc, scale);
-      storeGroupP(dst, o, n, outAligned, PT::narrow(acc));
-    }
-  } else {
-    const char* peer[kSlots];
-#pragma unroll
-    for (int q = 0; q < kSlots; q++) {
-      peer[q] = q < P ? static_cast<const char*>(stage.p[(me + q) % P]) + srcOff : nullptr;
-    }
-    for (size_t o0 = xt; o0 < ng; o0 += static_cast<size_t>(xn) * U) {
-      Pack16 v[U][kSlots];
-#pragma unroll
-      for (int u = 0; u < U; u++) {
-        const size_t o = o0 + static_cast<size_t>(u) * xn;
-        if (o < ng) {
-#pragma unroll
-          for (int q = 0; q < kSlots; q++) {
-            if (q < P) v[u][q] = ld128_stream(peer[q] + o * 16);
-          }
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < U; u++) {
-        const size_t o = o0 + static_cast<size_t>(u) * xn;
-        if (o < ng) {
-          typename PT::AccPack acc = PT::widen(v[u][0]);
-#pragma unroll
-          for (int q = 1; q < kSlots; q++) {
-            if (q < P) PT::combine(acc, v[u][q], op);
-          }
-          if (scale != 1.0f) PT::scale(acc, scale);
-          storeGroupP(dst, o, n, outAligned, PT::narrow(acc));
-        }
-      }
-    }
-  }
-}
-
-// A stage: chunk i of every share of `in` -> sub-slot q
-// of `slot` (tile b of it; `slot` already points at the tile).
-template <typename T>
-__device__ __forceinline__ void stageShares(const T* in, const PipeBlocks& pb, int P, size_t i, size_t chunkElems,
-                                            size_t tileElems, size_t C, char* slot, int ct, int cn) {
-  using PT = PackTraits<T>;
-  constexpr int CU = PT::kElems > 8 ? 2 : 4;
-  for (int q = 0; q < P; q++) {
-    const size_t n = tilePart(pb.len[q], i, chunkElems, tileElems);
-    if (n == 0) continue;
-    const size_t ng = (n + PT::kElems - 1) / PT::kElems;
-    const T* src = in + pb.off[q] + i * chunkElems + blockIdx.x * tileElems;
-    const bool aligned = reinterpret_cast<uintptr_t>(src) % 16 == 0;
-    for (size_t j0 = ct; j0 < ng; j0 += static_cast<size_t>(cn) * CU) {
-      Pack16 p[CU];
-#pragma unroll
-      for (int u = 0; u < CU; u++) {
-        const size_t j = j0 + static_cast<size_t>(u) * cn;
-        if (j < ng) p[u] = loadGroupP(src, j, n, aligned);
-      }
-#pragma unroll
-      for (int u = 0; u < CU; u++) {
-        const size_t j = j0 + static_cast<size_t>(u) * cn;
-        if (j < ng) st128(slot + q * C + j * 16, p[u]);
-      }
-    }
-  }
 }
 
 // reduce to `root`: the shares are those of reduce_scatter, with three stages and two more pool
@@ -679,8 +528,30 @@ pipelinedReduceKernel(CommArgs a, const T* in, T* out, PipeBlocks pb, int root, 
       if (n > 0) {
         T* dst = isRoot ? out + pb.off[me] + c * chunkElems + blockIdx.x * tileElems
                         : reinterpret_cast<T*>(myStage + resultOff + (c % 2) * C + tileOff);
-        reducePoolTile<T, NR>(stage, P, me, (c % 2) * slotBytes + me * C + tileOff, dst, n, op, 1.0f, outAligned, xt,
-                              xn);
+        const size_t srcOff = (c % 2) * slotBytes + me * C + tileOff;
+        const size_t ng = (n + PT::kElems - 1) / PT::kElems;
+        auto store = [&](size_t o, const Pack16& r) { storeGroupP(dst, o, n, outAligned, r); };
+        // Half of reduce_scatter's depth: the kernel also carries the root's pull stage. Any P takes
+        // each peer's address from `stage` at its load instead of holding 16 pointers in registers.
+        // Both keep every instantiation free of spills (-Xptxas -v).
+        constexpr int kSlots = NR > 0 ? NR : kMaxRanks;
+        constexpr int kWide = PT::kElems > 8 ? 2 : 1;
+        constexpr int U0 = NR == 2 ? 4 : (NR == 4 ? 2 : 1);
+        constexpr int U = U0 / kWide > 0 ? U0 / kWide : 1;
+        if constexpr (kSlots > 8) {
+          constexpr int kBatch = sizeof(T) == 8 || kWide > 1 ? 2 : 4;
+          auto peer = [&](int q) {
+            return static_cast<const char*>(stage.p[me + q < P ? me + q : me + q - P]) + srcOff;
+          };
+          reducePeers<T, kSlots, U, kBatch>(P, xt, ng, xn, op, 1.0f, peer, store);
+        } else {
+          const char* peer[kSlots];
+#pragma unroll
+          for (int q = 0; q < kSlots; q++) {
+            peer[q] = q < P ? static_cast<const char*>(stage.p[(me + q) % P]) + srcOff : nullptr;
+          }
+          reducePeers<T, kSlots, U, 0>(P, xt, ng, xn, op, 1.0f, [&](int q) { return peer[q]; }, store);
+        }
       }
     } else {
       // ---- C(i-2): the root pulls every peer's reduced share of chunk i-2 ----
