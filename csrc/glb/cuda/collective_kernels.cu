@@ -455,6 +455,94 @@ __device__ __forceinline__ unsigned long long blockExclusiveScan(unsigned long l
 
 __device__ __forceinline__ uint32_t ldPad(const uint32_t* p) { return *reinterpret_cast<const volatile uint32_t*>(p); }
 
+// Before barrier 1: my header and my P·E row counts (kA2aBad for one that is not a valid row count)
+// into column `me` of every rank's a2aHdr / a2aCount, spread over the grid.
+__device__ __forceinline__ void a2aPublish(const CommArgs& a, const long long* inSplits, int K, unsigned long long rb,
+                                           int E, int align, uint32_t direction, uint32_t capRows, bool localBad) {
+  const int P = a.nranks, me = a.rank, t = threadIdx.x;
+  const size_t gtid = static_cast<size_t>(blockIdx.x) * blockDim.x + t;
+  const size_t gthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
+  for (size_t i = gtid; i < static_cast<size_t>(P) * K; i += gthreads) {
+    const int peer = static_cast<int>(i / K), k = static_cast<int>(i % K);
+    const long long x = inSplits[k];
+    a.sig[peer]->a2aCount[k][me] = (x < 0 || x > 0x7fffffffll) ? kA2aBad : static_cast<uint32_t>(x);
+  }
+  if (blockIdx.x == 0 && t < P) {
+    uint32_t* h = &a.sig[t]->a2aHdr[0][me];
+    const uint32_t hdr[kA2aHdrWords] = {static_cast<uint32_t>(rb), static_cast<uint32_t>(E), static_cast<uint32_t>(align),
+                                        direction, capRows, localBad ? 1u : 0u};
+#pragma unroll
+    for (int w = 0; w < kA2aHdrWords; w++) h[w * kMaxRanks] = hdr[w];
+  }
+}
+
+// After barrier 1: whether any rank's header differs from mine or reports bad input of its own,
+// or any count is not a valid row count. sCap[s] gets rank s's capacity.
+__device__ __forceinline__ bool a2aHeadersBad(const SignalPad* pad, int P, int K, unsigned long long rb, int E, int align,
+                                              uint32_t direction, unsigned long long* sCap) {
+  const int t = threadIdx.x;
+  bool b = false;
+  if (t < P) {
+    const uint32_t want[4] = {static_cast<uint32_t>(rb), static_cast<uint32_t>(E), static_cast<uint32_t>(align), direction};
+#pragma unroll
+    for (int w = 0; w < 4; w++) b = b || ldPad(&pad->a2aHdr[w][t]) != want[w];
+    b = b || ldPad(&pad->a2aHdr[5][t]) != 0u;
+    sCap[t] = ldPad(&pad->a2aHdr[4][t]);
+  }
+  for (int i = t; i < P * K; i += blockDim.x) b = b || ldPad(&pad->a2aCount[i % K][i / K]) == kA2aBad;
+  return __syncthreads_or(b) != 0;
+}
+
+// The forward layout from the count matrix. Chunk k = j·E + e of my input lands on rank j at row
+// sDst[k] + sAux[k]: sDst[k] = rows of sources before me in that segment, sAux[k] = where expert e's
+// segment starts on j (a multiple of `align`). sNeed[j] = rows rank j needs, up to the end of its
+// last segment.
+__device__ __forceinline__ void a2aForwardLayout(const SignalPad* pad, int P, int E, int K, int me, int align,
+                                                 unsigned long long* sDst, unsigned long long* sAux,
+                                                 unsigned long long* sNeed) {
+  const int t = threadIdx.x;
+  if (t < K) {
+    unsigned long long before = 0, all = 0;
+    for (int s = 0; s < P; s++) {
+      const unsigned long long m = ldPad(&pad->a2aCount[t][s]);
+      before += s < me ? m : 0ull;
+      all += m;
+    }
+    sDst[t] = before;
+    sAux[t] = all;
+  }
+  __syncthreads();
+  if (t < P) {
+    unsigned long long base = 0;
+    for (int e = 0; e < E; e++) {
+      const unsigned long long n = sAux[t * E + e];
+      sAux[t * E + e] = base;
+      base += n;
+      if (e + 1 < E) base = (base + align - 1) / align * align;
+    }
+    sNeed[t] = base;
+  }
+  __syncthreads();
+}
+
+// Thread 0 of CTA 0, once every rank's input is known: raise the first error, if any, on the host.
+// An overflow names the first rank whose layout needs more rows than it has.
+__device__ __forceinline__ void a2aReport(InputStatus* status, bool invalid, int P, const unsigned long long* sNeed,
+                                          const unsigned long long* sCap) {
+  int over = -1;
+  if (!invalid) {
+    for (int j = P - 1; j >= 0; j--) over = sNeed[j] > sCap[j] ? j : over;
+  }
+  volatile InputStatus* st = status;
+  if (st != nullptr && (invalid || over >= 0) && st->code == kInputOk) {
+    st->rank = over >= 0 ? static_cast<uint32_t>(over) : 0u;
+    st->need = over >= 0 ? sNeed[over] : 0ull;
+    st->avail = over >= 0 ? sCap[over] : 0ull;
+    __threadfence_system();
+    st->code = invalid ? kInputInvalid : kInputOverflow;
+  }
+}
+
 }  // namespace
 
 struct A2aDevArgs {
@@ -584,67 +672,17 @@ alltoallvDevKernel(CommArgs a, PeerPtrs outs, A2aDevKernelArgs<kQuant> d) {
   const bool localBad = __syncthreads_or(bad || (!d.inverse && inTotal > d.inRows)) != 0;
 
   // ---- publish: header + counts into column `me` of every rank's tables, spread over the grid ----
-  {
-    const size_t gtid = static_cast<size_t>(blockIdx.x) * blockDim.x + t;
-    const size_t gthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
-    for (size_t i = gtid; i < static_cast<size_t>(P) * K; i += gthreads) {
-      const int peer = static_cast<int>(i / K), k = static_cast<int>(i % K);
-      const long long x = d.inSplits[k];
-      a.sig[peer]->a2aCount[k][me] = (x < 0 || x > 0x7fffffffll) ? kA2aBad : static_cast<uint32_t>(x);
-    }
-    if (blockIdx.x == 0 && t < P) {
-      uint32_t* h = &a.sig[t]->a2aHdr[0][me];
-      const uint32_t hdr[kA2aHdrWords] = {static_cast<uint32_t>(rb), static_cast<uint32_t>(E), static_cast<uint32_t>(d.align),
-                                          a2aDirection<kQuant>(d.inverse), d.capRows, localBad ? 1u : 0u};
-#pragma unroll
-      for (int w = 0; w < kA2aHdrWords; w++) h[w * kMaxRanks] = hdr[w];
-    }
-  }
+  a2aPublish(a, d.inSplits, K, rb, E, d.align, a2aDirection<kQuant>(d.inverse), d.capRows, localBad);
   // CTA b's release at the barrier must cover what the other CTAs published.
   const bool ok1 = localGridSync(a) && blockBarrier(a, ep + 1);
 
   // ---- the count matrix: validity, capacities, every offset ----
   const SignalPad* pad = a.self;
   bool invalid = false;
-  if (ok1) {
-    bool b = false;
-    if (t < P) {
-      const uint32_t want[4] = {static_cast<uint32_t>(rb), static_cast<uint32_t>(E), static_cast<uint32_t>(d.align),
-                                a2aDirection<kQuant>(d.inverse)};
-#pragma unroll
-      for (int w = 0; w < 4; w++) b = b || ldPad(&pad->a2aHdr[w][t]) != want[w];
-      b = b || ldPad(&pad->a2aHdr[5][t]) != 0u;
-      sCap[t] = ldPad(&pad->a2aHdr[4][t]);
-    }
-    for (int i = t; i < P * K; i += blockDim.x) b = b || ldPad(&pad->a2aCount[i % K][i / K]) == kA2aBad;
-    invalid = __syncthreads_or(b) != 0;
-  }
+  if (ok1) invalid = a2aHeadersBad(pad, P, K, rb, E, d.align, a2aDirection<kQuant>(d.inverse), sCap);
   if (ok1 && !invalid) {
     if (!d.inverse) {
-      // Column k = j·E + e: rows of sources before me, and of all sources.
-      if (t < K) {
-        unsigned long long before = 0, all = 0;
-        for (int s = 0; s < P; s++) {
-          const unsigned long long m = ldPad(&pad->a2aCount[t][s]);
-          before += s < me ? m : 0ull;
-          all += m;
-        }
-        sDst[t] = before;
-        sAux[t] = all;
-      }
-      __syncthreads();
-      // Destination j: expert segments start at multiples of `align`; it needs up to the end of the last.
-      if (t < P) {
-        unsigned long long base = 0;
-        for (int e = 0; e < E; e++) {
-          const unsigned long long n = sAux[t * E + e];
-          sAux[t * E + e] = base;
-          base += n;
-          if (e + 1 < E) base = (base + d.align - 1) / d.align * d.align;
-        }
-        sNeed[t] = base;
-      }
-      __syncthreads();
+      a2aForwardLayout(pad, P, E, K, me, d.align, sDst, sAux, sNeed);
       if (t < K) {
         sDst[t] += sAux[t];
         // My receive segment (e, s), t = e·P + s.
@@ -707,20 +745,7 @@ alltoallvDevKernel(CommArgs a, PeerPtrs outs, A2aDevKernelArgs<kQuant> d) {
 
   // ---- report, receive metadata, payload ----
   if (ok1 && blockIdx.x == 0) {
-    if (t == 0) {
-      int over = -1;
-      if (!invalid) {
-        for (int j = P - 1; j >= 0; j--) over = sNeed[j] > sCap[j] ? j : over;
-      }
-      volatile InputStatus* st = d.status;
-      if (st != nullptr && (invalid || over >= 0) && st->code == kInputOk) {
-        st->rank = over >= 0 ? static_cast<uint32_t>(over) : 0u;
-        st->need = over >= 0 ? sNeed[over] : 0ull;
-        st->avail = over >= 0 ? sCap[over] : 0ull;
-        __threadfence_system();
-        st->code = invalid ? kInputInvalid : kInputOverflow;
-      }
-    }
+    if (t == 0) a2aReport(d.status, invalid, P, sNeed, sCap);
     if (!invalid && !d.inverse && d.outSplits != nullptr && t < K) {
       d.outSplits[t] = sRcvCnt[t];
       d.outOffsets[t] = static_cast<long long>(sRcv[t]);
@@ -833,6 +858,197 @@ void launchAlltoallvDevFp8(const CommArgs& a, const PeerPtrs& outs, const PeerPt
   d.scales = scales;
   d.stagedScales = stagedScales;
   alltoallvDevKernel<true><<<blocks, kThreads, 0, stream>>>(a, outs, d);
+}
+
+// ---- top-k MoE combine: pull each token's expert rows and sum them with its gate weights ---------
+// The mirror of the forward dispatch, run by the source. Chunk k = j·E + e of my dispatch input
+// (splits[k] rows, starting at row sSrc[k]) lies on holder j from row sDst[k] on, sDst as the
+// dispatch computes it from the same count matrix; so input row p of chunk k is holder row
+// sDst[k] + (p - sSrc[k]). Each token's warp reads its k rows there and writes one row locally.
+//   barrier 1  headers and counts published, with the dispatch's code
+//   barrier 2  a plain expert_out copied into its holder's staging area; every rank's bad-pos word
+//              published. The grid sync before it puts every local CTA's stores under CTA b's release:
+//              the barrier pairs CTA b with CTA b only.
+//   barrier 3  every rank has read its rows: holders may reuse expert_out and the staging area.
+// Every path passes all three barriers, so ranks never wait for a different count.
+struct A2aTopkArgs {
+  const long long* splits;   // my dispatch in_splits, P·E entries in j·E + e order
+  const long long* pos;      // (tokens, topk): row of my dispatch input, -1 = not sent
+  const float* weights;      // (tokens, topk)
+  char* out;                 // (tokens, rowBytes), written locally
+  const char* stagedIn;      // plain expert_out: copied into my staging area (srcs.p[me]); null = zero copy
+  unsigned long long tokens;
+  unsigned long long rowBytes;
+  uint32_t capRows;
+  int topk;
+  int experts;
+  int align;
+  InputStatus* status;  // host-mapped
+};
+
+// Header word 3 of the top-k combine: bit 2 marks the form, bit 3 a staged (plain) expert_out, so
+// ranks that mix the form with the dispatch, or symmetric with plain expert_out, read it as invalid.
+constexpr uint32_t kA2aTopkDir = 4u;
+constexpr uint32_t kA2aTopkStaged = 8u;
+constexpr int kTopkInFlight = 4;  // choices whose packs a lane loads before it adds them
+constexpr int kTopkPacks = 2;     // packs of one row per lane per step
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+moeCombineTopkKernel(CommArgs a, PeerPtrs srcs, A2aTopkArgs d) {
+  using PT = PackTraits<T>;
+  constexpr int kMaxK = kMaxRanks * kMaxA2aExperts;
+  __shared__ unsigned long long sSrc[kMaxK];  // my chunk k: first row in my dispatch input
+  __shared__ unsigned long long sDst[kMaxK];  //             first row on its holder
+  __shared__ unsigned long long sAux[kMaxK];  // column sums, then expert bases
+  __shared__ unsigned long long sNeed[kMaxRanks], sCap[kMaxRanks];
+  __shared__ const char* sBase[kMaxRanks];
+  __shared__ unsigned long long sWarp[32];
+  const uint32_t ep = loadEpoch(a);
+  const int P = a.nranks, E = d.experts, K = P * E, me = a.rank, t = threadIdx.x;
+  const unsigned long long rb = d.rowBytes;
+  const uint32_t dir = kA2aTopkDir | (d.stagedIn != nullptr ? kA2aTopkStaged : 0u);
+  const size_t gtid = static_cast<size_t>(blockIdx.x) * blockDim.x + t;
+  const size_t gthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
+
+  // ---- 1. my splits, where each chunk starts in my input; publish; clear my bad-pos word ----
+  const long long v = t < K ? d.splits[t] : 0ll;
+  const bool bad = v < 0 || v > 0x7fffffffll;
+  unsigned long long inRows;
+  const unsigned long long prefix = blockExclusiveScan(bad ? 0ull : static_cast<unsigned long long>(v), sWarp, inRows);
+  if (t < K) sSrc[t] = prefix;
+  if (t < P) sBase[t] = static_cast<const char*>(srcs.p[t]);
+  const bool localBad = __syncthreads_or(bad) != 0;
+  a2aPublish(a, d.splits, K, rb, E, d.align, dir, d.capRows, localBad);
+  if (blockIdx.x == 0 && t < P) a.sig[t]->a2aPosBad[me] = 0u;
+  const bool ok1 = localGridSync(a) && blockBarrier(a, ep + 1);
+
+  // ---- 2. the layout; stage a plain expert_out; check pos ----
+  const SignalPad* pad = a.self;
+  bool invalid = false, over = false;
+  if (ok1) invalid = a2aHeadersBad(pad, P, K, rb, E, d.align, dir, sCap);
+  if (ok1 && !invalid) {
+    a2aForwardLayout(pad, P, E, K, me, d.align, sDst, sAux, sNeed);
+    if (t < K) sDst[t] += sAux[t];
+    over = __syncthreads_or(t < P && sNeed[t] > sCap[t]) != 0;
+  }
+  const bool go = ok1 && !invalid && !over;
+  if (go && d.stagedIn != nullptr) gridCopy(const_cast<char*>(sBase[me]), d.stagedIn, sNeed[me] * rb, true, gtid, gthreads);
+  if (go) {
+    bool b = false;
+    const unsigned long long n = d.tokens * static_cast<unsigned long long>(d.topk);
+    for (size_t i = gtid; i < n; i += gthreads) {
+      const long long p = d.pos[i];
+      b = b || p < -1 || (p >= 0 && static_cast<unsigned long long>(p) >= inRows);
+    }
+    if (__syncthreads_or(b) != 0 && t < P) a.sig[t]->a2aPosBad[me] = 1u;
+  }
+  const bool ok2 = localGridSync(a) && blockBarrier(a, ep + 2);
+
+  // ---- 3. every rank's verdict; pull and reduce ----
+  bool posBad = false;
+  if (ok2 && go) posBad = __syncthreads_or(t < P && ldPad(&pad->a2aPosBad[t]) != 0u) != 0;
+  if (ok1 && ok2 && blockIdx.x == 0 && t == 0) a2aReport(d.status, invalid || posBad, P, sNeed, sCap);
+  if (ok2 && go && !posBad) {
+    const int lane = t & 31, k = d.topk;
+    const unsigned long long npk = rb / 16;
+    for (unsigned long long tok = gtid / 32; tok < d.tokens; tok += gthreads / 32) {
+      // Lane j < k: where choice j's row lies. The last chunk starting at or before p holds it
+      // (an empty chunk starts where the next one does).
+      const char* src = nullptr;
+      float w = 0.0f;
+      if (lane < k) {
+        const long long p = d.pos[tok * k + lane];
+        if (p >= 0) {
+          int lo = 0, hi = K - 1;
+          while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (sSrc[mid] <= static_cast<unsigned long long>(p)) lo = mid; else hi = mid - 1;
+          }
+          src = sBase[lo / E] + (sDst[lo] + (static_cast<unsigned long long>(p) - sSrc[lo])) * rb;
+          w = d.weights[tok * k + lane];
+        }
+      }
+      char* dst = d.out + tok * rb;
+      // Warp-uniform trip count: every lane takes part in the shuffles, lanes past the row end idle.
+      for (unsigned long long v0 = lane; v0 - lane < npk; v0 += 32 * kTopkPacks) {
+        typename PT::AccPack acc[kTopkPacks];
+#pragma unroll
+        for (int u = 0; u < kTopkPacks; u++) {
+#pragma unroll
+          for (int i = 0; i < PT::kElems; i++) acc[u].v[i] = 0.0f;
+        }
+        for (int j0 = 0; j0 < k; j0 += kTopkInFlight) {
+          const char* s[kTopkInFlight];
+          float ws[kTopkInFlight];
+          Pack16 x[kTopkInFlight][kTopkPacks];
+#pragma unroll
+          for (int c = 0; c < kTopkInFlight; c++) {
+            s[c] = reinterpret_cast<const char*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(src), (j0 + c) & 31));
+            ws[c] = __shfl_sync(0xffffffffu, w, (j0 + c) & 31);
+            if (j0 + c >= k) s[c] = nullptr;
+#pragma unroll
+            for (int u = 0; u < kTopkPacks; u++) {
+              const unsigned long long pk = v0 + 32ull * u;
+              if (s[c] != nullptr && pk < npk) x[c][u] = ld128_stream(s[c] + pk * 16);
+            }
+          }
+#pragma unroll
+          for (int c = 0; c < kTopkInFlight; c++) {
+            if (s[c] == nullptr) continue;
+#pragma unroll
+            for (int u = 0; u < kTopkPacks; u++) {
+              const typename PT::AccPack xf = PT::widen(x[c][u]);
+#pragma unroll
+              for (int i = 0; i < PT::kElems; i++) acc[u].v[i] = __fadd_rn(acc[u].v[i], __fmul_rn(ws[c], xf.v[i]));
+            }
+          }
+        }
+#pragma unroll
+        for (int u = 0; u < kTopkPacks; u++) {
+          const unsigned long long pk = v0 + 32ull * u;
+          if (pk < npk) st128(dst + pk * 16, PT::narrow(acc[u]));
+        }
+      }
+    }
+  }
+  blockBarrier(a, ep + 3);
+  // NO pad table or peer reads from here on: a peer that has passed barrier 3 may start its next
+  // launch, which rewrites its columns of my tables and its staging area.
+  retire(a, 3, 0);
+}
+
+namespace {
+// The top-k combine instantiation for dt: float, bfloat16 or float16 rows (null for any other).
+using TopkCombineFn = void (*)(CommArgs, PeerPtrs, A2aTopkArgs);
+TopkCombineFn topkCombineFn(DataType dt) {
+  switch (dt) {
+    case DataType::FLOAT32: return moeCombineTopkKernel<float>;
+    case DataType::BFLOAT16: return moeCombineTopkKernel<__nv_bfloat16>;
+    case DataType::FLOAT16: return moeCombineTopkKernel<__half>;
+    default: return nullptr;
+  }
+}
+}  // namespace
+
+void launchMoeCombineTopk(const CommArgs& a, const PeerPtrs& srcs, const void* stagedIn, void* out, size_t tokens,
+                          int topk, const long long* pos, const float* weights, const long long* splits, size_t rowBytes,
+                          DataType dt, uint32_t capRows, int experts, int align, InputStatus* status, int blocks,
+                          cudaStream_t stream) {
+  A2aTopkArgs d;
+  d.splits = splits;
+  d.pos = pos;
+  d.weights = weights;
+  d.out = static_cast<char*>(out);
+  d.stagedIn = static_cast<const char*>(stagedIn);
+  d.tokens = tokens;
+  d.rowBytes = rowBytes;
+  d.capRows = capRows;
+  d.topk = topk;
+  d.experts = experts;
+  d.align = align;
+  d.status = status;
+  topkCombineFn(dt)<<<blocks, kThreads, 0, stream>>>(a, srcs, d);
 }
 
 // ---- reduce_scatter / reduce: pull my slice from every peer's input, reduce, store -----------
@@ -995,6 +1211,7 @@ const void* alltoallvDevKernelPtr(bool fp8) {
   return fp8 ? reinterpret_cast<const void*>(alltoallvDevKernel<true>)
              : reinterpret_cast<const void*>(alltoallvDevKernel<false>);
 }
+const void* moeCombineTopkKernelPtr(DataType dt) { return reinterpret_cast<const void*>(topkCombineFn(dt)); }
 const void* reducePullKernelPtr(DataType dt, int nranks) {
   const void* k = nullptr;
   dispatchType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(reducePullFn<decltype(tag)>(nranks)); });
@@ -1007,6 +1224,7 @@ void preloadCollectiveKernels() {
   touchKernel(alltoallPushKernel);
   touchKernel(alltoallvDevKernel<false>);
   touchKernel(alltoallvDevKernel<true>);
+  for (DataType dt : {DataType::FLOAT32, DataType::BFLOAT16, DataType::FLOAT16}) touchKernel(topkCombineFn(dt));
   touchKernel(llExchangeKernel);
   for (DataType dt : kAllDataTypes) {
     dispatchType(dt, [&](auto tag) {

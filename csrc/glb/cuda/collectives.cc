@@ -949,6 +949,61 @@ void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidd
                      outOffsets, experts, align, false, stream, &none, outScales);
 }
 
+namespace {
+// `srcs` are the ranks' expert_out (zero copy) or staging areas, `stagedIn` my plain expert_out.
+void combineTopkCommon(PeerContext& pc, void* out, size_t tokens, int topk, const int64_t* pos, const float* weights,
+                       const int64_t* splits, const void* expertOut, const PeerPtrs& srcs, const void* stagedIn,
+                       size_t capacityRows, size_t rowBytes, DataType dt, int experts, int align, cudaStream_t stream) {
+  GLB_TRACE_RANGE("glb::cuda::alltoallv_dev_combine_topk");
+  GLB_ENFORCE(dt == DataType::FLOAT32 || dt == DataType::BFLOAT16 || dt == DataType::FLOAT16,
+              "alltoallv_dev_combine_topk: rows must be float32, bfloat16 or float16");
+  GLB_ENFORCE(topk >= 1 && topk <= 32, "alltoallv_dev_combine_topk: topk must be in 1..32, got ", topk);
+  GLB_ENFORCE(experts >= 1 && experts <= kMaxA2aExperts, "alltoallv_dev_combine_topk: experts per rank must be in 1..",
+              kMaxA2aExperts, ", got ", experts);
+  GLB_ENFORCE(align >= 1, "alltoallv_dev_combine_topk: align must be at least 1, got ", align);
+  GLB_ENFORCE(rowBytes > 0 && rowBytes % 16 == 0 && rowBytes <= 0xffffffffull,
+              "alltoallv_dev_combine_topk: the row size must be a positive multiple of 16 bytes, got ", rowBytes);
+  GLB_ENFORCE(splits != nullptr && (tokens == 0 || (pos != nullptr && weights != nullptr && out != nullptr)),
+              "alltoallv_dev_combine_topk: missing splits, pos, weights or out");
+  GLB_ENFORCE(reinterpret_cast<uintptr_t>(out) % 16 == 0 && reinterpret_cast<uintptr_t>(expertOut) % 16 == 0,
+              "alltoallv_dev_combine_topk: out and expert_out must be 16-byte aligned");
+  const uint32_t cap = static_cast<uint32_t>(std::min<size_t>(capacityRows, 0xfffffffeull));
+  const int blocks =
+      std::max(1, std::min({tuning().alltoallvBlocks, pc.coResidentBlocks(moeCombineTopkKernelPtr(dt)), kMaxBlocks}));
+  prologue(pc, stream);
+  launchMoeCombineTopk(pc.comm(), srcs, stagedIn, out, tokens, topk, reinterpret_cast<const long long*>(pos), weights,
+                       reinterpret_cast<const long long*>(splits), rowBytes, dt, cap, experts, align,
+                       pc.inputStatusDevice(), blocks, stream);
+  finish(pc, stream, "alltoallv_dev_combine_topk");
+}
+}  // namespace
+
+void alltoallvDevCombineTopk(PeerContext& pc, void* out, size_t tokens, int topk, const int64_t* pos,
+                             const float* weights, const int64_t* splits, const PeerBuffer& expertOut, size_t offset,
+                             size_t capacityRows, size_t rowBytes, DataType dt, int experts, int align,
+                             cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  GLB_ENFORCE_LE(offset + capacityRows * rowBytes, expertOut.bytes,
+                 "alltoallv_dev_combine_topk: expert_out exceeds the registered buffer");
+  const char* mine = static_cast<const char*>(expertOut.local) + offset;
+  // Peers read my expert_out while I write my out.
+  rejectOverlap(mine, capacityRows * rowBytes, out, tokens * rowBytes, "alltoallv_dev_combine_topk");
+  combineTopkCommon(pc, out, tokens, topk, pos, weights, splits, mine,
+                    expertOut.ptrsAt(offset), nullptr, capacityRows, rowBytes, dt, experts, align, stream);
+}
+
+void alltoallvDevCombineTopk(PeerContext& pc, void* out, size_t tokens, int topk, const int64_t* pos,
+                             const float* weights, const int64_t* splits, const void* expertOut, size_t capacityRows,
+                             size_t rowBytes, DataType dt, int experts, int align, cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  GLB_ENFORCE(rowBytes > 0, "alltoallv_dev_combine_topk: row size must be positive");
+  rejectOverlap(expertOut, capacityRows * rowBytes, out, tokens * rowBytes, "alltoallv_dev_combine_topk");
+  // Each rank copies its rows into its own staging area, where its peers read them.
+  const auto l = layoutOf(pc);
+  combineTopkCommon(pc, out, tokens, topk, pos, weights, splits, expertOut, pc.stagePtrs(l.bulkOff), expertOut,
+                    std::min(capacityRows, l.bulkBytes / rowBytes), rowBytes, dt, experts, align, stream);
+}
+
 void scatter(PeerContext& pc, const void* in, const PeerBuffer& out, size_t outOffset, size_t bytes, int root,
              cudaStream_t stream) {
   DeviceGuard g(pc.device);

@@ -171,6 +171,25 @@ void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidd
 void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidden, const int64_t* inSplits,
                      void* out, float* outScales, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets,
                      int experts, int align, cudaStream_t stream);
+// Top-k MoE combine: the inverse of the forward alltoallvDev fused with the gate-weighted sum.
+// `splits` is the in_splits this rank passed to the dispatch; `expertOut` holds, on every rank, the
+// experts' output rows (`rowBytes` each, dtype dt: float, bfloat16 or float16) in that dispatch's
+// output layout, `capacityRows` of them. `pos` / `weights` are (tokens, topk): pos[t, j] is the row
+// of my dispatch input that carried token t's choice j (-1: not sent). out row t =
+// round(sum over j with pos[t, j] >= 0, in order, of weights[t, j] * float(row)), each step a
+// correctly rounded fp32 multiply and add, starting from +0. The source pulls its rows, so nothing
+// but `out` is written. Registered expertOut: read in place; plain: each rank stages its rows
+// through its pool, which caps the capacity. Rows must be a multiple of 16 bytes, expertOut and
+// out 16-byte aligned and disjoint, 1 <= topk <= 32. Errors found on the device (splits, a pos
+// out of range, arguments that differ between ranks, an overflowing holder) are raised like
+// alltoallvDev's, and no rank writes its out.
+void alltoallvDevCombineTopk(PeerContext& pc, void* out, size_t tokens, int topk, const int64_t* pos,
+                             const float* weights, const int64_t* splits, const PeerBuffer& expertOut, size_t offset,
+                             size_t capacityRows, size_t rowBytes, DataType dt, int experts, int align,
+                             cudaStream_t stream);
+void alltoallvDevCombineTopk(PeerContext& pc, void* out, size_t tokens, int topk, const int64_t* pos,
+                             const float* weights, const int64_t* splits, const void* expertOut, size_t capacityRows,
+                             size_t rowBytes, DataType dt, int experts, int align, cudaStream_t stream);
 // Fixed-size alltoall: every chunk is `bytes` long on every rank (this is known to all
 // ranks, so the small-message LL kernel and size-dependent grids are safe here).
 void alltoall(PeerContext& pc, const void* in, const PeerBuffer& out, size_t outOffset, size_t bytes,

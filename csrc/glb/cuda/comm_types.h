@@ -80,6 +80,11 @@ struct alignas(128) SignalPad {
   // steps, even when every block is empty. 32-bit entries: in the loopback self-test peer pads are
   // this pad shifted by one column, which keeps them aligned.
   uint32_t pipeChunks[kMaxRanks];
+  // Top-k MoE combine (moeCombineTopkKernel): rank s clears column s of this table in EVERY rank's
+  // pad with its header, before barrier 1, and sets it between barriers 1 and 2 if one of its `pos`
+  // entries is out of range; every rank reads its own row between barriers 2 and 3. Rank s rewrites
+  // its column only in a later launch, after every CTA of every rank has arrived at barrier 3.
+  uint32_t a2aPosBad[kMaxRanks];
 };
 
 struct CommArgs {

@@ -114,8 +114,18 @@ void launchAlltoallvDevFp8(const CommArgs& a, const PeerPtrs& outs, const PeerPt
                            size_t inRows, size_t hidden, const long long* inSplits, long long* outSplits,
                            long long* outOffsets, void* stagedOut, float* stagedScales, uint32_t capRows, int experts,
                            int align, InputStatus* status, int blocks, cudaStream_t stream);
+// Top-k MoE combine, the mirror of the forward form: for each of `tokens` tokens, out row t =
+// sum over j < topk with pos[t, j] >= 0, in order, of weights[t, j] * (row pos[t, j] of my dispatch
+// input, as it lies on the rank holding its expert), in fp32, rounded to dt (float, bfloat16 or
+// float16). `splits` is my dispatch in_splits. `srcs.p[r]` is rank r's expert_out (zero copy) or
+// staging area; with `stagedIn` set (my plain expert_out) each rank first copies its rows there.
+void launchMoeCombineTopk(const CommArgs& a, const PeerPtrs& srcs, const void* stagedIn, void* out, size_t tokens,
+                          int topk, const long long* pos, const float* weights, const long long* splits, size_t rowBytes,
+                          DataType dt, uint32_t capRows, int experts, int align, InputStatus* status, int blocks,
+                          cudaStream_t stream);
 // Entry points, for occupancy queries (every CTA of a collective kernel must be resident).
 const void* alltoallvDevKernelPtr(bool fp8 = false);
+const void* moeCombineTopkKernelPtr(DataType dt);
 const void* broadcastKernelPtr();
 const void* gatherPushKernelPtr();
 const void* alltoallPushKernelPtr();

@@ -429,7 +429,8 @@ void PeerContext::checkHealth() {
       }
       GLB_THROW(InputException,
                 "alltoallv_dev: invalid splits (a negative or > 2^31-1 count, an offset outside the input, splits "
-                "summing to more rows than the input has, or arguments that differ between ranks); nothing was sent");
+                "summing to more rows than the input has, a top-k position outside the dispatch input, or arguments "
+                "that differ between ranks); nothing was sent");
     }
     poisoned_ = true;
     const uint32_t code = st & 0xffu, who = st >> 8;

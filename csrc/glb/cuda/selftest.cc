@@ -442,6 +442,80 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
         }
         return "";
       });
+      // The top-k combine, zero copy, with the closed-form layout of the dispatch case above: rank 0's
+      // chunk k = j·E + e lies on virtual holder j from row base(j, e) on. Holder j's expert_out
+      // (pp.p[j]) holds bf16 halves of small integers; the host sums in the kernel's fp32 order.
+      R.run(strcat_all("moeCombineTopkKernel<bf16> (E=2, align=4, k=3, 64-element rows) P=", P), [&]() -> std::string {
+        const int E = 2, A = 4, K = P * E, H = 64, topk = 3;
+        const size_t rb = H * 2, cap = n * 4 / rb, T = 37;
+        std::vector<int64_t> sp(K), pre(K + 1, 0);
+        for (int k = 0; k < K; k++) {
+          sp[k] = (k * 5 + 2) % 4;
+          pre[k + 1] = pre[k] + sp[k];
+        }
+        auto base = [&](int j, int e) {
+          int64_t b = 0;
+          for (int x = 0; x < e; x++) b = (b + P * sp[j * E + x] + A - 1) / A * A;
+          return b;
+        };
+        auto value = [](int j, int64_t row, int c) { return static_cast<float>((j * 7 + row * 3 + c) % 17 - 8) * 0.5f; };
+        std::vector<int64_t> pos(T * topk);
+        std::vector<float> w(T * topk);
+        for (size_t t = 0; t < T; t++) {
+          for (int c = 0; c < topk; c++) {
+            pos[t * topk + c] = (t * c) % 5 == 1 || t == 4 ? -1 : static_cast<int64_t>((t * 7 + c * 11) % pre[K]);
+            w[t * topk + c] = static_cast<float>((t * 5 + c * 3) % 9) * 0.3f - 1.1f;
+          }
+        }
+        for (int j = 0; j < P; j++) {
+          std::vector<uint16_t> rows(cap * H);
+          for (size_t r = 0; r < cap; r++) {
+            for (int c = 0; c < H; c++) {
+              const float f = value(j, r, c);
+              uint32_t u;
+              std::memcpy(&u, &f, 4);
+              rows[r * H + c] = static_cast<uint16_t>(u >> 16);  // exact: halves of small integers
+            }
+          }
+          GLB_CUDA_CHECK(cudaMemcpyAsync(pp.p[j], rows.data(), rows.size() * 2, cudaMemcpyHostToDevice, stream));
+          GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+        }
+        DevBuf splits(K * 8), posDev(pos.size() * 8), wDev(w.size() * 4), out(T * rb);
+        GLB_CUDA_CHECK(cudaMemcpyAsync(splits.p, sp.data(), K * 8, cudaMemcpyHostToDevice, stream));
+        GLB_CUDA_CHECK(cudaMemcpyAsync(posDev.p, pos.data(), pos.size() * 8, cudaMemcpyHostToDevice, stream));
+        GLB_CUDA_CHECK(cudaMemcpyAsync(wDev.p, w.data(), w.size() * 4, cudaMemcpyHostToDevice, stream));
+        GLB_CUDA_CHECK(cudaMemsetAsync(out.p, 0xff, T * rb, stream));
+        const int blocks = std::min(pc.coResidentBlocks(moeCombineTopkKernelPtr(DataType::BFLOAT16)), 16);
+        launchMoeCombineTopk(ca, pp, nullptr, out.p, T, topk, static_cast<const long long*>(posDev.p),
+                             static_cast<const float*>(wDev.p), static_cast<const long long*>(splits.p), rb,
+                             DataType::BFLOAT16, static_cast<uint32_t>(cap), E, A, pc.inputStatusDevice(), blocks,
+                             stream);
+        noteLaunch();
+        std::vector<uint16_t> got(T * H);
+        GLB_CUDA_CHECK(cudaMemcpyAsync(got.data(), out.p, T * rb, cudaMemcpyDeviceToHost, stream));
+        GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+        for (size_t t = 0; t < T; t++) {
+          for (int c = 0; c < H; c++) {
+            float acc = 0.0f;
+            for (int x = 0; x < topk; x++) {
+              const int64_t p = pos[t * topk + x];
+              if (p < 0) continue;
+              int k = 0;
+              while (pre[k + 1] <= p) k++;
+              const float prod = w[t * topk + x] * value(k / E, base(k / E, k % E) + (p - pre[k]), c);
+              acc = acc + prod;
+            }
+            uint32_t u;
+            std::memcpy(&u, &acc, 4);
+            const uint16_t want = static_cast<uint16_t>((u + 0x7fffu + ((u >> 16) & 1u)) >> 16);  // round to nearest even
+            if (got[t * H + c] != want) {
+              return strcat_all("token ", t, " element ", c, ": got bf16 bits ", static_cast<int>(got[t * H + c]),
+                                ", want ", static_cast<int>(want));
+            }
+          }
+        }
+        return "";
+      });
     }
 
     // ---- literal schedule executor (halving-doubling, plain and pipelined) -------------------

@@ -222,6 +222,28 @@ void registerCudaAlgorithms(py::module_& m) {
      py::arg("buf_offset"), py::arg("out"), py::arg("scales_buf"), py::arg("scales_offset"), py::arg("out_scales"),
      py::arg("capacity_rows"), py::arg("out_splits"), py::arg("out_offsets"), py::arg("experts"), py::arg("align"),
      py::arg("stream"));
+  // Top-k MoE combine. `buf` is the registered expert_out (None: `expert_out` is a plain device
+  // pointer, staged); pos / weights / splits are addresses of device arrays.
+  m.def("alltoallv_dev_combine_topk", [](PeerContext& pc, uintptr_t out, size_t tokens, int topk, uintptr_t pos,
+                                         uintptr_t weights, uintptr_t splits, py::object buf, size_t off,
+                                         uintptr_t expertOut, size_t capacityRows, size_t rowBytes, int dtype,
+                                         int experts, int align, uintptr_t st) {
+    const PeerBuffer* reg = buf.is_none() ? nullptr : buf.cast<const PeerBuffer*>();
+    auto* ps = reinterpret_cast<const int64_t*>(pos);
+    auto* ws = reinterpret_cast<const float*>(weights);
+    auto* sp = reinterpret_cast<const int64_t*>(splits);
+    const DataType dt = static_cast<DataType>(dtype);
+    py::gil_scoped_release nogil;
+    if (reg != nullptr) {
+      alltoallvDevCombineTopk(pc, P(out), tokens, topk, ps, ws, sp, *reg, off, capacityRows, rowBytes, dt, experts,
+                              align, S(st));
+    } else {
+      alltoallvDevCombineTopk(pc, P(out), tokens, topk, ps, ws, sp, P(expertOut), capacityRows, rowBytes, dt, experts,
+                              align, S(st));
+    }
+  }, py::arg("pc"), py::arg("out"), py::arg("tokens"), py::arg("topk"), py::arg("pos"), py::arg("weights"),
+     py::arg("splits"), py::arg("buf"), py::arg("buf_offset"), py::arg("expert_out"), py::arg("capacity_rows"),
+     py::arg("row_bytes"), py::arg("dtype"), py::arg("experts"), py::arg("align"), py::arg("stream"));
   m.def("alltoall_reg",[](PeerContext& pc, uintptr_t in, const PeerBuffer& out, size_t off, size_t bytes, uintptr_t st) {
     py::gil_scoped_release nogil;
     alltoall(pc, P(in), out, off, bytes, S(st));

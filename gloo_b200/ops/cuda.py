@@ -452,6 +452,76 @@ class CudaContext:
                           int(out.shape[0]), 0, 0, int(experts), 1, True, _stream(stream))
         return out
 
+    def alltoallv_dev_combine_topk(self, out, expert_out, splits, pos, weights, experts: int = 1, align: int = 1,
+                                   stream=None):
+        """Top-k MoE combine: the inverse of :meth:`alltoallv_dev` fused with the gate-weighted sum over
+        each token's choices. One kernel, no host synchronisation, graph-capturable.
+
+        ``splits`` is the int64 ``(size * experts,)`` tensor this rank passed as ``in_splits`` to the
+        dispatch. ``expert_out`` holds, on every rank, the experts' output in that dispatch's output
+        layout (``experts`` and ``align`` as there), float32, bfloat16 or float16; ``expert_out.shape[0]``
+        is its capacity. ``pos`` is int64 ``(T, k)``: ``pos[t, j]`` is the row of this rank's dispatch
+        input that carried token t's choice j, -1 if it was not sent. ``weights`` is float32
+        ``(T, k)``; the weight of a -1 entry is ignored. ``out`` is ``(T, *expert_out.shape[1:])`` of
+        ``expert_out``'s dtype, written on this rank only:
+        ``out[t] = round(acc)``, ``acc`` starting at +0.0 and, for j = 0..k-1 with ``pos[t, j] >= 0``
+        in that order, ``acc = acc + w[t, j] * float(row)``, each a correctly rounded fp32 multiply or
+        add (no fused multiply-add), rounded to nearest even into the dtype. That is what torch
+        computes on the CPU for ``acc[m] = acc[m] + w[m, j, None] * rows[pos[m, j]].float()``, where
+        ``rows`` is what :meth:`alltoallv_dev_combine` would return.
+
+        Each rank pulls its tokens' rows from the ranks holding their experts, so no rank receives
+        ``T * k`` rows to reduce itself. Registered / symmetric ``expert_out``: read in place; any
+        other tensor is first copied into its rank's staging pool, which also caps the capacity.
+        Every rank must pass the same kind. Rows must be a multiple of 16 bytes, ``expert_out`` and
+        ``out`` 16-byte aligned, contiguous and disjoint, and 1 <= k <= 32; otherwise ``ValueError``
+        before launch. A ``pos`` entry below -1 or at least ``splits.sum()``, invalid splits,
+        arguments that differ between ranks, or an ``expert_out`` below the rows its layout needs
+        raise ``ValueError`` on every rank at the next host call after the kernel has run (see
+        :meth:`alltoallv_dev`), and no rank's ``out`` is written."""
+        import torch
+
+        name = "alltoallv_dev_combine_topk"
+        dtypes = (torch.float32, torch.bfloat16, torch.float16)
+        tensors = {"out": out, "expert_out": expert_out, "pos": pos, "weights": weights}
+        for what, t in tensors.items():
+            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
+                raise ValueError(f"{name}: {what} must be a CUDA tensor on cuda:{self.device}")
+            if not t.is_contiguous():
+                raise ValueError(f"{name}: {what} must be contiguous")
+        if expert_out.dtype not in dtypes or out.dtype != expert_out.dtype:
+            raise ValueError(f"{name}: expert_out and out must share a dtype of float32, bfloat16 or float16, got "
+                             f"{expert_out.dtype} and {out.dtype}")
+        if pos.dtype != torch.int64 or pos.dim() != 2 or weights.dtype != torch.float32 or weights.shape != pos.shape:
+            raise ValueError(f"{name}: pos must be int64 (T, k) and weights float32 of the same shape, got "
+                             f"{pos.dtype} {tuple(pos.shape)} and {weights.dtype} {tuple(weights.shape)}")
+        T, k = int(pos.shape[0]), int(pos.shape[1])
+        if not 1 <= k <= 32:
+            raise ValueError(f"{name}: k = {k} choices per token; 1..32 are supported")
+        if expert_out.dim() < 2 or tuple(out.shape) != (T, *expert_out.shape[1:]):
+            raise ValueError(f"{name}: out {tuple(out.shape)} must be (T, *expert_out.shape[1:]) with T = {T}, "
+                             f"expert_out {tuple(expert_out.shape)} at least 2-D")
+        rb = expert_out.element_size()
+        for d in expert_out.shape[1:]:
+            rb *= int(d)
+        if rb == 0 or rb % 16 != 0:
+            raise ValueError(f"{name}: rows of {rb} bytes; a positive multiple of 16 is required")
+        if expert_out.data_ptr() % 16 != 0 or out.data_ptr() % 16 != 0:
+            raise ValueError(f"{name}: expert_out and out must be 16-byte aligned")
+        e0, e1 = expert_out.data_ptr(), expert_out.data_ptr() + expert_out.numel() * expert_out.element_size()
+        o0, o1 = out.data_ptr(), out.data_ptr() + out.numel() * out.element_size()
+        if e0 < o1 and o0 < e1:
+            raise ValueError(f"{name}: out and expert_out overlap")
+        if not 1 <= int(experts) <= 32 or int(align) < 1:
+            raise ValueError(f"{name}: experts must be in 1..32 and align at least 1, got {experts} and {align}")
+        si = self._dev_index(splits, "splits", self.size * int(experts))
+        buf, off = self.lookup(expert_out)
+        _cu.alltoallv_dev_combine_topk(self.pc, out.data_ptr(), T, k, pos.data_ptr(), weights.data_ptr(), si, buf, off,
+                                       expert_out.data_ptr(), int(expert_out.shape[0]), rb,
+                                       int(_torch_dtype_to_glb(expert_out.dtype)), int(experts), int(align),
+                                       _stream(stream))
+        return out
+
     def scatter(self, output, input=None, root: int = 0, stream=None):
         """Block ``rank`` of the root's ``input`` -> ``output``. Any size; ``input`` is read on the
         root only (None elsewhere)."""

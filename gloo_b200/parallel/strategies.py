@@ -532,6 +532,40 @@ class MoEDispatcher(_Base):
         their sources; ``out`` gets them where the dispatched ``tokens`` rows were."""
         return self.cc.alltoallv_dev_combine(out, expert_out, out_splits, out_offsets, experts=experts)
 
+    def route(self, x, topk_idx, experts: int = 1):
+        """Dispatch input for top-k routing, in pure torch with no host synchronisation (CPU tensors
+        work too). ``topk_idx`` is ``(T, k)``: entry ``j * experts + e`` sends the token to local
+        expert ``e`` of rank ``j``; an entry outside ``0 .. size * experts - 1``, such as -1, is not
+        routed. Returns ``(rows, splits, pos)``:
+        - ``rows`` holds ``T * k`` rows of ``x``. The first ``splits.sum()`` are the routed
+          choices, packed in (rank, expert) order and by token within each, ready for
+          ``dispatch_dev``. The rest are unrouted choices and are never sent.
+        - ``splits`` is the int64 ``(size * experts,)`` row count per (rank, expert).
+        - ``pos`` is int64 ``(T, k)``: the row of ``rows`` that carries each choice, or -1. It is
+          what ``combine_dev_topk`` takes."""
+        import torch
+
+        T, k = int(topk_idx.shape[0]), int(topk_idx.shape[1])
+        G = self.size * int(experts)
+        flat = topk_idx.reshape(-1).long()
+        routed = (flat >= 0) & (flat < G)
+        key = torch.where(routed, flat, torch.full_like(flat, G))  # unrouted choices sort last
+        order = torch.argsort(key, stable=True)
+        counts = torch.zeros(G + 1, dtype=torch.int64, device=flat.device)
+        counts.index_add_(0, key, torch.ones_like(key))
+        pos = torch.empty_like(flat).scatter_(0, order, torch.arange(T * k, dtype=torch.int64, device=flat.device))
+        pos = torch.where(routed, pos, torch.full_like(pos, -1)).view(T, k)
+        return x.index_select(0, order // k), counts[:G], pos
+
+    def combine_dev_topk(self, expert_out, splits, pos, weights, out, experts: int = 1, align: int = 1):
+        """The inverse of dispatch_dev() fused with the gate-weighted sum: ``out[t]`` = sum over
+        token t's routed choices j of ``weights[t, j]`` times its expert's output row, in fp32 in
+        the order of j, rounded to ``out``'s dtype. ``splits`` and ``pos`` come from route() (or
+        describe the dispatch input the same way), ``expert_out`` is in dispatch_dev()'s output
+        layout with the same ``experts`` and ``align``. See
+        ``CudaContext.alltoallv_dev_combine_topk``."""
+        return self.cc.alltoallv_dev_combine_topk(out, expert_out, splits, pos, weights, experts=experts, align=align)
+
 
 class UlyssesAttention(_Base):
     """DeepSpeed-Ulysses: [S/P, H, D] <-> [S, H/P, D] with one alltoall each way."""

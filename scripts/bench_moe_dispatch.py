@@ -18,6 +18,13 @@ A second table times the FP8 dispatch of bf16 rows (dispatch only, median per ca
   fused     MoEDispatcher.dispatch_dev_fp8 (quantises inside the dispatch kernel)
 The three outputs are checked against each other before timing.
 
+A third table times the top-k combine, the end of a MoE layer (median per call, rank 0), with the
+experts' output symmetric (read in place) and plain (staged through each rank's pool):
+  composed  MoEDispatcher.combine_dev, un-permute, and the gate-weighted sum over k in torch (fp32)
+  topk      MoEDispatcher.combine_dev_topk (pulls each token's k rows and sums them in one kernel)
+Both arms' outputs are checked equal byte for byte before timing. MB/rank counts the expert rows
+that reach this rank plus its (tokens, hidden) result, from the shapes.
+
     python scripts/bench_moe_dispatch.py [--ranks 2] [--iters 20]
 """
 import argparse
@@ -192,6 +199,72 @@ def measure_fp8(ctx, args, dev):
     return res
 
 
+def run_rank_topk(ctx, args, shared):
+    if shared:
+        return measure_topk(ctx, args, 0)
+    torch.cuda.set_device(ctx.rank)
+    with torch.cuda.stream(gcu.new_stream(ctx.rank)):
+        return measure_topk(ctx, args, ctx.rank)
+
+
+def measure_topk(ctx, args, dev):
+    P, E, H, T = ctx.size, args.experts, args.hidden, args.tokens
+    G = P * E
+    k = min(args.topk, G)
+    rows = T * k
+    cap = P * rows
+    rb = H * 2
+    # A plain expert_out is staged through the pool, and so is combine_dev's plain output: room for
+    # a holder that receives every row.
+    cc = gcu.CudaContext(ctx, dev, stage_bytes=(cap + 1024) * rb)
+    moe = MoEDispatcher(ctx, cc)
+    g = torch.Generator(device="cuda").manual_seed(777 + ctx.rank)
+    x = torch.randn(T, H, device="cuda", generator=g).to(torch.bfloat16)
+    w, idx = torch.topk(torch.softmax(torch.randn(T, G, device="cuda", generator=g), -1), k, dim=-1)
+    tokens, splits, pos = moe.route(x, idx, E)
+    eo = {"symmetric": cc.empty((cap, H), torch.bfloat16)}
+    _, osp, ooff = moe.dispatch_dev(tokens, splits, eo["symmetric"], experts=E)  # identity experts
+    eo["plain"] = eo["symmetric"].clone()
+    backs = {"symmetric": cc.empty((rows, H), torch.bfloat16),
+             "plain": torch.empty((rows, H), dtype=torch.bfloat16, device="cuda")}
+    outs = {kind: [torch.empty((T, H), dtype=torch.bfloat16, device="cuda") for _ in range(2)] for kind in eo}
+
+    def composed(kind):
+        back = backs[kind]
+        moe.combine_dev(eo[kind], osp, ooff, back, experts=E)
+        acc = torch.zeros((T, H), device="cuda")
+        for j in range(k):  # the kernel's order: acc + w * x, one rounding each
+            acc = acc + w[:, j, None] * back.index_select(0, pos[:, j]).float()
+        outs[kind][0].copy_(acc)
+
+    def topk(kind):
+        moe.combine_dev_topk(eo[kind], splits, pos, w, outs[kind][1], experts=E)
+
+    def timed(fn):
+        fn()
+        cc.synchronize()
+        times = []
+        for _ in range(args.iters):
+            cc.pc.host_barrier()
+            t0 = time.perf_counter()
+            fn()
+            cc.synchronize()
+            times.append((time.perf_counter() - t0) * 1e3)
+        return statistics.median(times)
+
+    res = {}
+    for kind in eo:
+        composed(kind)
+        topk(kind)
+        cc.synchronize()
+        assert torch.equal(outs[kind][0].view(torch.int16), outs[kind][1].view(torch.int16)), kind
+        res[f"composed_{kind}"] = timed(lambda: composed(kind))
+        res[f"topk_{kind}"] = timed(lambda: topk(kind))
+        cc.pc.host_barrier()
+    res["bytes"] = (rows + T) * rb
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--ranks", type=int, default=2, help="threads sharing the GPU when only one is visible")
@@ -228,6 +301,19 @@ def main():
     for arm, nbytes in (("bf16", r["bytes_bf16"]), ("composed", r["bytes_fp8"]), ("fused", r["bytes_fp8"])):
         print(f"{arm:>10} {r[arm]:9.3f} {nbytes / 1e6:9.1f}", flush=True)
     print(json.dumps({"table": "fp8_dispatch", "ranks": P, "shared_gpu": shared, **r}), flush=True)
+
+    note = "; ranks share one GPU: local-HBM savings, not NVLink" if shared else ""
+    print(f"# top-k combine, bf16 ({label}{note}); median of {args.iters} calls (rank 0), outputs checked equal",
+          flush=True)
+    if shared:
+        r = gb.spawn_threads(P, run_rank_topk, args, True, cuda_device=0, timeout_ms=300000)[0]
+    else:
+        r = gb.spawn_threads(P, run_rank_topk, args, False, timeout_ms=300000)[0]
+    print(f"{'expert_out':>10} {'composed ms':>12} {'topk ms':>9} {'speed-up':>9} {'MB/rank':>9}")
+    for kind in ("symmetric", "plain"):
+        c, t = r[f"composed_{kind}"], r[f"topk_{kind}"]
+        print(f"{kind:>10} {c:12.3f} {t:9.3f} {c / t:9.2f} {r['bytes'] / 1e6:9.1f}", flush=True)
+    print(json.dumps({"table": "topk_combine", "ranks": P, "shared_gpu": shared, **r}), flush=True)
 
 
 if __name__ == "__main__":

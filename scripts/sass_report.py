@@ -40,6 +40,9 @@ KERNELS = [
     ("alltoall_push", r"alltoallPushKernel"),
     ("alltoallv_dev", r"alltoallvDevKernel<false>"),
     ("alltoallv_dev_fp8", r"alltoallvDevKernel<true>"),
+    ("combine_topk_bf16", r"moeCombineTopkKernel<__nv_bfloat16>"),
+    ("combine_topk_f16", r"moeCombineTopkKernel<__half>"),
+    ("combine_topk_f32", r"moeCombineTopkKernel<float>"),
     ("p2p_sendrecv", r"p2pKernel"),
     ("exchange_zero_copy", r"exchangeKernel<false>"),
     ("exchange_zero_copy_tma", r"exchangeKernel<true>"),
