@@ -550,11 +550,13 @@ nvlsAllreduceKernel(CommArgs a, char* mcBase, PeerPtrs bufs, size_t count, float
     const size_t tailStart = nvec * PT::kElems;
     size_t tb, te;
     shareOf(count - tailStart, P, a.rank, tb, te);
+    using TA = TailAcc<T>;
     for (size_t i = tailStart + tb + tid; i < tailStart + te; i += nthreads) {
-      T acc = static_cast<const T*>(bufs.p[0])[i];
-      for (int r = 1; r < P; r++) acc = PT::combineOne(acc, static_cast<const T*>(bufs.p[r])[i], DevOp::SUM);
-      if (scale != 1.0f) acc = PT::scaleOne(acc, scale);
-      for (int r = 0; r < P; r++) static_cast<T*>(bufs.p[r])[i] = acc;
+      typename TA::type acc = TA::load(static_cast<const T*>(bufs.p[0])[i]);
+      for (int r = 1; r < P; r++) acc = TA::combine(acc, TA::load(static_cast<const T*>(bufs.p[r])[i]), DevOp::SUM);
+      if (scale != 1.0f) acc = TA::scale(acc, scale);
+      const T res = TA::store(acc);
+      for (int r = 0; r < P; r++) static_cast<T*>(bufs.p[r])[i] = res;
     }
   }
   if (blockBarrier(a, e + 2) && extra.n > 0) fanOutLocalShares<T>(mine, extra, nvec, count, P, tid, nthreads);
@@ -610,11 +612,13 @@ hybridAllreduceKernel(CommArgs a, char* mcBase, PeerPtrs bufs, size_t count, flo
     const size_t tailStart = nvec * PT::kElems;
     size_t tb, te;
     shareOf(count - tailStart, P, a.rank, tb, te);
+    using TA = TailAcc<T>;
     for (size_t i = tailStart + tb + tid; i < tailStart + te; i += nthreads) {
-      T acc = static_cast<const T*>(bufs.p[0])[i];
-      for (int r = 1; r < P; r++) acc = PT::combineOne(acc, static_cast<const T*>(bufs.p[r])[i], DevOp::SUM);
-      if (scale != 1.0f) acc = PT::scaleOne(acc, scale);
-      for (int r = 0; r < P; r++) static_cast<T*>(bufs.p[r])[i] = acc;
+      typename TA::type acc = TA::load(static_cast<const T*>(bufs.p[0])[i]);
+      for (int r = 1; r < P; r++) acc = TA::combine(acc, TA::load(static_cast<const T*>(bufs.p[r])[i]), DevOp::SUM);
+      if (scale != 1.0f) acc = TA::scale(acc, scale);
+      const T res = TA::store(acc);
+      for (int r = 0; r < P; r++) static_cast<T*>(bufs.p[r])[i] = res;
     }
   }
   blockBarrier(a, e + 2);

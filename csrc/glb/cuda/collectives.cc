@@ -302,12 +302,19 @@ void allreduce(PeerContext& pc, const PeerBuffer& buf, size_t byteOffset, size_t
   }
   const bool hasMc = buf.mc != nullptr && byteOffset % 16 == 0;
   const BufKind kind = hasMc ? BufKind::SYMMETRIC : BufKind::REGISTERED;
+  // The two-shot and NVLS kernels fold and fan out the extra pointers in 16-byte packs.
+  bool extraAligned = true;
+  for (int k = 0; k < ep.extra.n; k++) extraAligned = extraAligned && reinterpret_cast<uintptr_t>(ep.extra.p[k]) % 16 == 0;
   AllreducePlan plan;
   if (algo == AllreduceAlgo::AUTO) {
     plan = planAllreduce(pc, bytes, dt, op, kind);
     algo = plan.algo;
     if (algo == AllreduceAlgo::HYBRID && ep.extra.n > 0) {  // the hybrid kernel takes one pointer
       algo = AllreduceAlgo::NVLS;
+      plan.cfg = LaunchCfg();
+    }
+    if (algo == AllreduceAlgo::NVLS && !extraAligned) {
+      algo = AllreduceAlgo::TWO_SHOT;
       plan.cfg = LaunchCfg();
     }
   }
@@ -324,6 +331,7 @@ void allreduce(PeerContext& pc, const PeerBuffer& buf, size_t byteOffset, size_t
     case AllreduceAlgo::NVLS: {
       GLB_ENFORCE(hasMc, "NVLS allreduce needs a multicast-bound (symmetric) buffer");
       GLB_ENFORCE(nvlsSupports(dt, op), "NVLS supports sum over float32/float16/bfloat16 only");
+      GLB_ENFORCE(extraAligned, "NVLS allreduce needs 16-byte aligned extra pointers");
       LaunchCfg cfg = plan.cfg;
       if (cfg.unroll == 0) cfg.unroll = defaultUnroll(algo, pc.size);
       cfg.blocks = clampBlocks(pc, nvlsKernelFor(dt, cfg.unroll), cfg.blocks > 0 ? cfg.blocks : tuning().maxBlocks,
@@ -345,7 +353,7 @@ void allreduce(PeerContext& pc, const PeerBuffer& buf, size_t byteOffset, size_t
       break;
     }
     case AllreduceAlgo::TWO_SHOT: {
-      const bool vectorOk = buf.vectorOk && byteOffset % 16 == 0;
+      const bool vectorOk = buf.vectorOk && byteOffset % 16 == 0 && extraAligned;
       LaunchCfg cfg = plan.cfg;
       if (cfg.unroll == 0) cfg.unroll = defaultUnroll(algo, pc.size);
       cfg.blocks = clampBlocks(pc, twoShotKernelFor(dt, pc.size, cfg.unroll), cfg.blocks > 0 ? cfg.blocks : tuning().maxBlocks,

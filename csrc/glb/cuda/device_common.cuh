@@ -474,9 +474,8 @@ constexpr bool isFp8Type() {
   return std::is_same<T, __nv_fp8_e4m3>::value || std::is_same<T, __nv_fp8_e5m2>::value;
 }
 
-// Scalar tails (elements after the last whole pack). FP8 accumulates them in fp32 and rounds
-// once, like its packs; every other type keeps its element-typed accumulator (16-bit tails
-// round after each combine, as they always have).
+// Scalar tails (elements after the last whole pack). 16-bit and FP8 types accumulate them in
+// fp32, scale in fp32 and round once, like their packs; every other type accumulates in itself.
 template <typename T>
 struct TailAcc {
   using type = T;
@@ -486,7 +485,7 @@ struct TailAcc {
   __device__ static T scale(T a, float s) { return PackTraits<T>::scaleOne(a, s); }
 };
 template <typename T>
-struct Fp8TailAcc {
+struct Fp32TailAcc {
   using type = float;
   __device__ static float load(T x) { return Scalar<T>::toAcc(x); }
   __device__ static T store(float x) { return Scalar<T>::fromAcc(x); }
@@ -494,9 +493,13 @@ struct Fp8TailAcc {
   __device__ static float scale(float a, float s) { return a * s; }
 };
 template <>
-struct TailAcc<__nv_fp8_e4m3> : Fp8TailAcc<__nv_fp8_e4m3> {};
+struct TailAcc<__half> : Fp32TailAcc<__half> {};
 template <>
-struct TailAcc<__nv_fp8_e5m2> : Fp8TailAcc<__nv_fp8_e5m2> {};
+struct TailAcc<__nv_bfloat16> : Fp32TailAcc<__nv_bfloat16> {};
+template <>
+struct TailAcc<__nv_fp8_e4m3> : Fp32TailAcc<__nv_fp8_e4m3> {};
+template <>
+struct TailAcc<__nv_fp8_e5m2> : Fp32TailAcc<__nv_fp8_e5m2> {};
 // Element types that get the P-specialised (two-shot, pipelined, reduce-pull) instantiations.
 template <typename T>
 constexpr bool isHotType() {

@@ -10,8 +10,7 @@ pytestmark = pytest.mark.gpu
 
 cu = gb._C.cuda
 DT = {torch.float32: gb.DataType.FLOAT32, torch.float16: gb.DataType.FLOAT16, torch.bfloat16: gb.DataType.BFLOAT16}
-# (rtol, atol): one rounding of the fp32-accumulated result, and a few for the last elements,
-# which round after every combine
+# (rtol, atol): one rounding of the fp32-accumulated result
 TOL = {torch.float32: (1e-6, 1e-6), torch.float16: (1e-3, 5e-3), torch.bfloat16: (8e-3, 4e-2)}
 # Largest number of buffers whose pipeline stages fit in an H100's shared memory (reduce_kernels.cu:
 # 3 stages of 16 KB per buffer): one more buffer runs the LDG/STG kernel.
