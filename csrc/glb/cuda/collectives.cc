@@ -807,6 +807,9 @@ void alltoall(PeerContext& pc, const void* in, const PeerBuffer& out, size_t out
     return;
   }
   if (tryLLExchange(pc, in, dst, bytes, 1, stream)) return;
+  // The push kernel stores my chunk for rank j into rank j's output while rank j may still be
+  // reading its own chunk for me from that address: in place, that would be a race.
+  rejectOverlap(in, bytes * pc.size, dst, bytes * pc.size, "alltoall");
   std::vector<size_t> sizes(pc.size, bytes);
   alltoallCommon(pc, in, sizes, out.ptrsAt(outOffset), out.vectorOk && outOffset % 16 == 0, sizes, true, stream);
 }
@@ -840,6 +843,8 @@ void alltoallv(PeerContext& pc, const void* in, const std::vector<size_t>& sendB
     if (dst != in && sendBytes[0] > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(dst, in, sendBytes[0], cudaMemcpyDeviceToDevice, stream));
     return;
   }
+  // As for alltoall: the push kernel writes peers' outputs while they still read their inputs.
+  rejectOverlap(in, prefix(sendBytes).back(), static_cast<const char*>(out.local) + outOffset, roff.back(), "alltoallv");
   alltoallCommon(pc, in, sendBytes, out.ptrsAt(outOffset), out.vectorOk && outOffset % 16 == 0, recvBytes, false, stream);
 }
 

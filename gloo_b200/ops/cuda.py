@@ -116,7 +116,11 @@ class CudaContext:
 
     def lookup(self, tensor) -> Tuple[Optional[Any], int]:
         """(PeerBuffer, byte offset) if ``tensor`` lies inside a registered region."""
-        ptr = tensor.data_ptr()
+        # torch reports data_ptr() 0 for an empty tensor; its place inside the storage still
+        # decides the path, which must match the peers' (e.g. a rank that receives nothing in an
+        # alltoallv into a registered buffer).
+        ptr = tensor.data_ptr() if tensor.numel() else \
+            tensor.untyped_storage().data_ptr() + tensor.storage_offset() * tensor.element_size()
         nbytes = tensor.numel() * tensor.element_size()
         dead = []
         found = (None, 0)
@@ -281,12 +285,16 @@ class CudaContext:
         return output
 
     def gather(self, output, input, root: int = 0, stream=None):
-        """Every rank's ``input`` into the root's ``output``, in rank order; any size. Other ranks
-        may pass ``output=None``; their output is never written."""
+        """Every rank's ``input`` into the root's ``output``, in rank order; any size. A non-root's
+        output is never written. Each rank picks the path from its own ``output``, so the ranks
+        must agree: when the root's output is registered / symmetric, every rank passes its copy
+        of that registered tensor at the same offset; when it is plain, other ranks pass None or a
+        plain tensor. Mixing the two gives a wrong result or leaves the ranks waiting."""
         return self.gatherv(output, input, [input.numel()] * self.size, root, stream)
 
     def gatherv(self, output, input, counts: Sequence[int], root: int = 0, stream=None):
-        """Like :meth:`gather` with ``counts[r]`` elements from rank r; any size."""
+        """Like :meth:`gather` with ``counts[r]`` elements from rank r; any size. The same rule on
+        registered and None outputs applies."""
         es = input.element_size()
         sizes = [int(c) * es for c in counts]
         optr = output.data_ptr() if output is not None else 0
@@ -299,7 +307,9 @@ class CudaContext:
 
     def alltoall(self, output, input, stream=None):
         """Fixed-size exchange: chunk j of ``input`` goes to rank j (one size for all ranks). Any size;
-        a plain ``input`` and ``output`` must not overlap (ValueError beyond the staged path)."""
+        a plain ``input`` and ``output`` must not overlap (ValueError beyond the staged path), nor
+        may ``input`` overlap a registered / symmetric ``output`` above the LL limit (ValueError:
+        the push kernel writes a peer's output while that peer still reads its input there)."""
         per = input.numel() // self.size * input.element_size()
         buf, off = self.lookup(output)
         if buf is not None:
@@ -314,7 +324,8 @@ class CudaContext:
         ``input`` and ``output`` must not overlap, at any size (``gloo_b200._C.InputError``, a
         ValueError): the plain alltoallv always runs the pipelined kernel, which writes the output
         while it still reads the input. Earlier versions staged a call that fit the pool, so a small
-        in-place call used to work; it now raises."""
+        in-place call used to work; it now raises. The same holds for a registered / symmetric
+        ``output``: its push kernel writes peers' outputs while they still read their inputs."""
         es = input.element_size()
         send = [int(c) * es for c in in_counts]
         recv = [int(c) * es for c in out_counts]
@@ -553,7 +564,10 @@ class CudaContext:
 
     def reduce(self, output, input, root: int = 0, op: ReduceOp = ReduceOp.SUM, stream=None):
         """``output`` on ``root`` := the reduction of every rank's ``input``. Any size; a non-root's
-        ``output`` is never written and may be None."""
+        ``output`` is never written. Each rank takes the registered path when its own ``input``
+        and ``output`` are both registered / symmetric, so the ranks must agree: when the root's
+        are, every rank passes registered input and output tensors at the root's offsets; a
+        non-root's ``output`` may be None only when the root's input or output is plain."""
         ptr, n, dt, _ = describe(input)
         ibuf, ioff = self.lookup(input)
         obuf, ooff = (self.lookup(output) if output is not None else (None, 0))
