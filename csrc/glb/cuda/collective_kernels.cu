@@ -593,6 +593,30 @@ __device__ __forceinline__ uint32_t a2aDirection(int inverse) {
 // each step a correctly rounded fp32 operation (no contraction, no approximate division). The
 // multiplier is a rounded reciprocal times 448, not a rounded 448 / amax: that is what torch
 // evaluates for `448.0 / amax` (a scalar over a tensor), so torch code reproduces every byte.
+// One block in a half-warp: `v` is this lane's 8 bf16 elements; returns its 8 codes and sets
+// `amax` (the scale is amax / 448). Every lane of the warp must call it: the amax shuffles run
+// with a full mask and stay within each half.
+__device__ __forceinline__ uint2 quantBlock(const uint4& v, float& amax) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+  float f[8];
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+    f[2 * i] = __uint_as_float(w[i] << 16);
+    f[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u);
+  }
+  amax = 0.0f;
+#pragma unroll
+  for (int i = 0; i < 8; i++) amax = fmaxf(amax, fabsf(f[i]));
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  amax = fmaxf(amax, kQuantMinAmax);
+  const float s = __fmul_rn(__frcp_rn(amax), kE4m3Max);
+  uint32_t c[4];
+#pragma unroll
+  for (int i = 0; i < 4; i++) c[i] = float2ToFp8x2<__nv_fp8_e4m3>(__fmul_rn(f[2 * i], s), __fmul_rn(f[2 * i + 1], s));
+  return make_uint2(c[0] | (c[1] << 16), c[2] | (c[3] << 16));
+}
+
 __device__ __forceinline__ void quantCopy(char* codes, float* scales, const char* in, unsigned long long nblk,
                                           size_t tid, size_t nthreads) {
   const int lane = static_cast<int>(tid & 31), half = lane >> 4, hl = lane & 15;
@@ -608,26 +632,47 @@ __device__ __forceinline__ void quantCopy(char* codes, float* scales, const char
 #pragma unroll
     for (int u = 0; u < kQuantUnroll; u++) {
       const unsigned long long blk = base + 2 * u + half;
-      const uint32_t w[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
-      float f[8];
-#pragma unroll
-      for (int i = 0; i < 4; i++) {
-        f[2 * i] = __uint_as_float(w[i] << 16);
-        f[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u);
-      }
-      float amax = 0.0f;
-#pragma unroll
-      for (int i = 0; i < 8; i++) amax = fmaxf(amax, fabsf(f[i]));
-#pragma unroll
-      for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
-      amax = fmaxf(amax, kQuantMinAmax);
-      const float s = __fmul_rn(__frcp_rn(amax), kE4m3Max);
-      uint32_t c[4];
-#pragma unroll
-      for (int i = 0; i < 4; i++) c[i] = float2ToFp8x2<__nv_fp8_e4m3>(__fmul_rn(f[2 * i], s), __fmul_rn(f[2 * i + 1], s));
+      float amax;
+      const uint2 c = quantBlock(v[u], amax);
       if (blk < nblk) {
-        *reinterpret_cast<uint2*>(codes + blk * kFp8Block + hl * 8) = make_uint2(c[0] | (c[1] << 16), c[2] | (c[3] << 16));
+        *reinterpret_cast<uint2*>(codes + blk * kFp8Block + hl * 8) = c;
         if (hl == 0) scales[blk] = __fdiv_rn(amax, kE4m3Max);
+      }
+    }
+  }
+}
+
+// Forward form, after a2aForwardLayout: my receive segment t = e·P + s starts at row sRcv[t] and
+// holds sRcvCnt[t] rows.
+__device__ __forceinline__ void a2aRecvSegments(const SignalPad* pad, int P, int E, int K, int me,
+                                                const unsigned long long* sAux, unsigned long long* sRcv,
+                                                uint32_t* sRcvCnt) {
+  const int t = threadIdx.x;
+  if (t < K) {
+    const int e = t / P, s = t % P;
+    unsigned long long off = sAux[me * E + e];
+    for (int s2 = 0; s2 < s; s2++) off += ldPad(&pad->a2aCount[me * E + e][s2]);
+    sRcv[t] = off;
+    sRcvCnt[t] = ldPad(&pad->a2aCount[me * E + e][s]);
+  }
+}
+
+// Forward form, plain output, once every CTA of every peer has pushed: my receive segments from my
+// staging area to `out`, segment by segment, so that alignment gaps of `out` stay untouched. The
+// quantising form's scales follow my capRows rows of codes in the staging area.
+template <bool kQuant>
+__device__ __forceinline__ void a2aCopyOutSegments(char* out, float* outScales, const char* stage,
+                                                   const unsigned long long* sRcv, const uint32_t* sRcvCnt, int K,
+                                                   unsigned long long rb, const unsigned long long& capRows /* in shared memory */, size_t tid,
+                                                   size_t nthreads) {
+  for (int k = 0; k < K; k++) {
+    const unsigned long long n = sRcvCnt[k];
+    if (n > 0) gridCopy(out + sRcv[k] * rb, stage + sRcv[k] * rb, n * rb, true, tid, nthreads);
+    if constexpr (kQuant) {
+      const unsigned long long sb = rb / kFp8Block * sizeof(float);  // scale bytes per row
+      if (n > 0) {
+        gridCopy(reinterpret_cast<char*>(outScales) + sRcv[k] * sb, stage + capRows * rb + sRcv[k] * sb, n * sb, true,
+                 tid, nthreads);
       }
     }
   }
@@ -683,15 +728,8 @@ alltoallvDevKernel(CommArgs a, PeerPtrs outs, A2aDevKernelArgs<kQuant> d) {
   if (ok1 && !invalid) {
     if (!d.inverse) {
       a2aForwardLayout(pad, P, E, K, me, d.align, sDst, sAux, sNeed);
-      if (t < K) {
-        sDst[t] += sAux[t];
-        // My receive segment (e, s), t = e·P + s.
-        const int e = t / P, s = t % P;
-        unsigned long long off = sAux[me * E + e];
-        for (int s2 = 0; s2 < s; s2++) off += ldPad(&pad->a2aCount[me * E + e][s2]);
-        sRcv[t] = off;
-        sRcvCnt[t] = ldPad(&pad->a2aCount[me * E + e][s]);
-      }
+      if (t < K) sDst[t] += sAux[t];
+      a2aRecvSegments(pad, P, E, K, me, sAux, sRcv, sRcvCnt);
     } else {
       // R[j][s] = rows holder j returns to rank s.
       for (int i = t; i < P * P; i += blockDim.x) {
@@ -797,19 +835,9 @@ alltoallvDevKernel(CommArgs a, PeerPtrs outs, A2aDevKernelArgs<kQuant> d) {
       if (d.inverse) {
         gridCopy(d.stagedOut, stage, sNeed[me] * rb, true, tid, nthreads);
       } else {
-        // Segment by segment: alignment gaps of `out` stay untouched.
-        for (int k = 0; k < K; k++) {
-          const unsigned long long n = sRcvCnt[k];
-          if (n > 0) gridCopy(d.stagedOut + sRcv[k] * rb, stage + sRcv[k] * rb, n * rb, true, tid, nthreads);
-          if constexpr (kQuant) {
-            // The scales follow my capRows rows of codes in my staging area.
-            const unsigned long long sb = rb / kFp8Block * sizeof(float);  // scale bytes per row
-            if (n > 0) {
-              gridCopy(reinterpret_cast<char*>(d.stagedScales) + sRcv[k] * sb, stage + sCap[me] * rb + sRcv[k] * sb,
-                       n * sb, true, tid, nthreads);
-            }
-          }
-        }
+        float* stagedScales = nullptr;
+        if constexpr (kQuant) stagedScales = d.stagedScales;
+        a2aCopyOutSegments<kQuant>(d.stagedOut, stagedScales, stage, sRcv, sRcvCnt, K, rb, sCap[me], tid, nthreads);
       }
     }
   }
@@ -1051,6 +1079,272 @@ void launchMoeCombineTopk(const CommArgs& a, const PeerPtrs& srcs, const void* s
   topkCombineFn(dt)<<<blocks, kThreads, 0, stream>>>(a, srcs, d);
 }
 
+// ---- top-k MoE dispatch: route each token from its gate indices and push its row to every choice ----
+// The forward dispatch of route(x, topk_idx) without its T·k-row copy: each token's row is read
+// once (and quantised once) and stored to each of its k destination rows. The layout, splits and
+// pos are those of route() + the forward alltoallvDevKernel, byte for byte.
+//   route (before barrier 1, local): group g = topk_idx entry, in 0..P·E-1 (anything else is not
+//     routed). CTA b owns a contiguous slice of tokens. It counts every choice of every token
+//     (the totals, which every CTA needs for pos) and those before its slice (its base), then ranks
+//     its slice's choices in (token, choice) order: within a warp by __match_any_sync, across the
+//     warps of a round in warp order through shared running counts. No atomic decides a place.
+//     pos = (rows of groups before g) + (choices of g before this one); CTA 0 writes splits.
+//   publish / barrier 1 / layout: the dispatch's helpers; header word 3 carries bit 4 (this form),
+//     bit 1 (quantising) and bit 3 (staged output), so ranks that mix forms read it as invalid.
+//   push: one warp per token of my slice; a lane per choice finds its destination row
+//     sDst[g] + (pos - sSrc[g]) on rank g / E, then the warp reads each 16-byte pack (or, quantising,
+//     each 128-element block) once and stores it to every destination that does not overflow.
+//   barrier 2, staged copy-out and retire as in the dispatch.
+struct MoeDispatchTopkArgs {
+  const char* x;              // (tokens, rowBytes); quantising: bf16 (tokens, rowBytes) elements
+  const long long* idx;       // (tokens, topk) group per choice
+  long long* splits;          // (P·E) out: routed choices per group
+  long long* pos;             // (tokens, topk) out: row of route()'s rows, -1 = not routed
+  long long* outSplits;
+  long long* outOffsets;
+  char* stagedOut;            // plain output: copied from my staging after barrier 2; null = zero copy
+  unsigned long long tokens;
+  unsigned long long rowBytes;  // of an output row (quantising: H codes)
+  uint32_t capRows;
+  int topk;
+  int experts;
+  int align;
+  InputStatus* status;  // host-mapped
+};
+template <bool kQuant>
+struct MoeDispatchTopkKernelArgs : MoeDispatchTopkArgs {};
+template <>
+struct MoeDispatchTopkKernelArgs<true> : MoeDispatchTopkArgs {
+  PeerPtrs scales;      // zero copy: every rank's out_scales
+  float* stagedScales;  // plain output: copied from my staging after barrier 2; null = zero copy
+};
+
+constexpr uint32_t kA2aTopkDispatchDir = 16u;  // header word 3, bit 4: the top-k dispatch
+constexpr int kTopkPushUnroll = 4;             // packs of a row in flight per lane
+static_assert(kThreads >= kMaxRanks * kMaxA2aExperts, "one scan slot per group");
+
+__device__ __forceinline__ int topkGroup(long long v, int K) { return v >= 0 && v < K ? static_cast<int>(v) : K; }
+
+template <bool kQuant>
+__global__ void __launch_bounds__(kThreads)
+moeDispatchTopkKernel(CommArgs a, PeerPtrs outs, MoeDispatchTopkKernelArgs<kQuant> d) {
+  constexpr int kMaxK = kMaxRanks * kMaxA2aExperts;
+  __shared__ unsigned long long sSrc[kMaxK];  // group g: first row of route()'s rows
+  __shared__ unsigned long long sDst[kMaxK];  //          first row on rank g / E
+  __shared__ unsigned long long sAux[kMaxK];  // my splits (published), then column sums / expert bases
+  __shared__ unsigned long long sRcv[kMaxK];  // first row of my receive segment e·P+s
+  __shared__ uint32_t sRcvCnt[kMaxK];         // and its rows
+  __shared__ uint32_t sTot[kMaxK];            // group g: routed choices of all my tokens
+  __shared__ uint32_t sRun[kMaxK];            //          of the tokens before my slice, then running
+  __shared__ unsigned long long sNeed[kMaxRanks], sCap[kMaxRanks];
+  __shared__ unsigned long long sWarp[32];
+  const uint32_t ep = loadEpoch(a);
+  const int P = a.nranks, E = d.experts, K = P * E, me = a.rank, t = threadIdx.x;
+  const int lane = t & 31, warp = t >> 5, nw = blockDim.x >> 5;
+  const unsigned long long rb = d.rowBytes, k = static_cast<unsigned long long>(d.topk);
+  const uint32_t dir = kA2aTopkDispatchDir | (kQuant ? 2u : 0u) | (d.stagedOut != nullptr ? kA2aTopkStaged : 0u);
+
+  // ---- route: counts, then pos of my slice ----
+  const unsigned long long n = d.tokens * k;
+  const unsigned long long per = (d.tokens + gridDim.x - 1) / gridDim.x;
+  const unsigned long long tok0 = min(d.tokens, blockIdx.x * per), tok1 = min(d.tokens, tok0 + per);
+  const unsigned long long lo = tok0 * k, hi = tok1 * k;
+  for (int g = t; g < K; g += blockDim.x) sTot[g] = sRun[g] = 0u;
+  __syncthreads();
+  for (unsigned long long b = static_cast<unsigned long long>(warp) * 32; b < n; b += blockDim.x) {
+    const unsigned long long i = b + lane;
+    const int g = i < n ? topkGroup(d.idx[i], K) : K;
+    const bool before = i < lo;
+    const unsigned m = __match_any_sync(0xffffffffu, 2 * g + (before ? 1 : 0));
+    if (g < K && lane == __ffs(m) - 1) {
+      atomicAdd(&sTot[g], static_cast<uint32_t>(__popc(m)));
+      if (before) atomicAdd(&sRun[g], static_cast<uint32_t>(__popc(m)));
+    }
+  }
+  __syncthreads();
+  unsigned long long routed;
+  const unsigned long long first = blockExclusiveScan(t < K ? sTot[t] : 0u, sWarp, routed);
+  if (t < K) {
+    sSrc[t] = first;
+    sAux[t] = sTot[t];
+    if (blockIdx.x == 0) d.splits[t] = sTot[t];
+  }
+  __syncthreads();
+  for (unsigned long long b = lo; b < hi; b += blockDim.x) {
+    const unsigned long long i = b + t;
+    const int g = i < hi ? topkGroup(d.idx[i], K) : K;
+    const unsigned m = __match_any_sync(0xffffffffu, g);
+    const unsigned below = m & ((1u << lane) - 1u);
+    long long p = -1;
+    for (int w = 0; w < nw; w++) {
+      if (warp == w && g < K) {
+        const uint32_t r = sRun[g];
+        __syncwarp(m);
+        if (below == 0u) sRun[g] = r + static_cast<uint32_t>(__popc(m));
+        p = static_cast<long long>(sSrc[g] + r + static_cast<uint32_t>(__popc(below)));
+      }
+      __syncthreads();
+    }
+    if (i < hi) d.pos[i] = p;
+  }
+
+  // ---- publish: header + my splits; the layout ----
+  a2aPublish(a, reinterpret_cast<const long long*>(sAux), K, rb, E, d.align, dir, d.capRows, false);
+  const bool ok1 = localGridSync(a) && blockBarrier(a, ep + 1);
+  const SignalPad* pad = a.self;
+  bool invalid = false;
+  if (ok1) invalid = a2aHeadersBad(pad, P, K, rb, E, d.align, dir, sCap);
+  if (ok1 && !invalid) {
+    a2aForwardLayout(pad, P, E, K, me, d.align, sDst, sAux, sNeed);
+    if (t < K) sDst[t] += sAux[t];
+    a2aRecvSegments(pad, P, E, K, me, sAux, sRcv, sRcvCnt);
+    __syncthreads();
+  }
+  if (ok1 && blockIdx.x == 0) {
+    if (t == 0) a2aReport(d.status, invalid, P, sNeed, sCap);
+    if (!invalid && t < K) {
+      d.outSplits[t] = sRcvCnt[t];
+      d.outOffsets[t] = static_cast<long long>(sRcv[t]);
+    }
+  }
+
+  // ---- push: one warp per token of my slice ----
+  if (ok1 && !invalid) {
+    for (unsigned long long tok = tok0 + warp; tok < tok1; tok += nw) {
+      // Lane c < k: where choice c's row goes; null when it is not routed or its rank overflows.
+      char* dst = nullptr;
+      float* dsc = nullptr;
+      if (static_cast<unsigned long long>(lane) < k) {
+        const unsigned long long i = tok * k + lane;
+        const int g = topkGroup(d.idx[i], K);
+        if (g < K && sNeed[g / E] <= sCap[g / E]) {
+          const int j = g / E;
+          const unsigned long long row = sDst[g] + (static_cast<unsigned long long>(d.pos[i]) - sSrc[g]);
+          dst = static_cast<char*>(outs.p[j]) + row * rb;
+          if constexpr (kQuant) {
+            float* sc = d.stagedScales != nullptr ? reinterpret_cast<float*>(static_cast<char*>(outs.p[j]) + sCap[j] * rb)
+                                                  : static_cast<float*>(d.scales.p[j]);
+            dsc = sc + row * (rb / kFp8Block);
+          }
+        }
+      }
+      if constexpr (kQuant) {
+        // Half-warps take 128-element blocks, as quantCopy: one amax and one set of codes per block.
+        const int half = lane >> 4, hl = lane & 15;
+        const unsigned long long nblk = rb / kFp8Block;
+        const char* src = d.x + tok * rb * 2;
+        for (unsigned long long b0 = 0; b0 < nblk; b0 += 2 * kQuantUnroll) {
+          uint4 v[kQuantUnroll];
+#pragma unroll
+          for (int u = 0; u < kQuantUnroll; u++) {
+            const unsigned long long blk = b0 + 2 * u + half;
+            v[u] = blk < nblk ? *reinterpret_cast<const uint4*>(src + blk * (2 * kFp8Block) + hl * 16)
+                              : make_uint4(0u, 0u, 0u, 0u);
+          }
+          uint2 c[kQuantUnroll];
+          float amax[kQuantUnroll];
+#pragma unroll
+          for (int u = 0; u < kQuantUnroll; u++) c[u] = quantBlock(v[u], amax[u]);
+          for (int ch = 0; ch < d.topk; ch++) {
+            char* q = reinterpret_cast<char*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(dst), ch));
+            float* qs = reinterpret_cast<float*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(dsc), ch));
+            if (q == nullptr) continue;
+#pragma unroll
+            for (int u = 0; u < kQuantUnroll; u++) {
+              const unsigned long long blk = b0 + 2 * u + half;
+              if (blk < nblk) {
+                *reinterpret_cast<uint2*>(q + blk * kFp8Block + hl * 8) = c[u];
+                if (hl == 0) qs[blk] = __fdiv_rn(amax[u], kE4m3Max);
+              }
+            }
+          }
+        }
+      } else {
+        const unsigned long long npk = rb / 16;
+        const char* src = d.x + tok * rb;
+        // Warp-uniform trip count: every lane takes part in the shuffles, lanes past the row end idle.
+        for (unsigned long long v0 = lane; v0 - lane < npk; v0 += 32 * kTopkPushUnroll) {
+          Pack16 x[kTopkPushUnroll];
+#pragma unroll
+          for (int u = 0; u < kTopkPushUnroll; u++) {
+            const unsigned long long pk = v0 + 32ull * u;
+            if (pk < npk) x[u] = ld128_stream(src + pk * 16);
+          }
+          for (int ch = 0; ch < d.topk; ch++) {
+            char* q = reinterpret_cast<char*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(dst), ch));
+            if (q == nullptr) continue;
+#pragma unroll
+            for (int u = 0; u < kTopkPushUnroll; u++) {
+              const unsigned long long pk = v0 + 32ull * u;
+              if (pk < npk) st128_stream(q + pk * 16, x[u]);
+            }
+          }
+        }
+      }
+    }
+  }
+  blockBarrier(a, ep + 2);
+  // NO pad table reads from here on (see alltoallvDevKernel).
+
+  // ---- plain output: my staging -> out, once every CTA of every peer has pushed ----
+  if (d.stagedOut != nullptr) {
+    const bool synced = localGridSync(a);
+    if (synced && ok1 && !invalid && sNeed[me] <= sCap[me] && ld_relaxed_sys(&a.self->abort) == 0u) {
+      const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + t;
+      const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
+      float* stagedScales = nullptr;
+      if constexpr (kQuant) stagedScales = d.stagedScales;
+      a2aCopyOutSegments<kQuant>(d.stagedOut, stagedScales, static_cast<const char*>(outs.p[me]), sRcv, sRcvCnt, K,
+                                 rb, sCap[me], tid, nthreads);
+    }
+  }
+  retire(a, 2, 0);
+}
+
+namespace {
+void fillDispatchTopk(MoeDispatchTopkArgs& d, const void* x, size_t tokens, int topk, const long long* idx,
+                      long long* splits, long long* pos, long long* outSplits, long long* outOffsets, void* stagedOut,
+                      size_t rowBytes, uint32_t capRows, int experts, int align, InputStatus* status) {
+  d.x = static_cast<const char*>(x);
+  d.idx = idx;
+  d.splits = splits;
+  d.pos = pos;
+  d.outSplits = outSplits;
+  d.outOffsets = outOffsets;
+  d.stagedOut = static_cast<char*>(stagedOut);
+  d.tokens = tokens;
+  d.rowBytes = rowBytes;
+  d.capRows = capRows;
+  d.topk = topk;
+  d.experts = experts;
+  d.align = align;
+  d.status = status;
+}
+}  // namespace
+
+void launchMoeDispatchTopk(const CommArgs& a, const PeerPtrs& outs, const void* x, size_t tokens, int topk,
+                           const long long* idx, long long* splits, long long* pos, long long* outSplits,
+                           long long* outOffsets, void* stagedOut, size_t rowBytes, uint32_t capRows, int experts,
+                           int align, InputStatus* status, int blocks, cudaStream_t stream) {
+  MoeDispatchTopkKernelArgs<false> d;
+  fillDispatchTopk(d, x, tokens, topk, idx, splits, pos, outSplits, outOffsets, stagedOut, rowBytes, capRows, experts,
+                   align, status);
+  moeDispatchTopkKernel<false><<<blocks, kThreads, 0, stream>>>(a, outs, d);
+}
+
+void launchMoeDispatchTopkFp8(const CommArgs& a, const PeerPtrs& outs, const PeerPtrs& scales, const void* x,
+                              size_t tokens, int topk, const long long* idx, long long* splits, long long* pos,
+                              long long* outSplits, long long* outOffsets, void* stagedOut, float* stagedScales,
+                              size_t hidden, uint32_t capRows, int experts, int align, InputStatus* status, int blocks,
+                              cudaStream_t stream) {
+  MoeDispatchTopkKernelArgs<true> d;
+  fillDispatchTopk(d, x, tokens, topk, idx, splits, pos, outSplits, outOffsets, stagedOut, hidden, capRows, experts,
+                   align, status);
+  d.scales = scales;
+  d.stagedScales = stagedScales;
+  moeDispatchTopkKernel<true><<<blocks, kThreads, 0, stream>>>(a, outs, d);
+}
+
 // ---- reduce_scatter / reduce: pull my slice from every peer's input, reduce, store -----------
 // Inputs are peer-mapped. Rank r reduces elements [elemOff[r], elemOff[r]+elemLen[r])
 // and writes them to `out` (local pointer; for reduce() it is the root's peer-mapped
@@ -1212,6 +1506,10 @@ const void* alltoallvDevKernelPtr(bool fp8) {
              : reinterpret_cast<const void*>(alltoallvDevKernel<false>);
 }
 const void* moeCombineTopkKernelPtr(DataType dt) { return reinterpret_cast<const void*>(topkCombineFn(dt)); }
+const void* moeDispatchTopkKernelPtr(bool fp8) {
+  return fp8 ? reinterpret_cast<const void*>(moeDispatchTopkKernel<true>)
+             : reinterpret_cast<const void*>(moeDispatchTopkKernel<false>);
+}
 const void* reducePullKernelPtr(DataType dt, int nranks) {
   const void* k = nullptr;
   dispatchType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(reducePullFn<decltype(tag)>(nranks)); });
@@ -1225,6 +1523,8 @@ void preloadCollectiveKernels() {
   touchKernel(alltoallvDevKernel<false>);
   touchKernel(alltoallvDevKernel<true>);
   for (DataType dt : {DataType::FLOAT32, DataType::BFLOAT16, DataType::FLOAT16}) touchKernel(topkCombineFn(dt));
+  touchKernel(moeDispatchTopkKernel<false>);
+  touchKernel(moeDispatchTopkKernel<true>);
   touchKernel(llExchangeKernel);
   for (DataType dt : kAllDataTypes) {
     dispatchType(dt, [&](auto tag) {

@@ -963,6 +963,105 @@ void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidd
 }
 
 namespace {
+// `outs` are the ranks' out (zero copy) or staging areas, `stagedOut` my plain out. `scales`
+// non-null: the quantising form (rowBytes = hidden, bf16 x), `stagedScales` with `stagedOut`.
+void dispatchTopkCommon(PeerContext& pc, const void* x, size_t tokens, size_t rowBytes, int topk,
+                        const int64_t* topkIdx, int64_t* splits, int64_t* pos, const PeerPtrs& outs, const void* out,
+                        void* stagedOut, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets, int experts,
+                        int align, cudaStream_t stream, const PeerPtrs* scales = nullptr,
+                        float* stagedScales = nullptr) {
+  GLB_TRACE_RANGE("glb::cuda::alltoallv_dev_topk");
+  const char* name = "alltoallv_dev_topk";
+  GLB_ENFORCE(topk >= 1 && topk <= 32, name, ": topk must be in 1..32, got ", topk);
+  GLB_ENFORCE(experts >= 1 && experts <= kMaxA2aExperts, name, ": experts per rank must be in 1..", kMaxA2aExperts,
+              ", got ", experts);
+  GLB_ENFORCE(align >= 1, name, ": align must be at least 1, got ", align);
+  GLB_ENFORCE(rowBytes > 0 && rowBytes % 16 == 0 && rowBytes <= 0xffffffffull, name,
+              ": the row size must be a positive multiple of 16 bytes, got ", rowBytes);
+  GLB_ENFORCE(tokens * static_cast<size_t>(topk) <= 0x7fffffffull, name, ": tokens x topk must be below 2^31, got ",
+              tokens, " x ", topk);
+  GLB_ENFORCE(splits != nullptr && outSplits != nullptr && outOffsets != nullptr &&
+                  (tokens == 0 || (x != nullptr && topkIdx != nullptr && pos != nullptr)),
+              name, ": missing x, topk_idx, splits, pos, out_splits or out_offsets");
+  GLB_ENFORCE(reinterpret_cast<uintptr_t>(x) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0, name,
+              ": x and out must be 16-byte aligned");
+  const bool fp8 = scales != nullptr;
+  // Peers write my out while I still read my x.
+  rejectOverlap(x, tokens * rowBytes * (fp8 ? 2 : 1), out, capacityRows * rowBytes, name);
+  const uint32_t cap = static_cast<uint32_t>(std::min<size_t>(capacityRows, 0xfffffffeull));
+  const int blocks =
+      std::max(1, std::min({tuning().alltoallvBlocks, pc.coResidentBlocks(moeDispatchTopkKernelPtr(fp8)), kMaxBlocks}));
+  auto* idx = reinterpret_cast<const long long*>(topkIdx);
+  auto* sp = reinterpret_cast<long long*>(splits);
+  auto* ps = reinterpret_cast<long long*>(pos);
+  auto* os = reinterpret_cast<long long*>(outSplits);
+  auto* oo = reinterpret_cast<long long*>(outOffsets);
+  prologue(pc, stream);
+  if (fp8) {
+    launchMoeDispatchTopkFp8(pc.comm(), outs, *scales, x, tokens, topk, idx, sp, ps, os, oo, stagedOut, stagedScales,
+                             rowBytes, cap, experts, align, pc.inputStatusDevice(), blocks, stream);
+  } else {
+    launchMoeDispatchTopk(pc.comm(), outs, x, tokens, topk, idx, sp, ps, os, oo, stagedOut, rowBytes, cap, experts,
+                          align, pc.inputStatusDevice(), blocks, stream);
+  }
+  finish(pc, stream, name);
+}
+}  // namespace
+
+void alltoallvDevTopk(PeerContext& pc, const void* x, size_t tokens, size_t rowBytes, int topk, const int64_t* topkIdx,
+                      int64_t* splits, int64_t* pos, const PeerBuffer& out, size_t outOffset, size_t capacityRows,
+                      int64_t* outSplits, int64_t* outOffsets, int experts, int align, cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  GLB_ENFORCE_LE(outOffset + capacityRows * rowBytes, out.bytes, "alltoallv_dev_topk output exceeds the registered buffer");
+  dispatchTopkCommon(pc, x, tokens, rowBytes, topk, topkIdx, splits, pos, out.ptrsAt(outOffset),
+                     static_cast<const char*>(out.local) + outOffset, nullptr, capacityRows, outSplits, outOffsets,
+                     experts, align, stream);
+}
+
+void alltoallvDevTopk(PeerContext& pc, const void* x, size_t tokens, size_t rowBytes, int topk, const int64_t* topkIdx,
+                      int64_t* splits, int64_t* pos, void* out, size_t capacityRows, int64_t* outSplits,
+                      int64_t* outOffsets, int experts, int align, cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  GLB_ENFORCE(rowBytes > 0, "alltoallv_dev_topk: row size must be positive");
+  // Peers push into my staging area; I copy my rows out of it inside the same kernel.
+  const auto l = layoutOf(pc);
+  dispatchTopkCommon(pc, x, tokens, rowBytes, topk, topkIdx, splits, pos, pc.stagePtrs(l.bulkOff), out, out,
+                     std::min(capacityRows, l.bulkBytes / rowBytes), outSplits, outOffsets, experts, align, stream);
+}
+
+void alltoallvDevTopkFp8(PeerContext& pc, const void* x, size_t tokens, size_t hidden, int topk,
+                         const int64_t* topkIdx, int64_t* splits, int64_t* pos, const PeerBuffer& out, size_t outOffset,
+                         const PeerBuffer& outScales, size_t scalesOffset, size_t capacityRows, int64_t* outSplits,
+                         int64_t* outOffsets, int experts, int align, cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  checkFp8Dispatch(x, static_cast<const char*>(out.local) + outOffset, hidden);
+  GLB_ENFORCE_LE(outOffset + capacityRows * hidden, out.bytes, "alltoallv_dev_topk output exceeds the registered buffer");
+  GLB_ENFORCE_LE(scalesOffset + capacityRows * (hidden / kFp8Block) * sizeof(float), outScales.bytes,
+                 "alltoallv_dev_topk output scales exceed the registered buffer");
+  GLB_ENFORCE(scalesOffset % sizeof(float) == 0, "alltoallv_dev_topk: output scales must be 4-byte aligned");
+  const PeerPtrs scales = outScales.ptrsAt(scalesOffset);
+  dispatchTopkCommon(pc, x, tokens, hidden, topk, topkIdx, splits, pos, out.ptrsAt(outOffset),
+                     static_cast<const char*>(out.local) + outOffset, nullptr, capacityRows, outSplits, outOffsets,
+                     experts, align, stream, &scales, nullptr);
+}
+
+void alltoallvDevTopkFp8(PeerContext& pc, const void* x, size_t tokens, size_t hidden, int topk,
+                         const int64_t* topkIdx, int64_t* splits, int64_t* pos, void* out, float* outScales,
+                         size_t capacityRows, int64_t* outSplits, int64_t* outOffsets, int experts, int align,
+                         cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  checkFp8Dispatch(x, out, hidden);
+  GLB_ENFORCE(reinterpret_cast<uintptr_t>(outScales) % sizeof(float) == 0,
+              "alltoallv_dev_topk: output scales must be 4-byte aligned");
+  // The staging layout of alltoallvDevFp8: codes, then the scales after the capacity's codes.
+  const auto l = layoutOf(pc);
+  const PeerPtrs none{};
+  dispatchTopkCommon(pc, x, tokens, hidden, topk, topkIdx, splits, pos, pc.stagePtrs(l.bulkOff), out, out,
+                     std::min(capacityRows, l.bulkBytes / (hidden + hidden / kFp8Block * sizeof(float))), outSplits,
+                     outOffsets, experts, align, stream, &none, outScales);
+}
+
+namespace {
 // `srcs` are the ranks' expert_out (zero copy) or staging areas, `stagedIn` my plain expert_out.
 void combineTopkCommon(PeerContext& pc, void* out, size_t tokens, int topk, const int64_t* pos, const float* weights,
                        const int64_t* splits, const void* expertOut, const PeerPtrs& srcs, const void* stagedIn,

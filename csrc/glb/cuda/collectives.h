@@ -171,6 +171,31 @@ void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidd
 void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidden, const int64_t* inSplits,
                      void* out, float* outScales, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets,
                      int experts, int align, cudaStream_t stream);
+// Top-k MoE dispatch: route() + the forward alltoallvDev in one kernel. `x` holds `tokens` rows
+// of `rowBytes` (a multiple of 16; x and out 16-byte aligned, disjoint); `topkIdx` is int64
+// (tokens, topk), 1 <= topk <= 32, tokens x topk < 2^31: entry j·E + e chooses local expert e
+// of rank j, anything outside 0..P·E-1 is not routed. Writes `splits` (P·E: routed choices per
+// (rank, expert)) and `pos` ((tokens, topk): the row of route()'s rows that carries each choice,
+// -1 if not routed), from this rank's input alone, even when the call fails. out, outSplits and
+// outOffsets then equal those of alltoallvDev(route()'s rows, splits) byte for byte: within a
+// (rank, expert) group rows go by token, then by choice. Each token is read once and stored to
+// each of its choices. Capacity, paths and error reporting are those of alltoallvDev.
+void alltoallvDevTopk(PeerContext& pc, const void* x, size_t tokens, size_t rowBytes, int topk, const int64_t* topkIdx,
+                      int64_t* splits, int64_t* pos, const PeerBuffer& out, size_t outOffset, size_t capacityRows,
+                      int64_t* outSplits, int64_t* outOffsets, int experts, int align, cudaStream_t stream);
+void alltoallvDevTopk(PeerContext& pc, const void* x, size_t tokens, size_t rowBytes, int topk, const int64_t* topkIdx,
+                      int64_t* splits, int64_t* pos, void* out, size_t capacityRows, int64_t* outSplits,
+                      int64_t* outOffsets, int experts, int align, cudaStream_t stream);
+// Its quantising form, with alltoallvDevFp8's input, outputs, numerics and checks: each token is
+// quantised once and the same codes and scales are stored to all its choices.
+void alltoallvDevTopkFp8(PeerContext& pc, const void* x, size_t tokens, size_t hidden, int topk,
+                         const int64_t* topkIdx, int64_t* splits, int64_t* pos, const PeerBuffer& out, size_t outOffset,
+                         const PeerBuffer& outScales, size_t scalesOffset, size_t capacityRows, int64_t* outSplits,
+                         int64_t* outOffsets, int experts, int align, cudaStream_t stream);
+void alltoallvDevTopkFp8(PeerContext& pc, const void* x, size_t tokens, size_t hidden, int topk,
+                         const int64_t* topkIdx, int64_t* splits, int64_t* pos, void* out, float* outScales,
+                         size_t capacityRows, int64_t* outSplits, int64_t* outOffsets, int experts, int align,
+                         cudaStream_t stream);
 // Top-k MoE combine: the inverse of the forward alltoallvDev fused with the gate-weighted sum.
 // `splits` is the in_splits this rank passed to the dispatch; `expertOut` holds, on every rank, the
 // experts' output rows (`rowBytes` each, dtype dt: float, bfloat16 or float16) in that dispatch's

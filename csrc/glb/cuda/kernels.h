@@ -123,9 +123,27 @@ void launchMoeCombineTopk(const CommArgs& a, const PeerPtrs& srcs, const void* s
                           int topk, const long long* pos, const float* weights, const long long* splits, size_t rowBytes,
                           DataType dt, uint32_t capRows, int experts, int align, InputStatus* status, int blocks,
                           cudaStream_t stream);
+// Top-k MoE dispatch: route x's `tokens` rows by `idx` ((tokens, topk) int64; entry j·E + e =
+// local expert e of rank j, anything outside 0..P·E-1 is not routed) and push each to every
+// choice. Writes `splits` (P·E) and `pos` (tokens, topk) as route() does; out, outSplits and
+// outOffsets are those of the forward launchAlltoallvDev on route()'s rows. Rows are `rowBytes`
+// (a multiple of 16), x 16-byte aligned. `outs` / `stagedOut` as there.
+void launchMoeDispatchTopk(const CommArgs& a, const PeerPtrs& outs, const void* x, size_t tokens, int topk,
+                           const long long* idx, long long* splits, long long* pos, long long* outSplits,
+                           long long* outOffsets, void* stagedOut, size_t rowBytes, uint32_t capRows, int experts,
+                           int align, InputStatus* status, int blocks, cudaStream_t stream);
+// Its quantising form: x holds bf16 rows of `hidden` elements (a multiple of 128), each token is
+// quantised once and its codes and scales stored to every choice; `scales` / `stagedScales` as
+// in launchAlltoallvDevFp8.
+void launchMoeDispatchTopkFp8(const CommArgs& a, const PeerPtrs& outs, const PeerPtrs& scales, const void* x,
+                              size_t tokens, int topk, const long long* idx, long long* splits, long long* pos,
+                              long long* outSplits, long long* outOffsets, void* stagedOut, float* stagedScales,
+                              size_t hidden, uint32_t capRows, int experts, int align, InputStatus* status, int blocks,
+                              cudaStream_t stream);
 // Entry points, for occupancy queries (every CTA of a collective kernel must be resident).
 const void* alltoallvDevKernelPtr(bool fp8 = false);
 const void* moeCombineTopkKernelPtr(DataType dt);
+const void* moeDispatchTopkKernelPtr(bool fp8);
 const void* broadcastKernelPtr();
 const void* gatherPushKernelPtr();
 const void* alltoallPushKernelPtr();

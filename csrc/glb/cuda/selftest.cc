@@ -442,6 +442,121 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
         }
         return "";
       });
+      // The top-k dispatch, both forms, zero copy. Every virtual rank holds rank 0's splits, so rank
+      // 0's rows for expert e of rank j start at base(j, e) (as above) and go by token, then choice.
+      // The host routes the indices itself (entries -1 and >= P·E are not routed, some tokens pick an
+      // expert twice) and checks splits, pos, out_splits / out_offsets and every pushed row.
+      for (const bool fp8 : {false, true}) {
+        const char* what = fp8 ? "moeDispatchTopkKernel<fp8> (E=2, align=4, k=3, H=256) P="
+                               : "moeDispatchTopkKernel (E=3, align=8, k=4, 32-byte rows) P=";
+        R.run(strcat_all(what, P), [&, fp8]() -> std::string {
+          const int E = fp8 ? 2 : 3, A = fp8 ? 4 : 8, K = P * E, topk = fp8 ? 3 : 4, H = fp8 ? 256 : 8, nb = H / kFp8Block;
+          const size_t T = 45, rb = fp8 ? H : H * 4, cap = 512;
+          std::vector<int64_t> idx(T * topk), sp(K, 0), pos(T * topk, -1), pre(K + 1, 0);
+          for (size_t i = 0; i < T * topk; i++) idx[i] = static_cast<int64_t>((i * 7 + i / topk * 3) % (K + 2)) - 1;
+          for (size_t i = 0; i < T * topk; i++) if (idx[i] >= 0 && idx[i] < K) sp[idx[i]]++;
+          for (int g = 0; g < K; g++) pre[g + 1] = pre[g] + sp[g];
+          std::vector<int64_t> seen(K, 0);
+          for (size_t i = 0; i < T * topk; i++) if (idx[i] >= 0 && idx[i] < K) pos[i] = pre[idx[i]] + seen[idx[i]]++;
+          auto base = [&](int j, int e) {
+            int64_t b = 0;
+            for (int x = 0; x < e; x++) b = (b + P * sp[j * E + x] + A - 1) / A * A;
+            return b;
+          };
+          // fp8: small integers and one +-448 per block (scale 1, codes exact); else row t = 8t .. 8t + 7.
+          auto value = [&](int64_t r, int i) -> float {
+            if (!fp8) return static_cast<float>(r * H + i);
+            const int b = i / kFp8Block, at = i % kFp8Block;
+            if (at == (r * 3 + b * 5) % kFp8Block) return (r + b) % 2 ? -448.0f : 448.0f;
+            return static_cast<float>((r * 7 + i * 3) % 33 - 16);
+          };
+          DevBuf x(T * H * 4), idxDev(idx.size() * 8), splits(K * 8), posDev(pos.size() * 8), outSplits(K * 8),
+              outOffsets(K * 8);
+          if (fp8) {
+            std::vector<uint16_t> rows(T * H);
+            for (size_t r = 0; r < T; r++) {
+              for (int i = 0; i < H; i++) {
+                const float f = value(r, i);
+                uint32_t w;
+                std::memcpy(&w, &f, 4);
+                rows[r * H + i] = static_cast<uint16_t>(w >> 16);  // exact
+              }
+            }
+            GLB_CUDA_CHECK(cudaMemcpyAsync(x.p, rows.data(), rows.size() * 2, cudaMemcpyHostToDevice, stream));
+          } else {
+            launchFill(x.p, T * H, DataType::FLOAT32, 0.0, 1.0, stream);
+          }
+          GLB_CUDA_CHECK(cudaMemcpyAsync(idxDev.p, idx.data(), idx.size() * 8, cudaMemcpyHostToDevice, stream));
+          std::vector<std::unique_ptr<DevBuf>> scaleBufs;
+          PeerPtrs sc;
+          std::memset(&sc, 0, sizeof(sc));
+          for (int r = 0; r < P; r++) {
+            scaleBufs.emplace_back(new DevBuf(cap * 4 * 4));
+            sc.p[r] = scaleBufs[r]->p;
+            GLB_CUDA_CHECK(cudaMemsetAsync(sc.p[r], 0xff, cap * 4 * 4, stream));
+            GLB_CUDA_CHECK(cudaMemsetAsync(pp.p[r], 0xff, cap * rb, stream));
+          }
+          const int blocks = std::min(pc.coResidentBlocks(moeDispatchTopkKernelPtr(fp8)), 16);
+          auto ll = [](DevBuf& b) { return static_cast<long long*>(b.p); };
+          if (fp8) {
+            launchMoeDispatchTopkFp8(ca, pp, sc, x.p, T, topk, ll(idxDev), ll(splits), ll(posDev), ll(outSplits),
+                                     ll(outOffsets), nullptr, nullptr, H, static_cast<uint32_t>(cap), E, A,
+                                     pc.inputStatusDevice(), blocks, stream);
+          } else {
+            launchMoeDispatchTopk(ca, pp, x.p, T, topk, ll(idxDev), ll(splits), ll(posDev), ll(outSplits),
+                                  ll(outOffsets), nullptr, rb, static_cast<uint32_t>(cap), E, A, pc.inputStatusDevice(),
+                                  blocks, stream);
+          }
+          noteLaunch();
+          std::vector<int64_t> gs(K), gp(T * topk), os(K), oo(K);
+          GLB_CUDA_CHECK(cudaMemcpyAsync(gs.data(), splits.p, K * 8, cudaMemcpyDeviceToHost, stream));
+          GLB_CUDA_CHECK(cudaMemcpyAsync(gp.data(), posDev.p, gp.size() * 8, cudaMemcpyDeviceToHost, stream));
+          GLB_CUDA_CHECK(cudaMemcpyAsync(os.data(), outSplits.p, K * 8, cudaMemcpyDeviceToHost, stream));
+          GLB_CUDA_CHECK(cudaMemcpyAsync(oo.data(), outOffsets.p, K * 8, cudaMemcpyDeviceToHost, stream));
+          GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+          if (gs != sp) return "splits differ from the host routing";
+          if (gp != pos) return "pos differs from the host routing";
+          for (int e = 0; e < E; e++) {
+            for (int s = 0; s < P; s++) {
+              if (os[e * P + s] != sp[e] || oo[e * P + s] != base(0, e) + s * sp[e]) {
+                return strcat_all("out_splits/out_offsets[", e * P + s, "] = ", os[e * P + s], "/", oo[e * P + s]);
+              }
+            }
+          }
+          for (int j = 0; j < P; j++) {
+            std::vector<uint8_t> out(cap * rb);
+            std::vector<float> scales(cap * 4);
+            GLB_CUDA_CHECK(cudaMemcpyAsync(out.data(), pp.p[j], out.size(), cudaMemcpyDeviceToHost, stream));
+            GLB_CUDA_CHECK(cudaMemcpyAsync(scales.data(), sc.p[j], scales.size() * 4, cudaMemcpyDeviceToHost, stream));
+            GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+            for (size_t i = 0; i < T * topk; i++) {
+              if (pos[i] < 0 || idx[i] / E != j) continue;
+              const int g = static_cast<int>(idx[i]);
+              const int64_t row = base(j, g % E) + (pos[i] - pre[g]), tok = static_cast<int64_t>(i / topk);
+              for (int c = 0; c < H; c++) {
+                bool ok;
+                if (fp8) {
+                  ok = out[row * rb + c] == float8_e4m3::fromFloat(value(tok, c));
+                } else {
+                  float f;
+                  std::memcpy(&f, &out[row * rb + c * 4], 4);
+                  ok = f == value(tok, c);
+                }
+                if (!ok) return strcat_all("dst ", j, " row ", row, " (token ", tok, ") element ", c, " differs");
+              }
+              for (int b = 0; fp8 && b < nb; b++) {
+                if (scales[row * nb + b] != 1.0f) return strcat_all("dst ", j, " row ", row, " scale ", b, " differs");
+              }
+            }
+            // Virtual rank 1's rows follow rank 0's in each segment and are never written.
+            for (int e = 0; e < E; e++) {
+              const int64_t end = base(j, e) + sp[j * E + e];
+              if (sp[j * E + e] > 0 && out[end * rb] != 0xff) return strcat_all("dst ", j, ": wrote past rank 0's rows");
+            }
+          }
+          return "";
+        });
+      }
       // The top-k combine, zero copy, with the closed-form layout of the dispatch case above: rank 0's
       // chunk k = j·E + e lies on virtual holder j from row base(j, e) on. Holder j's expert_out
       // (pp.p[j]) holds bf16 halves of small integers; the host sums in the kernel's fp32 order.

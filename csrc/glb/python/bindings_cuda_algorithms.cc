@@ -222,6 +222,41 @@ void registerCudaAlgorithms(py::module_& m) {
      py::arg("buf_offset"), py::arg("out"), py::arg("scales_buf"), py::arg("scales_offset"), py::arg("out_scales"),
      py::arg("capacity_rows"), py::arg("out_splits"), py::arg("out_offsets"), py::arg("experts"), py::arg("align"),
      py::arg("stream"));
+  // Top-k MoE dispatch. `buf` (and `scales_buf`, quantising) are the registered outputs (None:
+  // `out` / `out_scales` are plain device pointers, staged); `hidden` > 0 selects the quantising
+  // form (bf16 x of `hidden` elements a row), else rows are `row_bytes`.
+  m.def("alltoallv_dev_topk", [](PeerContext& pc, uintptr_t x, size_t tokens, size_t rowBytes, int topk,
+                                 uintptr_t topkIdx, uintptr_t splits, uintptr_t pos, py::object buf, size_t off,
+                                 uintptr_t out, size_t capacityRows, uintptr_t outSplits, uintptr_t outOffsets,
+                                 int experts, int align, size_t hidden, py::object scalesBuf, size_t scalesOff,
+                                 uintptr_t outScales, uintptr_t st) {
+    GLB_ENFORCE(buf.is_none() == scalesBuf.is_none() || hidden == 0,
+                "alltoallv_dev_topk: out and out_scales must both be registered or both be plain");
+    const PeerBuffer* reg = buf.is_none() ? nullptr : buf.cast<const PeerBuffer*>();
+    const PeerBuffer* sreg = scalesBuf.is_none() ? nullptr : scalesBuf.cast<const PeerBuffer*>();
+    auto* idx = reinterpret_cast<const int64_t*>(topkIdx);
+    auto* sp = reinterpret_cast<int64_t*>(splits);
+    auto* ps = reinterpret_cast<int64_t*>(pos);
+    auto* os = reinterpret_cast<int64_t*>(outSplits);
+    auto* oo = reinterpret_cast<int64_t*>(outOffsets);
+    py::gil_scoped_release nogil;
+    if (hidden > 0 && reg != nullptr) {
+      alltoallvDevTopkFp8(pc, P(x), tokens, hidden, topk, idx, sp, ps, *reg, off, *sreg, scalesOff, capacityRows, os,
+                          oo, experts, align, S(st));
+    } else if (hidden > 0) {
+      alltoallvDevTopkFp8(pc, P(x), tokens, hidden, topk, idx, sp, ps, P(out), reinterpret_cast<float*>(outScales),
+                          capacityRows, os, oo, experts, align, S(st));
+    } else if (reg != nullptr) {
+      alltoallvDevTopk(pc, P(x), tokens, rowBytes, topk, idx, sp, ps, *reg, off, capacityRows, os, oo, experts, align,
+                       S(st));
+    } else {
+      alltoallvDevTopk(pc, P(x), tokens, rowBytes, topk, idx, sp, ps, P(out), capacityRows, os, oo, experts, align,
+                       S(st));
+    }
+  }, py::arg("pc"), py::arg("x"), py::arg("tokens"), py::arg("row_bytes"), py::arg("topk"), py::arg("topk_idx"),
+     py::arg("splits"), py::arg("pos"), py::arg("buf"), py::arg("buf_offset"), py::arg("out"),
+     py::arg("capacity_rows"), py::arg("out_splits"), py::arg("out_offsets"), py::arg("experts"), py::arg("align"),
+     py::arg("hidden"), py::arg("scales_buf"), py::arg("scales_offset"), py::arg("out_scales"), py::arg("stream"));
   // Top-k MoE combine. `buf` is the registered expert_out (None: `expert_out` is a plain device
   // pointer, staged); pos / weights / splits are addresses of device arrays.
   m.def("alltoallv_dev_combine_topk", [](PeerContext& pc, uintptr_t out, size_t tokens, int topk, uintptr_t pos,

@@ -533,6 +533,107 @@ class CudaContext:
                                        _stream(stream))
         return out
 
+    def alltoallv_dev_topk(self, out, x, topk_idx, splits, pos, out_splits, out_offsets, experts: int = 1,
+                           align: int = 1, out_scales=None, stream=None):
+        """Top-k MoE dispatch: route every token from its gate indices and push its row to each chosen
+        expert, in one kernel with no host synchronisation (graph-capturable).
+
+        ``x`` is a contiguous ``(T, *row)`` CUDA tensor, rows a multiple of 16 bytes, 16-byte
+        aligned. ``topk_idx`` is int64 ``(T, k)``, 1 <= k <= 32: entry ``j * experts + e`` chooses
+        local expert ``e`` of rank ``j``; any entry outside ``0 .. size * experts - 1`` (such as -1)
+        is not routed. ``splits`` (int64 ``(size * experts,)``) and ``pos`` (int64 ``(T, k)``) are
+        written on this rank, from its own input alone and even when the call fails.
+
+        The result is byte for byte that of ``rows, splits, pos = MoEDispatcher.route(x, topk_idx,
+        experts)`` followed by :meth:`alltoallv_dev` ``(out, rows, splits, out_splits, out_offsets,
+        experts, align)``: ``splits``, ``pos``, ``out_splits``, ``out_offsets`` and every row of
+        ``out`` inside a segment. Within a (rank, expert) group rows go by token, then by choice; a
+        token that picks an expert twice sends two rows. Alignment gaps and rows past the last
+        segment are not written. No row is read more than once: each token's row goes from ``x`` to
+        all its destinations, so nothing of size ``T * k`` is written locally.
+        ``combine_dev_topk`` / :meth:`alltoallv_dev_combine_topk` take the returned ``splits`` and
+        ``pos`` unchanged.
+
+        ``out``, ``out_splits``, ``out_offsets``, the capacity (``out.shape[0]``), the zero-copy
+        (registered / symmetric) and staged (plain) paths and the errors found on the device are those
+        of :meth:`alltoallv_dev`; every rank must call this form, with the same row size, ``experts``,
+        ``align`` and kind of ``out``, or the call is invalid on every rank. An ``out`` too small on
+        one rank leaves it empty, serves the others and raises on every rank at the next host call.
+
+        Quantising form: ``out_scales`` given, ``x`` bfloat16 ``(T, H)`` with H a multiple of 128,
+        ``out`` float8_e4m3fn ``(cap, H)``, ``out_scales`` float32 ``(cap, H // 128)``, both registered
+        / symmetric or both plain. Each token is quantised once, with :meth:`alltoallv_dev`'s numerics,
+        and the same codes and scales are stored to all its destinations.
+
+        Wrong dtypes (int32 ``topk_idx`` included), shapes, non-contiguous or misaligned tensors,
+        k outside 1..32, ``T * k`` above 2^31 - 1 and an ``out`` that overlaps ``x`` raise
+        ``ValueError`` before launch. Limits: ``size <= 16``, ``1 <= experts <= 32``; T = 0 is allowed."""
+        import torch
+
+        name = "alltoallv_dev_topk"
+        G = self.size * int(experts)
+        if not 1 <= int(experts) <= 32 or int(align) < 1:
+            raise ValueError(f"{name}: experts must be in 1..32 and align at least 1, got {experts} and {align}")
+        named = (("x", x), ("out", out), ("topk_idx", topk_idx), ("pos", pos))
+        for what, t in named:
+            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
+                raise ValueError(f"{name}: {what} must be a CUDA tensor on cuda:{self.device}")
+        if topk_idx.dtype != torch.int64 or topk_idx.dim() != 2 or x.dim() < 1 or topk_idx.shape[0] != x.shape[0]:
+            raise ValueError(f"{name}: topk_idx must be int64 (T, k) with T = x.shape[0], got {topk_idx.dtype} "
+                             f"{tuple(topk_idx.shape)} for x {tuple(x.shape)}")
+        T, k = int(topk_idx.shape[0]), int(topk_idx.shape[1])
+        if not 1 <= k <= 32:
+            raise ValueError(f"{name}: k = {k} choices per token; 1..32 are supported")
+        if T * k > 2**31 - 1:
+            raise ValueError(f"{name}: T * k = {T * k} choices; at most 2^31 - 1 are supported")
+        if pos.dtype != torch.int64 or tuple(pos.shape) != (T, k):
+            raise ValueError(f"{name}: pos must be int64 {(T, k)}, got {pos.dtype} {tuple(pos.shape)}")
+        for what, t in named:
+            if not t.is_contiguous():
+                raise ValueError(f"{name}: {what} must be contiguous")
+        si = self._dev_index(splits, "splits", G)
+        so = self._dev_index(out_splits, "out_splits", G)
+        oo = self._dev_index(out_offsets, "out_offsets", G)
+        hidden, sbuf, soff, sptr = 0, None, 0, 0
+        if out_scales is not None or self._is_fp8_dispatch(out, x):
+            form = ("the quantising alltoallv_dev_topk takes bfloat16 x (T, H) with H a multiple of 128, "
+                    "float8_e4m3fn out (cap, H) and float32 out_scales (cap, H // 128)")
+            if out_scales is None:
+                raise ValueError(f"{name}: out_scales missing; {form}")
+            if x.dtype != torch.bfloat16 or out.dtype != torch.float8_e4m3fn:
+                raise ValueError(f"{name}: got {x.dtype} x and {out.dtype} out; {form}")
+            if (not isinstance(out_scales, torch.Tensor) or out_scales.dtype != torch.float32 or not out_scales.is_cuda
+                    or out_scales.device.index != self.device or not out_scales.is_contiguous()):
+                raise ValueError(f"{name}: out_scales must be a contiguous float32 tensor on cuda:{self.device}; {form}")
+            if x.dim() != 2 or out.dim() != 2 or out_scales.dim() != 2:
+                raise ValueError(f"{name}: x, out and out_scales must be 2-D; {form}")
+            hidden = int(x.shape[1])
+            if hidden == 0 or hidden % 128 != 0:
+                raise ValueError(f"{name}: row length {hidden} is not a positive multiple of 128; {form}")
+            if int(out.shape[1]) != hidden or tuple(out_scales.shape) != (int(out.shape[0]), hidden // 128):
+                raise ValueError(f"{name}: out {tuple(out.shape)} and out_scales {tuple(out_scales.shape)} do not "
+                                 f"match rows of {hidden}; {form}")
+            rb = hidden
+            sbuf, soff = self.lookup(out_scales)
+            sptr = out_scales.data_ptr()
+        else:
+            rb = self._dev_rows(out, x)
+            if rb % 16 != 0:
+                raise ValueError(f"{name}: rows of {rb} bytes; a positive multiple of 16 is required")
+        if x.data_ptr() % 16 != 0 or out.data_ptr() % 16 != 0:
+            raise ValueError(f"{name}: x and out must be 16-byte aligned")
+        x0, x1 = x.data_ptr(), x.data_ptr() + x.numel() * x.element_size()
+        o0, o1 = out.data_ptr(), out.data_ptr() + out.numel() * out.element_size()
+        if x0 < o1 and o0 < x1:
+            raise ValueError(f"{name}: out and x overlap")
+        buf, off = self.lookup(out)
+        if hidden and (buf is None) != (sbuf is None):
+            raise ValueError(f"{name}: out and out_scales must both be registered / symmetric or both plain")
+        _cu.alltoallv_dev_topk(self.pc, x.data_ptr(), T, rb, k, topk_idx.data_ptr(), si, pos.data_ptr(), buf, off,
+                               out.data_ptr(), int(out.shape[0]), so, oo, int(experts), int(align), hidden, sbuf, soff,
+                               sptr, _stream(stream))
+        return out
+
     def scatter(self, output, input=None, root: int = 0, stream=None):
         """Block ``rank`` of the root's ``input`` -> ``output``. Any size; ``input`` is read on the
         root only (None elsewhere)."""

@@ -557,6 +557,27 @@ class MoEDispatcher(_Base):
         pos = torch.where(routed, pos, torch.full_like(pos, -1)).view(T, k)
         return x.index_select(0, order // k), counts[:G], pos
 
+    def dispatch_dev_topk(self, x, topk_idx, out, experts: int = 1, align: int = 1, out_scales=None):
+        """route() + dispatch_dev() (or dispatch_dev_fp8() when ``out_scales`` is given) in one kernel:
+        ``x (T, H)`` and ``topk_idx (T, k)`` in, each token's row read once and stored to each of its
+        k destinations, with no host sync and no ``T * k`` copy of the rows. The results equal route()
+        followed by the dispatch byte for byte (see ``CudaContext.alltoallv_dev_topk``). Returns
+        ``(out, out_splits, out_offsets, splits, pos)``, with ``out_scales`` after ``out`` in the FP8
+        form; ``splits`` and ``pos`` are what combine_dev_topk() takes."""
+        import torch
+
+        G = self.size * int(experts)
+        dev = x.device
+        splits = torch.empty(G, dtype=torch.int64, device=dev)
+        out_splits = torch.empty_like(splits)
+        out_offsets = torch.empty_like(splits)
+        pos = torch.empty(tuple(topk_idx.shape), dtype=torch.int64, device=dev)
+        self.cc.alltoallv_dev_topk(out, x, topk_idx, splits, pos, out_splits, out_offsets, experts=experts, align=align,
+                                   out_scales=out_scales)
+        if out_scales is not None:
+            return out, out_scales, out_splits, out_offsets, splits, pos
+        return out, out_splits, out_offsets, splits, pos
+
     def combine_dev_topk(self, expert_out, splits, pos, weights, out, experts: int = 1, align: int = 1):
         """The inverse of dispatch_dev() fused with the gate-weighted sum: ``out[t]`` = sum over
         token t's routed choices j of ``weights[t, j]`` times its expert's output row, in fp32 in

@@ -25,7 +25,15 @@ experts' output symmetric (read in place) and plain (staged through each rank's 
 Both arms' outputs are checked equal byte for byte before timing. MB/rank counts the expert rows
 that reach this rank plus its (tokens, hidden) result, from the shapes.
 
-    python scripts/bench_moe_dispatch.py [--ranks 2] [--iters 20]
+A fourth table times the top-k dispatch, the start of a MoE layer (median per call, rank 0, the two
+arms alternating), with symmetric outputs:
+  dispatch  route() + dispatch_dev (bf16) or + dispatch_dev_fp8 (fp8), against dispatch_dev_topk
+  layer     route() + dispatch_dev + identity experts + combine_dev_topk, against
+            dispatch_dev_topk + identity experts + combine_dev_topk
+Both arms' outputs are checked equal byte for byte before timing. "MB avoided" is route()'s copy of
+the T x k rows, written once and read back by the dispatch, from the shapes.
+
+    python scripts/bench_moe_dispatch.py [--ranks 2] [--iters 20] [--tables pairs,fp8,combine,dispatch]
 """
 import argparse
 import json
@@ -265,6 +273,82 @@ def measure_topk(ctx, args, dev):
     return res
 
 
+def run_rank_dispatch_topk(ctx, args, shared):
+    if shared:
+        return measure_dispatch_topk(ctx, args, 0)
+    torch.cuda.set_device(ctx.rank)
+    with torch.cuda.stream(gcu.new_stream(ctx.rank)):
+        return measure_dispatch_topk(ctx, args, ctx.rank)
+
+
+def measure_dispatch_topk(ctx, args, dev):
+    P, E, H, T = ctx.size, args.experts, args.hidden, args.tokens
+    G = P * E
+    k = min(args.topk, G)
+    cap = P * T * k
+    cc = gcu.CudaContext(ctx, dev, stage_bytes=16 << 20)
+    moe = MoEDispatcher(ctx, cc)
+    g = torch.Generator(device="cuda").manual_seed(999 + ctx.rank)
+    x = torch.randn(T, H, device="cuda", generator=g).to(torch.bfloat16)
+    w, idx = torch.topk(torch.softmax(torch.randn(T, G, device="cuda", generator=g), -1), k, dim=-1)
+    outs = [cc.empty((cap, H), torch.bfloat16) for _ in range(2)]
+    codes = [cc.empty((cap, H), torch.float8_e4m3fn) for _ in range(2)]
+    scales = [cc.empty((cap, H // 128), torch.float32) for _ in range(2)]
+    ys = [torch.empty((T, H), dtype=torch.bfloat16, device="cuda") for _ in range(2)]
+    for t in outs + codes + scales:
+        t.view(torch.uint8).zero_()
+    got = {}
+
+    def composed_bf16(i=0):
+        rows, splits, pos = moe.route(x, idx, E)
+        moe.dispatch_dev(rows, splits, outs[i], experts=E)
+        return splits, pos
+
+    def fused_bf16(i=1):
+        return moe.dispatch_dev_topk(x, idx, outs[i], experts=E)[3:]
+
+    def composed_fp8():
+        rows, splits, _ = moe.route(x, idx, E)
+        moe.dispatch_dev_fp8(rows, splits, codes[0], scales[0], experts=E)
+
+    def fused_fp8():
+        moe.dispatch_dev_topk(x, idx, codes[1], experts=E, out_scales=scales[1])
+
+    def layer(dispatch, i):
+        def fn():
+            splits, pos = dispatch(i)
+            moe.combine_dev_topk(outs[i], splits, pos, w, ys[i], experts=E)  # identity experts
+        return fn
+
+    arms = {
+        "dispatch_bf16": (composed_bf16, fused_bf16, lambda: (outs[0], outs[1])),
+        "dispatch_fp8": (composed_fp8, fused_fp8, lambda: (torch.cat([codes[0].view(torch.uint8).view(-1),
+                                                                       scales[0].view(torch.uint8).view(-1)]),
+                                                            torch.cat([codes[1].view(torch.uint8).view(-1),
+                                                                       scales[1].view(torch.uint8).view(-1)]))),
+        "layer_bf16": (layer(composed_bf16, 0), layer(fused_bf16, 1), lambda: (ys[0], ys[1])),
+    }
+    for name, (a, b, results) in arms.items():
+        a()
+        b()
+        cc.synchronize()
+        u, v = results()
+        assert torch.equal(u.view(torch.uint8), v.view(torch.uint8)), name
+        ta, tb = [], []
+        for _ in range(args.iters):
+            for fn, times in ((a, ta), (b, tb)):
+                cc.pc.host_barrier()
+                t0 = time.perf_counter()
+                fn()
+                cc.synchronize()
+                times.append((time.perf_counter() - t0) * 1e3)
+        got[f"{name}_composed"] = statistics.median(ta)
+        got[f"{name}_topk"] = statistics.median(tb)
+        cc.pc.host_barrier()
+    got["bytes_avoided"] = 2 * T * k * H * 2
+    return got
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--ranks", type=int, default=2, help="threads sharing the GPU when only one is visible")
@@ -273,7 +357,9 @@ def main():
     ap.add_argument("--hidden", type=int, default=7168)
     ap.add_argument("--experts", type=int, default=8, help="local experts per rank")
     ap.add_argument("--iters", type=int, default=20)
+    ap.add_argument("--tables", default="pairs,fp8,combine,dispatch", help="comma-separated tables to run")
     args = ap.parse_args()
+    tables = set(args.tables.split(","))
     assert torch.cuda.is_available(), "needs a GPU"
     ngpu = torch.cuda.device_count()
     shared = ngpu == 1
@@ -282,8 +368,9 @@ def main():
     print(f"# card: {card()}", flush=True)
     print(f"# ranks: {label}; {args.tokens} tokens x top-{args.topk}, hidden {args.hidden}, "
           f"{args.experts} experts per rank; median of {args.iters} dispatch + combine pairs (rank 0)", flush=True)
-    print(f"{'dtype':>14} {'host ms':>9} {'dev ms':>9} {'graph ms':>9} {'host/dev':>9} {'MB/rank':>9}")
-    for dtype in (torch.bfloat16, torch.float8_e4m3fn):
+    if "pairs" in tables:
+        print(f"{'dtype':>14} {'host ms':>9} {'dev ms':>9} {'graph ms':>9} {'host/dev':>9} {'MB/rank':>9}")
+    for dtype in (torch.bfloat16, torch.float8_e4m3fn) if "pairs" in tables else ():
         if shared:
             r = gb.spawn_threads(P, run_rank, args, dtype, True, cuda_device=0, timeout_ms=300000)[0]
         else:
@@ -292,28 +379,43 @@ def main():
               f"{r['host'] / r['dev']:9.2f} {r['bytes_per_rank'] / 1e6:9.1f}", flush=True)
         print(json.dumps({"dtype": str(dtype), "ranks": P, "shared_gpu": shared, **r}), flush=True)
 
-    print(f"# FP8 dispatch of bf16 rows ({label}); median of {args.iters} dispatch calls (rank 0)", flush=True)
-    if shared:
-        r = gb.spawn_threads(P, run_rank_fp8, args, True, cuda_device=0, timeout_ms=300000)[0]
-    else:
-        r = gb.spawn_threads(P, run_rank_fp8, args, False, timeout_ms=300000)[0]
-    print(f"{'arm':>10} {'ms':>9} {'MB/rank':>9}")
-    for arm, nbytes in (("bf16", r["bytes_bf16"]), ("composed", r["bytes_fp8"]), ("fused", r["bytes_fp8"])):
-        print(f"{arm:>10} {r[arm]:9.3f} {nbytes / 1e6:9.1f}", flush=True)
-    print(json.dumps({"table": "fp8_dispatch", "ranks": P, "shared_gpu": shared, **r}), flush=True)
+    if "fp8" in tables:
+        print(f"# FP8 dispatch of bf16 rows ({label}); median of {args.iters} dispatch calls (rank 0)", flush=True)
+        if shared:
+            r = gb.spawn_threads(P, run_rank_fp8, args, True, cuda_device=0, timeout_ms=300000)[0]
+        else:
+            r = gb.spawn_threads(P, run_rank_fp8, args, False, timeout_ms=300000)[0]
+        print(f"{'arm':>10} {'ms':>9} {'MB/rank':>9}")
+        for arm, nbytes in (("bf16", r["bytes_bf16"]), ("composed", r["bytes_fp8"]), ("fused", r["bytes_fp8"])):
+            print(f"{arm:>10} {r[arm]:9.3f} {nbytes / 1e6:9.1f}", flush=True)
+        print(json.dumps({"table": "fp8_dispatch", "ranks": P, "shared_gpu": shared, **r}), flush=True)
 
     note = "; ranks share one GPU: local-HBM savings, not NVLink" if shared else ""
-    print(f"# top-k combine, bf16 ({label}{note}); median of {args.iters} calls (rank 0), outputs checked equal",
-          flush=True)
-    if shared:
-        r = gb.spawn_threads(P, run_rank_topk, args, True, cuda_device=0, timeout_ms=300000)[0]
-    else:
-        r = gb.spawn_threads(P, run_rank_topk, args, False, timeout_ms=300000)[0]
-    print(f"{'expert_out':>10} {'composed ms':>12} {'topk ms':>9} {'speed-up':>9} {'MB/rank':>9}")
-    for kind in ("symmetric", "plain"):
-        c, t = r[f"composed_{kind}"], r[f"topk_{kind}"]
-        print(f"{kind:>10} {c:12.3f} {t:9.3f} {c / t:9.2f} {r['bytes'] / 1e6:9.1f}", flush=True)
-    print(json.dumps({"table": "topk_combine", "ranks": P, "shared_gpu": shared, **r}), flush=True)
+    if "combine" in tables:
+        print(f"# top-k combine, bf16 ({label}{note}); median of {args.iters} calls (rank 0), outputs checked equal",
+              flush=True)
+        if shared:
+            r = gb.spawn_threads(P, run_rank_topk, args, True, cuda_device=0, timeout_ms=300000)[0]
+        else:
+            r = gb.spawn_threads(P, run_rank_topk, args, False, timeout_ms=300000)[0]
+        print(f"{'expert_out':>10} {'composed ms':>12} {'topk ms':>9} {'speed-up':>9} {'MB/rank':>9}")
+        for kind in ("symmetric", "plain"):
+            c, t = r[f"composed_{kind}"], r[f"topk_{kind}"]
+            print(f"{kind:>10} {c:12.3f} {t:9.3f} {c / t:9.2f} {r['bytes'] / 1e6:9.1f}", flush=True)
+        print(json.dumps({"table": "topk_combine", "ranks": P, "shared_gpu": shared, **r}), flush=True)
+
+    if "dispatch" in tables:
+        print(f"# top-k dispatch ({label}{note}); median of {args.iters} calls (rank 0), arms alternating, "
+              "outputs checked equal", flush=True)
+        if shared:
+            r = gb.spawn_threads(P, run_rank_dispatch_topk, args, True, cuda_device=0, timeout_ms=300000)[0]
+        else:
+            r = gb.spawn_threads(P, run_rank_dispatch_topk, args, False, timeout_ms=300000)[0]
+        print(f"{'arm':>14} {'composed ms':>12} {'topk ms':>9} {'speed-up':>9} {'MB avoided':>11}")
+        for arm in ("dispatch_bf16", "dispatch_fp8", "layer_bf16"):
+            c, t = r[f"{arm}_composed"], r[f"{arm}_topk"]
+            print(f"{arm:>14} {c:12.3f} {t:9.3f} {c / t:9.2f} {r['bytes_avoided'] / 1e6:11.1f}", flush=True)
+        print(json.dumps({"table": "topk_dispatch", "ranks": P, "shared_gpu": shared, **r}), flush=True)
 
 
 if __name__ == "__main__":

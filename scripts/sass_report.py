@@ -43,6 +43,8 @@ KERNELS = [
     ("combine_topk_bf16", r"moeCombineTopkKernel<__nv_bfloat16>"),
     ("combine_topk_f16", r"moeCombineTopkKernel<__half>"),
     ("combine_topk_f32", r"moeCombineTopkKernel<float>"),
+    ("dispatch_topk", r"moeDispatchTopkKernel<false>"),
+    ("dispatch_topk_fp8", r"moeDispatchTopkKernel<true>"),
     ("p2p_sendrecv", r"p2pKernel"),
     ("exchange_zero_copy", r"exchangeKernel<false>"),
     ("exchange_zero_copy_tma", r"exchangeKernel<true>"),
