@@ -863,257 +863,169 @@ void alltoallv(PeerContext& pc, const void* in, const std::vector<size_t>& sendB
 }
 
 namespace {
-// Like the host-count v-variant the grid is fixed (the sizes are only known on the device, the
-// grid must be the same on every rank), and P = 1 runs the same kernel: the expert-major layout
-// still applies.
-// `scales` non-null: the quantising form (rowBytes = hidden, bf16 input); `stagedScales` goes
-// with `stagedOut`.
-void alltoallvDevCommon(PeerContext& pc, const void* in, size_t inRows, size_t rowBytes, const int64_t* inSplits,
-                        const int64_t* inOffsets, const PeerPtrs& outs, void* stagedOut, size_t capacityRows,
-                        int64_t* outSplits, int64_t* outOffsets, int experts, int align, bool inverse,
-                        cudaStream_t stream, const PeerPtrs* scales = nullptr, float* stagedScales = nullptr) {
-  GLB_TRACE_RANGE("glb::cuda::alltoallv_dev");
-  GLB_ENFORCE(experts >= 1 && experts <= kMaxA2aExperts, "alltoallv_dev: experts per rank must be in 1..",
-              kMaxA2aExperts, ", got ", experts);
-  GLB_ENFORCE(align >= 1, "alltoallv_dev: align must be at least 1, got ", align);
-  GLB_ENFORCE(rowBytes > 0 && rowBytes <= 0xffffffffull, "alltoallv_dev: row size must be 1 byte .. 4 GB, got ",
-              rowBytes);
-  GLB_ENFORCE(inSplits != nullptr, "alltoallv_dev: no input splits");
-  GLB_ENFORCE(!inverse || inOffsets != nullptr, "alltoallv_dev: the inverse exchange needs the input offsets");
-  GLB_ENFORCE(inverse || (outSplits != nullptr && outOffsets != nullptr),
-              "alltoallv_dev: the forward exchange needs output splits and offsets");
-  const uint32_t cap = static_cast<uint32_t>(std::min<size_t>(capacityRows, 0xfffffffeull));
-  const bool fp8 = scales != nullptr;
-  const int blocks =
-      std::max(1, std::min({tuning().alltoallvBlocks, pc.coResidentBlocks(alltoallvDevKernelPtr(fp8)), kMaxBlocks}));
-  prologue(pc, stream);
-  if (fp8) {
-    launchAlltoallvDevFp8(pc.comm(), outs, *scales, in, inRows, rowBytes, reinterpret_cast<const long long*>(inSplits),
-                          reinterpret_cast<long long*>(outSplits), reinterpret_cast<long long*>(outOffsets), stagedOut,
-                          stagedScales, cap, experts, align, pc.inputStatusDevice(), blocks, stream);
-  } else {
-    launchAlltoallvDev(pc.comm(), outs, in, inRows, rowBytes, reinterpret_cast<const long long*>(inSplits),
-                       reinterpret_cast<const long long*>(inOffsets), reinterpret_cast<long long*>(outSplits),
-                       reinterpret_cast<long long*>(outOffsets), stagedOut, cap, experts, align, inverse,
-                       pc.inputStatusDevice(), blocks, stream);
-  }
-  finish(pc, stream, "alltoallv_dev");
+// The limits the device-split MoE calls share, named after the public operation. Rows are
+// `rowBytes` (quantising: H codes, H a multiple of kFp8Block) and a multiple of `rowMultiple`.
+void checkMoeLimits(const char* name, int experts, int align, size_t rowBytes, size_t rowMultiple) {
+  GLB_ENFORCE(experts >= 1 && experts <= kMaxA2aExperts, name, ": experts per rank must be in 1..", kMaxA2aExperts,
+              ", got ", experts);
+  GLB_ENFORCE(align >= 1, name, ": align must be at least 1, got ", align);
+  GLB_ENFORCE(rowBytes > 0 && rowBytes <= 0xffffffffull, name, ": row size must be 1 byte .. 4 GB, got ", rowBytes);
+  GLB_ENFORCE(rowBytes % rowMultiple == 0, name, ": the row size must be a positive multiple of ", rowMultiple,
+              " bytes, got ", rowBytes);
 }
 
-void checkFp8Dispatch(const void* in, const void* out, size_t hidden) {
-  GLB_ENFORCE(hidden > 0 && hidden % kFp8Block == 0, "alltoallv_dev (bf16 -> e4m3): the row length must be a "
-              "positive multiple of ", kFp8Block, ", got ", hidden);
-  GLB_ENFORCE(reinterpret_cast<uintptr_t>(in) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0,
-              "alltoallv_dev (bf16 -> e4m3): input and output must be 16-byte aligned");
+void checkTopk(const char* name, int topk) {
+  GLB_ENFORCE(topk >= 1 && topk <= 32, name, ": topk must be in 1..32, got ", topk);
+}
+
+void checkAligned16(const char* name, const void* a, const void* b, const char* what) {
+  GLB_ENFORCE(reinterpret_cast<uintptr_t>(a) % 16 == 0 && reinterpret_cast<uintptr_t>(b) % 16 == 0, name, ": ", what,
+              " must be 16-byte aligned");
+}
+
+// What a kernel needs from a MoeOut (and, quantising, its scales): every rank's rows in place or
+// its staging area, my staged pointers, and the capacity in rows. Registered: bounds-checked
+// against the registration, zero copy. Plain: staged through the pool's bulk region, where a row
+// takes rowBytes, plus its scales after the capacity's codes (hidden is a multiple of 128, so they
+// start 16-byte aligned); that caps the capacity.
+struct MoeTarget {
+  PeerPtrs peers;
+  MoeScales scales;
+  const char* mine;  // my rows, wherever they are read or written by this rank's caller
+  char* staged;      // my plain tensor (null if it is empty)
+  bool plain;
+  size_t capRows;
+};
+
+MoeTarget resolveMoeOut(const PeerContext& pc, const char* name, const char* what, const MoeOut& out,
+                        const MoeOut* scales, size_t capacityRows, size_t rowBytes) {
+  if (scales != nullptr && (out.buf == nullptr) != (scales->buf == nullptr)) {
+    GLB_THROW(InputException, name, ": out and out_scales must both be registered / symmetric or both plain");
+  }
+  const size_t scaleBytes = scales != nullptr ? rowBytes / kFp8Block * sizeof(float) : 0;
+  MoeTarget t{};
+  if (out.buf != nullptr) {
+    GLB_ENFORCE_LE(out.offset + capacityRows * rowBytes, out.buf->bytes, name, ": ", what,
+                   " exceeds the registered buffer");
+    t.peers = out.buf->ptrsAt(out.offset);
+    t.mine = static_cast<const char*>(out.buf->local) + out.offset;
+    t.capRows = capacityRows;
+    if (scales != nullptr) {
+      GLB_ENFORCE_LE(scales->offset + capacityRows * scaleBytes, scales->buf->bytes, name,
+                     ": output scales exceed the registered buffer");
+      GLB_ENFORCE(scales->offset % sizeof(float) == 0, name, ": output scales must be 4-byte aligned");
+      t.scales.scales = scales->buf->ptrsAt(scales->offset);
+    }
+  } else {
+    const auto l = layoutOf(pc);
+    t.peers = pc.stagePtrs(l.bulkOff);
+    t.mine = static_cast<const char*>(out.ptr);
+    t.staged = static_cast<char*>(out.ptr);
+    t.plain = true;
+    t.capRows = std::min(capacityRows, l.bulkBytes / (rowBytes + scaleBytes));
+    if (scales != nullptr) {
+      GLB_ENFORCE(reinterpret_cast<uintptr_t>(scales->ptr) % sizeof(float) == 0, name,
+                  ": output scales must be 4-byte aligned");
+      t.scales.stagedScales = static_cast<float*>(scales->ptr);
+    }
+  }
+  return t;
+}
+
+MoeArgs moeArgs(PeerContext& pc, const MoeTarget& t, size_t rowBytes, int experts, int align) {
+  MoeArgs d{};
+  d.rowBytes = rowBytes;
+  d.staged = t.staged;
+  d.status = pc.inputStatusDevice();
+  d.capRows = static_cast<uint32_t>(std::min<size_t>(t.capRows, 0xfffffffeull));
+  d.experts = experts;
+  d.align = align;
+  d.plain = t.plain ? 1 : 0;
+  return d;
+}
+
+// Like the host-count v-variant the grid is fixed (the sizes are only known on the device, the
+// grid must be the same on every rank), and P = 1 runs the same kernel: the layouts still apply.
+int moeBlocks(PeerContext& pc, const void* kernel) {
+  return std::max(1, std::min({tuning().alltoallvBlocks, pc.coResidentBlocks(kernel), kMaxBlocks}));
 }
 }  // namespace
 
 void alltoallvDev(PeerContext& pc, const void* in, size_t inRows, size_t rowBytes, const int64_t* inSplits,
-                  const int64_t* inOffsets, const PeerBuffer& out, size_t outOffset, size_t capacityRows,
-                  int64_t* outSplits, int64_t* outOffsets, int experts, int align, bool inverse, cudaStream_t stream) {
+                  const int64_t* inOffsets, const MoeOut& out, size_t capacityRows, int64_t* outSplits,
+                  int64_t* outOffsets, int experts, int align, bool inverse, cudaStream_t stream,
+                  const MoeOut* outScales) {
   DeviceGuard g(pc.device);
-  GLB_ENFORCE(rowBytes > 0, "alltoallv_dev: row size must be positive");
-  GLB_ENFORCE_LE(outOffset + capacityRows * rowBytes, out.bytes, "alltoallv_dev output exceeds the registered buffer");
-  alltoallvDevCommon(pc, in, inRows, rowBytes, inSplits, inOffsets, out.ptrsAt(outOffset), nullptr, capacityRows,
-                     outSplits, outOffsets, experts, align, inverse, stream);
-}
-
-void alltoallvDev(PeerContext& pc, const void* in, size_t inRows, size_t rowBytes, const int64_t* inSplits,
-                  const int64_t* inOffsets, void* out, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets,
-                  int experts, int align, bool inverse, cudaStream_t stream) {
-  DeviceGuard g(pc.device);
-  GLB_ENFORCE(rowBytes > 0, "alltoallv_dev: row size must be positive");
-  // Peers push into my staging area; I copy my rows out of it inside the same kernel.
-  const auto l = layoutOf(pc);
-  alltoallvDevCommon(pc, in, inRows, rowBytes, inSplits, inOffsets, pc.stagePtrs(l.bulkOff), out,
-                     std::min(capacityRows, l.bulkBytes / rowBytes), outSplits, outOffsets, experts, align, inverse,
+  GLB_TRACE_RANGE("glb::cuda::alltoallv_dev");
+  const char* name = "alltoallv_dev";
+  const bool fp8 = outScales != nullptr;
+  checkMoeLimits(name, experts, align, rowBytes, fp8 ? kFp8Block : 1);
+  GLB_ENFORCE(inSplits != nullptr, name, ": no input splits");
+  GLB_ENFORCE(!inverse || (inOffsets != nullptr && !fp8), name,
+              ": the inverse exchange needs the input offsets and does not quantise");
+  GLB_ENFORCE(inverse || (outSplits != nullptr && outOffsets != nullptr),
+              name, ": the forward exchange needs output splits and offsets");
+  const MoeTarget t = resolveMoeOut(pc, name, "out", out, outScales, capacityRows, rowBytes);
+  if (fp8) checkAligned16(name, in, t.mine, "input and output");
+  const int blocks = moeBlocks(pc, alltoallvDevKernelPtr(fp8));
+  prologue(pc, stream);
+  launchAlltoallvDev(pc.comm(), t.peers, moeArgs(pc, t, rowBytes, experts, align), fp8 ? &t.scales : nullptr, in,
+                     inRows, reinterpret_cast<const long long*>(inSplits), reinterpret_cast<const long long*>(inOffsets),
+                     reinterpret_cast<long long*>(outSplits), reinterpret_cast<long long*>(outOffsets), inverse, blocks,
                      stream);
+  finish(pc, stream, name);
 }
 
-void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidden, const int64_t* inSplits,
-                     const PeerBuffer& out, size_t outOffset, const PeerBuffer& outScales, size_t scalesOffset,
-                     size_t capacityRows, int64_t* outSplits, int64_t* outOffsets, int experts, int align,
-                     cudaStream_t stream) {
+void alltoallvDevTopk(PeerContext& pc, const void* x, size_t tokens, size_t rowBytes, int topk, const int64_t* topkIdx,
+                      int64_t* splits, int64_t* pos, const MoeOut& out, size_t capacityRows, int64_t* outSplits,
+                      int64_t* outOffsets, int experts, int align, cudaStream_t stream, const MoeOut* outScales) {
   DeviceGuard g(pc.device);
-  checkFp8Dispatch(in, static_cast<const char*>(out.local) + outOffset, hidden);
-  GLB_ENFORCE_LE(outOffset + capacityRows * hidden, out.bytes, "alltoallv_dev output exceeds the registered buffer");
-  GLB_ENFORCE_LE(scalesOffset + capacityRows * (hidden / kFp8Block) * sizeof(float), outScales.bytes,
-                 "alltoallv_dev output scales exceed the registered buffer");
-  GLB_ENFORCE(scalesOffset % sizeof(float) == 0, "alltoallv_dev: output scales must be 4-byte aligned");
-  const PeerPtrs scales = outScales.ptrsAt(scalesOffset);
-  alltoallvDevCommon(pc, in, inRows, hidden, inSplits, nullptr, out.ptrsAt(outOffset), nullptr, capacityRows, outSplits,
-                     outOffsets, experts, align, false, stream, &scales, nullptr);
-}
-
-void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidden, const int64_t* inSplits,
-                     void* out, float* outScales, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets,
-                     int experts, int align, cudaStream_t stream) {
-  DeviceGuard g(pc.device);
-  checkFp8Dispatch(in, out, hidden);
-  GLB_ENFORCE(reinterpret_cast<uintptr_t>(outScales) % sizeof(float) == 0,
-              "alltoallv_dev: output scales must be 4-byte aligned");
-  // Peers push codes into my staging area and the scales after my capacity's worth of codes; a
-  // row takes hidden + hidden / 32 bytes there (hidden is a multiple of 128, so the scales start
-  // 16-byte aligned).
-  const auto l = layoutOf(pc);
-  const PeerPtrs none{};
-  alltoallvDevCommon(pc, in, inRows, hidden, inSplits, nullptr, pc.stagePtrs(l.bulkOff), out,
-                     std::min(capacityRows, l.bulkBytes / (hidden + hidden / kFp8Block * sizeof(float))), outSplits,
-                     outOffsets, experts, align, false, stream, &none, outScales);
-}
-
-namespace {
-// `outs` are the ranks' out (zero copy) or staging areas, `stagedOut` my plain out. `scales`
-// non-null: the quantising form (rowBytes = hidden, bf16 x), `stagedScales` with `stagedOut`.
-void dispatchTopkCommon(PeerContext& pc, const void* x, size_t tokens, size_t rowBytes, int topk,
-                        const int64_t* topkIdx, int64_t* splits, int64_t* pos, const PeerPtrs& outs, const void* out,
-                        void* stagedOut, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets, int experts,
-                        int align, cudaStream_t stream, const PeerPtrs* scales = nullptr,
-                        float* stagedScales = nullptr) {
   GLB_TRACE_RANGE("glb::cuda::alltoallv_dev_topk");
   const char* name = "alltoallv_dev_topk";
-  GLB_ENFORCE(topk >= 1 && topk <= 32, name, ": topk must be in 1..32, got ", topk);
-  GLB_ENFORCE(experts >= 1 && experts <= kMaxA2aExperts, name, ": experts per rank must be in 1..", kMaxA2aExperts,
-              ", got ", experts);
-  GLB_ENFORCE(align >= 1, name, ": align must be at least 1, got ", align);
-  GLB_ENFORCE(rowBytes > 0 && rowBytes % 16 == 0 && rowBytes <= 0xffffffffull, name,
-              ": the row size must be a positive multiple of 16 bytes, got ", rowBytes);
+  const bool fp8 = outScales != nullptr;
+  checkTopk(name, topk);
+  checkMoeLimits(name, experts, align, rowBytes, fp8 ? kFp8Block : 16);
   GLB_ENFORCE(tokens * static_cast<size_t>(topk) <= 0x7fffffffull, name, ": tokens x topk must be below 2^31, got ",
               tokens, " x ", topk);
   GLB_ENFORCE(splits != nullptr && outSplits != nullptr && outOffsets != nullptr &&
                   (tokens == 0 || (x != nullptr && topkIdx != nullptr && pos != nullptr)),
               name, ": missing x, topk_idx, splits, pos, out_splits or out_offsets");
-  GLB_ENFORCE(reinterpret_cast<uintptr_t>(x) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0, name,
-              ": x and out must be 16-byte aligned");
-  const bool fp8 = scales != nullptr;
+  const MoeTarget t = resolveMoeOut(pc, name, "out", out, outScales, capacityRows, rowBytes);
+  checkAligned16(name, x, t.mine, "x and out");
   // Peers write my out while I still read my x.
-  rejectOverlap(x, tokens * rowBytes * (fp8 ? 2 : 1), out, capacityRows * rowBytes, name);
-  const uint32_t cap = static_cast<uint32_t>(std::min<size_t>(capacityRows, 0xfffffffeull));
-  const int blocks =
-      std::max(1, std::min({tuning().alltoallvBlocks, pc.coResidentBlocks(moeDispatchTopkKernelPtr(fp8)), kMaxBlocks}));
-  auto* idx = reinterpret_cast<const long long*>(topkIdx);
-  auto* sp = reinterpret_cast<long long*>(splits);
-  auto* ps = reinterpret_cast<long long*>(pos);
-  auto* os = reinterpret_cast<long long*>(outSplits);
-  auto* oo = reinterpret_cast<long long*>(outOffsets);
+  rejectOverlap(x, tokens * rowBytes * (fp8 ? 2 : 1), t.mine, capacityRows * rowBytes, name);
+  const int blocks = moeBlocks(pc, moeDispatchTopkKernelPtr(fp8));
   prologue(pc, stream);
-  if (fp8) {
-    launchMoeDispatchTopkFp8(pc.comm(), outs, *scales, x, tokens, topk, idx, sp, ps, os, oo, stagedOut, stagedScales,
-                             rowBytes, cap, experts, align, pc.inputStatusDevice(), blocks, stream);
-  } else {
-    launchMoeDispatchTopk(pc.comm(), outs, x, tokens, topk, idx, sp, ps, os, oo, stagedOut, rowBytes, cap, experts,
-                          align, pc.inputStatusDevice(), blocks, stream);
-  }
+  launchMoeDispatchTopk(pc.comm(), t.peers, moeArgs(pc, t, rowBytes, experts, align), fp8 ? &t.scales : nullptr, x,
+                        tokens, topk, reinterpret_cast<const long long*>(topkIdx), reinterpret_cast<long long*>(splits),
+                        reinterpret_cast<long long*>(pos), reinterpret_cast<long long*>(outSplits),
+                        reinterpret_cast<long long*>(outOffsets), blocks, stream);
   finish(pc, stream, name);
 }
-}  // namespace
-
-void alltoallvDevTopk(PeerContext& pc, const void* x, size_t tokens, size_t rowBytes, int topk, const int64_t* topkIdx,
-                      int64_t* splits, int64_t* pos, const PeerBuffer& out, size_t outOffset, size_t capacityRows,
-                      int64_t* outSplits, int64_t* outOffsets, int experts, int align, cudaStream_t stream) {
-  DeviceGuard g(pc.device);
-  GLB_ENFORCE_LE(outOffset + capacityRows * rowBytes, out.bytes, "alltoallv_dev_topk output exceeds the registered buffer");
-  dispatchTopkCommon(pc, x, tokens, rowBytes, topk, topkIdx, splits, pos, out.ptrsAt(outOffset),
-                     static_cast<const char*>(out.local) + outOffset, nullptr, capacityRows, outSplits, outOffsets,
-                     experts, align, stream);
-}
-
-void alltoallvDevTopk(PeerContext& pc, const void* x, size_t tokens, size_t rowBytes, int topk, const int64_t* topkIdx,
-                      int64_t* splits, int64_t* pos, void* out, size_t capacityRows, int64_t* outSplits,
-                      int64_t* outOffsets, int experts, int align, cudaStream_t stream) {
-  DeviceGuard g(pc.device);
-  GLB_ENFORCE(rowBytes > 0, "alltoallv_dev_topk: row size must be positive");
-  // Peers push into my staging area; I copy my rows out of it inside the same kernel.
-  const auto l = layoutOf(pc);
-  dispatchTopkCommon(pc, x, tokens, rowBytes, topk, topkIdx, splits, pos, pc.stagePtrs(l.bulkOff), out, out,
-                     std::min(capacityRows, l.bulkBytes / rowBytes), outSplits, outOffsets, experts, align, stream);
-}
-
-void alltoallvDevTopkFp8(PeerContext& pc, const void* x, size_t tokens, size_t hidden, int topk,
-                         const int64_t* topkIdx, int64_t* splits, int64_t* pos, const PeerBuffer& out, size_t outOffset,
-                         const PeerBuffer& outScales, size_t scalesOffset, size_t capacityRows, int64_t* outSplits,
-                         int64_t* outOffsets, int experts, int align, cudaStream_t stream) {
-  DeviceGuard g(pc.device);
-  checkFp8Dispatch(x, static_cast<const char*>(out.local) + outOffset, hidden);
-  GLB_ENFORCE_LE(outOffset + capacityRows * hidden, out.bytes, "alltoallv_dev_topk output exceeds the registered buffer");
-  GLB_ENFORCE_LE(scalesOffset + capacityRows * (hidden / kFp8Block) * sizeof(float), outScales.bytes,
-                 "alltoallv_dev_topk output scales exceed the registered buffer");
-  GLB_ENFORCE(scalesOffset % sizeof(float) == 0, "alltoallv_dev_topk: output scales must be 4-byte aligned");
-  const PeerPtrs scales = outScales.ptrsAt(scalesOffset);
-  dispatchTopkCommon(pc, x, tokens, hidden, topk, topkIdx, splits, pos, out.ptrsAt(outOffset),
-                     static_cast<const char*>(out.local) + outOffset, nullptr, capacityRows, outSplits, outOffsets,
-                     experts, align, stream, &scales, nullptr);
-}
-
-void alltoallvDevTopkFp8(PeerContext& pc, const void* x, size_t tokens, size_t hidden, int topk,
-                         const int64_t* topkIdx, int64_t* splits, int64_t* pos, void* out, float* outScales,
-                         size_t capacityRows, int64_t* outSplits, int64_t* outOffsets, int experts, int align,
-                         cudaStream_t stream) {
-  DeviceGuard g(pc.device);
-  checkFp8Dispatch(x, out, hidden);
-  GLB_ENFORCE(reinterpret_cast<uintptr_t>(outScales) % sizeof(float) == 0,
-              "alltoallv_dev_topk: output scales must be 4-byte aligned");
-  // The staging layout of alltoallvDevFp8: codes, then the scales after the capacity's codes.
-  const auto l = layoutOf(pc);
-  const PeerPtrs none{};
-  dispatchTopkCommon(pc, x, tokens, hidden, topk, topkIdx, splits, pos, pc.stagePtrs(l.bulkOff), out, out,
-                     std::min(capacityRows, l.bulkBytes / (hidden + hidden / kFp8Block * sizeof(float))), outSplits,
-                     outOffsets, experts, align, stream, &none, outScales);
-}
-
-namespace {
-// `srcs` are the ranks' expert_out (zero copy) or staging areas, `stagedIn` my plain expert_out.
-void combineTopkCommon(PeerContext& pc, void* out, size_t tokens, int topk, const int64_t* pos, const float* weights,
-                       const int64_t* splits, const void* expertOut, const PeerPtrs& srcs, const void* stagedIn,
-                       size_t capacityRows, size_t rowBytes, DataType dt, int experts, int align, cudaStream_t stream) {
-  GLB_TRACE_RANGE("glb::cuda::alltoallv_dev_combine_topk");
-  GLB_ENFORCE(dt == DataType::FLOAT32 || dt == DataType::BFLOAT16 || dt == DataType::FLOAT16,
-              "alltoallv_dev_combine_topk: rows must be float32, bfloat16 or float16");
-  GLB_ENFORCE(topk >= 1 && topk <= 32, "alltoallv_dev_combine_topk: topk must be in 1..32, got ", topk);
-  GLB_ENFORCE(experts >= 1 && experts <= kMaxA2aExperts, "alltoallv_dev_combine_topk: experts per rank must be in 1..",
-              kMaxA2aExperts, ", got ", experts);
-  GLB_ENFORCE(align >= 1, "alltoallv_dev_combine_topk: align must be at least 1, got ", align);
-  GLB_ENFORCE(rowBytes > 0 && rowBytes % 16 == 0 && rowBytes <= 0xffffffffull,
-              "alltoallv_dev_combine_topk: the row size must be a positive multiple of 16 bytes, got ", rowBytes);
-  GLB_ENFORCE(splits != nullptr && (tokens == 0 || (pos != nullptr && weights != nullptr && out != nullptr)),
-              "alltoallv_dev_combine_topk: missing splits, pos, weights or out");
-  GLB_ENFORCE(reinterpret_cast<uintptr_t>(out) % 16 == 0 && reinterpret_cast<uintptr_t>(expertOut) % 16 == 0,
-              "alltoallv_dev_combine_topk: out and expert_out must be 16-byte aligned");
-  const uint32_t cap = static_cast<uint32_t>(std::min<size_t>(capacityRows, 0xfffffffeull));
-  const int blocks =
-      std::max(1, std::min({tuning().alltoallvBlocks, pc.coResidentBlocks(moeCombineTopkKernelPtr(dt)), kMaxBlocks}));
-  prologue(pc, stream);
-  launchMoeCombineTopk(pc.comm(), srcs, stagedIn, out, tokens, topk, reinterpret_cast<const long long*>(pos), weights,
-                       reinterpret_cast<const long long*>(splits), rowBytes, dt, cap, experts, align,
-                       pc.inputStatusDevice(), blocks, stream);
-  finish(pc, stream, "alltoallv_dev_combine_topk");
-}
-}  // namespace
 
 void alltoallvDevCombineTopk(PeerContext& pc, void* out, size_t tokens, int topk, const int64_t* pos,
-                             const float* weights, const int64_t* splits, const PeerBuffer& expertOut, size_t offset,
-                             size_t capacityRows, size_t rowBytes, DataType dt, int experts, int align,
-                             cudaStream_t stream) {
-  DeviceGuard g(pc.device);
-  GLB_ENFORCE_LE(offset + capacityRows * rowBytes, expertOut.bytes,
-                 "alltoallv_dev_combine_topk: expert_out exceeds the registered buffer");
-  const char* mine = static_cast<const char*>(expertOut.local) + offset;
-  // Peers read my expert_out while I write my out.
-  rejectOverlap(mine, capacityRows * rowBytes, out, tokens * rowBytes, "alltoallv_dev_combine_topk");
-  combineTopkCommon(pc, out, tokens, topk, pos, weights, splits, mine,
-                    expertOut.ptrsAt(offset), nullptr, capacityRows, rowBytes, dt, experts, align, stream);
-}
-
-void alltoallvDevCombineTopk(PeerContext& pc, void* out, size_t tokens, int topk, const int64_t* pos,
-                             const float* weights, const int64_t* splits, const void* expertOut, size_t capacityRows,
+                             const float* weights, const int64_t* splits, const MoeOut& expertOut, size_t capacityRows,
                              size_t rowBytes, DataType dt, int experts, int align, cudaStream_t stream) {
   DeviceGuard g(pc.device);
-  GLB_ENFORCE(rowBytes > 0, "alltoallv_dev_combine_topk: row size must be positive");
-  rejectOverlap(expertOut, capacityRows * rowBytes, out, tokens * rowBytes, "alltoallv_dev_combine_topk");
-  // Each rank copies its rows into its own staging area, where its peers read them.
-  const auto l = layoutOf(pc);
-  combineTopkCommon(pc, out, tokens, topk, pos, weights, splits, expertOut, pc.stagePtrs(l.bulkOff), expertOut,
-                    std::min(capacityRows, l.bulkBytes / rowBytes), rowBytes, dt, experts, align, stream);
+  GLB_TRACE_RANGE("glb::cuda::alltoallv_dev_combine_topk");
+  const char* name = "alltoallv_dev_combine_topk";
+  GLB_ENFORCE(dt == DataType::FLOAT32 || dt == DataType::BFLOAT16 || dt == DataType::FLOAT16, name,
+              ": rows must be float32, bfloat16 or float16");
+  checkTopk(name, topk);
+  checkMoeLimits(name, experts, align, rowBytes, 16);
+  GLB_ENFORCE(splits != nullptr && (tokens == 0 || (pos != nullptr && weights != nullptr && out != nullptr)),
+              name, ": missing splits, pos, weights or out");
+  // A plain expert_out is copied into my staging area, where my peers read it.
+  const MoeTarget t = resolveMoeOut(pc, name, "expert_out", expertOut, nullptr, capacityRows, rowBytes);
+  checkAligned16(name, out, t.mine, "out and expert_out");
+  // Peers read my expert_out while I write my out.
+  rejectOverlap(t.mine, capacityRows * rowBytes, out, tokens * rowBytes, name);
+  const int blocks = moeBlocks(pc, moeCombineTopkKernelPtr(dt));
+  prologue(pc, stream);
+  launchMoeCombineTopk(pc.comm(), t.peers, moeArgs(pc, t, rowBytes, experts, align), out, tokens, topk,
+                       reinterpret_cast<const long long*>(pos), weights, reinterpret_cast<const long long*>(splits), dt,
+                       blocks, stream);
+  finish(pc, stream, name);
 }
 
 void scatter(PeerContext& pc, const void* in, const PeerBuffer& out, size_t outOffset, size_t bytes, int root,

@@ -136,6 +136,15 @@ void alltoallv(PeerContext& pc, const void* in, const std::vector<size_t>& sendB
 void alltoallv(PeerContext& pc, const void* in, const std::vector<size_t>& sendBytes, void* out,
                const std::vector<size_t>& recvBytes, cudaStream_t stream);
 
+// Where the rows of a device-split MoE call live on this rank: a registered buffer at `offset`
+// (zero copy), or, with `buf` null, a plain device pointer (staged through the pool, which also
+// caps the capacity). Every rank must pass the same kind; a mix is invalid input on every rank.
+struct MoeOut {
+  const PeerBuffer* buf = nullptr;
+  size_t offset = 0;
+  void* ptr = nullptr;
+};
+
 // All-to-all-v whose row counts live on the device (expert-parallel dispatch / combine): one
 // kernel, no host value depends on the device data, so it needs no synchronisation and can be
 // captured in a CUDA graph. A row is `rowBytes` on every rank; `in` holds `inRows` rows.
@@ -150,27 +159,18 @@ void alltoallv(PeerContext& pc, const void* in, const std::vector<size_t>& sendB
 // what fits the staging pool) receives nothing; invalid splits or offsets move nothing. Either
 // is raised as InputException by the next checkHealth() on every rank that runs after the kernel
 // has (synchronize() is the dependable place: earlier calls may not see it yet).
+// `outScales` set: the quantising forward form (FP8 expert dispatch). `in` holds `inRows` bf16
+// rows of `rowBytes` = hidden elements (a multiple of kFp8Block); each row arrives as `hidden`
+// e4m3 codes in `out` and hidden / kFp8Block fp32 scales in `outScales` (row-major, capacityRows
+// rows), at the same row index, so x ~= code * scale. Per block of kFp8Block elements: amax =
+// max(max|x|, 1e-4), code = e4m3(x * (448 * (1 / amax))) (round to nearest even, saturating),
+// scale = amax / 448, each a correctly rounded fp32 operation. `in` and `out` must be 16-byte
+// aligned, and out and outScales of one kind. For plain pointers the capacity is capped by what
+// fits the staging pool at hidden + hidden / 32 bytes a row.
 void alltoallvDev(PeerContext& pc, const void* in, size_t inRows, size_t rowBytes, const int64_t* inSplits,
-                  const int64_t* inOffsets, const PeerBuffer& out, size_t outOffset, size_t capacityRows,
-                  int64_t* outSplits, int64_t* outOffsets, int experts, int align, bool inverse, cudaStream_t stream);
-void alltoallvDev(PeerContext& pc, const void* in, size_t inRows, size_t rowBytes, const int64_t* inSplits,
-                  const int64_t* inOffsets, void* out, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets,
-                  int experts, int align, bool inverse, cudaStream_t stream);
-// The quantising form of the forward alltoallvDev (FP8 expert dispatch): `in` holds `inRows` bf16
-// rows of `hidden` elements (a multiple of kFp8Block); each row arrives as `hidden` e4m3 codes in
-// `out` and hidden / kFp8Block fp32 scales in `outScales` (row-major, capacityRows rows), at the
-// same row index, so x ~= code * scale. Per block of kFp8Block elements: amax = max(max|x|, 1e-4),
-// code = e4m3(x * (448 * (1 / amax))) (round to nearest even, saturating), scale = amax / 448,
-// each a correctly rounded fp32 operation. Splits, layout, capacity and error reporting are those of
-// alltoallvDev. `in` and `out` must be 16-byte aligned. For plain pointers the capacity is also
-// capped by what fits the staging pool at hidden + hidden / 32 bytes a row.
-void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidden, const int64_t* inSplits,
-                     const PeerBuffer& out, size_t outOffset, const PeerBuffer& outScales, size_t scalesOffset,
-                     size_t capacityRows, int64_t* outSplits, int64_t* outOffsets, int experts, int align,
-                     cudaStream_t stream);
-void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidden, const int64_t* inSplits,
-                     void* out, float* outScales, size_t capacityRows, int64_t* outSplits, int64_t* outOffsets,
-                     int experts, int align, cudaStream_t stream);
+                  const int64_t* inOffsets, const MoeOut& out, size_t capacityRows, int64_t* outSplits,
+                  int64_t* outOffsets, int experts, int align, bool inverse, cudaStream_t stream,
+                  const MoeOut* outScales = nullptr);
 // Top-k MoE dispatch: route() + the forward alltoallvDev in one kernel. `x` holds `tokens` rows
 // of `rowBytes` (a multiple of 16; x and out 16-byte aligned, disjoint); `topkIdx` is int64
 // (tokens, topk), 1 <= topk <= 32, tokens x topk < 2^31: entry j·E + e chooses local expert e
@@ -180,22 +180,12 @@ void alltoallvDevFp8(PeerContext& pc, const void* in, size_t inRows, size_t hidd
 // outOffsets then equal those of alltoallvDev(route()'s rows, splits) byte for byte: within a
 // (rank, expert) group rows go by token, then by choice. Each token is read once and stored to
 // each of its choices. Capacity, paths and error reporting are those of alltoallvDev.
+// `outScales` set: the quantising form, with alltoallvDev's input, outputs, numerics and checks;
+// each token is quantised once and the same codes and scales are stored to all its choices.
 void alltoallvDevTopk(PeerContext& pc, const void* x, size_t tokens, size_t rowBytes, int topk, const int64_t* topkIdx,
-                      int64_t* splits, int64_t* pos, const PeerBuffer& out, size_t outOffset, size_t capacityRows,
-                      int64_t* outSplits, int64_t* outOffsets, int experts, int align, cudaStream_t stream);
-void alltoallvDevTopk(PeerContext& pc, const void* x, size_t tokens, size_t rowBytes, int topk, const int64_t* topkIdx,
-                      int64_t* splits, int64_t* pos, void* out, size_t capacityRows, int64_t* outSplits,
-                      int64_t* outOffsets, int experts, int align, cudaStream_t stream);
-// Its quantising form, with alltoallvDevFp8's input, outputs, numerics and checks: each token is
-// quantised once and the same codes and scales are stored to all its choices.
-void alltoallvDevTopkFp8(PeerContext& pc, const void* x, size_t tokens, size_t hidden, int topk,
-                         const int64_t* topkIdx, int64_t* splits, int64_t* pos, const PeerBuffer& out, size_t outOffset,
-                         const PeerBuffer& outScales, size_t scalesOffset, size_t capacityRows, int64_t* outSplits,
-                         int64_t* outOffsets, int experts, int align, cudaStream_t stream);
-void alltoallvDevTopkFp8(PeerContext& pc, const void* x, size_t tokens, size_t hidden, int topk,
-                         const int64_t* topkIdx, int64_t* splits, int64_t* pos, void* out, float* outScales,
-                         size_t capacityRows, int64_t* outSplits, int64_t* outOffsets, int experts, int align,
-                         cudaStream_t stream);
+                      int64_t* splits, int64_t* pos, const MoeOut& out, size_t capacityRows, int64_t* outSplits,
+                      int64_t* outOffsets, int experts, int align, cudaStream_t stream,
+                      const MoeOut* outScales = nullptr);
 // Top-k MoE combine: the inverse of the forward alltoallvDev fused with the gate-weighted sum.
 // `splits` is the in_splits this rank passed to the dispatch; `expertOut` holds, on every rank, the
 // experts' output rows (`rowBytes` each, dtype dt: float, bfloat16 or float16) in that dispatch's
@@ -209,11 +199,7 @@ void alltoallvDevTopkFp8(PeerContext& pc, const void* x, size_t tokens, size_t h
 // out of range, arguments that differ between ranks, an overflowing holder) are raised like
 // alltoallvDev's, and no rank writes its out.
 void alltoallvDevCombineTopk(PeerContext& pc, void* out, size_t tokens, int topk, const int64_t* pos,
-                             const float* weights, const int64_t* splits, const PeerBuffer& expertOut, size_t offset,
-                             size_t capacityRows, size_t rowBytes, DataType dt, int experts, int align,
-                             cudaStream_t stream);
-void alltoallvDevCombineTopk(PeerContext& pc, void* out, size_t tokens, int topk, const int64_t* pos,
-                             const float* weights, const int64_t* splits, const void* expertOut, size_t capacityRows,
+                             const float* weights, const int64_t* splits, const MoeOut& expertOut, size_t capacityRows,
                              size_t rowBytes, DataType dt, int experts, int align, cudaStream_t stream);
 // Fixed-size alltoall: every chunk is `bytes` long on every rank (this is known to all
 // ranks, so the small-message LL kernel and size-dependent grids are safe here).

@@ -12,6 +12,7 @@ namespace cuda {
 // Force-load all kernels of the library on the current device (idempotent, cheap).
 void preloadAllreduceKernels();
 void preloadCollectiveKernels();
+void preloadMoeKernels();
 void preloadScheduleKernels();
 void preloadLocalKernels();
 void preloadPipelineKernels();
@@ -98,52 +99,7 @@ void launchAlltoallPush(const CommArgs& a, const void* in, const PeerPtrs& outs,
 void launchReducePull(const CommArgs& a, const PeerPtrs& ins, void* mcIn, void* out, const size_t* elemOff,
                       const size_t* elemLen, DataType dt, ReduceOp op, float scale, bool vec, bool useMc, int blocks,
                       cudaStream_t stream);
-// Device-split all-to-all-v: row counts come from device arrays (int64, P·E entries) and are
-// exchanged inside the kernel. `outs.p[r]` is rank r's output (zero copy) or staging area; with
-// `stagedOut` set, each rank copies its rows from its staging area to stagedOut after the second
-// barrier. See collective_kernels.cu for the two layouts.
-void launchAlltoallvDev(const CommArgs& a, const PeerPtrs& outs, const void* in, size_t inRows, size_t rowBytes,
-                        const long long* inSplits, const long long* inOffsets, long long* outSplits,
-                        long long* outOffsets, void* stagedOut, uint32_t capRows, int experts, int align, bool inverse,
-                        InputStatus* status, int blocks, cudaStream_t stream);
-// Its quantising forward form: `in` holds bf16 rows of `hidden` elements (a multiple of 128);
-// each destination receives e4m3 codes in `outs.p[r]` and one fp32 scale per 128-element block
-// in `scales.p[r]` (rows x hidden / 128). With `stagedOut` / `stagedScales` set, `outs.p[r]` is
-// rank r's staging area and holds its codes, followed by its scales after capRows rows.
-void launchAlltoallvDevFp8(const CommArgs& a, const PeerPtrs& outs, const PeerPtrs& scales, const void* in,
-                           size_t inRows, size_t hidden, const long long* inSplits, long long* outSplits,
-                           long long* outOffsets, void* stagedOut, float* stagedScales, uint32_t capRows, int experts,
-                           int align, InputStatus* status, int blocks, cudaStream_t stream);
-// Top-k MoE combine, the mirror of the forward form: for each of `tokens` tokens, out row t =
-// sum over j < topk with pos[t, j] >= 0, in order, of weights[t, j] * (row pos[t, j] of my dispatch
-// input, as it lies on the rank holding its expert), in fp32, rounded to dt (float, bfloat16 or
-// float16). `splits` is my dispatch in_splits. `srcs.p[r]` is rank r's expert_out (zero copy) or
-// staging area; with `stagedIn` set (my plain expert_out) each rank first copies its rows there.
-void launchMoeCombineTopk(const CommArgs& a, const PeerPtrs& srcs, const void* stagedIn, void* out, size_t tokens,
-                          int topk, const long long* pos, const float* weights, const long long* splits, size_t rowBytes,
-                          DataType dt, uint32_t capRows, int experts, int align, InputStatus* status, int blocks,
-                          cudaStream_t stream);
-// Top-k MoE dispatch: route x's `tokens` rows by `idx` ((tokens, topk) int64; entry j·E + e =
-// local expert e of rank j, anything outside 0..P·E-1 is not routed) and push each to every
-// choice. Writes `splits` (P·E) and `pos` (tokens, topk) as route() does; out, outSplits and
-// outOffsets are those of the forward launchAlltoallvDev on route()'s rows. Rows are `rowBytes`
-// (a multiple of 16), x 16-byte aligned. `outs` / `stagedOut` as there.
-void launchMoeDispatchTopk(const CommArgs& a, const PeerPtrs& outs, const void* x, size_t tokens, int topk,
-                           const long long* idx, long long* splits, long long* pos, long long* outSplits,
-                           long long* outOffsets, void* stagedOut, size_t rowBytes, uint32_t capRows, int experts,
-                           int align, InputStatus* status, int blocks, cudaStream_t stream);
-// Its quantising form: x holds bf16 rows of `hidden` elements (a multiple of 128), each token is
-// quantised once and its codes and scales stored to every choice; `scales` / `stagedScales` as
-// in launchAlltoallvDevFp8.
-void launchMoeDispatchTopkFp8(const CommArgs& a, const PeerPtrs& outs, const PeerPtrs& scales, const void* x,
-                              size_t tokens, int topk, const long long* idx, long long* splits, long long* pos,
-                              long long* outSplits, long long* outOffsets, void* stagedOut, float* stagedScales,
-                              size_t hidden, uint32_t capRows, int experts, int align, InputStatus* status, int blocks,
-                              cudaStream_t stream);
 // Entry points, for occupancy queries (every CTA of a collective kernel must be resident).
-const void* alltoallvDevKernelPtr(bool fp8 = false);
-const void* moeCombineTopkKernelPtr(DataType dt);
-const void* moeDispatchTopkKernelPtr(bool fp8);
 const void* broadcastKernelPtr();
 const void* gatherPushKernelPtr();
 const void* alltoallPushKernelPtr();
@@ -152,6 +108,56 @@ const void* reducePullKernelPtr(DataType dt, int nranks);
 // everyone), 1 = alltoall (block j of my input to rank j). `bytes` per block, uniform.
 void launchLLExchange(const CommArgs& a, const void* in, void* out, size_t bytes, int mode, const PeerPtrs& ll,
                       size_t srcStride, size_t parityStride, int blocks, int threads, cudaStream_t stream);
+
+// moe_kernels.cu — device-split MoE exchange ----------------------------------------------------
+// What every form shares. `peers.p[r]` (the launchers' `outs` / `srcs`) is rank r's output
+// (dispatch) or expert_out (combine) in place, or its staging area when `plain` is set: my plain
+// output `staged` is then copied out of my staging area after the last push (dispatch), or my
+// plain expert_out into it before the first pull (combine).
+struct MoeArgs {
+  unsigned long long rowBytes;  // of an output row; quantising: H codes
+  char* staged;                 // null = zero copy (or an empty plain output)
+  InputStatus* status;          // host-mapped
+  uint32_t capRows;             // rows this rank's output can hold
+  int experts;
+  int align;
+  int plain;                    // the rows go through the staging areas: set even when `staged` is null
+};
+// The quantising dispatches' extension: each destination receives e4m3 codes and one fp32 scale
+// per 128-element block, rank r's in `scales.p[r]` (rows x H / 128), or, when `plain` is set, in
+// its staging area after capRows rows of codes; my plain out_scales `stagedScales` is copied from
+// there like `staged`. Which of the two a destination uses follows `plain`, never these pointers:
+// a plain tensor with no rows has a null data pointer.
+struct MoeScales {
+  PeerPtrs scales;      // zero copy only
+  float* stagedScales;  // plain only (null if it is empty)
+};
+struct MoeQuantArgs : MoeArgs, MoeScales {};
+
+// Device-split all-to-all-v: row counts come from device arrays (int64, P·E entries) and are
+// exchanged inside the kernel; see moe_kernels.cu for the two layouts. `scales` set: the
+// quantising forward form, `in` holding bf16 rows of rowBytes elements (a multiple of 128).
+void launchAlltoallvDev(const CommArgs& a, const PeerPtrs& outs, const MoeArgs& d, const MoeScales* scales,
+                        const void* in, size_t inRows, const long long* inSplits, const long long* inOffsets,
+                        long long* outSplits, long long* outOffsets, bool inverse, int blocks, cudaStream_t stream);
+// Top-k MoE combine, the mirror of the forward form: for each of `tokens` tokens, out row t =
+// sum over j < topk with pos[t, j] >= 0, in order, of weights[t, j] * (row pos[t, j] of my dispatch
+// input, as it lies on the rank holding its expert), in fp32, rounded to dt (float, bfloat16 or
+// float16). `splits` is my dispatch in_splits.
+void launchMoeCombineTopk(const CommArgs& a, const PeerPtrs& srcs, const MoeArgs& d, void* out, size_t tokens,
+                          int topk, const long long* pos, const float* weights, const long long* splits, DataType dt,
+                          int blocks, cudaStream_t stream);
+// Top-k MoE dispatch: route x's `tokens` rows by `idx` ((tokens, topk) int64; entry j·E + e =
+// local expert e of rank j, anything outside 0..P·E-1 is not routed) and push each to every
+// choice. Writes `splits` (P·E) and `pos` (tokens, topk) as route() does; out, outSplits and
+// outOffsets are those of the forward launchAlltoallvDev on route()'s rows. Rows are a multiple
+// of 16 bytes, x 16-byte aligned. `scales` set: the quantising form, each token quantised once.
+void launchMoeDispatchTopk(const CommArgs& a, const PeerPtrs& outs, const MoeArgs& d, const MoeScales* scales,
+                           const void* x, size_t tokens, int topk, const long long* idx, long long* splits,
+                           long long* pos, long long* outSplits, long long* outOffsets, int blocks, cudaStream_t stream);
+const void* alltoallvDevKernelPtr(bool fp8 = false);
+const void* moeCombineTopkKernelPtr(DataType dt);
+const void* moeDispatchTopkKernelPtr(bool fp8);
 
 // p2p_kernels.cu — point-to-point between two ranks through the receiver's mailbox ring.
 // sendBytes == 0 / recvBytes == 0 disables that role; both set = fused send+recv (one launch).

@@ -189,6 +189,7 @@ PeerContext::PeerContext(std::shared_ptr<Context> context, int dev, PeerOptions 
   // Load every kernel now, while no peer can be spinning on this device yet.
   preloadAllreduceKernels();
   preloadCollectiveKernels();
+  preloadMoeKernels();
   preloadScheduleKernels();
   preloadLocalKernels();
   preloadPipelineKernels();

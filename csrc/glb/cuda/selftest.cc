@@ -32,6 +32,16 @@ struct DevBuf {
   DevBuf(const DevBuf&) = delete;
 };
 
+MoeArgs moeArgs(size_t rowBytes, size_t cap, int experts, int align, InputStatus* status) {
+  MoeArgs d{};
+  d.rowBytes = rowBytes;
+  d.status = status;
+  d.capRows = static_cast<uint32_t>(cap);
+  d.experts = experts;
+  d.align = align;
+  return d;
+}
+
 void shareOfHost(size_t n, int parts, int r, size_t& b, size_t& e) {
   const size_t base = n / parts, rem = n % parts;
   b = r * base + std::min<size_t>(r, rem);
@@ -305,9 +315,9 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
       GLB_CUDA_CHECK(cudaMemcpyAsync(splits.p, sp.data(), K * 8, cudaMemcpyHostToDevice, stream));
       for (int r = 0; r < P; r++) GLB_CUDA_CHECK(cudaMemsetAsync(pp.p[r], 0xff, n * 4, stream));
       const int blocks = std::min(pc.coResidentBlocks(alltoallvDevKernelPtr()), 16);
-      launchAlltoallvDev(ca, pp, in.p, pre[K], rb, static_cast<const long long*>(splits.p), nullptr,
-                         static_cast<long long*>(outSplits.p), static_cast<long long*>(outOffsets.p), nullptr,
-                         static_cast<uint32_t>(cap), E, A, false, pc.inputStatusDevice(), blocks, stream);
+      launchAlltoallvDev(ca, pp, moeArgs(rb, cap, E, A, pc.inputStatusDevice()), nullptr, in.p, pre[K],
+                         static_cast<const long long*>(splits.p), nullptr, static_cast<long long*>(outSplits.p),
+                         static_cast<long long*>(outOffsets.p), false, blocks, stream);
       noteLaunch();
       std::vector<int64_t> os(K), oo(K);
       GLB_CUDA_CHECK(cudaMemcpyAsync(os.data(), outSplits.p, K * 8, cudaMemcpyDeviceToHost, stream));
@@ -342,9 +352,9 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
       PeerPtrs bp = pp;
       bp.p[0] = back.p;
       GLB_CUDA_CHECK(cudaMemsetAsync(back.p, 0, n * 4, stream));
-      launchAlltoallvDev(ca, bp, pp.p[0], cap, rb, static_cast<const long long*>(outSplits.p),
-                         static_cast<const long long*>(outOffsets.p), nullptr, nullptr, nullptr,
-                         static_cast<uint32_t>(cap), E, 1, true, pc.inputStatusDevice(), blocks, stream);
+      launchAlltoallvDev(ca, bp, moeArgs(rb, cap, E, 1, pc.inputStatusDevice()), nullptr, pp.p[0], cap,
+                         static_cast<const long long*>(outSplits.p), static_cast<const long long*>(outOffsets.p),
+                         nullptr, nullptr, true, blocks, stream);
       noteLaunch();
       auto h = download(back.p, n, stream);
       for (int64_t i = 0; i < pre[E] * 3; i++) {
@@ -397,9 +407,10 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
         GLB_CUDA_CHECK(cudaMemcpyAsync(in.p, rows.data(), rows.size() * 2, cudaMemcpyHostToDevice, stream));
         GLB_CUDA_CHECK(cudaMemcpyAsync(splits.p, sp.data(), K * 8, cudaMemcpyHostToDevice, stream));
         const int blocks = std::min(pc.coResidentBlocks(alltoallvDevKernelPtr(true)), 16);
-        launchAlltoallvDevFp8(ca, pp, sc, in.p, pre[K], H, static_cast<const long long*>(splits.p),
-                              static_cast<long long*>(outSplits.p), static_cast<long long*>(outOffsets.p), nullptr,
-                              nullptr, static_cast<uint32_t>(cap), E, A, pc.inputStatusDevice(), blocks, stream);
+        const MoeScales scales{sc, nullptr};
+        launchAlltoallvDev(ca, pp, moeArgs(H, cap, E, A, pc.inputStatusDevice()), &scales, in.p, pre[K],
+                           static_cast<const long long*>(splits.p), nullptr, static_cast<long long*>(outSplits.p),
+                           static_cast<long long*>(outOffsets.p), false, blocks, stream);
         noteLaunch();
         std::vector<int64_t> os(K), oo(K);
         GLB_CUDA_CHECK(cudaMemcpyAsync(os.data(), outSplits.p, K * 8, cudaMemcpyDeviceToHost, stream));
@@ -498,15 +509,10 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
           }
           const int blocks = std::min(pc.coResidentBlocks(moeDispatchTopkKernelPtr(fp8)), 16);
           auto ll = [](DevBuf& b) { return static_cast<long long*>(b.p); };
-          if (fp8) {
-            launchMoeDispatchTopkFp8(ca, pp, sc, x.p, T, topk, ll(idxDev), ll(splits), ll(posDev), ll(outSplits),
-                                     ll(outOffsets), nullptr, nullptr, H, static_cast<uint32_t>(cap), E, A,
-                                     pc.inputStatusDevice(), blocks, stream);
-          } else {
-            launchMoeDispatchTopk(ca, pp, x.p, T, topk, ll(idxDev), ll(splits), ll(posDev), ll(outSplits),
-                                  ll(outOffsets), nullptr, rb, static_cast<uint32_t>(cap), E, A, pc.inputStatusDevice(),
-                                  blocks, stream);
-          }
+          const MoeScales scales{sc, nullptr};
+          launchMoeDispatchTopk(ca, pp, moeArgs(rb, cap, E, A, pc.inputStatusDevice()),
+                                fp8 ? &scales : nullptr, x.p, T, topk, ll(idxDev), ll(splits), ll(posDev),
+                                ll(outSplits), ll(outOffsets), blocks, stream);
           noteLaunch();
           std::vector<int64_t> gs(K), gp(T * topk), os(K), oo(K);
           GLB_CUDA_CHECK(cudaMemcpyAsync(gs.data(), splits.p, K * 8, cudaMemcpyDeviceToHost, stream));
@@ -601,10 +607,9 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
         GLB_CUDA_CHECK(cudaMemcpyAsync(wDev.p, w.data(), w.size() * 4, cudaMemcpyHostToDevice, stream));
         GLB_CUDA_CHECK(cudaMemsetAsync(out.p, 0xff, T * rb, stream));
         const int blocks = std::min(pc.coResidentBlocks(moeCombineTopkKernelPtr(DataType::BFLOAT16)), 16);
-        launchMoeCombineTopk(ca, pp, nullptr, out.p, T, topk, static_cast<const long long*>(posDev.p),
-                             static_cast<const float*>(wDev.p), static_cast<const long long*>(splits.p), rb,
-                             DataType::BFLOAT16, static_cast<uint32_t>(cap), E, A, pc.inputStatusDevice(), blocks,
-                             stream);
+        launchMoeCombineTopk(ca, pp, moeArgs(rb, cap, E, A, pc.inputStatusDevice()), out.p, T, topk,
+                             static_cast<const long long*>(posDev.p), static_cast<const float*>(wDev.p),
+                             static_cast<const long long*>(splits.p), DataType::BFLOAT16, blocks, stream);
         noteLaunch();
         std::vector<uint16_t> got(T * H);
         GLB_CUDA_CHECK(cudaMemcpyAsync(got.data(), out.p, T * rb, cudaMemcpyDeviceToHost, stream));

@@ -21,6 +21,11 @@ std::vector<void*> ptrs(const std::vector<uintptr_t>& v) {
   for (auto p : v) o.push_back(P(p));
   return o;
 }
+// A registered buffer at an offset, or (None) a plain device pointer.
+MoeOut moeOut(const py::object& buf, size_t off, uintptr_t ptr) {
+  if (buf.is_none()) return MoeOut{nullptr, 0, P(ptr)};
+  return MoeOut{buf.cast<const PeerBuffer*>(), off, nullptr};
+}
 std::vector<cudaStream_t> streams(const std::vector<uintptr_t>& v) {
   std::vector<cudaStream_t> o;
   for (auto s : v) o.push_back(S(s));
@@ -175,107 +180,47 @@ void registerCudaAlgorithms(py::module_& m) {
     py::gil_scoped_release nogil;
     alltoallv(pc, P(in), sendBytes, P(out), recvBytes, S(st));
   });
-  // Device-split all-to-all-v. Splits / offsets are addresses of int64 device arrays (0 = none);
-  // `buf` is the registered output (None: `out` is a plain device pointer, staged).
+  // Device-split MoE exchange. Splits, offsets, pos and weights are addresses of device arrays
+  // (0 = none). `buf` is the registered output / expert_out at `buf_offset` (None: `out` /
+  // `expert_out` is a plain device pointer, staged); `quant` selects the quantising form, whose
+  // scales are given the same way by `scales_buf`, `scales_offset` and `out_scales`.
   m.def("alltoallv_dev", [](PeerContext& pc, uintptr_t in, size_t inRows, size_t rowBytes, uintptr_t inSplits,
                             uintptr_t inOffsets, py::object buf, size_t off, uintptr_t out, size_t capacityRows,
                             uintptr_t outSplits, uintptr_t outOffsets, int experts, int align, bool inverse,
-                            uintptr_t st) {
-    const PeerBuffer* reg = buf.is_none() ? nullptr : buf.cast<const PeerBuffer*>();
-    auto* is = reinterpret_cast<const int64_t*>(inSplits);
-    auto* io = reinterpret_cast<const int64_t*>(inOffsets);
-    auto* os = reinterpret_cast<int64_t*>(outSplits);
-    auto* oo = reinterpret_cast<int64_t*>(outOffsets);
+                            bool quant, py::object scalesBuf, size_t scalesOff, uintptr_t outScales, uintptr_t st) {
+    const MoeOut o = moeOut(buf, off, out), so = moeOut(scalesBuf, scalesOff, outScales);
     py::gil_scoped_release nogil;
-    if (reg != nullptr) {
-      alltoallvDev(pc, P(in), inRows, rowBytes, is, io, *reg, off, capacityRows, os, oo, experts, align, inverse, S(st));
-    } else {
-      alltoallvDev(pc, P(in), inRows, rowBytes, is, io, P(out), capacityRows, os, oo, experts, align, inverse, S(st));
-    }
+    alltoallvDev(pc, P(in), inRows, rowBytes, reinterpret_cast<const int64_t*>(inSplits),
+                 reinterpret_cast<const int64_t*>(inOffsets), o, capacityRows, reinterpret_cast<int64_t*>(outSplits),
+                 reinterpret_cast<int64_t*>(outOffsets), experts, align, inverse, S(st), quant ? &so : nullptr);
   }, py::arg("pc"), py::arg("input"), py::arg("in_rows"), py::arg("row_bytes"), py::arg("in_splits"),
      py::arg("in_offsets"), py::arg("buf"), py::arg("buf_offset"), py::arg("out"), py::arg("capacity_rows"),
      py::arg("out_splits"), py::arg("out_offsets"), py::arg("experts"), py::arg("align"), py::arg("inverse"),
-     py::arg("stream"));
-  // Its quantising forward form (bf16 rows of `hidden` elements -> e4m3 codes + fp32 block scales).
-  // `buf` / `scales_buf` are the registered outputs (both None: `out` / `out_scales` are plain
-  // device pointers, staged).
-  m.def("alltoallv_dev_fp8", [](PeerContext& pc, uintptr_t in, size_t inRows, size_t hidden, uintptr_t inSplits,
-                                py::object buf, size_t off, uintptr_t out, py::object scalesBuf, size_t scalesOff,
-                                uintptr_t outScales, size_t capacityRows, uintptr_t outSplits, uintptr_t outOffsets,
-                                int experts, int align, uintptr_t st) {
-    GLB_ENFORCE(buf.is_none() == scalesBuf.is_none(),
-                "alltoallv_dev: out and out_scales must both be registered or both be plain");
-    const PeerBuffer* reg = buf.is_none() ? nullptr : buf.cast<const PeerBuffer*>();
-    const PeerBuffer* sreg = scalesBuf.is_none() ? nullptr : scalesBuf.cast<const PeerBuffer*>();
-    auto* is = reinterpret_cast<const int64_t*>(inSplits);
-    auto* os = reinterpret_cast<int64_t*>(outSplits);
-    auto* oo = reinterpret_cast<int64_t*>(outOffsets);
-    py::gil_scoped_release nogil;
-    if (reg != nullptr) {
-      alltoallvDevFp8(pc, P(in), inRows, hidden, is, *reg, off, *sreg, scalesOff, capacityRows, os, oo, experts, align,
-                      S(st));
-    } else {
-      alltoallvDevFp8(pc, P(in), inRows, hidden, is, P(out), reinterpret_cast<float*>(outScales), capacityRows, os, oo,
-                      experts, align, S(st));
-    }
-  }, py::arg("pc"), py::arg("input"), py::arg("in_rows"), py::arg("hidden"), py::arg("in_splits"), py::arg("buf"),
-     py::arg("buf_offset"), py::arg("out"), py::arg("scales_buf"), py::arg("scales_offset"), py::arg("out_scales"),
-     py::arg("capacity_rows"), py::arg("out_splits"), py::arg("out_offsets"), py::arg("experts"), py::arg("align"),
-     py::arg("stream"));
-  // Top-k MoE dispatch. `buf` (and `scales_buf`, quantising) are the registered outputs (None:
-  // `out` / `out_scales` are plain device pointers, staged); `hidden` > 0 selects the quantising
-  // form (bf16 x of `hidden` elements a row), else rows are `row_bytes`.
+     py::arg("quant"), py::arg("scales_buf"), py::arg("scales_offset"), py::arg("out_scales"), py::arg("stream"));
   m.def("alltoallv_dev_topk", [](PeerContext& pc, uintptr_t x, size_t tokens, size_t rowBytes, int topk,
                                  uintptr_t topkIdx, uintptr_t splits, uintptr_t pos, py::object buf, size_t off,
                                  uintptr_t out, size_t capacityRows, uintptr_t outSplits, uintptr_t outOffsets,
-                                 int experts, int align, size_t hidden, py::object scalesBuf, size_t scalesOff,
+                                 int experts, int align, bool quant, py::object scalesBuf, size_t scalesOff,
                                  uintptr_t outScales, uintptr_t st) {
-    GLB_ENFORCE(buf.is_none() == scalesBuf.is_none() || hidden == 0,
-                "alltoallv_dev_topk: out and out_scales must both be registered or both be plain");
-    const PeerBuffer* reg = buf.is_none() ? nullptr : buf.cast<const PeerBuffer*>();
-    const PeerBuffer* sreg = scalesBuf.is_none() ? nullptr : scalesBuf.cast<const PeerBuffer*>();
-    auto* idx = reinterpret_cast<const int64_t*>(topkIdx);
-    auto* sp = reinterpret_cast<int64_t*>(splits);
-    auto* ps = reinterpret_cast<int64_t*>(pos);
-    auto* os = reinterpret_cast<int64_t*>(outSplits);
-    auto* oo = reinterpret_cast<int64_t*>(outOffsets);
+    const MoeOut o = moeOut(buf, off, out), so = moeOut(scalesBuf, scalesOff, outScales);
     py::gil_scoped_release nogil;
-    if (hidden > 0 && reg != nullptr) {
-      alltoallvDevTopkFp8(pc, P(x), tokens, hidden, topk, idx, sp, ps, *reg, off, *sreg, scalesOff, capacityRows, os,
-                          oo, experts, align, S(st));
-    } else if (hidden > 0) {
-      alltoallvDevTopkFp8(pc, P(x), tokens, hidden, topk, idx, sp, ps, P(out), reinterpret_cast<float*>(outScales),
-                          capacityRows, os, oo, experts, align, S(st));
-    } else if (reg != nullptr) {
-      alltoallvDevTopk(pc, P(x), tokens, rowBytes, topk, idx, sp, ps, *reg, off, capacityRows, os, oo, experts, align,
-                       S(st));
-    } else {
-      alltoallvDevTopk(pc, P(x), tokens, rowBytes, topk, idx, sp, ps, P(out), capacityRows, os, oo, experts, align,
-                       S(st));
-    }
+    alltoallvDevTopk(pc, P(x), tokens, rowBytes, topk, reinterpret_cast<const int64_t*>(topkIdx),
+                     reinterpret_cast<int64_t*>(splits), reinterpret_cast<int64_t*>(pos), o, capacityRows,
+                     reinterpret_cast<int64_t*>(outSplits), reinterpret_cast<int64_t*>(outOffsets), experts, align,
+                     S(st), quant ? &so : nullptr);
   }, py::arg("pc"), py::arg("x"), py::arg("tokens"), py::arg("row_bytes"), py::arg("topk"), py::arg("topk_idx"),
      py::arg("splits"), py::arg("pos"), py::arg("buf"), py::arg("buf_offset"), py::arg("out"),
      py::arg("capacity_rows"), py::arg("out_splits"), py::arg("out_offsets"), py::arg("experts"), py::arg("align"),
-     py::arg("hidden"), py::arg("scales_buf"), py::arg("scales_offset"), py::arg("out_scales"), py::arg("stream"));
-  // Top-k MoE combine. `buf` is the registered expert_out (None: `expert_out` is a plain device
-  // pointer, staged); pos / weights / splits are addresses of device arrays.
+     py::arg("quant"), py::arg("scales_buf"), py::arg("scales_offset"), py::arg("out_scales"), py::arg("stream"));
   m.def("alltoallv_dev_combine_topk", [](PeerContext& pc, uintptr_t out, size_t tokens, int topk, uintptr_t pos,
                                          uintptr_t weights, uintptr_t splits, py::object buf, size_t off,
                                          uintptr_t expertOut, size_t capacityRows, size_t rowBytes, int dtype,
                                          int experts, int align, uintptr_t st) {
-    const PeerBuffer* reg = buf.is_none() ? nullptr : buf.cast<const PeerBuffer*>();
-    auto* ps = reinterpret_cast<const int64_t*>(pos);
-    auto* ws = reinterpret_cast<const float*>(weights);
-    auto* sp = reinterpret_cast<const int64_t*>(splits);
-    const DataType dt = static_cast<DataType>(dtype);
+    const MoeOut eo = moeOut(buf, off, expertOut);
     py::gil_scoped_release nogil;
-    if (reg != nullptr) {
-      alltoallvDevCombineTopk(pc, P(out), tokens, topk, ps, ws, sp, *reg, off, capacityRows, rowBytes, dt, experts,
-                              align, S(st));
-    } else {
-      alltoallvDevCombineTopk(pc, P(out), tokens, topk, ps, ws, sp, P(expertOut), capacityRows, rowBytes, dt, experts,
-                              align, S(st));
-    }
+    alltoallvDevCombineTopk(pc, P(out), tokens, topk, reinterpret_cast<const int64_t*>(pos),
+                            reinterpret_cast<const float*>(weights), reinterpret_cast<const int64_t*>(splits), eo,
+                            capacityRows, rowBytes, static_cast<DataType>(dtype), experts, align, S(st));
   }, py::arg("pc"), py::arg("out"), py::arg("tokens"), py::arg("topk"), py::arg("pos"), py::arg("weights"),
      py::arg("splits"), py::arg("buf"), py::arg("buf_offset"), py::arg("expert_out"), py::arg("capacity_rows"),
      py::arg("row_bytes"), py::arg("dtype"), py::arg("experts"), py::arg("align"), py::arg("stream"));

@@ -361,6 +361,59 @@ class CudaContext:
                              f"cuda:{self.device}")
         return t.data_ptr()
 
+    def _dev_tensors(self, name: str, tensors, contiguous: bool = True) -> None:
+        """Every tensor of ``tensors`` (a name -> tensor mapping) is a CUDA tensor on this context's
+        device and, unless ``contiguous`` is False, contiguous."""
+        import torch
+
+        for what, t in tensors.items():
+            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
+                raise ValueError(f"{name}: {what} must be a CUDA tensor on cuda:{self.device}")
+            if contiguous and not t.is_contiguous():
+                raise ValueError(f"{name}: {what} must be contiguous")
+
+    @staticmethod
+    def _dev_disjoint(name: str, a, a_name: str, b, b_name: str) -> None:
+        """``a`` and ``b`` share no byte."""
+        a0, a1 = a.data_ptr(), a.data_ptr() + a.numel() * a.element_size()
+        b0, b1 = b.data_ptr(), b.data_ptr() + b.numel() * b.element_size()
+        if a0 < b1 and b0 < a1:
+            raise ValueError(f"{name}: {a_name} and {b_name} overlap")
+
+    def _fp8_dispatch(self, name: str, in_name: str, inp, out, out_scales):
+        """The quantising dispatch's tensors: ``inp`` bfloat16 ``(rows, H)`` with H a multiple of 128,
+        ``out`` float8_e4m3fn ``(cap, H)`` and ``out_scales`` float32 ``(cap, H // 128)``, contiguous
+        CUDA tensors on this device, ``inp`` and ``out`` 16-byte aligned. Returns H and the binding's
+        scales arguments (registration, offset, pointer)."""
+        import torch
+
+        form = (f"the quantising {name} takes bfloat16 {in_name} (rows, H) with H a multiple of 128, "
+                "float8_e4m3fn out (cap, H) and float32 out_scales (cap, H // 128)")
+        if out_scales is None:
+            raise ValueError(f"{name}: out_scales missing; {form}")
+        if inp.dtype != torch.bfloat16 or out.dtype != torch.float8_e4m3fn:
+            raise ValueError(f"{name}: got {inp.dtype} {in_name} and {out.dtype} out; {form}")
+        if not isinstance(out_scales, torch.Tensor) or out_scales.dtype != torch.float32:
+            raise ValueError(f"{name}: out_scales must be a float32 tensor; {form}")
+        tensors = (inp, out, out_scales)
+        if not all(t.is_cuda and t.device.index == self.device for t in tensors):
+            raise ValueError(f"{name}: {in_name}, out and out_scales must be CUDA tensors on cuda:{self.device}")
+        if inp.dim() != 2 or out.dim() != 2 or out_scales.dim() != 2:
+            raise ValueError(f"{name}: {in_name} {tuple(inp.shape)}, out {tuple(out.shape)} and out_scales "
+                             f"{tuple(out_scales.shape)} must be 2-D; {form}")
+        H, cap = int(inp.shape[1]), int(out.shape[0])
+        if H == 0 or H % 128 != 0:
+            raise ValueError(f"{name}: row length {H} is not a positive multiple of 128; {form}")
+        if int(out.shape[1]) != H or tuple(out_scales.shape) != (cap, H // 128):
+            raise ValueError(f"{name}: out {tuple(out.shape)} and out_scales {tuple(out_scales.shape)} do not "
+                             f"match {in_name} rows of {H}; {form}")
+        if not all(t.is_contiguous() for t in tensors):
+            raise ValueError(f"{name}: {in_name}, out and out_scales must be contiguous")
+        if inp.data_ptr() % 16 != 0 or out.data_ptr() % 16 != 0:
+            raise ValueError(f"{name}: {in_name} and out must be 16-byte aligned for the quantising form")
+        sbuf, soff = self.lookup(out_scales)
+        return H, sbuf, soff, out_scales.data_ptr()
+
     def alltoallv_dev(self, out, inp, in_splits, out_splits, out_offsets, experts: int = 1, align: int = 1,
                       out_scales=None, stream=None):
         """All-to-all-v whose row counts stay on the device: no host synchronisation, graph-capturable.
@@ -390,17 +443,20 @@ class CudaContext:
         ``out`` must be 16-byte aligned, and ``out`` and ``out_scales`` both registered / symmetric
         (zero copy) or both plain (staged; the capacity is then also capped by what fits the pool at
         H + H / 32 bytes a row). Other dtype pairs (other inputs, e5m2) raise ``ValueError``."""
-        if out_scales is not None or self._is_fp8_dispatch(out, inp):
-            return self._alltoallv_dev_fp8(out, inp, in_splits, out_splits, out_offsets, experts, align, out_scales,
-                                           stream)
-        rb = self._dev_rows(out, inp)
+        quant = out_scales is not None or self._is_fp8_dispatch(out, inp)
+        sbuf, soff, sptr = None, 0, 0
+        if quant:
+            rb, sbuf, soff, sptr = self._fp8_dispatch("alltoallv_dev", "input", inp, out, out_scales)
+        else:
+            rb = self._dev_rows(out, inp)
         k = self.size * int(experts)
         si = self._dev_index(in_splits, "in_splits", k)
         so = self._dev_index(out_splits, "out_splits", k)
         oo = self._dev_index(out_offsets, "out_offsets", k)
         buf, off = self.lookup(out)
         _cu.alltoallv_dev(self.pc, inp.data_ptr(), int(inp.shape[0]), rb, si, 0, buf, off, out.data_ptr(),
-                          int(out.shape[0]), so, oo, int(experts), int(align), False, _stream(stream))
+                          int(out.shape[0]), so, oo, int(experts), int(align), False, quant, sbuf, soff, sptr,
+                          _stream(stream))
         return out
 
     @staticmethod
@@ -409,45 +465,6 @@ class CudaContext:
         import torch
 
         return (out.dtype in (torch.float8_e4m3fn, torch.float8_e5m2) and inp.dtype != out.dtype)
-
-    def _alltoallv_dev_fp8(self, out, inp, in_splits, out_splits, out_offsets, experts, align, out_scales, stream):
-        import torch
-
-        form = ("the quantising alltoallv_dev takes bfloat16 input (rows, H) with H a multiple of 128, "
-                "float8_e4m3fn out (cap, H) and float32 out_scales (cap, H // 128)")
-        if out_scales is None:
-            raise ValueError(f"alltoallv_dev: out_scales missing; {form}")
-        if inp.dtype != torch.bfloat16 or out.dtype != torch.float8_e4m3fn:
-            raise ValueError(f"alltoallv_dev: got {inp.dtype} input and {out.dtype} out; {form}")
-        if not isinstance(out_scales, torch.Tensor) or out_scales.dtype != torch.float32:
-            raise ValueError(f"alltoallv_dev: out_scales must be a float32 tensor; {form}")
-        tensors = (inp, out, out_scales)
-        if not all(t.is_cuda and t.device.index == self.device for t in tensors):
-            raise ValueError(f"alltoallv_dev: input, out and out_scales must be CUDA tensors on cuda:{self.device}")
-        if inp.dim() != 2 or out.dim() != 2 or out_scales.dim() != 2:
-            raise ValueError(f"alltoallv_dev: input {tuple(inp.shape)}, out {tuple(out.shape)} and out_scales "
-                             f"{tuple(out_scales.shape)} must be 2-D; {form}")
-        H, cap = int(inp.shape[1]), int(out.shape[0])
-        if H == 0 or H % 128 != 0:
-            raise ValueError(f"alltoallv_dev: row length {H} is not a positive multiple of 128; {form}")
-        if int(out.shape[1]) != H or tuple(out_scales.shape) != (cap, H // 128):
-            raise ValueError(f"alltoallv_dev: out {tuple(out.shape)} and out_scales {tuple(out_scales.shape)} do not "
-                             f"match input rows of {H}; {form}")
-        if not all(t.is_contiguous() for t in tensors):
-            raise ValueError("alltoallv_dev: input, out and out_scales must be contiguous")
-        if inp.data_ptr() % 16 != 0 or out.data_ptr() % 16 != 0:
-            raise ValueError("alltoallv_dev: input and out must be 16-byte aligned for the quantising form")
-        buf, off = self.lookup(out)
-        sbuf, soff = self.lookup(out_scales)
-        if (buf is None) != (sbuf is None):
-            raise ValueError("alltoallv_dev: out and out_scales must both be registered / symmetric or both plain")
-        k = self.size * int(experts)
-        si = self._dev_index(in_splits, "in_splits", k)
-        so = self._dev_index(out_splits, "out_splits", k)
-        oo = self._dev_index(out_offsets, "out_offsets", k)
-        _cu.alltoallv_dev_fp8(self.pc, inp.data_ptr(), int(inp.shape[0]), H, si, buf, off, out.data_ptr(), sbuf, soff,
-                              out_scales.data_ptr(), cap, so, oo, int(experts), int(align), _stream(stream))
-        return out
 
     def alltoallv_dev_combine(self, out, inp, in_splits, in_offsets, experts: int = 1, stream=None):
         """Inverse of :meth:`alltoallv_dev`: ``inp`` is laid out as a dispatch output, described by
@@ -460,7 +477,7 @@ class CudaContext:
         io = self._dev_index(in_offsets, "in_offsets", k)
         buf, off = self.lookup(out)
         _cu.alltoallv_dev(self.pc, inp.data_ptr(), int(inp.shape[0]), rb, si, io, buf, off, out.data_ptr(),
-                          int(out.shape[0]), 0, 0, int(experts), 1, True, _stream(stream))
+                          int(out.shape[0]), 0, 0, int(experts), 1, True, False, None, 0, 0, _stream(stream))
         return out
 
     def alltoallv_dev_combine_topk(self, out, expert_out, splits, pos, weights, experts: int = 1, align: int = 1,
@@ -494,12 +511,7 @@ class CudaContext:
 
         name = "alltoallv_dev_combine_topk"
         dtypes = (torch.float32, torch.bfloat16, torch.float16)
-        tensors = {"out": out, "expert_out": expert_out, "pos": pos, "weights": weights}
-        for what, t in tensors.items():
-            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
-                raise ValueError(f"{name}: {what} must be a CUDA tensor on cuda:{self.device}")
-            if not t.is_contiguous():
-                raise ValueError(f"{name}: {what} must be contiguous")
+        self._dev_tensors(name, {"out": out, "expert_out": expert_out, "pos": pos, "weights": weights})
         if expert_out.dtype not in dtypes or out.dtype != expert_out.dtype:
             raise ValueError(f"{name}: expert_out and out must share a dtype of float32, bfloat16 or float16, got "
                              f"{expert_out.dtype} and {out.dtype}")
@@ -519,10 +531,7 @@ class CudaContext:
             raise ValueError(f"{name}: rows of {rb} bytes; a positive multiple of 16 is required")
         if expert_out.data_ptr() % 16 != 0 or out.data_ptr() % 16 != 0:
             raise ValueError(f"{name}: expert_out and out must be 16-byte aligned")
-        e0, e1 = expert_out.data_ptr(), expert_out.data_ptr() + expert_out.numel() * expert_out.element_size()
-        o0, o1 = out.data_ptr(), out.data_ptr() + out.numel() * out.element_size()
-        if e0 < o1 and o0 < e1:
-            raise ValueError(f"{name}: out and expert_out overlap")
+        self._dev_disjoint(name, out, "out", expert_out, "expert_out")
         if not 1 <= int(experts) <= 32 or int(align) < 1:
             raise ValueError(f"{name}: experts must be in 1..32 and align at least 1, got {experts} and {align}")
         si = self._dev_index(splits, "splits", self.size * int(experts))
@@ -574,10 +583,10 @@ class CudaContext:
         G = self.size * int(experts)
         if not 1 <= int(experts) <= 32 or int(align) < 1:
             raise ValueError(f"{name}: experts must be in 1..32 and align at least 1, got {experts} and {align}")
-        named = (("x", x), ("out", out), ("topk_idx", topk_idx), ("pos", pos))
-        for what, t in named:
-            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
-                raise ValueError(f"{name}: {what} must be a CUDA tensor on cuda:{self.device}")
+        named = {"x": x, "out": out, "topk_idx": topk_idx, "pos": pos}
+        # Device first and contiguity after the shape checks, so that the T * k limit is reported
+        # for broadcast views of any size.
+        self._dev_tensors(name, named, contiguous=False)
         if topk_idx.dtype != torch.int64 or topk_idx.dim() != 2 or x.dim() < 1 or topk_idx.shape[0] != x.shape[0]:
             raise ValueError(f"{name}: topk_idx must be int64 (T, k) with T = x.shape[0], got {topk_idx.dtype} "
                              f"{tuple(topk_idx.shape)} for x {tuple(x.shape)}")
@@ -588,49 +597,24 @@ class CudaContext:
             raise ValueError(f"{name}: T * k = {T * k} choices; at most 2^31 - 1 are supported")
         if pos.dtype != torch.int64 or tuple(pos.shape) != (T, k):
             raise ValueError(f"{name}: pos must be int64 {(T, k)}, got {pos.dtype} {tuple(pos.shape)}")
-        for what, t in named:
-            if not t.is_contiguous():
-                raise ValueError(f"{name}: {what} must be contiguous")
+        self._dev_tensors(name, named)
         si = self._dev_index(splits, "splits", G)
         so = self._dev_index(out_splits, "out_splits", G)
         oo = self._dev_index(out_offsets, "out_offsets", G)
-        hidden, sbuf, soff, sptr = 0, None, 0, 0
-        if out_scales is not None or self._is_fp8_dispatch(out, x):
-            form = ("the quantising alltoallv_dev_topk takes bfloat16 x (T, H) with H a multiple of 128, "
-                    "float8_e4m3fn out (cap, H) and float32 out_scales (cap, H // 128)")
-            if out_scales is None:
-                raise ValueError(f"{name}: out_scales missing; {form}")
-            if x.dtype != torch.bfloat16 or out.dtype != torch.float8_e4m3fn:
-                raise ValueError(f"{name}: got {x.dtype} x and {out.dtype} out; {form}")
-            if (not isinstance(out_scales, torch.Tensor) or out_scales.dtype != torch.float32 or not out_scales.is_cuda
-                    or out_scales.device.index != self.device or not out_scales.is_contiguous()):
-                raise ValueError(f"{name}: out_scales must be a contiguous float32 tensor on cuda:{self.device}; {form}")
-            if x.dim() != 2 or out.dim() != 2 or out_scales.dim() != 2:
-                raise ValueError(f"{name}: x, out and out_scales must be 2-D; {form}")
-            hidden = int(x.shape[1])
-            if hidden == 0 or hidden % 128 != 0:
-                raise ValueError(f"{name}: row length {hidden} is not a positive multiple of 128; {form}")
-            if int(out.shape[1]) != hidden or tuple(out_scales.shape) != (int(out.shape[0]), hidden // 128):
-                raise ValueError(f"{name}: out {tuple(out.shape)} and out_scales {tuple(out_scales.shape)} do not "
-                                 f"match rows of {hidden}; {form}")
-            rb = hidden
-            sbuf, soff = self.lookup(out_scales)
-            sptr = out_scales.data_ptr()
+        quant = out_scales is not None or self._is_fp8_dispatch(out, x)
+        sbuf, soff, sptr = None, 0, 0
+        if quant:
+            rb, sbuf, soff, sptr = self._fp8_dispatch(name, "x", x, out, out_scales)
         else:
             rb = self._dev_rows(out, x)
             if rb % 16 != 0:
                 raise ValueError(f"{name}: rows of {rb} bytes; a positive multiple of 16 is required")
-        if x.data_ptr() % 16 != 0 or out.data_ptr() % 16 != 0:
-            raise ValueError(f"{name}: x and out must be 16-byte aligned")
-        x0, x1 = x.data_ptr(), x.data_ptr() + x.numel() * x.element_size()
-        o0, o1 = out.data_ptr(), out.data_ptr() + out.numel() * out.element_size()
-        if x0 < o1 and o0 < x1:
-            raise ValueError(f"{name}: out and x overlap")
+            if x.data_ptr() % 16 != 0 or out.data_ptr() % 16 != 0:
+                raise ValueError(f"{name}: x and out must be 16-byte aligned")
+        self._dev_disjoint(name, out, "out", x, "x")
         buf, off = self.lookup(out)
-        if hidden and (buf is None) != (sbuf is None):
-            raise ValueError(f"{name}: out and out_scales must both be registered / symmetric or both plain")
         _cu.alltoallv_dev_topk(self.pc, x.data_ptr(), T, rb, k, topk_idx.data_ptr(), si, pos.data_ptr(), buf, off,
-                               out.data_ptr(), int(out.shape[0]), so, oo, int(experts), int(align), hidden, sbuf, soff,
+                               out.data_ptr(), int(out.shape[0]), so, oo, int(experts), int(align), quant, sbuf, soff,
                                sptr, _stream(stream))
         return out
 

@@ -354,6 +354,103 @@ def test_overflow_and_invalid_input(symmetric):
     assert all(gb.spawn_threads(P, fn, cuda_device=0))
 
 
+@pytest.mark.gpu
+@pytest.mark.parametrize("fp8", [False, True])
+def test_mixed_registered_and_plain_out(fp8):
+    """Rank 0 passes a plain out (and out_scales) while its peer passes symmetric ones: the ranks
+    would push into different places, so the call is invalid input on every rank, nothing moves,
+    and a correct call on the same context right after works."""
+    from test_moe_fp8_dispatch import _ref as _fp8_ref, _rows as _bf16_rows
+
+    gcu = _cuda()
+    P, E, align, H = 2, 2, 4, 256
+    sp = [[2, 1, 3, 0], [1, 0, 2, 2]]
+    caps = [_layout(sp, P, E, align, d)[2] + 3 for d in range(P)]
+
+    def fn(ctx):
+        cc = gcu.CudaContext(ctx, 0, stage_bytes=8 << 20)
+        me = ctx.rank
+        cap = caps[me]
+        sym = cc.empty(1 << 16, torch.uint8)
+        sym_scales = cc.empty(1 << 14, torch.uint8)
+        splits = torch.tensor(sp[me], dtype=torch.int64, device="cuda")
+        osp = torch.empty(P * E, dtype=torch.int64, device="cuda")
+        ooff = torch.empty_like(osp)
+        if fp8:
+            inputs = [_bf16_rows(sum(sp[s]), H, 40 + s) for s in range(P)]
+            want_codes, want_scales, _, _ = _fp8_ref(inputs, sp, P, E, align, me, cap)
+        else:
+            inputs = [_rows(torch.float32, 4, sum(sp[s]), 40 + s) for s in range(P)]
+            want_codes = _ref_dispatch(inputs, sp, P, E, align, me, cap)[0]
+        inp = inputs[me].cuda()
+
+        def outputs(symmetric):
+            if not fp8:
+                return _alloc(cc, sym, cap, 4, torch.float32, symmetric), None
+            out = _alloc(cc, sym, cap, H, torch.float8_e4m3fn, symmetric)
+            scales = _alloc(cc, sym_scales, cap, H // 128, torch.float32, symmetric)
+            return out, scales
+
+        out, scales = outputs(symmetric=me != 0)
+        before = [_bytes(t) for t in (out, scales) if t is not None]
+        cc.alltoallv_dev(out, inp, splits, osp, ooff, experts=E, align=align, out_scales=scales)
+        with pytest.raises(ValueError, match="invalid"):
+            cc.synchronize()
+        assert all(torch.equal(b, _bytes(t)) for b, t in zip(before, (out, scales)))
+        cc.pc.host_barrier()
+
+        out, scales = outputs(symmetric=True)
+        cc.alltoallv_dev(out, inp, splits, osp, ooff, experts=E, align=align, out_scales=scales)
+        cc.synchronize()
+        assert torch.equal(_bytes(out), want_codes)
+        if fp8:
+            assert torch.equal(_bytes(scales), want_scales)
+        return True
+
+    assert all(gb.spawn_threads(P, fn, cuda_device=0))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("fp8", [False, True])
+def test_empty_plain_out(fp8):
+    """Both ranks pass plain outputs and rank 1's has no rows (a null data pointer): nobody sends
+    it anything, while it still sends its own rows to rank 0. The call is valid and rank 0 gets
+    every row, with its scales in the quantising form."""
+    from test_moe_fp8_dispatch import _ref as _fp8_ref, _rows as _bf16_rows
+
+    gcu = _cuda()
+    P, E, H = 2, 2, 256
+    sp = [[2, 3, 0, 0], [1, 2, 0, 0]]
+    cap0 = _layout(sp, P, E, 1, 0)[2] + 3
+
+    def fn(ctx):
+        cc = gcu.CudaContext(ctx, 0, stage_bytes=8 << 20)
+        me = ctx.rank
+        cap = cap0 if me == 0 else 0
+        splits = torch.tensor(sp[me], dtype=torch.int64, device="cuda")
+        osp = torch.empty(P * E, dtype=torch.int64, device="cuda")
+        ooff = torch.empty_like(osp)
+        scales = None
+        if fp8:
+            inputs = [_bf16_rows(sum(sp[s]), H, 80 + s) for s in range(P)]
+            out = _alloc(cc, None, cap, H, torch.float8_e4m3fn, False)
+            scales = _alloc(cc, None, cap, H // 128, torch.float32, False)
+        else:
+            inputs = [_rows(torch.float32, 4, sum(sp[s]), 80 + s) for s in range(P)]
+            out = _alloc(cc, None, cap, 4, torch.float32, False)
+        cc.alltoallv_dev(out, inputs[me].cuda(), splits, osp, ooff, experts=E, out_scales=scales)
+        cc.synchronize()
+        assert osp.tolist() == _layout(sp, P, E, 1, me)[0]
+        if me == 0 and fp8:
+            want_codes, want_scales, _, _ = _fp8_ref(inputs, sp, P, E, 1, 0, cap)
+            assert torch.equal(_bytes(out), want_codes) and torch.equal(_bytes(scales), want_scales)
+        elif me == 0:
+            assert torch.equal(_bytes(out), _ref_dispatch(inputs, sp, P, E, 1, 0, cap)[0])
+        return True
+
+    assert all(gb.spawn_threads(P, fn, cuda_device=0))
+
+
 def _moe_expert(x, e_global):
     """A per-row expert (elementwise, so its result does not depend on how rows are batched)."""
     a = 0.5 + 0.125 * e_global

@@ -403,6 +403,64 @@ def test_no_host_sync(symmetric):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("fp8", [False, True])
+def test_empty_plain_out(fp8):
+    """Every rank passes a plain out and rank 1's has no rows (a null data pointer), as no token
+    chooses one of its experts; rank 1 still sends its own tokens. The call is valid and rank 0
+    receives route()'s rows. The copying form then combines from those outputs, rank 1's
+    expert_out still empty, and each rank gets the reference sum."""
+    from test_moe_fp8_dispatch import _ref as _fp8_ref
+
+    gcu = _cuda()
+    P, E, k, T, W, H = 2, 2, 2, 9, 4, 256
+
+    def problem(s):
+        g = torch.Generator().manual_seed(60 + s)
+        idx = torch.randint(0, E, (T, k), generator=g)  # experts of rank 0 only
+        idx[0, 1] = -1
+        x = torch.randn(T, H, generator=g).to(torch.bfloat16) if fp8 else torch.randn(T, W, generator=g)
+        w = torch.rand(T, k, generator=g)
+        return x, idx, w
+
+    probs = [problem(s) for s in range(P)]
+    routed = [_route(P, x, idx, E) for x, idx, _ in probs]
+    sp = [[int(c) for c in splits] for _, splits, _ in routed]
+    cap0 = _layout(sp, P, E, 1, 0)[2] + 3
+
+    def fn(ctx):
+        cc = gcu.CudaContext(ctx, 0, stage_bytes=8 << 20)
+        me = ctx.rank
+        cap = cap0 if me == 0 else 0
+        x, idx, w = (t.cuda() for t in probs[me])
+        out = torch.empty((cap, H if fp8 else W), dtype=torch.float8_e4m3fn if fp8 else torch.float32, device="cuda")
+        out.view(torch.uint8).fill_(SENTINEL)
+        scales = None
+        if fp8:
+            scales = torch.empty((cap, H // 128), dtype=torch.float32, device="cuda")
+            scales.view(torch.uint8).fill_(SENTINEL)
+        splits = torch.empty(P * E, dtype=torch.int64, device="cuda")
+        pos = torch.empty((T, k), dtype=torch.int64, device="cuda")
+        osp, ooff = torch.empty_like(splits), torch.empty_like(splits)
+        cc.alltoallv_dev_topk(out, x, idx, splits, pos, osp, ooff, experts=E, out_scales=scales)
+        cc.synchronize()
+        assert splits.tolist() == sp[me] and torch.equal(pos.cpu(), routed[me][2])
+        rows = [r for r, _, _ in routed]
+        if me == 0 and fp8:
+            want_codes, want_scales, _, _ = _fp8_ref(rows, sp, P, E, 1, 0, cap)
+            assert torch.equal(_bytes(out), want_codes) and torch.equal(_bytes(scales), want_scales)
+        elif me == 0:
+            assert torch.equal(_bytes(out), _ref_dispatch(rows, sp, P, E, 1, 0, cap)[0])
+        if not fp8:
+            res = torch.empty((T, W), device="cuda")
+            cc.alltoallv_dev_combine_topk(res, out, splits, pos, w, experts=E)
+            cc.synchronize()
+            assert torch.equal(res.cpu(), _reference(rows[me], routed[me][2], probs[me][2], torch.float32))
+        return True
+
+    assert all(gb.spawn_threads(P, fn, cuda_device=0))
+
+
+@pytest.mark.gpu
 def test_host_errors():
     """Every malformed call raises ValueError before launch, alike on every rank; a correct call
     afterwards works, so none of them launched."""
