@@ -888,6 +888,9 @@ void checkAligned16(const char* name, const void* a, const void* b, const char* 
 // against the registration, zero copy. Plain: staged through the pool's bulk region, where a row
 // takes rowBytes, plus its scales after the capacity's codes (hidden is a multiple of 128, so they
 // start 16-byte aligned); that caps the capacity.
+// The combine's backward adds a gradient buffer of expert_out's shape (`grad`), of the same kind:
+// registered, every rank's in place; plain, the rows after the staged expert_out's capacity in
+// each staging area, so a row then takes 2·rowBytes of the pool.
 struct MoeTarget {
   PeerPtrs peers;
   MoeScales scales;
@@ -895,14 +898,20 @@ struct MoeTarget {
   char* staged;      // my plain tensor (null if it is empty)
   bool plain;
   size_t capRows;
+  PeerPtrs grads;       // registered grad only
+  char* gradMine;       // my grad rows
 };
 
 MoeTarget resolveMoeOut(const PeerContext& pc, const char* name, const char* what, const MoeOut& out,
-                        const MoeOut* scales, size_t capacityRows, size_t rowBytes) {
+                        const MoeOut* scales, size_t capacityRows, size_t rowBytes, const MoeOut* grad = nullptr) {
   if (scales != nullptr && (out.buf == nullptr) != (scales->buf == nullptr)) {
     GLB_THROW(InputException, name, ": out and out_scales must both be registered / symmetric or both plain");
   }
+  if (grad != nullptr && (out.buf == nullptr) != (grad->buf == nullptr)) {
+    GLB_THROW(InputException, name, ": expert_out and grad_expert_out must both be registered / symmetric or both plain");
+  }
   const size_t scaleBytes = scales != nullptr ? rowBytes / kFp8Block * sizeof(float) : 0;
+  const size_t gradBytes = grad != nullptr ? rowBytes : 0;
   MoeTarget t{};
   if (out.buf != nullptr) {
     GLB_ENFORCE_LE(out.offset + capacityRows * rowBytes, out.buf->bytes, name, ": ", what,
@@ -910,6 +919,12 @@ MoeTarget resolveMoeOut(const PeerContext& pc, const char* name, const char* wha
     t.peers = out.buf->ptrsAt(out.offset);
     t.mine = static_cast<const char*>(out.buf->local) + out.offset;
     t.capRows = capacityRows;
+    if (grad != nullptr) {
+      GLB_ENFORCE_LE(grad->offset + capacityRows * rowBytes, grad->buf->bytes, name,
+                     ": grad_expert_out exceeds the registered buffer");
+      t.grads = grad->buf->ptrsAt(grad->offset);
+      t.gradMine = static_cast<char*>(grad->buf->local) + grad->offset;
+    }
     if (scales != nullptr) {
       GLB_ENFORCE_LE(scales->offset + capacityRows * scaleBytes, scales->buf->bytes, name,
                      ": output scales exceed the registered buffer");
@@ -922,7 +937,8 @@ MoeTarget resolveMoeOut(const PeerContext& pc, const char* name, const char* wha
     t.mine = static_cast<const char*>(out.ptr);
     t.staged = static_cast<char*>(out.ptr);
     t.plain = true;
-    t.capRows = std::min(capacityRows, l.bulkBytes / (rowBytes + scaleBytes));
+    t.capRows = std::min(capacityRows, l.bulkBytes / (rowBytes + scaleBytes + gradBytes));
+    if (grad != nullptr) t.gradMine = static_cast<char*>(grad->ptr);
     if (scales != nullptr) {
       GLB_ENFORCE(reinterpret_cast<uintptr_t>(scales->ptr) % sizeof(float) == 0, name,
                   ": output scales must be 4-byte aligned");
@@ -1013,8 +1029,8 @@ void alltoallvDevCombineTopk(PeerContext& pc, void* out, size_t tokens, int topk
               ": rows must be float32, bfloat16 or float16");
   checkTopk(name, topk);
   checkMoeLimits(name, experts, align, rowBytes, 16);
-  GLB_ENFORCE(splits != nullptr && (tokens == 0 || (pos != nullptr && weights != nullptr && out != nullptr)),
-              name, ": missing splits, pos, weights or out");
+  GLB_ENFORCE(splits != nullptr && (tokens == 0 || (pos != nullptr && out != nullptr)), name,
+              ": missing splits, pos or out");
   // A plain expert_out is copied into my staging area, where my peers read it.
   const MoeTarget t = resolveMoeOut(pc, name, "expert_out", expertOut, nullptr, capacityRows, rowBytes);
   checkAligned16(name, out, t.mine, "out and expert_out");
@@ -1025,6 +1041,39 @@ void alltoallvDevCombineTopk(PeerContext& pc, void* out, size_t tokens, int topk
   launchMoeCombineTopk(pc.comm(), t.peers, moeArgs(pc, t, rowBytes, experts, align), out, tokens, topk,
                        reinterpret_cast<const long long*>(pos), weights, reinterpret_cast<const long long*>(splits), dt,
                        blocks, stream);
+  finish(pc, stream, name);
+}
+
+void alltoallvDevCombineTopkBackward(PeerContext& pc, const MoeOut& gradExpertOut, float* gradWeights,
+                                     const void* gradOut, const MoeOut& expertOut, size_t tokens, int topk,
+                                     const int64_t* pos, const float* weights, const int64_t* splits,
+                                     size_t capacityRows, size_t rowBytes, DataType dt, int experts, int align,
+                                     cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  GLB_TRACE_RANGE("glb::cuda::alltoallv_dev_combine_topk_backward");
+  const char* name = "alltoallv_dev_combine_topk_backward";
+  GLB_ENFORCE(dt == DataType::FLOAT32 || dt == DataType::BFLOAT16 || dt == DataType::FLOAT16, name,
+              ": rows must be float32, bfloat16 or float16");
+  checkTopk(name, topk);
+  checkMoeLimits(name, experts, align, rowBytes, 16);
+  GLB_ENFORCE(splits != nullptr &&
+                  (tokens == 0 || (pos != nullptr && weights != nullptr && gradOut != nullptr && gradWeights != nullptr)),
+              name, ": missing splits, pos, weights, grad_out or grad_weights");
+  // Plain expert_out and grad_expert_out both go through my staging area: rows, then gradient rows.
+  const MoeTarget t = resolveMoeOut(pc, name, "expert_out", expertOut, nullptr, capacityRows, rowBytes, &gradExpertOut);
+  checkAligned16(name, gradOut, t.mine, "grad_out and expert_out");
+  checkAligned16(name, t.gradMine, t.gradMine, "grad_expert_out");
+  // Peers write my grad_expert_out while I read my expert_out, grad_out and write grad_weights.
+  const size_t capBytes = capacityRows * rowBytes;
+  rejectOverlap(t.mine, capBytes, t.gradMine, capBytes, name);
+  rejectOverlap(gradOut, tokens * rowBytes, t.gradMine, capBytes, name);
+  rejectOverlap(gradWeights, tokens * topk * sizeof(float), t.gradMine, capBytes, name);
+  const int blocks = moeBlocks(pc, moeCombineTopkBackwardKernelPtr(dt));
+  prologue(pc, stream);
+  launchMoeCombineTopkBackward(pc.comm(), t.peers, t.plain ? t.peers : t.grads, moeArgs(pc, t, rowBytes, experts, align),
+                               t.plain ? t.gradMine : nullptr, capacityRows, gradOut, gradWeights, tokens, topk,
+                               reinterpret_cast<const long long*>(pos), weights,
+                               reinterpret_cast<const long long*>(splits), dt, blocks, stream);
   finish(pc, stream, name);
 }
 

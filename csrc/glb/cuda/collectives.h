@@ -197,10 +197,26 @@ void alltoallvDevTopk(PeerContext& pc, const void* x, size_t tokens, size_t rowB
 // through its pool, which caps the capacity. Rows must be a multiple of 16 bytes, expertOut and
 // out 16-byte aligned and disjoint, 1 <= topk <= 32. Errors found on the device (splits, a pos
 // out of range, arguments that differ between ranks, an overflowing holder) are raised like
-// alltoallvDev's, and no rank writes its out.
+// alltoallvDev's, and no rank writes its out. Null `weights`: every weight is 1 (the unweighted
+// sum, the backward of the top-k dispatch), byte for byte a call with a tensor of ones.
 void alltoallvDevCombineTopk(PeerContext& pc, void* out, size_t tokens, int topk, const int64_t* pos,
                              const float* weights, const int64_t* splits, const MoeOut& expertOut, size_t capacityRows,
                              size_t rowBytes, DataType dt, int experts, int align, cudaStream_t stream);
+// Backward of alltoallvDevCombineTopk, in one kernel, with its arguments and `gradOut` (dy, tokens
+// rows of dt). For each routed choice (t, j): gradWeights[t, j] = sum over h of float(dy[t, h]) ·
+// float(row[h]), in fp32 (+0 where pos = -1), and the holder's gradExpertOut row (same layout and
+// capacity as expertOut) = round(weights[t, j] · float(dy[t])), one correctly rounded multiply. Each
+// holder writes +0 to every gradExpertOut row outside its receive segments. expertOut and
+// gradExpertOut are both registered (zero copy) or both plain (staged: each rank's pool then holds
+// both, which caps the capacity at half that of the combine). gradExpertOut must not overlap
+// expertOut, gradOut or gradWeights. pos must name each dispatch-input row at most once. Errors
+// found on the device are raised like the combine's, and no rank writes gradExpertOut or
+// gradWeights.
+void alltoallvDevCombineTopkBackward(PeerContext& pc, const MoeOut& gradExpertOut, float* gradWeights,
+                                     const void* gradOut, const MoeOut& expertOut, size_t tokens, int topk,
+                                     const int64_t* pos, const float* weights, const int64_t* splits,
+                                     size_t capacityRows, size_t rowBytes, DataType dt, int experts, int align,
+                                     cudaStream_t stream);
 // Fixed-size alltoall: every chunk is `bytes` long on every rank (this is known to all
 // ranks, so the small-message LL kernel and size-dependent grids are safe here).
 void alltoall(PeerContext& pc, const void* in, const PeerBuffer& out, size_t outOffset, size_t bytes,

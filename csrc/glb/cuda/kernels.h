@@ -144,9 +144,20 @@ void launchAlltoallvDev(const CommArgs& a, const PeerPtrs& outs, const MoeArgs& 
 // sum over j < topk with pos[t, j] >= 0, in order, of weights[t, j] * (row pos[t, j] of my dispatch
 // input, as it lies on the rank holding its expert), in fp32, rounded to dt (float, bfloat16 or
 // float16). `splits` is my dispatch in_splits.
+// Null `weights`: every routed choice has weight 1 (the backward of the top-k dispatch).
 void launchMoeCombineTopk(const CommArgs& a, const PeerPtrs& srcs, const MoeArgs& d, void* out, size_t tokens,
                           int topk, const long long* pos, const float* weights, const long long* splits, DataType dt,
                           int blocks, cudaStream_t stream);
+// Its backward, run by the source with the combine's arguments and dy (tokens rows): for each routed
+// choice, gradWeights[t, j] = <dy[t], its expert row> in fp32 (+0 where pos = -1), and
+// round(weights[t, j] · dy[t]) pushed to the same row of the holder's grad_expert_out: `grads.p[r]`,
+// or, when `plain` is set, rank r's staging area after its capRows rows of staged expert_out, copied
+// out to my plain `stagedGrad` at the end. Each holder zeroes the rows of its grad_expert_out
+// (capacityRows) outside its receive segments.
+void launchMoeCombineTopkBackward(const CommArgs& a, const PeerPtrs& srcs, const PeerPtrs& grads, const MoeArgs& d,
+                                  void* stagedGrad, size_t capacityRows, const void* dy, float* gradWeights,
+                                  size_t tokens, int topk, const long long* pos, const float* weights,
+                                  const long long* splits, DataType dt, int blocks, cudaStream_t stream);
 // Top-k MoE dispatch: route x's `tokens` rows by `idx` ((tokens, topk) int64; entry j·E + e =
 // local expert e of rank j, anything outside 0..P·E-1 is not routed) and push each to every
 // choice. Writes `splits` (P·E) and `pos` (tokens, topk) as route() does; out, outSplits and
@@ -157,6 +168,7 @@ void launchMoeDispatchTopk(const CommArgs& a, const PeerPtrs& outs, const MoeArg
                            long long* pos, long long* outSplits, long long* outOffsets, int blocks, cudaStream_t stream);
 const void* alltoallvDevKernelPtr(bool fp8 = false);
 const void* moeCombineTopkKernelPtr(DataType dt);
+const void* moeCombineTopkBackwardKernelPtr(DataType dt);
 const void* moeDispatchTopkKernelPtr(bool fp8);
 
 // p2p_kernels.cu — point-to-point between two ranks through the receiver's mailbox ring.

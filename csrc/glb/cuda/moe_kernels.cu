@@ -33,7 +33,13 @@ constexpr int kMaxK = kMaxRanks * kMaxA2aExperts;
 // call as invalid, like differing row sizes. Bit 1 marks the quantising forms, bit 3 a staged
 // (plain) output or expert_out: a rank whose peers push into its registered buffer and a rank
 // whose peers push into its staging area would each write where the other does not read.
-enum class A2aForm : uint32_t { kForward = 0u, kInverse = 1u, kCombineTopk = 4u, kDispatchTopk = 16u };
+enum class A2aForm : uint32_t {
+  kForward = 0u,
+  kInverse = 1u,
+  kCombineTopk = 4u,
+  kDispatchTopk = 16u,
+  kCombineTopkBackward = 32u
+};
 __device__ __forceinline__ uint32_t a2aHeaderWord(A2aForm form, bool quant, bool staged) {
   return static_cast<uint32_t>(form) | (quant ? 2u : 0u) | (staged ? 8u : 0u);
 }
@@ -218,9 +224,23 @@ __device__ __forceinline__ void a2aForwardLayout(const SignalPad* pad, int P, in
   if (t < K) sDst[t] += sAux[t];
 }
 
-// The dispatches' layout: a2aForwardLayout, then my receive segment t = e·P + s (first row
-// sRcv[t], sRcvCnt[t] rows); CTA 0 reports the outcome and, when the call is valid and they are
-// given, stores the segments to outSplits / outOffsets.
+// After a2aForwardLayout: my receive segment t = e·P + s (first row sRcv[t], sRcvCnt[t] rows).
+__device__ __forceinline__ void a2aReceiveSegments(const SignalPad* pad, int P, int E, int me,
+                                                   const unsigned long long* sAux, unsigned long long* sRcv,
+                                                   uint32_t* sRcvCnt) {
+  const int t = threadIdx.x;
+  if (t < P * E) {
+    const int e = t / P, s = t % P;
+    unsigned long long off = sAux[me * E + e];
+    for (int s2 = 0; s2 < s; s2++) off += ldPad(&pad->a2aCount[me * E + e][s2]);
+    sRcv[t] = off;
+    sRcvCnt[t] = ldPad(&pad->a2aCount[me * E + e][s]);
+  }
+  __syncthreads();
+}
+
+// The dispatches' layout: a2aForwardLayout and a2aReceiveSegments; CTA 0 reports the outcome and,
+// when the call is valid and they are given, stores the segments to outSplits / outOffsets.
 __device__ __forceinline__ void a2aDispatchLayout(const CommArgs& a, bool ok1, bool invalid, const MoeArgs& d,
                                                   long long* outSplits, long long* outOffsets,
                                                   unsigned long long* sDst, unsigned long long* sAux,
@@ -230,14 +250,7 @@ __device__ __forceinline__ void a2aDispatchLayout(const CommArgs& a, bool ok1, b
   const SignalPad* pad = a.self;
   if (ok1 && !invalid) {
     a2aForwardLayout(pad, P, E, me, d.align, sDst, sAux, sNeed);
-    if (t < K) {
-      const int e = t / P, s = t % P;
-      unsigned long long off = sAux[me * E + e];
-      for (int s2 = 0; s2 < s; s2++) off += ldPad(&pad->a2aCount[me * E + e][s2]);
-      sRcv[t] = off;
-      sRcvCnt[t] = ldPad(&pad->a2aCount[me * E + e][s]);
-    }
-    __syncthreads();
+    a2aReceiveSegments(pad, P, E, me, sAux, sRcv, sRcvCnt);
   }
   if (ok1 && blockIdx.x == 0) {
     if (t == 0) a2aReport(d.status, invalid, P, sNeed, sCap);
@@ -251,7 +264,26 @@ __device__ __forceinline__ void a2aDispatchLayout(const CommArgs& a, bool ok1, b
 // ---- finish a dispatch: barrier 2, staged copy-out, retire --------------------------------------
 // A plain output is copied from my staging area (`stage`) once every CTA of every peer has pushed:
 // the forward forms segment by segment, so that alignment gaps of the output stay untouched (the
-// quantising forms' scales follow my capRows rows of codes there); the inverse form in one piece.
+// quantising forms' scales follow my `capRows` rows of codes there); the inverse form in one piece.
+// The segment-by-segment copy: rows of `rb` bytes from `stage` to `out`, and, quantising, their
+// scales from after `capRows` rows of codes in `stage` to `outScales`.
+template <bool kQuant>
+__device__ __forceinline__ void a2aCopyOut(char* out, float* outScales, const char* stage, unsigned long long rb,
+                                           unsigned long long capRows, int K, const unsigned long long* sRcv,
+                                           const uint32_t* sRcvCnt, size_t tid, size_t nthreads) {
+  for (int k = 0; k < K; k++) {
+    const unsigned long long n = sRcvCnt[k];
+    if (n > 0) gridCopy(out + sRcv[k] * rb, stage + sRcv[k] * rb, n * rb, true, tid, nthreads);
+    if constexpr (kQuant) {
+      const unsigned long long sb = rb / kFp8Block * sizeof(float);  // scale bytes per row
+      if (n > 0) {
+        gridCopy(reinterpret_cast<char*>(outScales) + sRcv[k] * sb, stage + capRows * rb + sRcv[k] * sb, n * sb, true,
+                 tid, nthreads);
+      }
+    }
+  }
+}
+
 template <bool kQuant>
 __device__ __forceinline__ void a2aFinish(const CommArgs& a, uint32_t ep, bool moved, const MoeKernelArgs<kQuant>& d,
                                           bool inverse, const unsigned long long* sRcv, const uint32_t* sRcvCnt,
@@ -271,17 +303,9 @@ __device__ __forceinline__ void a2aFinish(const CommArgs& a, uint32_t ep, bool m
       if (inverse) {
         gridCopy(d.staged, stage, sNeed[me] * rb, true, tid, nthreads);
       } else {
-        for (int k = 0; k < K; k++) {
-          const unsigned long long n = sRcvCnt[k];
-          if (n > 0) gridCopy(d.staged + sRcv[k] * rb, stage + sRcv[k] * rb, n * rb, true, tid, nthreads);
-          if constexpr (kQuant) {
-            const unsigned long long sb = rb / kFp8Block * sizeof(float);  // scale bytes per row
-            if (n > 0) {
-              gridCopy(reinterpret_cast<char*>(d.stagedScales) + sRcv[k] * sb, stage + sCap[me] * rb + sRcv[k] * sb,
-                       n * sb, true, tid, nthreads);
-            }
-          }
-        }
+        float* outScales = nullptr;
+        if constexpr (kQuant) outScales = d.stagedScales;
+        a2aCopyOut<kQuant>(d.staged, outScales, stage, rb, sCap[me], K, sRcv, sRcvCnt, tid, nthreads);
       }
     }
   }
@@ -531,22 +555,24 @@ void launchAlltoallvDev(const CommArgs& a, const PeerPtrs& outs, const MoeArgs& 
 //              published. The grid sync before it puts every local CTA's stores under CTA b's release:
 //              the barrier pairs CTA b with CTA b only.
 //   barrier 3  every rank has read its rows: holders may reuse expert_out and the staging area.
-// Every path passes all three barriers, so ranks never wait for a different count.
+// Every path passes all three barriers, so ranks never wait for a different count. The backward
+// below runs the same protocol up to the pull (topkPullPrologue) and the same choice lookup.
 constexpr int kTopkInFlight = 4;  // choices whose packs a lane loads before it adds them
 constexpr int kTopkPacks = 2;     // packs of one row per lane per step
 
-template <typename T>
-__global__ void __launch_bounds__(kThreads)
-moeCombineTopkKernel(CommArgs a, PeerPtrs srcs, const long long* splits, const long long* posIn, const float* weights,
-                     char* out, unsigned long long tokens, int topk, MoeArgs d) {
-  using PT = PackTraits<T>;
-  __shared__ unsigned long long sSrc[kMaxK];  // my chunk k: first row in my dispatch input
-  __shared__ unsigned long long sDst[kMaxK];  //             first row on its holder
-  __shared__ unsigned long long sAux[kMaxK];  // column sums, then expert bases
-  __shared__ unsigned long long sNeed[kMaxRanks], sCap[kMaxRanks];
-  __shared__ const char* sBase[kMaxRanks];
-  __shared__ unsigned long long sWarp[32];
-  const uint32_t ep = loadEpoch(a);
+namespace {
+// The pulling forms up to barrier 2 and its verdict: where each chunk of my dispatch input starts
+// (sSrc), every holder's expert_out (sBase), agree on `word`, the forward layout, a plain expert_out
+// (d.staged) copied into my staging area, my `choices` pos entries checked, the grid sync and
+// barrier 2, and every rank's verdict, which CTA 0 reports. Returns whether this rank may pull:
+// every rank's input is valid and no holder overflows.
+__device__ __forceinline__ bool topkPullPrologue(const CommArgs& a, uint32_t ep, const PeerPtrs& srcs,
+                                                 const long long* splits, const long long* posIn,
+                                                 unsigned long long choices, const MoeArgs& d, uint32_t word,
+                                                 unsigned long long* sSrc, unsigned long long* sDst,
+                                                 unsigned long long* sAux, unsigned long long* sNeed,
+                                                 unsigned long long* sCap, const char** sBase,
+                                                 unsigned long long* sWarp) {
   const int P = a.nranks, E = d.experts, K = P * E, me = a.rank, t = threadIdx.x;
   const unsigned long long rb = d.rowBytes;
   const size_t gtid = static_cast<size_t>(blockIdx.x) * blockDim.x + t;
@@ -561,8 +587,7 @@ moeCombineTopkKernel(CommArgs a, PeerPtrs srcs, const long long* splits, const l
   if (t < P) sBase[t] = static_cast<const char*>(srcs.p[t]);
   const bool localBad = __syncthreads_or(bad) != 0;
   bool invalid;
-  const bool ok1 = a2aAgree(a, ep, splits, d, a2aHeaderWord(A2aForm::kCombineTopk, false, d.plain != 0),
-                            localBad, true, sCap, invalid);
+  const bool ok1 = a2aAgree(a, ep, splits, d, word, localBad, true, sCap, invalid);
 
   // ---- 2. the layout; stage a plain expert_out; check pos ----
   const SignalPad* pad = a.self;
@@ -575,8 +600,7 @@ moeCombineTopkKernel(CommArgs a, PeerPtrs srcs, const long long* splits, const l
   if (go && d.staged != nullptr) gridCopy(const_cast<char*>(sBase[me]), d.staged, sNeed[me] * rb, true, gtid, gthreads);
   if (go) {
     bool b = false;
-    const unsigned long long n = tokens * static_cast<unsigned long long>(topk);
-    for (size_t i = gtid; i < n; i += gthreads) {
+    for (size_t i = gtid; i < choices; i += gthreads) {
       const long long p = posIn[i];
       b = b || p < -1 || (p >= 0 && static_cast<unsigned long long>(p) >= inRows);
     }
@@ -584,28 +608,63 @@ moeCombineTopkKernel(CommArgs a, PeerPtrs srcs, const long long* splits, const l
   }
   const bool ok2 = localGridSync(a) && blockBarrier(a, ep + 2);
 
-  // ---- 3. every rank's verdict; pull and reduce ----
+  // ---- 3. every rank's verdict ----
   bool posBad = false;
   if (ok2 && go) posBad = __syncthreads_or(t < P && ldPad(&pad->a2aPosBad[t]) != 0u) != 0;
   if (ok1 && ok2 && blockIdx.x == 0 && t == 0) a2aReport(d.status, invalid || posBad, P, sNeed, sCap);
-  if (ok2 && go && !posBad) {
+  return ok2 && go && !posBad;
+}
+
+// Where row p of my dispatch input lies: the last chunk starting at or before p holds it (an empty
+// chunk starts where the next one does); its holder is chunk / E, the row there is returned.
+__device__ __forceinline__ unsigned long long topkHolderRow(const unsigned long long* sSrc,
+                                                            const unsigned long long* sDst, int K, int E,
+                                                            unsigned long long p, int& holder) {
+  int lo = 0, hi = K - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (sSrc[mid] <= p) lo = mid; else hi = mid - 1;
+  }
+  holder = lo / E;
+  return sDst[lo] + (p - sSrc[lo]);
+}
+}  // namespace
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+moeCombineTopkKernel(CommArgs a, PeerPtrs srcs, const long long* splits, const long long* posIn, const float* weights,
+                     char* out, unsigned long long tokens, int topk, MoeArgs d) {
+  using PT = PackTraits<T>;
+  __shared__ unsigned long long sSrc[kMaxK];  // my chunk k: first row in my dispatch input
+  __shared__ unsigned long long sDst[kMaxK];  //             first row on its holder
+  __shared__ unsigned long long sAux[kMaxK];  // column sums, then expert bases
+  __shared__ unsigned long long sNeed[kMaxRanks], sCap[kMaxRanks];
+  __shared__ const char* sBase[kMaxRanks];
+  __shared__ unsigned long long sWarp[32];
+  const uint32_t ep = loadEpoch(a);
+  const int K = a.nranks * d.experts, t = threadIdx.x;
+  const unsigned long long rb = d.rowBytes;
+  const size_t gtid = static_cast<size_t>(blockIdx.x) * blockDim.x + t;
+  const size_t gthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
+
+  const bool pull = topkPullPrologue(a, ep, srcs, splits, posIn, tokens * static_cast<unsigned long long>(topk), d,
+                                     a2aHeaderWord(A2aForm::kCombineTopk, false, d.plain != 0), sSrc, sDst, sAux,
+                                     sNeed, sCap, sBase, sWarp);
+  // ---- pull and reduce ----
+  if (pull) {
     const int lane = t & 31, k = topk;
     const unsigned long long npk = rb / 16;
     for (unsigned long long tok = gtid / 32; tok < tokens; tok += gthreads / 32) {
-      // Lane j < k: where choice j's row lies. The last chunk starting at or before p holds it
-      // (an empty chunk starts where the next one does).
+      // Lane j < k: where choice j's row lies, and its weight (1 without weights).
       const char* src = nullptr;
       float w = 0.0f;
       if (lane < k) {
         const long long p = posIn[tok * k + lane];
         if (p >= 0) {
-          int lo = 0, hi = K - 1;
-          while (lo < hi) {
-            const int mid = (lo + hi + 1) >> 1;
-            if (sSrc[mid] <= static_cast<unsigned long long>(p)) lo = mid; else hi = mid - 1;
-          }
-          src = sBase[lo / E] + (sDst[lo] + (static_cast<unsigned long long>(p) - sSrc[lo])) * rb;
-          w = weights[tok * k + lane];
+          int j;
+          const unsigned long long row = topkHolderRow(sSrc, sDst, K, d.experts, static_cast<unsigned long long>(p), j);
+          src = sBase[j] + row * rb;
+          w = weights != nullptr ? weights[tok * k + lane] : 1.0f;
         }
       }
       char* dst = out + tok * rb;
@@ -657,6 +716,167 @@ moeCombineTopkKernel(CommArgs a, PeerPtrs srcs, const long long* splits, const l
   retire(a, 3, 0);
 }
 
+// ---- top-k MoE combine backward: pull, dot and push in one pass --------------------------------
+// The backward of the weighted combine y[t] = sum_j w[t, j] · expert_out[row(t, j)], run by the
+// source like the combine, with the same protocol up to the pull and the same (holder, row) of each
+// choice. For each routed choice it reads the expert row over NVLink once and
+//   grad_w[t, j]                  = <dy[t], expert_out[row]>, fp32 (+0.0 when pos = -1)
+//   grad_expert_out[row] on holder = round_T(w[t, j] · float(dy[t])), one correctly rounded multiply
+// The dot's order is fixed, so its bits do not depend on the grid: lane l sums, in fp32 with one
+// fused multiply-add per element, the elements of packs l, l + 32, l + 64, ... in that order (each
+// pack's elements in order), then a shfl_xor butterfly over distances 16, 8, 4, 2, 1 adds the lanes.
+//   barrier 1, barrier 2  as in the combine
+//   between 2 and 3       only if every rank's verdict is valid: pull, dot and push; each holder also
+//                         writes +0 to every row of its grad_expert_out outside its receive segments
+//                         (alignment gaps and the tail), so no rank writes anything when a call fails.
+//   barrier 3             every rank has read its rows and pushed its gradient rows
+//   after barrier 3       a plain grad_expert_out is copied out of my staging area, segment by segment.
+// Staged (plain expert_out and grad_expert_out), a holder's staging area holds its expert_out copy
+// in rows [0, cap) and the pushed gradient rows in [cap, 2·cap); senders take cap from its header.
+// pos must name each routed dispatch-input row at most once (route() and the top-k dispatch do);
+// staged, a segment row that no choice names is copied out with unspecified contents.
+constexpr int kTopkBackPacks = 1;  // packs of one row per lane per step: dy, 4 choices' rows, 4 dots in registers
+
+namespace {
+__device__ __forceinline__ void gridZero(char* dst, unsigned long long bytes, size_t tid, size_t nthreads) {
+  const Pack16 z = {{0u, 0u, 0u, 0u}};
+  for (unsigned long long i = tid; i < bytes / 16; i += nthreads) st128(dst + i * 16, z);
+}
+}  // namespace
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+moeCombineTopkBackwardKernel(CommArgs a, PeerPtrs srcs, PeerPtrs grads, const long long* splits,
+                             const long long* posIn, const float* weights, const char* dy, float* gradW,
+                             char* stagedGrad, unsigned long long tokens, unsigned long long capacity, int topk,
+                             MoeArgs d) {
+  using PT = PackTraits<T>;
+  __shared__ unsigned long long sSrc[kMaxK];  // my chunk k: first row in my dispatch input
+  __shared__ unsigned long long sDst[kMaxK];  //             first row on its holder
+  __shared__ unsigned long long sAux[kMaxK];  // column sums, then expert bases
+  __shared__ unsigned long long sRcv[kMaxK];  // first row of my receive segment e·P+s
+  __shared__ uint32_t sRcvCnt[kMaxK];         // and its rows
+  __shared__ unsigned long long sNeed[kMaxRanks], sCap[kMaxRanks];
+  __shared__ const char* sBase[kMaxRanks];
+  __shared__ char* sGrad[kMaxRanks];
+  __shared__ unsigned long long sWarp[32];
+  const uint32_t ep = loadEpoch(a);
+  const int P = a.nranks, E = d.experts, K = P * E, me = a.rank, t = threadIdx.x;
+  const unsigned long long rb = d.rowBytes;
+  const size_t gtid = static_cast<size_t>(blockIdx.x) * blockDim.x + t;
+  const size_t gthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
+
+  const bool pull = topkPullPrologue(a, ep, srcs, splits, posIn, tokens * static_cast<unsigned long long>(topk), d,
+                                     a2aHeaderWord(A2aForm::kCombineTopkBackward, false, d.plain != 0), sSrc, sDst,
+                                     sAux, sNeed, sCap, sBase, sWarp);
+  if (pull) {
+    a2aReceiveSegments(a.self, P, E, me, sAux, sRcv, sRcvCnt);
+    if (t < P) sGrad[t] = d.plain ? const_cast<char*>(sBase[t]) + sCap[t] * rb : static_cast<char*>(grads.p[t]);
+    __syncthreads();
+
+    // ---- zero my rows outside the receive segments: the gap after each expert, the tail ----
+    char* mine = d.plain ? stagedGrad : sGrad[me];
+    if (mine != nullptr) {
+      for (int e = 0; e < E; e++) {
+        const int last = e * P + P - 1;
+        const unsigned long long lo = sRcv[last] + sRcvCnt[last];
+        const unsigned long long hi = e + 1 < E ? sAux[me * E + e + 1] : capacity;
+        if (hi > lo) gridZero(mine + lo * rb, (hi - lo) * rb, gtid, gthreads);
+      }
+    }
+
+    // ---- pull, dot and push: one warp per token ----
+    const int lane = t & 31, k = topk;
+    const unsigned long long npk = rb / 16;
+    for (unsigned long long tok = gtid / 32; tok < tokens; tok += gthreads / 32) {
+      // Lane j < k: choice j's expert row, its gradient row and its weight.
+      const char* src = nullptr;
+      char* dstG = nullptr;
+      float w = 0.0f;
+      if (lane < k) {
+        const long long p = posIn[tok * k + lane];
+        if (p >= 0) {
+          int j;
+          const unsigned long long row = topkHolderRow(sSrc, sDst, K, E, static_cast<unsigned long long>(p), j);
+          src = sBase[j] + row * rb;
+          dstG = sGrad[j] + row * rb;
+          w = weights[tok * k + lane];
+        }
+      }
+      const char* g = dy + tok * rb;
+      for (int j0 = 0; j0 < k; j0 += kTopkInFlight) {
+        const char* s[kTopkInFlight];
+        char* q[kTopkInFlight];
+        float ws[kTopkInFlight], part[kTopkInFlight];
+#pragma unroll
+        for (int c = 0; c < kTopkInFlight; c++) {
+          s[c] = reinterpret_cast<const char*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(src), (j0 + c) & 31));
+          q[c] = reinterpret_cast<char*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(dstG), (j0 + c) & 31));
+          ws[c] = __shfl_sync(0xffffffffu, w, (j0 + c) & 31);
+          if (j0 + c >= k) s[c] = nullptr;
+          part[c] = 0.0f;
+        }
+        // Warp-uniform trip count: every lane takes part in the shuffles, lanes past the row end idle.
+        for (unsigned long long v0 = lane; v0 - lane < npk; v0 += 32 * kTopkBackPacks) {
+          Pack16 gv[kTopkBackPacks], x[kTopkInFlight][kTopkBackPacks];
+#pragma unroll
+          for (int u = 0; u < kTopkBackPacks; u++) {
+            const unsigned long long pk = v0 + 32ull * u;
+            if (pk < npk) gv[u] = ld128(g + pk * 16);
+          }
+#pragma unroll
+          for (int c = 0; c < kTopkInFlight; c++) {
+#pragma unroll
+            for (int u = 0; u < kTopkBackPacks; u++) {
+              const unsigned long long pk = v0 + 32ull * u;
+              if (s[c] != nullptr && pk < npk) x[c][u] = ld128_stream(s[c] + pk * 16);
+            }
+          }
+#pragma unroll
+          for (int u = 0; u < kTopkBackPacks; u++) {
+            const unsigned long long pk = v0 + 32ull * u;
+            if (pk >= npk) continue;
+            const typename PT::AccPack gf = PT::widen(gv[u]);
+#pragma unroll
+            for (int c = 0; c < kTopkInFlight; c++) {
+              if (s[c] == nullptr) continue;
+              const typename PT::AccPack xf = PT::widen(x[c][u]);
+              typename PT::AccPack o;
+#pragma unroll
+              for (int i = 0; i < PT::kElems; i++) {
+                part[c] = __fmaf_rn(gf.v[i], xf.v[i], part[c]);
+                o.v[i] = __fmul_rn(ws[c], gf.v[i]);
+              }
+              st128(q[c] + pk * 16, PT::narrow(o));
+            }
+          }
+        }
+#pragma unroll
+        for (int c = 0; c < kTopkInFlight; c++) {
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) part[c] = __fadd_rn(part[c], __shfl_xor_sync(0xffffffffu, part[c], o));
+        }
+        if (lane == 0) {
+#pragma unroll
+          for (int c = 0; c < kTopkInFlight; c++) {
+            if (j0 + c < k) gradW[tok * k + j0 + c] = s[c] != nullptr ? part[c] : 0.0f;
+          }
+        }
+      }
+    }
+  }
+  blockBarrier(a, ep + 3);
+  // NO pad table or peer reads from here on (as in the combine). Every peer has pushed its rows
+  // into my staging area: once every local CTA is past barrier 3, copy them out.
+  if (stagedGrad != nullptr) {
+    const bool synced = localGridSync(a);
+    if (synced && pull && ld_relaxed_sys(&a.self->abort) == 0u) {
+      a2aCopyOut<false>(stagedGrad, nullptr, sGrad[me], rb, 0, K, sRcv, sRcvCnt, gtid, gthreads);
+    }
+  }
+  retire(a, 3, 0);
+}
+
 namespace {
 // The top-k combine instantiation for dt: float, bfloat16 or float16 rows (null for any other).
 using TopkCombineFn = void (*)(CommArgs, PeerPtrs, const long long*, const long long*, const float*, char*,
@@ -669,7 +889,28 @@ TopkCombineFn topkCombineFn(DataType dt) {
     default: return nullptr;
   }
 }
+// Its backward, for the same row types.
+using TopkCombineBackwardFn = void (*)(CommArgs, PeerPtrs, PeerPtrs, const long long*, const long long*, const float*,
+                                       const char*, float*, char*, unsigned long long, unsigned long long, int, MoeArgs);
+TopkCombineBackwardFn topkCombineBackwardFn(DataType dt) {
+  switch (dt) {
+    case DataType::FLOAT32: return moeCombineTopkBackwardKernel<float>;
+    case DataType::BFLOAT16: return moeCombineTopkBackwardKernel<__nv_bfloat16>;
+    case DataType::FLOAT16: return moeCombineTopkBackwardKernel<__half>;
+    default: return nullptr;
+  }
+}
 }  // namespace
+
+void launchMoeCombineTopkBackward(const CommArgs& a, const PeerPtrs& srcs, const PeerPtrs& grads, const MoeArgs& d,
+                                  void* stagedGrad, size_t capacityRows, const void* dy, float* gradWeights,
+                                  size_t tokens, int topk, const long long* pos, const float* weights,
+                                  const long long* splits, DataType dt, int blocks, cudaStream_t stream) {
+  topkCombineBackwardFn(dt)<<<blocks, kThreads, 0, stream>>>(a, srcs, grads, splits, pos, weights,
+                                                             static_cast<const char*>(dy), gradWeights,
+                                                             static_cast<char*>(stagedGrad), tokens, capacityRows,
+                                                             topk, d);
+}
 
 void launchMoeCombineTopk(const CommArgs& a, const PeerPtrs& srcs, const MoeArgs& d, void* out, size_t tokens,
                           int topk, const long long* pos, const float* weights, const long long* splits, DataType dt,
@@ -853,6 +1094,9 @@ const void* alltoallvDevKernelPtr(bool fp8) {
              : reinterpret_cast<const void*>(alltoallvDevKernel<false>);
 }
 const void* moeCombineTopkKernelPtr(DataType dt) { return reinterpret_cast<const void*>(topkCombineFn(dt)); }
+const void* moeCombineTopkBackwardKernelPtr(DataType dt) {
+  return reinterpret_cast<const void*>(topkCombineBackwardFn(dt));
+}
 const void* moeDispatchTopkKernelPtr(bool fp8) {
   return fp8 ? reinterpret_cast<const void*>(moeDispatchTopkKernel<true>)
              : reinterpret_cast<const void*>(moeDispatchTopkKernel<false>);
@@ -861,7 +1105,10 @@ const void* moeDispatchTopkKernelPtr(bool fp8) {
 void preloadMoeKernels() {
   touchKernel(alltoallvDevKernel<false>);
   touchKernel(alltoallvDevKernel<true>);
-  for (DataType dt : {DataType::FLOAT32, DataType::BFLOAT16, DataType::FLOAT16}) touchKernel(topkCombineFn(dt));
+  for (DataType dt : {DataType::FLOAT32, DataType::BFLOAT16, DataType::FLOAT16}) {
+    touchKernel(topkCombineFn(dt));
+    touchKernel(topkCombineBackwardFn(dt));
+  }
   touchKernel(moeDispatchTopkKernel<false>);
   touchKernel(moeDispatchTopkKernel<true>);
   cudaGetLastError();

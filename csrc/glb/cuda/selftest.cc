@@ -12,6 +12,7 @@
 
 #include <cmath>
 #include <cstring>
+#include <numeric>
 #include <sstream>
 
 #include "glb/common/utils.h"
@@ -637,6 +638,125 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
         return "";
       });
     }
+    // The top-k combine's backward, zero copy, with the combine case's closed-form layout. pos names
+    // every routed row of rank 0's dispatch input at most once. dy holds quarters and expert_out halves
+    // of small integers, so every product and partial sum of the dot is exact in fp32 and grad_w is
+    // the exact dot product. Holder j's gradient rows of rank 0 must be bf16(w · dy); holder 0 (rank 0
+    // itself) zeroes its alignment gaps and tail; a guard row after the capacity stays untouched.
+    R.run(strcat_all("moeCombineTopkBackwardKernel<bf16> (E=2, align=4, k=3, 64-element rows) P=", P),
+          [&]() -> std::string {
+      const int E = 2, A = 4, K = P * E, H = 64, topk = 3;
+      const size_t rb = H * 2, cap = n * 4 / rb - 1, T = 37;
+      std::vector<int64_t> sp(K), pre(K + 1, 0);
+      for (int k = 0; k < K; k++) {
+        sp[k] = (k * 5 + 2) % 4;
+        pre[k + 1] = pre[k] + sp[k];
+      }
+      auto base = [&](int j, int e) {
+        int64_t b = 0;
+        for (int x = 0; x < e; x++) b = (b + P * sp[j * E + x] + A - 1) / A * A;
+        return b;
+      };
+      auto value = [](int j, int64_t row, int c) { return static_cast<float>((j * 7 + row * 3 + c) % 17 - 8) * 0.5f; };
+      auto dyv = [](size_t t, int c) { return static_cast<float>(static_cast<int>((t * 5 + c * 3) % 9) - 4) * 0.25f; };
+      auto bf16 = [](float f) {
+        uint32_t u;
+        std::memcpy(&u, &f, 4);
+        return static_cast<uint16_t>((u + 0x7fffu + ((u >> 16) & 1u)) >> 16);  // round to nearest even
+      };
+      // pos: a stride permutation of the routed rows, dealt to the choices that are not dropped.
+      const int64_t N = pre[K];
+      int64_t stride = 7;
+      while (std::gcd(stride, N) != 1) stride++;
+      std::vector<int64_t> pos(T * topk, -1);
+      std::vector<float> w(T * topk);
+      int64_t next = 0;
+      for (size_t t = 0; t < T; t++) {
+        for (int c = 0; c < topk; c++) {
+          const bool dropped = (t * c) % 5 == 1 || t == 4;
+          if (!dropped && next < N) pos[t * topk + c] = (next++ * stride) % N;
+          w[t * topk + c] = static_cast<float>((t * 5 + c * 3) % 9) * 0.3f - 1.1f;
+        }
+      }
+      std::vector<uint16_t> dyHost(T * H);
+      for (size_t t = 0; t < T; t++) {
+        for (int c = 0; c < H; c++) dyHost[t * H + c] = bf16(dyv(t, c));
+      }
+      std::vector<std::unique_ptr<DevBuf>> gradBufs;
+      PeerPtrs gp;
+      std::memset(&gp, 0, sizeof(gp));
+      for (int j = 0; j < P; j++) {
+        std::vector<uint16_t> rows(cap * H);
+        for (size_t r = 0; r < cap; r++) {
+          for (int c = 0; c < H; c++) rows[r * H + c] = bf16(value(j, r, c));  // exact
+        }
+        GLB_CUDA_CHECK(cudaMemcpyAsync(pp.p[j], rows.data(), rows.size() * 2, cudaMemcpyHostToDevice, stream));
+        GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+        gradBufs.emplace_back(new DevBuf((cap + 1) * rb));  // + a guard row
+        gp.p[j] = gradBufs[j]->p;
+        GLB_CUDA_CHECK(cudaMemsetAsync(gp.p[j], 0xff, (cap + 1) * rb, stream));
+      }
+      DevBuf splits(K * 8), posDev(pos.size() * 8), wDev(w.size() * 4), dy(T * rb), gw(T * topk * 4);
+      GLB_CUDA_CHECK(cudaMemcpyAsync(splits.p, sp.data(), K * 8, cudaMemcpyHostToDevice, stream));
+      GLB_CUDA_CHECK(cudaMemcpyAsync(posDev.p, pos.data(), pos.size() * 8, cudaMemcpyHostToDevice, stream));
+      GLB_CUDA_CHECK(cudaMemcpyAsync(wDev.p, w.data(), w.size() * 4, cudaMemcpyHostToDevice, stream));
+      GLB_CUDA_CHECK(cudaMemcpyAsync(dy.p, dyHost.data(), T * rb, cudaMemcpyHostToDevice, stream));
+      GLB_CUDA_CHECK(cudaMemsetAsync(gw.p, 0xff, T * topk * 4, stream));
+      const int blocks = std::min(pc.coResidentBlocks(moeCombineTopkBackwardKernelPtr(DataType::BFLOAT16)), 16);
+      launchMoeCombineTopkBackward(ca, pp, gp, moeArgs(rb, cap, E, A, pc.inputStatusDevice()), nullptr, cap, dy.p,
+                                   static_cast<float*>(gw.p), T, topk, static_cast<const long long*>(posDev.p),
+                                   static_cast<const float*>(wDev.p), static_cast<const long long*>(splits.p),
+                                   DataType::BFLOAT16, blocks, stream);
+      noteLaunch();
+      std::vector<float> gotW(T * topk);
+      GLB_CUDA_CHECK(cudaMemcpyAsync(gotW.data(), gw.p, gotW.size() * 4, cudaMemcpyDeviceToHost, stream));
+      std::vector<std::vector<uint16_t>> grads(P, std::vector<uint16_t>((cap + 1) * H));
+      for (int j = 0; j < P; j++) {
+        GLB_CUDA_CHECK(cudaMemcpyAsync(grads[j].data(), gp.p[j], (cap + 1) * rb, cudaMemcpyDeviceToHost, stream));
+      }
+      GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+      for (size_t i = 0; i < T * topk; i++) {
+        const size_t t = i / topk;
+        const int64_t p = pos[i];
+        if (p < 0) {
+          uint32_t u;
+          std::memcpy(&u, &gotW[i], 4);
+          if (u != 0u) return strcat_all("token ", t, " choice ", i % topk, ": grad_w of a dropped choice is not +0");
+          continue;
+        }
+        int k = 0;
+        while (pre[k + 1] <= p) k++;
+        const int j = k / E;
+        const int64_t row = base(j, k % E) + (p - pre[k]);
+        double dot = 0.0;
+        for (int c = 0; c < H; c++) {
+          dot += static_cast<double>(dyv(t, c)) * value(j, row, c);
+          const uint16_t want = bf16(w[i] * bf16ToFloat(dyHost[t * H + c]));
+          if (grads[j][row * H + c] != want) {
+            return strcat_all("holder ", j, " row ", row, " element ", c, ": got bf16 bits ",
+                              static_cast<int>(grads[j][row * H + c]), ", want ", static_cast<int>(want));
+          }
+        }
+        if (static_cast<double>(gotW[i]) != dot) {
+          return strcat_all("token ", t, " choice ", i % topk, ": grad_w ", gotW[i], ", want ", dot);
+        }
+      }
+      // Holder 0's rows outside its segments (every source sends rank 0's splits): zero.
+      for (int e = 0; e < E; e++) {
+        const int64_t lo = base(0, e) + P * sp[e], hi = e + 1 < E ? base(0, e + 1) : static_cast<int64_t>(cap);
+        for (int64_t r = lo; r < hi; r++) {
+          for (int c = 0; c < H; c++) {
+            if (grads[0][r * H + c] != 0) return strcat_all("holder 0 row ", r, " (outside its segments) is not zero");
+          }
+        }
+      }
+      for (int j = 0; j < P; j++) {
+        for (int c = 0; c < H; c++) {
+          if (grads[j][cap * H + c] != 0xffffu) return strcat_all("holder ", j, ": wrote past its capacity");
+        }
+      }
+      return "";
+    });
 
     // ---- literal schedule executor (halving-doubling, plain and pipelined) -------------------
     R.run(strcat_all("scheduleKernel<float>(halving_doubling) P=", P), [&]() -> std::string {

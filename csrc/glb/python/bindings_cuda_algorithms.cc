@@ -224,6 +224,23 @@ void registerCudaAlgorithms(py::module_& m) {
   }, py::arg("pc"), py::arg("out"), py::arg("tokens"), py::arg("topk"), py::arg("pos"), py::arg("weights"),
      py::arg("splits"), py::arg("buf"), py::arg("buf_offset"), py::arg("expert_out"), py::arg("capacity_rows"),
      py::arg("row_bytes"), py::arg("dtype"), py::arg("experts"), py::arg("align"), py::arg("stream"));
+  m.def("alltoallv_dev_combine_topk_backward", [](PeerContext& pc, py::object gradBuf, size_t gradOff,
+                                                  uintptr_t gradExpertOut, uintptr_t gradWeights, uintptr_t gradOut,
+                                                  py::object buf, size_t off, uintptr_t expertOut, size_t tokens,
+                                                  int topk, uintptr_t pos, uintptr_t weights, uintptr_t splits,
+                                                  size_t capacityRows, size_t rowBytes, int dtype, int experts,
+                                                  int align, uintptr_t st) {
+    const MoeOut geo = moeOut(gradBuf, gradOff, gradExpertOut), eo = moeOut(buf, off, expertOut);
+    py::gil_scoped_release nogil;
+    alltoallvDevCombineTopkBackward(pc, geo, reinterpret_cast<float*>(gradWeights), P(gradOut), eo, tokens, topk,
+                                    reinterpret_cast<const int64_t*>(pos), reinterpret_cast<const float*>(weights),
+                                    reinterpret_cast<const int64_t*>(splits), capacityRows, rowBytes,
+                                    static_cast<DataType>(dtype), experts, align, S(st));
+  }, py::arg("pc"), py::arg("grad_buf"), py::arg("grad_buf_offset"), py::arg("grad_expert_out"),
+     py::arg("grad_weights"), py::arg("grad_out"), py::arg("buf"), py::arg("buf_offset"), py::arg("expert_out"),
+     py::arg("tokens"), py::arg("topk"), py::arg("pos"), py::arg("weights"), py::arg("splits"),
+     py::arg("capacity_rows"), py::arg("row_bytes"), py::arg("dtype"), py::arg("experts"), py::arg("align"),
+     py::arg("stream"));
   m.def("alltoall_reg",[](PeerContext& pc, uintptr_t in, const PeerBuffer& out, size_t off, size_t bytes, uintptr_t st) {
     py::gil_scoped_release nogil;
     alltoall(pc, P(in), out, off, bytes, S(st));

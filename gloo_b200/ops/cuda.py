@@ -491,7 +491,9 @@ class CudaContext:
         is its capacity. ``pos`` is int64 ``(T, k)``: ``pos[t, j]`` is the row of this rank's dispatch
         input that carried token t's choice j, -1 if it was not sent. ``weights`` is float32
         ``(T, k)``; the weight of a -1 entry is ignored. ``out`` is ``(T, *expert_out.shape[1:])`` of
-        ``expert_out``'s dtype, written on this rank only:
+        ``expert_out``'s dtype, written on this rank only. ``weights=None`` gives every routed choice
+        weight 1 (the unweighted sum, which is the backward of :meth:`alltoallv_dev_topk`), byte for
+        byte what a tensor of ones gives:
         ``out[t] = round(acc)``, ``acc`` starting at +0.0 and, for j = 0..k-1 with ``pos[t, j] >= 0``
         in that order, ``acc = acc + w[t, j] * float(row)``, each a correctly rounded fp32 multiply or
         add (no fused multiply-add), rounded to nearest even into the dtype. That is what torch
@@ -511,13 +513,18 @@ class CudaContext:
 
         name = "alltoallv_dev_combine_topk"
         dtypes = (torch.float32, torch.bfloat16, torch.float16)
-        self._dev_tensors(name, {"out": out, "expert_out": expert_out, "pos": pos, "weights": weights})
+        named = {"out": out, "expert_out": expert_out, "pos": pos}
+        if weights is not None:
+            named["weights"] = weights
+        self._dev_tensors(name, named)
         if expert_out.dtype not in dtypes or out.dtype != expert_out.dtype:
             raise ValueError(f"{name}: expert_out and out must share a dtype of float32, bfloat16 or float16, got "
                              f"{expert_out.dtype} and {out.dtype}")
-        if pos.dtype != torch.int64 or pos.dim() != 2 or weights.dtype != torch.float32 or weights.shape != pos.shape:
+        if pos.dtype != torch.int64 or pos.dim() != 2 or (weights is not None and (
+                weights.dtype != torch.float32 or weights.shape != pos.shape)):
             raise ValueError(f"{name}: pos must be int64 (T, k) and weights float32 of the same shape, got "
-                             f"{pos.dtype} {tuple(pos.shape)} and {weights.dtype} {tuple(weights.shape)}")
+                             f"{pos.dtype} {tuple(pos.shape)} and "
+                             f"{None if weights is None else (weights.dtype, tuple(weights.shape))}")
         T, k = int(pos.shape[0]), int(pos.shape[1])
         if not 1 <= k <= 32:
             raise ValueError(f"{name}: k = {k} choices per token; 1..32 are supported")
@@ -536,11 +543,93 @@ class CudaContext:
             raise ValueError(f"{name}: experts must be in 1..32 and align at least 1, got {experts} and {align}")
         si = self._dev_index(splits, "splits", self.size * int(experts))
         buf, off = self.lookup(expert_out)
-        _cu.alltoallv_dev_combine_topk(self.pc, out.data_ptr(), T, k, pos.data_ptr(), weights.data_ptr(), si, buf, off,
+        wp = weights.data_ptr() if weights is not None else 0
+        _cu.alltoallv_dev_combine_topk(self.pc, out.data_ptr(), T, k, pos.data_ptr(), wp, si, buf, off,
                                        expert_out.data_ptr(), int(expert_out.shape[0]), rb,
                                        int(_torch_dtype_to_glb(expert_out.dtype)), int(experts), int(align),
                                        _stream(stream))
         return out
+
+    def alltoallv_dev_combine_topk_backward(self, grad_expert_out, grad_weights, grad_out, expert_out, splits, pos,
+                                            weights, experts: int = 1, align: int = 1, stream=None):
+        """Backward of :meth:`alltoallv_dev_combine_topk` in one kernel, with no host synchronisation
+        (graph-capturable). ``expert_out``, ``splits``, ``pos``, ``weights``, ``experts`` and
+        ``align`` are the combine's; ``grad_out`` is the gradient of its ``out``, ``(T, *row)`` of
+        ``expert_out``'s dtype. For every routed choice ``(t, j)`` (``pos[t, j] >= 0``) this rank
+        reads the expert row ``r`` over the link once and writes:
+
+        - ``grad_weights[t, j]`` (float32 ``(T, k)``, this rank) = ``sum_h float(grad_out[t, h]) *
+          float(r[h])`` in fp32. The order is fixed, so the bits do not depend on the grid or the
+          run: lane ``l`` of the token's warp adds, with one fused multiply-add per element, the
+          elements of 16-byte packs ``l, l + 32, l + 64, ...`` of the row in that order, then a
+          ``shfl_xor`` butterfly over lane distances 16, 8, 4, 2, 1 sums the 32 lane totals. Where
+          ``pos[t, j] = -1`` it is ``+0.0``.
+        - the same row of the holder's ``grad_expert_out`` (``expert_out``'s shape, dtype and
+          layout, on every rank) = ``(weights[t, j, None] * grad_out[t].float()).to(dtype)``: one
+          correctly rounded fp32 multiply, then round to nearest even, byte for byte.
+
+        Every holder writes ``+0`` to each row of its ``grad_expert_out`` outside its receive
+        segments (alignment gaps and the rows past the last segment), so experts that run over the
+        whole buffer get zero gradient for padded rows. ``pos`` must name each dispatch-input row
+        at most once, as :meth:`route <gloo_b200.parallel.strategies.MoEDispatcher.route>` and
+        :meth:`alltoallv_dev_topk` produce; with plain tensors a segment row that no choice names is
+        left unspecified.
+
+        ``expert_out`` and ``grad_expert_out`` are both registered / symmetric (zero copy: peers
+        write ``grad_expert_out`` in place) or both plain (staged: each rank's pool holds its
+        ``expert_out`` rows and then its gradient rows, so the capacity is capped at half the
+        combine's), else ``ValueError``. Wrong dtypes or shapes, non-contiguous or misaligned
+        tensors (``expert_out``, ``grad_expert_out`` and ``grad_out`` 16-byte aligned, rows a
+        multiple of 16 bytes), k outside 1..32 and a ``grad_expert_out`` that overlaps
+        ``expert_out``, ``grad_out`` or ``grad_weights`` raise ``ValueError`` before launch. Errors
+        found on the device (as for the combine, including a peer that runs another form) raise
+        ``ValueError`` on every rank at the next host call, and then no rank has written its
+        ``grad_expert_out`` or ``grad_weights``."""
+        import torch
+
+        name = "alltoallv_dev_combine_topk_backward"
+        dtypes = (torch.float32, torch.bfloat16, torch.float16)
+        self._dev_tensors(name, {"grad_expert_out": grad_expert_out, "grad_weights": grad_weights,
+                                 "grad_out": grad_out, "expert_out": expert_out, "pos": pos, "weights": weights})
+        if expert_out.dtype not in dtypes or grad_out.dtype != expert_out.dtype:
+            raise ValueError(f"{name}: expert_out and grad_out must share a dtype of float32, bfloat16 or float16, "
+                             f"got {expert_out.dtype} and {grad_out.dtype}")
+        if grad_expert_out.dtype != expert_out.dtype or grad_expert_out.shape != expert_out.shape:
+            raise ValueError(f"{name}: grad_expert_out {grad_expert_out.dtype} {tuple(grad_expert_out.shape)} must "
+                             f"match expert_out {expert_out.dtype} {tuple(expert_out.shape)}")
+        if pos.dtype != torch.int64 or pos.dim() != 2 or weights.dtype != torch.float32 or weights.shape != pos.shape:
+            raise ValueError(f"{name}: pos must be int64 (T, k) and weights float32 of the same shape, got "
+                             f"{pos.dtype} {tuple(pos.shape)} and {weights.dtype} {tuple(weights.shape)}")
+        if grad_weights.dtype != torch.float32 or grad_weights.shape != pos.shape:
+            raise ValueError(f"{name}: grad_weights must be float32 {tuple(pos.shape)}, got {grad_weights.dtype} "
+                             f"{tuple(grad_weights.shape)}")
+        T, k = int(pos.shape[0]), int(pos.shape[1])
+        if not 1 <= k <= 32:
+            raise ValueError(f"{name}: k = {k} choices per token; 1..32 are supported")
+        if expert_out.dim() < 2 or tuple(grad_out.shape) != (T, *expert_out.shape[1:]):
+            raise ValueError(f"{name}: grad_out {tuple(grad_out.shape)} must be (T, *expert_out.shape[1:]) with "
+                             f"T = {T}, expert_out {tuple(expert_out.shape)} at least 2-D")
+        rb = expert_out.element_size()
+        for d in expert_out.shape[1:]:
+            rb *= int(d)
+        if rb == 0 or rb % 16 != 0:
+            raise ValueError(f"{name}: rows of {rb} bytes; a positive multiple of 16 is required")
+        if expert_out.data_ptr() % 16 or grad_expert_out.data_ptr() % 16 or grad_out.data_ptr() % 16:
+            raise ValueError(f"{name}: expert_out, grad_expert_out and grad_out must be 16-byte aligned")
+        for other, what in ((expert_out, "expert_out"), (grad_out, "grad_out"), (grad_weights, "grad_weights")):
+            self._dev_disjoint(name, grad_expert_out, "grad_expert_out", other, what)
+        if not 1 <= int(experts) <= 32 or int(align) < 1:
+            raise ValueError(f"{name}: experts must be in 1..32 and align at least 1, got {experts} and {align}")
+        si = self._dev_index(splits, "splits", self.size * int(experts))
+        buf, off = self.lookup(expert_out)
+        gbuf, goff = self.lookup(grad_expert_out)
+        _cu.alltoallv_dev_combine_topk_backward(self.pc, gbuf, goff, grad_expert_out.data_ptr(),
+                                                grad_weights.data_ptr(), grad_out.data_ptr(), buf, off,
+                                                expert_out.data_ptr(), T, k, pos.data_ptr(), weights.data_ptr(), si,
+                                                int(expert_out.shape[0]), rb,
+                                                int(_torch_dtype_to_glb(expert_out.dtype)), int(experts),
+                                                int(align), _stream(stream))
+        return grad_expert_out, grad_weights
 
     def alltoallv_dev_topk(self, out, x, topk_idx, splits, pos, out_splits, out_offsets, experts: int = 1,
                            align: int = 1, out_scales=None, stream=None):

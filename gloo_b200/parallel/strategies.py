@@ -587,6 +587,93 @@ class MoEDispatcher(_Base):
         ``CudaContext.alltoallv_dev_combine_topk``."""
         return self.cc.alltoallv_dev_combine_topk(out, expert_out, splits, pos, weights, experts=experts, align=align)
 
+    def combine_dev_topk_backward(self, grad_out, expert_out, splits, pos, weights, grad_expert_out, grad_weights,
+                                  experts: int = 1, align: int = 1):
+        """The backward of combine_dev_topk() in one kernel: ``grad_weights[t, j]`` = the fp32 dot of
+        ``grad_out[t]`` with choice j's expert row, and ``weights[t, j] * grad_out[t]`` written to that
+        row of its holder's ``grad_expert_out`` (zero in every row outside the received segments).
+        Returns ``(grad_expert_out, grad_weights)``. See
+        ``CudaContext.alltoallv_dev_combine_topk_backward``."""
+        return self.cc.alltoallv_dev_combine_topk_backward(grad_expert_out, grad_weights, grad_out, expert_out, splits,
+                                                           pos, weights, experts=experts, align=align)
+
+    # ---- autograd ------------------------------------------------------------------------------
+    # Each backward is a collective: every rank's backward pass must reach it, in the same order. The
+    # backward kernels run on the stream current in the backward pass, on plain gradient tensors, so
+    # they take the staged path.
+    def dispatch_topk_autograd(self, x, topk_idx, out, experts: int = 1, align: int = 1):
+        """dispatch_dev_topk() that autograd can differentiate in ``x``. Returns ``(expert_in,
+        out_splits, out_offsets, routing)``: ``expert_in`` is a view of ``out``; ``routing`` holds
+        ``splits``, ``pos``, ``experts`` and ``align`` for combine_topk_autograd(). The backward
+        sums each token's k expert-input gradient rows (the top-k combine with every weight 1)
+        into a fresh ``grad_x``. FP8 dispatch is not differentiable."""
+        import torch
+
+        moe = self
+
+        class _Dispatch(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, inp):
+                _, out_splits, out_offsets, splits, pos = moe.dispatch_dev_topk(inp, topk_idx, out, experts=experts,
+                                                                               align=align)
+                ctx.routing = MoERouting(splits, pos, experts, align)
+                ctx.mark_non_differentiable(out_splits, out_offsets, splits, pos)
+                return out.view_as(out), out_splits, out_offsets, splits, pos
+
+            @staticmethod
+            def backward(ctx, grad, *_):
+                r = ctx.routing
+                g = grad.contiguous()
+                grad_x = torch.empty((r.pos.shape[0], *g.shape[1:]), dtype=g.dtype, device=g.device)
+                moe.cc.alltoallv_dev_combine_topk(grad_x, g, r.splits, r.pos, None, experts=r.experts, align=r.align)
+                return grad_x
+
+        expert_in, out_splits, out_offsets, splits, pos = _Dispatch.apply(x)
+        return expert_in, out_splits, out_offsets, MoERouting(splits, pos, experts, align)
+
+    def combine_topk_autograd(self, expert_out, weights, routing):
+        """combine_dev_topk() into a fresh ``y`` that autograd can differentiate in ``expert_out``
+        and ``weights`` (float32 ``(T, k)``); ``routing`` comes from dispatch_topk_autograd(). The
+        backward is one kernel (combine_dev_topk_backward()): the gradient rows go back to the
+        experts' holders and the weight gradients are computed where the weights live. A registered
+        or symmetric ``expert_out`` is copied to a plain tensor for the backward, whose gradient
+        tensors are plain."""
+        import torch
+
+        moe, r = self, routing
+
+        class _Combine(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, eo, w):
+                eo, w = eo.contiguous(), w.contiguous()
+                y = torch.empty((r.pos.shape[0], *eo.shape[1:]), dtype=eo.dtype, device=eo.device)
+                moe.cc.alltoallv_dev_combine_topk(y, eo, r.splits, r.pos, w, experts=r.experts, align=r.align)
+                ctx.save_for_backward(eo, w)
+                return y
+
+            @staticmethod
+            def backward(ctx, dy):
+                eo, w = ctx.saved_tensors
+                if moe.cc.lookup(eo)[0] is not None:
+                    eo = eo.clone()
+                grad_eo = torch.empty_like(eo)
+                grad_w = torch.empty_like(w)
+                moe.combine_dev_topk_backward(dy.contiguous(), eo, r.splits, r.pos, w, grad_eo, grad_w,
+                                              experts=r.experts, align=r.align)
+                return grad_eo, grad_w
+
+        return _Combine.apply(expert_out, weights)
+
+
+class MoERouting:
+    """Where dispatch_topk_autograd() sent each token's choices: the dispatch ``splits`` and ``pos``
+    (device tensors) and its ``experts`` and ``align``. Not differentiable."""
+
+    __slots__ = ("splits", "pos", "experts", "align")
+
+    def __init__(self, splits, pos, experts: int, align: int):
+        self.splits, self.pos, self.experts, self.align = splits, pos, int(experts), int(align)
+
 
 class UlyssesAttention(_Base):
     """DeepSpeed-Ulysses: [S/P, H, D] <-> [S, H/P, D] with one alltoall each way."""

@@ -33,7 +33,17 @@ arms alternating), with symmetric outputs:
 Both arms' outputs are checked equal byte for byte before timing. "MB avoided" is route()'s copy of
 the T x k rows, written once and read back by the dispatch, from the shapes.
 
-    python scripts/bench_moe_dispatch.py [--ranks 2] [--iters 20] [--tables pairs,fp8,combine,dispatch]
+A fifth table times the top-k combine's backward (median per call, rank 0, the two arms
+alternating), with expert_out and grad_expert_out symmetric and plain, at the combine table's sizes:
+  composed  MoEDispatcher.combine_dev of expert_out, un-permute, the fp32 dot with dy per choice in
+            torch, w * dy permuted into route order, then dispatch_dev into grad_expert_out
+  fused     MoEDispatcher.combine_dev_topk_backward (one kernel: pull, dot and push)
+Before timing, grad_expert_out is checked equal byte for byte between the arms, and grad_w within
+n * 2^-23 * sum |dy * x| of each other (n = hidden: the bound of any fp32 summation order of n
+terms; the two arms sum in different orders). MB/rank is the T x k expert rows read plus the T x k
+gradient rows written, from the shapes.
+
+    python scripts/bench_moe_dispatch.py [--ranks 2] [--iters 20] [--tables pairs,fp8,combine,dispatch,backward]
 """
 import argparse
 import json
@@ -273,6 +283,76 @@ def measure_topk(ctx, args, dev):
     return res
 
 
+def run_rank_backward(ctx, args, shared):
+    if shared:
+        return measure_backward(ctx, args, 0)
+    torch.cuda.set_device(ctx.rank)
+    with torch.cuda.stream(gcu.new_stream(ctx.rank)):
+        return measure_backward(ctx, args, ctx.rank)
+
+
+def measure_backward(ctx, args, dev):
+    P, E, H, T = ctx.size, args.experts, args.hidden, args.tokens
+    G = P * E
+    k = min(args.topk, G)
+    rows = T * k
+    cap = P * rows
+    rb = H * 2
+    # Plain, the backward stages expert_out and the gradient rows: room for two holders' worth.
+    cc = gcu.CudaContext(ctx, dev, stage_bytes=(2 * cap + 2048) * rb)
+    moe = MoEDispatcher(ctx, cc)
+    g = torch.Generator(device="cuda").manual_seed(991 + ctx.rank)
+    x = torch.randn(T, H, device="cuda", generator=g).to(torch.bfloat16)
+    dy = torch.randn(T, H, device="cuda", generator=g).to(torch.bfloat16)
+    w, idx = torch.topk(torch.softmax(torch.randn(T, G, device="cuda", generator=g), -1), k, dim=-1)
+    tokens, splits, pos = moe.route(x, idx, E)  # every choice is routed: pos is a permutation
+    eo = {"symmetric": cc.empty((cap, H), torch.bfloat16)}
+    _, osp, ooff = moe.dispatch_dev(tokens, splits, eo["symmetric"], experts=E)  # identity experts
+    eo["plain"] = eo["symmetric"].clone()
+    mk = {"symmetric": lambda shape: cc.empty(shape, torch.bfloat16),
+          "plain": lambda shape: torch.empty(shape, dtype=torch.bfloat16, device="cuda")}
+    backs = {kind: mk[kind]((rows, H)) for kind in eo}
+    gins = {kind: mk[kind]((rows, H)) for kind in eo}
+    geos = {kind: [mk[kind]((cap, H)).zero_() for _ in range(2)] for kind in eo}
+    gws = {kind: [torch.empty((T, k), device="cuda") for _ in range(2)] for kind in eo}
+    flat = pos.view(-1)
+
+    def composed(kind):
+        back = backs[kind]
+        moe.combine_dev(eo[kind], osp, ooff, back, experts=E)
+        xr = back.index_select(0, flat).view(T, k, H)
+        gws[kind][0].copy_((xr.float() * dy.float()[:, None, :]).sum(-1))
+        scaled = (w[:, :, None] * dy.float()[:, None, :]).to(torch.bfloat16)
+        gins[kind].index_copy_(0, flat, scaled.view(rows, H))
+        moe.dispatch_dev(gins[kind], splits, geos[kind][0], experts=E)
+
+    def fused(kind):
+        moe.combine_dev_topk_backward(dy, eo[kind], splits, pos, w, geos[kind][1], gws[kind][1], experts=E)
+
+    res = {}
+    for kind in eo:
+        composed(kind)
+        fused(kind)
+        cc.synchronize()
+        assert torch.equal(geos[kind][0].view(torch.int16), geos[kind][1].view(torch.int16)), kind
+        xr = backs[kind].index_select(0, flat).view(T, k, H).float()
+        bound = H * 2.0 ** -23 * (xr.abs() * dy.float().abs()[:, None, :]).sum(-1)
+        assert bool(((gws[kind][0] - gws[kind][1]).abs() <= bound).all()), kind
+        times = {"composed": [], "fused": []}
+        for _ in range(args.iters):
+            for arm, fn in (("composed", composed), ("fused", fused)):
+                cc.pc.host_barrier()
+                t0 = time.perf_counter()
+                fn(kind)
+                cc.synchronize()
+                times[arm].append((time.perf_counter() - t0) * 1e3)
+        res[f"composed_{kind}"] = statistics.median(times["composed"])
+        res[f"fused_{kind}"] = statistics.median(times["fused"])
+        cc.pc.host_barrier()
+    res["bytes"] = 2 * rows * rb
+    return res
+
+
 def run_rank_dispatch_topk(ctx, args, shared):
     if shared:
         return measure_dispatch_topk(ctx, args, 0)
@@ -357,7 +437,7 @@ def main():
     ap.add_argument("--hidden", type=int, default=7168)
     ap.add_argument("--experts", type=int, default=8, help="local experts per rank")
     ap.add_argument("--iters", type=int, default=20)
-    ap.add_argument("--tables", default="pairs,fp8,combine,dispatch", help="comma-separated tables to run")
+    ap.add_argument("--tables", default="pairs,fp8,combine,dispatch,backward", help="comma-separated tables to run")
     args = ap.parse_args()
     tables = set(args.tables.split(","))
     assert torch.cuda.is_available(), "needs a GPU"
@@ -416,6 +496,19 @@ def main():
             c, t = r[f"{arm}_composed"], r[f"{arm}_topk"]
             print(f"{arm:>14} {c:12.3f} {t:9.3f} {c / t:9.2f} {r['bytes_avoided'] / 1e6:11.1f}", flush=True)
         print(json.dumps({"table": "topk_dispatch", "ranks": P, "shared_gpu": shared, **r}), flush=True)
+
+    if "backward" in tables:
+        print(f"# top-k combine backward, bf16 ({label}{note}); median of {args.iters} calls (rank 0), arms "
+              "alternating, grad_expert_out checked equal, grad_w within the fp32 summation bound", flush=True)
+        if shared:
+            r = gb.spawn_threads(P, run_rank_backward, args, True, cuda_device=0, timeout_ms=300000)[0]
+        else:
+            r = gb.spawn_threads(P, run_rank_backward, args, False, timeout_ms=300000)[0]
+        print(f"{'tensors':>10} {'composed ms':>12} {'fused ms':>9} {'speed-up':>9} {'MB/rank':>9}")
+        for kind in ("symmetric", "plain"):
+            c, t = r[f"composed_{kind}"], r[f"fused_{kind}"]
+            print(f"{kind:>10} {c:12.3f} {t:9.3f} {c / t:9.2f} {r['bytes'] / 1e6:9.1f}", flush=True)
+        print(json.dumps({"table": "topk_combine_backward", "ranks": P, "shared_gpu": shared, **r}), flush=True)
 
 
 if __name__ == "__main__":

@@ -43,6 +43,9 @@ KERNELS = [
     ("combine_topk_bf16", r"moeCombineTopkKernel<__nv_bfloat16>"),
     ("combine_topk_f16", r"moeCombineTopkKernel<__half>"),
     ("combine_topk_f32", r"moeCombineTopkKernel<float>"),
+    ("combine_topk_backward_bf16", r"moeCombineTopkBackwardKernel<__nv_bfloat16>"),
+    ("combine_topk_backward_f16", r"moeCombineTopkBackwardKernel<__half>"),
+    ("combine_topk_backward_f32", r"moeCombineTopkBackwardKernel<float>"),
     ("dispatch_topk", r"moeDispatchTopkKernel<false>"),
     ("dispatch_topk_fp8", r"moeDispatchTopkKernel<true>"),
     ("p2p_sendrecv", r"p2pKernel"),
