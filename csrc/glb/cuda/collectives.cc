@@ -1077,6 +1077,96 @@ void alltoallvDevCombineTopkBackward(PeerContext& pc, const MoeOut& gradExpertOu
   finish(pc, stream, name);
 }
 
+MoeLLLayout moeLLLayout(int nranks, int experts, int maxTokens, int topk, size_t hidden, size_t elemBytes, bool fp8) {
+  const char* name = "moe_ll_buffer";
+  GLB_ENFORCE(nranks >= 1 && nranks <= kMaxRanks, name, ": at most ", kMaxRanks, " ranks, got ", nranks);
+  checkTopk(name, topk);
+  GLB_ENFORCE(maxTokens >= 1 && static_cast<int64_t>(maxTokens) * topk <= 0x7fffffffll, name,
+              ": max_tokens must be at least 1 and max_tokens x topk at most 2^31 - 1, got ", maxTokens, " x ", topk);
+  GLB_ENFORCE(!fp8 || elemBytes == 2, name, ": the quantising form takes bfloat16 rows");
+  checkMoeLimits(name, experts, 1, fp8 ? hidden : hidden * elemBytes, fp8 ? kFp8Block : 16);
+  MoeLLLayout l{};
+  l.rowBytes = fp8 ? hidden : hidden * elemBytes;
+  l.scaleBytes = fp8 ? hidden / kFp8Block * sizeof(float) : 0;
+  l.combineRowBytes = hidden * elemBytes;
+  const unsigned long long slots = static_cast<unsigned long long>(experts) * nranks * maxTokens;
+  const unsigned long long choices = static_cast<unsigned long long>(maxTokens) * topk;
+  unsigned long long at = 0;
+  auto take = [&](unsigned long long n) {
+    const unsigned long long o = at;
+    at += (n + 15) / 16 * 16;
+    return o;
+  };
+  l.slots = take(slots * l.rowBytes);
+  l.scales = take(slots * l.scaleBytes);
+  l.tags = take(slots * sizeof(int32_t));
+  l.dispatchSig = take(static_cast<unsigned long long>(experts) * nranks * 8);
+  l.combineSlots = take(choices * l.combineRowBytes);
+  l.combineSig = take(static_cast<unsigned long long>(nranks) * 8);
+  l.choices = take(choices * sizeof(int32_t));
+  l.ctrl = take(16);
+  l.bytes = at;
+  l.experts = experts;
+  l.maxTokens = maxTokens;
+  l.topk = topk;
+  l.fp8 = fp8 ? 1 : 0;
+  return l;
+}
+
+namespace {
+MoeLLArgs moeLLArgs(PeerContext& pc, const char* name, const PeerBuffer& buf, size_t offset, const MoeLLLayout& l) {
+  GLB_ENFORCE(offset % 16 == 0 && offset + l.bytes <= buf.bytes, name, ": the buffer (", l.bytes,
+              " bytes) does not fit the registration at offset ", offset);
+  MoeLLArgs L{};
+  L.bufs = buf.ptrsAt(offset);
+  L.l = l;
+  L.status = pc.inputStatusDevice();
+  return L;
+}
+}  // namespace
+
+void alltoallvLLTopk(PeerContext& pc, const PeerBuffer& buf, size_t offset, const MoeLLLayout& l, const void* x,
+                     size_t tokens, const int64_t* topkIdx, void* out, float* outScales, int64_t* outSplits,
+                     cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  GLB_TRACE_RANGE("glb::cuda::alltoallv_ll_topk");
+  const char* name = "alltoallv_ll_topk";
+  GLB_ENFORCE(tokens <= static_cast<size_t>(l.maxTokens), name, ": ", tokens, " tokens; the buffer holds max_tokens = ",
+              l.maxTokens);
+  GLB_ENFORCE(out != nullptr && outSplits != nullptr && (!l.fp8 || outScales != nullptr) &&
+                  (tokens == 0 || (x != nullptr && topkIdx != nullptr)),
+              name, ": missing x, topk_idx, out, out_scales or out_splits");
+  checkAligned16(name, x, out, "x and out");
+  const MoeLLArgs L = moeLLArgs(pc, name, buf, offset, l);
+  const int blocks = moeBlocks(pc, moeLLDispatchKernelPtr(l.fp8 != 0));
+  prologue(pc, stream);
+  launchMoeLLDispatch(pc.comm(), L, x, tokens, reinterpret_cast<const long long*>(topkIdx), out, outScales,
+                      reinterpret_cast<long long*>(outSplits), blocks, stream);
+  finish(pc, stream, name);
+}
+
+void alltoallvLLCombineTopk(PeerContext& pc, const PeerBuffer& buf, size_t offset, const MoeLLLayout& l, void* y,
+                            size_t tokens, const void* expertOut, const float* weights, DataType dt,
+                            cudaStream_t stream) {
+  DeviceGuard g(pc.device);
+  GLB_TRACE_RANGE("glb::cuda::alltoallv_ll_combine_topk");
+  const char* name = "alltoallv_ll_combine_topk";
+  GLB_ENFORCE(dt == DataType::FLOAT32 || dt == DataType::BFLOAT16 || dt == DataType::FLOAT16, name,
+              ": rows must be float32, bfloat16 or float16");
+  GLB_ENFORCE(l.combineRowBytes % 16 == 0, name, ": rows must be a multiple of 16 bytes");
+  GLB_ENFORCE(tokens <= static_cast<size_t>(l.maxTokens), name, ": ", tokens, " tokens; the buffer holds max_tokens = ",
+              l.maxTokens);
+  GLB_ENFORCE(expertOut != nullptr && (tokens == 0 || y != nullptr), name, ": missing expert_out or y");
+  checkAligned16(name, y, expertOut, "y and expert_out");
+  const MoeLLArgs L = moeLLArgs(pc, name, buf, offset, l);
+  // Sized like the dispatch, whose CTAs need more of an SM: ranks sharing a GPU may run one rank's
+  // dispatch beside the others' combines, and every CTA of that dispatch must still be resident.
+  const int blocks = moeBlocks(pc, moeLLDispatchKernelPtr(l.fp8 != 0));
+  prologue(pc, stream);
+  launchMoeLLCombine(pc.comm(), L, expertOut, weights, y, tokens, dt, blocks, stream);
+  finish(pc, stream, name);
+}
+
 void scatter(PeerContext& pc, const void* in, const PeerBuffer& out, size_t outOffset, size_t bytes, int root,
              cudaStream_t stream) {
   DeviceGuard g(pc.device);

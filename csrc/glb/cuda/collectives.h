@@ -14,6 +14,7 @@
 #include <string>
 #include <vector>
 
+#include "glb/cuda/kernels.h"
 #include "glb/cuda/peer_context.h"
 #include "glb/cuda/tuning.h"
 #include "glb/types.h"
@@ -217,6 +218,32 @@ void alltoallvDevCombineTopkBackward(PeerContext& pc, const MoeOut& gradExpertOu
                                      const int64_t* pos, const float* weights, const int64_t* splits,
                                      size_t capacityRows, size_t rowBytes, DataType dt, int experts, int align,
                                      cudaStream_t stream);
+// Low-latency top-k MoE exchange for decoding (moe_kernels.cu): fixed per-(expert, source) slots in a
+// buffer every rank allocates with the same arguments, one signal round each way, no barrier, static
+// shapes. The layout of that buffer for P ranks, E experts per rank, max_tokens tokens per rank, top-k
+// and rows of `hidden` elements of `elemBytes` (fp8: bf16 in, e4m3 codes + fp32 scales per 128 in the
+// slots, bf16 combine rows). Every region starts at a multiple of 16 bytes:
+//   E·P·max_tokens dispatch rows of rowBytes, their scales (fp8) and int32 tags; E·P 64-bit dispatch
+//   words; max_tokens·k combine rows; P 64-bit combine words; max_tokens·k int32 choice marks; 16
+//   bytes of call count and ticket.
+// Limits: 1 <= E <= 32, 1 <= k <= 32, max_tokens >= 1, max_tokens·k <= 2^31 - 1, rows a positive
+// multiple of 16 bytes (fp8: hidden a multiple of 128).
+MoeLLLayout moeLLLayout(int nranks, int experts, int maxTokens, int topk, size_t hidden, size_t elemBytes, bool fp8);
+// Dispatch on the buffer at `offset` of `buf` (symmetric, layout `l`): x (tokens <= max_tokens rows;
+// fp8: bf16), topkIdx int64 (tokens, k); out / outScales plain (E, P·max_tokens, ...) and outSplits
+// int64 (E·P). Expert e's rows land in out[e, 0 : sum_s outSplits[e·P + s]] in source order, then
+// by token and choice: the bytes of expert e's segment from alltoallvDevTopk. Rows past it are not
+// written. A (source, expert) group above max_tokens rows sends nothing and is raised on the source
+// and the holder at the next host call.
+void alltoallvLLTopk(PeerContext& pc, const PeerBuffer& buf, size_t offset, const MoeLLLayout& l, const void* x,
+                     size_t tokens, const int64_t* topkIdx, void* out, float* outScales, int64_t* outSplits,
+                     cudaStream_t stream);
+// Combine on the same buffer after its dispatch: expertOut (E, P·max_tokens, H) of dt in the
+// dispatch's out layout; y (tokens, H) of dt; weights float32 (tokens, k) or null (weight 1). y
+// equals alltoallvDevCombineTopk's on the same expert rows byte for byte.
+void alltoallvLLCombineTopk(PeerContext& pc, const PeerBuffer& buf, size_t offset, const MoeLLLayout& l, void* y,
+                            size_t tokens, const void* expertOut, const float* weights, DataType dt,
+                            cudaStream_t stream);
 // Fixed-size alltoall: every chunk is `bytes` long on every rank (this is known to all
 // ranks, so the small-message LL kernel and size-dependent grids are safe here).
 void alltoall(PeerContext& pc, const void* in, const PeerBuffer& out, size_t outOffset, size_t bytes,

@@ -30,12 +30,14 @@ enum InputCode : uint32_t {
   kInputOk = 0,
   kInputOverflow = 1,  // a destination needs more output rows than it has
   kInputInvalid = 2,   // a negative or oversized split, an offset out of range, or headers that differ
+  kInputSlotOverflow = 3,  // low-latency exchange: a (source, expert) group has more rows than max_tokens
 };
 struct InputStatus {
   uint32_t code;             // InputCode; written last, cleared by the host when it raises
-  uint32_t rank;             // the overflowing destination
+  uint32_t rank;             // the overflowing destination (slot overflow: the source)
   unsigned long long need;   // rows it needs
-  unsigned long long avail;  // rows it has
+  unsigned long long avail;  // rows it has (slot overflow: max_tokens)
+  uint32_t expert;           // slot overflow: the global expert index j·E + e
 };
 
 // One per rank, at the start of its symmetric pool. `flag[b][s]` is written by

@@ -166,6 +166,47 @@ void launchMoeCombineTopkBackward(const CommArgs& a, const PeerPtrs& srcs, const
 void launchMoeDispatchTopk(const CommArgs& a, const PeerPtrs& outs, const MoeArgs& d, const MoeScales* scales,
                            const void* x, size_t tokens, int topk, const long long* idx, long long* splits,
                            long long* pos, long long* outSplits, long long* outOffsets, int blocks, cudaStream_t stream);
+// Low-latency top-k exchange for decoding: fixed per-(expert, source) slots instead of a layout agreed
+// at a barrier. Every rank owns one buffer of the same layout (symmetric memory); offsets are bytes
+// from its start, each a multiple of 16. See moe_kernels.cu for the protocol.
+struct MoeLLLayout {
+  unsigned long long rowBytes;         // a dispatch slot row: H elements, or H e4m3 codes (fp8)
+  unsigned long long scaleBytes;       // its fp32 scales: H / 128 · 4 (fp8), else 0
+  unsigned long long combineRowBytes;  // a combine slot row, and a row of y
+  unsigned long long slots;            // E · P · maxTokens dispatch rows, [e][s][r]
+  unsigned long long scales;           // their scales (fp8)
+  unsigned long long tags;             // int32 t·k + j of each dispatch row
+  unsigned long long dispatchSig;      // E · P 64-bit words, [e][s]
+  unsigned long long combineSlots;     // maxTokens · topk combine rows, by t·k + j
+  unsigned long long combineSig;       // P 64-bit words, [holder]
+  unsigned long long choices;          // int32 per (t, j) of my last dispatch: routed and sent (>= 0) or -1
+  unsigned long long ctrl;             // uint32 call count, uint32 completion ticket
+  unsigned long long bytes;            // the whole buffer
+  int experts, maxTokens, topk, fp8;
+};
+struct MoeLLArgs {
+  PeerPtrs bufs;        // rank r's buffer
+  MoeLLLayout l;
+  InputStatus* status;  // host-mapped
+};
+// The signal word a rank stores for call `seq` (the buffer's call count + 1) of `form` with `count`
+// rows; exposed for the loopback self-test, which stands in for the virtual peers.
+enum MoeLLForm : uint32_t { kMoeLLDispatch = 1, kMoeLLDispatchFp8 = 2, kMoeLLCombine = 3 };
+unsigned long long moeLLSignal(uint32_t seq, uint32_t form, uint32_t count);
+// Low-latency dispatch: route x's `tokens` rows by idx ((tokens, topk) int64) and push each routed
+// choice to slot (e, me, r) of rank j, r its rank in its group in (token, choice) order; then receive
+// and pack expert e's rows into out[e, 0 : n] (out: E · P · maxTokens rows of rowBytes, plain), in
+// source order, writing outSplits[e·P + s] (int64). fp8: x is bf16, out holds codes and outScales
+// the fp32 scales.
+void launchMoeLLDispatch(const CommArgs& a, const MoeLLArgs& L, const void* x, size_t tokens, const long long* idx,
+                         void* out, float* outScales, long long* outSplits, int blocks, cudaStream_t stream);
+// Low-latency combine: every packed row of my experts (expertOut, the dispatch's out layout, dt)
+// goes back to its source's combine slot; then y[t] = round(sum over my routed, sent choices j of
+// weights[t, j] · float(row)), as launchMoeCombineTopk (null weights: 1).
+void launchMoeLLCombine(const CommArgs& a, const MoeLLArgs& L, const void* expertOut, const float* weights, void* y,
+                        size_t tokens, DataType dt, int blocks, cudaStream_t stream);
+const void* moeLLDispatchKernelPtr(bool fp8);
+const void* moeLLCombineKernelPtr(DataType dt);
 const void* alltoallvDevKernelPtr(bool fp8 = false);
 const void* moeCombineTopkKernelPtr(DataType dt);
 const void* moeCombineTopkBackwardKernelPtr(DataType dt);

@@ -628,6 +628,16 @@ __device__ __forceinline__ unsigned long long topkHolderRow(const unsigned long 
   holder = lo / E;
   return sDst[lo] + (p - sSrc[lo]);
 }
+
+// The combines' accumulate step: acc += w · float(x) for each element of a 16-byte pack, a correctly
+// rounded fp32 multiply, then a correctly rounded add (never contracted to a fused multiply-add).
+template <typename T>
+__device__ __forceinline__ void topkAccumulate(typename PackTraits<T>::AccPack& acc, float w, const Pack16& x) {
+  using PT = PackTraits<T>;
+  const typename PT::AccPack xf = PT::widen(x);
+#pragma unroll
+  for (int i = 0; i < PT::kElems; i++) acc.v[i] = __fadd_rn(acc.v[i], __fmul_rn(w, xf.v[i]));
+}
 }  // namespace
 
 template <typename T>
@@ -695,11 +705,7 @@ moeCombineTopkKernel(CommArgs a, PeerPtrs srcs, const long long* splits, const l
           for (int c = 0; c < kTopkInFlight; c++) {
             if (s[c] == nullptr) continue;
 #pragma unroll
-            for (int u = 0; u < kTopkPacks; u++) {
-              const typename PT::AccPack xf = PT::widen(x[c][u]);
-#pragma unroll
-              for (int i = 0; i < PT::kElems; i++) acc[u].v[i] = __fadd_rn(acc[u].v[i], __fmul_rn(ws[c], xf.v[i]));
-            }
+            for (int u = 0; u < kTopkPacks; u++) topkAccumulate<T>(acc[u], ws[c], x[c][u]);
           }
         }
 #pragma unroll
@@ -939,6 +945,111 @@ static_assert(kThreads >= kMaxRanks * kMaxA2aExperts, "one scan slot per group")
 
 __device__ __forceinline__ int topkGroup(long long v, int K) { return v >= 0 && v < K ? static_cast<int>(v) : K; }
 
+namespace {
+// Route, first half: the routed choices of every group g over all `n` choices (sTot[g]), route()'s
+// first row of g (sSrc[g], their exclusive prefix) and the choices of g before choice `lo`, where my
+// CTA's slice starts (sRun[g]). `totals(g)` runs for each g on thread g once sTot[g] is final.
+template <typename Totals>
+__device__ __forceinline__ void topkRouteCount(const long long* idx, unsigned long long n, unsigned long long lo, int K,
+                                               uint32_t* sTot, uint32_t* sRun, unsigned long long* sSrc,
+                                               unsigned long long* sWarp, Totals&& totals) {
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  for (int g = t; g < K; g += blockDim.x) sTot[g] = sRun[g] = 0u;
+  __syncthreads();
+  for (unsigned long long b = static_cast<unsigned long long>(warp) * 32; b < n; b += blockDim.x) {
+    const unsigned long long i = b + lane;
+    const int g = i < n ? topkGroup(idx[i], K) : K;
+    const bool before = i < lo;
+    const unsigned m = __match_any_sync(0xffffffffu, 2 * g + (before ? 1 : 0));
+    if (g < K && lane == __ffs(m) - 1) {
+      atomicAdd(&sTot[g], static_cast<uint32_t>(__popc(m)));
+      if (before) atomicAdd(&sRun[g], static_cast<uint32_t>(__popc(m)));
+    }
+  }
+  __syncthreads();
+  unsigned long long routed;
+  const unsigned long long first = blockExclusiveScan(t < K ? sTot[t] : 0u, sWarp, routed);
+  if (t < K) {
+    sSrc[t] = first;
+    totals(t);
+  }
+  __syncthreads();
+}
+
+// Route, second half: rank the choices [lo, hi) of my slice in (token, choice) order, within a warp by
+// __match_any_sync, across the warps of a round in warp order through the running counts sRun.
+// `emit(i, g, p)` gets choice i's group (K: not routed) and pos (-1: not routed).
+template <typename Emit>
+__device__ __forceinline__ void topkRouteRank(const long long* idx, unsigned long long lo, unsigned long long hi, int K,
+                                              const unsigned long long* sSrc, uint32_t* sRun, Emit&& emit) {
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5, nw = blockDim.x >> 5;
+  for (unsigned long long b = lo; b < hi; b += blockDim.x) {
+    const unsigned long long i = b + t;
+    const int g = i < hi ? topkGroup(idx[i], K) : K;
+    const unsigned m = __match_any_sync(0xffffffffu, g);
+    const unsigned below = m & ((1u << lane) - 1u);
+    long long p = -1;
+    for (int w = 0; w < nw; w++) {
+      if (warp == w && g < K) {
+        const uint32_t r = sRun[g];
+        __syncwarp(m);
+        if (below == 0u) sRun[g] = r + static_cast<uint32_t>(__popc(m));
+        p = static_cast<long long>(sSrc[g] + r + static_cast<uint32_t>(__popc(below)));
+      }
+      __syncthreads();
+    }
+    if (i < hi) emit(i, g, p);
+  }
+}
+
+// Push one token's row `src` (rb bytes; quantising: rb / 128 bf16 blocks of 2 · 128 bytes) to every
+// choice c < topk whose lane holds a destination `dst` (and, quantising, its scales `dsc`): each
+// 16-byte pack, or each 128-element block, is read and quantised once. Called by the whole warp.
+template <bool kQuant>
+__device__ __forceinline__ void topkPushRow(const char* src, unsigned long long rb, int lane, int topk, char* dst,
+                                            float* dsc) {
+  if constexpr (kQuant) {
+    // Half-warps take 128-element blocks, as quantCopy: one amax and one set of codes per block.
+    const unsigned long long nblk = rb / kFp8Block;
+    for (unsigned long long b0 = 0; b0 < nblk; b0 += 2 * kQuantUnroll) {
+      uint2 c[kQuantUnroll];
+      float amax[kQuantUnroll];
+      quantStep(src, b0, nblk, lane, [&](int u, unsigned long long, uint2 cu, float au) {
+        c[u] = cu;
+        amax[u] = au;
+      });
+      for (int ch = 0; ch < topk; ch++) {
+        char* q = reinterpret_cast<char*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(dst), ch));
+        float* qs = reinterpret_cast<float*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(dsc), ch));
+        if (q == nullptr) continue;
+#pragma unroll
+        for (int u = 0; u < kQuantUnroll; u++) quantStore(q, qs, b0 + 2 * u + (lane >> 4), nblk, lane, c[u], amax[u]);
+      }
+    }
+  } else {
+    const unsigned long long npk = rb / 16;
+    // Warp-uniform trip count: every lane takes part in the shuffles, lanes past the row end idle.
+    for (unsigned long long v0 = lane; v0 - lane < npk; v0 += 32 * kTopkPushUnroll) {
+      Pack16 xv[kTopkPushUnroll];
+#pragma unroll
+      for (int u = 0; u < kTopkPushUnroll; u++) {
+        const unsigned long long pk = v0 + 32ull * u;
+        if (pk < npk) xv[u] = ld128_stream(src + pk * 16);
+      }
+      for (int ch = 0; ch < topk; ch++) {
+        char* q = reinterpret_cast<char*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(dst), ch));
+        if (q == nullptr) continue;
+#pragma unroll
+        for (int u = 0; u < kTopkPushUnroll; u++) {
+          const unsigned long long pk = v0 + 32ull * u;
+          if (pk < npk) st128_stream(q + pk * 16, xv[u]);
+        }
+      }
+    }
+  }
+}
+}  // namespace
+
 template <bool kQuant>
 __global__ void __launch_bounds__(kThreads)
 moeDispatchTopkKernel(CommArgs a, PeerPtrs outs, const char* x, const long long* idx, long long* splits, long long* pos,
@@ -959,48 +1070,14 @@ moeDispatchTopkKernel(CommArgs a, PeerPtrs outs, const char* x, const long long*
   const unsigned long long rb = d.rowBytes, k = static_cast<unsigned long long>(topk);
 
   // ---- route: counts, then pos of my slice ----
-  const unsigned long long n = tokens * k;
   const unsigned long long per = (tokens + gridDim.x - 1) / gridDim.x;
   const unsigned long long tok0 = min(tokens, blockIdx.x * per), tok1 = min(tokens, tok0 + per);
   const unsigned long long lo = tok0 * k, hi = tok1 * k;
-  for (int g = t; g < K; g += blockDim.x) sTot[g] = sRun[g] = 0u;
-  __syncthreads();
-  for (unsigned long long b = static_cast<unsigned long long>(warp) * 32; b < n; b += blockDim.x) {
-    const unsigned long long i = b + lane;
-    const int g = i < n ? topkGroup(idx[i], K) : K;
-    const bool before = i < lo;
-    const unsigned m = __match_any_sync(0xffffffffu, 2 * g + (before ? 1 : 0));
-    if (g < K && lane == __ffs(m) - 1) {
-      atomicAdd(&sTot[g], static_cast<uint32_t>(__popc(m)));
-      if (before) atomicAdd(&sRun[g], static_cast<uint32_t>(__popc(m)));
-    }
-  }
-  __syncthreads();
-  unsigned long long routed;
-  const unsigned long long first = blockExclusiveScan(t < K ? sTot[t] : 0u, sWarp, routed);
-  if (t < K) {
-    sSrc[t] = first;
-    sAux[t] = sTot[t];
-    if (blockIdx.x == 0) splits[t] = sTot[t];
-  }
-  __syncthreads();
-  for (unsigned long long b = lo; b < hi; b += blockDim.x) {
-    const unsigned long long i = b + t;
-    const int g = i < hi ? topkGroup(idx[i], K) : K;
-    const unsigned m = __match_any_sync(0xffffffffu, g);
-    const unsigned below = m & ((1u << lane) - 1u);
-    long long p = -1;
-    for (int w = 0; w < nw; w++) {
-      if (warp == w && g < K) {
-        const uint32_t r = sRun[g];
-        __syncwarp(m);
-        if (below == 0u) sRun[g] = r + static_cast<uint32_t>(__popc(m));
-        p = static_cast<long long>(sSrc[g] + r + static_cast<uint32_t>(__popc(below)));
-      }
-      __syncthreads();
-    }
-    if (i < hi) pos[i] = p;
-  }
+  topkRouteCount(idx, tokens * k, lo, K, sTot, sRun, sSrc, sWarp, [&](int g) {
+    sAux[g] = sTot[g];
+    if (blockIdx.x == 0) splits[g] = sTot[g];
+  });
+  topkRouteRank(idx, lo, hi, K, sSrc, sRun, [&](unsigned long long i, int, long long p) { pos[i] = p; });
 
   // ---- agree on my splits; the layout ----
   bool invalid;
@@ -1029,47 +1106,7 @@ moeDispatchTopkKernel(CommArgs a, PeerPtrs outs, const char* x, const long long*
           }
         }
       }
-      if constexpr (kQuant) {
-        // Half-warps take 128-element blocks, as quantCopy: one amax and one set of codes per block.
-        const unsigned long long nblk = rb / kFp8Block;
-        const char* src = x + tok * rb * 2;
-        for (unsigned long long b0 = 0; b0 < nblk; b0 += 2 * kQuantUnroll) {
-          uint2 c[kQuantUnroll];
-          float amax[kQuantUnroll];
-          quantStep(src, b0, nblk, lane, [&](int u, unsigned long long, uint2 cu, float au) {
-            c[u] = cu;
-            amax[u] = au;
-          });
-          for (int ch = 0; ch < topk; ch++) {
-            char* q = reinterpret_cast<char*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(dst), ch));
-            float* qs = reinterpret_cast<float*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(dsc), ch));
-            if (q == nullptr) continue;
-#pragma unroll
-            for (int u = 0; u < kQuantUnroll; u++) quantStore(q, qs, b0 + 2 * u + (lane >> 4), nblk, lane, c[u], amax[u]);
-          }
-        }
-      } else {
-        const unsigned long long npk = rb / 16;
-        const char* src = x + tok * rb;
-        // Warp-uniform trip count: every lane takes part in the shuffles, lanes past the row end idle.
-        for (unsigned long long v0 = lane; v0 - lane < npk; v0 += 32 * kTopkPushUnroll) {
-          Pack16 xv[kTopkPushUnroll];
-#pragma unroll
-          for (int u = 0; u < kTopkPushUnroll; u++) {
-            const unsigned long long pk = v0 + 32ull * u;
-            if (pk < npk) xv[u] = ld128_stream(src + pk * 16);
-          }
-          for (int ch = 0; ch < topk; ch++) {
-            char* q = reinterpret_cast<char*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(dst), ch));
-            if (q == nullptr) continue;
-#pragma unroll
-            for (int u = 0; u < kTopkPushUnroll; u++) {
-              const unsigned long long pk = v0 + 32ull * u;
-              if (pk < npk) st128_stream(q + pk * 16, xv[u]);
-            }
-          }
-        }
-      }
+      topkPushRow<kQuant>(x + tok * rb * (kQuant ? 2 : 1), rb, lane, topk, dst, dsc);
     }
   }
   a2aFinish<kQuant>(a, ep, ok1 && !invalid, d, false, sRcv, sRcvCnt, sNeed, sCap, K,
@@ -1088,6 +1125,353 @@ void launchMoeDispatchTopk(const CommArgs& a, const PeerPtrs& outs, const MoeArg
                                                                   tokens, topk, d);
   }
 }
+
+// ---- low-latency top-k exchange: fixed slots, one signal round each way ------------------------
+// For decoding, where a layer moves a handful of rows and the variable layout's barriers dominate.
+// Every rank owns a buffer of one layout (MoeLLLayout, agreed on the host when it is created), so
+// nothing about shapes is agreed on the device: expert e of rank j has a fixed slot range
+// [e][s][0, maxTokens) for each source s, and a source writes there without asking.
+//   dispatch  route (as moeDispatchTopkKernel); push each routed choice of group g = j·E + e to slot
+//             (e, me, r) of rank j, r its rank in g in (token, choice) order, with the int32 tag t·k + c;
+//             a group with more than maxTokens rows (a token that picks an expert twice) sends nothing
+//             and its choices are marked unsent. Local grid sync, then one release word per (j, e):
+//             [e][me] on rank j = (call, form, rows). Wait for my E·P words of this call, pack expert
+//             e's rows into out[e] in source order, write out_splits.
+//   combine   every packed row of my experts goes to its source's combine slot named by its tag;
+//             local grid sync, one release word to each source; wait for my P words and sum each
+//             token's sent choices with its weights, as moeCombineTopkKernel.
+// Waits are bounded by the context timeout and the abort word, as every barrier is. The call count
+// lives in the buffer: every CTA reads it at entry and the last CTA to finish advances it, so CUDA
+// graph replays keep counting. Dispatch and combine alternate on a buffer (the host enforces it):
+// a source's next dispatch starts only after its combine has seen every holder's word, which each
+// holder sends after it has read its slots and tags, so one set of slots serves every call.
+namespace {
+__device__ __forceinline__ void st_release_sys_u64(unsigned long long* p, unsigned long long v) {
+  asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long ld_acquire_sys_u64(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// A signal word: bits 63..36 the call (count + 1, modulo 2^28), 35..32 the form, 31..0 the rows. A
+// word is only ever compared for equality with the call a reader expects; the stale word it replaces
+// is two calls older, and a fresh buffer's zero never names a call.
+__host__ __device__ __forceinline__ unsigned long long llWord(uint32_t seq, uint32_t form, uint32_t count) {
+  return (static_cast<unsigned long long>(((seq & 0x0fffffffu) << 4) | form) << 32) | count;
+}
+__device__ __forceinline__ bool llArrived(unsigned long long w, uint32_t seq) {
+  return static_cast<uint32_t>(w >> 36) == (seq & 0x0fffffffu);
+}
+__device__ __forceinline__ uint32_t llForm(unsigned long long w) { return static_cast<uint32_t>(w >> 32) & 15u; }
+
+__device__ __forceinline__ uint32_t llWaitSlow(const unsigned long long* w, uint32_t seq, uint32_t* abortWord,
+                                                   unsigned long long timeoutNs) {
+  const unsigned long long t0 = globalTimerNs();
+  uint32_t polls = 0;
+  while (!llArrived(ld_acquire_sys_u64(w), seq)) {
+    if ((++polls & 127u) == 0u) {
+      if (ld_relaxed_sys(abortWord) != 0u) return kAbortPeer;
+      if (timeoutNs != 0ull && globalTimerNs() - t0 > timeoutNs) {
+        atomicCAS(abortWord, 0u, static_cast<uint32_t>(kAbortTimeout));
+        return kAbortTimeout;
+      }
+    }
+  }
+  return 0u;
+}
+
+// Wait for call `seq`'s word at `w`, written by `peer`; false when the wait was abandoned.
+__device__ __forceinline__ bool llWait(const CommArgs& a, const unsigned long long* w, uint32_t seq, int peer,
+                                       unsigned long long& v) {
+  v = ld_acquire_sys_u64(w);
+  if (llArrived(v, seq)) return true;
+  const uint32_t rc = llWaitSlow(w, seq, &a.self->abort, a.timeoutNs);
+  if (rc == 0u) {
+    v = ld_acquire_sys_u64(w);
+    return true;
+  }
+  reportAbort(a, rc, peer);
+  return false;
+}
+
+// Thread 0 of CTA 0: raise an input error on the host, unless one is pending.
+__device__ __forceinline__ void llReport(InputStatus* status, uint32_t code, uint32_t source, uint32_t expert,
+                                         unsigned long long rows, unsigned long long maxTokens) {
+  volatile InputStatus* st = status;
+  if (st != nullptr && st->code == kInputOk) {
+    st->rank = source;
+    st->expert = expert;
+    st->need = rows;
+    st->avail = maxTokens;
+    __threadfence_system();
+    st->code = code;
+  }
+}
+
+// Every CTA at its end: the last one advances the buffer's call count.
+__device__ __forceinline__ void llRetire(uint32_t* ctrl) {
+  __syncthreads();
+  if (threadIdx.x == 0 && atomicAdd(&ctrl[1], 1u) == gridDim.x - 1) {
+    ctrl[1] = 0u;
+    ctrl[0] += 1u;
+  }
+}
+
+// My receive groups g = e·P + s from the dispatch words: sN[g] rows (0 for an overflowed group or a
+// word of another form) and sAll[g], their exclusive prefix over g; `bad` when a word is of another
+// form. Expert e's rows from source s start at row sAll[g] - sAll[e·P] of its packed segment.
+__device__ __forceinline__ bool llGroups(const unsigned long long* words, uint32_t form, unsigned long long M, int K,
+                                         uint32_t* sN, unsigned long long* sAll, unsigned long long* sWarp,
+                                         unsigned long long& total) {
+  const int t = threadIdx.x;
+  uint32_t n = 0u;
+  bool bad = false;
+  if (t < K) {
+    const unsigned long long w = ld_acquire_sys_u64(words + t);
+    bad = llForm(w) != form;
+    n = bad || static_cast<uint32_t>(w) > M ? 0u : static_cast<uint32_t>(w);
+    sN[t] = n;
+  }
+  const unsigned long long first = blockExclusiveScan(n, sWarp, total);
+  if (t < K) sAll[t] = first;
+  return __syncthreads_or(bad) != 0;
+}
+
+// The last group starting at or before packed row q (an empty group starts where the next one does).
+__device__ __forceinline__ int llGroupOf(const unsigned long long* sAll, int K, unsigned long long q) {
+  int lo = 0, hi = K - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (sAll[mid] <= q) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+}  // namespace
+
+unsigned long long moeLLSignal(uint32_t seq, uint32_t form, uint32_t count) { return llWord(seq, form, count); }
+
+template <bool kQuant>
+__global__ void __launch_bounds__(kThreads)
+moeLLDispatchKernel(CommArgs a, MoeLLArgs L, const char* x, const long long* idx, unsigned long long tokens, char* out,
+                    float* outScales, long long* outSplits) {
+  __shared__ unsigned long long sSrc[kMaxK];  // group g = j·E + e: route()'s first row of g
+  __shared__ uint32_t sTot[kMaxK];            //   routed choices of all my tokens
+  __shared__ uint32_t sRun[kMaxK];            //   of the tokens before my slice, then running
+  __shared__ uint32_t sN[kMaxK];              // my receive group e·P + s: rows
+  __shared__ unsigned long long sAll[kMaxK];  //   their exclusive prefix
+  __shared__ unsigned long long sWarp[32];
+  const int P = a.nranks, E = L.l.experts, K = P * E, me = a.rank, t = threadIdx.x;
+  const int lane = t & 31, warp = t >> 5, nw = blockDim.x >> 5;
+  const unsigned long long rb = L.l.rowBytes, sb = L.l.scaleBytes, k = L.l.topk, M = L.l.maxTokens;
+  char* mine = static_cast<char*>(L.bufs.p[me]);
+  uint32_t* ctrl = reinterpret_cast<uint32_t*>(mine + L.l.ctrl);
+  int* choices = reinterpret_cast<int*>(mine + L.l.choices);
+  const unsigned long long* words = reinterpret_cast<const unsigned long long*>(mine + L.l.dispatchSig);
+  const uint32_t seq = *reinterpret_cast<volatile uint32_t*>(ctrl) + 1u;
+  const uint32_t form = kQuant ? kMoeLLDispatchFp8 : kMoeLLDispatch;
+
+  // ---- 1. route: my slice's choices get their rank in their group, or -1 (not routed, overflow) ----
+  const unsigned long long per = (tokens + gridDim.x - 1) / gridDim.x;
+  const unsigned long long tok0 = min(tokens, blockIdx.x * per), tok1 = min(tokens, tok0 + per);
+  topkRouteCount(idx, tokens * k, tok0 * k, K, sTot, sRun, sSrc, sWarp, [](int) {});
+  topkRouteRank(idx, tok0 * k, tok1 * k, K, sSrc, sRun, [&](unsigned long long i, int g, long long p) {
+    choices[i] = p >= 0 && sTot[g] <= M ? static_cast<int>(p - static_cast<long long>(sSrc[g])) : -1;
+  });
+  __syncthreads();
+
+  // ---- 2. push: one warp per token of my slice, to slot (e, me, r) of rank j with its tag ----
+  for (unsigned long long tok = tok0 + warp; tok < tok1; tok += nw) {
+    char* dst = nullptr;
+    float* dsc = nullptr;
+    if (static_cast<unsigned long long>(lane) < k) {
+      const unsigned long long i = tok * k + lane;
+      const int r = choices[i];
+      if (r >= 0) {
+        const int g = topkGroup(idx[i], K), j = g / E, e = g % E;
+        const unsigned long long slot = (static_cast<unsigned long long>(e) * P + me) * M + r;
+        char* b = static_cast<char*>(L.bufs.p[j]);
+        dst = b + L.l.slots + slot * rb;
+        if constexpr (kQuant) dsc = reinterpret_cast<float*>(b + L.l.scales + slot * sb);
+        reinterpret_cast<int*>(b + L.l.tags)[slot] = static_cast<int>(i);
+      }
+    }
+    topkPushRow<kQuant>(x + tok * rb * (kQuant ? 2 : 1), rb, lane, static_cast<int>(k), dst, dsc);
+  }
+
+  // ---- 3. signal: word [e][me] on rank j ----
+  bool ok = localGridSync(a);
+  if (ok && blockIdx.x == 0 && t < K) {
+    const int j = t / E, e = t % E;
+    unsigned long long* w = reinterpret_cast<unsigned long long*>(static_cast<char*>(L.bufs.p[j]) + L.l.dispatchSig);
+    st_release_sys_u64(w + e * P + me, llWord(seq, form, sTot[t]));
+  }
+
+  // ---- 4. receive my E·P words, pack ----
+  if (ok) {
+    bool gone = false;
+    if (t < K) {
+      unsigned long long w;
+      gone = !llWait(a, words + t, seq, t % P, w);
+    }
+    ok = __syncthreads_or(gone) == 0;
+  }
+  if (ok) {
+    unsigned long long total;
+    const bool bad = llGroups(words, form, M, K, sN, sAll, sWarp, total);
+    if (!bad) {
+      const size_t gtid = static_cast<size_t>(blockIdx.x) * blockDim.x + t;
+      const size_t gthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
+      for (int g = 0; g < K; g++) {
+        const unsigned long long n = sN[g];
+        if (n == 0) continue;
+        const int e = g / P;
+        const unsigned long long row = static_cast<unsigned long long>(e) * P * M + (sAll[g] - sAll[e * P]);
+        gridCopy(out + row * rb, mine + L.l.slots + g * M * rb, n * rb, true, gtid, gthreads);
+        if constexpr (kQuant) {
+          gridCopy(reinterpret_cast<char*>(outScales) + row * sb, mine + L.l.scales + g * M * sb, n * sb, true, gtid,
+                   gthreads);
+        }
+      }
+      if (blockIdx.x == 0 && t < K) outSplits[t] = sN[t];
+    }
+    // An overflow is raised on its source and on its holder; the first error of a call wins.
+    if (blockIdx.x == 0 && t == 0) {
+      if (bad) llReport(L.status, kInputInvalid, 0u, 0u, 0ull, 0ull);
+      for (int g = 0; g < K; g++) {
+        if (sTot[g] > M) llReport(L.status, kInputSlotOverflow, me, g, sTot[g], M);
+      }
+      for (int g = 0; g < K && !bad; g++) {
+        const uint32_t n = static_cast<uint32_t>(words[g]);
+        if (n > M) llReport(L.status, kInputSlotOverflow, g % P, me * E + g / P, n, M);
+      }
+    }
+  }
+  llRetire(ctrl);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+moeLLCombineKernel(CommArgs a, MoeLLArgs L, const char* expertOut, const float* weights, char* y,
+                   unsigned long long tokens) {
+  using PT = PackTraits<T>;
+  __shared__ uint32_t sN[kMaxK];              // my receive group e·P + s: rows
+  __shared__ unsigned long long sAll[kMaxK];  //   their exclusive prefix
+  __shared__ unsigned long long sWarp[32];
+  const int P = a.nranks, me = a.rank, t = threadIdx.x, lane = t & 31;
+  const unsigned long long crb = L.l.combineRowBytes, k = L.l.topk, M = L.l.maxTokens;
+  // Derived from the parameters where they are used: little stays live across the grid sync's call.
+  auto mine = [&]() { return static_cast<char*>(L.bufs.p[me]); };
+  uint32_t* ctrl = reinterpret_cast<uint32_t*>(mine() + L.l.ctrl);
+  const uint32_t seq = *reinterpret_cast<volatile uint32_t*>(ctrl) + 1u;
+  const size_t gwarp = (static_cast<size_t>(blockIdx.x) * blockDim.x + t) / 32;
+  const size_t nwarps = static_cast<size_t>(gridDim.x) * blockDim.x / 32;
+
+  // ---- 1. holder push: packed row q of my experts goes to its source's combine slot, by its tag ----
+  {
+    const int K = P * L.l.experts;
+    const int* tags = reinterpret_cast<const int*>(mine() + L.l.tags);
+    unsigned long long total;
+    llGroups(reinterpret_cast<const unsigned long long*>(mine() + L.l.dispatchSig),
+             L.l.fp8 ? kMoeLLDispatchFp8 : kMoeLLDispatch, M, K, sN, sAll, sWarp, total);
+    for (unsigned long long q = gwarp; q < total; q += nwarps) {
+      const int g = llGroupOf(sAll, K, q), e = g / P, s = g % P;
+      const unsigned long long r = q - sAll[g];
+      const long long tag = tags[g * M + r];
+      if (tag < 0 || static_cast<unsigned long long>(tag) >= M * k) continue;
+      const char* src = expertOut + (static_cast<unsigned long long>(e) * P * M + (sAll[g] - sAll[e * P]) + r) * crb;
+      char* dst = static_cast<char*>(L.bufs.p[s]) + L.l.combineSlots + static_cast<unsigned long long>(tag) * crb;
+      for (unsigned long long pk = lane; pk < crb / 16; pk += 32) st128(dst + pk * 16, ld128(src + pk * 16));
+    }
+  }
+
+  // ---- 2. signal every source ----
+  bool ok = localGridSync(a);
+  const int* choices = reinterpret_cast<const int*>(mine() + L.l.choices);
+  const unsigned long long* cwords = reinterpret_cast<const unsigned long long*>(mine() + L.l.combineSig);
+  const unsigned long long npk = crb / 16;
+  if (ok && blockIdx.x == 0 && t < P) {
+    unsigned long long* w = reinterpret_cast<unsigned long long*>(static_cast<char*>(L.bufs.p[t]) + L.l.combineSig);
+    st_release_sys_u64(w + me, llWord(seq, kMoeLLCombine, 0u));
+  }
+
+  // ---- 3. wait for every holder, then sum each token's sent choices ----
+  bool bad = false;
+  if (ok) {
+    bool gone = false;
+    if (t < P) {
+      unsigned long long w;
+      gone = !llWait(a, cwords + t, seq, t, w);
+      bad = !gone && llForm(w) != kMoeLLCombine;
+    }
+    ok = __syncthreads_or(gone) == 0;
+    bad = __syncthreads_or(bad) != 0;
+  }
+  if (ok && !bad) {
+    for (unsigned long long tok = gwarp; tok < tokens; tok += nwarps) {
+      // Lane c < k: choice c's row in my combine slots and its weight, when it was sent.
+      const char* src = nullptr;
+      float w = 0.0f;
+      if (static_cast<unsigned long long>(lane) < k) {
+        const unsigned long long i = tok * k + lane;
+        if (choices[i] >= 0) {
+          src = mine() + L.l.combineSlots + i * crb;
+          w = weights != nullptr ? weights[i] : 1.0f;
+        }
+      }
+      // Warp-uniform trip count: every lane takes part in the shuffles, lanes past the row end idle.
+      for (unsigned long long pk = lane; pk - lane < npk; pk += 32) {
+        typename PT::AccPack acc;
+#pragma unroll
+        for (int i = 0; i < PT::kElems; i++) acc.v[i] = 0.0f;
+        for (int c = 0; c < static_cast<int>(k); c++) {
+          const char* sc = reinterpret_cast<const char*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(src), c));
+          const float wc = __shfl_sync(0xffffffffu, w, c);
+          if (sc != nullptr && pk < npk) topkAccumulate<T>(acc, wc, ld128(sc + pk * 16));
+        }
+        if (pk < npk) st128(y + tok * crb + pk * 16, PT::narrow(acc));
+      }
+    }
+  }
+  if (ok && bad && blockIdx.x == 0 && t == 0) llReport(L.status, kInputInvalid, 0u, 0u, 0ull, 0ull);
+  llRetire(ctrl);
+}
+
+namespace {
+using LLCombineFn = void (*)(CommArgs, MoeLLArgs, const char*, const float*, char*, unsigned long long);
+LLCombineFn llCombineFn(DataType dt) {
+  switch (dt) {
+    case DataType::FLOAT32: return moeLLCombineKernel<float>;
+    case DataType::BFLOAT16: return moeLLCombineKernel<__nv_bfloat16>;
+    case DataType::FLOAT16: return moeLLCombineKernel<__half>;
+    default: return nullptr;
+  }
+}
+}  // namespace
+
+void launchMoeLLDispatch(const CommArgs& a, const MoeLLArgs& L, const void* x, size_t tokens, const long long* idx,
+                         void* out, float* outScales, long long* outSplits, int blocks, cudaStream_t stream) {
+  const char* xc = static_cast<const char*>(x);
+  char* o = static_cast<char*>(out);
+  if (L.l.fp8) {
+    moeLLDispatchKernel<true><<<blocks, kThreads, 0, stream>>>(a, L, xc, idx, tokens, o, outScales, outSplits);
+  } else {
+    moeLLDispatchKernel<false><<<blocks, kThreads, 0, stream>>>(a, L, xc, idx, tokens, o, outScales, outSplits);
+  }
+}
+
+void launchMoeLLCombine(const CommArgs& a, const MoeLLArgs& L, const void* expertOut, const float* weights, void* y,
+                        size_t tokens, DataType dt, int blocks, cudaStream_t stream) {
+  llCombineFn(dt)<<<blocks, kThreads, 0, stream>>>(a, L, static_cast<const char*>(expertOut), weights,
+                                                   static_cast<char*>(y), tokens);
+}
+
+const void* moeLLDispatchKernelPtr(bool fp8) {
+  return fp8 ? reinterpret_cast<const void*>(moeLLDispatchKernel<true>)
+             : reinterpret_cast<const void*>(moeLLDispatchKernel<false>);
+}
+const void* moeLLCombineKernelPtr(DataType dt) { return reinterpret_cast<const void*>(llCombineFn(dt)); }
 
 const void* alltoallvDevKernelPtr(bool fp8) {
   return fp8 ? reinterpret_cast<const void*>(alltoallvDevKernel<true>)
@@ -1108,9 +1492,12 @@ void preloadMoeKernels() {
   for (DataType dt : {DataType::FLOAT32, DataType::BFLOAT16, DataType::FLOAT16}) {
     touchKernel(topkCombineFn(dt));
     touchKernel(topkCombineBackwardFn(dt));
+    touchKernel(llCombineFn(dt));
   }
   touchKernel(moeDispatchTopkKernel<false>);
   touchKernel(moeDispatchTopkKernel<true>);
+  touchKernel(moeLLDispatchKernel<false>);
+  touchKernel(moeLLDispatchKernel<true>);
   cudaGetLastError();
 }
 

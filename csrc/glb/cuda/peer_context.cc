@@ -263,6 +263,21 @@ std::vector<T> PeerContext::allgatherStruct(const T& mine) {
   return all;
 }
 
+bool PeerContext::hostAllSame(const std::vector<int64_t>& words) {
+  struct Words {
+    int64_t n;
+    int64_t w[16];
+  };
+  GLB_ENFORCE(words.size() <= 16, "hostAllSame: at most 16 words");
+  Words mine{};
+  mine.n = static_cast<int64_t>(words.size());
+  std::copy(words.begin(), words.end(), mine.w);
+  for (const Words& o : allgatherStruct(mine)) {
+    if (std::memcmp(&o, &mine, sizeof(Words)) != 0) return false;
+  }
+  return true;
+}
+
 void PeerContext::hostBarrier() {
   BarrierOptions o(context());
   o.setTag(nextTag());
@@ -423,7 +438,13 @@ void PeerContext::checkHealth() {
       if (code == kInputOk) return;
       const uint32_t who = in->rank;
       const unsigned long long need = in->need, avail = in->avail;
+      const uint32_t expert = in->expert;
       in->code = kInputOk;  // raised once; the next call starts clean
+      if (code == kInputSlotOverflow) {
+        GLB_THROW(InputException, "alltoallv_ll_topk: source rank ", who, " routed ", need, " rows to expert ", expert,
+                  " (index rank * experts + e) but a (source, expert) slot group holds max_tokens = ", avail,
+                  " rows; none of those rows were sent (a token picked that expert more than once)");
+      }
       if (code == kInputOverflow) {
         GLB_THROW(InputException, "alltoallv_dev: rank ", who, " needs ", need, " output rows but has room for ", avail,
                   "; no rows were sent to it");

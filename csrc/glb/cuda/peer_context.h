@@ -152,6 +152,8 @@ class PeerContext : public std::enable_shared_from_this<PeerContext> {
   // (NVLS-capable); otherwise the range is registered through cudaIpc. Collective.
   std::shared_ptr<PeerBuffer> resolveBuffer(void* ptr, size_t bytes, size_t* byteOffset);
   void hostBarrier();
+  // Collective: whether every rank passed the same words (at most 16), by an allgather over the context.
+  bool hostAllSame(const std::vector<int64_t>& words);
   // Call right before launching a kernel that waits for its peers. When several ranks
   // share one GPU (threads-as-ranks tests) a peer that is still inside a device-
   // synchronising call (cudaMalloc from an allocator, cudaFree, ...) would block behind

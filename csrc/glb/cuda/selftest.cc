@@ -16,6 +16,7 @@
 #include <sstream>
 
 #include "glb/common/utils.h"
+#include "glb/cuda/collectives.h"
 #include "glb/cuda/kernels.h"
 #include "glb/cuda/local_ops.h"
 #include "glb/cuda/schedules.h"
@@ -757,6 +758,157 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
       }
       return "";
     });
+    // The low-latency dispatch and combine, both forms, at P = 2 and 8. Virtual rank 0 pushes to slot
+    // (e, 0, r) of every virtual holder and packs its own experts' rows; the host stands in for the
+    // other sources by storing their signal words (no rows) into rank 0's buffer. The combine pushes
+    // rank 0's packed rows back to its own combine slots; the slots of choices held by the virtual
+    // holders are filled by the host. bf16 values are halves / quarters of small integers, FP8 rows
+    // small integers with one +-448 per block (scale 1, codes exact), so every sum is exact in order.
+    for (const bool fp8 : {false, true}) {
+      if (P != 2 && P != 8) break;
+      const char* what = fp8 ? "moeLLDispatchKernel<fp8> + moeLLCombineKernel<bf16> (E=2, k=3, H=256) P="
+                             : "moeLLDispatchKernel + moeLLCombineKernel<bf16> (E=2, k=3, H=64) P=";
+      R.run(strcat_all(what, P), [&, fp8]() -> std::string {
+        const int E = 2, K = P * E, topk = 3, H = fp8 ? 256 : 64, T = 13, M = T * topk, nb = H / kFp8Block;
+        const MoeLLLayout l = moeLLLayout(P, E, M, topk, H, 2, fp8);
+        const uint32_t form = fp8 ? kMoeLLDispatchFp8 : kMoeLLDispatch;
+        std::vector<std::unique_ptr<DevBuf>> bufs;
+        MoeLLArgs L{};
+        for (int r = 0; r < P; r++) {
+          bufs.emplace_back(new DevBuf(l.bytes));
+          L.bufs.p[r] = bufs[r]->p;
+          GLB_CUDA_CHECK(cudaMemsetAsync(L.bufs.p[r], 0, l.bytes, stream));
+        }
+        L.l = l;
+        L.status = pc.inputStatusDevice();
+        char* b0 = static_cast<char*>(L.bufs.p[0]);
+        auto bf16 = [](float f) {
+          uint32_t u;
+          std::memcpy(&u, &f, 4);
+          return static_cast<uint16_t>(u >> 16);  // exact for the values used here
+        };
+        auto value = [&](int t, int c) -> float {
+          if (!fp8) return static_cast<float>((t * 3 + c) % 17 - 8) * 0.5f;
+          const int b = c / kFp8Block;
+          if (c % kFp8Block == (t * 3 + b * 5) % kFp8Block) return (t + b) % 2 ? -448.0f : 448.0f;
+          return static_cast<float>((t * 7 + c * 3) % 33 - 16);
+        };
+        std::vector<int64_t> idx(T * topk);
+        std::vector<int> rank(T * topk, -1), cnt(K, 0);
+        for (int i = 0; i < T * topk; i++) {
+          idx[i] = static_cast<int64_t>((i * 5 + i / topk * 3) % (K + 2)) - 1;
+          if (idx[i] >= 0 && idx[i] < K) rank[i] = cnt[idx[i]]++;
+        }
+        std::vector<uint16_t> xh(T * H);
+        for (int t = 0; t < T; t++) for (int c = 0; c < H; c++) xh[t * H + c] = bf16(value(t, c));
+        const size_t rb = l.rowBytes, slotsRows = static_cast<size_t>(E) * P * M;
+        DevBuf x(xh.size() * 2), idxDev(idx.size() * 8), out(slotsRows * rb), outScales(slotsRows * nb * 4 + 16),
+            outSplits(K * 8);
+        GLB_CUDA_CHECK(cudaMemcpyAsync(x.p, xh.data(), xh.size() * 2, cudaMemcpyHostToDevice, stream));
+        GLB_CUDA_CHECK(cudaMemcpyAsync(idxDev.p, idx.data(), idx.size() * 8, cudaMemcpyHostToDevice, stream));
+        GLB_CUDA_CHECK(cudaMemsetAsync(out.p, 0xff, out.bytes, stream));
+        std::vector<unsigned long long> words(K, 0ull);
+        for (int e = 0; e < E; e++) for (int s2 = 1; s2 < P; s2++) words[e * P + s2] = moeLLSignal(1, form, 0);
+        GLB_CUDA_CHECK(cudaMemcpyAsync(b0 + l.dispatchSig, words.data(), K * 8, cudaMemcpyHostToDevice, stream));
+        const int blocks = std::min(pc.coResidentBlocks(moeLLDispatchKernelPtr(fp8)), 16);
+        launchMoeLLDispatch(ca, L, x.p, T, static_cast<const long long*>(idxDev.p), out.p,
+                            static_cast<float*>(outScales.p), static_cast<long long*>(outSplits.p), blocks, stream);
+        noteLaunch();
+        std::vector<int64_t> os(K);
+        std::vector<uint8_t> outH(out.bytes);
+        std::vector<float> scH(slotsRows * nb);
+        GLB_CUDA_CHECK(cudaMemcpyAsync(os.data(), outSplits.p, K * 8, cudaMemcpyDeviceToHost, stream));
+        GLB_CUDA_CHECK(cudaMemcpyAsync(outH.data(), out.p, out.bytes, cudaMemcpyDeviceToHost, stream));
+        if (fp8) GLB_CUDA_CHECK(cudaMemcpyAsync(scH.data(), outScales.p, scH.size() * 4, cudaMemcpyDeviceToHost, stream));
+        GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+        for (int e = 0; e < E; e++) {
+          for (int s2 = 0; s2 < P; s2++) {
+            if (os[e * P + s2] != (s2 == 0 ? cnt[e] : 0)) return strcat_all("out_splits[", e * P + s2, "] = ", os[e * P + s2]);
+          }
+        }
+        // Every routed choice: its slot row and tag on its holder; rank 0's own experts: the packed row.
+        auto rowOk = [&](const uint8_t* row, int t) {
+          for (int c = 0; c < H; c++) {
+            if (fp8 ? row[c] != float8_e4m3::fromFloat(value(t, c))
+                    : std::memcmp(row + 2 * c, &xh[t * H + c], 2) != 0) return false;
+          }
+          return true;
+        };
+        for (int j = 0; j < P; j++) {
+          std::vector<uint8_t> slots(l.tags - l.slots);
+          std::vector<int32_t> tags(slotsRows);
+          GLB_CUDA_CHECK(cudaMemcpyAsync(slots.data(), static_cast<char*>(L.bufs.p[j]) + l.slots, slots.size(),
+                                         cudaMemcpyDeviceToHost, stream));
+          GLB_CUDA_CHECK(cudaMemcpyAsync(tags.data(), static_cast<char*>(L.bufs.p[j]) + l.tags, tags.size() * 4,
+                                         cudaMemcpyDeviceToHost, stream));
+          GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+          for (int i = 0; i < T * topk; i++) {
+            if (rank[i] < 0 || idx[i] / E != j) continue;
+            const int e = static_cast<int>(idx[i] % E), t = i / topk;
+            const size_t slot = static_cast<size_t>(e) * P * M + rank[i];  // (e, source 0, r)
+            if (tags[slot] != i) return strcat_all("holder ", j, " slot ", slot, ": tag ", tags[slot], ", want ", i);
+            if (!rowOk(&slots[slot * rb], t)) return strcat_all("holder ", j, " slot ", slot, " (token ", t, ") differs");
+            if (j == 0) {
+              const size_t row = static_cast<size_t>(e) * P * M + rank[i];
+              if (!rowOk(&outH[row * rb], t)) return strcat_all("out[", e, ", ", rank[i], "] (token ", t, ") differs");
+              for (int b = 0; fp8 && b < nb; b++) {
+                if (scH[row * nb + b] != 1.0f) return strcat_all("out_scales[", e, ", ", rank[i], "] differs");
+              }
+            }
+          }
+        }
+        for (int e = 0; e < E; e++) {
+          if (outH[(static_cast<size_t>(e) * P * M + cnt[e]) * rb] != 0xff) return strcat_all("wrote past expert ", e);
+        }
+
+        // ---- combine ----
+        const size_t crb = l.combineRowBytes;
+        auto eoValue = [](int e, size_t q, int c) { return static_cast<float>((e * 5 + q * 3 + c) % 13 - 6) * 0.5f; };
+        auto preValue = [](int i, int c) { return static_cast<float>((i * 7 + c) % 11 - 5) * 0.25f; };
+        std::vector<uint16_t> eo(slotsRows * H), pre(static_cast<size_t>(T) * topk * H);
+        for (int e = 0; e < E; e++) {
+          for (size_t q = 0; q < static_cast<size_t>(P) * M; q++) {
+            for (int c = 0; c < H; c++) eo[(e * P * M + q) * H + c] = bf16(eoValue(e, q, c));
+          }
+        }
+        for (int i = 0; i < T * topk; i++) for (int c = 0; c < H; c++) pre[i * H + c] = bf16(preValue(i, c));
+        std::vector<float> w(T * topk);
+        for (int i = 0; i < T * topk; i++) w[i] = static_cast<float>((i * 5) % 9) * 0.25f - 1.0f;
+        DevBuf eoDev(eo.size() * 2), wDev(w.size() * 4), y(static_cast<size_t>(T) * crb);
+        GLB_CUDA_CHECK(cudaMemcpyAsync(eoDev.p, eo.data(), eo.size() * 2, cudaMemcpyHostToDevice, stream));
+        GLB_CUDA_CHECK(cudaMemcpyAsync(wDev.p, w.data(), w.size() * 4, cudaMemcpyHostToDevice, stream));
+        GLB_CUDA_CHECK(cudaMemcpyAsync(b0 + l.combineSlots, pre.data(), pre.size() * 2, cudaMemcpyHostToDevice, stream));
+        std::vector<unsigned long long> cw(P, moeLLSignal(2, kMoeLLCombine, 0));
+        GLB_CUDA_CHECK(cudaMemcpyAsync(b0 + l.combineSig + 8, cw.data(), (P - 1) * 8, cudaMemcpyHostToDevice, stream));
+        launchMoeLLCombine(ca, L, eoDev.p, static_cast<const float*>(wDev.p), y.p, T, DataType::BFLOAT16,
+                           std::min(pc.coResidentBlocks(moeLLCombineKernelPtr(DataType::BFLOAT16)), 16), stream);
+        noteLaunch();
+        std::vector<uint16_t> got(static_cast<size_t>(T) * H);
+        GLB_CUDA_CHECK(cudaMemcpyAsync(got.data(), y.p, got.size() * 2, cudaMemcpyDeviceToHost, stream));
+        GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+        for (int t = 0; t < T; t++) {
+          for (int c = 0; c < H; c++) {
+            float acc = 0.0f;
+            for (int x2 = 0; x2 < topk; x2++) {
+              const int i = t * topk + x2;
+              if (rank[i] < 0) continue;
+              const float row = idx[i] / E == 0 ? bf16ToFloat(bf16(eoValue(static_cast<int>(idx[i] % E), rank[i], c)))
+                                                : bf16ToFloat(pre[i * H + c]);
+              const float prod = w[i] * row;
+              acc = acc + prod;
+            }
+            uint32_t u;
+            std::memcpy(&u, &acc, 4);
+            const uint16_t want = static_cast<uint16_t>((u + 0x7fffu + ((u >> 16) & 1u)) >> 16);
+            if (got[t * H + c] != want) {
+              return strcat_all("y token ", t, " element ", c, ": got bf16 bits ", static_cast<int>(got[t * H + c]),
+                                ", want ", static_cast<int>(want));
+            }
+          }
+        }
+        return "";
+      });
+    }
 
     // ---- literal schedule executor (halving-doubling, plain and pipelined) -------------------
     R.run(strcat_all("scheduleKernel<float>(halving_doubling) P=", P), [&]() -> std::string {

@@ -108,6 +108,10 @@ void registerCuda(py::module_& root) {
         py::gil_scoped_release nogil;
         pc.hostBarrier();
       })
+      .def("host_all_same", [](PeerContext& pc, std::vector<int64_t> words) {
+        py::gil_scoped_release nogil;
+        return pc.hostAllSame(words);
+      }, "Collective: whether every rank passed the same list of at most 16 integers.")
       .def("set_timeout", [](PeerContext& pc, long ms) { pc.setTimeout(std::chrono::milliseconds(ms)); },
            "Device-side waits give up after this many milliseconds (0 = never).")
       .def("timeout_ms", [](PeerContext& pc) { return static_cast<long>(pc.timeout().count()); })

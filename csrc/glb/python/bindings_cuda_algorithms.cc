@@ -254,6 +254,48 @@ void registerCudaAlgorithms(py::module_& m) {
     py::gil_scoped_release nogil;
     scatter(pc, P(in), out, off, bytes, root, S(st));
   });
+  // Low-latency top-k exchange: the buffer's layout, then dispatch and combine on a buffer of it.
+  m.def("moe_ll_layout", [](int nranks, int experts, int maxTokens, int topk, size_t hidden, size_t elemBytes,
+                            bool fp8) {
+    const MoeLLLayout l = moeLLLayout(nranks, experts, maxTokens, topk, hidden, elemBytes, fp8);
+    py::dict d;
+    d["row_bytes"] = l.rowBytes;
+    d["scale_bytes"] = l.scaleBytes;
+    d["combine_row_bytes"] = l.combineRowBytes;
+    d["slots"] = l.slots;
+    d["scales"] = l.scales;
+    d["tags"] = l.tags;
+    d["dispatch_signals"] = l.dispatchSig;
+    d["combine_slots"] = l.combineSlots;
+    d["combine_signals"] = l.combineSig;
+    d["choices"] = l.choices;
+    d["ctrl"] = l.ctrl;
+    d["bytes"] = l.bytes;
+    return d;
+  }, py::arg("nranks"), py::arg("experts"), py::arg("max_tokens"), py::arg("topk"), py::arg("hidden"),
+     py::arg("elem_bytes"), py::arg("fp8"));
+  m.def("alltoallv_ll_topk", [](PeerContext& pc, const PeerBuffer& buf, size_t off, int experts, int maxTokens,
+                                int topk, size_t hidden, size_t elemBytes, bool fp8, uintptr_t x, size_t tokens,
+                                uintptr_t topkIdx, uintptr_t out, uintptr_t outScales, uintptr_t outSplits,
+                                uintptr_t st) {
+    py::gil_scoped_release nogil;
+    const MoeLLLayout l = moeLLLayout(pc.size, experts, maxTokens, topk, hidden, elemBytes, fp8);
+    alltoallvLLTopk(pc, buf, off, l, P(x), tokens, reinterpret_cast<const int64_t*>(topkIdx), P(out),
+                    static_cast<float*>(P(outScales)), reinterpret_cast<int64_t*>(outSplits), S(st));
+  }, py::arg("pc"), py::arg("buf"), py::arg("buf_offset"), py::arg("experts"), py::arg("max_tokens"), py::arg("topk"),
+     py::arg("hidden"), py::arg("elem_bytes"), py::arg("fp8"), py::arg("x"), py::arg("tokens"), py::arg("topk_idx"),
+     py::arg("out"), py::arg("out_scales"), py::arg("out_splits"), py::arg("stream"));
+  m.def("alltoallv_ll_combine_topk", [](PeerContext& pc, const PeerBuffer& buf, size_t off, int experts,
+                                        int maxTokens, int topk, size_t hidden, size_t elemBytes, bool fp8,
+                                        uintptr_t y, size_t tokens, uintptr_t expertOut, uintptr_t weights,
+                                        int dtype, uintptr_t st) {
+    py::gil_scoped_release nogil;
+    const MoeLLLayout l = moeLLLayout(pc.size, experts, maxTokens, topk, hidden, elemBytes, fp8);
+    alltoallvLLCombineTopk(pc, buf, off, l, P(y), tokens, P(expertOut), static_cast<const float*>(P(weights)),
+                           static_cast<DataType>(dtype), S(st));
+  }, py::arg("pc"), py::arg("buf"), py::arg("buf_offset"), py::arg("experts"), py::arg("max_tokens"), py::arg("topk"),
+     py::arg("hidden"), py::arg("elem_bytes"), py::arg("fp8"), py::arg("y"), py::arg("tokens"),
+     py::arg("expert_out"), py::arg("weights"), py::arg("dtype"), py::arg("stream"));
   m.def("scatter", [](PeerContext& pc, uintptr_t in, uintptr_t out, size_t bytes, int root, uintptr_t st) {
     py::gil_scoped_release nogil;
     scatter(pc, P(in), P(out), bytes, root, S(st));

@@ -707,6 +707,127 @@ class CudaContext:
                                sptr, _stream(stream))
         return out
 
+    # ---- low-latency top-k MoE exchange (decoding) ----------------------------------------------
+    def moe_ll_buffer(self, experts: int, max_tokens: int, topk: int, hidden: int, dtype=None, fp8: bool = False):
+        """Collective: a :class:`MoELLBuffer` for :meth:`alltoallv_ll_topk` and
+        :meth:`alltoallv_ll_combine_topk`. Every rank must pass the same arguments, else ``ValueError``
+        on every rank. ``dtype`` (default bfloat16) is the row dtype of ``x``, ``out`` and the combine;
+        ``fp8=True`` takes bfloat16 rows and sends e4m3 codes with fp32 scales per 128 elements."""
+        import torch
+
+        return MoELLBuffer(self, experts, max_tokens, topk, hidden, torch.bfloat16 if dtype is None else dtype, fp8)
+
+    def alltoallv_ll_topk(self, buf, out, x, topk_idx, out_splits, out_scales=None, stream=None):
+        """Low-latency top-k MoE dispatch for decoding: one kernel, one signal round, no barrier, static
+        shapes (graph-capturable). ``buf`` is a :class:`MoELLBuffer`; ``x`` is ``(T, hidden)`` of its
+        dtype (FP8 form: bfloat16) with ``T <= max_tokens``; ``topk_idx`` int64 ``(T, topk)``, entry
+        ``j * experts + e`` = local expert ``e`` of rank ``j``, anything outside ``0 .. size * experts - 1``
+        not routed. Each routed choice is pushed to a fixed slot of its expert on rank ``j``, reserved
+        for this rank; no layout is agreed first.
+
+        ``out`` ``(experts, size * max_tokens, hidden)`` (FP8: float8_e4m3fn, plus ``out_scales`` float32
+        ``(experts, size * max_tokens, hidden // 128)``) receives expert ``e``'s rows in
+        ``out[e, :out_splits[e*size:(e+1)*size].sum()]``: source 0's rows, then source 1's, each by token
+        and then choice. That is byte for byte expert ``e``'s segment of :meth:`alltoallv_dev_topk` on the
+        same inputs (FP8: the same codes and scales). ``out_splits`` (int64 ``(experts * size,)``, entry
+        ``e * size + s``) gets the rows from each source. Rows past the count are not written. ``out``
+        and ``out_scales`` may be plain tensors: the rows are copied out of the buffer locally.
+
+        A (source, expert) group holds at most ``max_tokens`` rows; only a token that picks one expert
+        twice can exceed it. Such a group sends nothing, its choices count as unrouted in the
+        combine, the rest of the call is served, and ``ValueError`` naming the source, the expert, the
+        rows and ``max_tokens`` is raised on the source and on the holder at the next host call
+        (``synchronize()``). Wrong dtypes, shapes, contiguity or alignment, ``T > max_tokens``, a k
+        other than the buffer's, overlapping tensors and a dispatch on a buffer whose previous
+        dispatch has not been combined raise ``ValueError`` before launch."""
+        import torch
+
+        name = "alltoallv_ll_topk"
+        if not isinstance(buf, MoELLBuffer) or buf.cc is not self:
+            raise ValueError(f"{name}: buf must be a MoELLBuffer of this context")
+        if buf._pending is not None:
+            raise ValueError(f"{name}: the buffer's previous dispatch has not been combined; dispatch and combine "
+                             "must alternate on a buffer")
+        named = {"x": x, "topk_idx": topk_idx, "out": out, "out_splits": out_splits}
+        if buf.fp8:
+            if out_scales is None:
+                raise ValueError(f"{name}: the FP8 buffer needs out_scales")
+            named["out_scales"] = out_scales
+        elif out_scales is not None:
+            raise ValueError(f"{name}: out_scales is only for an FP8 buffer")
+        self._dev_tensors(name, named)
+        E, M, k, H, P = buf.experts, buf.max_tokens, buf.topk, buf.hidden, self.size
+        if x.dtype != buf.dtype or x.dim() != 2 or int(x.shape[1]) != H:
+            raise ValueError(f"{name}: x must be {buf.dtype} (T, {H}), got {x.dtype} {tuple(x.shape)}")
+        T = int(x.shape[0])
+        if T > M:
+            raise ValueError(f"{name}: {T} tokens; the buffer holds max_tokens = {M}")
+        if topk_idx.dtype != torch.int64 or tuple(topk_idx.shape) != (T, k):
+            raise ValueError(f"{name}: topk_idx must be int64 {(T, k)} (the buffer's topk), got {topk_idx.dtype} "
+                             f"{tuple(topk_idx.shape)}")
+        odt = torch.float8_e4m3fn if buf.fp8 else buf.dtype
+        if out.dtype != odt or tuple(out.shape) != (E, P * M, H):
+            raise ValueError(f"{name}: out must be {odt} {(E, P * M, H)}, got {out.dtype} {tuple(out.shape)}")
+        if buf.fp8 and (out_scales.dtype != torch.float32 or tuple(out_scales.shape) != (E, P * M, H // 128)):
+            raise ValueError(f"{name}: out_scales must be float32 {(E, P * M, H // 128)}, got {out_scales.dtype} "
+                             f"{tuple(out_scales.shape)}")
+        if out_splits.dtype != torch.int64 or tuple(out_splits.shape) != (E * P,):
+            raise ValueError(f"{name}: out_splits must be int64 ({E * P},), got {out_splits.dtype} "
+                             f"{tuple(out_splits.shape)}")
+        if x.data_ptr() % 16 or out.data_ptr() % 16:
+            raise ValueError(f"{name}: x and out must be 16-byte aligned")
+        buf._check_disjoint(name, named)
+        _cu.alltoallv_ll_topk(self.pc, buf._pbuf, buf._off, E, M, k, H, buf._elem, buf.fp8, x.data_ptr(), T,
+                              topk_idx.data_ptr(), out.data_ptr(), out_scales.data_ptr() if buf.fp8 else 0,
+                              out_splits.data_ptr(), _stream(stream))
+        buf._pending = T
+        return out
+
+    def alltoallv_ll_combine_topk(self, buf, y, expert_out, weights, stream=None):
+        """Low-latency top-k MoE combine, after :meth:`alltoallv_ll_topk` on the same ``buf``: every
+        row of this rank's experts goes back to its source, one signal round, and each source sums its
+        tokens' choices with their gate weights in one kernel (graph-capturable).
+
+        ``expert_out`` is ``(experts, size * max_tokens, hidden)`` of the buffer's dtype (FP8 buffer:
+        bfloat16), in the dispatch's ``out`` layout; rows past each expert's count are not read. ``y`` is
+        ``(T, hidden)`` of that dtype with the dispatch's T; ``weights`` float32 ``(T, topk)`` or None
+        (weight 1). ``y[t] = round(acc)``, ``acc`` from +0.0 adding ``w[t, j] * float(row)`` for
+        j = 0..k-1 over the routed choices that were sent, each a correctly rounded fp32 multiply and
+        add: byte for byte what :meth:`alltoallv_dev_combine_topk` gives on the same expert rows.
+        Combine dtypes are float32, bfloat16 and float16. Wrong dtypes, shapes, contiguity or
+        alignment, overlaps and a combine with no dispatch before it raise ``ValueError`` before
+        launch."""
+        import torch
+
+        name = "alltoallv_ll_combine_topk"
+        if not isinstance(buf, MoELLBuffer) or buf.cc is not self:
+            raise ValueError(f"{name}: buf must be a MoELLBuffer of this context")
+        if buf._pending is None:
+            raise ValueError(f"{name}: no dispatch on this buffer to combine")
+        named = {"y": y, "expert_out": expert_out}
+        if weights is not None:
+            named["weights"] = weights
+        self._dev_tensors(name, named)
+        E, M, k, H, P, T = buf.experts, buf.max_tokens, buf.topk, buf.hidden, self.size, buf._pending
+        cdt = torch.bfloat16 if buf.fp8 else buf.dtype
+        if cdt not in (torch.float32, torch.bfloat16, torch.float16):
+            raise ValueError(f"{name}: a buffer of {buf.dtype} rows cannot combine; float32, bfloat16 and float16 can")
+        if expert_out.dtype != cdt or tuple(expert_out.shape) != (E, P * M, H):
+            raise ValueError(f"{name}: expert_out must be {cdt} {(E, P * M, H)}, got {expert_out.dtype} "
+                             f"{tuple(expert_out.shape)}")
+        if y.dtype != cdt or tuple(y.shape) != (T, H):
+            raise ValueError(f"{name}: y must be {cdt} {(T, H)} (T of the dispatch), got {y.dtype} {tuple(y.shape)}")
+        if weights is not None and (weights.dtype != torch.float32 or tuple(weights.shape) != (T, k)):
+            raise ValueError(f"{name}: weights must be float32 {(T, k)}, got {weights.dtype} {tuple(weights.shape)}")
+        if y.data_ptr() % 16 or expert_out.data_ptr() % 16:
+            raise ValueError(f"{name}: y and expert_out must be 16-byte aligned")
+        buf._check_disjoint(name, named)
+        _cu.alltoallv_ll_combine_topk(self.pc, buf._pbuf, buf._off, E, M, k, H, buf._elem, buf.fp8, y.data_ptr(), T,
+                                      expert_out.data_ptr(), weights.data_ptr() if weights is not None else 0,
+                                      int(_torch_dtype_to_glb(cdt)), _stream(stream))
+        buf._pending = None
+        return y
+
     def scatter(self, output, input=None, root: int = 0, stream=None):
         """Block ``rank`` of the root's ``input`` -> ``output``. Any size; ``input`` is read on the
         root only (None elsewhere)."""
@@ -751,6 +872,86 @@ class CudaContext:
             optr = output.data_ptr() if output is not None else 0
             _cu.reduce(self.pc, ptr, optr, n, int(dt), int(op), root, _stream(stream))
         return output
+
+
+class MoELLBuffer:
+    """Symmetric memory for the low-latency top-k MoE exchange, made by :meth:`CudaContext.moe_ll_buffer`
+    with the same arguments on every rank (checked by an allgather: a mismatch raises ``ValueError``
+    on every rank). It holds, per rank, in this order, each part rounded up to 16 bytes:
+
+    - dispatch slots: ``experts * size * max_tokens`` rows of ``row_bytes`` (``hidden`` elements of
+      ``dtype``; FP8: ``hidden`` e4m3 codes), then FP8 only their scales, ``hidden / 128 * 4`` bytes a
+      row, then an int32 tag a row (``t * topk + j`` of the source's token and choice);
+    - ``experts * size`` 64-bit dispatch signal words;
+    - combine slots: ``max_tokens * topk`` rows of ``hidden`` elements (FP8: bfloat16);
+    - ``size`` 64-bit combine signal words, ``max_tokens * topk`` int32 choice marks and 16 bytes of
+      call count and completion ticket.
+
+    So ``bytes ~= E * P * M * (row_bytes + scale_bytes + 4) + M * k * (combine_row_bytes + 4)``: at
+    E = 32, P = 8, M = 128, k = 8 and H = 7168 that is 484 MB in bfloat16 (470 MB of slots) and 257 MB
+    in FP8 (242 MB of slots and scales). ``layout`` has every offset. Limits: ``size <= 16``,
+    ``1 <= experts <= 32``, ``1 <= topk <= 32``, ``max_tokens * topk <= 2^31 - 1``, rows a multiple of
+    16 bytes (FP8: ``hidden`` a multiple of 128).
+
+    Dispatch and combine must alternate on a buffer; that is what lets one set of slots serve every
+    call. The buffer counts its calls on the device, so a captured dispatch / combine pair can be
+    replayed as a CUDA graph."""
+
+    def __init__(self, cc: "CudaContext", experts, max_tokens, topk, hidden, dtype, fp8):
+        import torch
+
+        name = "moe_ll_buffer"
+        dtypes = [torch.float32, torch.bfloat16, torch.float16, torch.uint8, torch.int8, torch.int16, torch.int32,
+                  torch.int64, torch.float64]
+
+        def as_int(v):
+            try:
+                return int(v) if int(v) == v else -1
+            except (TypeError, ValueError):
+                return -1
+
+        words = [as_int(experts), as_int(max_tokens), as_int(topk), as_int(hidden),
+                 dtypes.index(dtype) if dtype in dtypes else -1, 1 if fp8 else 0]
+        if not cc.pc.host_all_same(words):
+            raise ValueError(f"{name}: the arguments (experts, max_tokens, topk, hidden, dtype, fp8) differ between "
+                             "ranks; every rank must pass the same")
+        E, M, k, H = words[:4]
+        if not 1 <= E <= 32 or not 1 <= k <= 32 or M < 1 or M * k > 2**31 - 1 or H < 1 or words[4] < 0:
+            raise ValueError(f"{name}: need 1 <= experts <= 32, 1 <= topk <= 32, max_tokens >= 1 with max_tokens * "
+                             f"topk <= 2^31 - 1, hidden >= 1 and a tensor dtype; got {experts}, {topk}, {max_tokens}, "
+                             f"{hidden}, {dtype}")
+        es = torch.empty((), dtype=dtype).element_size()
+        if fp8 and (dtype != torch.bfloat16 or H % 128):
+            raise ValueError(f"{name}: the FP8 form takes bfloat16 rows of a multiple of 128 elements, got {dtype} "
+                             f"and {H}")
+        if (H * es) % 16:
+            raise ValueError(f"{name}: rows of {H * es} bytes; a multiple of 16 is required")
+        self.layout = _cu.moe_ll_layout(cc.size, E, M, k, H, es, bool(fp8))
+        nbytes = int(self.layout["bytes"])
+        free, _ = torch.cuda.mem_get_info(cc.device)
+        fits = free >= nbytes * max(1, cc.pc.ranks_on_my_device())
+        if not cc.pc.host_all_same([1 if fits else 0]) or not fits:
+            raise ValueError(f"{name}: {nbytes} bytes per rank do not fit the free device memory of every rank")
+        self.cc, self.experts, self.max_tokens, self.topk, self.hidden = cc, E, M, k, H
+        self.dtype, self.fp8, self._elem = dtype, bool(fp8), es
+        self.tensor = cc.empty(nbytes, torch.uint8)
+        self.tensor.zero_()  # signal words, call count: no call has happened
+        torch.cuda.current_stream(cc.device).synchronize()
+        cc.pc.host_barrier()  # no peer signals into a buffer that is still being cleared
+        self._pbuf, self._off = cc.lookup(self.tensor)
+        self._pending = None  # T of a dispatch not yet combined
+
+    @property
+    def nbytes(self) -> int:
+        return int(self.layout["bytes"])
+
+    def _check_disjoint(self, name, named):
+        """No two of ``named`` share a byte, and none lies in the buffer."""
+        items = list(named.items()) + [("the buffer", self.tensor)]
+        for i, (an, a) in enumerate(items):
+            for bn, b in items[i + 1:]:
+                if a.numel() and b.numel():
+                    CudaContext._dev_disjoint(name, a, an, b, bn)
 
 
 # ---- old-style class wrappers -----------------------------------------------------------------

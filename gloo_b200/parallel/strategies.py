@@ -597,6 +597,27 @@ class MoEDispatcher(_Base):
         return self.cc.alltoallv_dev_combine_topk_backward(grad_expert_out, grad_weights, grad_out, expert_out, splits,
                                                            pos, weights, experts=experts, align=align)
 
+    # ---- low-latency form, for decoding ---------------------------------------------------------
+    def dispatch_ll(self, x, topk_idx, buf, out, out_scales=None):
+        """The low-latency top-k dispatch on ``buf`` (``cc.moe_ll_buffer``): fixed per-expert slots,
+        one signal round, static shapes, so a decode step can be captured in a CUDA graph. ``out`` is
+        ``(experts, size * max_tokens, hidden)``; expert ``e``'s rows are ``out[e, :count]``, byte for
+        byte its segment of dispatch_dev_topk(). Returns ``(out, out_splits)``, or for an FP8 buffer
+        ``(out, out_scales, out_splits)``. See ``CudaContext.alltoallv_ll_topk``."""
+        import torch
+
+        out_splits = torch.empty(self.size * buf.experts, dtype=torch.int64, device=x.device)
+        self.cc.alltoallv_ll_topk(buf, out, x, topk_idx, out_splits, out_scales=out_scales)
+        if out_scales is not None:
+            return out, out_scales, out_splits
+        return out, out_splits
+
+    def combine_ll(self, expert_out, weights, buf, y):
+        """The low-latency combine after dispatch_ll() on the same ``buf``: ``y[t]`` = the weighted sum
+        of token t's expert rows, byte for byte combine_dev_topk()'s. ``weights`` may be None (weight
+        1). See ``CudaContext.alltoallv_ll_combine_topk``."""
+        return self.cc.alltoallv_ll_combine_topk(buf, y, expert_out, weights)
+
     # ---- autograd ------------------------------------------------------------------------------
     # Each backward is a collective: every rank's backward pass must reach it, in the same order. The
     # backward kernels run on the stream current in the backward pass, on plain gradient tensors, so

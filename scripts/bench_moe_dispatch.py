@@ -43,7 +43,15 @@ n * 2^-23 * sum |dy * x| of each other (n = hidden: the bound of any fp32 summat
 terms; the two arms sum in different orders). MB/rank is the T x k expert rows read plus the T x k
 gradient rows written, from the shapes.
 
-    python scripts/bench_moe_dispatch.py [--ranks 2] [--iters 20] [--tables pairs,fp8,combine,dispatch,backward]
+A sixth table (--tables ll) times a decode-sized MoE layer with identity experts (median per layer,
+rank 0), each arm captured once in a CUDA graph and replayed, the arms alternating, CUDA events around
+each replay, at T = 1, 32 and 128 tokens per rank, bf16 and FP8:
+  dev  dispatch_dev_topk + combine_dev_topk (the variable layout agreed at barriers)
+  ll   dispatch_ll + combine_ll on a buffer of max_tokens = 128 (fixed slots, one signal round each way)
+Before timing, every expert's rows (FP8: codes and scales) and the layer outputs are checked equal byte
+for byte between the arms. The FP8 arms combine bf16 rows dequantised once from each arm's codes.
+
+    python scripts/bench_moe_dispatch.py [--ranks 2] [--iters 20] [--tables pairs,fp8,combine,dispatch,backward,ll]
 """
 import argparse
 import json
@@ -429,6 +437,97 @@ def measure_dispatch_topk(ctx, args, dev):
     return got
 
 
+def run_rank_ll(ctx, args, shared):
+    if shared:
+        return measure_ll(ctx, args, 0)
+    torch.cuda.set_device(ctx.rank)
+    with torch.cuda.stream(gcu.new_stream(ctx.rank)):
+        return measure_ll(ctx, args, ctx.rank)
+
+
+def measure_ll(ctx, args, dev):
+    P, E, H, M = ctx.size, args.experts, args.hidden, 128
+    G = P * E
+    k = min(args.topk, G)
+    cc = gcu.CudaContext(ctx, dev, stage_bytes=16 << 20)
+    moe = MoEDispatcher(ctx, cc)
+    got = {}
+    for fp8 in (False, True):
+        buf = cc.moe_ll_buffer(E, M, k, H, fp8=fp8)
+        cap = P * M * k
+        dt = torch.float8_e4m3fn if fp8 else torch.bfloat16
+        dout, lout = cc.empty((cap, H), dt), torch.empty((E, P * M, H), dtype=dt, device="cuda")
+        dsc = cc.empty((cap, H // 128), torch.float32) if fp8 else None
+        lsc = torch.empty((E, P * M, H // 128), dtype=torch.float32, device="cuda") if fp8 else None
+        for T in (1, 32, 128):
+            g = torch.Generator(device="cuda").manual_seed(77 + 1000 * T + ctx.rank)
+            x = torch.randn(T, H, device="cuda", generator=g).to(torch.bfloat16)
+            w, idx = torch.topk(torch.softmax(torch.randn(T, G, device="cuda", generator=g), -1), k, dim=-1)
+            ys = [torch.empty((T, H), dtype=torch.bfloat16, device="cuda") for _ in range(2)]
+            # Identity experts: the bf16 rows each arm's combine reads are its dispatch output (FP8:
+            # dequantised once, below, outside the timed layer).
+            res = moe.dispatch_dev_topk(x, idx, dout, experts=E, out_scales=dsc)
+            osp, ooff, splits, pos = res[-4:]
+            lres = moe.dispatch_ll(x, idx, buf, lout, out_scales=lsc)
+            lsp = lres[-1]
+            cc.synchronize()
+            assert torch.equal(osp, lsp), "out_splits"
+            sp, off = osp.cpu(), ooff.cpu()
+            for e in range(E):
+                n, o = int(sp[e * P:(e + 1) * P].sum()), int(off[e * P])
+                assert torch.equal(dout[o:o + n].view(torch.uint8), lout[e, :n].view(torch.uint8)), ("rows", e)
+                if fp8:
+                    assert torch.equal(dsc[o:o + n], lsc[e, :n]), ("scales", e)
+            if fp8:
+                deo = (dout.float().view(cap, H // 128, 128) * dsc.unsqueeze(-1)).view(cap, H).to(torch.bfloat16)
+                leo = (lout.float().view(E, P * M, H // 128, 128) * lsc.unsqueeze(-1)).view(E, P * M, H)
+                leo = leo.to(torch.bfloat16)
+            else:
+                deo, leo = dout, lout
+            moe.combine_ll(leo, w, buf, ys[1])
+
+            def dev_layer():
+                r = moe.dispatch_dev_topk(x, idx, dout, experts=E, out_scales=dsc)
+                moe.combine_dev_topk(deo, r[-2], r[-1], w, ys[0], experts=E)
+
+            def ll_layer():
+                moe.dispatch_ll(x, idx, buf, lout, out_scales=lsc)
+                moe.combine_ll(leo, w, buf, ys[1])
+
+            dev_layer()
+            cc.synchronize()
+            assert torch.equal(ys[0].view(torch.uint8), ys[1].view(torch.uint8)), "y"
+            graphs = []
+            for fn in (dev_layer, ll_layer):
+                cc.pc.host_barrier()
+                # On this rank's stream, without torch.cuda.graph's device-wide synchronize: the other
+                # ranks' threads may be capturing already.
+                gr = torch.cuda.CUDAGraph()
+                gr.capture_begin(capture_error_mode="thread_local")
+                fn()
+                gr.capture_end()
+                graphs.append(gr)
+            cc.pc.host_barrier()
+            times = ([], [])
+            for it in range(args.iters + 3):
+                for gr, tl in zip(graphs, times):
+                    cc.pc.host_barrier()
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    gr.replay()
+                    e1.record()
+                    cc.synchronize()
+                    if it >= 3:  # warm-up replays
+                        tl.append(e0.elapsed_time(e1))
+            name = f"{'fp8' if fp8 else 'bf16'}_T{T}"
+            got[f"{name}_dev"] = statistics.median(times[0])
+            got[f"{name}_ll"] = statistics.median(times[1])
+            cc.pc.host_barrier()
+            del graphs
+        got[f"{'fp8' if fp8 else 'bf16'}_buffer_bytes"] = buf.nbytes
+    return got
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--ranks", type=int, default=2, help="threads sharing the GPU when only one is visible")
@@ -496,6 +595,21 @@ def main():
             c, t = r[f"{arm}_composed"], r[f"{arm}_topk"]
             print(f"{arm:>14} {c:12.3f} {t:9.3f} {c / t:9.2f} {r['bytes_avoided'] / 1e6:11.1f}", flush=True)
         print(json.dumps({"table": "topk_dispatch", "ranks": P, "shared_gpu": shared, **r}), flush=True)
+
+    if "ll" in tables:
+        print(f"# decode MoE layer, top-{args.topk}, hidden {args.hidden}, {args.experts} experts per rank ({label}{note}); "
+              f"median of {args.iters} graph replays (rank 0, CUDA events), arms alternating, outputs checked equal",
+              flush=True)
+        if shared:
+            r = gb.spawn_threads(P, run_rank_ll, args, True, cuda_device=0, timeout_ms=300000)[0]
+        else:
+            r = gb.spawn_threads(P, run_rank_ll, args, False, timeout_ms=300000)[0]
+        print(f"{'form':>6} {'T':>5} {'dev ms':>9} {'ll ms':>9} {'dev/ll':>8}")
+        for form in ("bf16", "fp8"):
+            for T in (1, 32, 128):
+                d, ll = r[f"{form}_T{T}_dev"], r[f"{form}_T{T}_ll"]
+                print(f"{form:>6} {T:>5} {d:9.3f} {ll:9.3f} {d / ll:8.2f}", flush=True)
+        print(json.dumps({"table": "ll_layer", "ranks": P, "shared_gpu": shared, **r}), flush=True)
 
     if "backward" in tables:
         print(f"# top-k combine backward, bf16 ({label}{note}); median of {args.iters} calls (rank 0), arms "

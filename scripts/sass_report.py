@@ -48,6 +48,11 @@ KERNELS = [
     ("combine_topk_backward_f32", r"moeCombineTopkBackwardKernel<float>"),
     ("dispatch_topk", r"moeDispatchTopkKernel<false>"),
     ("dispatch_topk_fp8", r"moeDispatchTopkKernel<true>"),
+    ("ll_dispatch_topk", r"moeLLDispatchKernel<false>"),
+    ("ll_dispatch_topk_fp8", r"moeLLDispatchKernel<true>"),
+    ("ll_combine_topk_bf16", r"moeLLCombineKernel<__nv_bfloat16>"),
+    ("ll_combine_topk_f16", r"moeLLCombineKernel<__half>"),
+    ("ll_combine_topk_f32", r"moeLLCombineKernel<float>"),
     ("p2p_sendrecv", r"p2pKernel"),
     ("exchange_zero_copy", r"exchangeKernel<false>"),
     ("exchange_zero_copy_tma", r"exchangeKernel<true>"),
