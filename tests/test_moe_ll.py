@@ -7,6 +7,7 @@ import torch
 
 import gloo_b200 as gb
 from gloo_b200.parallel.strategies import MoEDispatcher
+from test_moe_combine_topk import _reference
 from test_moe_dev import SENTINEL, _bytes
 from test_moe_dispatch_topk import ROWS, _x
 
@@ -88,8 +89,9 @@ def _cases(P):
 def test_ll_dispatch_identity(size):
     """A spread of (E, k, row dtype, symmetric / plain out) at this P: every expert's packed rows and
     out_splits equal alltoallv_dev_topk's segment byte for byte, rows past the count keep the
-    sentinel and x is unchanged. Inputs have -1 and out-of-range entries, an idle rank, T = max_tokens
-    and tokens that pick an expert twice (max_tokens is large enough that no group overflows)."""
+    sentinel and x is unchanged; combine_ll over those rows equals the CPU combine. Inputs have -1 and
+    out-of-range entries, an idle rank, T = max_tokens and tokens that pick an expert twice (max_tokens
+    is large enough that no group overflows)."""
     gcu = _cuda()
     P = size
 
@@ -112,6 +114,14 @@ def test_ll_dispatch_identity(size):
             if dtype in COMBINE_DTYPES:  # rows of other dtypes have no combine; the buffer is dropped
                 y = torch.empty((x.shape[0], width), dtype=dtype, device="cuda")
                 moe.combine_ll(out, None, buf, y)
+                # out holds each routed choice's own token row, and no group overflows: the CPU
+                # combine of row t * k + j = x[t] over every routed choice
+                T = x.shape[0]
+                flat = idx.cpu().reshape(-1)
+                pos = torch.where((flat >= 0) & (flat < P * E), torch.arange(T * k), -1).view(T, k)
+                want = _reference(x.cpu().repeat_interleave(k, 0), pos, torch.ones(T, k), dtype)
+                cc.synchronize()
+                assert torch.equal(_bytes(y), _bytes(want)), (E, k, str(dtype), symmetric)
             cc.synchronize()
             cc.pc.host_barrier()
         return True
