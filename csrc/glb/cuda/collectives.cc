@@ -471,6 +471,146 @@ void allreduceCast(PeerContext& pc, const PeerBuffer& in, size_t inOffset, const
 }
 
 
+// ---- allreduce fused with bias, residual add and a norm ----------------------------------
+
+NormPlan planResidualNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, AllreduceAlgo algo) {
+  const size_t rowBytes = hidden * elementSize(dt);
+  const size_t bytes = rows * rowBytes;
+  const auto l = layoutOf(pc);
+  NormPlan p;
+  p.variant = kNormLocal;
+  p.chunkRows = std::max<size_t>(rows, 1);
+  if (pc.size > 1) {
+    if (algo != AllreduceAlgo::AUTO && algo != AllreduceAlgo::LL && algo != AllreduceAlgo::ONE_SHOT &&
+        algo != AllreduceAlgo::TWO_SHOT) {
+      GLB_THROW(InputException, "allreduce_residual_norm: algo must be auto, ll, one_shot or two_shot, got ",
+                allreduceAlgoName(algo));
+    }
+    // The allreduce's choice for a plain buffer of the same size: the tuning table and the
+    // CUDA_LL_MAX / CUDA_ONESHOT_MAX knobs govern this operation too. As in allreduce(algo=), a
+    // variant whose region cannot hold the rows runs as the row-sharded two-shot.
+    if (algo == AllreduceAlgo::AUTO) algo = planAllreduce(pc, bytes, dt, ReduceOp::SUM, BufKind::USER).algo;
+    if (algo == AllreduceAlgo::LL && bytes <= pc.llMaxBytes()) {
+      p.variant = kNormLL;
+    } else if (algo == AllreduceAlgo::ONE_SHOT && roundUp(bytes, 16) <= l.half) {
+      p.variant = kNormOneShot;
+    } else {
+      p.variant = kNormTwoShot;
+      // One launch while the staged rows (partials, and out with a norm) fit the bulk region.
+      const size_t perRow = (norm != kNormNone ? 2 : 1) * rowBytes;
+      if (perRow > l.bulkBytes) {
+        GLB_THROW(InputException, "allreduce_residual_norm: the pool's bulk region holds no row of ", rowBytes,
+                  " bytes; raise GLB_CUDA_STAGE_MB (CudaContext stage_bytes)");
+      }
+      p.chunkRows = std::min(p.chunkRows, l.bulkBytes / perRow);
+    }
+  }
+  p.launches = rows == 0 ? 0 : ceilDiv(rows, p.chunkRows);
+  return p;
+}
+
+const char* normVariantName(int variant) {
+  switch (variant) {
+    case kNormLL: return "ll";
+    case kNormOneShot: return "one_shot";
+    case kNormTwoShot: return "two_shot";
+    default: return "local";
+  }
+}
+
+#define GLB_NORM_CHECK(cond, ...) \
+  do {                            \
+    if (!(cond)) GLB_THROW(InputException, "allreduce_residual_norm: ", __VA_ARGS__); \
+  } while (0)
+
+int allreduceResidualNorm(PeerContext& pc, const void* partial, const void* residual, void* residualOut, void* out,
+                          const void* bias, const void* gamma, const void* beta, size_t rows, size_t hidden,
+                          DataType dt, int norm, float eps, AllreduceAlgo algo, cudaStream_t stream) {
+  GLB_TRACE_RANGE("glb::cuda::allreduceResidualNorm");
+  pc.checkHealth();
+  GLB_NORM_CHECK(normSupports(dt), "rows must be float32, bfloat16 or float16, got ", dataTypeName(dt));
+  GLB_NORM_CHECK(norm == kNormNone || norm == kNormRms || norm == kNormLayer, "unknown norm ", norm);
+  const size_t es = elementSize(dt);
+  GLB_NORM_CHECK(hidden > 0 && hidden * es % 16 == 0, "a row of ", hidden, " ", dataTypeName(dt),
+                 " elements is not a positive multiple of 16 bytes");
+  GLB_NORM_CHECK(hidden <= static_cast<size_t>(kMaxNormHidden), "rows of ", hidden, " elements exceed the limit of ",
+                 kMaxNormHidden);
+  const size_t rowsBytes = rows * hidden * es, vecBytes = hidden * es;
+  struct Range {
+    const char* name;
+    const void* p;
+    size_t bytes;
+  };
+  const Range inputs[] = {{"partial", partial, rowsBytes}, {"residual", residual, rowsBytes}, {"bias", bias, vecBytes},
+                          {"weight", gamma, vecBytes}, {"norm_bias", beta, vecBytes}};
+  const Range outputs[] = {{"residual_out", residualOut, rowsBytes}, {"out", norm != kNormNone ? out : nullptr, rowsBytes}};
+  GLB_NORM_CHECK(rows == 0 || (partial != nullptr && residual != nullptr && residualOut != nullptr &&
+                               (norm == kNormNone || out != nullptr)),
+                 "partial, residual, residual_out and (with a norm) out are required");
+  for (const Range& r : inputs) {
+    GLB_NORM_CHECK(reinterpret_cast<uintptr_t>(r.p) % 16 == 0, r.name, " must be 16-byte aligned");
+  }
+  for (const Range& r : outputs) {
+    GLB_NORM_CHECK(reinterpret_cast<uintptr_t>(r.p) % 16 == 0, r.name, " must be 16-byte aligned");
+  }
+  auto overlap = [](const Range& a, const Range& b) {
+    const uintptr_t x = reinterpret_cast<uintptr_t>(a.p), y = reinterpret_cast<uintptr_t>(b.p);
+    return a.p != nullptr && b.p != nullptr && a.bytes > 0 && b.bytes > 0 && x < y + b.bytes && y < x + a.bytes;
+  };
+  for (const Range& o : outputs) {
+    for (const Range& i : inputs) {
+      // residual_out may be residual itself (in place: each row is read before it is written).
+      const bool inPlace = o.p == residualOut && i.p == residual && residualOut == residual;
+      GLB_NORM_CHECK(inPlace || !overlap(o, i), o.name, " overlaps ", i.name);
+    }
+  }
+  GLB_NORM_CHECK(!overlap(outputs[0], outputs[1]), "residual_out overlaps out");
+  if (rows == 0) return kNormLocal;
+  const NormPlan plan = planResidualNorm(pc, rows, hidden, dt, norm, algo);
+  DeviceGuard g(pc.device);
+  const auto l = layoutOf(pc);
+  const size_t rowBytes = vecBytes;
+  const void* kernel = allreduceNormKernelFor(dt, norm, plan.variant);
+  for (size_t r0 = 0; r0 < rows; r0 += plan.chunkRows) {
+    const size_t n = std::min(plan.chunkRows, rows - r0);
+    NormArgs a;
+    a.partial = static_cast<const char*>(partial) + r0 * rowBytes;
+    a.residual = static_cast<const char*>(residual) + r0 * rowBytes;
+    a.residualOut = static_cast<char*>(residualOut) + r0 * rowBytes;
+    a.out = norm != kNormNone ? static_cast<char*>(out) + r0 * rowBytes : nullptr;
+    a.bias = bias;
+    a.gamma = gamma;
+    a.beta = beta;
+    a.rows = n;
+    a.hidden = hidden;
+    a.eps = eps;
+    NormXchg x{};
+    switch (plan.variant) {
+      case kNormLL:
+        x.peers = pc.llPtrs();
+        x.srcStride = pc.llSrcStride();
+        x.parityStride = pc.llParityStride();
+        break;
+      case kNormOneShot:
+        x.peers = pc.stagePtrs(0);
+        x.parityStride = l.half;
+        break;
+      case kNormTwoShot: x.peers = pc.stagePtrs(l.bulkOff); break;
+      default: break;
+    }
+    x.mine = x.peers.p[pc.rank];
+    // Every CTA waits for its twin on the peers: the grid must be co-resident.
+    const int blocks = static_cast<int>(std::min<size_t>(n, static_cast<size_t>(pc.coResidentBlocks(kernel))));
+    prologue(pc, stream);
+    launchAllreduceNorm(pc.comm(), a, x, dt, norm, plan.variant, blocks, stream);
+    finish(pc, stream, "allreduce_residual_norm");
+  }
+  return plan.variant;
+}
+
+#undef GLB_NORM_CHECK
+
+
 // ---- data movement ---------------------------------------------------------------------
 
 namespace {

@@ -110,6 +110,29 @@ void allreduceCast(PeerContext& pc, const PeerBuffer& in, size_t inOffset, const
                    const Epilogue& ep = Epilogue());
 
 
+// Allreduce of the partial sums `partial` ((rows, hidden), dt) fused with bias, residual add and
+// a norm, one launch (docs/cuda.md, "Allreduce + residual + norm"): residualOut = round(sum of
+// the partials + bias + residual), out = norm(residualOut) (kNormRms / kNormLayer; kNormNone
+// writes residualOut only). dt is float32, bfloat16 or float16 for every tensor; hidden * element
+// size is a multiple of 16 bytes and at most kMaxNormHidden elements; pointers are 16-byte aligned;
+// bias / gamma / beta may be null. residualOut may be residual; no other output may overlap an
+// input. Every rank passes the same residual, bias, gamma and beta, and gets the same bytes.
+// Invalid arguments raise InputException before anything is launched. Returns the NormVariant.
+int allreduceResidualNorm(PeerContext& pc, const void* partial, const void* residual, void* residualOut, void* out,
+                          const void* bias, const void* gamma, const void* beta, size_t rows, size_t hidden,
+                          DataType dt, int norm, float eps, AllreduceAlgo algo, cudaStream_t stream);
+// The variant that call runs (the planAllreduce choice for a plain buffer of its bytes, or an
+// explicit LL / ONE_SHOT / TWO_SHOT), and its launches: the two-shot stages its rows in the pool's
+// bulk region, so beyond what that holds it runs as consecutive chunks of chunkRows rows.
+struct NormPlan {
+  int variant;
+  size_t chunkRows;
+  size_t launches;
+};
+NormPlan planResidualNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, AllreduceAlgo algo);
+const char* normVariantName(int variant);
+
+
 // ---- data movement -------------------------------------------------------------------
 // `buf`/`out` arguments are registered or symmetric buffers; plain-pointer
 // overloads stage through the pool (payload limited to the pool's bulk region).

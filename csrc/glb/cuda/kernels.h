@@ -17,6 +17,7 @@ void preloadScheduleKernels();
 void preloadLocalKernels();
 void preloadPipelineKernels();
 void preloadP2pKernels();
+void preloadAllreduceNormKernels();
 
 // allreduce_kernels.cu ---------------------------------------------------------------------
 void launchBarrier(const CommArgs& a, cudaStream_t stream);
@@ -53,6 +54,41 @@ void launchCastAllreduce(const CommArgs& a, const PeerPtrs& ins, void* mcIn, con
 const void* twoShotKernelFor(DataType dt, int nranks, int unroll);
 const void* nvlsKernelFor(DataType dt, int unroll);
 const void* castKernelFor(DataType in, DataType out);
+
+// allreduce_norm_kernels.cu — allreduce fused with bias, residual add and RMSNorm / LayerNorm ------
+// Widest row (elements) of the fused operation: a CTA holds a whole row in registers.
+constexpr int kMaxNormHidden = 16384;
+enum NormKind : int { kNormNone = 0, kNormRms = 1, kNormLayer = 2 };
+// The exchange of the partials: LL lines, one-shot pool halves, row-sharded two-shot through the
+// pool's bulk region, or none (one rank).
+enum NormVariant : int { kNormLL = 0, kNormOneShot = 1, kNormTwoShot = 2, kNormLocal = 3 };
+// One (rows, hidden) problem: contiguous rows of hidden elements, 16-byte aligned. bias / gamma /
+// beta may be null (none, 1, 0); out is unused without a norm.
+struct NormArgs {
+  const void* partial;
+  const void* residual;
+  void* residualOut;
+  void* out;
+  const void* bias;
+  const void* gamma;
+  const void* beta;
+  unsigned long long rows;
+  unsigned long long hidden;
+  float eps;
+};
+// Where the partials travel. LL: peers.p[r] = rank r's LL region, mine = mine, srcStride and
+// parityStride its layout. One-shot: rank r's pool halves, parityStride = one half. Two-shot: rank
+// r's 2 x rows rows of the bulk region.
+struct NormXchg {
+  PeerPtrs peers;
+  void* mine;
+  unsigned long long srcStride;
+  unsigned long long parityStride;
+};
+bool normSupports(DataType dt);
+const void* allreduceNormKernelFor(DataType dt, int norm, int variant);
+void launchAllreduceNorm(const CommArgs& a, const NormArgs& n, const NormXchg& x, DataType dt, int norm, int variant,
+                         int blocks, cudaStream_t stream);
 
 // pipeline_kernels.cu — arbitrary pointers through the pool, in-kernel pipelines (allreduce:
 // 3 stages).

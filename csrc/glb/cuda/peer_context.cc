@@ -194,6 +194,7 @@ PeerContext::PeerContext(std::shared_ptr<Context> context, int dev, PeerOptions 
   preloadLocalKernels();
   preloadPipelineKernels();
   preloadP2pKernels();
+  preloadAllreduceNormKernels();
   ensureTuningLoaded();
   fdChannel_ = std::make_unique<FdChannel>(rank);
   exchangeTopology();

@@ -66,6 +66,56 @@ float bf16ToFloat(uint16_t h) {
   return f;
 }
 
+// Fused allreduce + residual + norm in loopback: rank 0's partial row i, element j is 1 + i * H + j,
+// the residual 0.5 * (i * H + j), the bias j, gamma 1 + j / H and beta -j / H, all exact in fp32.
+// Every virtual peer's partial is rank 0's (their staging aliases mine), so row i reduces to
+// P * partial + bias + residual; `rows` says which rows rank 0 computes (the two-shot: its share).
+std::string checkAllreduceNorm(const CommArgs& ca, const NormXchg& x, int variant, int norm, size_t rows, size_t H,
+                               size_t rowsBegin, size_t rowsEnd, int blocks, cudaStream_t s) {
+  const int P = ca.nranks;
+  DevBuf partial(rows * H * 4), residual(rows * H * 4), resOut(rows * H * 4), out(rows * H * 4), vec(3 * H * 4);
+  launchFill(partial.p, rows * H, DataType::FLOAT32, 1.0, 1.0, s);
+  launchFill(residual.p, rows * H, DataType::FLOAT32, 0.0, 0.5, s);
+  launchFill(vec.p, H, DataType::FLOAT32, 0.0, 1.0, s);
+  launchFill(static_cast<float*>(vec.p) + H, H, DataType::FLOAT32, 1.0, 1.0 / H, s);
+  launchFill(static_cast<float*>(vec.p) + 2 * H, H, DataType::FLOAT32, 0.0, -1.0 / H, s);
+  NormArgs a;
+  a.partial = partial.p;
+  a.residual = residual.p;
+  a.residualOut = resOut.p;
+  a.out = out.p;
+  a.bias = vec.p;
+  a.gamma = static_cast<float*>(vec.p) + H;
+  a.beta = static_cast<float*>(vec.p) + 2 * H;
+  a.rows = rows;
+  a.hidden = H;
+  a.eps = 1e-5f;
+  launchAllreduceNorm(ca, a, x, DataType::FLOAT32, norm, variant, blocks, s);
+  noteLaunch();
+  auto r = download(resOut.p, rows * H, s);
+  auto o = download(out.p, rows * H, s);
+  for (size_t i = rowsBegin; i < rowsEnd; i++) {
+    std::vector<double> v(H);
+    double mean = 0, sq = 0;
+    for (size_t j = 0; j < H; j++) {
+      const double e = static_cast<double>(i * H + j);
+      v[j] = P * (1.0 + e) + 0.5 * e + static_cast<double>(j);
+      if (r[i * H + j] != static_cast<float>(v[j])) return strcat_all("residual_out[", i, ", ", j, "]: got ", r[i * H + j], " want ", v[j]);
+      mean += v[j] / H;
+    }
+    if (norm == kNormNone) continue;
+    for (size_t j = 0; j < H; j++) sq += (norm == kNormLayer ? (v[j] - mean) * (v[j] - mean) : v[j] * v[j]) / H;
+    for (size_t j = 0; j < H; j++) {
+      const double g = 1.0 + static_cast<double>(j) / H, b = -static_cast<double>(j) / H;
+      const double want = norm == kNormLayer ? (v[j] - mean) / std::sqrt(sq + 1e-5) * g + b : v[j] / std::sqrt(sq + 1e-5) * g;
+      if (std::fabs(o[i * H + j] - want) > 1e-5 * std::fabs(want) + 1e-5) {
+        return strcat_all("out[", i, ", ", j, "]: got ", o[i * H + j], " want ", want);
+      }
+    }
+  }
+  return "";
+}
+
 class Runner {
  public:
   Runner(PeerContext& pc, cudaStream_t s) : pc_(pc), s_(s) {}
@@ -252,6 +302,39 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
       }
       return "";
     });
+
+    // ---- allreduce + residual + norm: LL, one-shot and row-sharded two-shot ----------------------
+    {
+      const size_t rows = 5, H = 1024;  // 20 KB: one LL slot of every virtual peer holds it at P = 8
+      const char* norms[] = {"none", "rms", "layer"};
+      for (int variant : {kNormLL, kNormOneShot, kNormTwoShot}) {
+        for (int norm : {kNormNone, kNormRms, kNormLayer}) {
+          R.run(strcat_all("allreduceNormKernel<float,", norms[norm], ",", normVariantName(variant), "> P=", P),
+                [&]() -> std::string {
+            NormXchg x{};
+            size_t rb = 0, re = rows;
+            if (variant == kNormLL) {
+              // Virtual peer r's region is mine shifted by r source slots: my store for "peer r" lands
+              // in the slot I poll for rank r. The slots shrink to fit P of them in my region.
+              const size_t region = pc.llParityStride() * 2;
+              x.srcStride = region / 2 / P / 16 * 16;
+              x.parityStride = x.srcStride * P;
+              if (rows * H * 4 * 2 > x.srcStride) return "skipped: LL region too small";
+              char* myLL = static_cast<char*>(pc.llPtrs().p[pc.rank]);
+              for (int r = 0; r < P; r++) x.peers.p[r] = myLL + r * x.srcStride;
+            } else if (variant == kNormOneShot) {
+              for (int r = 0; r < P; r++) x.peers.p[r] = myStage;
+              x.parityStride = half;
+            } else {
+              for (int r = 0; r < P; r++) x.peers.p[r] = myStage + 2 * half;
+              shareOfHost(rows, P, 0, rb, re);
+            }
+            x.mine = x.peers.p[0];
+            return checkAllreduceNorm(ca, x, variant, norm, rows, H, rb, re, 3, stream);
+          });
+        }
+      }
+    }
 
     // ---- data movement ---------------------------------------------------------------------
     R.run(strcat_all("broadcastKernel(direct) P=", P), [&]() -> std::string {
@@ -930,6 +1013,9 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
   // ---- flag-in-data kernels: one rank (no peers to hear from), fused scale + cast -------------
   {
     const CommArgs one = pc.loopbackComm(1);
+    R.run("allreduceNormKernel<float,layer,local>", [&]() -> std::string {
+      return checkAllreduceNorm(one, NormXchg{}, kNormLocal, kNormLayer, 7, 4096, 0, 7, 4, stream);
+    });
     R.run("llAllreduceKernel<float,float>", [&]() -> std::string {
       const size_t m = std::min<size_t>(pc.llMaxBytes() / 4, 4099);
       DevBuf in(m * 4), out(m * 4);

@@ -192,6 +192,33 @@ void registerCuda(py::module_& root) {
      py::arg("dtype"), py::arg("out_dtype"), py::arg("op") = 1, py::arg("stream") = 0, py::arg("scale") = 1.0,
      py::arg("blocks") = 0);
 
+  m.def("allreduce_residual_norm", [](PeerContext& pc, uintptr_t partial, uintptr_t residual, uintptr_t residualOut,
+                                      uintptr_t out, uintptr_t bias, uintptr_t gamma, uintptr_t beta, size_t rows,
+                                      size_t hidden, int dtype, int norm, double eps, int algo, uintptr_t stream) {
+    int v;
+    {
+      py::gil_scoped_release nogil;
+      v = allreduceResidualNorm(pc, P(partial), P(residual), P(residualOut), P(out), P(bias), P(gamma), P(beta), rows,
+                                hidden, static_cast<DataType>(dtype), norm, static_cast<float>(eps),
+                                static_cast<AllreduceAlgo>(algo), S(stream));
+    }
+    return std::string(normVariantName(v));
+  }, py::arg("pc"), py::arg("partial"), py::arg("residual"), py::arg("residual_out"), py::arg("out"), py::arg("bias"),
+     py::arg("gamma"), py::arg("beta"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"),
+     py::arg("eps"), py::arg("algo") = 0, py::arg("stream") = 0,
+     "Allreduce of partial sums fused with bias, residual add and a norm (0 none, 1 rms, 2 layer); null pointers are 0. "
+     "Returns the variant that ran.");
+  m.def("plan_residual_norm", [](PeerContext& pc, size_t rows, size_t hidden, int dtype, int norm, int algo) {
+    const NormPlan p = planResidualNorm(pc, rows, hidden, static_cast<DataType>(dtype), norm,
+                                        static_cast<AllreduceAlgo>(algo));
+    py::dict d;
+    d["variant"] = std::string(normVariantName(p.variant));
+    d["chunk_rows"] = p.chunkRows;
+    d["launches"] = p.launches;
+    return d;
+  }, py::arg("pc"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"), py::arg("algo") = 0);
+  m.attr("MAX_NORM_HIDDEN") = kMaxNormHidden;
+
   m.def("plan_allreduce", [](PeerContext& pc, size_t bytes, int dtype, int op, int kind) {
     AllreducePlan p = planAllreduce(pc, bytes, static_cast<DataType>(dtype), static_cast<ReduceOp>(op),
                                     static_cast<BufKind>(kind));

@@ -3,7 +3,9 @@
 Attention: the QKV projection is column-parallel (every rank owns H/P heads), attention runs
 locally over those heads, the output projection is row-parallel -> ONE allreduce. MLP: column-
 parallel up-projection, GELU, row-parallel down-projection -> ONE allreduce. Backward mirrors it
-(one allreduce per half). CUDA tensors run the fused NVLink kernels, CPU tensors the TCP transport.
+(one allreduce per half). CUDA tensors run the fused NVLink kernels, where each row-parallel
+allreduce also adds the bias and the residual and, after the attention, applies ln2
+(``TensorParallel.reduce_residual_norm``); CPU tensors run the TCP transport.
 ``DenseBlock`` is the single-process reference with the same parameters (tests load one into the other).
 """
 from __future__ import annotations
@@ -65,5 +67,11 @@ class TPBlock(nn.Module):
         h = self.ln1(x)
         q, k, v = (lin(h).view(B, S, self.local_heads, hd).transpose(1, 2) for lin in (self.q, self.k, self.v))
         a = nn.functional.scaled_dot_product_attention(q, k, v, is_causal=True)
-        x = x + self.proj(a.transpose(1, 2).reshape(B, S, self.local_heads * hd))
+        a = a.transpose(1, 2).reshape(B, S, self.local_heads * hd)
+        if x.is_cuda:
+            # each row-parallel output: allreduce + bias + residual add (+ ln2) in one kernel
+            x, h = self.tp.reduce_residual_norm(nn.functional.linear(a, self.proj.weight), x, self.ln2, self.proj.bias)
+            p = nn.functional.linear(nn.functional.gelu(self.up(h)), self.down.weight)
+            return self.tp.reduce_residual_norm(p, x, None, self.down.bias)
+        x = x + self.proj(a)
         return x + self.down(nn.functional.gelu(self.up(self.ln2(x))))

@@ -198,6 +198,62 @@ class CudaContext:
         kind = 2 if buf is None else (0 if (buf.has_multicast and off % 16 == 0) else 1)
         return _cu.plan_allreduce(self.pc, n * element_size(dt), int(dt), int(op), kind)
 
+    def allreduce_residual_norm(self, partial, residual, weight=None, norm_bias=None, *, norm: Optional[str] = "rms",
+                                eps: float = 1e-6, bias=None, residual_out=None, out=None, algo="auto", stream=None):
+        """The row-parallel output step of tensor parallelism in ONE kernel launch: allreduce of the
+        partial sums, ``+ bias``, ``+ residual`` and the next norm.
+
+        For every row (the last dimension is the hidden size H): ``residual_out = round(sum over ranks
+        of partial + bias + residual)`` in fp32, rounded once; ``out`` = RMSNorm (``norm="rms"``:
+        ``x / sqrt(mean(x^2) + eps) * weight``) or LayerNorm (``norm="layer"``: ``(x - mean) /
+        sqrt(var + eps) * weight + norm_bias``) of that rounded ``residual_out``, statistics in fp32,
+        rounded once. ``norm=None`` writes ``residual_out`` only.
+
+        Every tensor is float32, bfloat16 or float16 (one dtype), contiguous and 16-byte aligned; H *
+        element size is a multiple of 16 bytes and H is at most ``MAX_NORM_HIDDEN`` (16384).
+        ``residual``, ``bias``, ``weight`` and ``norm_bias`` must be the same on every rank; every rank
+        then gets the same bytes. ``residual_out`` defaults to ``residual`` (in place); ``out`` is
+        allocated when not given. ``algo``: ``"auto"`` (the allreduce's choice for a plain tensor of
+        the same size), ``"ll"``, ``"one_shot"`` or ``"two_shot"``. Invalid arguments raise
+        ``ValueError`` before anything is launched.
+
+        Returns ``(residual_out, out)``, or ``residual_out`` when ``norm`` is None."""
+        import torch
+
+        kinds = {None: 0, "rms": 1, "layer": 2}
+        if norm not in kinds:
+            raise ValueError(f"allreduce_residual_norm: norm must be 'rms', 'layer' or None, got {norm!r}")
+        if algo not in ("auto", "ll", "one_shot", "two_shot"):
+            raise ValueError(f"allreduce_residual_norm: algo must be auto, ll, one_shot or two_shot, got {algo!r}")
+        if norm != "layer" and norm_bias is not None:
+            raise ValueError("allreduce_residual_norm: norm_bias needs norm='layer'")
+        if norm is None and weight is not None:
+            raise ValueError("allreduce_residual_norm: weight needs a norm")
+        if partial.dim() == 0:
+            raise ValueError("allreduce_residual_norm: partial must have a hidden dimension")
+        H = partial.shape[-1]
+        if residual_out is None:
+            residual_out = residual
+        if norm is not None and out is None:
+            out = torch.empty_like(partial, memory_format=torch.contiguous_format)
+        named = {"partial": partial, "residual": residual, "residual_out": residual_out, "out": out, "bias": bias,
+                 "weight": weight, "norm_bias": norm_bias}
+        for name, t in named.items():
+            if t is None:
+                continue
+            if not t.is_cuda or t.dtype != partial.dtype or not t.is_contiguous():
+                raise ValueError(f"allreduce_residual_norm: {name} must be a contiguous CUDA tensor of {partial.dtype}, "
+                                 f"got {t.dtype} on {t.device}{'' if t.is_contiguous() else ', not contiguous'}")
+            want = (H,) if name in ("bias", "weight", "norm_bias") else tuple(partial.shape)
+            if tuple(t.shape) != want:
+                raise ValueError(f"allreduce_residual_norm: {name} has shape {tuple(t.shape)}, expected {want}")
+        _, _, dt, _ = describe(partial)
+        ptr = lambda t: 0 if t is None else t.data_ptr()  # noqa: E731
+        _cu.allreduce_residual_norm(self.pc, ptr(partial), ptr(residual), ptr(residual_out), ptr(out), ptr(bias),
+                                    ptr(weight), ptr(norm_bias), partial.numel() // max(H, 1), H, int(dt), kinds[norm],
+                                    float(eps), _algo(algo), _stream(stream))
+        return residual_out if norm is None else (residual_out, out)
+
     # ---- health ---------------------------------------------------------------------------
     def set_timeout(self, ms: int):
         """Device-side waits give up after ``ms`` milliseconds (then the context is poisoned)."""

@@ -11,6 +11,20 @@ def _is_cuda(t) -> bool:
     return bool(getattr(t, "is_cuda", False))
 
 
+def _norm_parts(module, dtype):
+    """(kind, weight, bias, eps) of a norm module as the fused kernel takes them; kind is None for
+    no module and "unsupported" for a module it does not implement."""
+    import torch
+
+    if module is None:
+        return None, None, None, 0.0
+    if isinstance(module, torch.nn.LayerNorm):
+        return "layer", module.weight, module.bias, module.eps
+    if isinstance(module, getattr(torch.nn, "RMSNorm", ())):
+        return "rms", module.weight, None, module.eps if module.eps is not None else torch.finfo(dtype).eps
+    return "unsupported", None, None, 0.0
+
+
 class _Base:
     def __init__(self, ctx, cuda_ctx=None):
         """ctx: host context (control plane, CPU tensors); cuda_ctx: ops.cuda.CudaContext."""
@@ -390,6 +404,88 @@ class TensorParallel(_Base):
                 return grad
 
         return _G.apply(x)
+
+    def reduce_residual_norm(self, partial, residual, norm_module=None, bias=None):
+        """g fused with what follows a row-parallel matmul: ``s = allreduce(partial) + bias +
+        residual`` and the next norm. Returns ``(s, norm_module(s))``, or ``s`` when
+        ``norm_module`` is None. ``norm_module`` is an ``nn.LayerNorm``, an ``nn.RMSNorm`` or None.
+
+        CUDA tensors within the fused operation's limits run it as one kernel
+        (``CudaContext.allreduce_residual_norm``), into a fresh ``s``. The backward is g's: the
+        gradient of ``s`` plus the norm's input gradient (recomputed from the saved ``s``) goes to
+        both ``partial`` and ``residual``, its row sum to ``bias``, and the norm's weights get
+        theirs from the recompute. Anything else runs ``reduce_from_region``, ``+ bias``,
+        ``+ residual`` and the module."""
+        import torch
+
+        F = torch.nn.functional
+        kind, weight, norm_bias, eps = _norm_parts(norm_module, partial.dtype)
+        if not self._fusable(partial, residual, norm_module, kind, (bias, weight, norm_bias)):
+            y = self.reduce_from_region(partial)
+            if bias is not None:
+                y = y + bias
+            s = y + residual
+            return s if norm_module is None else (s, norm_module(s))
+        H = partial.shape[-1]
+        tp = self
+
+        def recompute(x, w, b):
+            if kind == "rms":
+                return F.rms_norm(x, (H,), w, eps)
+            return F.layer_norm(x, (H,), w, b, eps)
+
+        class _R(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, p, res, b, w, nb):
+                s = torch.empty_like(res, memory_format=torch.contiguous_format)
+                got = tp.cc.allreduce_residual_norm(p.contiguous(), res.contiguous(), w, nb, norm=kind, eps=eps, bias=b,
+                                                   residual_out=s)
+                ctx.save_for_backward(s, w, nb)
+                ctx.has_bias = b is not None
+                return got
+
+            @staticmethod
+            def backward(ctx, grad_s, grad_out=None):
+                s, w, nb = ctx.saved_tensors
+                grad_s = torch.zeros_like(s) if grad_s is None else grad_s
+                gw = gnb = None
+                if kind is not None and grad_out is not None:
+                    with torch.enable_grad():
+                        x = s.detach().requires_grad_(True)
+                        ws = [t.detach().requires_grad_(True) if t is not None else None for t in (w, nb)]
+                        y = recompute(x, *ws)
+                        need = [x] + [t for t in ws if t is not None]
+                        got = list(torch.autograd.grad(y, need, grad_out))
+                    grad_s = grad_s + got.pop(0)
+                    gw = got.pop(0) if w is not None else None
+                    gnb = got.pop(0) if nb is not None else None
+                gb = grad_s.reshape(-1, H).sum(0) if ctx.has_bias else None
+                return grad_s, grad_s, gb, gw, gnb
+
+        return _R.apply(partial, residual, bias, weight, norm_bias)
+
+    def _fusable(self, partial, residual, norm_module, kind, vectors) -> bool:
+        """Whether reduce_residual_norm can run the fused kernel on these tensors."""
+        import torch
+
+        if self.cc is None or not _is_cuda(partial) or kind == "unsupported" or partial.dim() == 0:
+            return False
+        H = partial.shape[-1]
+        if partial.dtype not in (torch.float32, torch.bfloat16, torch.float16) or residual.shape != partial.shape:
+            return False
+        if H * partial.element_size() % 16 or H > _C.cuda.MAX_NORM_HIDDEN:
+            return False
+        if norm_module is not None and tuple(norm_module.normalized_shape) != (H,):
+            return False
+        for t in (partial, residual):
+            # a non-contiguous tensor is copied, and the copy is aligned
+            if t.dtype != partial.dtype or (t.is_contiguous() and t.data_ptr() % 16):
+                return False
+        for t in vectors:
+            if t is not None and (not t.is_cuda or t.dtype != partial.dtype or not t.is_contiguous() or
+                                  t.data_ptr() % 16 or tuple(t.shape) != (H,)):
+                return False
+        return True
 
     def column_linear(self, in_features: int, out_features: int, bias: bool = True, device=None, dtype=None):
         return ColumnParallelLinear(self, in_features, out_features, bias, device, dtype)

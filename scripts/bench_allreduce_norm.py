@@ -1,0 +1,184 @@
+#!/usr/bin/env python
+"""The fused tensor-parallel step (allreduce + bias + residual add + RMSNorm / LayerNorm, one kernel:
+`CudaContext.allreduce_residual_norm`) against the unfused sequence on the same inputs: clone of the
+partial, `cc.allreduce`, bias add, residual add, `F.rms_norm` / `F.layer_norm`.
+
+Run one rank per GPU under torch.distributed.run:
+
+    python -m torch.distributed.run --nproc_per_node 8 scripts/bench_allreduce_norm.py --out norm.json
+
+or, for a rehearsal on one GPU, `--threads P` (P ranks as threads sharing cuda:0). Ranks that share
+a card pay for each other's kernels and exchange through local memory, so those numbers measure
+the per-call overhead only, not the link; the JSON says so.
+
+Time per call: CUDA events around `--iters` back-to-back calls after `--warmup` calls, median over
+`--reps` windows, the maximum over ranks. Launches per call: the library's launch counter for the
+fused path, kernels counted by torch.profiler for the unfused one (one rank per process only). Prints one JSON document and
+writes it to `--out` when given.
+"""
+import argparse
+import json
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+import torch.nn.functional as F  # noqa: E402
+
+import gloo_b200 as gb  # noqa: E402
+from gloo_b200.ops import cuda as gcu  # noqa: E402
+
+DECODE_T = (1, 8, 32, 128)
+PREFILL_T = (4096,)
+HIDDEN = (4096, 8192)
+
+
+def gpu_info(device):
+    name = torch.cuda.get_device_name(device)
+    power = None
+    try:
+        import subprocess
+
+        q = subprocess.run(["nvidia-smi", f"--id={device}", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        power = float(q.stdout.strip().splitlines()[0]) if q.returncode == 0 and q.stdout.strip() else None
+    except Exception:  # noqa: BLE001
+        power = None
+    return {"gpu": name, "power_limit_w": power}
+
+
+def bench_rank(ctx, device, args, world, profile_unfused=True):
+    cc = gcu.CudaContext(ctx, device, stage_bytes=args.stage_mb << 20)
+    cc.set_timeout(600000)
+    stream = torch.cuda.current_stream()
+    dtype = torch.bfloat16
+    rows = []
+    for H in HIDDEN:
+        for T in DECODE_T + PREFILL_T:
+            g = torch.Generator(device="cpu").manual_seed(T * 131 + H)
+            partial = torch.randn(T, H, generator=g).to(dtype).cuda()
+            residual = torch.randn(T, H, generator=g).to(dtype).cuda()
+            bias = torch.randn(H, generator=g).to(dtype).cuda()
+            weight = (1 + 0.1 * torch.randn(H, generator=g)).to(dtype).cuda()
+            norm_bias = (0.1 * torch.randn(H, generator=g)).to(dtype).cuda()
+            res_out, out = torch.empty_like(residual), torch.empty_like(residual)
+            for norm in ("rms", "layer"):
+                nb = norm_bias if norm == "layer" else None
+
+                def fused():
+                    cc.allreduce_residual_norm(partial, residual, weight, nb, norm=norm, eps=1e-6, bias=bias,
+                                               residual_out=res_out, out=out)
+
+                def unfused():
+                    y = partial.clone()
+                    cc.allreduce(y)
+                    y = y + bias
+                    s = residual + y
+                    if norm == "rms":
+                        return s, F.rms_norm(s, (H,), weight, 1e-6)
+                    return s, F.layer_norm(s, (H,), weight, nb, 1e-6)
+
+                # same results (the unfused sequence rounds after each step, the fused one once)
+                s_ref, o_ref = unfused()
+                fused()
+                torch.cuda.synchronize()
+                err = float((out.float() - o_ref.float()).abs().max())
+                plan = gb._C.cuda.plan_residual_norm(cc.pc, T, H, int(gb.DataType.BFLOAT16), {"rms": 1, "layer": 2}[norm], 0)
+                row = {"T": T, "H": H, "dtype": "bfloat16", "norm": norm, "bytes": T * H * 2, "variant": plan["variant"],
+                       "max_abs_diff_out": err}
+                for name, fn in (("fused", fused), ("unfused", unfused)):
+                    row[f"{name}_us"] = timed(ctx, cc, fn, stream, args, world)
+                row["fused_launches_per_call"] = launches_fused(cc, fused)
+                row["unfused_kernels_per_call"] = kernels_unfused(unfused, profile_unfused)
+                row["speedup"] = row["unfused_us"] / row["fused_us"]
+                rows.append(row)
+    return rows
+
+
+def timed(ctx, cc, fn, stream, args, world):
+    for _ in range(args.warmup):
+        fn()
+    per = []
+    for _ in range(args.reps):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        cc.pc.host_barrier()
+        a.record(stream)
+        for _ in range(args.iters):
+            fn()
+        b.record(stream)
+        b.synchronize()
+        per.append(a.elapsed_time(b) * 1e3 / args.iters)
+    v = np.asarray([float(np.median(per))], dtype=np.float64)
+    if world > 1:
+        gb.allreduce(ctx, v, op=gb.ReduceOp.MAX)
+    return float(v[0])
+
+
+def launches_fused(cc, fn):
+    torch.cuda.synchronize()
+    cc.pc.host_barrier()
+    before = gb._C.cuda.launch_count()
+    fn()
+    torch.cuda.synchronize()
+    cc.pc.host_barrier()
+    after = gb._C.cuda.launch_count()
+    cc.pc.host_barrier()
+    return (after - before) // cc.pc.ranks_on_my_device()
+
+
+def kernels_unfused(fn, count):
+    """Device kernels and copies of one call of the unfused sequence (the library's own kernel
+    included), from torch.profiler. The profiler must run on the main thread, so with ranks as
+    threads it is not run (None) and the call only takes part in the allreduce."""
+    from torch.profiler import ProfilerActivity, profile
+
+    torch.cuda.synchronize()
+    if not count:
+        fn()
+        torch.cuda.synchronize()
+        return None
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    return sum(1 for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", default="")
+    ap.add_argument("--threads", type=int, default=0, help="rehearsal: this many ranks as threads on cuda:0")
+    ap.add_argument("--iters", type=int, default=200)
+    ap.add_argument("--warmup", type=int, default=50)
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--stage-mb", type=int, default=128)
+    args = ap.parse_args()
+    if args.threads:
+        world = args.threads
+        rows = gb.spawn_threads(world, lambda ctx: bench_rank(ctx, 0, args, 1, False), cuda_device=0,
+                               timeout_ms=600000)[0]
+        mode = f"{world} ranks as threads on one GPU: overhead only, not link numbers"
+        info = gpu_info(0)
+        rank = 0
+    else:
+        rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
+        local = int(os.environ.get("LOCAL_RANK", 0))
+        torch.cuda.set_device(local)
+        ctx = gb.init_context(rank, world, path=f"/tmp/glb_norm_{os.environ.get('MASTER_PORT', '0')}_{os.getppid()}",
+                              timeout_ms=120000)
+        rows = bench_rank(ctx, local, args, world)
+        mode = f"{world} ranks, one per GPU"
+        info = gpu_info(local)
+    if rank == 0:
+        doc = {"benchmark": "allreduce_residual_norm", "mode": mode, "ranks": world, **info, "iters": args.iters,
+               "warmup": args.warmup, "reps": args.reps, "rows": rows}
+        text = json.dumps(doc)
+        print(text)
+        if args.out:
+            with open(args.out, "w") as f:
+                f.write(text + "\n")
+
+
+if __name__ == "__main__":
+    main()
