@@ -24,6 +24,11 @@
 //             which only the row's owner reads; out after the partials), barrier, every rank
 //             copies its pool rows out to its own residualOut / out.
 //   LOCAL     one rank: the epilogue on the partial, no exchange.
+//   SCATTER   the reduce-scatter form (sequence parallelism): residual / residualOut / an
+//             ungathered out are this rank's shard of the rows. Stage every shard's chunk in the
+//             bulk region, barrier, rank r reduces the rows of shard r and writes residualOut
+//             (and an ungathered out) straight to its own tensors; with `gather` it stores out
+//             into every peer's pool, barrier, and every rank copies all P shards of out.
 #include "glb/cuda/device_common.cuh"
 #include "glb/cuda/kernels.h"
 
@@ -245,7 +250,7 @@ allreduceNormKernel(CommArgs a, NormArgs n, NormXchg x) {
       rowEpilogue<T, NORM>(acc, n, i, npacks, sh, toUser(i));
     }
     retire(a, 1, 1);
-  } else {
+  } else if constexpr (V == kNormTwoShot) {
     // Pool rows: [0, rows) the staged partials, overwritten with residualOut by the row's owner;
     // [rows, 2 rows) out.
     const uint32_t e = loadEpoch(a);
@@ -279,6 +284,45 @@ allreduceNormKernel(CommArgs a, NormArgs n, NormXchg x) {
       }
     }
     retire(a, 2, 0);
+  } else {
+    // n.rows rows of every shard. Pool rows: [0, P rows) the staged partials, row q * rows + i =
+    // the user's partial row q * shardRows + i; with a gathered out, [P rows, 2 P rows) out in the
+    // same order. Rank me owns pool rows [me * rows, (me + 1) * rows), shard row i = j - me * rows.
+    // Two barriers either way: with a gathered out the second orders the out stores before the
+    // copy out; without one it is a closing barrier, so that no rank restages its pool (in its
+    // next launch) while a peer may still be reading the rows it staged.
+    const uint32_t e = loadEpoch(a);
+    char* mine = static_cast<char*>(x.mine);
+    const size_t rows = n.rows, all = static_cast<size_t>(P) * rows;
+    const bool gather = NORM != kNormNone && x.gather != 0;
+    auto userRow = [&](size_t j) { return j / rows * x.shardRows + j % rows; };
+    for (size_t j = blockIdx.x; j < all; j += gridDim.x) copyRow<T>(mine + j * rb, rowPtr(n.partial, userRow(j), rb), npacks);
+    if (!blockBarrier(a, e + 1)) {
+      retire(a, 2, 0);
+      return;
+    }
+    const size_t sb = me * rows, se = sb + rows;
+    const size_t first = sb + (blockIdx.x + gridDim.x - sb % gridDim.x) % gridDim.x;
+    for (size_t j = first; j < se; j += gridDim.x) {
+      const size_t i = j - sb;
+      zeroAcc<T>(acc);
+      for (int r = 0; r < P; r++) addRow<T>(acc, peers[r] + j * rb, npacks);
+      rowEpilogue<T, NORM>(acc, n, i, npacks, sh, [&](int pk, const Pack16& rr, const Pack16& o) {
+        st128(static_cast<char*>(n.residualOut) + i * rb + pk * 16, rr);
+        if (NORM == kNormNone) return;
+        if (gather) {
+          for (int r = 0; r < P; r++) st128_stream(peers[r] + (all + j) * rb + pk * 16, o);
+        } else {
+          st128(static_cast<char*>(n.out) + i * rb + pk * 16, o);
+        }
+      });
+    }
+    if (blockBarrier(a, e + 2) && gather) {
+      for (size_t j = blockIdx.x; j < all; j += gridDim.x) {
+        copyRow<T>(static_cast<char*>(n.out) + userRow(j) * rb, mine + (all + j) * rb, npacks);
+      }
+    }
+    retire(a, 2, 0);
   }
 }
 
@@ -292,6 +336,7 @@ auto normFn(int norm, int variant) -> decltype(&allreduceNormKernel<T, kNormNone
       case kNormOneShot: return allreduceNormKernel<T, N, kNormOneShot>;
       case kNormTwoShot: return allreduceNormKernel<T, N, kNormTwoShot>;
       case kNormLocal: return allreduceNormKernel<T, N, kNormLocal>;
+      case kNormScatter: return allreduceNormKernel<T, N, kNormScatter>;
       default: return nullptr;
     }
   };
@@ -329,7 +374,7 @@ const void* allreduceNormKernelFor(DataType dt, int norm, int variant) {
 void preloadAllreduceNormKernels() {
   for (DataType dt : {DataType::FLOAT32, DataType::BFLOAT16, DataType::FLOAT16}) {
     for (int norm : {kNormNone, kNormRms, kNormLayer}) {
-      for (int v : {kNormLL, kNormOneShot, kNormTwoShot, kNormLocal}) {
+      for (int v : {kNormLL, kNormOneShot, kNormTwoShot, kNormLocal, kNormScatter}) {
         dispatchNormType(dt, [&](auto tag) { touchKernel(normFn<decltype(tag)>(norm, v)); });
       }
     }

@@ -509,25 +509,57 @@ NormPlan planResidualNorm(PeerContext& pc, size_t rows, size_t hidden, DataType 
   return p;
 }
 
+NormPlan planReduceScatterNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, bool gatherOut) {
+  const size_t P = static_cast<size_t>(pc.size);
+  if (rows % P != 0) {
+    GLB_THROW(InputException, "reduce_scatter_residual_norm: ", rows, " rows do not split into ", P, " equal shards");
+  }
+  // One rank: the shard is every row, and the allreduce form's local launch computes it.
+  if (P == 1) return planResidualNorm(pc, rows, hidden, dt, norm, AllreduceAlgo::AUTO);
+  const size_t rowBytes = hidden * elementSize(dt), shard = rows / P;
+  const auto l = layoutOf(pc);
+  // One launch while the staged rows of every shard (and the gathered out) fit the bulk region;
+  // beyond it, consecutive chunks of chunkRows rows of every shard.
+  const size_t perRow = P * (norm != kNormNone && gatherOut ? 2 : 1) * rowBytes;
+  if (perRow > l.bulkBytes) {
+    GLB_THROW(InputException, "reduce_scatter_residual_norm: the pool's bulk region holds no row of ", rowBytes,
+              " bytes from each of ", P, " shards; raise GLB_CUDA_STAGE_MB (CudaContext stage_bytes)");
+  }
+  NormPlan p;
+  p.variant = kNormScatter;
+  p.chunkRows = std::min(std::max<size_t>(shard, 1), l.bulkBytes / perRow);
+  p.launches = shard == 0 ? 0 : ceilDiv(shard, p.chunkRows);
+  return p;
+}
+
 const char* normVariantName(int variant) {
   switch (variant) {
     case kNormLL: return "ll";
     case kNormOneShot: return "one_shot";
     case kNormTwoShot: return "two_shot";
+    case kNormScatter: return "reduce_scatter";
     default: return "local";
   }
 }
 
+namespace {
+
+// A tensor argument of the fused operations: `rows` rows of `hidden` elements (1 for a vector).
+struct NormRange {
+  const char* name;
+  const void* p;
+  size_t rows;
+};
+
 #define GLB_NORM_CHECK(cond, ...) \
   do {                            \
-    if (!(cond)) GLB_THROW(InputException, "allreduce_residual_norm: ", __VA_ARGS__); \
+    if (!(cond)) GLB_THROW(InputException, op, ": ", __VA_ARGS__); \
   } while (0)
 
-int allreduceResidualNorm(PeerContext& pc, const void* partial, const void* residual, void* residualOut, void* out,
-                          const void* bias, const void* gamma, const void* beta, size_t rows, size_t hidden,
-                          DataType dt, int norm, float eps, AllreduceAlgo algo, cudaStream_t stream) {
-  GLB_TRACE_RANGE("glb::cuda::allreduceResidualNorm");
-  pc.checkHealth();
+// What both fused operations check before anything is launched. inputs: partial, residual, bias,
+// weight, norm_bias; outputs: residual_out and out (null without a norm). Null vectors are absent.
+void checkNormCall(const char* op, DataType dt, int norm, size_t hidden, bool empty, const NormRange (&inputs)[5],
+                   const NormRange (&outputs)[2]) {
   GLB_NORM_CHECK(normSupports(dt), "rows must be float32, bfloat16 or float16, got ", dataTypeName(dt));
   GLB_NORM_CHECK(norm == kNormNone || norm == kNormRms || norm == kNormLayer, "unknown norm ", norm);
   const size_t es = elementSize(dt);
@@ -535,55 +567,79 @@ int allreduceResidualNorm(PeerContext& pc, const void* partial, const void* resi
                  " elements is not a positive multiple of 16 bytes");
   GLB_NORM_CHECK(hidden <= static_cast<size_t>(kMaxNormHidden), "rows of ", hidden, " elements exceed the limit of ",
                  kMaxNormHidden);
-  const size_t rowsBytes = rows * hidden * es, vecBytes = hidden * es;
-  struct Range {
-    const char* name;
-    const void* p;
-    size_t bytes;
-  };
-  const Range inputs[] = {{"partial", partial, rowsBytes}, {"residual", residual, rowsBytes}, {"bias", bias, vecBytes},
-                          {"weight", gamma, vecBytes}, {"norm_bias", beta, vecBytes}};
-  const Range outputs[] = {{"residual_out", residualOut, rowsBytes}, {"out", norm != kNormNone ? out : nullptr, rowsBytes}};
-  GLB_NORM_CHECK(rows == 0 || (partial != nullptr && residual != nullptr && residualOut != nullptr &&
-                               (norm == kNormNone || out != nullptr)),
+  GLB_NORM_CHECK(empty || (inputs[0].p != nullptr && inputs[1].p != nullptr && outputs[0].p != nullptr &&
+                           (norm == kNormNone || outputs[1].p != nullptr)),
                  "partial, residual, residual_out and (with a norm) out are required");
-  for (const Range& r : inputs) {
+  for (const NormRange& r : inputs) {
     GLB_NORM_CHECK(reinterpret_cast<uintptr_t>(r.p) % 16 == 0, r.name, " must be 16-byte aligned");
   }
-  for (const Range& r : outputs) {
+  for (const NormRange& r : outputs) {
     GLB_NORM_CHECK(reinterpret_cast<uintptr_t>(r.p) % 16 == 0, r.name, " must be 16-byte aligned");
   }
-  auto overlap = [](const Range& a, const Range& b) {
+  const size_t rowBytes = hidden * es;
+  auto overlap = [&](const NormRange& a, const NormRange& b) {
     const uintptr_t x = reinterpret_cast<uintptr_t>(a.p), y = reinterpret_cast<uintptr_t>(b.p);
-    return a.p != nullptr && b.p != nullptr && a.bytes > 0 && b.bytes > 0 && x < y + b.bytes && y < x + a.bytes;
+    const size_t ab = a.rows * rowBytes, bb = b.rows * rowBytes;
+    return a.p != nullptr && b.p != nullptr && ab > 0 && bb > 0 && x < y + bb && y < x + ab;
   };
-  for (const Range& o : outputs) {
-    for (const Range& i : inputs) {
+  for (const NormRange& o : outputs) {
+    for (const NormRange& i : inputs) {
       // residual_out may be residual itself (in place: each row is read before it is written).
-      const bool inPlace = o.p == residualOut && i.p == residual && residualOut == residual;
+      const bool inPlace = &o == &outputs[0] && &i == &inputs[1] && o.p == i.p;
       GLB_NORM_CHECK(inPlace || !overlap(o, i), o.name, " overlaps ", i.name);
     }
   }
   GLB_NORM_CHECK(!overlap(outputs[0], outputs[1]), "residual_out overlaps out");
+}
+
+// The arguments of one chunk: n rows from `off` bytes into every row tensor.
+NormArgs chunkArgs(const void* partial, const void* residual, void* residualOut, void* out, const void* bias,
+                   const void* gamma, const void* beta, size_t off, size_t n, size_t hidden, int norm, float eps) {
+  NormArgs a;
+  a.partial = static_cast<const char*>(partial) + off;
+  a.residual = static_cast<const char*>(residual) + off;
+  a.residualOut = static_cast<char*>(residualOut) + off;
+  a.out = norm != kNormNone ? static_cast<char*>(out) + off : nullptr;
+  a.bias = bias;
+  a.gamma = gamma;
+  a.beta = beta;
+  a.rows = n;
+  a.hidden = hidden;
+  a.eps = eps;
+  return a;
+}
+
+// One launch of the fused kernel whose grid-stride loops cover `gridRows` rows.
+void launchNormChunk(PeerContext& pc, const NormArgs& a, const NormXchg& x, DataType dt, int norm, int variant,
+                     size_t gridRows, cudaStream_t stream, const char* op) {
+  // Every CTA waits for its twin on the peers: the grid must be co-resident.
+  const void* kernel = allreduceNormKernelFor(dt, norm, variant);
+  const int blocks = static_cast<int>(std::min<size_t>(gridRows, static_cast<size_t>(pc.coResidentBlocks(kernel))));
+  prologue(pc, stream);
+  launchAllreduceNorm(pc.comm(), a, x, dt, norm, variant, blocks, stream);
+  finish(pc, stream, op);
+}
+
+}  // namespace
+
+int allreduceResidualNorm(PeerContext& pc, const void* partial, const void* residual, void* residualOut, void* out,
+                          const void* bias, const void* gamma, const void* beta, size_t rows, size_t hidden,
+                          DataType dt, int norm, float eps, AllreduceAlgo algo, cudaStream_t stream) {
+  GLB_TRACE_RANGE("glb::cuda::allreduceResidualNorm");
+  pc.checkHealth();
+  const char* op = "allreduce_residual_norm";
+  const NormRange inputs[] = {{"partial", partial, rows}, {"residual", residual, rows}, {"bias", bias, 1},
+                              {"weight", gamma, 1}, {"norm_bias", beta, 1}};
+  const NormRange outputs[] = {{"residual_out", residualOut, rows}, {"out", norm != kNormNone ? out : nullptr, rows}};
+  checkNormCall(op, dt, norm, hidden, rows == 0, inputs, outputs);
   if (rows == 0) return kNormLocal;
   const NormPlan plan = planResidualNorm(pc, rows, hidden, dt, norm, algo);
   DeviceGuard g(pc.device);
   const auto l = layoutOf(pc);
-  const size_t rowBytes = vecBytes;
-  const void* kernel = allreduceNormKernelFor(dt, norm, plan.variant);
+  const size_t rowBytes = hidden * elementSize(dt);
   for (size_t r0 = 0; r0 < rows; r0 += plan.chunkRows) {
     const size_t n = std::min(plan.chunkRows, rows - r0);
-    NormArgs a;
-    a.partial = static_cast<const char*>(partial) + r0 * rowBytes;
-    a.residual = static_cast<const char*>(residual) + r0 * rowBytes;
-    a.residualOut = static_cast<char*>(residualOut) + r0 * rowBytes;
-    a.out = norm != kNormNone ? static_cast<char*>(out) + r0 * rowBytes : nullptr;
-    a.bias = bias;
-    a.gamma = gamma;
-    a.beta = beta;
-    a.rows = n;
-    a.hidden = hidden;
-    a.eps = eps;
+    const NormArgs a = chunkArgs(partial, residual, residualOut, out, bias, gamma, beta, r0 * rowBytes, n, hidden, norm, eps);
     NormXchg x{};
     switch (plan.variant) {
       case kNormLL:
@@ -599,13 +655,45 @@ int allreduceResidualNorm(PeerContext& pc, const void* partial, const void* resi
       default: break;
     }
     x.mine = x.peers.p[pc.rank];
-    // Every CTA waits for its twin on the peers: the grid must be co-resident.
-    const int blocks = static_cast<int>(std::min<size_t>(n, static_cast<size_t>(pc.coResidentBlocks(kernel))));
-    prologue(pc, stream);
-    launchAllreduceNorm(pc.comm(), a, x, dt, norm, plan.variant, blocks, stream);
-    finish(pc, stream, "allreduce_residual_norm");
+    launchNormChunk(pc, a, x, dt, norm, plan.variant, n, stream, op);
   }
   return plan.variant;
+}
+
+int reduceScatterResidualNorm(PeerContext& pc, const void* partial, const void* residual, void* residualOut, void* out,
+                              const void* bias, const void* gamma, const void* beta, size_t rows, size_t hidden,
+                              DataType dt, int norm, float eps, bool gatherOut, cudaStream_t stream) {
+  GLB_TRACE_RANGE("glb::cuda::reduceScatterResidualNorm");
+  pc.checkHealth();
+  const char* op = "reduce_scatter_residual_norm";
+  const size_t P = static_cast<size_t>(pc.size), shard = rows / P;
+  const NormRange inputs[] = {{"partial", partial, rows}, {"residual", residual, shard}, {"bias", bias, 1},
+                              {"weight", gamma, 1}, {"norm_bias", beta, 1}};
+  const NormRange outputs[] = {{"residual_out", residualOut, shard},
+                               {"out", norm != kNormNone ? out : nullptr, gatherOut ? rows : shard}};
+  checkNormCall(op, dt, norm, hidden, rows == 0, inputs, outputs);
+  GLB_NORM_CHECK(rows % P == 0, rows, " rows do not split into ", P, " equal shards");
+  if (P == 1) {
+    return allreduceResidualNorm(pc, partial, residual, residualOut, out, bias, gamma, beta, rows, hidden, dt, norm,
+                                 eps, AllreduceAlgo::AUTO, stream);
+  }
+  if (rows == 0) return kNormScatter;
+  const NormPlan plan = planReduceScatterNorm(pc, rows, hidden, dt, norm, gatherOut);
+  DeviceGuard g(pc.device);
+  const size_t rowBytes = hidden * elementSize(dt);
+  NormXchg x{};
+  x.peers = pc.stagePtrs(layoutOf(pc).bulkOff);
+  x.mine = x.peers.p[pc.rank];
+  x.shardRows = shard;
+  x.gather = gatherOut ? 1 : 0;
+  // Chunk rows [r0, r0 + n) of every shard: the same byte offset into the partial, the shard
+  // tensors and a gathered out, whose other shards lie shardRows further on.
+  for (size_t r0 = 0; r0 < shard; r0 += plan.chunkRows) {
+    const size_t n = std::min(plan.chunkRows, shard - r0);
+    const NormArgs a = chunkArgs(partial, residual, residualOut, out, bias, gamma, beta, r0 * rowBytes, n, hidden, norm, eps);
+    launchNormChunk(pc, a, x, dt, norm, kNormScatter, P * n, stream, op);
+  }
+  return kNormScatter;
 }
 
 #undef GLB_NORM_CHECK

@@ -132,6 +132,22 @@ struct NormPlan {
 NormPlan planResidualNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, AllreduceAlgo algo);
 const char* normVariantName(int variant);
 
+// The reduce-scatter form of allreduceResidualNorm, for sequence parallelism (docs/cuda.md,
+// "Reduce-scatter + residual + norm"). `partial` holds rows = P x Ts rows on every rank; rank r
+// owns rows [r Ts, (r + 1) Ts), and residual / residualOut are its shard of Ts rows:
+// residualOut[i] = round(sum of the partials' row r Ts + i + bias + residual[i]), with the sum
+// order, rounding and limits of allreduceResidualNorm, so the bytes equal the matching rows of
+// its outputs. out = norm(residualOut): this rank's Ts rows, or with gatherOut all P shards
+// (rows rows, shard q at row q Ts) on every rank. rows % P == 0. One rank runs the allreduce
+// form's local launch. Invalid arguments raise InputException before anything is launched.
+int reduceScatterResidualNorm(PeerContext& pc, const void* partial, const void* residual, void* residualOut, void* out,
+                              const void* bias, const void* gamma, const void* beta, size_t rows, size_t hidden,
+                              DataType dt, int norm, float eps, bool gatherOut, cudaStream_t stream);
+// Its variant (kNormScatter, or kNormLocal for one rank) and launches: it stages every shard's rows
+// (and a gathered out) in the pool's bulk region, so beyond what that holds it runs as consecutive
+// chunks of chunkRows rows of every shard.
+NormPlan planReduceScatterNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, bool gatherOut);
+
 
 // ---- data movement -------------------------------------------------------------------
 // `buf`/`out` arguments are registered or symmetric buffers; plain-pointer

@@ -60,8 +60,9 @@ const void* castKernelFor(DataType in, DataType out);
 constexpr int kMaxNormHidden = 16384;
 enum NormKind : int { kNormNone = 0, kNormRms = 1, kNormLayer = 2 };
 // The exchange of the partials: LL lines, one-shot pool halves, row-sharded two-shot through the
-// pool's bulk region, or none (one rank).
-enum NormVariant : int { kNormLL = 0, kNormOneShot = 1, kNormTwoShot = 2, kNormLocal = 3 };
+// pool's bulk region, or none (one rank). kNormScatter is the reduce-scatter form (sequence
+// parallelism): each rank keeps the rows of its own token shard, out optionally gathered.
+enum NormVariant : int { kNormLL = 0, kNormOneShot = 1, kNormTwoShot = 2, kNormLocal = 3, kNormScatter = 4 };
 // One (rows, hidden) problem: contiguous rows of hidden elements, 16-byte aligned. bias / gamma /
 // beta may be null (none, 1, 0); out is unused without a norm.
 struct NormArgs {
@@ -78,12 +79,16 @@ struct NormArgs {
 };
 // Where the partials travel. LL: peers.p[r] = rank r's LL region, mine = mine, srcStride and
 // parityStride its layout. One-shot: rank r's pool halves, parityStride = one half. Two-shot: rank
-// r's 2 x rows rows of the bulk region.
+// r's 2 x rows rows of the bulk region. Reduce-scatter: rank r's bulk region (P x rows staged rows,
+// then P x rows gathered out rows when `gather`); shardRows = rows between the shards of the
+// user's partial and gathered out (NormArgs::rows is the chunk of every shard).
 struct NormXchg {
   PeerPtrs peers;
   void* mine;
   unsigned long long srcStride;
   unsigned long long parityStride;
+  unsigned long long shardRows;
+  int gather;
 };
 bool normSupports(DataType dt);
 const void* allreduceNormKernelFor(DataType dt, int norm, int variant);

@@ -69,12 +69,30 @@ float bf16ToFloat(uint16_t h) {
 // Fused allreduce + residual + norm in loopback: rank 0's partial row i, element j is 1 + i * H + j,
 // the residual 0.5 * (i * H + j), the bias j, gamma 1 + j / H and beta -j / H, all exact in fp32.
 // Every virtual peer's partial is rank 0's (their staging aliases mine), so row i reduces to
-// P * partial + bias + residual; `rows` says which rows rank 0 computes (the two-shot: its share).
-std::string checkAllreduceNorm(const CommArgs& ca, const NormXchg& x, int variant, int norm, size_t rows, size_t H,
-                               size_t rowsBegin, size_t rowsEnd, int blocks, cudaStream_t s) {
-  const int P = ca.nranks;
-  DevBuf partial(rows * H * 4), residual(rows * H * 4), resOut(rows * H * 4), out(rows * H * 4), vec(3 * H * 4);
-  launchFill(partial.p, rows * H, DataType::FLOAT32, 1.0, 1.0, s);
+// P * partial + bias + residual. Checks row i of residual_out (r) and, with a norm, out (o).
+std::string checkNormRow(const float* r, const float* o, size_t i, int P, size_t H, int norm) {
+  std::vector<double> v(H);
+  double mean = 0, sq = 0;
+  for (size_t j = 0; j < H; j++) {
+    const double e = static_cast<double>(i * H + j);
+    v[j] = P * (1.0 + e) + 0.5 * e + static_cast<double>(j);
+    if (r[j] != static_cast<float>(v[j])) return strcat_all("residual_out[", i, ", ", j, "]: got ", r[j], " want ", v[j]);
+    mean += v[j] / H;
+  }
+  if (norm == kNormNone) return "";
+  for (size_t j = 0; j < H; j++) sq += (norm == kNormLayer ? (v[j] - mean) * (v[j] - mean) : v[j] * v[j]) / H;
+  for (size_t j = 0; j < H; j++) {
+    const double g = 1.0 + static_cast<double>(j) / H, b = -static_cast<double>(j) / H;
+    const double want = norm == kNormLayer ? (v[j] - mean) / std::sqrt(sq + 1e-5) * g + b : v[j] / std::sqrt(sq + 1e-5) * g;
+    if (std::fabs(o[j] - want) > 1e-5 * std::fabs(want) + 1e-5) return strcat_all("out[", i, ", ", j, "]: got ", o[j], " want ", want);
+  }
+  return "";
+}
+
+// The arguments of checkNormRow's problem over buffers of `rows` rows of H floats.
+NormArgs fillNormProblem(const DevBuf& partial, const DevBuf& residual, const DevBuf& resOut, const DevBuf& out,
+                         const DevBuf& vec, size_t partialRows, size_t rows, size_t H, cudaStream_t s) {
+  launchFill(partial.p, partialRows * H, DataType::FLOAT32, 1.0, 1.0, s);
   launchFill(residual.p, rows * H, DataType::FLOAT32, 0.0, 0.5, s);
   launchFill(vec.p, H, DataType::FLOAT32, 0.0, 1.0, s);
   launchFill(static_cast<float*>(vec.p) + H, H, DataType::FLOAT32, 1.0, 1.0 / H, s);
@@ -90,28 +108,40 @@ std::string checkAllreduceNorm(const CommArgs& ca, const NormXchg& x, int varian
   a.rows = rows;
   a.hidden = H;
   a.eps = 1e-5f;
+  return a;
+}
+
+// `rows` says which rows rank 0 computes (the two-shot: its share).
+std::string checkAllreduceNorm(const CommArgs& ca, const NormXchg& x, int variant, int norm, size_t rows, size_t H,
+                               size_t rowsBegin, size_t rowsEnd, int blocks, cudaStream_t s) {
+  DevBuf partial(rows * H * 4), residual(rows * H * 4), resOut(rows * H * 4), out(rows * H * 4), vec(3 * H * 4);
+  const NormArgs a = fillNormProblem(partial, residual, resOut, out, vec, rows, rows, H, s);
   launchAllreduceNorm(ca, a, x, DataType::FLOAT32, norm, variant, blocks, s);
   noteLaunch();
   auto r = download(resOut.p, rows * H, s);
   auto o = download(out.p, rows * H, s);
   for (size_t i = rowsBegin; i < rowsEnd; i++) {
-    std::vector<double> v(H);
-    double mean = 0, sq = 0;
-    for (size_t j = 0; j < H; j++) {
-      const double e = static_cast<double>(i * H + j);
-      v[j] = P * (1.0 + e) + 0.5 * e + static_cast<double>(j);
-      if (r[i * H + j] != static_cast<float>(v[j])) return strcat_all("residual_out[", i, ", ", j, "]: got ", r[i * H + j], " want ", v[j]);
-      mean += v[j] / H;
-    }
-    if (norm == kNormNone) continue;
-    for (size_t j = 0; j < H; j++) sq += (norm == kNormLayer ? (v[j] - mean) * (v[j] - mean) : v[j] * v[j]) / H;
-    for (size_t j = 0; j < H; j++) {
-      const double g = 1.0 + static_cast<double>(j) / H, b = -static_cast<double>(j) / H;
-      const double want = norm == kNormLayer ? (v[j] - mean) / std::sqrt(sq + 1e-5) * g + b : v[j] / std::sqrt(sq + 1e-5) * g;
-      if (std::fabs(o[i * H + j] - want) > 1e-5 * std::fabs(want) + 1e-5) {
-        return strcat_all("out[", i, ", ", j, "]: got ", o[i * H + j], " want ", want);
-      }
-    }
+    std::string why = checkNormRow(&r[i * H], &o[i * H], i, ca.nranks, H, norm);
+    if (!why.empty()) return why;
+  }
+  return "";
+}
+
+// The reduce-scatter form as one chunk of `rows` rows of shards of x.shardRows rows: rank 0 owns the
+// chunk's rows of shard 0, and a gathered out holds them at the same rows (the other shards come
+// from virtual peers that do not run).
+std::string checkScatterNorm(const CommArgs& ca, const NormXchg& x, int norm, size_t rows, size_t H, int blocks,
+                             cudaStream_t s) {
+  const size_t all = ca.nranks * x.shardRows, outRows = x.gather ? all : rows;
+  DevBuf partial(all * H * 4), residual(rows * H * 4), resOut(rows * H * 4), out(outRows * H * 4), vec(3 * H * 4);
+  const NormArgs a = fillNormProblem(partial, residual, resOut, out, vec, all, rows, H, s);
+  launchAllreduceNorm(ca, a, x, DataType::FLOAT32, norm, kNormScatter, blocks, s);
+  noteLaunch();
+  auto r = download(resOut.p, rows * H, s);
+  auto o = download(out.p, outRows * H, s);
+  for (size_t i = 0; i < rows; i++) {
+    std::string why = checkNormRow(&r[i * H], &o[i * H], i, ca.nranks, H, norm);
+    if (!why.empty()) return why;
   }
   return "";
 }
@@ -331,6 +361,20 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
             }
             x.mine = x.peers.p[0];
             return checkAllreduceNorm(ca, x, variant, norm, rows, H, rb, re, 3, stream);
+          });
+        }
+      }
+      // the reduce-scatter form: a chunk of 3 rows of shards of 5, out gathered or not
+      for (int gather : {0, 1}) {
+        for (int norm : {kNormNone, kNormRms, kNormLayer}) {
+          R.run(strcat_all("allreduceNormKernel<float,", norms[norm], ",reduce_scatter> P=", P, gather ? " gather" : ""),
+                [&]() -> std::string {
+            NormXchg x{};
+            for (int r = 0; r < P; r++) x.peers.p[r] = myStage + 2 * half;
+            x.mine = x.peers.p[0];
+            x.shardRows = 5;
+            x.gather = gather;
+            return checkScatterNorm(ca, x, norm, 3, H, 3, stream);
           });
         }
       }

@@ -217,6 +217,33 @@ void registerCuda(py::module_& root) {
     d["launches"] = p.launches;
     return d;
   }, py::arg("pc"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"), py::arg("algo") = 0);
+  m.def("reduce_scatter_residual_norm", [](PeerContext& pc, uintptr_t partial, uintptr_t residual,
+                                           uintptr_t residualOut, uintptr_t out, uintptr_t bias, uintptr_t gamma,
+                                           uintptr_t beta, size_t rows, size_t hidden, int dtype, int norm, double eps,
+                                           bool gatherOut, uintptr_t stream) {
+    int v;
+    {
+      py::gil_scoped_release nogil;
+      v = reduceScatterResidualNorm(pc, P(partial), P(residual), P(residualOut), P(out), P(bias), P(gamma), P(beta),
+                                    rows, hidden, static_cast<DataType>(dtype), norm, static_cast<float>(eps),
+                                    gatherOut, S(stream));
+    }
+    return std::string(normVariantName(v));
+  }, py::arg("pc"), py::arg("partial"), py::arg("residual"), py::arg("residual_out"), py::arg("out"), py::arg("bias"),
+     py::arg("gamma"), py::arg("beta"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"),
+     py::arg("eps"), py::arg("gather_out") = true, py::arg("stream") = 0,
+     "Reduce-scatter of partial sums over row shards fused with bias, residual add and a norm (0 none, 1 rms, "
+     "2 layer), out optionally allgathered; rows is the full row count; null pointers are 0. Returns the variant "
+     "that ran.");
+  m.def("plan_reduce_scatter_norm", [](PeerContext& pc, size_t rows, size_t hidden, int dtype, int norm,
+                                       bool gatherOut) {
+    const NormPlan p = planReduceScatterNorm(pc, rows, hidden, static_cast<DataType>(dtype), norm, gatherOut);
+    py::dict d;
+    d["variant"] = std::string(normVariantName(p.variant));
+    d["chunk_rows"] = p.chunkRows;
+    d["launches"] = p.launches;
+    return d;
+  }, py::arg("pc"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"), py::arg("gather_out") = true);
   m.attr("MAX_NORM_HIDDEN") = kMaxNormHidden;
 
   m.def("plan_allreduce", [](PeerContext& pc, size_t bytes, int dtype, int op, int kind) {

@@ -6,6 +6,9 @@ parallel up-projection, GELU, row-parallel down-projection -> ONE allreduce. Bac
 (one allreduce per half). CUDA tensors run the fused NVLink kernels, where each row-parallel
 allreduce also adds the bias and the residual and, after the attention, applies ln2
 (``TensorParallel.reduce_residual_norm``); CPU tensors run the TCP transport.
+With ``sequence_parallel=True`` the residual stream and both norms live on this rank's shard of the
+sequence (Megatron sequence parallelism): an allgather feeds each column-parallel half, and each
+row-parallel output is reduce-scattered back to the shard instead of allreduced.
 ``DenseBlock`` is the single-process reference with the same parameters (tests load one into the other).
 """
 from __future__ import annotations
@@ -13,7 +16,7 @@ from __future__ import annotations
 import torch
 from torch import nn
 
-from ..parallel import TensorParallel
+from ..parallel import SequenceParallel, TensorParallel
 
 
 class DenseBlock(nn.Module):
@@ -34,10 +37,16 @@ class DenseBlock(nn.Module):
 
 
 class TPBlock(nn.Module):
-    def __init__(self, tp: TensorParallel, d_model=64, n_heads=4, d_ff=256, device=None, dtype=None):
+    def __init__(self, tp: TensorParallel, d_model=64, n_heads=4, d_ff=256, device=None, dtype=None,
+                 sequence_parallel: bool = False):
+        """``sequence_parallel``: ``forward`` takes and returns this rank's shard ``[S / P, B,
+        d_model]`` of a sequence-first ``[S, B, d_model]`` input (S divisible by P); after the
+        backward, ``SequenceParallel.allreduce_sequence_parallel_grads(block.sequence_parallel_parameters())``
+        completes the gradients of the parameters applied to the shard."""
         super().__init__()
         assert n_heads % tp.size == 0 and d_ff % tp.size == 0
         self.tp, self.n_heads, self.d_model = tp, n_heads, d_model
+        self.sp = SequenceParallel(tp.ctx, tp.cc) if sequence_parallel else None
         self.local_heads = n_heads // tp.size
         self.ln1, self.ln2 = nn.LayerNorm(d_model, device=device, dtype=dtype), nn.LayerNorm(d_model, device=device, dtype=dtype)
         # q, k and v each column-parallel over heads (one fused parameter per projection kind)
@@ -61,7 +70,15 @@ class TPBlock(nn.Module):
         self.ln1.load_state_dict(dense.ln1.state_dict())
         self.ln2.load_state_dict(dense.ln2.state_dict())
 
+    def sequence_parallel_parameters(self):
+        """The replicated parameters that sequence parallelism applies to the token shard: ln1, ln2
+        and the row-parallel biases. Their gradients must be summed over the group."""
+        return [p for m in (self.ln1, self.ln2) for p in m.parameters()] + \
+            [lin.bias for lin in (self.proj, self.down) if lin.bias is not None]
+
     def forward(self, x):
+        if self.sp is not None:
+            return self._forward_sequence_parallel(x)
         B, S, E = x.shape
         hd = E // self.n_heads
         h = self.ln1(x)
@@ -75,3 +92,17 @@ class TPBlock(nn.Module):
             return self.tp.reduce_residual_norm(p, x, None, self.down.bias)
         x = x + self.proj(a)
         return x + self.down(nn.functional.gelu(self.up(self.ln2(x))))
+
+    def _forward_sequence_parallel(self, x):                      # x: [S/P, B, d_model]
+        F, sp = nn.functional, self.sp
+        # The column-parallel layers take the gathered input directly: gather_from_sequence's
+        # backward reduce-scatters its gradient, so copy_to_region's allreduce would count it P times.
+        h = sp.gather_from_sequence(self.ln1(x))                 # [S, B, E]
+        S, B, _ = h.shape
+        hd = self.d_model // self.n_heads
+        q, k, v = (F.linear(h, lin.weight, lin.bias).view(S, B, self.local_heads, hd).permute(1, 2, 0, 3)
+                   for lin in (self.q, self.k, self.v))
+        a = F.scaled_dot_product_attention(q, k, v, is_causal=True).permute(2, 0, 1, 3).reshape(S, B, -1)
+        x, h = sp.reduce_scatter_residual_norm(F.linear(a, self.proj.weight), x, self.ln2, self.proj.bias)
+        p = F.linear(F.gelu(F.linear(h, self.up.weight, self.up.bias)), self.down.weight)
+        return sp.reduce_scatter_residual_norm(p, x, None, self.down.bias, gather_out=False)

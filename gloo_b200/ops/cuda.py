@@ -254,6 +254,67 @@ class CudaContext:
                                     float(eps), _algo(algo), _stream(stream))
         return residual_out if norm is None else (residual_out, out)
 
+    def reduce_scatter_residual_norm(self, partial, residual, weight=None, norm_bias=None, *,
+                                     norm: Optional[str] = "rms", eps: float = 1e-6, bias=None, residual_out=None,
+                                     out=None, gather_out: bool = True, stream=None):
+        """The row-parallel output step of sequence parallelism in ONE kernel launch: reduce-scatter
+        of the partial sums over token shards, ``+ bias``, ``+ residual`` and the next norm, whose
+        output is optionally allgathered.
+
+        ``partial`` is ``(T, ...)`` with T = P * Ts on every rank; this rank owns rows ``[rank * Ts,
+        (rank + 1) * Ts)`` along dim 0, and ``residual`` / ``residual_out`` are that shard, shape
+        ``(Ts, ...)``. ``residual_out = round(sum over ranks of partial[shard rows] + bias +
+        residual)`` and ``out`` = the norm of it, with the sum order, rounding and limits of
+        :meth:`allreduce_residual_norm`, so the bytes equal the matching rows of its outputs.
+        ``out`` has ``partial``'s shape with ``gather_out`` (every rank gets every shard, shard q at
+        rows ``q * Ts``) and ``residual``'s shape without. ``bias``, ``weight`` and ``norm_bias`` must
+        be the same on every rank. ``residual_out`` defaults to ``residual`` (in place); ``out`` is
+        allocated when not given. Invalid arguments raise ``ValueError`` before anything is launched.
+
+        Returns ``(residual_out, out)``, or ``residual_out`` when ``norm`` is None."""
+        import torch
+
+        kinds = {None: 0, "rms": 1, "layer": 2}
+        name = "reduce_scatter_residual_norm"
+        if norm not in kinds:
+            raise ValueError(f"{name}: norm must be 'rms', 'layer' or None, got {norm!r}")
+        if norm != "layer" and norm_bias is not None:
+            raise ValueError(f"{name}: norm_bias needs norm='layer'")
+        if norm is None and weight is not None:
+            raise ValueError(f"{name}: weight needs a norm")
+        if partial.dim() < 2:
+            raise ValueError(f"{name}: partial must have a token and a hidden dimension")
+        T, H = partial.shape[0], partial.shape[-1]
+        if T % self.size:
+            raise ValueError(f"{name}: {T} rows do not split into {self.size} equal shards")
+        shard = (T // self.size, *partial.shape[1:])
+        if residual_out is None:
+            residual_out = residual
+        if norm is not None and out is None:
+            out = torch.empty(tuple(partial.shape) if gather_out else shard, dtype=partial.dtype, device=partial.device)
+        named = {"partial": partial, "residual": residual, "residual_out": residual_out, "out": out, "bias": bias,
+                 "weight": weight, "norm_bias": norm_bias}
+        for key, t in named.items():
+            if t is None:
+                continue
+            if not t.is_cuda or t.dtype != partial.dtype or not t.is_contiguous():
+                raise ValueError(f"{name}: {key} must be a contiguous CUDA tensor of {partial.dtype}, "
+                                 f"got {t.dtype} on {t.device}{'' if t.is_contiguous() else ', not contiguous'}")
+            if key in ("bias", "weight", "norm_bias"):
+                want = (H,)
+            elif key == "partial" or (key == "out" and gather_out):
+                want = tuple(partial.shape)
+            else:
+                want = shard
+            if tuple(t.shape) != want:
+                raise ValueError(f"{name}: {key} has shape {tuple(t.shape)}, expected {want}")
+        _, _, dt, _ = describe(partial)
+        ptr = lambda t: 0 if t is None else t.data_ptr()  # noqa: E731
+        _cu.reduce_scatter_residual_norm(self.pc, ptr(partial), ptr(residual), ptr(residual_out), ptr(out), ptr(bias),
+                                         ptr(weight), ptr(norm_bias), partial.numel() // max(H, 1), H, int(dt),
+                                         kinds[norm], float(eps), bool(gather_out), _stream(stream))
+        return residual_out if norm is None else (residual_out, out)
+
     # ---- health ---------------------------------------------------------------------------
     def set_timeout(self, ms: int):
         """Device-side waits give up after ``ms`` milliseconds (then the context is poisoned)."""

@@ -25,6 +25,50 @@ def _norm_parts(module, dtype):
     return "unsupported", None, None, 0.0
 
 
+def _norm_fusable(cc, partial, residual, residual_shape, norm_module, kind, vectors) -> bool:
+    """Whether a fused residual-norm kernel can run on these tensors: a CUDA context, a
+    supported norm and dtype, a hidden size within the kernel's limits, ``residual`` of
+    ``residual_shape``, and aligned tensors of one dtype."""
+    import torch
+
+    if cc is None or not _is_cuda(partial) or kind == "unsupported" or partial.dim() == 0:
+        return False
+    H = partial.shape[-1]
+    if partial.dtype not in (torch.float32, torch.bfloat16, torch.float16) or tuple(residual.shape) != residual_shape:
+        return False
+    if H * partial.element_size() % 16 or H > _C.cuda.MAX_NORM_HIDDEN:
+        return False
+    if norm_module is not None and tuple(norm_module.normalized_shape) != (H,):
+        return False
+    for t in (partial, residual):
+        # a non-contiguous tensor is copied, and the copy is aligned
+        if t.dtype != partial.dtype or (t.is_contiguous() and t.data_ptr() % 16):
+            return False
+    for t in vectors:
+        if t is not None and (not t.is_cuda or t.dtype != partial.dtype or not t.is_contiguous() or
+                              t.data_ptr() % 16 or tuple(t.shape) != (H,)):
+            return False
+    return True
+
+
+def _norm_input_grad(kind, H, eps, s, w, nb, grad_out):
+    """The norm's gradients, recomputed with torch from its saved input ``s``: ``(grad_s,
+    grad_weight, grad_norm_bias)``, None for an absent weight or bias."""
+    import torch
+
+    F = torch.nn.functional
+    with torch.enable_grad():
+        x = s.detach().requires_grad_(True)
+        ws = [t.detach().requires_grad_(True) if t is not None else None for t in (w, nb)]
+        y = F.rms_norm(x, (H,), ws[0], eps) if kind == "rms" else F.layer_norm(x, (H,), ws[0], ws[1], eps)
+        need = [x] + [t for t in ws if t is not None]
+        got = list(torch.autograd.grad(y, need, grad_out))
+    gs = got.pop(0)
+    gw = got.pop(0) if w is not None else None
+    gnb = got.pop(0) if nb is not None else None
+    return gs, gw, gnb
+
+
 class _Base:
     def __init__(self, ctx, cuda_ctx=None):
         """ctx: host context (control plane, CPU tensors); cuda_ctx: ops.cuda.CudaContext."""
@@ -418,7 +462,6 @@ class TensorParallel(_Base):
         ``+ residual`` and the module."""
         import torch
 
-        F = torch.nn.functional
         kind, weight, norm_bias, eps = _norm_parts(norm_module, partial.dtype)
         if not self._fusable(partial, residual, norm_module, kind, (bias, weight, norm_bias)):
             y = self.reduce_from_region(partial)
@@ -428,11 +471,6 @@ class TensorParallel(_Base):
             return s if norm_module is None else (s, norm_module(s))
         H = partial.shape[-1]
         tp = self
-
-        def recompute(x, w, b):
-            if kind == "rms":
-                return F.rms_norm(x, (H,), w, eps)
-            return F.layer_norm(x, (H,), w, b, eps)
 
         class _R(torch.autograd.Function):
             @staticmethod
@@ -450,15 +488,8 @@ class TensorParallel(_Base):
                 grad_s = torch.zeros_like(s) if grad_s is None else grad_s
                 gw = gnb = None
                 if kind is not None and grad_out is not None:
-                    with torch.enable_grad():
-                        x = s.detach().requires_grad_(True)
-                        ws = [t.detach().requires_grad_(True) if t is not None else None for t in (w, nb)]
-                        y = recompute(x, *ws)
-                        need = [x] + [t for t in ws if t is not None]
-                        got = list(torch.autograd.grad(y, need, grad_out))
-                    grad_s = grad_s + got.pop(0)
-                    gw = got.pop(0) if w is not None else None
-                    gnb = got.pop(0) if nb is not None else None
+                    gs, gw, gnb = _norm_input_grad(kind, H, eps, s, w, nb, grad_out)
+                    grad_s = grad_s + gs
                 gb = grad_s.reshape(-1, H).sum(0) if ctx.has_bias else None
                 return grad_s, grad_s, gb, gw, gnb
 
@@ -466,26 +497,7 @@ class TensorParallel(_Base):
 
     def _fusable(self, partial, residual, norm_module, kind, vectors) -> bool:
         """Whether reduce_residual_norm can run the fused kernel on these tensors."""
-        import torch
-
-        if self.cc is None or not _is_cuda(partial) or kind == "unsupported" or partial.dim() == 0:
-            return False
-        H = partial.shape[-1]
-        if partial.dtype not in (torch.float32, torch.bfloat16, torch.float16) or residual.shape != partial.shape:
-            return False
-        if H * partial.element_size() % 16 or H > _C.cuda.MAX_NORM_HIDDEN:
-            return False
-        if norm_module is not None and tuple(norm_module.normalized_shape) != (H,):
-            return False
-        for t in (partial, residual):
-            # a non-contiguous tensor is copied, and the copy is aligned
-            if t.dtype != partial.dtype or (t.is_contiguous() and t.data_ptr() % 16):
-                return False
-        for t in vectors:
-            if t is not None and (not t.is_cuda or t.dtype != partial.dtype or not t.is_contiguous() or
-                                  t.data_ptr() % 16 or tuple(t.shape) != (H,)):
-                return False
-        return True
+        return _norm_fusable(self.cc, partial, residual, tuple(partial.shape), norm_module, kind, vectors)
 
     def column_linear(self, in_features: int, out_features: int, bias: bool = True, device=None, dtype=None):
         return ColumnParallelLinear(self, in_features, out_features, bias, device, dtype)
@@ -550,13 +562,167 @@ except ImportError:  # pragma: no cover
 
 class SequenceParallel(_Base):
     """Megatron sequence parallelism: reduce_scatter along the sequence going in,
-    allgather coming out."""
+    allgather coming out.
+
+    The autograd operators shard along dim 0 (the sequence, in Megatron's sequence-first layout
+    ``[S, B, E]``); rank r holds rows ``[r * S / P, (r + 1) * S / P)``. ``gather_from_sequence``
+    feeds a column-parallel layer from the shard, ``reduce_scatter_to_sequence`` brings a
+    row-parallel output back to it, and ``reduce_scatter_residual_norm`` fuses the latter with bias,
+    residual add and the next norm. Replicated parameters applied to the shard (norm weights and
+    biases, row-parallel biases) get gradients from this rank's tokens only:
+    ``allreduce_sequence_parallel_grads`` sums them after the backward."""
 
     def scatter_reduce(self, full, shard):
         return ZeroShard(self.ctx, self.cc).reduce_scatter_gradients(full, shard, average=False)
 
     def gather(self, shard, full):
         return ZeroShard(self.ctx, self.cc).allgather_parameters(full, shard)
+
+    # ---- autograd-aware operators --------------------------------------------------------------
+    def _allgather_rows(self, shard):
+        import torch
+
+        shard = shard.contiguous()
+        full = torch.empty((self.size * shard.shape[0], *shard.shape[1:]), dtype=shard.dtype, device=shard.device)
+        if _is_cuda(shard):
+            self.cc.allgather(full, shard)
+        else:
+            H.allgather(self.ctx, full, shard)
+        return full
+
+    def _reduce_scatter_rows(self, full):
+        import torch
+
+        if full.shape[0] % self.size:
+            raise ValueError(f"{full.shape[0]} rows do not split into {self.size} equal shards")
+        full = full.contiguous()
+        out = torch.empty((full.shape[0] // self.size, *full.shape[1:]), dtype=full.dtype, device=full.device)
+        if _is_cuda(full):
+            self.cc.reduce_scatter(out, full)
+        else:
+            H.reduce_scatter(self.ctx, out, full, [out.numel()] * self.size)
+        return out
+
+    def gather_from_sequence(self, x_shard):
+        """Allgather of the shards along dim 0 in the forward pass, reduce-scatter of the gradient
+        in the backward pass."""
+        import torch
+
+        sp = self
+
+        class _Gather(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, inp):
+                return sp._allgather_rows(inp)
+
+            @staticmethod
+            def backward(ctx, grad):
+                return sp._reduce_scatter_rows(grad)
+
+        return _Gather.apply(x_shard)
+
+    def reduce_scatter_to_sequence(self, x):
+        """Reduce-scatter along dim 0 in the forward pass, allgather of the gradient in the
+        backward pass."""
+        import torch
+
+        sp = self
+
+        class _Scatter(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, inp):
+                return sp._reduce_scatter_rows(inp)
+
+            @staticmethod
+            def backward(ctx, grad):
+                return sp._allgather_rows(grad)
+
+        return _Scatter.apply(x)
+
+    def reduce_scatter_residual_norm(self, partial, residual_shard, norm_module=None, bias=None,
+                                     gather_out: bool = True):
+        """``reduce_scatter_to_sequence`` fused with what follows a row-parallel matmul: ``s =
+        reduce_scatter(partial) + bias + residual_shard`` on this rank's shard and the next norm,
+        whose output is allgathered when ``gather_out``. Returns ``(s, out)``, or ``s`` when
+        ``norm_module`` (an ``nn.LayerNorm``, an ``nn.RMSNorm`` or None) is None.
+
+        CUDA tensors within the fused operation's limits run it as one kernel
+        (``CudaContext.reduce_scatter_residual_norm``), into a fresh ``s``. Its backward
+        reduce-scatters the gradient of a gathered ``out``, adds the norm's input gradient
+        (recomputed with torch from the saved ``s``) to the gradient of ``s``, and allgathers that
+        sum into the gradient of ``partial``; ``residual_shard`` gets the sum, ``bias`` its row sum
+        and the norm's weights theirs from the recompute, all from this rank's tokens. Anything else
+        runs ``reduce_scatter_to_sequence``, ``+ bias``, ``+ residual_shard``, the module and
+        ``gather_from_sequence``."""
+        import torch
+
+        kind, weight, norm_bias, eps = _norm_parts(norm_module, partial.dtype)
+        fused = (partial.dim() > 0 and partial.shape[0] % self.size == 0 and
+                 _norm_fusable(self.cc, partial, residual_shard, (partial.shape[0] // self.size, *partial.shape[1:]),
+                               norm_module, kind, (bias, weight, norm_bias)))
+        if fused:
+            from ..types import _torch_map
+
+            try:  # a row too wide for the staging pool is outside the limits too
+                _C.cuda.plan_reduce_scatter_norm(self.cc.pc, partial.numel() // partial.shape[-1], partial.shape[-1],
+                                                 int(_torch_map()[partial.dtype]), {None: 0, "rms": 1, "layer": 2}[kind],
+                                                 gather_out)
+            except ValueError:
+                fused = False
+        if not fused:
+            y = self.reduce_scatter_to_sequence(partial)
+            if bias is not None:
+                y = y + bias
+            s = y + residual_shard
+            if norm_module is None:
+                return s
+            out = norm_module(s)
+            return s, (self.gather_from_sequence(out) if gather_out else out)
+        H = partial.shape[-1]
+        sp = self
+
+        class _RS(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, p, res, b, w, nb):
+                s = torch.empty_like(res, memory_format=torch.contiguous_format)
+                got = sp.cc.reduce_scatter_residual_norm(p.contiguous(), res.contiguous(), w, nb, norm=kind, eps=eps,
+                                                         bias=b, residual_out=s, gather_out=gather_out)
+                ctx.save_for_backward(s, w, nb)
+                ctx.has_bias = b is not None
+                return got
+
+            @staticmethod
+            def backward(ctx, grad_s, grad_out=None):
+                s, w, nb = ctx.saved_tensors
+                grad_s = torch.zeros_like(s) if grad_s is None else grad_s
+                gw = gnb = None
+                if kind is not None and grad_out is not None:
+                    if gather_out:
+                        grad_out = sp._reduce_scatter_rows(grad_out)
+                    gs, gw, gnb = _norm_input_grad(kind, H, eps, s, w, nb, grad_out)
+                    grad_s = grad_s + gs
+                gb = grad_s.reshape(-1, H).sum(0) if ctx.has_bias else None
+                return sp._allgather_rows(grad_s), grad_s, gb, gw, gnb
+
+        return _RS.apply(partial, residual_shard, bias, weight, norm_bias)
+
+    def allreduce_sequence_parallel_grads(self, params: Iterable):
+        """Sum over the group, in place, the gradients of replicated parameters that each rank
+        applied to its token shard only (norm weights and biases, row-parallel biases): one
+        allreduce per dtype and device. Call after the backward, before the optimizer step."""
+        import torch
+
+        groups = {}
+        for p in params:
+            if getattr(p, "grad", None) is not None:
+                groups.setdefault((p.grad.dtype, p.grad.device), []).append(p.grad)
+        for grads in groups.values():
+            flat = torch.cat([g.reshape(-1) for g in grads])
+            self._allreduce(flat)
+            off = 0
+            for g in grads:
+                g.copy_(flat[off:off + g.numel()].view_as(g))
+                off += g.numel()
 
 
 class MoEDispatcher(_Base):

@@ -1,0 +1,128 @@
+#!/usr/bin/env python
+"""The fused sequence-parallel step (reduce-scatter + bias + residual add + RMSNorm / LayerNorm +
+allgather of the normed rows, one kernel: `CudaContext.reduce_scatter_residual_norm`) against the
+unfused sequence on the same inputs: `cc.reduce_scatter`, bias add, residual add, `F.rms_norm` /
+`F.layer_norm`, `cc.allgather`.
+
+Before timing, every shape checks that the fused call's shard and gathered out equal, byte for
+byte, the matching rows of `allreduce_residual_norm` on the same inputs (the same sum order), and
+records how far the unfused sequence, which rounds after each step, lands from it.
+
+Run one rank per GPU under torch.distributed.run:
+
+    python -m torch.distributed.run --nproc_per_node 8 scripts/bench_sequence_parallel_norm.py --out sp.json
+
+or, for a rehearsal on one GPU, `--threads P` (P ranks as threads sharing cuda:0). Ranks that share
+a card pay for each other's kernels and exchange through local memory, so those numbers measure
+the per-call overhead only, not the link; the JSON says so. Timing as in bench_allreduce_norm.py:
+CUDA events around `--iters` back-to-back calls after `--warmup`, median over `--reps` windows,
+the maximum over ranks. T is the whole sequence (tokens of every rank).
+"""
+import argparse
+import json
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+
+import torch  # noqa: E402
+import torch.nn.functional as F  # noqa: E402
+
+import gloo_b200 as gb  # noqa: E402
+from bench_allreduce_norm import gpu_info, launches_fused, timed  # noqa: E402
+from gloo_b200.ops import cuda as gcu  # noqa: E402
+
+DECODE_T = (8, 64, 256)
+PREFILL_T = (4096,)
+HIDDEN = (4096, 8192)
+
+
+def bench_rank(ctx, device, args, world):
+    cc = gcu.CudaContext(ctx, device, stage_bytes=args.stage_mb << 20)
+    cc.set_timeout(600000)
+    stream = torch.cuda.current_stream()
+    dtype, P, rank = torch.bfloat16, ctx.size, ctx.rank
+    rows = []
+    for H in HIDDEN:
+        for T in DECODE_T + PREFILL_T:
+            Ts = T // P
+            shard = slice(rank * Ts, (rank + 1) * Ts)
+            g = torch.Generator(device="cpu").manual_seed(T * 131 + H)
+            residual_full = torch.randn(T, H, generator=g).to(dtype).cuda()
+            bias = torch.randn(H, generator=g).to(dtype).cuda()
+            weight = (1 + 0.1 * torch.randn(H, generator=g)).to(dtype).cuda()
+            norm_bias = (0.1 * torch.randn(H, generator=g)).to(dtype).cuda()
+            partial = torch.randn(T, H, generator=torch.Generator().manual_seed(T * 131 + H + 7 + rank)).to(dtype).cuda()
+            residual = residual_full[shard].contiguous()
+            res_out, out = torch.empty_like(residual), torch.empty(T, H, dtype=dtype, device="cuda")
+            for norm in ("rms", "layer"):
+                nb = norm_bias if norm == "layer" else None
+
+                def fused():
+                    cc.reduce_scatter_residual_norm(partial, residual, weight, nb, norm=norm, eps=1e-6, bias=bias,
+                                                    residual_out=res_out, out=out)
+
+                def unfused():
+                    y = torch.empty_like(residual)
+                    cc.reduce_scatter(y, partial)
+                    s = residual + (y + bias)
+                    o = F.rms_norm(s, (H,), weight, 1e-6) if norm == "rms" else F.layer_norm(s, (H,), weight, nb, 1e-6)
+                    full = torch.empty(T, H, dtype=dtype, device="cuda")
+                    cc.allgather(full, o)
+                    return full
+
+                s_ar, o_ar = cc.allreduce_residual_norm(partial, residual_full, weight, nb, norm=norm, eps=1e-6,
+                                                        bias=bias, residual_out=torch.empty_like(residual_full))
+                fused()
+                o_ref = unfused()
+                torch.cuda.synchronize()
+                assert torch.equal(res_out, s_ar[shard]) and torch.equal(out, o_ar), f"T={T} H={H} {norm}: not identical"
+                plan = gb._C.cuda.plan_reduce_scatter_norm(cc.pc, T, H, int(gb.DataType.BFLOAT16),
+                                                           {"rms": 1, "layer": 2}[norm], True)
+                row = {"T": T, "H": H, "dtype": "bfloat16", "norm": norm, "shard_bytes": Ts * H * 2,
+                       "variant": plan["variant"], "launches": plan["launches"],
+                       "max_abs_diff_unfused": float((out.float() - o_ref.float()).abs().max())}
+                for name, fn in (("fused", fused), ("unfused", unfused)):
+                    row[f"{name}_us"] = timed(ctx, cc, fn, stream, args, world)
+                row["fused_launches_per_call"] = launches_fused(cc, fused)
+                row["speedup"] = row["unfused_us"] / row["fused_us"]
+                rows.append(row)
+    return rows
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", default="")
+    ap.add_argument("--threads", type=int, default=0, help="rehearsal: this many ranks as threads on cuda:0")
+    ap.add_argument("--iters", type=int, default=200)
+    ap.add_argument("--warmup", type=int, default=50)
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--stage-mb", type=int, default=128)
+    args = ap.parse_args()
+    if args.threads:
+        world = args.threads
+        rows = gb.spawn_threads(world, lambda ctx: bench_rank(ctx, 0, args, 1), cuda_device=0, timeout_ms=600000)[0]
+        mode = f"{world} ranks as threads on one GPU: overhead only, not link numbers"
+        info, rank = gpu_info(0), 0
+    else:
+        rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
+        local = int(os.environ.get("LOCAL_RANK", 0))
+        torch.cuda.set_device(local)
+        ctx = gb.init_context(rank, world, path=f"/tmp/glb_sp_{os.environ.get('MASTER_PORT', '0')}_{os.getppid()}",
+                              timeout_ms=120000)
+        rows = bench_rank(ctx, local, args, world)
+        mode = f"{world} ranks, one per GPU"
+        info = gpu_info(local)
+    if rank == 0:
+        doc = {"benchmark": "reduce_scatter_residual_norm", "mode": mode, "ranks": world, **info, "iters": args.iters,
+               "warmup": args.warmup, "reps": args.reps, "rows": rows}
+        text = json.dumps(doc)
+        print(text)
+        if args.out:
+            with open(args.out, "w") as f:
+                f.write(text + "\n")
+
+
+if __name__ == "__main__":
+    main()

@@ -53,6 +53,8 @@ KERNELS = [
     ("ll_combine_topk_bf16", r"moeLLCombineKernel<__nv_bfloat16>"),
     ("ll_combine_topk_f16", r"moeLLCombineKernel<__half>"),
     ("ll_combine_topk_f32", r"moeLLCombineKernel<float>"),
+    ("reduce_scatter_norm_bf16_rms", r"allreduceNormKernel<__nv_bfloat16, 1, 4>"),
+    ("reduce_scatter_norm_f32_layer", r"allreduceNormKernel<float, 2, 4>"),
     ("p2p_sendrecv", r"p2pKernel"),
     ("exchange_zero_copy", r"exchangeKernel<false>"),
     ("exchange_zero_copy_tma", r"exchangeKernel<true>"),
