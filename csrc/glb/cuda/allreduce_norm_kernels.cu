@@ -63,6 +63,49 @@ __device__ __forceinline__ const char* rowPtr(const void* base, size_t row, size
   return static_cast<const char*>(base) + row * rowBytes;
 }
 
+// The norm's statistics of a row whose rounded values are x (pack k of this thread at x[k]), in
+// one fixed order: the forward epilogue and the backward both compute them so, and the backward
+// sees the forward's statistics bit for bit. statAdd folds one pack (the packs in k order) into
+// this thread's sum; rowStats finishes from it: mean (0 for rms) and rinv = 1 / sqrt(var + eps)
+// (layer) or 1 / sqrt(mean(x^2) + eps) (rms).
+template <typename T, int NORM>
+__device__ __forceinline__ void statAdd(float& sum, const typename NormRow<T>::Acc& x) {
+#pragma unroll
+  for (int e = 0; e < NormRow<T>::kE; e++) {
+    if constexpr (NORM == kNormLayer) {
+      sum += x.v[e];
+    } else if constexpr (NORM == kNormRms) {
+      sum = fmaf(x.v[e], x.v[e], sum);
+    }
+  }
+}
+
+template <typename T, int NORM>
+__device__ __forceinline__ void rowStats(const typename NormRow<T>::Acc (&x)[NormRow<T>::kPacks], float sum, int npacks,
+                                         float eps, float* sh, float& mean, float& rinv) {
+  using R = NormRow<T>;
+  const int t = threadIdx.x;
+  const float hidden = static_cast<float>(npacks * R::kE);
+  mean = 0.0f;
+  if constexpr (NORM == kNormLayer) {
+    mean = blockSum(sum, sh) / hidden;
+    float sq = 0.0f;
+#pragma unroll
+    for (int k = 0; k < R::kPacks; k++) {
+      if (t + k * kThreads < npacks) {
+#pragma unroll
+        for (int e = 0; e < R::kE; e++) {
+          const float d = x[k].v[e] - mean;
+          sq = fmaf(d, d, sq);
+        }
+      }
+    }
+    rinv = 1.0f / sqrtf(blockSum(sq, sh) / hidden + eps);
+  } else {
+    rinv = 1.0f / sqrtf(blockSum(sum, sh) / hidden + eps);
+  }
+}
+
 // The row epilogue on the reduced partials `acc` of row `row`: adds bias and residual, rounds
 // once, and hands each pack of residualOut and out to store(k, resid, out). `npacks` packs per
 // row; pack k of this thread is t + k * kThreads.
@@ -83,35 +126,12 @@ __device__ __forceinline__ void rowEpilogue(typename NormRow<T>::Acc (&acc)[Norm
       const Pack16 r = PT::narrow(acc[k]);
       if constexpr (NORM == kNormNone) store(pk, r, r);
       acc[k] = PT::widen(r);  // the rounded value: what the next layer sees
-      if constexpr (NORM == kNormLayer) {
-#pragma unroll
-        for (int e = 0; e < R::kE; e++) sum += acc[k].v[e];
-      } else if constexpr (NORM == kNormRms) {
-#pragma unroll
-        for (int e = 0; e < R::kE; e++) sum = fmaf(acc[k].v[e], acc[k].v[e], sum);
-      }
+      statAdd<T, NORM>(sum, acc[k]);
     }
   }
   if constexpr (NORM != kNormNone) {
-    const float hidden = static_cast<float>(npacks * R::kE);
-    float mean = 0.0f, rinv;
-    if constexpr (NORM == kNormLayer) {
-      mean = blockSum(sum, sh) / hidden;
-      float sq = 0.0f;
-#pragma unroll
-      for (int k = 0; k < R::kPacks; k++) {
-        if (t + k * kThreads < npacks) {
-#pragma unroll
-          for (int e = 0; e < R::kE; e++) {
-            const float d = acc[k].v[e] - mean;
-            sq = fmaf(d, d, sq);
-          }
-        }
-      }
-      rinv = 1.0f / sqrtf(blockSum(sq, sh) / hidden + n.eps);
-    } else {
-      rinv = 1.0f / sqrtf(blockSum(sum, sh) / hidden + n.eps);
-    }
+    float mean, rinv;
+    rowStats<T, NORM>(acc, sum, npacks, n.eps, sh, mean, rinv);
 #pragma unroll
     for (int k = 0; k < R::kPacks; k++) {
       const int pk = t + k * kThreads;
@@ -326,6 +346,272 @@ allreduceNormKernel(CommArgs a, NormArgs n, NormXchg x) {
   }
 }
 
+// ---- backward of the reduce-scatter form -----------------------------------------------------
+// Per row, in fp32, with g the row's gradient of out and s the saved residual_out row:
+//   mean, rinv from s (rowStats: the forward's statistics bit for bit), xh = (s - mean) rinv,
+//   gg = g gamma, dx = rinv (gg - mean(gg) - xh mean(gg xh))   (rms: no mean(gg) term),
+//   gradResidual = round(gradS + dx);  column sums: g xh (weight), g (norm bias), the rounded
+//   gradResidual (bias).
+
+// The CTA's column sums in dynamic shared memory, one fixed region of kMaxNormHidden floats per
+// kind (0 weight, 1 norm bias, 2 bias): slot (k, e) of thread t at ((kind * kPacks + k) * kE + e)
+// * kThreads + t. Thread t holds the same packs of every row, so only it touches its slots: no
+// synchronisation, no bank conflicts, and every address is a constant offset. At this kernel's
+// registers a CTA fills an SM's register file, so the fixed size costs no occupancy.
+template <typename T>
+__device__ __forceinline__ float& colSum(float* sums, int kind, int k, int e) {
+  using R = NormRow<T>;
+  return sums[((kind * R::kPacks + k) * R::kE + e) * kThreads + threadIdx.x];
+}
+
+// gridDim.x read again where used (a volatile read of %nctaid.x) rather than held across the row
+// loop, where it would spill at the widest rows (fp32 LayerNorm).
+__device__ __forceinline__ unsigned gridCtas() {
+  unsigned n;
+  asm volatile("mov.u32 %0, %%nctaid.x;" : "=r"(n));
+  return n;
+}
+
+// Moves this thread's column sums between shared memory and the CTA's vectors in ws: in before
+// the rows (zero in the first chunk), out after them.
+template <typename T>
+__device__ __forceinline__ void moveSums(const NormBwdArgs& n, float* sums, int npacks, bool in) {
+  using R = NormRow<T>;
+  // The base through a volatile move: the two calls (before and after the row loop) each compute
+  // the address rather than share one held across the loop, where it would spill.
+  float* ws = n.ws;
+  asm volatile("mov.b64 %0, %0;" : "+l"(ws));
+  ws += static_cast<size_t>(blockIdx.x) * n.vectors * n.hidden;
+  const int vec[3] = {n.vecWeight, n.vecNormBias, n.vecBias};
+#pragma unroll
+  for (int kind = 0; kind < 3; kind++) {
+    if (vec[kind] < 0) continue;
+#pragma unroll
+    for (int k = 0; k < R::kPacks; k++) {
+      const int pk = threadIdx.x + k * kThreads;
+      if (pk >= npacks) continue;
+#pragma unroll
+      for (int e = 0; e < R::kE; e += 4) {
+        float4* p = reinterpret_cast<float4*>(ws + vec[kind] * n.hidden + pk * R::kE + e);
+        if (in) {
+          const float4 v = n.first ? make_float4(0.0f, 0.0f, 0.0f, 0.0f) : *p;
+          colSum<T>(sums, kind, k, e) = v.x;
+          colSum<T>(sums, kind, k, e + 1) = v.y;
+          colSum<T>(sums, kind, k, e + 2) = v.z;
+          colSum<T>(sums, kind, k, e + 3) = v.w;
+        } else {
+          *p = make_float4(colSum<T>(sums, kind, k, e), colSum<T>(sums, kind, k, e + 1), colSum<T>(sums, kind, k, e + 2),
+                           colSum<T>(sums, kind, k, e + 3));
+        }
+      }
+    }
+  }
+}
+
+// The address p, opaque to the optimiser: per-pack pointers of a row then stay immediate offsets
+// of one base instead of becoming loop-carried 64-bit pointers, one per pack, which spill at the
+// widest rows.
+template <typename P>
+__device__ __forceinline__ P* opaque(P* p) {
+  asm("mov.b64 %0, %0;" : "+l"(p));
+  return p;
+}
+
+// Row i of the shard: loadG(g) puts the row's fp32 gradient of out in g (pack k of this thread
+// at g[k]) once the statistics are known. Hands each pack of gradResidual to store(pk, pack) and
+// adds this thread's columns to the CTA's sums. Only g stays in registers across the block
+// reductions; the s row is read again where xh is needed (from L1 / L2), which keeps the widest
+// rows free of spills.
+template <typename T, int NORM, typename LoadG, typename Store>
+__device__ __forceinline__ void rowBackward(const NormBwdArgs& n, size_t i, int npacks, float* sh,
+                                            float* sums, LoadG&& loadG, Store&& store) {
+  using R = NormRow<T>;
+  using PT = typename R::PT;
+  const int t = threadIdx.x;
+  const size_t rb = static_cast<size_t>(npacks) * 16;
+  const char* s = opaque(rowPtr(n.s, i, rb));
+  const char* gs = n.gradS != nullptr ? opaque(rowPtr(n.gradS, i, rb)) : nullptr;
+  const char* gamma = n.gamma != nullptr ? opaque(static_cast<const char*>(n.gamma)) : nullptr;
+  float mean, rinv;
+  {
+    typename R::Acc x[R::kPacks];
+    float sum = 0.0f;
+#pragma unroll
+    for (int k = 0; k < R::kPacks; k++) {
+      const int pk = t + k * kThreads;
+      if (pk < npacks) {
+        x[k] = PT::widen(ld128(s + pk * 16));
+        statAdd<T, NORM>(sum, x[k]);
+      }
+    }
+    rowStats<T, NORM>(x, sum, npacks, n.eps, sh, mean, rinv);
+  }
+  typename R::Acc g[R::kPacks];
+  loadG(g);
+  float sgg = 0.0f, sggx = 0.0f;
+#pragma unroll
+  for (int k = 0; k < R::kPacks; k++) {
+    const int pk = t + k * kThreads;
+    if (pk < npacks) {
+      const typename R::Acc x = PT::widen(ld128(s + pk * 16));
+      typename R::Acc w;
+      if (gamma != nullptr) w = PT::widen(ld128(gamma + pk * 16));
+#pragma unroll
+      for (int e = 0; e < R::kE; e++) {
+        const float xh = (x.v[e] - mean) * rinv;
+        if (n.vecWeight >= 0) colSum<T>(sums, 0, k, e) += g[k].v[e] * xh;
+        if (n.vecNormBias >= 0) colSum<T>(sums, 1, k, e) += g[k].v[e];
+        if (gamma != nullptr) g[k].v[e] *= w.v[e];
+        sgg += g[k].v[e];
+        sggx = fmaf(g[k].v[e], xh, sggx);
+      }
+    }
+  }
+  const float hidden = static_cast<float>(npacks * R::kE);
+  const float mggx = blockSum(sggx, sh) / hidden;
+  float mgg = 0.0f;
+  if constexpr (NORM == kNormLayer) mgg = blockSum(sgg, sh) / hidden;
+#pragma unroll
+  for (int k = 0; k < R::kPacks; k++) {
+    const int pk = t + k * kThreads;
+    if (pk < npacks) {
+      const typename R::Acc x = PT::widen(ld128(s + pk * 16));
+      typename R::Acc r;
+      if (gs != nullptr) {
+        r = PT::widen(ld128(gs + pk * 16));
+      } else {
+#pragma unroll
+        for (int e = 0; e < R::kE; e++) r.v[e] = 0.0f;
+      }
+#pragma unroll
+      for (int e = 0; e < R::kE; e++) {
+        const float xh = (x.v[e] - mean) * rinv;
+        const float dx = NORM == kNormLayer ? rinv * (g[k].v[e] - mgg - xh * mggx) : rinv * (g[k].v[e] - xh * mggx);
+        r.v[e] += dx;
+      }
+      const Pack16 o = PT::narrow(r);
+      if (n.vecBias >= 0) {
+        const typename R::Acc ro = PT::widen(o);
+#pragma unroll
+        for (int e = 0; e < R::kE; e++) colSum<T>(sums, 2, k, e) += ro.v[e];
+      }
+      store(pk, o);
+    }
+  }
+}
+
+// The backward, V = kNormScatter (P ranks) or kNormLocal (one rank). Scatter: with a gathered out,
+// stage every shard's chunk of gradOut in the bulk region (pool rows [0, P rows), in the forward's
+// order); barrier; the owner of each row reduces its P staged rows (in rank order, fp32, not
+// rounded), runs rowBackward and stores gradResidual into every peer's pool (rows [P rows,
+// 2 P rows), or [0, P rows) without a gather); barrier; every rank copies all P shards out to
+// gradPartial. Row j of the pool belongs to CTA j % gridDim.x in every phase, so each barrier
+// pairs the CTAs that touch the same rows. Without a gather nothing is staged, and the first
+// barrier only keeps the owners' stores out of a peer's pool until that peer has finished the
+// launch before, which may still be reading it.
+template <typename T, int NORM, int V>
+__global__ void __launch_bounds__(kThreads, 1)
+normBackwardKernel(CommArgs a, NormBwdArgs n, NormXchg x) {
+  using R = NormRow<T>;
+  extern __shared__ float colSums[];
+  __shared__ float sh[kThreads / 32];
+  __shared__ char* peers[kMaxRanks];
+  if (threadIdx.x < kMaxRanks) peers[threadIdx.x] = static_cast<char*>(x.peers.p[threadIdx.x]);
+  const int npacks = static_cast<int>(n.hidden * sizeof(T) / 16);
+  const size_t rb = static_cast<size_t>(npacks) * 16;
+  moveSums<T>(n, colSums, npacks, true);
+  __syncthreads();
+
+  if constexpr (V == kNormLocal) {
+    for (size_t i = blockIdx.x; i < n.rows; i += gridDim.x) {
+      auto loadG = [&](typename R::Acc(&g)[R::kPacks]) {
+        zeroAcc<T>(g);
+        addRow<T>(g, rowPtr(n.gradOut, i, rb), npacks);
+      };
+      rowBackward<T, NORM>(n, i, npacks, sh, colSums, loadG, [&](int pk, const Pack16& o) {
+        if (n.gradResidual != nullptr) st128(static_cast<char*>(n.gradResidual) + i * rb + pk * 16, o);
+        st128(static_cast<char*>(n.gradPartial) + i * rb + pk * 16, o);
+      });
+    }
+  } else {
+    const int P = a.nranks;
+    char* mine = static_cast<char*>(x.mine);
+    const size_t rows = n.rows, all = static_cast<size_t>(P) * rows;
+    const bool gather = x.gather != 0;
+    const size_t gathered = gather ? all : 0;  // the pool row of gradResidual row 0
+    auto userRow = [&](size_t j) { return j / rows * x.shardRows + j % rows; };
+    if (gather) {
+      for (size_t j = blockIdx.x; j < all; j += gridCtas()) copyRow<T>(mine + j * rb, rowPtr(n.gradOut, userRow(j), rb), npacks);
+    }
+    if (!blockBarrier(a, loadEpoch(a) + 1)) {
+      retire(a, 2, 0);
+      return;
+    }
+    const size_t sb = static_cast<size_t>(a.rank) * rows, se = sb + rows;
+    const unsigned ctas = gridCtas();
+    const size_t first = sb + (blockIdx.x + ctas - sb % ctas) % ctas;
+    for (size_t j = first; j < se; j += gridCtas()) {
+      const size_t i = j - sb;
+      auto loadG = [&](typename R::Acc(&g)[R::kPacks]) {
+        zeroAcc<T>(g);
+        if (gather) {
+          for (int r = 0; r < P; r++) addRow<T>(g, opaque(peers[r] + j * rb), npacks);
+        } else {
+          addRow<T>(g, opaque(rowPtr(n.gradOut, i, rb)), npacks);
+        }
+      };
+      rowBackward<T, NORM>(n, i, npacks, sh, colSums, loadG, [&](int pk, const Pack16& o) {
+        if (n.gradResidual != nullptr) st128(static_cast<char*>(n.gradResidual) + i * rb + pk * 16, o);
+        for (int r = 0; r < P; r++) st128_stream(opaque(peers[r] + (gathered + j) * rb) + pk * 16, o);
+      });
+    }
+    // The epoch read again rather than held across the row loop, where it would spill: it only
+    // changes when the launch's last CTA retires.
+    if (blockBarrier(a, loadEpoch(a) + 2)) {
+      for (size_t j = blockIdx.x; j < all; j += gridCtas()) {
+        copyRow<T>(static_cast<char*>(n.gradPartial) + userRow(j) * rb, mine + (gathered + j) * rb, npacks);
+      }
+    }
+  }
+  moveSums<T>(n, colSums, npacks, false);
+  if constexpr (V != kNormLocal) retire(a, 2, 0);
+}
+
+constexpr int kFinishThreads = 256;
+struct VecOuts {
+  void* p[3];
+};
+
+// One column of one vector per thread: the CTAs' sums in CTA order, rounded once.
+template <typename T>
+__global__ void __launch_bounds__(kFinishThreads)
+normBackwardFinishKernel(const float* ws, int slots, int vectors, unsigned long long hidden, VecOuts outs) {
+  const size_t c = static_cast<size_t>(blockIdx.x) * kFinishThreads + threadIdx.x;
+  const int v = blockIdx.y;
+  if (c >= hidden || outs.p[v] == nullptr) return;
+  float s = 0.0f;
+  for (int b = 0; b < slots; b++) s += ws[(static_cast<size_t>(b) * vectors + v) * hidden + c];
+  static_cast<T*>(outs.p[v])[c] = Scalar<T>::fromAcc(s);
+}
+
+// The one place that names a backward instantiation: the launch, the occupancy query and the preload.
+template <typename T>
+auto normBwdFn(int norm, int variant) -> decltype(&normBackwardKernel<T, kNormRms, kNormLocal>) {
+  auto byVariant = [&](auto normTag) -> decltype(&normBackwardKernel<T, kNormRms, kNormLocal>) {
+    constexpr int N = decltype(normTag)::value;
+    switch (variant) {
+      case kNormScatter: return normBackwardKernel<T, N, kNormScatter>;
+      case kNormLocal: return normBackwardKernel<T, N, kNormLocal>;
+      default: return nullptr;
+    }
+  };
+  switch (norm) {
+    case kNormRms: return byVariant(std::integral_constant<int, kNormRms>{});
+    case kNormLayer: return byVariant(std::integral_constant<int, kNormLayer>{});
+    default: return nullptr;
+  }
+}
+
 // The one place that names an instantiation: the launch, the occupancy query and the preload.
 template <typename T>
 auto normFn(int norm, int variant) -> decltype(&allreduceNormKernel<T, kNormNone, kNormLocal>) {
@@ -378,6 +664,18 @@ void preloadAllreduceNormKernels() {
         dispatchNormType(dt, [&](auto tag) { touchKernel(normFn<decltype(tag)>(norm, v)); });
       }
     }
+    // The backward's column sums of the widest row take more than the default 48 KB.
+    for (int norm : {kNormRms, kNormLayer}) {
+      for (int v : {kNormScatter, kNormLocal}) {
+        dispatchNormType(dt, [&](auto tag) {
+          const auto k = normBwdFn<decltype(tag)>(norm, v);
+          touchKernel(k);
+          cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               static_cast<int>(normBackwardSmemBytes(3)));
+        });
+      }
+    }
+    dispatchNormType(dt, [&](auto tag) { touchKernel(normBackwardFinishKernel<decltype(tag)>); });
   }
   cudaGetLastError();
 }
@@ -386,6 +684,31 @@ void launchAllreduceNorm(const CommArgs& a, const NormArgs& n, const NormXchg& x
                          int blocks, cudaStream_t stream) {
   dispatchNormType(dt, [&](auto tag) {
     if (auto k = normFn<decltype(tag)>(norm, variant)) k<<<blocks, kThreads, 0, stream>>>(a, n, x);
+  });
+}
+
+const void* normBackwardKernelFor(DataType dt, int norm, int variant) {
+  const void* k = nullptr;
+  dispatchNormType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(normBwdFn<decltype(tag)>(norm, variant)); });
+  return k;
+}
+
+size_t normBackwardSmemBytes(int vectors) { return vectors > 0 ? 3 * kMaxNormHidden * sizeof(float) : 0; }
+
+void launchNormBackward(const CommArgs& a, const NormBwdArgs& n, const NormXchg& x, DataType dt, int norm, int variant,
+                        int blocks, cudaStream_t stream) {
+  const size_t smem = normBackwardSmemBytes(n.vectors);
+  dispatchNormType(dt, [&](auto tag) {
+    if (auto k = normBwdFn<decltype(tag)>(norm, variant)) k<<<blocks, kThreads, smem, stream>>>(a, n, x);
+  });
+}
+
+void launchNormBackwardFinish(const float* ws, int slots, int vectors, size_t hidden, void* const (&outs)[3],
+                              DataType dt, cudaStream_t stream) {
+  VecOuts o{{outs[0], outs[1], outs[2]}};
+  const dim3 grid(static_cast<unsigned>((hidden + kFinishThreads - 1) / kFinishThreads), static_cast<unsigned>(vectors));
+  dispatchNormType(dt, [&](auto tag) {
+    normBackwardFinishKernel<decltype(tag)><<<grid, kFinishThreads, 0, stream>>>(ws, slots, vectors, hidden, o);
   });
 }
 

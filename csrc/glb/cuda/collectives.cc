@@ -532,6 +532,45 @@ NormPlan planReduceScatterNorm(PeerContext& pc, size_t rows, size_t hidden, Data
   return p;
 }
 
+NormBackwardPlan planReduceScatterNormBackward(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm,
+                                               bool gatherOut, int vectors) {
+  const char* op = "reduce_scatter_residual_norm_backward";
+  const size_t P = static_cast<size_t>(pc.size);
+  if (rows % P != 0) GLB_THROW(InputException, op, ": ", rows, " rows do not split into ", P, " equal shards");
+  if (norm != kNormRms && norm != kNormLayer) GLB_THROW(InputException, op, ": needs a norm (rms or layer)");
+  if (!normSupports(dt)) GLB_THROW(InputException, op, ": rows must be float32, bfloat16 or float16");
+  if (vectors < 0 || vectors > 3) GLB_THROW(InputException, op, ": ", vectors, " vector gradients asked for");
+  const size_t rowBytes = hidden * elementSize(dt), shard = rows / P;
+  NormBackwardPlan p;
+  size_t gridRows;
+  if (P == 1) {
+    // One rank: the local launch over every row, no exchange.
+    p.variant = kNormLocal;
+    p.chunkRows = std::max<size_t>(rows, 1);
+    gridRows = p.chunkRows;
+  } else {
+    // The forward's chunking: P rows of pool per chunk row for grad_partial, and P more for the
+    // staged grad_out when it was gathered.
+    const auto l = layoutOf(pc);
+    const size_t perRow = P * (gatherOut ? 2 : 1) * rowBytes;
+    if (perRow > l.bulkBytes) {
+      GLB_THROW(InputException, op, ": the pool's bulk region holds no row of ", rowBytes, " bytes from each of ", P,
+                " shards; raise GLB_CUDA_STAGE_MB (CudaContext stage_bytes)");
+    }
+    p.variant = kNormScatter;
+    p.chunkRows = std::min(std::max<size_t>(shard, 1), l.bulkBytes / perRow);
+    gridRows = P * p.chunkRows;
+  }
+  const void* kernel = normBackwardKernelFor(dt, norm, p.variant);
+  p.blocks = static_cast<int>(std::min<size_t>(
+      gridRows, static_cast<size_t>(pc.coResidentBlocks(kernel, kThreads, normBackwardSmemBytes(vectors)))));
+  p.launches = shard == 0 ? 0 : ceilDiv(shard, p.chunkRows);
+  // The column sums: one fp32 vector per CTA and vector, finished by one more launch.
+  p.workspaceBytes = vectors > 0 ? static_cast<size_t>(p.blocks) * vectors * hidden * sizeof(float) : 0;
+  if (vectors > 0 && p.launches > 0) p.launches += 1;
+  return p;
+}
+
 const char* normVariantName(int variant) {
   switch (variant) {
     case kNormLL: return "ll";
@@ -544,11 +583,11 @@ const char* normVariantName(int variant) {
 
 namespace {
 
-// A tensor argument of the fused operations: `rows` rows of `hidden` elements (1 for a vector).
+// A tensor argument of the fused operations: `bytes` bytes at p (null: absent).
 struct NormRange {
   const char* name;
   const void* p;
-  size_t rows;
+  size_t bytes;
 };
 
 #define GLB_NORM_CHECK(cond, ...) \
@@ -556,10 +595,13 @@ struct NormRange {
     if (!(cond)) GLB_THROW(InputException, op, ": ", __VA_ARGS__); \
   } while (0)
 
-// What both fused operations check before anything is launched. inputs: partial, residual, bias,
-// weight, norm_bias; outputs: residual_out and out (null without a norm). Null vectors are absent.
-void checkNormCall(const char* op, DataType dt, int norm, size_t hidden, bool empty, const NormRange (&inputs)[5],
-                   const NormRange (&outputs)[2]) {
+// What the fused operations check before anything is launched: dtype, norm, row width,
+// `required` (whether the tensors `requiredWhat` names are there), 16-byte alignment, and that no
+// output overlaps an input or another output, except outputs[0] == inputs[inPlace] exactly (in
+// place: each row is read before it is written). Null tensors are absent.
+template <size_t NI, size_t NO>
+void checkNormCall(const char* op, DataType dt, int norm, size_t hidden, bool required, const char* requiredWhat,
+                   const NormRange (&inputs)[NI], const NormRange (&outputs)[NO], size_t inPlace) {
   GLB_NORM_CHECK(normSupports(dt), "rows must be float32, bfloat16 or float16, got ", dataTypeName(dt));
   GLB_NORM_CHECK(norm == kNormNone || norm == kNormRms || norm == kNormLayer, "unknown norm ", norm);
   const size_t es = elementSize(dt);
@@ -567,29 +609,35 @@ void checkNormCall(const char* op, DataType dt, int norm, size_t hidden, bool em
                  " elements is not a positive multiple of 16 bytes");
   GLB_NORM_CHECK(hidden <= static_cast<size_t>(kMaxNormHidden), "rows of ", hidden, " elements exceed the limit of ",
                  kMaxNormHidden);
-  GLB_NORM_CHECK(empty || (inputs[0].p != nullptr && inputs[1].p != nullptr && outputs[0].p != nullptr &&
-                           (norm == kNormNone || outputs[1].p != nullptr)),
-                 "partial, residual, residual_out and (with a norm) out are required");
+  GLB_NORM_CHECK(required, requiredWhat);
   for (const NormRange& r : inputs) {
     GLB_NORM_CHECK(reinterpret_cast<uintptr_t>(r.p) % 16 == 0, r.name, " must be 16-byte aligned");
   }
   for (const NormRange& r : outputs) {
     GLB_NORM_CHECK(reinterpret_cast<uintptr_t>(r.p) % 16 == 0, r.name, " must be 16-byte aligned");
   }
-  const size_t rowBytes = hidden * es;
   auto overlap = [&](const NormRange& a, const NormRange& b) {
     const uintptr_t x = reinterpret_cast<uintptr_t>(a.p), y = reinterpret_cast<uintptr_t>(b.p);
-    const size_t ab = a.rows * rowBytes, bb = b.rows * rowBytes;
-    return a.p != nullptr && b.p != nullptr && ab > 0 && bb > 0 && x < y + bb && y < x + ab;
+    return a.p != nullptr && b.p != nullptr && a.bytes > 0 && b.bytes > 0 && x < y + b.bytes && y < x + a.bytes;
   };
   for (const NormRange& o : outputs) {
     for (const NormRange& i : inputs) {
-      // residual_out may be residual itself (in place: each row is read before it is written).
-      const bool inPlace = &o == &outputs[0] && &i == &inputs[1] && o.p == i.p;
-      GLB_NORM_CHECK(inPlace || !overlap(o, i), o.name, " overlaps ", i.name);
+      const bool inPlaceOk = &o == &outputs[0] && &i == &inputs[inPlace] && o.p == i.p;
+      GLB_NORM_CHECK(inPlaceOk || !overlap(o, i), o.name, " overlaps ", i.name);
     }
   }
-  GLB_NORM_CHECK(!overlap(outputs[0], outputs[1]), "residual_out overlaps out");
+  for (size_t a = 0; a < NO; a++) {
+    for (size_t b = a + 1; b < NO; b++) {
+      GLB_NORM_CHECK(!overlap(outputs[a], outputs[b]), outputs[a].name, " overlaps ", outputs[b].name);
+    }
+  }
+}
+
+// The forward's required tensors: partial, residual, residual_out and, with a norm, out.
+constexpr const char* kNormRequired = "partial, residual, residual_out and (with a norm) out are required";
+bool normRequired(size_t rows, const NormRange (&inputs)[5], const NormRange (&outputs)[2], int norm) {
+  return rows == 0 || (inputs[0].p != nullptr && inputs[1].p != nullptr && outputs[0].p != nullptr &&
+                       (norm == kNormNone || outputs[1].p != nullptr));
 }
 
 // The arguments of one chunk: n rows from `off` bytes into every row tensor.
@@ -628,10 +676,12 @@ int allreduceResidualNorm(PeerContext& pc, const void* partial, const void* resi
   GLB_TRACE_RANGE("glb::cuda::allreduceResidualNorm");
   pc.checkHealth();
   const char* op = "allreduce_residual_norm";
-  const NormRange inputs[] = {{"partial", partial, rows}, {"residual", residual, rows}, {"bias", bias, 1},
-                              {"weight", gamma, 1}, {"norm_bias", beta, 1}};
-  const NormRange outputs[] = {{"residual_out", residualOut, rows}, {"out", norm != kNormNone ? out : nullptr, rows}};
-  checkNormCall(op, dt, norm, hidden, rows == 0, inputs, outputs);
+  const size_t rb = hidden * elementSize(dt);
+  const NormRange inputs[] = {{"partial", partial, rows * rb}, {"residual", residual, rows * rb}, {"bias", bias, rb},
+                              {"weight", gamma, rb}, {"norm_bias", beta, rb}};
+  const NormRange outputs[] = {{"residual_out", residualOut, rows * rb},
+                               {"out", norm != kNormNone ? out : nullptr, rows * rb}};
+  checkNormCall(op, dt, norm, hidden, normRequired(rows, inputs, outputs, norm), kNormRequired, inputs, outputs, 1);
   if (rows == 0) return kNormLocal;
   const NormPlan plan = planResidualNorm(pc, rows, hidden, dt, norm, algo);
   DeviceGuard g(pc.device);
@@ -667,11 +717,12 @@ int reduceScatterResidualNorm(PeerContext& pc, const void* partial, const void* 
   pc.checkHealth();
   const char* op = "reduce_scatter_residual_norm";
   const size_t P = static_cast<size_t>(pc.size), shard = rows / P;
-  const NormRange inputs[] = {{"partial", partial, rows}, {"residual", residual, shard}, {"bias", bias, 1},
-                              {"weight", gamma, 1}, {"norm_bias", beta, 1}};
-  const NormRange outputs[] = {{"residual_out", residualOut, shard},
-                               {"out", norm != kNormNone ? out : nullptr, gatherOut ? rows : shard}};
-  checkNormCall(op, dt, norm, hidden, rows == 0, inputs, outputs);
+  const size_t rb = hidden * elementSize(dt);
+  const NormRange inputs[] = {{"partial", partial, rows * rb}, {"residual", residual, shard * rb}, {"bias", bias, rb},
+                              {"weight", gamma, rb}, {"norm_bias", beta, rb}};
+  const NormRange outputs[] = {{"residual_out", residualOut, shard * rb},
+                               {"out", norm != kNormNone ? out : nullptr, (gatherOut ? rows : shard) * rb}};
+  checkNormCall(op, dt, norm, hidden, normRequired(rows, inputs, outputs, norm), kNormRequired, inputs, outputs, 1);
   GLB_NORM_CHECK(rows % P == 0, rows, " rows do not split into ", P, " equal shards");
   if (P == 1) {
     return allreduceResidualNorm(pc, partial, residual, residualOut, out, bias, gamma, beta, rows, hidden, dt, norm,
@@ -694,6 +745,89 @@ int reduceScatterResidualNorm(PeerContext& pc, const void* partial, const void* 
     launchNormChunk(pc, a, x, dt, norm, kNormScatter, P * n, stream, op);
   }
   return kNormScatter;
+}
+
+int reduceScatterResidualNormBackward(PeerContext& pc, const void* gradOut, const void* s, const void* gradS,
+                                      void* gradResidual, void* gradPartial, const void* gamma, void* gradWeight,
+                                      void* gradNormBias, void* gradBias, void* workspace, size_t workspaceBytes,
+                                      size_t rows, size_t hidden, DataType dt, int norm, float eps, bool gatherOut,
+                                      cudaStream_t stream) {
+  GLB_TRACE_RANGE("glb::cuda::reduceScatterResidualNormBackward");
+  pc.checkHealth();
+  const char* op = "reduce_scatter_residual_norm_backward";
+  const size_t P = static_cast<size_t>(pc.size), shard = rows / P;
+  GLB_NORM_CHECK(norm == kNormRms || norm == kNormLayer, "needs a norm (rms or layer), got ", norm);
+  GLB_NORM_CHECK(norm == kNormLayer || gradNormBias == nullptr, "grad_norm_bias needs a layer norm");
+  const size_t rb = hidden * elementSize(dt);
+  const NormRange inputs[] = {{"grad_out", gradOut, (gatherOut ? rows : shard) * rb},
+                              {"residual_out", s, shard * rb},
+                              {"grad_residual_out", gradS, shard * rb},
+                              {"weight", gamma, rb}};
+  const NormRange outputs[] = {{"grad_residual", gradResidual, shard * rb}, {"grad_partial", gradPartial, rows * rb},
+                               {"grad_weight", gradWeight, rb}, {"grad_norm_bias", gradNormBias, rb},
+                               {"grad_bias", gradBias, rb}, {"workspace", workspace, workspaceBytes}};
+  checkNormCall(op, dt, norm, hidden, rows == 0 || (gradOut != nullptr && s != nullptr && gradPartial != nullptr),
+                "grad_out, residual_out and grad_partial are required", inputs, outputs, 2);
+  GLB_NORM_CHECK(rows % P == 0, rows, " rows do not split into ", P, " equal shards");
+  void* const vecOut[3] = {gradWeight, gradNormBias, gradBias};
+  // The requested vectors, in workspace order: vec[kind] is the slot of kind k, wsOut[slot] its output.
+  int vec[3], vectors = 0;
+  void* wsOut[3] = {nullptr, nullptr, nullptr};
+  for (int k = 0; k < 3; k++) {
+    vec[k] = vecOut[k] != nullptr ? vectors : -1;
+    if (vecOut[k] != nullptr) wsOut[vectors++] = vecOut[k];
+  }
+  const NormBackwardPlan plan = planReduceScatterNormBackward(pc, rows, hidden, dt, norm, gatherOut, vectors);
+  GLB_NORM_CHECK(workspaceBytes >= plan.workspaceBytes, "the workspace of ", workspaceBytes, " bytes is below the ",
+                 plan.workspaceBytes, " the plan needs");
+  GLB_NORM_CHECK(plan.workspaceBytes == 0 || workspace != nullptr, "the column sums need a workspace");
+  DeviceGuard g(pc.device);
+  if (shard == 0) {
+    // Nothing to sum: the vector gradients are zero.
+    for (void* v : vecOut) {
+      if (v != nullptr) GLB_CUDA_CHECK(cudaMemsetAsync(v, 0, rb, stream));
+    }
+    return plan.variant;
+  }
+  NormXchg x{};
+  if (plan.variant == kNormScatter) {
+    x.peers = pc.stagePtrs(layoutOf(pc).bulkOff);
+    x.mine = x.peers.p[pc.rank];
+    x.shardRows = shard;
+    x.gather = gatherOut ? 1 : 0;
+  }
+  // Chunk rows [r0, r0 + n) of every shard, as in the forward. The grid of every chunk but a
+  // shorter last one is plan.blocks; CTA b carries its column sums in workspace slot b.
+  for (size_t r0 = 0; r0 < shard; r0 += plan.chunkRows) {
+    const size_t n = std::min(plan.chunkRows, shard - r0), off = r0 * rb;
+    NormBwdArgs a;
+    a.gradOut = static_cast<const char*>(gradOut) + off;
+    a.s = static_cast<const char*>(s) + off;
+    a.gradS = gradS != nullptr ? static_cast<const char*>(gradS) + off : nullptr;
+    a.gradResidual = gradResidual != nullptr ? static_cast<char*>(gradResidual) + off : nullptr;
+    a.gradPartial = static_cast<char*>(gradPartial) + off;
+    a.gamma = gamma;
+    a.ws = static_cast<float*>(workspace);
+    a.rows = n;
+    a.hidden = hidden;
+    a.eps = eps;
+    a.vectors = vectors;
+    a.vecWeight = vec[0];
+    a.vecNormBias = vec[1];
+    a.vecBias = vec[2];
+    a.first = r0 == 0 ? 1 : 0;
+    const size_t gridRows = plan.variant == kNormScatter ? P * n : n;
+    const int blocks = static_cast<int>(std::min<size_t>(gridRows, static_cast<size_t>(plan.blocks)));
+    prologue(pc, stream);
+    launchNormBackward(pc.comm(), a, x, dt, norm, plan.variant, blocks, stream);
+    finish(pc, stream, op);
+  }
+  if (vectors > 0) {
+    // The first chunk's grid is plan.blocks and wrote every slot; later chunks use a prefix.
+    launchNormBackwardFinish(static_cast<const float*>(workspace), plan.blocks, vectors, hidden, wsOut, dt, stream);
+    checkLaunch(op);
+  }
+  return plan.variant;
 }
 
 #undef GLB_NORM_CHECK

@@ -148,6 +148,37 @@ int reduceScatterResidualNorm(PeerContext& pc, const void* partial, const void* 
 // chunks of chunkRows rows of every shard.
 NormPlan planReduceScatterNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, bool gatherOut);
 
+// The backward of reduceScatterResidualNorm with a norm (kNormRms / kNormLayer), for training with
+// sequence parallelism (docs/cuda.md, "Backward of the reduce-scatter norm"), on the forward's
+// exchange and chunking. rows = P x Ts; s is the saved residualOut shard (Ts rows), gradS the
+// gradient of it (null: zero), gradOut the gradient of out: rows rows (a partial per rank) with
+// gatherOut, this rank's Ts rows without. Per shard row, in fp32: g = the sum over ranks of gradOut
+// in rank order (or gradOut), the statistics recomputed from s exactly as the forward computed
+// them, gradResidual = round(gradS + the norm's input gradient). gradPartial (rows rows) gets every
+// rank's gradResidual shards, shard q at row q Ts, the same bytes on every rank; gradResidual
+// (optional, may be gradS) this rank's. Optional column sums over this rank's rows, fp32, rounded
+// once, in a fixed order (no floating-point atomics): gradWeight = sum g xh, gradNormBias = sum g
+// (layer only), gradBias = sum of the rounded gradResidual rows. They need `workspace` (16-byte
+// aligned, at least the plan's workspaceBytes). Ts = 0 launches nothing and zeroes the column sums.
+// One rank runs a local launch. Invalid arguments raise InputException before anything is launched.
+int reduceScatterResidualNormBackward(PeerContext& pc, const void* gradOut, const void* s, const void* gradS,
+                                      void* gradResidual, void* gradPartial, const void* gamma, void* gradWeight,
+                                      void* gradNormBias, void* gradBias, void* workspace, size_t workspaceBytes,
+                                      size_t rows, size_t hidden, DataType dt, int norm, float eps, bool gatherOut,
+                                      cudaStream_t stream);
+// Its variant (kNormScatter, or kNormLocal for one rank), chunk rows and launches (the chunks, plus
+// one that finishes the column sums when `vectors` > 0 of them are asked for), the grid, and the
+// fp32 workspace of the column sums: blocks x vectors x hidden floats.
+struct NormBackwardPlan {
+  int variant;
+  size_t chunkRows;
+  size_t launches;
+  int blocks;
+  size_t workspaceBytes;
+};
+NormBackwardPlan planReduceScatterNormBackward(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm,
+                                               bool gatherOut, int vectors);
+
 
 // ---- data movement -------------------------------------------------------------------
 // `buf`/`out` arguments are registered or symmetric buffers; plain-pointer

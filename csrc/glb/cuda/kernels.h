@@ -94,6 +94,39 @@ bool normSupports(DataType dt);
 const void* allreduceNormKernelFor(DataType dt, int norm, int variant);
 void launchAllreduceNorm(const CommArgs& a, const NormArgs& n, const NormXchg& x, DataType dt, int norm, int variant,
                          int blocks, cudaStream_t stream);
+// The backward of the reduce-scatter form with a norm, one chunk of `rows` rows of every shard
+// (kNormScatter; the NormXchg as in the forward, with the pool rows of docs/cuda.md) or of the
+// one rank's rows (kNormLocal). s / gradS / gradResidual are this rank's shard rows; gradOut is
+// its shard, or with x.gather P shards x.shardRows apart; gradPartial is P shards x.shardRows
+// apart. gradS / gradResidual / gamma may be null. ws: per-CTA fp32 column sums, [CTA][vectors]
+// [hidden]; vecWeight / vecNormBias / vecBias index the vectors (-1: not asked for). `first`: the
+// first chunk starts the sums from zero, later chunks from ws.
+struct NormBwdArgs {
+  const void* gradOut;
+  const void* s;
+  const void* gradS;
+  void* gradResidual;
+  void* gradPartial;
+  const void* gamma;
+  float* ws;
+  unsigned long long rows;
+  unsigned long long hidden;
+  float eps;
+  int vectors;
+  int vecWeight;
+  int vecNormBias;
+  int vecBias;
+  int first;
+};
+const void* normBackwardKernelFor(DataType dt, int norm, int variant);
+// Dynamic shared memory of that kernel: the CTA's fp32 column sums (none without vectors).
+size_t normBackwardSmemBytes(int vectors);
+void launchNormBackward(const CommArgs& a, const NormBwdArgs& n, const NormXchg& x, DataType dt, int norm, int variant,
+                        int blocks, cudaStream_t stream);
+// out_v[c] = round(sum over slots b < `slots` in order of ws[b][v][c]) for each vector v whose
+// out is non-null (outs in the order of ws's vectors).
+void launchNormBackwardFinish(const float* ws, int slots, int vectors, size_t hidden, void* const (&outs)[3],
+                              DataType dt, cudaStream_t stream);
 
 // pipeline_kernels.cu — arbitrary pointers through the pool, in-kernel pipelines (allreduce:
 // 3 stages).

@@ -491,18 +491,19 @@ void PeerContext::markLaunched(cudaStream_t stream) {
   haveLastStream_ = true;
 }
 
-int PeerContext::coResidentBlocks(const void* kernel, int threads) {
+int PeerContext::coResidentBlocks(const void* kernel, int threads, size_t dynamicSmem) {
   std::lock_guard<std::mutex> g(occMu_);
-  auto it = occupancy_.find(kernel);
+  const auto key = std::make_pair(kernel, dynamicSmem);
+  auto it = occupancy_.find(key);
   int perSm = 1;
   if (it != occupancy_.end()) {
     perSm = it->second;
   } else {
     DeviceGuard dg(device);
     int n = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, threads, 0) == cudaSuccess && n > 0) perSm = n;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, threads, dynamicSmem) == cudaSuccess && n > 0) perSm = n;
     cudaGetLastError();
-    occupancy_[kernel] = perSm;
+    occupancy_[key] = perSm;
   }
   return std::max(1, std::min(kMaxBlocks, minSms_ * perSm / std::max(1, worstRanksPerDevice_)));
 }

@@ -115,8 +115,9 @@ class PeerContext : public std::enable_shared_from_this<PeerContext> {
   // Largest grid a collective kernel may use so that all ranks' CTAs are co-resident
   // (one CTA per SM, shared between the ranks that live on this device).
   int maxBlocks() const { return maxBlocks_; }
-  // Same, for a specific kernel: SMs x resident CTAs per SM (occupancy at `threads`).
-  int coResidentBlocks(const void* kernel, int threads = kThreads);
+  // Same, for a specific kernel: SMs x resident CTAs per SM (occupancy at `threads` and
+  // `dynamicSmem` bytes of dynamic shared memory per CTA).
+  int coResidentBlocks(const void* kernel, int threads = kThreads, size_t dynamicSmem = 0);
   std::string describe() const;
 
   // ---- failure detection ---------------------------------------------------------------
@@ -235,7 +236,7 @@ class PeerContext : public std::enable_shared_from_this<PeerContext> {
   bool haveLastStream_ = false;
   cudaEvent_t orderEvent_ = nullptr;
   std::mutex occMu_;
-  std::map<const void*, int> occupancy_;
+  std::map<std::pair<const void*, size_t>, int> occupancy_;  // (kernel, dynamic smem) -> CTAs per SM
   // cudaIpc mappings are per (peer, allocation): cache them, opening twice is an error.
   std::mutex ipcMu_;
   std::map<std::pair<int, std::string>, void*> ipcCache_;

@@ -146,6 +146,96 @@ std::string checkScatterNorm(const CommArgs& ca, const NormXchg& x, int norm, si
   return "";
 }
 
+// The backward of the reduce-scatter norm as one chunk of `rows` rows (shards of x.shardRows rows;
+// kNormLocal: the one rank's rows): s[i, j] = 1 + i + j / H, grad_out 0.5 - k / (4 H) at flat index
+// k, grad_s 0.25 + k / (2 H), gamma 1 + j / H, all exact in fp32. Rank 0 owns the chunk's rows of
+// shard 0; with a gather its virtual peers staged the same grad_out rows, so g = P grad_out. Checks
+// grad_residual, rank 0's rows of grad_partial and the weight, norm bias and bias column sums
+// against a CPU double-precision row.
+std::string checkNormBackward(const CommArgs& ca, const NormXchg& x, int variant, int norm, size_t rows, size_t H,
+                              int blocks, cudaStream_t st) {
+  const bool scatter = variant == kNormScatter;
+  const size_t all = scatter ? ca.nranks * x.shardRows : rows, outRows = scatter && x.gather ? all : rows;
+  const int vectors = norm == kNormLayer ? 3 : 2;
+  DevBuf gradOut(outRows * H * 4), sv(rows * H * 4), gs(rows * H * 4), gr(rows * H * 4), gp(all * H * 4),
+      gamma(H * 4), vecs(3 * H * 4), ws(static_cast<size_t>(blocks) * vectors * H * 4);
+  launchFill(gradOut.p, outRows * H, DataType::FLOAT32, 0.5, -0.25 / H, st);
+  launchFill(sv.p, rows * H, DataType::FLOAT32, 1.0, 1.0 / H, st);
+  launchFill(gs.p, rows * H, DataType::FLOAT32, 0.25, 0.5 / H, st);
+  launchFill(gamma.p, H, DataType::FLOAT32, 1.0, 1.0 / H, st);
+  NormBwdArgs a;
+  a.gradOut = gradOut.p;
+  a.s = sv.p;
+  a.gradS = gs.p;
+  a.gradResidual = gr.p;
+  a.gradPartial = gp.p;
+  a.gamma = gamma.p;
+  a.ws = static_cast<float*>(ws.p);
+  a.rows = rows;
+  a.hidden = H;
+  a.eps = 1e-5f;
+  a.vectors = vectors;
+  a.vecWeight = 0;
+  a.vecNormBias = norm == kNormLayer ? 1 : -1;
+  a.vecBias = vectors - 1;
+  a.first = 1;
+  launchNormBackward(ca, a, x, DataType::FLOAT32, norm, variant, blocks, st);
+  float* v = static_cast<float*>(vecs.p);
+  void* const outs[3] = {v, norm == kNormLayer ? v + H : nullptr, v + 2 * H};
+  void* const packed[3] = {outs[0], outs[1] != nullptr ? outs[1] : outs[2], outs[1] != nullptr ? outs[2] : nullptr};
+  launchNormBackwardFinish(a.ws, blocks, vectors, H, packed, DataType::FLOAT32, st);
+  noteLaunch(2);
+  const auto r = download(gr.p, rows * H, st), p = download(gp.p, all * H, st), go = download(gradOut.p, outRows * H, st);
+  const auto vw = download(v, H, st), vnb = download(v + H, H, st), vb = download(v + 2 * H, H, st);
+  const double mult = scatter && x.gather ? ca.nranks : 1;
+  std::vector<double> sw(H, 0), snb(H, 0), sb(H, 0), aw(H, 0), anb(H, 0), ab(H, 0);
+  for (size_t i = 0; i < rows; i++) {
+    std::vector<double> xs(H), g(H);
+    double mean = 0, sq = 0, mg = 0, mgx = 0, scale = 0;
+    for (size_t j = 0; j < H; j++) {
+      xs[j] = 1.0 + static_cast<double>(i) + static_cast<double>(j) / H;
+      g[j] = mult * go[i * H + j];
+      mean += xs[j] / H;
+    }
+    if (norm == kNormRms) mean = 0;
+    for (size_t j = 0; j < H; j++) sq += (xs[j] - mean) * (xs[j] - mean) / H;
+    const double rinv = 1.0 / std::sqrt(sq + 1e-5);
+    for (size_t j = 0; j < H; j++) {
+      xs[j] = (xs[j] - mean) * rinv;
+      const double gg = g[j] * (1.0 + static_cast<double>(j) / H);
+      mg += gg / H;
+      mgx += gg * xs[j] / H;
+      sw[j] += g[j] * xs[j];
+      snb[j] += g[j];
+      aw[j] += std::fabs(g[j] * xs[j]);
+      anb[j] += std::fabs(g[j]);
+    }
+    if (norm == kNormRms) mg = 0;
+    std::vector<double> want(H);
+    for (size_t j = 0; j < H; j++) {
+      const double gg = g[j] * (1.0 + static_cast<double>(j) / H);
+      want[j] = 0.25 + static_cast<double>(i * H + j) * 0.5 / H + rinv * (gg - mg - xs[j] * mgx);
+      scale = std::max(scale, std::fabs(want[j]));
+    }
+    for (size_t j = 0; j < H; j++) {
+      if (std::fabs(r[i * H + j] - want[j]) > 1e-4 * scale + 1e-6) {
+        return strcat_all("grad_residual[", i, ", ", j, "]: got ", r[i * H + j], " want ", want[j]);
+      }
+      if (p[i * H + j] != r[i * H + j]) return strcat_all("grad_partial[", i, ", ", j, "] differs from grad_residual");
+      sb[j] += r[i * H + j];
+      ab[j] += std::fabs(r[i * H + j]);
+    }
+  }
+  for (size_t j = 0; j < H; j++) {
+    if (std::fabs(vw[j] - sw[j]) > 1e-4 * aw[j] + 1e-6) return strcat_all("grad_weight[", j, "]: got ", vw[j], " want ", sw[j]);
+    if (norm == kNormLayer && std::fabs(vnb[j] - snb[j]) > 1e-4 * anb[j] + 1e-6) {
+      return strcat_all("grad_norm_bias[", j, "]: got ", vnb[j], " want ", snb[j]);
+    }
+    if (std::fabs(vb[j] - sb[j]) > 1e-5 * ab[j] + 1e-6) return strcat_all("grad_bias[", j, "]: got ", vb[j], " want ", sb[j]);
+  }
+  return "";
+}
+
 class Runner {
  public:
   Runner(PeerContext& pc, cudaStream_t s) : pc_(pc), s_(s) {}
@@ -375,6 +465,27 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
             x.shardRows = 5;
             x.gather = gather;
             return checkScatterNorm(ca, x, norm, 3, H, 3, stream);
+          });
+        }
+      }
+      // its backward: the same chunk, grad_out gathered or not, and the one-rank form
+      for (int gather : {0, 1}) {
+        for (int norm : {kNormRms, kNormLayer}) {
+          R.run(strcat_all("normBackwardKernel<float,", norms[norm], ",reduce_scatter> P=", P, gather ? " gather" : ""),
+                [&]() -> std::string {
+            NormXchg x{};
+            for (int r = 0; r < P; r++) x.peers.p[r] = myStage + 2 * half;
+            x.mine = x.peers.p[0];
+            x.shardRows = 5;
+            x.gather = gather;
+            return checkNormBackward(ca, x, kNormScatter, norm, 3, H, 3, stream);
+          });
+        }
+      }
+      if (P == 2) {
+        for (int norm : {kNormRms, kNormLayer}) {
+          R.run(strcat_all("normBackwardKernel<float,", norms[norm], ",local>"), [&]() -> std::string {
+            return checkNormBackward(ca, NormXchg{}, kNormLocal, norm, 5, H, 3, stream);
           });
         }
       }

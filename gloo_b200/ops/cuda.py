@@ -315,6 +315,87 @@ class CudaContext:
                                          kinds[norm], float(eps), bool(gather_out), _stream(stream))
         return residual_out if norm is None else (residual_out, out)
 
+    def reduce_scatter_residual_norm_backward(self, grad_out, residual_out, grad_residual_out=None, weight=None, *,
+                                              norm: str, eps: float = 1e-6, gather_out: bool = True,
+                                              grad_partial=None, grad_residual=None, grad_weight=None,
+                                              grad_norm_bias=None, grad_bias=None, stream=None):
+        """The backward of :meth:`reduce_scatter_residual_norm` with a norm, in ONE kernel launch
+        per chunk: the reduce-scatter of a gathered ``out``'s gradient, the norm's backward on
+        this rank's shard, the add of ``residual_out``'s gradient and the allgather of the sum.
+
+        ``residual_out`` is the forward's saved shard ``(Ts, ...)``; ``grad_residual_out`` its
+        gradient (None counts as zero); ``grad_out`` the gradient of ``out``: ``(T, ...)`` with
+        ``gather_out`` (this rank's partial of it), ``(Ts, ...)`` without. ``norm``, ``eps``,
+        ``weight`` and ``gather_out`` are the forward's. Per row, in fp32, with ``g`` the sum over
+        ranks of ``grad_out`` (rank order) and the statistics recomputed exactly as the forward
+        computed them: ``grad_residual = round(grad_residual_out + the norm's input gradient)``.
+        ``grad_partial`` ``(T, ...)`` gets every rank's ``grad_residual`` shards (shard q at rows
+        ``q * Ts``), the same bytes on every rank: the gradient of ``partial``. ``grad_residual``
+        (this rank's rows of it) may be ``grad_residual_out`` itself. Both are allocated when not
+        given. ``grad_weight`` (sum of ``g * xhat``), ``grad_norm_bias`` (sum of ``g``, layer only)
+        and ``grad_bias`` (sum of the rounded ``grad_residual`` rows) are column sums over this
+        rank's rows, fp32, rounded once, in a fixed order: each is computed into the ``(H,)`` tensor
+        given and skipped when None. The fp32 workspace they need comes from torch's allocator, on
+        the stream the call runs on.
+        Invalid arguments raise ``ValueError`` before anything is launched.
+
+        Returns ``(grad_partial, grad_residual, grad_weight, grad_norm_bias, grad_bias)``."""
+        import torch
+
+        kinds = {"rms": 1, "layer": 2}
+        name = "reduce_scatter_residual_norm_backward"
+        if norm not in kinds:
+            raise ValueError(f"{name}: norm must be 'rms' or 'layer', got {norm!r}")
+        if norm != "layer" and grad_norm_bias is not None:
+            raise ValueError(f"{name}: grad_norm_bias needs norm='layer'")
+        if residual_out.dim() < 2:
+            raise ValueError(f"{name}: residual_out must have a token and a hidden dimension")
+        shard, H = tuple(residual_out.shape), residual_out.shape[-1]
+        full = (self.size * shard[0], *shard[1:])
+        if grad_partial is None:
+            grad_partial = torch.empty(full, dtype=residual_out.dtype, device=residual_out.device)
+        if grad_residual is None:
+            grad_residual = torch.empty(shard, dtype=residual_out.dtype, device=residual_out.device)
+        named = {"grad_out": grad_out, "residual_out": residual_out, "grad_residual_out": grad_residual_out,
+                 "weight": weight, "grad_partial": grad_partial, "grad_residual": grad_residual,
+                 "grad_weight": grad_weight, "grad_norm_bias": grad_norm_bias, "grad_bias": grad_bias}
+        for key, t in named.items():
+            if t is None:
+                continue
+            if not t.is_cuda or t.dtype != residual_out.dtype or not t.is_contiguous():
+                raise ValueError(f"{name}: {key} must be a contiguous CUDA tensor of {residual_out.dtype}, "
+                                 f"got {t.dtype} on {t.device}{'' if t.is_contiguous() else ', not contiguous'}")
+            if key in ("weight", "grad_weight", "grad_norm_bias", "grad_bias"):
+                want = (H,)
+            elif key == "grad_partial" or (key == "grad_out" and gather_out):
+                want = full
+            else:
+                want = shard
+            if tuple(t.shape) != want:
+                raise ValueError(f"{name}: {key} has shape {tuple(t.shape)}, expected {want}")
+        _, _, dt, _ = describe(residual_out)
+        rows = self.size * (residual_out.numel() // max(H, 1))
+        vectors = sum(t is not None for t in (grad_weight, grad_norm_bias, grad_bias))
+        plan = _cu.plan_reduce_scatter_norm_backward(self.pc, rows, H, int(dt), kinds[norm], bool(gather_out), vectors)
+        launch = _stream(stream)
+        ws = None
+        if plan["workspace_bytes"]:
+            # The workspace is this call's own temporary: allocate it on the stream the kernels run
+            # on, so that the caching allocator reuses it only for work ordered after them.
+            dev = residual_out.device
+            if launch == torch.cuda.current_stream(dev).cuda_stream:
+                ws = torch.empty(plan["workspace_bytes"], dtype=torch.uint8, device=dev)
+            else:
+                on = stream if isinstance(stream, torch.cuda.Stream) else torch.cuda.ExternalStream(launch, device=dev)
+                with torch.cuda.stream(on):
+                    ws = torch.empty(plan["workspace_bytes"], dtype=torch.uint8, device=dev)
+        ptr = lambda t: 0 if t is None else t.data_ptr()  # noqa: E731
+        _cu.reduce_scatter_residual_norm_backward(
+            self.pc, ptr(grad_out), ptr(residual_out), ptr(grad_residual_out), ptr(grad_residual), ptr(grad_partial),
+            ptr(weight), ptr(grad_weight), ptr(grad_norm_bias), ptr(grad_bias), ptr(ws),
+            0 if ws is None else ws.numel(), rows, H, int(dt), kinds[norm], float(eps), bool(gather_out), launch)
+        return grad_partial, grad_residual, grad_weight, grad_norm_bias, grad_bias
+
     # ---- health ---------------------------------------------------------------------------
     def set_timeout(self, ms: int):
         """Device-side waits give up after ``ms`` milliseconds (then the context is poisoned)."""

@@ -51,6 +51,16 @@ def _norm_fusable(cc, partial, residual, residual_shape, norm_module, kind, vect
     return True
 
 
+def _aligned_like(s, *grads) -> bool:
+    """Whether the gradients (None: absent) have ``s``'s dtype and device and, made contiguous,
+    the 16-byte alignment the fused backward needs."""
+    for g in grads:
+        if g is not None and (g.dtype != s.dtype or g.device != s.device or
+                              (g.is_contiguous() and g.data_ptr() % 16)):
+            return False
+    return True
+
+
 def _norm_input_grad(kind, H, eps, s, w, nb, grad_out):
     """The norm's gradients, recomputed with torch from its saved input ``s``: ``(grad_s,
     grad_weight, grad_norm_bias)``, None for an absent weight or bias."""
@@ -649,9 +659,11 @@ class SequenceParallel(_Base):
         CUDA tensors within the fused operation's limits run it as one kernel
         (``CudaContext.reduce_scatter_residual_norm``), into a fresh ``s``. Its backward
         reduce-scatters the gradient of a gathered ``out``, adds the norm's input gradient
-        (recomputed with torch from the saved ``s``) to the gradient of ``s``, and allgathers that
-        sum into the gradient of ``partial``; ``residual_shard`` gets the sum, ``bias`` its row sum
-        and the norm's weights theirs from the recompute, all from this rank's tokens. Anything else
+        (recomputed from the saved ``s``) to the gradient of ``s``, and allgathers that sum into the
+        gradient of ``partial``; ``residual_shard`` gets the sum, ``bias`` its row sum and the norm's
+        weights theirs, all from this rank's tokens. With a norm whose ``out`` got a gradient that is
+        one fused kernel too (``CudaContext.reduce_scatter_residual_norm_backward``); otherwise it
+        runs the collectives and a torch recompute of the norm. Anything else
         runs ``reduce_scatter_to_sequence``, ``+ bias``, ``+ residual_shard``, the module and
         ``gather_from_sequence``."""
         import torch
@@ -694,6 +706,14 @@ class SequenceParallel(_Base):
             @staticmethod
             def backward(ctx, grad_s, grad_out=None):
                 s, w, nb = ctx.saved_tensors
+                if kind is not None and grad_out is not None and _aligned_like(s, grad_out, grad_s):
+                    need_b, need_w, need_nb = ctx.needs_input_grad[2:5]
+                    vec = lambda t, need: torch.empty(H, dtype=s.dtype, device=s.device) if t and need else None  # noqa: E731
+                    gp, gr, gw, gnb, gb = sp.cc.reduce_scatter_residual_norm_backward(
+                        grad_out.contiguous(), s, None if grad_s is None else grad_s.contiguous(), w, norm=kind,
+                        eps=eps, gather_out=gather_out, grad_weight=vec(w is not None, need_w),
+                        grad_norm_bias=vec(nb is not None, need_nb), grad_bias=vec(ctx.has_bias, need_b))
+                    return gp, gr, gb, gw, gnb
                 grad_s = torch.zeros_like(s) if grad_s is None else grad_s
                 gw = gnb = None
                 if kind is not None and grad_out is not None:

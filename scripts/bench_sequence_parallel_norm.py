@@ -17,6 +17,13 @@ a card pay for each other's kernels and exchange through local memory, so those 
 the per-call overhead only, not the link; the JSON says so. Timing as in bench_allreduce_norm.py:
 CUDA events around `--iters` back-to-back calls after `--warmup`, median over `--reps` windows,
 the maximum over ranks. T is the whole sequence (tokens of every rank).
+
+`--backward` times the fused backward instead (`CudaContext.reduce_scatter_residual_norm_backward`:
+reduce-scatter of the gathered out's gradient, the norm's backward, the add of the residual
+stream's gradient and the allgather, one kernel per chunk plus one that finishes the column sums)
+against the composition SequenceParallel's autograd ran before it: `cc.reduce_scatter`, the norm
+recomputed under torch autograd, the add, the bias row sum and `cc.allgather`. Before timing, each
+shape records how far the two gradients of `partial` lie apart.
 """
 import argparse
 import json
@@ -32,6 +39,7 @@ import torch.nn.functional as F  # noqa: E402
 import gloo_b200 as gb  # noqa: E402
 from bench_allreduce_norm import gpu_info, launches_fused, timed  # noqa: E402
 from gloo_b200.ops import cuda as gcu  # noqa: E402
+from gloo_b200.parallel.strategies import _norm_input_grad  # noqa: E402
 
 DECODE_T = (8, 64, 256)
 PREFILL_T = (4096,)
@@ -91,6 +99,63 @@ def bench_rank(ctx, device, args, world):
     return rows
 
 
+BACKWARD_T = (4096, 8192)
+
+
+def bench_backward_rank(ctx, device, args, world):
+    cc = gcu.CudaContext(ctx, device, stage_bytes=args.stage_mb << 20)
+    cc.set_timeout(600000)
+    stream = torch.cuda.current_stream()
+    dtype, P, rank = torch.bfloat16, ctx.size, ctx.rank
+    rows = []
+    for H in HIDDEN:
+        for T in BACKWARD_T:
+            Ts = T // P
+            g = torch.Generator(device="cpu").manual_seed(T * 131 + H)
+            s = torch.randn(T, H, generator=g).to(dtype)[rank * Ts:(rank + 1) * Ts].contiguous().cuda()
+            weight = (1 + 0.1 * torch.randn(H, generator=g)).to(dtype).cuda()
+            norm_bias = (0.1 * torch.randn(H, generator=g)).to(dtype).cuda()
+            mine = torch.Generator().manual_seed(T * 131 + H + 7 + rank)
+            g_out = torch.randn(T, H, generator=mine).to(dtype).cuda()
+            g_s = torch.randn(Ts, H, generator=mine).to(dtype).cuda()
+            gp, gr = torch.empty(T, H, dtype=dtype, device="cuda"), torch.empty_like(s)
+            gw, gnb, gb_ = (torch.empty(H, dtype=dtype, device="cuda") for _ in range(3))
+            for norm in ("rms", "layer"):
+                nb = norm_bias if norm == "layer" else None
+
+                def fused():
+                    cc.reduce_scatter_residual_norm_backward(g_out, s, g_s, weight, norm=norm, eps=1e-6,
+                                                             grad_partial=gp, grad_residual=gr, grad_weight=gw,
+                                                             grad_norm_bias=gnb if norm == "layer" else None,
+                                                             grad_bias=gb_)
+
+                def composed():
+                    y = torch.empty_like(s)
+                    cc.reduce_scatter(y, g_out)
+                    gs, _, _ = _norm_input_grad(norm, H, 1e-6, s, weight, nb, y)
+                    total = g_s + gs
+                    total.sum(0)
+                    full = torch.empty(T, H, dtype=dtype, device="cuda")
+                    cc.allgather(full, total)
+                    return full
+
+                fused()
+                ref = composed()
+                torch.cuda.synchronize()
+                vectors = 3 if norm == "layer" else 2
+                plan = gb._C.cuda.plan_reduce_scatter_norm_backward(cc.pc, T, H, int(gb.DataType.BFLOAT16),
+                                                                    {"rms": 1, "layer": 2}[norm], True, vectors)
+                row = {"T": T, "H": H, "dtype": "bfloat16", "norm": norm, "shard_bytes": Ts * H * 2,
+                       "variant": plan["variant"], "launches": plan["launches"], "chunk_rows": plan["chunk_rows"],
+                       "max_abs_diff_composed": float((gp.float() - ref.float()).abs().max()),
+                       "max_abs_grad": float(ref.float().abs().max())}
+                for name, fn in (("fused", fused), ("composed", composed)):
+                    row[f"{name}_us"] = timed(ctx, cc, fn, stream, args, world)
+                row["speedup"] = row["composed_us"] / row["fused_us"]
+                rows.append(row)
+    return rows
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default="")
@@ -99,10 +164,12 @@ def main():
     ap.add_argument("--warmup", type=int, default=50)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--stage-mb", type=int, default=128)
+    ap.add_argument("--backward", action="store_true", help="time the fused backward against its composition")
     args = ap.parse_args()
+    run = bench_backward_rank if args.backward else bench_rank
     if args.threads:
         world = args.threads
-        rows = gb.spawn_threads(world, lambda ctx: bench_rank(ctx, 0, args, 1), cuda_device=0, timeout_ms=600000)[0]
+        rows = gb.spawn_threads(world, lambda ctx: run(ctx, 0, args, 1), cuda_device=0, timeout_ms=600000)[0]
         mode = f"{world} ranks as threads on one GPU: overhead only, not link numbers"
         info, rank = gpu_info(0), 0
     else:
@@ -111,11 +178,12 @@ def main():
         torch.cuda.set_device(local)
         ctx = gb.init_context(rank, world, path=f"/tmp/glb_sp_{os.environ.get('MASTER_PORT', '0')}_{os.getppid()}",
                               timeout_ms=120000)
-        rows = bench_rank(ctx, local, args, world)
+        rows = run(ctx, local, args, world)
         mode = f"{world} ranks, one per GPU"
         info = gpu_info(local)
     if rank == 0:
-        doc = {"benchmark": "reduce_scatter_residual_norm", "mode": mode, "ranks": world, **info, "iters": args.iters,
+        name = "reduce_scatter_residual_norm" + ("_backward" if args.backward else "")
+        doc = {"benchmark": name, "mode": mode, "ranks": world, **info, "iters": args.iters,
                "warmup": args.warmup, "reps": args.reps, "rows": rows}
         text = json.dumps(doc)
         print(text)

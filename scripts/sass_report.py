@@ -55,6 +55,7 @@ KERNELS = [
     ("ll_combine_topk_f32", r"moeLLCombineKernel<float>"),
     ("reduce_scatter_norm_bf16_rms", r"allreduceNormKernel<__nv_bfloat16, 1, 4>"),
     ("reduce_scatter_norm_f32_layer", r"allreduceNormKernel<float, 2, 4>"),
+    ("reduce_scatter_norm_backward_bf16_rms", r"normBackwardKernel<__nv_bfloat16, 1, 4>"),
     ("p2p_sendrecv", r"p2pKernel"),
     ("exchange_zero_copy", r"exchangeKernel<false>"),
     ("exchange_zero_copy_tma", r"exchangeKernel<true>"),
