@@ -509,6 +509,17 @@ __device__ __forceinline__ void rowBackward(const NormBwdArgs& n, size_t i, int 
 // pairs the CTAs that touch the same rows. Without a gather nothing is staged, and the first
 // barrier only keeps the owners' stores out of a peer's pool until that peer has finished the
 // launch before, which may still be reading it.
+//
+// The allreduce forms (tensor parallelism): every rank holds all rows of s and gradS, gradOut is
+// its partial of out's gradient, and gradPartial = round(gradS + dx) gets every row.
+//   ONE_SHOT  stage gradOut in the pool half of this launch's parity, barrier, every rank sums the
+//             P staged copies of every row in rank order and runs rowBackward on all of them, so
+//             its column sums cover every row.
+//   TWO_SHOT  stage gradOut in the bulk region, barrier, the owner of each row (the forward
+//             two-shot's row split) sums the P staged rows in rank order, runs rowBackward and
+//             stores gradPartial into every peer's pool over the staged row (which only the owner
+//             reads), barrier, every rank copies all rows out. The column sums cover this rank's
+//             rows: normBackwardFinishAllreduceKernel completes them.
 template <typename T, int NORM, int V>
 __global__ void __launch_bounds__(kThreads, 1)
 normBackwardKernel(CommArgs a, NormBwdArgs n, NormXchg x) {
@@ -516,7 +527,12 @@ normBackwardKernel(CommArgs a, NormBwdArgs n, NormXchg x) {
   extern __shared__ float colSums[];
   __shared__ float sh[kThreads / 32];
   __shared__ char* peers[kMaxRanks];
-  if (threadIdx.x < kMaxRanks) peers[threadIdx.x] = static_cast<char*>(x.peers.p[threadIdx.x]);
+  if (threadIdx.x < kMaxRanks) {
+    char* p = static_cast<char*>(x.peers.p[threadIdx.x]);
+    // One-shot: the pool half of this launch, folded into the peers' pointers once.
+    if constexpr (V == kNormOneShot) p += (ld_relaxed_sys(&a.self->stageSeq) & 1u) * x.parityStride;
+    peers[threadIdx.x] = p;
+  }
   const int npacks = static_cast<int>(n.hidden * sizeof(T) / 16);
   const size_t rb = static_cast<size_t>(npacks) * 16;
   moveSums<T>(n, colSums, npacks, true);
@@ -532,6 +548,57 @@ normBackwardKernel(CommArgs a, NormBwdArgs n, NormXchg x) {
         if (n.gradResidual != nullptr) st128(static_cast<char*>(n.gradResidual) + i * rb + pk * 16, o);
         st128(static_cast<char*>(n.gradPartial) + i * rb + pk * 16, o);
       });
+    }
+  } else if constexpr (V == kNormOneShot) {
+    for (size_t i = blockIdx.x; i < n.rows; i += gridCtas()) {
+      copyRow<T>(peers[a.rank] + i * rb, rowPtr(n.gradOut, i, rb), npacks);
+    }
+    if (!blockBarrier(a, loadEpoch(a) + 1)) {
+      retire(a, 1, 1);
+      return;
+    }
+    for (size_t i = blockIdx.x; i < n.rows; i += gridCtas()) {
+      auto loadG = [&](typename R::Acc(&g)[R::kPacks]) {
+        zeroAcc<T>(g);
+        for (int r = 0; r < a.nranks; r++) addRow<T>(g, opaque(peers[r] + i * rb), npacks);
+      };
+      rowBackward<T, NORM>(n, i, npacks, sh, colSums, loadG, [&](int pk, const Pack16& o) {
+        st128(static_cast<char*>(n.gradPartial) + i * rb + pk * 16, o);
+      });
+    }
+  } else if constexpr (V == kNormTwoShot) {
+    // Pool rows [0, rows): the staged gradOut, overwritten with gradPartial by the row's owner.
+    const int P = a.nranks;
+    char* mine = static_cast<char*>(x.mine);
+    for (size_t i = blockIdx.x; i < n.rows; i += gridCtas()) copyRow<T>(mine + i * rb, rowPtr(n.gradOut, i, rb), npacks);
+    if (!blockBarrier(a, loadEpoch(a) + 1)) {
+      retire(a, 2, 0);
+      return;
+    }
+    // This rank's rows [sb, se), the forward two-shot's split. The end is read from shared memory
+    // where it is tested rather than held across the row loop, where it would spill (fp32 layer).
+    __shared__ size_t ownEnd;
+    size_t sb;
+    {
+      const size_t q = n.rows / P, rem = n.rows % P, me = static_cast<size_t>(a.rank);
+      sb = me * q + (me < rem ? me : rem);
+      if (threadIdx.x == 0) ownEnd = sb + q + (me < rem ? 1 : 0);
+    }
+    __syncthreads();
+    const unsigned ctas = gridCtas();
+    for (size_t i = sb + (blockIdx.x + ctas - sb % ctas) % ctas; i < ownEnd; i += gridCtas()) {
+      auto loadG = [&](typename R::Acc(&g)[R::kPacks]) {
+        zeroAcc<T>(g);
+        for (int r = 0; r < P; r++) addRow<T>(g, opaque(peers[r] + i * rb), npacks);
+      };
+      rowBackward<T, NORM>(n, i, npacks, sh, colSums, loadG, [&](int pk, const Pack16& o) {
+        for (int r = 0; r < P; r++) st128_stream(opaque(peers[r] + i * rb) + pk * 16, o);
+      });
+    }
+    if (blockBarrier(a, loadEpoch(a) + 2)) {
+      for (size_t i = blockIdx.x; i < n.rows; i += gridCtas()) {
+        copyRow<T>(static_cast<char*>(n.gradPartial) + i * rb, mine + i * rb, npacks);
+      }
     }
   } else {
     const int P = a.nranks;
@@ -574,7 +641,11 @@ normBackwardKernel(CommArgs a, NormBwdArgs n, NormXchg x) {
     }
   }
   moveSums<T>(n, colSums, npacks, false);
-  if constexpr (V != kNormLocal) retire(a, 2, 0);
+  if constexpr (V == kNormOneShot) {
+    retire(a, 1, 1);
+  } else if constexpr (V != kNormLocal) {
+    retire(a, 2, 0);
+  }
 }
 
 constexpr int kFinishThreads = 256;
@@ -594,6 +665,47 @@ normBackwardFinishKernel(const float* ws, int slots, int vectors, unsigned long 
   static_cast<T*>(outs.p[v])[c] = Scalar<T>::fromAcc(s);
 }
 
+// The two-shot allreduce backward's finish, a collective: its CTA sums cover this rank's rows only.
+// Element k of the [vectors][hidden] vector per thread (grid-stride): this rank's CTA sums in CTA
+// order (fp32), staged in its pool; barrier; the P staged vectors in rank order, rounded once, the
+// same bytes on every rank; a closing barrier, so that no rank restages its pool while a peer still
+// reads it. CTA b handles the same elements on every rank, so each barrier pairs the right CTAs.
+template <typename T>
+__global__ void __launch_bounds__(kFinishThreads)
+normBackwardFinishAllreduceKernel(CommArgs a, const float* ws, int slots, int vectors, unsigned long long hidden,
+                                  VecOuts outs, PeerPtrs pool) {
+  // Indexed by a run-time rank / vector: from shared memory, filled with constant indices (a
+  // dynamic index into the parameter space copies the struct to local memory).
+  __shared__ const float* peers[kMaxRanks];
+  __shared__ T* out[3];
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int r = 0; r < kMaxRanks; r++) peers[r] = static_cast<const float*>(pool.p[r]);
+#pragma unroll
+    for (int v = 0; v < 3; v++) out[v] = static_cast<T*>(outs.p[v]);
+  }
+  __syncthreads();
+  const uint32_t e = loadEpoch(a);
+  const size_t len = static_cast<size_t>(vectors) * hidden, stride = static_cast<size_t>(gridDim.x) * kFinishThreads;
+  float* mine = const_cast<float*>(peers[a.rank]);
+  for (size_t k = static_cast<size_t>(blockIdx.x) * kFinishThreads + threadIdx.x; k < len; k += stride) {
+    float s = 0.0f;
+    for (int b = 0; b < slots; b++) s += ws[static_cast<size_t>(b) * len + k];
+    mine[k] = s;
+  }
+  if (!blockBarrier(a, e + 1)) {
+    retire(a, 2, 0);
+    return;
+  }
+  for (size_t k = static_cast<size_t>(blockIdx.x) * kFinishThreads + threadIdx.x; k < len; k += stride) {
+    float s = 0.0f;
+    for (int r = 0; r < a.nranks; r++) s += peers[r][k];
+    out[k / hidden][k % hidden] = Scalar<T>::fromAcc(s);
+  }
+  blockBarrier(a, e + 2);
+  retire(a, 2, 0);
+}
+
 // The one place that names a backward instantiation: the launch, the occupancy query and the preload.
 template <typename T>
 auto normBwdFn(int norm, int variant) -> decltype(&normBackwardKernel<T, kNormRms, kNormLocal>) {
@@ -602,6 +714,8 @@ auto normBwdFn(int norm, int variant) -> decltype(&normBackwardKernel<T, kNormRm
     switch (variant) {
       case kNormScatter: return normBackwardKernel<T, N, kNormScatter>;
       case kNormLocal: return normBackwardKernel<T, N, kNormLocal>;
+      case kNormOneShot: return normBackwardKernel<T, N, kNormOneShot>;
+      case kNormTwoShot: return normBackwardKernel<T, N, kNormTwoShot>;
       default: return nullptr;
     }
   };
@@ -666,7 +780,7 @@ void preloadAllreduceNormKernels() {
     }
     // The backward's column sums of the widest row take more than the default 48 KB.
     for (int norm : {kNormRms, kNormLayer}) {
-      for (int v : {kNormScatter, kNormLocal}) {
+      for (int v : {kNormScatter, kNormLocal, kNormOneShot, kNormTwoShot}) {
         dispatchNormType(dt, [&](auto tag) {
           const auto k = normBwdFn<decltype(tag)>(norm, v);
           touchKernel(k);
@@ -675,7 +789,10 @@ void preloadAllreduceNormKernels() {
         });
       }
     }
-    dispatchNormType(dt, [&](auto tag) { touchKernel(normBackwardFinishKernel<decltype(tag)>); });
+    dispatchNormType(dt, [&](auto tag) {
+      touchKernel(normBackwardFinishKernel<decltype(tag)>);
+      touchKernel(normBackwardFinishAllreduceKernel<decltype(tag)>);
+    });
   }
   cudaGetLastError();
 }
@@ -709,6 +826,24 @@ void launchNormBackwardFinish(const float* ws, int slots, int vectors, size_t hi
   const dim3 grid(static_cast<unsigned>((hidden + kFinishThreads - 1) / kFinishThreads), static_cast<unsigned>(vectors));
   dispatchNormType(dt, [&](auto tag) {
     normBackwardFinishKernel<decltype(tag)><<<grid, kFinishThreads, 0, stream>>>(ws, slots, vectors, hidden, o);
+  });
+}
+
+const void* normBackwardFinishAllreduceKernelFor(DataType dt) {
+  const void* k = nullptr;
+  dispatchNormType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(normBackwardFinishAllreduceKernel<decltype(tag)>); });
+  return k;
+}
+
+int normBackwardFinishThreads() { return kFinishThreads; }
+
+void launchNormBackwardFinishAllreduce(const CommArgs& a, const float* ws, int slots, int vectors, size_t hidden,
+                                       void* const (&outs)[3], const PeerPtrs& pool, DataType dt, int blocks,
+                                       cudaStream_t stream) {
+  VecOuts o{{outs[0], outs[1], outs[2]}};
+  dispatchNormType(dt, [&](auto tag) {
+    normBackwardFinishAllreduceKernel<decltype(tag)><<<blocks, kFinishThreads, 0, stream>>>(a, ws, slots, vectors, hidden,
+                                                                                           o, pool);
   });
 }
 

@@ -571,6 +571,45 @@ NormBackwardPlan planReduceScatterNormBackward(PeerContext& pc, size_t rows, siz
   return p;
 }
 
+NormBackwardPlan planResidualNormBackward(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm,
+                                          int vectors, AllreduceAlgo algo) {
+  const char* op = "allreduce_residual_norm_backward";
+  if (norm != kNormRms && norm != kNormLayer) GLB_THROW(InputException, op, ": needs a norm (rms or layer)");
+  if (!normSupports(dt)) GLB_THROW(InputException, op, ": rows must be float32, bfloat16 or float16");
+  if (vectors < 0 || vectors > 3) GLB_THROW(InputException, op, ": ", vectors, " vector gradients asked for");
+  if (algo != AllreduceAlgo::AUTO && algo != AllreduceAlgo::ONE_SHOT && algo != AllreduceAlgo::TWO_SHOT) {
+    GLB_THROW(InputException, op, ": algo must be auto, one_shot or two_shot, got ", allreduceAlgoName(algo));
+  }
+  const size_t rowBytes = hidden * elementSize(dt);
+  NormBackwardPlan p;
+  p.variant = kNormLocal;
+  p.chunkRows = std::max<size_t>(rows, 1);
+  if (pc.size > 1) {
+    // auto: the forward's variant for these rows (no LL backward: its LL is the one-shot here);
+    // a one-shot whose rows do not fit a pool half runs as the two-shot, as in the forward.
+    const auto l = layoutOf(pc);
+    int v = algo == AllreduceAlgo::ONE_SHOT ? kNormOneShot : kNormTwoShot;
+    if (algo == AllreduceAlgo::AUTO) v = planResidualNorm(pc, rows, hidden, dt, kNormNone, algo).variant;
+    p.variant = (v == kNormLL || v == kNormOneShot) && roundUp(rows * rowBytes, 16) <= l.half ? kNormOneShot
+                                                                                               : kNormTwoShot;
+    if (p.variant == kNormTwoShot) {
+      if (rowBytes > l.bulkBytes || vectors * hidden * sizeof(float) > l.bulkBytes) {
+        GLB_THROW(InputException, op, ": the pool's bulk region holds no row of ", rowBytes, " bytes or no ",
+                  vectors, " fp32 column sums of ", hidden, "; raise GLB_CUDA_STAGE_MB (CudaContext stage_bytes)");
+      }
+      // One pool row per row: the owner's gradPartial overwrites the staged gradOut.
+      p.chunkRows = std::min(p.chunkRows, l.bulkBytes / rowBytes);
+    }
+  }
+  const void* kernel = normBackwardKernelFor(dt, norm, p.variant);
+  p.blocks = static_cast<int>(std::min<size_t>(
+      p.chunkRows, static_cast<size_t>(pc.coResidentBlocks(kernel, kThreads, normBackwardSmemBytes(vectors)))));
+  p.launches = rows == 0 ? 0 : ceilDiv(rows, p.chunkRows);
+  p.workspaceBytes = vectors > 0 ? static_cast<size_t>(p.blocks) * vectors * hidden * sizeof(float) : 0;
+  if (vectors > 0 && p.launches > 0) p.launches += 1;
+  return p;
+}
+
 const char* normVariantName(int variant) {
   switch (variant) {
     case kNormLL: return "ll";
@@ -666,6 +705,45 @@ void launchNormChunk(PeerContext& pc, const NormArgs& a, const NormXchg& x, Data
   prologue(pc, stream);
   launchAllreduceNorm(pc.comm(), a, x, dt, norm, variant, blocks, stream);
   finish(pc, stream, op);
+}
+
+// The column sums a backward call asks for, in workspace order: vec[kind] is the slot of kind k
+// (0 weight, 1 norm bias, 2 bias; -1: not asked for), out[slot] its output.
+struct VecSlots {
+  int vec[3];
+  int vectors = 0;
+  void* out[3] = {nullptr, nullptr, nullptr};
+};
+VecSlots vecSlots(void* const (&vecOut)[3]) {
+  VecSlots v;
+  for (int k = 0; k < 3; k++) {
+    v.vec[k] = vecOut[k] != nullptr ? v.vectors : -1;
+    if (vecOut[k] != nullptr) v.out[v.vectors++] = vecOut[k];
+  }
+  return v;
+}
+
+// The backward's arguments of one chunk: n rows from `off` bytes into every row tensor.
+NormBwdArgs bwdChunkArgs(const void* gradOut, const void* s, const void* gradS, void* gradResidual, void* gradPartial,
+                         const void* gamma, void* workspace, size_t off, size_t n, size_t hidden, float eps,
+                         const VecSlots& v, bool first) {
+  NormBwdArgs a;
+  a.gradOut = static_cast<const char*>(gradOut) + off;
+  a.s = static_cast<const char*>(s) + off;
+  a.gradS = gradS != nullptr ? static_cast<const char*>(gradS) + off : nullptr;
+  a.gradResidual = gradResidual != nullptr ? static_cast<char*>(gradResidual) + off : nullptr;
+  a.gradPartial = static_cast<char*>(gradPartial) + off;
+  a.gamma = gamma;
+  a.ws = static_cast<float*>(workspace);
+  a.rows = n;
+  a.hidden = hidden;
+  a.eps = eps;
+  a.vectors = v.vectors;
+  a.vecWeight = v.vec[0];
+  a.vecNormBias = v.vec[1];
+  a.vecBias = v.vec[2];
+  a.first = first ? 1 : 0;
+  return a;
 }
 
 }  // namespace
@@ -770,13 +848,8 @@ int reduceScatterResidualNormBackward(PeerContext& pc, const void* gradOut, cons
                 "grad_out, residual_out and grad_partial are required", inputs, outputs, 2);
   GLB_NORM_CHECK(rows % P == 0, rows, " rows do not split into ", P, " equal shards");
   void* const vecOut[3] = {gradWeight, gradNormBias, gradBias};
-  // The requested vectors, in workspace order: vec[kind] is the slot of kind k, wsOut[slot] its output.
-  int vec[3], vectors = 0;
-  void* wsOut[3] = {nullptr, nullptr, nullptr};
-  for (int k = 0; k < 3; k++) {
-    vec[k] = vecOut[k] != nullptr ? vectors : -1;
-    if (vecOut[k] != nullptr) wsOut[vectors++] = vecOut[k];
-  }
+  const VecSlots slots = vecSlots(vecOut);
+  const int vectors = slots.vectors;
   const NormBackwardPlan plan = planReduceScatterNormBackward(pc, rows, hidden, dt, norm, gatherOut, vectors);
   GLB_NORM_CHECK(workspaceBytes >= plan.workspaceBytes, "the workspace of ", workspaceBytes, " bytes is below the ",
                  plan.workspaceBytes, " the plan needs");
@@ -799,23 +872,9 @@ int reduceScatterResidualNormBackward(PeerContext& pc, const void* gradOut, cons
   // Chunk rows [r0, r0 + n) of every shard, as in the forward. The grid of every chunk but a
   // shorter last one is plan.blocks; CTA b carries its column sums in workspace slot b.
   for (size_t r0 = 0; r0 < shard; r0 += plan.chunkRows) {
-    const size_t n = std::min(plan.chunkRows, shard - r0), off = r0 * rb;
-    NormBwdArgs a;
-    a.gradOut = static_cast<const char*>(gradOut) + off;
-    a.s = static_cast<const char*>(s) + off;
-    a.gradS = gradS != nullptr ? static_cast<const char*>(gradS) + off : nullptr;
-    a.gradResidual = gradResidual != nullptr ? static_cast<char*>(gradResidual) + off : nullptr;
-    a.gradPartial = static_cast<char*>(gradPartial) + off;
-    a.gamma = gamma;
-    a.ws = static_cast<float*>(workspace);
-    a.rows = n;
-    a.hidden = hidden;
-    a.eps = eps;
-    a.vectors = vectors;
-    a.vecWeight = vec[0];
-    a.vecNormBias = vec[1];
-    a.vecBias = vec[2];
-    a.first = r0 == 0 ? 1 : 0;
+    const size_t n = std::min(plan.chunkRows, shard - r0);
+    const NormBwdArgs a = bwdChunkArgs(gradOut, s, gradS, gradResidual, gradPartial, gamma, workspace, r0 * rb, n,
+                                       hidden, eps, slots, r0 == 0);
     const size_t gridRows = plan.variant == kNormScatter ? P * n : n;
     const int blocks = static_cast<int>(std::min<size_t>(gridRows, static_cast<size_t>(plan.blocks)));
     prologue(pc, stream);
@@ -824,7 +883,80 @@ int reduceScatterResidualNormBackward(PeerContext& pc, const void* gradOut, cons
   }
   if (vectors > 0) {
     // The first chunk's grid is plan.blocks and wrote every slot; later chunks use a prefix.
-    launchNormBackwardFinish(static_cast<const float*>(workspace), plan.blocks, vectors, hidden, wsOut, dt, stream);
+    launchNormBackwardFinish(static_cast<const float*>(workspace), plan.blocks, vectors, hidden, slots.out, dt, stream);
+    checkLaunch(op);
+  }
+  return plan.variant;
+}
+
+int allreduceResidualNormBackward(PeerContext& pc, const void* gradOut, const void* s, const void* gradS,
+                                  void* gradPartial, const void* gamma, void* gradWeight, void* gradNormBias,
+                                  void* gradBias, void* workspace, size_t workspaceBytes, size_t rows, size_t hidden,
+                                  DataType dt, int norm, float eps, AllreduceAlgo algo, cudaStream_t stream) {
+  GLB_TRACE_RANGE("glb::cuda::allreduceResidualNormBackward");
+  pc.checkHealth();
+  const char* op = "allreduce_residual_norm_backward";
+  GLB_NORM_CHECK(norm == kNormRms || norm == kNormLayer, "needs a norm (rms or layer), got ", norm);
+  GLB_NORM_CHECK(norm == kNormLayer || gradNormBias == nullptr, "grad_norm_bias needs a layer norm");
+  const size_t rb = hidden * elementSize(dt);
+  const NormRange inputs[] = {{"grad_out", gradOut, rows * rb},
+                              {"residual_out", s, rows * rb},
+                              {"grad_residual_out", gradS, rows * rb},
+                              {"weight", gamma, rb}};
+  const NormRange outputs[] = {{"grad_partial", gradPartial, rows * rb}, {"grad_weight", gradWeight, rb},
+                               {"grad_norm_bias", gradNormBias, rb},     {"grad_bias", gradBias, rb},
+                               {"workspace", workspace, workspaceBytes}};
+  checkNormCall(op, dt, norm, hidden, rows == 0 || (gradOut != nullptr && s != nullptr && gradPartial != nullptr),
+                "grad_out, residual_out and grad_partial are required", inputs, outputs, 2);
+  void* const vecOut[3] = {gradWeight, gradNormBias, gradBias};
+  const VecSlots slots = vecSlots(vecOut);
+  const int vectors = slots.vectors;
+  const NormBackwardPlan plan = planResidualNormBackward(pc, rows, hidden, dt, norm, vectors, algo);
+  GLB_NORM_CHECK(workspaceBytes >= plan.workspaceBytes, "the workspace of ", workspaceBytes, " bytes is below the ",
+                 plan.workspaceBytes, " the plan needs");
+  GLB_NORM_CHECK(plan.workspaceBytes == 0 || workspace != nullptr, "the column sums need a workspace");
+  DeviceGuard g(pc.device);
+  if (rows == 0) {
+    // Nothing to sum: the vector gradients are zero.
+    for (void* v : vecOut) {
+      if (v != nullptr) GLB_CUDA_CHECK(cudaMemsetAsync(v, 0, rb, stream));
+    }
+    return plan.variant;
+  }
+  const auto l = layoutOf(pc);
+  NormXchg x{};
+  if (plan.variant == kNormOneShot) {
+    x.peers = pc.stagePtrs(0);
+    x.parityStride = l.half;
+  } else if (plan.variant == kNormTwoShot) {
+    x.peers = pc.stagePtrs(l.bulkOff);
+  }
+  x.mine = x.peers.p[pc.rank];
+  // The grid of every chunk but a shorter last one is plan.blocks; CTA b carries its column sums in
+  // workspace slot b.
+  for (size_t r0 = 0; r0 < rows; r0 += plan.chunkRows) {
+    const size_t n = std::min(plan.chunkRows, rows - r0);
+    const NormBwdArgs a = bwdChunkArgs(gradOut, s, gradS, nullptr, gradPartial, gamma, workspace, r0 * rb, n, hidden,
+                                       eps, slots, r0 == 0);
+    const int blocks = static_cast<int>(std::min<size_t>(n, static_cast<size_t>(plan.blocks)));
+    prologue(pc, stream);
+    launchNormBackward(pc.comm(), a, x, dt, norm, plan.variant, blocks, stream);
+    finish(pc, stream, op);
+  }
+  if (vectors == 0) return plan.variant;
+  const float* ws = static_cast<const float*>(workspace);
+  if (plan.variant == kNormTwoShot) {
+    // The CTA sums cover this rank's rows: a collective finish sums them over the ranks.
+    const int threads = normBackwardFinishThreads();
+    const int blocks = static_cast<int>(std::min<size_t>(
+        ceilDiv(static_cast<size_t>(vectors) * hidden, static_cast<size_t>(threads)),
+        static_cast<size_t>(pc.coResidentBlocks(normBackwardFinishAllreduceKernelFor(dt), threads))));
+    prologue(pc, stream);
+    launchNormBackwardFinishAllreduce(pc.comm(), ws, plan.blocks, vectors, hidden, slots.out, x.peers, dt, blocks,
+                                      stream);
+    finish(pc, stream, op);
+  } else {
+    launchNormBackwardFinish(ws, plan.blocks, vectors, hidden, slots.out, dt, stream);
     checkLaunch(op);
   }
   return plan.variant;

@@ -179,6 +179,29 @@ struct NormBackwardPlan {
 NormBackwardPlan planReduceScatterNormBackward(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm,
                                                bool gatherOut, int vectors);
 
+// The backward of allreduceResidualNorm with a norm (kNormRms / kNormLayer), for training with
+// tensor parallelism (docs/cuda.md, "Backward of the allreduce norm"). Every rank holds all rows of
+// s (the saved residualOut) and gradS (its gradient, null: zero); gradOut is this rank's partial of
+// out's gradient. Per row, in fp32: g = the sum over ranks of gradOut in rank order, the statistics
+// recomputed from s exactly as the forward computed them, gradPartial = round(gradS + the norm's
+// input gradient), the same bytes on every rank and for both variants; it is also the gradient of
+// the residual, and may be gradS itself. Optional column sums over all rows, fp32, rounded once, in
+// a fixed order, the same bytes on every rank: gradWeight = sum g xh, gradNormBias = sum g (layer
+// only), gradBias = sum of the rounded gradPartial rows. They need `workspace` (16-byte aligned, at
+// least the plan's workspaceBytes). rows = 0 launches nothing and zeroes the column sums. algo:
+// AUTO, ONE_SHOT or TWO_SHOT; one rank runs a local launch. Invalid arguments raise InputException
+// before anything is launched. Returns the NormVariant.
+int allreduceResidualNormBackward(PeerContext& pc, const void* gradOut, const void* s, const void* gradS,
+                                  void* gradPartial, const void* gamma, void* gradWeight, void* gradNormBias,
+                                  void* gradBias, void* workspace, size_t workspaceBytes, size_t rows, size_t hidden,
+                                  DataType dt, int norm, float eps, AllreduceAlgo algo, cudaStream_t stream);
+// Its variant (kNormOneShot, kNormTwoShot or kNormLocal; AUTO takes the forward's variant for these
+// rows, its LL as the one-shot), chunk rows (the two-shot stages one pool row per row), launches
+// (chunks, plus one that finishes the column sums when `vectors` > 0), grid and workspace, as
+// planReduceScatterNormBackward reports them.
+NormBackwardPlan planResidualNormBackward(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm,
+                                          int vectors, AllreduceAlgo algo);
+
 
 // ---- data movement -------------------------------------------------------------------
 // `buf`/`out` arguments are registered or symmetric buffers; plain-pointer

@@ -101,6 +101,9 @@ void launchAllreduceNorm(const CommArgs& a, const NormArgs& n, const NormXchg& x
 // apart. gradS / gradResidual / gamma may be null. ws: per-CTA fp32 column sums, [CTA][vectors]
 // [hidden]; vecWeight / vecNormBias / vecBias index the vectors (-1: not asked for). `first`: the
 // first chunk starts the sums from zero, later chunks from ws.
+// The allreduce forms (kNormOneShot: x as the forward's one-shot; kNormTwoShot: x.peers the bulk
+// regions) take `rows` rows of s, gradS, gradOut (this rank's partial) and gradPartial; gradResidual
+// is unused.
 struct NormBwdArgs {
   const void* gradOut;
   const void* s;
@@ -127,6 +130,15 @@ void launchNormBackward(const CommArgs& a, const NormBwdArgs& n, const NormXchg&
 // out is non-null (outs in the order of ws's vectors).
 void launchNormBackwardFinish(const float* ws, int slots, int vectors, size_t hidden, void* const (&outs)[3],
                               DataType dt, cudaStream_t stream);
+// The same for the two-shot allreduce backward, whose slots hold this rank's rows only: a collective
+// that stages this rank's fp32 sums at pool.p[rank] (vectors x hidden floats), sums the P staged
+// vectors in rank order and rounds once, the same bytes on every rank. Every rank launches the same
+// co-resident grid of normBackwardFinishThreads() threads per CTA.
+const void* normBackwardFinishAllreduceKernelFor(DataType dt);
+int normBackwardFinishThreads();
+void launchNormBackwardFinishAllreduce(const CommArgs& a, const float* ws, int slots, int vectors, size_t hidden,
+                                       void* const (&outs)[3], const PeerPtrs& pool, DataType dt, int blocks,
+                                       cudaStream_t stream);
 
 // pipeline_kernels.cu — arbitrary pointers through the pool, in-kernel pipelines (allreduce:
 // 3 stages).

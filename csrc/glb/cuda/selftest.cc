@@ -152,9 +152,13 @@ std::string checkScatterNorm(const CommArgs& ca, const NormXchg& x, int norm, si
 // shard 0; with a gather its virtual peers staged the same grad_out rows, so g = P grad_out. Checks
 // grad_residual, rank 0's rows of grad_partial and the weight, norm bias and bias column sums
 // against a CPU double-precision row.
+// The allreduce forms (kNormOneShot / kNormTwoShot) take `rows` rows of every tensor, and their
+// virtual peers staged the same grad_out, so g = P grad_out; they write grad_partial only. The
+// one-shot computes every row and sums; the two-shot rank 0's share of the rows, and its collective
+// finish sums P staged copies of rank 0's column sums.
 std::string checkNormBackward(const CommArgs& ca, const NormXchg& x, int variant, int norm, size_t rows, size_t H,
                               int blocks, cudaStream_t st) {
-  const bool scatter = variant == kNormScatter;
+  const bool scatter = variant == kNormScatter, tp = variant == kNormOneShot || variant == kNormTwoShot;
   const size_t all = scatter ? ca.nranks * x.shardRows : rows, outRows = scatter && x.gather ? all : rows;
   const int vectors = norm == kNormLayer ? 3 : 2;
   DevBuf gradOut(outRows * H * 4), sv(rows * H * 4), gs(rows * H * 4), gr(rows * H * 4), gp(all * H * 4),
@@ -167,7 +171,7 @@ std::string checkNormBackward(const CommArgs& ca, const NormXchg& x, int variant
   a.gradOut = gradOut.p;
   a.s = sv.p;
   a.gradS = gs.p;
-  a.gradResidual = gr.p;
+  a.gradResidual = tp ? nullptr : gr.p;
   a.gradPartial = gp.p;
   a.gamma = gamma.p;
   a.ws = static_cast<float*>(ws.p);
@@ -183,13 +187,21 @@ std::string checkNormBackward(const CommArgs& ca, const NormXchg& x, int variant
   float* v = static_cast<float*>(vecs.p);
   void* const outs[3] = {v, norm == kNormLayer ? v + H : nullptr, v + 2 * H};
   void* const packed[3] = {outs[0], outs[1] != nullptr ? outs[1] : outs[2], outs[1] != nullptr ? outs[2] : nullptr};
-  launchNormBackwardFinish(a.ws, blocks, vectors, H, packed, DataType::FLOAT32, st);
+  if (variant == kNormTwoShot) {
+    launchNormBackwardFinishAllreduce(ca, a.ws, blocks, vectors, H, packed, x.peers, DataType::FLOAT32, 2, st);
+  } else {
+    launchNormBackwardFinish(a.ws, blocks, vectors, H, packed, DataType::FLOAT32, st);
+  }
   noteLaunch(2);
-  const auto r = download(gr.p, rows * H, st), p = download(gp.p, all * H, st), go = download(gradOut.p, outRows * H, st);
+  const auto p = download(gp.p, all * H, st), go = download(gradOut.p, outRows * H, st);
+  const auto r = tp ? p : download(gr.p, rows * H, st);
   const auto vw = download(v, H, st), vnb = download(v + H, H, st), vb = download(v + 2 * H, H, st);
-  const double mult = scatter && x.gather ? ca.nranks : 1;
+  const double mult = (scatter && x.gather) || tp ? ca.nranks : 1;
+  const double vmult = variant == kNormTwoShot ? ca.nranks : 1;
+  size_t rb = 0, re = rows;
+  if (variant == kNormTwoShot) shareOfHost(rows, ca.nranks, 0, rb, re);
   std::vector<double> sw(H, 0), snb(H, 0), sb(H, 0), aw(H, 0), anb(H, 0), ab(H, 0);
-  for (size_t i = 0; i < rows; i++) {
+  for (size_t i = rb; i < re; i++) {
     std::vector<double> xs(H), g(H);
     double mean = 0, sq = 0, mg = 0, mgx = 0, scale = 0;
     for (size_t j = 0; j < H; j++) {
@@ -225,6 +237,9 @@ std::string checkNormBackward(const CommArgs& ca, const NormXchg& x, int variant
       sb[j] += r[i * H + j];
       ab[j] += std::fabs(r[i * H + j]);
     }
+  }
+  for (auto* acc : {&sw, &snb, &sb, &aw, &anb, &ab}) {
+    for (double& e : *acc) e *= vmult;
   }
   for (size_t j = 0; j < H; j++) {
     if (std::fabs(vw[j] - sw[j]) > 1e-4 * aw[j] + 1e-6) return strcat_all("grad_weight[", j, "]: got ", vw[j], " want ", sw[j]);
@@ -479,6 +494,19 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
             x.shardRows = 5;
             x.gather = gather;
             return checkNormBackward(ca, x, kNormScatter, norm, 3, H, 3, stream);
+          });
+        }
+      }
+      // the allreduce form's backward (tensor parallelism): one-shot and row-sharded two-shot
+      for (int variant : {kNormOneShot, kNormTwoShot}) {
+        for (int norm : {kNormRms, kNormLayer}) {
+          R.run(strcat_all("normBackwardKernel<float,", norms[norm], ",", normVariantName(variant), "> P=", P),
+                [&]() -> std::string {
+            NormXchg x{};
+            for (int r = 0; r < P; r++) x.peers.p[r] = myStage + (variant == kNormOneShot ? 0 : 2 * half);
+            x.mine = x.peers.p[0];
+            x.parityStride = half;
+            return checkNormBackward(ca, x, variant, norm, rows, H, 3, stream);
           });
         }
       }

@@ -281,6 +281,40 @@ void registerCuda(py::module_& root) {
     return d;
   }, py::arg("pc"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"), py::arg("gather_out") = true,
      py::arg("vectors") = 0);
+  m.def("allreduce_residual_norm_backward", [](PeerContext& pc, uintptr_t gradOut, uintptr_t s, uintptr_t gradS,
+                                               uintptr_t gradPartial, uintptr_t gamma, uintptr_t gradWeight,
+                                               uintptr_t gradNormBias, uintptr_t gradBias, uintptr_t workspace,
+                                               size_t workspaceBytes, size_t rows, size_t hidden, int dtype, int norm,
+                                               double eps, int algo, uintptr_t stream) {
+    int v;
+    {
+      py::gil_scoped_release nogil;
+      v = allreduceResidualNormBackward(pc, P(gradOut), P(s), P(gradS), P(gradPartial), P(gamma), P(gradWeight),
+                                        P(gradNormBias), P(gradBias), P(workspace), workspaceBytes, rows, hidden,
+                                        static_cast<DataType>(dtype), norm, static_cast<float>(eps),
+                                        static_cast<AllreduceAlgo>(algo), S(stream));
+    }
+    return std::string(normVariantName(v));
+  }, py::arg("pc"), py::arg("grad_out"), py::arg("residual_out"), py::arg("grad_residual_out"),
+     py::arg("grad_partial"), py::arg("weight"), py::arg("grad_weight"), py::arg("grad_norm_bias"),
+     py::arg("grad_bias"), py::arg("workspace"), py::arg("workspace_bytes"), py::arg("rows"), py::arg("hidden"),
+     py::arg("dtype"), py::arg("norm"), py::arg("eps"), py::arg("algo") = 0, py::arg("stream") = 0,
+     "Backward of allreduce_residual_norm with a norm (1 rms, 2 layer): allreduce of this rank's partial grad_out, "
+     "the norm's backward and the add of grad_residual_out into grad_partial, in one kernel; optional column sums "
+     "(weight, norm bias, bias) need the plan's workspace. Null pointers are 0. Returns the variant that ran.");
+  m.def("plan_residual_norm_backward", [](PeerContext& pc, size_t rows, size_t hidden, int dtype, int norm,
+                                          int vectors, int algo) {
+    const NormBackwardPlan p = planResidualNormBackward(pc, rows, hidden, static_cast<DataType>(dtype), norm, vectors,
+                                                        static_cast<AllreduceAlgo>(algo));
+    py::dict d;
+    d["variant"] = std::string(normVariantName(p.variant));
+    d["chunk_rows"] = p.chunkRows;
+    d["launches"] = p.launches;
+    d["blocks"] = p.blocks;
+    d["workspace_bytes"] = p.workspaceBytes;
+    return d;
+  }, py::arg("pc"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"), py::arg("vectors"),
+     py::arg("algo") = 0);
   m.attr("MAX_NORM_HIDDEN") = kMaxNormHidden;
 
   m.def("plan_allreduce", [](PeerContext& pc, size_t bytes, int dtype, int op, int kind) {

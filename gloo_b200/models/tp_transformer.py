@@ -87,8 +87,12 @@ class TPBlock(nn.Module):
         a = a.transpose(1, 2).reshape(B, S, self.local_heads * hd)
         if x.is_cuda:
             # each row-parallel output: allreduce + bias + residual add (+ ln2) in one kernel
-            x, h = self.tp.reduce_residual_norm(nn.functional.linear(a, self.proj.weight), x, self.ln2, self.proj.bias)
-            p = nn.functional.linear(nn.functional.gelu(self.up(h)), self.down.weight)
+            # copy_out: h's gradient is allreduced inside the fused backward, so self.up(h)'s
+            # copy_to_region would count it P times.
+            x, h = self.tp.reduce_residual_norm(nn.functional.linear(a, self.proj.weight), x, self.ln2, self.proj.bias,
+                                                copy_out=True)
+            h = nn.functional.linear(h, self.up.weight, self.up.bias)
+            p = nn.functional.linear(nn.functional.gelu(h), self.down.weight)
             return self.tp.reduce_residual_norm(p, x, None, self.down.bias)
         x = x + self.proj(a)
         return x + self.down(nn.functional.gelu(self.up(self.ln2(x))))

@@ -378,23 +378,92 @@ class CudaContext:
         vectors = sum(t is not None for t in (grad_weight, grad_norm_bias, grad_bias))
         plan = _cu.plan_reduce_scatter_norm_backward(self.pc, rows, H, int(dt), kinds[norm], bool(gather_out), vectors)
         launch = _stream(stream)
-        ws = None
-        if plan["workspace_bytes"]:
-            # The workspace is this call's own temporary: allocate it on the stream the kernels run
-            # on, so that the caching allocator reuses it only for work ordered after them.
-            dev = residual_out.device
-            if launch == torch.cuda.current_stream(dev).cuda_stream:
-                ws = torch.empty(plan["workspace_bytes"], dtype=torch.uint8, device=dev)
-            else:
-                on = stream if isinstance(stream, torch.cuda.Stream) else torch.cuda.ExternalStream(launch, device=dev)
-                with torch.cuda.stream(on):
-                    ws = torch.empty(plan["workspace_bytes"], dtype=torch.uint8, device=dev)
+        ws = self._norm_workspace(plan["workspace_bytes"], residual_out.device, stream, launch)
         ptr = lambda t: 0 if t is None else t.data_ptr()  # noqa: E731
         _cu.reduce_scatter_residual_norm_backward(
             self.pc, ptr(grad_out), ptr(residual_out), ptr(grad_residual_out), ptr(grad_residual), ptr(grad_partial),
             ptr(weight), ptr(grad_weight), ptr(grad_norm_bias), ptr(grad_bias), ptr(ws),
             0 if ws is None else ws.numel(), rows, H, int(dt), kinds[norm], float(eps), bool(gather_out), launch)
         return grad_partial, grad_residual, grad_weight, grad_norm_bias, grad_bias
+
+    def allreduce_residual_norm_backward(self, grad_out, residual_out, grad_residual_out=None, weight=None, *,
+                                         norm: str, eps: float = 1e-6, grad_partial=None, grad_weight=None,
+                                         grad_norm_bias=None, grad_bias=None, algo: str = "auto", stream=None):
+        """The backward of :meth:`allreduce_residual_norm` with a norm, in ONE kernel launch per
+        chunk: the allreduce of this rank's partial of ``out``'s gradient, the norm's backward and
+        the add of ``residual_out``'s gradient.
+
+        ``residual_out`` is the forward's saved output ``(T, ...)``, the same on every rank;
+        ``grad_residual_out`` its gradient (None counts as zero), also the same on every rank;
+        ``grad_out`` this rank's partial of the gradient of ``out``, ``(T, ...)``. ``norm``, ``eps``
+        and ``weight`` are the forward's. Per row, in fp32, with ``g`` the sum over ranks of
+        ``grad_out`` (rank order) and the statistics recomputed exactly as the forward computed
+        them: ``grad_partial = round(grad_residual_out + the norm's input gradient)``, the gradient
+        of both ``partial`` and ``residual``, the same bytes on every rank and for every ``algo``.
+        It may be ``grad_residual_out`` itself and is allocated when not given. ``grad_weight`` (sum
+        of ``g * xhat``), ``grad_norm_bias`` (sum of ``g``, layer only) and ``grad_bias`` (sum of the
+        rounded ``grad_partial`` rows) are column sums over all rows, fp32, rounded once, in a fixed
+        order, the same bytes on every rank: each is computed into the ``(H,)`` tensor given and
+        skipped when None. The fp32 workspace they need comes from torch's allocator, on the stream
+        the call runs on. ``algo``: ``"auto"`` (the forward's choice for these rows, its LL as the
+        one-shot), ``"one_shot"`` or ``"two_shot"``. Invalid arguments raise ``ValueError`` before
+        anything is launched.
+
+        Returns ``(grad_partial, grad_weight, grad_norm_bias, grad_bias)``."""
+        import torch
+
+        kinds = {"rms": 1, "layer": 2}
+        name = "allreduce_residual_norm_backward"
+        if norm not in kinds:
+            raise ValueError(f"{name}: norm must be 'rms' or 'layer', got {norm!r}")
+        if algo not in ("auto", "one_shot", "two_shot"):
+            raise ValueError(f"{name}: algo must be auto, one_shot or two_shot, got {algo!r}")
+        if norm != "layer" and grad_norm_bias is not None:
+            raise ValueError(f"{name}: grad_norm_bias needs norm='layer'")
+        if residual_out.dim() == 0:
+            raise ValueError(f"{name}: residual_out must have a hidden dimension")
+        H = residual_out.shape[-1]
+        if grad_partial is None:
+            grad_partial = torch.empty_like(residual_out, memory_format=torch.contiguous_format)
+        named = {"grad_out": grad_out, "residual_out": residual_out, "grad_residual_out": grad_residual_out,
+                 "weight": weight, "grad_partial": grad_partial, "grad_weight": grad_weight,
+                 "grad_norm_bias": grad_norm_bias, "grad_bias": grad_bias}
+        for key, t in named.items():
+            if t is None:
+                continue
+            if not t.is_cuda or t.dtype != residual_out.dtype or not t.is_contiguous():
+                raise ValueError(f"{name}: {key} must be a contiguous CUDA tensor of {residual_out.dtype}, "
+                                 f"got {t.dtype} on {t.device}{'' if t.is_contiguous() else ', not contiguous'}")
+            want = (H,) if key in ("weight", "grad_weight", "grad_norm_bias", "grad_bias") else tuple(residual_out.shape)
+            if tuple(t.shape) != want:
+                raise ValueError(f"{name}: {key} has shape {tuple(t.shape)}, expected {want}")
+        _, _, dt, _ = describe(residual_out)
+        rows = residual_out.numel() // max(H, 1)
+        vectors = sum(t is not None for t in (grad_weight, grad_norm_bias, grad_bias))
+        plan = _cu.plan_residual_norm_backward(self.pc, rows, H, int(dt), kinds[norm], vectors, _algo(algo))
+        launch = _stream(stream)
+        ws = self._norm_workspace(plan["workspace_bytes"], residual_out.device, stream, launch)
+        ptr = lambda t: 0 if t is None else t.data_ptr()  # noqa: E731
+        _cu.allreduce_residual_norm_backward(
+            self.pc, ptr(grad_out), ptr(residual_out), ptr(grad_residual_out), ptr(grad_partial), ptr(weight),
+            ptr(grad_weight), ptr(grad_norm_bias), ptr(grad_bias), ptr(ws), 0 if ws is None else ws.numel(), rows, H,
+            int(dt), kinds[norm], float(eps), _algo(algo), launch)
+        return grad_partial, grad_weight, grad_norm_bias, grad_bias
+
+    @staticmethod
+    def _norm_workspace(nbytes, dev, stream, launch):
+        """The column sums' fp32 workspace of a norm backward, or None: a temporary of the call,
+        allocated on the stream its kernels run on, so that the caching allocator reuses it only for
+        work ordered after them."""
+        import torch
+
+        if not nbytes:
+            return None
+        if launch == torch.cuda.current_stream(dev).cuda_stream:
+            return torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        on = stream if isinstance(stream, torch.cuda.Stream) else torch.cuda.ExternalStream(launch, device=dev)
+        with torch.cuda.stream(on):
+            return torch.empty(nbytes, dtype=torch.uint8, device=dev)
 
     # ---- health ---------------------------------------------------------------------------
     def set_timeout(self, ms: int):

@@ -459,7 +459,7 @@ class TensorParallel(_Base):
 
         return _G.apply(x)
 
-    def reduce_residual_norm(self, partial, residual, norm_module=None, bias=None):
+    def reduce_residual_norm(self, partial, residual, norm_module=None, bias=None, copy_out: bool = False):
         """g fused with what follows a row-parallel matmul: ``s = allreduce(partial) + bias +
         residual`` and the next norm. Returns ``(s, norm_module(s))``, or ``s`` when
         ``norm_module`` is None. ``norm_module`` is an ``nn.LayerNorm``, an ``nn.RMSNorm`` or None.
@@ -469,16 +469,29 @@ class TensorParallel(_Base):
         gradient of ``s`` plus the norm's input gradient (recomputed from the saved ``s``) goes to
         both ``partial`` and ``residual``, its row sum to ``bias``, and the norm's weights get
         theirs from the recompute. Anything else runs ``reduce_from_region``, ``+ bias``,
-        ``+ residual`` and the module."""
+        ``+ residual`` and the module.
+
+        ``copy_out``: ``out`` is returned inside the tensor-parallel region, as
+        ``copy_to_region(norm_module(s))`` (Megatron's f, fused; it needs a norm). The gradient of
+        ``out`` that reaches the backward is then this rank's partial, which the backward
+        allreduces. After a fused forward that is one fused kernel
+        (``CudaContext.allreduce_residual_norm_backward``), which gives every rank the same bytes of
+        every gradient and computes only the vector gradients autograd needs; a gradient it cannot
+        take (dtype, alignment) is allreduced and the norm recomputed with torch."""
         import torch
 
+        if copy_out and norm_module is None:
+            raise ValueError("reduce_residual_norm: copy_out needs a norm_module")
         kind, weight, norm_bias, eps = _norm_parts(norm_module, partial.dtype)
         if not self._fusable(partial, residual, norm_module, kind, (bias, weight, norm_bias)):
             y = self.reduce_from_region(partial)
             if bias is not None:
                 y = y + bias
             s = y + residual
-            return s if norm_module is None else (s, norm_module(s))
+            if norm_module is None:
+                return s
+            out = norm_module(s)
+            return s, (self.copy_to_region(out) if copy_out else out)
         H = partial.shape[-1]
         tp = self
 
@@ -495,6 +508,16 @@ class TensorParallel(_Base):
             @staticmethod
             def backward(ctx, grad_s, grad_out=None):
                 s, w, nb = ctx.saved_tensors
+                if copy_out and grad_out is not None:
+                    if _aligned_like(s, grad_out, grad_s):
+                        need_b, need_w, need_nb = ctx.needs_input_grad[2:5]
+                        vec = lambda t, need: torch.empty(H, dtype=s.dtype, device=s.device) if t and need else None  # noqa: E731
+                        gp, gw, gnb, gb = tp.cc.allreduce_residual_norm_backward(
+                            grad_out.contiguous(), s, None if grad_s is None else grad_s.contiguous(), w, norm=kind,
+                            eps=eps, grad_weight=vec(w is not None, need_w), grad_norm_bias=vec(nb is not None, need_nb),
+                            grad_bias=vec(ctx.has_bias, need_b))
+                        return gp, gp, gb, gw, gnb
+                    grad_out = tp._allreduce(grad_out.contiguous().clone())
                 grad_s = torch.zeros_like(s) if grad_s is None else grad_s
                 gw = gnb = None
                 if kind is not None and grad_out is not None:

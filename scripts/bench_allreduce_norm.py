@@ -15,6 +15,14 @@ Time per call: CUDA events around `--iters` back-to-back calls after `--warmup` 
 `--reps` windows, the maximum over ranks. Launches per call: the library's launch counter for the
 fused path, kernels counted by torch.profiler for the unfused one (one rank per process only). Prints one JSON document and
 writes it to `--out` when given.
+
+`--backward` times the fused backward instead (`CudaContext.allreduce_residual_norm_backward`: the
+allreduce of out's gradient, the norm's backward and the add of the residual stream's gradient, one
+kernel per chunk plus one that finishes the column sums), with algo auto, one_shot and two_shot,
+against the composition TensorParallel's autograd runs without it: clone + `cc.allreduce` of out's
+gradient, the norm recomputed under torch autograd, the add and the bias row sum. bf16, with weight
+and bias gradients (and the norm bias for layer); T on both sides of the one-shot / two-shot
+threshold. Before timing, each shape records how far the two gradients of `partial` lie apart.
 """
 import argparse
 import json
@@ -29,6 +37,7 @@ import torch.nn.functional as F  # noqa: E402
 
 import gloo_b200 as gb  # noqa: E402
 from gloo_b200.ops import cuda as gcu  # noqa: E402
+from gloo_b200.parallel.strategies import _norm_input_grad  # noqa: E402
 
 DECODE_T = (1, 8, 32, 128)
 PREFILL_T = (4096,)
@@ -97,6 +106,61 @@ def bench_rank(ctx, device, args, world, profile_unfused=True):
     return rows
 
 
+BACKWARD_T = (8, 32, 128, 1024, 4096)
+
+
+def bench_backward_rank(ctx, device, args, world):
+    cc = gcu.CudaContext(ctx, device, stage_bytes=args.stage_mb << 20)
+    cc.set_timeout(600000)
+    stream = torch.cuda.current_stream()
+    dtype, rank = torch.bfloat16, ctx.rank
+    rows = []
+    for H in HIDDEN:
+        for T in BACKWARD_T:
+            g = torch.Generator(device="cpu").manual_seed(T * 131 + H)
+            s = torch.randn(T, H, generator=g).to(dtype).cuda()
+            g_s = torch.randn(T, H, generator=g).to(dtype).cuda()
+            weight = (1 + 0.1 * torch.randn(H, generator=g)).to(dtype).cuda()
+            norm_bias = (0.1 * torch.randn(H, generator=g)).to(dtype).cuda()
+            g_out = torch.randn(T, H, generator=torch.Generator().manual_seed(T * 131 + H + 7 + rank)).to(dtype).cuda()
+            gp = torch.empty(T, H, dtype=dtype, device="cuda")
+            gw, gnb, gb_ = (torch.empty(H, dtype=dtype, device="cuda") for _ in range(3))
+            for norm in ("rms", "layer"):
+                nb = norm_bias if norm == "layer" else None
+
+                def fused(algo):
+                    return lambda: cc.allreduce_residual_norm_backward(
+                        g_out, s, g_s, weight, norm=norm, eps=1e-6, grad_partial=gp, grad_weight=gw,
+                        grad_norm_bias=gnb if norm == "layer" else None, grad_bias=gb_, algo=algo)
+
+                def composed():
+                    y = g_out.clone()
+                    cc.allreduce(y)
+                    gs, _, _ = _norm_input_grad(norm, H, 1e-6, s, weight, nb, y)
+                    total = g_s + gs
+                    total.sum(0)
+                    return total
+
+                fused("auto")()
+                ref = composed()
+                torch.cuda.synchronize()
+                vectors = 3 if norm == "layer" else 2
+                row = {"T": T, "H": H, "dtype": "bfloat16", "norm": norm, "bytes": T * H * 2,
+                       "max_abs_diff_composed": float((gp.float() - ref.float()).abs().max()),
+                       "max_abs_grad": float(ref.float().abs().max())}
+                for algo in ("auto", "one_shot", "two_shot"):
+                    plan = gb._C.cuda.plan_residual_norm_backward(cc.pc, T, H, int(gb.DataType.BFLOAT16),
+                                                                  {"rms": 1, "layer": 2}[norm], vectors,
+                                                                  gcu.ALGOS[algo])
+                    row[f"{algo}_variant"] = plan["variant"]
+                    row[f"{algo}_launches"] = plan["launches"]
+                    row[f"{algo}_us"] = timed(ctx, cc, fused(algo), stream, args, world)
+                row["composed_us"] = timed(ctx, cc, composed, stream, args, world)
+                row["speedup"] = row["composed_us"] / row["auto_us"]
+                rows.append(row)
+    return rows
+
+
 def timed(ctx, cc, fn, stream, args, world):
     for _ in range(args.warmup):
         fn()
@@ -153,11 +217,12 @@ def main():
     ap.add_argument("--warmup", type=int, default=50)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--stage-mb", type=int, default=128)
+    ap.add_argument("--backward", action="store_true", help="time the fused backward against its composition")
     args = ap.parse_args()
     if args.threads:
         world = args.threads
-        rows = gb.spawn_threads(world, lambda ctx: bench_rank(ctx, 0, args, 1, False), cuda_device=0,
-                               timeout_ms=600000)[0]
+        run = bench_backward_rank if args.backward else lambda ctx, dev, a, w: bench_rank(ctx, dev, a, w, False)
+        rows = gb.spawn_threads(world, lambda ctx: run(ctx, 0, args, 1), cuda_device=0, timeout_ms=600000)[0]
         mode = f"{world} ranks as threads on one GPU: overhead only, not link numbers"
         info = gpu_info(0)
         rank = 0
@@ -167,11 +232,11 @@ def main():
         torch.cuda.set_device(local)
         ctx = gb.init_context(rank, world, path=f"/tmp/glb_norm_{os.environ.get('MASTER_PORT', '0')}_{os.getppid()}",
                               timeout_ms=120000)
-        rows = bench_rank(ctx, local, args, world)
+        rows = (bench_backward_rank if args.backward else bench_rank)(ctx, local, args, world)
         mode = f"{world} ranks, one per GPU"
         info = gpu_info(local)
     if rank == 0:
-        doc = {"benchmark": "allreduce_residual_norm", "mode": mode, "ranks": world, **info, "iters": args.iters,
+        doc = {"benchmark": "allreduce_residual_norm" + ("_backward" if args.backward else ""), "mode": mode, "ranks": world, **info, "iters": args.iters,
                "warmup": args.warmup, "reps": args.reps, "rows": rows}
         text = json.dumps(doc)
         print(text)

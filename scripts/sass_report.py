@@ -56,6 +56,10 @@ KERNELS = [
     ("reduce_scatter_norm_bf16_rms", r"allreduceNormKernel<__nv_bfloat16, 1, 4>"),
     ("reduce_scatter_norm_f32_layer", r"allreduceNormKernel<float, 2, 4>"),
     ("reduce_scatter_norm_backward_bf16_rms", r"normBackwardKernel<__nv_bfloat16, 1, 4>"),
+    ("allreduce_norm_backward_bf16_rms_one_shot", r"normBackwardKernel<__nv_bfloat16, 1, 1>"),
+    ("allreduce_norm_backward_bf16_rms_two_shot", r"normBackwardKernel<__nv_bfloat16, 1, 2>"),
+    ("allreduce_norm_backward_f32_layer_two_shot", r"normBackwardKernel<float, 2, 2>"),
+    ("allreduce_norm_backward_finish_bf16", r"normBackwardFinishAllreduceKernel<__nv_bfloat16>"),
     ("p2p_sendrecv", r"p2pKernel"),
     ("exchange_zero_copy", r"exchangeKernel<false>"),
     ("exchange_zero_copy_tma", r"exchangeKernel<true>"),
