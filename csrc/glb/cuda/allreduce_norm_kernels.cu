@@ -29,6 +29,12 @@
 //             bulk region, barrier, rank r reduces the rows of shard r and writes residualOut
 //             (and an ungathered out) straight to its own tensors; with `gather` it stores out
 //             into every peer's pool, barrier, and every rank copies all P shards of out.
+//
+// The quantising form (Q, with a norm): out is e4m3 codes (rows, H) and n.outScales one fp32 scale
+// per row. The epilogue rounds each out value to T (the bytes the unquantised form writes), takes
+// the row's amax with one more block reduction and stores quantAmax / e4m3Multiplier codes and the
+// e4m3Scale (device_common.cuh) from the registers. What the two-shot and the gathered scatter
+// exchange is then H code bytes and one scale per row instead of an H-element row of T.
 #include "glb/cuda/device_common.cuh"
 #include "glb/cuda/kernels.h"
 
@@ -57,6 +63,49 @@ __device__ __forceinline__ float blockSum(float v, float* sh) {
 #pragma unroll
   for (int w = 0; w < kThreads / 32; w++) s += sh[w];
   return s;
+}
+
+// gridDim.x read again where used (a volatile read of %nctaid.x) rather than held across the row
+// loop, where it would spill at the widest rows (fp32 LayerNorm).
+__device__ __forceinline__ unsigned gridCtas() {
+  unsigned n;
+  asm volatile("mov.u32 %0, %%nctaid.x;" : "=r"(n));
+  return n;
+}
+
+// Max of v over the CTA, the same value on every thread; blockSum's order.
+__device__ __forceinline__ float blockMax(float v, float* sh) {
+#pragma unroll
+  for (int d = 16; d >= 1; d /= 2) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, d));
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float m = 0.0f;
+#pragma unroll
+  for (int w = 0; w < kThreads / 32; w++) m = fmaxf(m, sh[w]);
+  return m;
+}
+
+// The e4m3 codes of one pack of T (kE elements, kE bytes: a uint32_t for float, a uint2 for the
+// 16-bit types), and their store at `p`.
+template <typename T>
+using QCodes = typename std::conditional<NormRow<T>::kE == 8, uint2, uint32_t>::type;
+__device__ __forceinline__ void stCodes(char* p, uint32_t c) { *reinterpret_cast<uint32_t*>(p) = c; }
+__device__ __forceinline__ void stCodes(char* p, uint2 c) { *reinterpret_cast<uint2*>(p) = c; }
+
+template <typename T>
+__device__ __forceinline__ QCodes<T> packCodes(const typename NormRow<T>::Acc& x, float multiplier) {
+  uint32_t w[NormRow<T>::kE / 4];
+#pragma unroll
+  for (int i = 0; i < NormRow<T>::kE / 4; i++) {
+    w[i] = e4m3Codes2(x.v[4 * i], x.v[4 * i + 1], multiplier) |
+           (e4m3Codes2(x.v[4 * i + 2], x.v[4 * i + 3], multiplier) << 16);
+  }
+  if constexpr (NormRow<T>::kE == 8) {
+    return make_uint2(w[0], w[1]);
+  } else {
+    return w[0];
+  }
 }
 
 __device__ __forceinline__ const char* rowPtr(const void* base, size_t row, size_t rowBytes) {
@@ -108,10 +157,12 @@ __device__ __forceinline__ void rowStats(const typename NormRow<T>::Acc (&x)[Nor
 
 // The row epilogue on the reduced partials `acc` of row `row`: adds bias and residual, rounds
 // once, and hands each pack of residualOut and out to store(k, resid, out). `npacks` packs per
-// row; pack k of this thread is t + k * kThreads.
-template <typename T, int NORM, typename Store>
+// row; pack k of this thread is t + k * kThreads. Q (with a norm): store's out is to be dropped;
+// the row's codes go to storeQ(pk, codes, scale) once its amax is known, pack by pack, and the
+// thread that has pack 0 stores the scale.
+template <typename T, int NORM, bool Q, typename Store, typename StoreQ>
 __device__ __forceinline__ void rowEpilogue(typename NormRow<T>::Acc (&acc)[NormRow<T>::kPacks], const NormArgs& n,
-                                            size_t row, int npacks, float* sh, Store&& store) {
+                                            size_t row, int npacks, float* sh, Store&& store, StoreQ&& storeQ) {
   using R = NormRow<T>;
   using PT = typename R::PT;
   const int t = threadIdx.x;
@@ -130,7 +181,7 @@ __device__ __forceinline__ void rowEpilogue(typename NormRow<T>::Acc (&acc)[Norm
     }
   }
   if constexpr (NORM != kNormNone) {
-    float mean, rinv;
+    float mean, rinv, absMax = 0.0f;
     rowStats<T, NORM>(acc, sum, npacks, n.eps, sh, mean, rinv);
 #pragma unroll
     for (int k = 0; k < R::kPacks; k++) {
@@ -147,7 +198,24 @@ __device__ __forceinline__ void rowEpilogue(typename NormRow<T>::Acc (&acc)[Norm
           if (NORM == kNormLayer && n.beta != nullptr) y += b.v[e];
           acc[k].v[e] = y;
         }
-        store(pk, r, PT::narrow(acc[k]));
+        if constexpr (Q) {
+          const Pack16 o = PT::narrow(acc[k]);
+          store(pk, r, o);
+          acc[k] = PT::widen(o);  // out as the unquantised form writes it
+#pragma unroll
+          for (int e = 0; e < R::kE; e++) absMax = fmaxf(absMax, fabsf(acc[k].v[e]));
+        } else {
+          store(pk, r, PT::narrow(acc[k]));
+        }
+      }
+    }
+    if constexpr (Q) {
+      const float amax = quantAmax(blockMax(absMax, sh));
+      const float mul = e4m3Multiplier(amax), scale = e4m3Scale(amax);
+#pragma unroll
+      for (int k = 0; k < R::kPacks; k++) {
+        const int pk = t + k * kThreads;
+        if (pk < npacks) storeQ(pk, packCodes<T>(acc[k], mul), scale);
       }
     }
   }
@@ -178,8 +246,8 @@ __device__ __forceinline__ void copyRow(char* dst, const char* src, int npacks) 
   for (int pk = threadIdx.x; pk < npacks; pk += kThreads) st128(dst + pk * 16, ld128(src + pk * 16));
 }
 
-// Row i of the problem is handled by CTA i % gridDim.x of every rank.
-template <typename T, int NORM, int V>
+// Row i of the problem is handled by CTA i % gridDim.x of every rank. Q: the quantising form.
+template <typename T, int NORM, int V, bool Q>
 __global__ void __launch_bounds__(kThreads, 1)
 allreduceNormKernel(CommArgs a, NormArgs n, NormXchg x) {
   using R = NormRow<T>;
@@ -194,10 +262,18 @@ allreduceNormKernel(CommArgs a, NormArgs n, NormXchg x) {
   const int me = a.rank;
   const int npacks = static_cast<int>(n.hidden * sizeof(T) / 16);
   const size_t rb = static_cast<size_t>(npacks) * 16;
+  // Q: a row of codes is hidden bytes; the pools hold a region of code rows, then its scales.
+  const size_t qb = n.hidden;
   auto toUser = [&](size_t row) {
     return [&, row](int pk, const Pack16& r, const Pack16& o) {
       st128(static_cast<char*>(n.residualOut) + row * rb + pk * 16, r);
-      if (NORM != kNormNone) st128(static_cast<char*>(n.out) + row * rb + pk * 16, o);
+      if (NORM != kNormNone && !Q) st128(static_cast<char*>(n.out) + row * rb + pk * 16, o);
+    };
+  };
+  auto toUserQ = [&](size_t row) {
+    return [&, row](int pk, const QCodes<T>& c, float scale) {
+      stCodes(static_cast<char*>(n.out) + row * qb + pk * R::kE, c);
+      if (pk == 0) n.outScales[row] = scale;
     };
   };
   typename R::Acc acc[R::kPacks];
@@ -206,7 +282,7 @@ allreduceNormKernel(CommArgs a, NormArgs n, NormXchg x) {
     for (size_t i = blockIdx.x; i < n.rows; i += gridDim.x) {
       zeroAcc<T>(acc);
       addRow<T>(acc, rowPtr(n.partial, i, rb), npacks);
-      rowEpilogue<T, NORM>(acc, n, i, npacks, sh, toUser(i));
+      rowEpilogue<T, NORM, Q>(acc, n, i, npacks, sh, toUser(i), toUserQ(i));
     }
   } else if constexpr (V == kNormLL) {
     // x.peers.p[r]: rank r's LL region; lines [parity][source][unit], two 8-byte units per pack.
@@ -252,7 +328,7 @@ allreduceNormKernel(CommArgs a, NormArgs n, NormXchg x) {
       // A timed-out poll ends the row loop on the whole CTA before the block reductions.
       alive = __syncthreads_and(alive) != 0;
       if (!alive) break;
-      rowEpilogue<T, NORM>(acc, n, i, npacks, sh, toUser(i));
+      rowEpilogue<T, NORM, Q>(acc, n, i, npacks, sh, toUser(i), toUserQ(i));
     }
     retire(a, 0, 0, 1);
   } else if constexpr (V == kNormOneShot) {
@@ -267,14 +343,24 @@ allreduceNormKernel(CommArgs a, NormArgs n, NormXchg x) {
     for (size_t i = blockIdx.x; i < n.rows; i += gridDim.x) {
       zeroAcc<T>(acc);
       for (int r = 0; r < P; r++) addRow<T>(acc, peers[r] + off + i * rb, npacks);
-      rowEpilogue<T, NORM>(acc, n, i, npacks, sh, toUser(i));
+      rowEpilogue<T, NORM, Q>(acc, n, i, npacks, sh, toUser(i), toUserQ(i));
     }
     retire(a, 1, 1);
   } else if constexpr (V == kNormTwoShot) {
     // Pool rows: [0, rows) the staged partials, overwritten with residualOut by the row's owner;
-    // [rows, 2 rows) out.
+    // [rows, 2 rows) out, or with Q rows code rows of qb bytes and then rows fp32 scales.
     const uint32_t e = loadEpoch(a);
     char* mine = static_cast<char*>(x.mine);
+    // Q: each peer's code rows and scales, from shared memory like `peers`: held in registers across
+    // the row loop, their offsets spill at 16-bit LayerNorm. So do the grid size and the epoch,
+    // which Q reads again where it uses them (the epoch only changes when the launch's last CTA
+    // retires).
+    __shared__ char* qPeers[Q ? kMaxRanks : 1];
+    __shared__ float* sPeers[Q ? kMaxRanks : 1];
+    if (Q && threadIdx.x < kMaxRanks) {
+      qPeers[threadIdx.x] = peers[threadIdx.x] + n.rows * rb;
+      sPeers[threadIdx.x] = reinterpret_cast<float*>(peers[threadIdx.x] + n.rows * (rb + qb));
+    }
     for (size_t i = blockIdx.x; i < n.rows; i += gridDim.x) copyRow<T>(mine + i * rb, rowPtr(n.partial, i, rb), npacks);
     if (!blockBarrier(a, e + 1)) {
       retire(a, 2, 0);
@@ -287,27 +373,41 @@ allreduceNormKernel(CommArgs a, NormArgs n, NormXchg x) {
       se = sb + q + (static_cast<size_t>(me) < rem ? 1 : 0);
     }
     const size_t first = sb + (blockIdx.x + gridDim.x - sb % gridDim.x) % gridDim.x;
-    for (size_t i = first; i < se; i += gridDim.x) {
+    for (size_t i = first; i < se; i += (Q ? gridCtas() : gridDim.x)) {
       zeroAcc<T>(acc);
       for (int r = 0; r < P; r++) addRow<T>(acc, peers[r] + i * rb, npacks);
-      rowEpilogue<T, NORM>(acc, n, i, npacks, sh, [&](int pk, const Pack16& rr, const Pack16& o) {
-        for (int r = 0; r < P; r++) {
-          st128_stream(peers[r] + i * rb + pk * 16, rr);
-          if (NORM != kNormNone) st128_stream(peers[r] + (n.rows + i) * rb + pk * 16, o);
-        }
-      });
+      rowEpilogue<T, NORM, Q>(
+          acc, n, i, npacks, sh,
+          [&](int pk, const Pack16& rr, const Pack16& o) {
+            for (int r = 0; r < P; r++) {
+              st128_stream(peers[r] + i * rb + pk * 16, rr);
+              if (NORM != kNormNone && !Q) st128_stream(peers[r] + (n.rows + i) * rb + pk * 16, o);
+            }
+          },
+          [&](int pk, const QCodes<T>& c, float scale) {
+            for (int r = 0; r < P; r++) {
+              stCodes(qPeers[r] + i * qb + pk * R::kE, c);
+              if (pk == 0) sPeers[r][i] = scale;
+            }
+          });
     }
-    if (blockBarrier(a, e + 2)) {
+    if (blockBarrier(a, (Q ? loadEpoch(a) : e) + 2)) {
       for (size_t i = blockIdx.x; i < n.rows; i += gridDim.x) {
         copyRow<T>(static_cast<char*>(n.residualOut) + i * rb, mine + i * rb, npacks);
-        if (NORM != kNormNone) copyRow<T>(static_cast<char*>(n.out) + i * rb, mine + (n.rows + i) * rb, npacks);
+        if constexpr (Q) {
+          copyRow<T>(static_cast<char*>(n.out) + i * qb, qPeers[me] + i * qb, static_cast<int>(qb / 16));
+          if (threadIdx.x == 0) n.outScales[i] = sPeers[me][i];
+        } else if (NORM != kNormNone) {
+          copyRow<T>(static_cast<char*>(n.out) + i * rb, mine + (n.rows + i) * rb, npacks);
+        }
       }
     }
     retire(a, 2, 0);
   } else {
     // n.rows rows of every shard. Pool rows: [0, P rows) the staged partials, row q * rows + i =
     // the user's partial row q * shardRows + i; with a gathered out, [P rows, 2 P rows) out in the
-    // same order. Rank me owns pool rows [me * rows, (me + 1) * rows), shard row i = j - me * rows.
+    // same order (Q: P rows code rows of qb bytes, then P rows fp32 scales). Rank me owns pool rows
+    // [me * rows, (me + 1) * rows), shard row i = j - me * rows.
     // Two barriers either way: with a gathered out the second orders the out stores before the
     // copy out; without one it is a closing barrier, so that no rank restages its pool (in its
     // next launch) while a peer may still be reading the rows it staged.
@@ -327,19 +427,39 @@ allreduceNormKernel(CommArgs a, NormArgs n, NormXchg x) {
       const size_t i = j - sb;
       zeroAcc<T>(acc);
       for (int r = 0; r < P; r++) addRow<T>(acc, peers[r] + j * rb, npacks);
-      rowEpilogue<T, NORM>(acc, n, i, npacks, sh, [&](int pk, const Pack16& rr, const Pack16& o) {
-        st128(static_cast<char*>(n.residualOut) + i * rb + pk * 16, rr);
-        if (NORM == kNormNone) return;
-        if (gather) {
-          for (int r = 0; r < P; r++) st128_stream(peers[r] + (all + j) * rb + pk * 16, o);
-        } else {
-          st128(static_cast<char*>(n.out) + i * rb + pk * 16, o);
-        }
-      });
+      rowEpilogue<T, NORM, Q>(
+          acc, n, i, npacks, sh,
+          [&](int pk, const Pack16& rr, const Pack16& o) {
+            st128(static_cast<char*>(n.residualOut) + i * rb + pk * 16, rr);
+            if (NORM == kNormNone || Q) return;
+            if (gather) {
+              for (int r = 0; r < P; r++) st128_stream(peers[r] + (all + j) * rb + pk * 16, o);
+            } else {
+              st128(static_cast<char*>(n.out) + i * rb + pk * 16, o);
+            }
+          },
+          [&](int pk, const QCodes<T>& c, float scale) {
+            if (gather) {
+              for (int r = 0; r < P; r++) {
+                char* q = peers[r] + all * rb;
+                stCodes(q + j * qb + pk * R::kE, c);
+                if (pk == 0) reinterpret_cast<float*>(q + all * qb)[j] = scale;
+              }
+            } else {
+              stCodes(static_cast<char*>(n.out) + i * qb + pk * R::kE, c);
+              if (pk == 0) n.outScales[i] = scale;
+            }
+          });
     }
-    if (blockBarrier(a, e + 2) && gather) {
+    if (blockBarrier(a, (Q ? loadEpoch(a) : e) + 2) && gather) {  // Q: the epoch as in the two-shot
       for (size_t j = blockIdx.x; j < all; j += gridDim.x) {
-        copyRow<T>(static_cast<char*>(n.out) + userRow(j) * rb, mine + (all + j) * rb, npacks);
+        if constexpr (Q) {
+          const char* q = mine + all * rb;
+          copyRow<T>(static_cast<char*>(n.out) + userRow(j) * qb, q + j * qb, static_cast<int>(qb / 16));
+          if (threadIdx.x == 0) n.outScales[userRow(j)] = reinterpret_cast<const float*>(q + all * qb)[j];
+        } else {
+          copyRow<T>(static_cast<char*>(n.out) + userRow(j) * rb, mine + (all + j) * rb, npacks);
+        }
       }
     }
     retire(a, 2, 0);
@@ -362,14 +482,6 @@ template <typename T>
 __device__ __forceinline__ float& colSum(float* sums, int kind, int k, int e) {
   using R = NormRow<T>;
   return sums[((kind * R::kPacks + k) * R::kE + e) * kThreads + threadIdx.x];
-}
-
-// gridDim.x read again where used (a volatile read of %nctaid.x) rather than held across the row
-// loop, where it would spill at the widest rows (fp32 LayerNorm).
-__device__ __forceinline__ unsigned gridCtas() {
-  unsigned n;
-  asm volatile("mov.u32 %0, %%nctaid.x;" : "=r"(n));
-  return n;
 }
 
 // Moves this thread's column sums between shared memory and the CTA's vectors in ws: in before
@@ -727,23 +839,31 @@ auto normBwdFn(int norm, int variant) -> decltype(&normBackwardKernel<T, kNormRm
 }
 
 // The one place that names an instantiation: the launch, the occupancy query and the preload.
+// The quantising form exists with a norm only.
 template <typename T>
-auto normFn(int norm, int variant) -> decltype(&allreduceNormKernel<T, kNormNone, kNormLocal>) {
-  auto byVariant = [&](auto normTag) -> decltype(&allreduceNormKernel<T, kNormNone, kNormLocal>) {
+auto normFn(int norm, int variant, bool quant) -> decltype(&allreduceNormKernel<T, kNormNone, kNormLocal, false>) {
+  using Fn = decltype(&allreduceNormKernel<T, kNormNone, kNormLocal, false>);
+  auto byVariant = [&](auto normTag, auto quantTag) -> Fn {
     constexpr int N = decltype(normTag)::value;
+    constexpr bool Q = decltype(quantTag)::value;
     switch (variant) {
-      case kNormLL: return allreduceNormKernel<T, N, kNormLL>;
-      case kNormOneShot: return allreduceNormKernel<T, N, kNormOneShot>;
-      case kNormTwoShot: return allreduceNormKernel<T, N, kNormTwoShot>;
-      case kNormLocal: return allreduceNormKernel<T, N, kNormLocal>;
-      case kNormScatter: return allreduceNormKernel<T, N, kNormScatter>;
+      case kNormLL: return allreduceNormKernel<T, N, kNormLL, Q>;
+      case kNormOneShot: return allreduceNormKernel<T, N, kNormOneShot, Q>;
+      case kNormTwoShot: return allreduceNormKernel<T, N, kNormTwoShot, Q>;
+      case kNormLocal: return allreduceNormKernel<T, N, kNormLocal, Q>;
+      case kNormScatter: return allreduceNormKernel<T, N, kNormScatter, Q>;
       default: return nullptr;
     }
   };
+  auto byQuant = [&](auto normTag) -> Fn {
+    if (!quant) return byVariant(normTag, std::false_type{});
+    if constexpr (decltype(normTag)::value != kNormNone) return byVariant(normTag, std::true_type{});
+    return nullptr;
+  };
   switch (norm) {
-    case kNormNone: return byVariant(std::integral_constant<int, kNormNone>{});
-    case kNormRms: return byVariant(std::integral_constant<int, kNormRms>{});
-    case kNormLayer: return byVariant(std::integral_constant<int, kNormLayer>{});
+    case kNormNone: return byQuant(std::integral_constant<int, kNormNone>{});
+    case kNormRms: return byQuant(std::integral_constant<int, kNormRms>{});
+    case kNormLayer: return byQuant(std::integral_constant<int, kNormLayer>{});
     default: return nullptr;
   }
 }
@@ -765,9 +885,9 @@ bool normSupports(DataType dt) {
   return dispatchNormType(dt, [](auto) {});
 }
 
-const void* allreduceNormKernelFor(DataType dt, int norm, int variant) {
+const void* allreduceNormKernelFor(DataType dt, int norm, int variant, bool quant) {
   const void* k = nullptr;
-  dispatchNormType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(normFn<decltype(tag)>(norm, variant)); });
+  dispatchNormType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(normFn<decltype(tag)>(norm, variant, quant)); });
   return k;
 }
 
@@ -775,7 +895,10 @@ void preloadAllreduceNormKernels() {
   for (DataType dt : {DataType::FLOAT32, DataType::BFLOAT16, DataType::FLOAT16}) {
     for (int norm : {kNormNone, kNormRms, kNormLayer}) {
       for (int v : {kNormLL, kNormOneShot, kNormTwoShot, kNormLocal, kNormScatter}) {
-        dispatchNormType(dt, [&](auto tag) { touchKernel(normFn<decltype(tag)>(norm, v)); });
+        for (bool quant : {false, true}) {
+          if (quant && norm == kNormNone) continue;
+          dispatchNormType(dt, [&](auto tag) { touchKernel(normFn<decltype(tag)>(norm, v, quant)); });
+        }
       }
     }
     // The backward's column sums of the widest row take more than the default 48 KB.
@@ -800,7 +923,7 @@ void preloadAllreduceNormKernels() {
 void launchAllreduceNorm(const CommArgs& a, const NormArgs& n, const NormXchg& x, DataType dt, int norm, int variant,
                          int blocks, cudaStream_t stream) {
   dispatchNormType(dt, [&](auto tag) {
-    if (auto k = normFn<decltype(tag)>(norm, variant)) k<<<blocks, kThreads, 0, stream>>>(a, n, x);
+    if (auto k = normFn<decltype(tag)>(norm, variant, n.outScales != nullptr)) k<<<blocks, kThreads, 0, stream>>>(a, n, x);
   });
 }
 

@@ -473,7 +473,13 @@ void allreduceCast(PeerContext& pc, const PeerBuffer& in, size_t inOffset, const
 
 // ---- allreduce fused with bias, residual add and a norm ----------------------------------
 
-NormPlan planResidualNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, AllreduceAlgo algo) {
+// The bytes of one row of out in the pool: a T row, or with `quant` hidden e4m3 codes and a scale.
+size_t poolOutRowBytes(size_t hidden, DataType dt, bool quant) {
+  return quant ? hidden + sizeof(float) : hidden * elementSize(dt);
+}
+
+NormPlan planResidualNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, AllreduceAlgo algo,
+                          bool quant) {
   const size_t rowBytes = hidden * elementSize(dt);
   const size_t bytes = rows * rowBytes;
   const auto l = layoutOf(pc);
@@ -497,7 +503,7 @@ NormPlan planResidualNorm(PeerContext& pc, size_t rows, size_t hidden, DataType 
     } else {
       p.variant = kNormTwoShot;
       // One launch while the staged rows (partials, and out with a norm) fit the bulk region.
-      const size_t perRow = (norm != kNormNone ? 2 : 1) * rowBytes;
+      const size_t perRow = rowBytes + (norm != kNormNone ? poolOutRowBytes(hidden, dt, quant) : 0);
       if (perRow > l.bulkBytes) {
         GLB_THROW(InputException, "allreduce_residual_norm: the pool's bulk region holds no row of ", rowBytes,
                   " bytes; raise GLB_CUDA_STAGE_MB (CudaContext stage_bytes)");
@@ -509,18 +515,19 @@ NormPlan planResidualNorm(PeerContext& pc, size_t rows, size_t hidden, DataType 
   return p;
 }
 
-NormPlan planReduceScatterNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, bool gatherOut) {
+NormPlan planReduceScatterNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, bool gatherOut,
+                               bool quant) {
   const size_t P = static_cast<size_t>(pc.size);
   if (rows % P != 0) {
     GLB_THROW(InputException, "reduce_scatter_residual_norm: ", rows, " rows do not split into ", P, " equal shards");
   }
   // One rank: the shard is every row, and the allreduce form's local launch computes it.
-  if (P == 1) return planResidualNorm(pc, rows, hidden, dt, norm, AllreduceAlgo::AUTO);
+  if (P == 1) return planResidualNorm(pc, rows, hidden, dt, norm, AllreduceAlgo::AUTO, quant);
   const size_t rowBytes = hidden * elementSize(dt), shard = rows / P;
   const auto l = layoutOf(pc);
   // One launch while the staged rows of every shard (and the gathered out) fit the bulk region;
   // beyond it, consecutive chunks of chunkRows rows of every shard.
-  const size_t perRow = P * (norm != kNormNone && gatherOut ? 2 : 1) * rowBytes;
+  const size_t perRow = P * (rowBytes + (norm != kNormNone && gatherOut ? poolOutRowBytes(hidden, dt, quant) : 0));
   if (perRow > l.bulkBytes) {
     GLB_THROW(InputException, "reduce_scatter_residual_norm: the pool's bulk region holds no row of ", rowBytes,
               " bytes from each of ", P, " shards; raise GLB_CUDA_STAGE_MB (CudaContext stage_bytes)");
@@ -674,9 +681,37 @@ void checkNormCall(const char* op, DataType dt, int norm, size_t hidden, bool re
 
 // The forward's required tensors: partial, residual, residual_out and, with a norm, out.
 constexpr const char* kNormRequired = "partial, residual, residual_out and (with a norm) out are required";
-bool normRequired(size_t rows, const NormRange (&inputs)[5], const NormRange (&outputs)[2], int norm) {
+bool normRequired(size_t rows, const NormRange (&inputs)[5], const NormRange (&outputs)[3], int norm) {
   return rows == 0 || (inputs[0].p != nullptr && inputs[1].p != nullptr && outputs[0].p != nullptr &&
                        (norm == kNormNone || outputs[1].p != nullptr));
+}
+
+// The forward's outputs: residual_out (`residualRows` rows) and out (`outRows` rows of T, or with
+// outScales of e4m3 codes, plus their fp32 scales).
+struct NormOutputs {
+  NormRange r[3];
+};
+NormOutputs normOutputs(void* residualOut, void* out, float* outScales, size_t residualRows, size_t outRows,
+                        size_t hidden, DataType dt, int norm) {
+  const size_t rb = hidden * elementSize(dt);
+  const bool quant = outScales != nullptr;
+  return {{{"residual_out", residualOut, residualRows * rb},
+           {"out", norm != kNormNone ? out : nullptr, outRows * (quant ? hidden : rb)},
+           {"out_scales", outScales, outRows * sizeof(float)}}};
+}
+
+// The quantising form's own limits: a norm, and rows of codes that are whole 16-byte packs.
+void checkNormQuant(const char* op, int norm, size_t hidden, const float* outScales) {
+  if (outScales == nullptr) return;
+  GLB_NORM_CHECK(norm != kNormNone, "the FP8 out (out_scales) needs a norm (rms or layer)");
+  GLB_NORM_CHECK(hidden % 16 == 0, "the FP8 out needs rows of a multiple of 16 elements, got ", hidden);
+}
+
+// Points a chunk's out at its codes and scales (the quantising form): rows from row r0 on.
+void quantChunk(NormArgs& a, void* out, float* outScales, size_t r0, size_t hidden) {
+  if (outScales == nullptr) return;
+  a.out = static_cast<char*>(out) + r0 * hidden;
+  a.outScales = outScales + r0;
 }
 
 // The arguments of one chunk: n rows from `off` bytes into every row tensor.
@@ -700,7 +735,7 @@ NormArgs chunkArgs(const void* partial, const void* residual, void* residualOut,
 void launchNormChunk(PeerContext& pc, const NormArgs& a, const NormXchg& x, DataType dt, int norm, int variant,
                      size_t gridRows, cudaStream_t stream, const char* op) {
   // Every CTA waits for its twin on the peers: the grid must be co-resident.
-  const void* kernel = allreduceNormKernelFor(dt, norm, variant);
+  const void* kernel = allreduceNormKernelFor(dt, norm, variant, a.outScales != nullptr);
   const int blocks = static_cast<int>(std::min<size_t>(gridRows, static_cast<size_t>(pc.coResidentBlocks(kernel))));
   prologue(pc, stream);
   launchAllreduceNorm(pc.comm(), a, x, dt, norm, variant, blocks, stream);
@@ -750,24 +785,26 @@ NormBwdArgs bwdChunkArgs(const void* gradOut, const void* s, const void* gradS, 
 
 int allreduceResidualNorm(PeerContext& pc, const void* partial, const void* residual, void* residualOut, void* out,
                           const void* bias, const void* gamma, const void* beta, size_t rows, size_t hidden,
-                          DataType dt, int norm, float eps, AllreduceAlgo algo, cudaStream_t stream) {
+                          DataType dt, int norm, float eps, AllreduceAlgo algo, cudaStream_t stream,
+                          float* outScales) {
   GLB_TRACE_RANGE("glb::cuda::allreduceResidualNorm");
   pc.checkHealth();
   const char* op = "allreduce_residual_norm";
   const size_t rb = hidden * elementSize(dt);
   const NormRange inputs[] = {{"partial", partial, rows * rb}, {"residual", residual, rows * rb}, {"bias", bias, rb},
                               {"weight", gamma, rb}, {"norm_bias", beta, rb}};
-  const NormRange outputs[] = {{"residual_out", residualOut, rows * rb},
-                               {"out", norm != kNormNone ? out : nullptr, rows * rb}};
-  checkNormCall(op, dt, norm, hidden, normRequired(rows, inputs, outputs, norm), kNormRequired, inputs, outputs, 1);
+  const NormOutputs outputs = normOutputs(residualOut, out, outScales, rows, rows, hidden, dt, norm);
+  checkNormCall(op, dt, norm, hidden, normRequired(rows, inputs, outputs.r, norm), kNormRequired, inputs, outputs.r, 1);
+  checkNormQuant(op, norm, hidden, outScales);
   if (rows == 0) return kNormLocal;
-  const NormPlan plan = planResidualNorm(pc, rows, hidden, dt, norm, algo);
+  const NormPlan plan = planResidualNorm(pc, rows, hidden, dt, norm, algo, outScales != nullptr);
   DeviceGuard g(pc.device);
   const auto l = layoutOf(pc);
   const size_t rowBytes = hidden * elementSize(dt);
   for (size_t r0 = 0; r0 < rows; r0 += plan.chunkRows) {
     const size_t n = std::min(plan.chunkRows, rows - r0);
-    const NormArgs a = chunkArgs(partial, residual, residualOut, out, bias, gamma, beta, r0 * rowBytes, n, hidden, norm, eps);
+    NormArgs a = chunkArgs(partial, residual, residualOut, out, bias, gamma, beta, r0 * rowBytes, n, hidden, norm, eps);
+    quantChunk(a, out, outScales, r0, hidden);
     NormXchg x{};
     switch (plan.variant) {
       case kNormLL:
@@ -790,7 +827,8 @@ int allreduceResidualNorm(PeerContext& pc, const void* partial, const void* resi
 
 int reduceScatterResidualNorm(PeerContext& pc, const void* partial, const void* residual, void* residualOut, void* out,
                               const void* bias, const void* gamma, const void* beta, size_t rows, size_t hidden,
-                              DataType dt, int norm, float eps, bool gatherOut, cudaStream_t stream) {
+                              DataType dt, int norm, float eps, bool gatherOut, cudaStream_t stream,
+                              float* outScales) {
   GLB_TRACE_RANGE("glb::cuda::reduceScatterResidualNorm");
   pc.checkHealth();
   const char* op = "reduce_scatter_residual_norm";
@@ -798,16 +836,16 @@ int reduceScatterResidualNorm(PeerContext& pc, const void* partial, const void* 
   const size_t rb = hidden * elementSize(dt);
   const NormRange inputs[] = {{"partial", partial, rows * rb}, {"residual", residual, shard * rb}, {"bias", bias, rb},
                               {"weight", gamma, rb}, {"norm_bias", beta, rb}};
-  const NormRange outputs[] = {{"residual_out", residualOut, shard * rb},
-                               {"out", norm != kNormNone ? out : nullptr, (gatherOut ? rows : shard) * rb}};
-  checkNormCall(op, dt, norm, hidden, normRequired(rows, inputs, outputs, norm), kNormRequired, inputs, outputs, 1);
+  const NormOutputs outputs = normOutputs(residualOut, out, outScales, shard, gatherOut ? rows : shard, hidden, dt, norm);
+  checkNormCall(op, dt, norm, hidden, normRequired(rows, inputs, outputs.r, norm), kNormRequired, inputs, outputs.r, 1);
+  checkNormQuant(op, norm, hidden, outScales);
   GLB_NORM_CHECK(rows % P == 0, rows, " rows do not split into ", P, " equal shards");
   if (P == 1) {
     return allreduceResidualNorm(pc, partial, residual, residualOut, out, bias, gamma, beta, rows, hidden, dt, norm,
-                                 eps, AllreduceAlgo::AUTO, stream);
+                                 eps, AllreduceAlgo::AUTO, stream, outScales);
   }
   if (rows == 0) return kNormScatter;
-  const NormPlan plan = planReduceScatterNorm(pc, rows, hidden, dt, norm, gatherOut);
+  const NormPlan plan = planReduceScatterNorm(pc, rows, hidden, dt, norm, gatherOut, outScales != nullptr);
   DeviceGuard g(pc.device);
   const size_t rowBytes = hidden * elementSize(dt);
   NormXchg x{};
@@ -819,7 +857,8 @@ int reduceScatterResidualNorm(PeerContext& pc, const void* partial, const void* 
   // tensors and a gathered out, whose other shards lie shardRows further on.
   for (size_t r0 = 0; r0 < shard; r0 += plan.chunkRows) {
     const size_t n = std::min(plan.chunkRows, shard - r0);
-    const NormArgs a = chunkArgs(partial, residual, residualOut, out, bias, gamma, beta, r0 * rowBytes, n, hidden, norm, eps);
+    NormArgs a = chunkArgs(partial, residual, residualOut, out, bias, gamma, beta, r0 * rowBytes, n, hidden, norm, eps);
+    quantChunk(a, out, outScales, r0, hidden);
     launchNormChunk(pc, a, x, dt, norm, kNormScatter, P * n, stream, op);
   }
   return kNormScatter;

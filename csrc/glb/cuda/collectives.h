@@ -118,18 +118,26 @@ void allreduceCast(PeerContext& pc, const PeerBuffer& in, size_t inOffset, const
 // bias / gamma / beta may be null. residualOut may be residual; no other output may overlap an
 // input. Every rank passes the same residual, bias, gamma and beta, and gets the same bytes.
 // Invalid arguments raise InputException before anything is launched. Returns the NormVariant.
+// outScales set: the FP8 form (docs/cuda.md, "FP8 out"), with a norm and hidden a multiple of 16.
+// out then holds e4m3 codes (rows, hidden) of the row o that the call without outScales writes,
+// and outScales one fp32 scale per row (16-byte aligned): amax = max(max |o|, 1e-4), code =
+// e4m3(o * (448 * (1 / amax))), scale = amax / 448. residualOut is unchanged; neither range may
+// overlap an input or another output.
 int allreduceResidualNorm(PeerContext& pc, const void* partial, const void* residual, void* residualOut, void* out,
                           const void* bias, const void* gamma, const void* beta, size_t rows, size_t hidden,
-                          DataType dt, int norm, float eps, AllreduceAlgo algo, cudaStream_t stream);
+                          DataType dt, int norm, float eps, AllreduceAlgo algo, cudaStream_t stream,
+                          float* outScales = nullptr);
 // The variant that call runs (the planAllreduce choice for a plain buffer of its bytes, or an
 // explicit LL / ONE_SHOT / TWO_SHOT), and its launches: the two-shot stages its rows in the pool's
-// bulk region, so beyond what that holds it runs as consecutive chunks of chunkRows rows.
+// bulk region, so beyond what that holds it runs as consecutive chunks of chunkRows rows (`quant`:
+// the FP8 form, whose out rows there are hidden code bytes and a scale).
 struct NormPlan {
   int variant;
   size_t chunkRows;
   size_t launches;
 };
-NormPlan planResidualNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, AllreduceAlgo algo);
+NormPlan planResidualNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, AllreduceAlgo algo,
+                          bool quant = false);
 const char* normVariantName(int variant);
 
 // The reduce-scatter form of allreduceResidualNorm, for sequence parallelism (docs/cuda.md,
@@ -140,13 +148,17 @@ const char* normVariantName(int variant);
 // its outputs. out = norm(residualOut): this rank's Ts rows, or with gatherOut all P shards
 // (rows rows, shard q at row q Ts) on every rank. rows % P == 0. One rank runs the allreduce
 // form's local launch. Invalid arguments raise InputException before anything is launched.
+// outScales set: the FP8 form of allreduceResidualNorm, out and outScales with out's rows (a
+// gathered out: shard q's codes and scales at row q Ts).
 int reduceScatterResidualNorm(PeerContext& pc, const void* partial, const void* residual, void* residualOut, void* out,
                               const void* bias, const void* gamma, const void* beta, size_t rows, size_t hidden,
-                              DataType dt, int norm, float eps, bool gatherOut, cudaStream_t stream);
+                              DataType dt, int norm, float eps, bool gatherOut, cudaStream_t stream,
+                              float* outScales = nullptr);
 // Its variant (kNormScatter, or kNormLocal for one rank) and launches: it stages every shard's rows
 // (and a gathered out) in the pool's bulk region, so beyond what that holds it runs as consecutive
 // chunks of chunkRows rows of every shard.
-NormPlan planReduceScatterNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, bool gatherOut);
+NormPlan planReduceScatterNorm(PeerContext& pc, size_t rows, size_t hidden, DataType dt, int norm, bool gatherOut,
+                               bool quant = false);
 
 // The backward of reduceScatterResidualNorm with a norm (kNormRms / kNormLayer), for training with
 // sequence parallelism (docs/cuda.md, "Backward of the reduce-scatter norm"), on the forward's

@@ -474,6 +474,26 @@ constexpr bool isFp8Type() {
   return std::is_same<T, __nv_fp8_e4m3>::value || std::is_same<T, __nv_fp8_e5m2>::value;
 }
 
+// Quantisation to e4m3 codes with one fp32 scale per block of values (the MoE FP8 dispatch: 1 x
+// 128 blocks; the fused residual norm's FP8 out: one block per row). Numerics: amax = max(max |x|,
+// 1e-4f); code = e4m3(x * (448 * (1 / amax))) (round to nearest even, saturating); scale = amax /
+// 448, each step a correctly rounded fp32 operation (no contraction, no approximate division). The
+// multiplier is a rounded reciprocal times 448, not a rounded 448 / amax: that is what torch
+// evaluates for `448.0 / amax` (a scalar over a tensor), so torch code reproduces every byte.
+constexpr float kE4m3Max = 448.0f;
+constexpr float kQuantMinAmax = 1e-4f;
+
+// The block's amax from the largest |x| of its values.
+__device__ __forceinline__ float quantAmax(float absMax) { return fmaxf(absMax, kQuantMinAmax); }
+// The multiplier that takes the block's values to codes.
+__device__ __forceinline__ float e4m3Multiplier(float amax) { return __fmul_rn(__frcp_rn(amax), kE4m3Max); }
+// Two values to two codes (low byte: a).
+__device__ __forceinline__ uint32_t e4m3Codes2(float a, float b, float multiplier) {
+  return float2ToFp8x2<__nv_fp8_e4m3>(__fmul_rn(a, multiplier), __fmul_rn(b, multiplier));
+}
+// The block's scale: x ~= code * scale.
+__device__ __forceinline__ float e4m3Scale(float amax) { return __fdiv_rn(amax, kE4m3Max); }
+
 // Scalar tails (elements after the last whole pack). 16-bit and FP8 types accumulate them in
 // fp32, scale in fp32 and round once, like their packs; every other type accumulates in itself.
 template <typename T>

@@ -64,7 +64,9 @@ enum NormKind : int { kNormNone = 0, kNormRms = 1, kNormLayer = 2 };
 // parallelism): each rank keeps the rows of its own token shard, out optionally gathered.
 enum NormVariant : int { kNormLL = 0, kNormOneShot = 1, kNormTwoShot = 2, kNormLocal = 3, kNormScatter = 4 };
 // One (rows, hidden) problem: contiguous rows of hidden elements, 16-byte aligned. bias / gamma /
-// beta may be null (none, 1, 0); out is unused without a norm.
+// beta may be null (none, 1, 0); out is unused without a norm. outScales set (the quantising form,
+// with a norm, hidden a multiple of 16): out holds e4m3 codes (rows, hidden) and outScales one
+// fp32 scale per row.
 struct NormArgs {
   const void* partial;
   const void* residual;
@@ -76,12 +78,14 @@ struct NormArgs {
   unsigned long long rows;
   unsigned long long hidden;
   float eps;
+  float* outScales = nullptr;
 };
 // Where the partials travel. LL: peers.p[r] = rank r's LL region, mine = mine, srcStride and
 // parityStride its layout. One-shot: rank r's pool halves, parityStride = one half. Two-shot: rank
 // r's 2 x rows rows of the bulk region. Reduce-scatter: rank r's bulk region (P x rows staged rows,
 // then P x rows gathered out rows when `gather`); shardRows = rows between the shards of the
-// user's partial and gathered out (NormArgs::rows is the chunk of every shard).
+// user's partial and gathered out (NormArgs::rows is the chunk of every shard). The quantising
+// form's out in the pool is its rows of hidden code bytes, then one fp32 scale per row.
 struct NormXchg {
   PeerPtrs peers;
   void* mine;
@@ -91,7 +95,7 @@ struct NormXchg {
   int gather;
 };
 bool normSupports(DataType dt);
-const void* allreduceNormKernelFor(DataType dt, int norm, int variant);
+const void* allreduceNormKernelFor(DataType dt, int norm, int variant, bool quant = false);
 void launchAllreduceNorm(const CommArgs& a, const NormArgs& n, const NormXchg& x, DataType dt, int norm, int variant,
                          int blocks, cudaStream_t stream);
 // The backward of the reduce-scatter form with a norm, one chunk of `rows` rows of every shard

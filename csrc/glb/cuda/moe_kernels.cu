@@ -314,15 +314,10 @@ __device__ __forceinline__ void a2aFinish(const CommArgs& a, uint32_t ep, bool m
 
 // ---- quantise: bf16 blocks of kFp8Block elements to e4m3 codes and one fp32 scale ---------------
 constexpr int kQuantUnroll = 4;      // blocks in flight per half-warp
-constexpr float kE4m3Max = 448.0f;
-constexpr float kQuantMinAmax = 1e-4f;
 
 // A half-warp owns a block: each lane loads 8 elements (16 bytes), the block amax takes 4 shuffles
 // within the 16 lanes, each lane stores 8 codes (8 bytes), lane 0 of the half stores the scale.
-// Numerics: amax = max(max |x|, 1e-4f); code = e4m3(x * (448 * (1 / amax))); scale = amax / 448,
-// each step a correctly rounded fp32 operation (no contraction, no approximate division). The
-// multiplier is a rounded reciprocal times 448, not a rounded 448 / amax: that is what torch
-// evaluates for `448.0 / amax` (a scalar over a tensor), so torch code reproduces every byte.
+// Numerics: quantAmax / e4m3Multiplier / e4m3Codes2 / e4m3Scale (device_common.cuh).
 // One block in a half-warp: `v` is this lane's 8 bf16 elements; returns its 8 codes and sets
 // `amax` (the scale is amax / 448). Every lane of the warp must call it: the amax shuffles run
 // with a full mask and stay within each half.
@@ -339,11 +334,11 @@ __device__ __forceinline__ uint2 quantBlock(const uint4& v, float& amax) {
   for (int i = 0; i < 8; i++) amax = fmaxf(amax, fabsf(f[i]));
 #pragma unroll
   for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
-  amax = fmaxf(amax, kQuantMinAmax);
-  const float s = __fmul_rn(__frcp_rn(amax), kE4m3Max);
+  amax = quantAmax(amax);
+  const float s = e4m3Multiplier(amax);
   uint32_t c[4];
 #pragma unroll
-  for (int i = 0; i < 4; i++) c[i] = float2ToFp8x2<__nv_fp8_e4m3>(__fmul_rn(f[2 * i], s), __fmul_rn(f[2 * i + 1], s));
+  for (int i = 0; i < 4; i++) c[i] = e4m3Codes2(f[2 * i], f[2 * i + 1], s);
   return make_uint2(c[0] | (c[1] << 16), c[2] | (c[3] << 16));
 }
 
@@ -374,7 +369,7 @@ __device__ __forceinline__ void quantStore(char* codes, float* scales, unsigned 
   const int hl = lane & 15;
   if (blk < nblk) {
     *reinterpret_cast<uint2*>(codes + blk * kFp8Block + hl * 8) = c;
-    if (hl == 0) scales[blk] = __fdiv_rn(amax, kE4m3Max);
+    if (hl == 0) scales[blk] = e4m3Scale(amax);
   }
 }
 

@@ -194,56 +194,59 @@ void registerCuda(py::module_& root) {
 
   m.def("allreduce_residual_norm", [](PeerContext& pc, uintptr_t partial, uintptr_t residual, uintptr_t residualOut,
                                       uintptr_t out, uintptr_t bias, uintptr_t gamma, uintptr_t beta, size_t rows,
-                                      size_t hidden, int dtype, int norm, double eps, int algo, uintptr_t stream) {
+                                      size_t hidden, int dtype, int norm, double eps, int algo, uintptr_t stream,
+                                      uintptr_t outScales) {
     int v;
     {
       py::gil_scoped_release nogil;
       v = allreduceResidualNorm(pc, P(partial), P(residual), P(residualOut), P(out), P(bias), P(gamma), P(beta), rows,
                                 hidden, static_cast<DataType>(dtype), norm, static_cast<float>(eps),
-                                static_cast<AllreduceAlgo>(algo), S(stream));
+                                static_cast<AllreduceAlgo>(algo), S(stream), reinterpret_cast<float*>(outScales));
     }
     return std::string(normVariantName(v));
   }, py::arg("pc"), py::arg("partial"), py::arg("residual"), py::arg("residual_out"), py::arg("out"), py::arg("bias"),
      py::arg("gamma"), py::arg("beta"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"),
-     py::arg("eps"), py::arg("algo") = 0, py::arg("stream") = 0,
+     py::arg("eps"), py::arg("algo") = 0, py::arg("stream") = 0, py::arg("out_scales") = 0,
      "Allreduce of partial sums fused with bias, residual add and a norm (0 none, 1 rms, 2 layer); null pointers are 0. "
-     "Returns the variant that ran.");
-  m.def("plan_residual_norm", [](PeerContext& pc, size_t rows, size_t hidden, int dtype, int norm, int algo) {
+     "out_scales set: out holds e4m3 codes and out_scales one fp32 scale per row. Returns the variant that ran.");
+  m.def("plan_residual_norm", [](PeerContext& pc, size_t rows, size_t hidden, int dtype, int norm, int algo, bool fp8) {
     const NormPlan p = planResidualNorm(pc, rows, hidden, static_cast<DataType>(dtype), norm,
-                                        static_cast<AllreduceAlgo>(algo));
+                                        static_cast<AllreduceAlgo>(algo), fp8);
     py::dict d;
     d["variant"] = std::string(normVariantName(p.variant));
     d["chunk_rows"] = p.chunkRows;
     d["launches"] = p.launches;
     return d;
-  }, py::arg("pc"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"), py::arg("algo") = 0);
+  }, py::arg("pc"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"), py::arg("algo") = 0,
+     py::arg("fp8") = false);
   m.def("reduce_scatter_residual_norm", [](PeerContext& pc, uintptr_t partial, uintptr_t residual,
                                            uintptr_t residualOut, uintptr_t out, uintptr_t bias, uintptr_t gamma,
                                            uintptr_t beta, size_t rows, size_t hidden, int dtype, int norm, double eps,
-                                           bool gatherOut, uintptr_t stream) {
+                                           bool gatherOut, uintptr_t stream, uintptr_t outScales) {
     int v;
     {
       py::gil_scoped_release nogil;
       v = reduceScatterResidualNorm(pc, P(partial), P(residual), P(residualOut), P(out), P(bias), P(gamma), P(beta),
                                     rows, hidden, static_cast<DataType>(dtype), norm, static_cast<float>(eps),
-                                    gatherOut, S(stream));
+                                    gatherOut, S(stream), reinterpret_cast<float*>(outScales));
     }
     return std::string(normVariantName(v));
   }, py::arg("pc"), py::arg("partial"), py::arg("residual"), py::arg("residual_out"), py::arg("out"), py::arg("bias"),
      py::arg("gamma"), py::arg("beta"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"),
-     py::arg("eps"), py::arg("gather_out") = true, py::arg("stream") = 0,
+     py::arg("eps"), py::arg("gather_out") = true, py::arg("stream") = 0, py::arg("out_scales") = 0,
      "Reduce-scatter of partial sums over row shards fused with bias, residual add and a norm (0 none, 1 rms, "
-     "2 layer), out optionally allgathered; rows is the full row count; null pointers are 0. Returns the variant "
-     "that ran.");
+     "2 layer), out optionally allgathered; rows is the full row count; null pointers are 0. out_scales set: out "
+     "holds e4m3 codes and out_scales one fp32 scale per row. Returns the variant that ran.");
   m.def("plan_reduce_scatter_norm", [](PeerContext& pc, size_t rows, size_t hidden, int dtype, int norm,
-                                       bool gatherOut) {
-    const NormPlan p = planReduceScatterNorm(pc, rows, hidden, static_cast<DataType>(dtype), norm, gatherOut);
+                                       bool gatherOut, bool fp8) {
+    const NormPlan p = planReduceScatterNorm(pc, rows, hidden, static_cast<DataType>(dtype), norm, gatherOut, fp8);
     py::dict d;
     d["variant"] = std::string(normVariantName(p.variant));
     d["chunk_rows"] = p.chunkRows;
     d["launches"] = p.launches;
     return d;
-  }, py::arg("pc"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"), py::arg("gather_out") = true);
+  }, py::arg("pc"), py::arg("rows"), py::arg("hidden"), py::arg("dtype"), py::arg("norm"), py::arg("gather_out") = true,
+     py::arg("fp8") = false);
   m.def("reduce_scatter_residual_norm_backward", [](PeerContext& pc, uintptr_t gradOut, uintptr_t s, uintptr_t gradS,
                                                     uintptr_t gradResidual, uintptr_t gradPartial, uintptr_t gamma,
                                                     uintptr_t gradWeight, uintptr_t gradNormBias, uintptr_t gradBias,

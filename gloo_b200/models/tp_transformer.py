@@ -9,6 +9,9 @@ allreduce also adds the bias and the residual and, after the attention, applies 
 With ``sequence_parallel=True`` the residual stream and both norms live on this rank's shard of the
 sequence (Megatron sequence parallelism): an allgather feeds each column-parallel half, and each
 row-parallel output is reduce-scattered back to the shard instead of allreduced.
+``TPBlock.enable_fp8()`` runs the MLP's up-projection as a row-wise scaled FP8 GEMM for inference:
+ln2's fused step emits e4m3 codes and per-token scales, the weight is quantised once per output
+channel.
 ``DenseBlock`` is the single-process reference with the same parameters (tests load one into the other).
 """
 from __future__ import annotations
@@ -17,6 +20,7 @@ import torch
 from torch import nn
 
 from ..parallel import SequenceParallel, TensorParallel
+from ..parallel.strategies import fp8_rows
 
 
 class DenseBlock(nn.Module):
@@ -56,6 +60,7 @@ class TPBlock(nn.Module):
         self.proj = tp.row_linear(d_model, d_model, device=device, dtype=dtype)
         self.up = tp.column_linear(d_model, d_ff, device=device, dtype=dtype)
         self.down = tp.row_linear(d_ff, d_model, device=device, dtype=dtype)
+        self._fp8_up = None  # (codes, scales) of up.weight in FP8 inference mode
 
     def load_dense(self, dense: DenseBlock):
         """Take this rank's shards of a DenseBlock's parameters."""
@@ -76,7 +81,38 @@ class TPBlock(nn.Module):
         return [p for m in (self.ln1, self.ln2) for p in m.parameters()] + \
             [lin.bias for lin in (self.proj, self.down) if lin.bias is not None]
 
+    def enable_fp8(self, enabled: bool = True):
+        """FP8 inference (CUDA, bfloat16): the up-projection becomes a row-wise scaled FP8 GEMM
+        (``torch._scaled_mm``, bf16 out) of ln2's output, which the fused residual-norm step emits as
+        e4m3 codes with one fp32 scale per token, and of ``up.weight``, quantised here once per output
+        channel by the same ``amax / 448`` rule (``strategies.fp8_rows``). Everything else stays
+        bfloat16. Forward-only: the forward raises ``ValueError`` in grad mode while parameters
+        require grad. Call it again after changing ``up.weight``; ``enabled=False`` turns it off."""
+        if not enabled:
+            self._fp8_up = None
+            return self
+        w = self.up.weight
+        if not w.is_cuda or w.dtype != torch.bfloat16:
+            raise ValueError(f"enable_fp8: needs bfloat16 CUDA parameters, got {w.dtype} on {w.device}")
+        if self.d_model % 16 or w.shape[0] % 16:
+            raise ValueError(f"enable_fp8: the FP8 GEMM needs d_model ({self.d_model}) and d_ff / P ({w.shape[0]}) "
+                             "to be multiples of 16")
+        with torch.no_grad():
+            codes, scales = fp8_rows(w.detach())                   # (d_ff / P, E), (d_ff / P, 1)
+        self._fp8_up = (codes, scales.reshape(1, -1).contiguous())
+        return self
+
+    def _up_fp8(self, codes, scales):
+        """up(ln2(x)) from ln2's FP8 codes (..., E) and per-token scales (..., 1)."""
+        wq, ws = self._fp8_up
+        lead = codes.shape[:-1]
+        h = torch._scaled_mm(codes.reshape(-1, self.d_model), wq.t(), scale_a=scales.reshape(-1, 1), scale_b=ws,
+                             out_dtype=torch.bfloat16)
+        return (h + self.up.bias).view(*lead, -1)
+
     def forward(self, x):
+        if self._fp8_up is not None and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            raise ValueError("TPBlock: FP8 mode is for inference; run the forward under torch.no_grad()")
         if self.sp is not None:
             return self._forward_sequence_parallel(x)
         B, S, E = x.shape
@@ -85,6 +121,12 @@ class TPBlock(nn.Module):
         q, k, v = (lin(h).view(B, S, self.local_heads, hd).transpose(1, 2) for lin in (self.q, self.k, self.v))
         a = nn.functional.scaled_dot_product_attention(q, k, v, is_causal=True)
         a = a.transpose(1, 2).reshape(B, S, self.local_heads * hd)
+        if x.is_cuda and self._fp8_up is not None:
+            # ln2's output as FP8 codes and per-token scales from the fused step, then the FP8 GEMM
+            x, (q8, s8) = self.tp.reduce_residual_norm(nn.functional.linear(a, self.proj.weight), x, self.ln2,
+                                                       self.proj.bias, fp8=True)
+            p = nn.functional.linear(nn.functional.gelu(self._up_fp8(q8, s8)), self.down.weight)
+            return self.tp.reduce_residual_norm(p, x, None, self.down.bias)
         if x.is_cuda:
             # each row-parallel output: allreduce + bias + residual add (+ ln2) in one kernel
             # copy_out: h's gradient is allreduced inside the fused backward, so self.up(h)'s
@@ -107,6 +149,11 @@ class TPBlock(nn.Module):
         q, k, v = (F.linear(h, lin.weight, lin.bias).view(S, B, self.local_heads, hd).permute(1, 2, 0, 3)
                    for lin in (self.q, self.k, self.v))
         a = F.scaled_dot_product_attention(q, k, v, is_causal=True).permute(2, 0, 1, 3).reshape(S, B, -1)
+        if self._fp8_up is not None:
+            x, (q8, s8) = sp.reduce_scatter_residual_norm(F.linear(a, self.proj.weight), x, self.ln2, self.proj.bias,
+                                                          fp8=True)
+            p = F.linear(F.gelu(self._up_fp8(q8, s8)), self.down.weight)
+            return sp.reduce_scatter_residual_norm(p, x, None, self.down.bias, gather_out=False)
         x, h = sp.reduce_scatter_residual_norm(F.linear(a, self.proj.weight), x, self.ln2, self.proj.bias)
         p = F.linear(F.gelu(F.linear(h, self.up.weight, self.up.bias)), self.down.weight)
         return sp.reduce_scatter_residual_norm(p, x, None, self.down.bias, gather_out=False)

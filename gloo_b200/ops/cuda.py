@@ -198,8 +198,36 @@ class CudaContext:
         kind = 2 if buf is None else (0 if (buf.has_multicast and off % 16 == 0) else 1)
         return _cu.plan_allreduce(self.pc, n * element_size(dt), int(dt), int(op), kind)
 
+    @staticmethod
+    def _norm_fp8_out(name, partial, norm, out, out_scales, shape):
+        """The FP8 form's checks of ``out`` / ``out_scales`` (``shape``: out's shape): ``(quant, out)``,
+        with ``out`` allocated when not given. An FP8 ``out`` needs ``out_scales``."""
+        import torch
+
+        fp8 = (torch.float8_e4m3fn, torch.float8_e5m2)
+        if out_scales is None:
+            if out is not None and out.dtype in fp8:
+                raise ValueError(f"{name}: an FP8 out needs out_scales (float32 {(*shape[:-1], 1)})")
+            return False, out
+        form = f"the FP8 form takes float8_e4m3fn out {tuple(shape)} and float32 out_scales {(*shape[:-1], 1)}"
+        if norm is None:
+            raise ValueError(f"{name}: out_scales needs a norm; {form}")
+        if shape[-1] % 16:
+            raise ValueError(f"{name}: the FP8 out needs rows of a multiple of 16 elements, got {shape[-1]}")
+        if out is None:
+            out = torch.empty(tuple(shape), dtype=torch.float8_e4m3fn, device=partial.device)
+        for key, t, dtype, want in (("out", out, torch.float8_e4m3fn, tuple(shape)),
+                                    ("out_scales", out_scales, torch.float32, (*shape[:-1], 1))):
+            if not isinstance(t, torch.Tensor) or t.dtype != dtype:
+                raise ValueError(f"{name}: {key} must be a {dtype} tensor, got {getattr(t, 'dtype', type(t))}; {form}")
+            if not t.is_cuda or not t.is_contiguous() or tuple(t.shape) != want:
+                raise ValueError(f"{name}: {key} must be a contiguous CUDA tensor of shape {want}, got "
+                                 f"{tuple(t.shape)} on {t.device}{'' if t.is_contiguous() else ', not contiguous'}")
+        return True, out
+
     def allreduce_residual_norm(self, partial, residual, weight=None, norm_bias=None, *, norm: Optional[str] = "rms",
-                                eps: float = 1e-6, bias=None, residual_out=None, out=None, algo="auto", stream=None):
+                                eps: float = 1e-6, bias=None, residual_out=None, out=None, algo="auto", stream=None,
+                                out_scales=None):
         """The row-parallel output step of tensor parallelism in ONE kernel launch: allreduce of the
         partial sums, ``+ bias``, ``+ residual`` and the next norm.
 
@@ -216,6 +244,15 @@ class CudaContext:
         allocated when not given. ``algo``: ``"auto"`` (the allreduce's choice for a plain tensor of
         the same size), ``"ll"``, ``"one_shot"`` or ``"two_shot"``. Invalid arguments raise
         ``ValueError`` before anything is launched.
+
+        FP8 ``out`` for an FP8 GEMM: passing ``out_scales`` (float32, shape ``out.shape[:-1] + (1,)``,
+        the ``(M, 1)`` row-wise scales of ``scaled_mm``) makes ``out`` float8_e4m3fn codes (allocated
+        when not given) of the row ``o`` that the call without it writes, in the same launch: per
+        row ``amax = max(max |o|, 1e-4)``, ``out = e4m3(o * (448 / amax))`` (round to nearest even,
+        saturating) and ``out_scales = amax / 448``, so ``o ~= out * out_scales``. It needs a norm and
+        H a multiple of 16; ``residual_out`` is what the call without it writes. torch reproduces
+        every byte: ``(o.float() * (448.0 / a)).to(torch.float8_e4m3fn)`` and ``a /
+        torch.full_like(a, 448.0)`` with ``a = o.float().abs().amax(-1, keepdim=True).clamp_min(1e-4)``.
 
         Returns ``(residual_out, out)``, or ``residual_out`` when ``norm`` is None."""
         import torch
@@ -234,12 +271,13 @@ class CudaContext:
         H = partial.shape[-1]
         if residual_out is None:
             residual_out = residual
+        quant, out = self._norm_fp8_out("allreduce_residual_norm", partial, norm, out, out_scales, tuple(partial.shape))
         if norm is not None and out is None:
             out = torch.empty_like(partial, memory_format=torch.contiguous_format)
         named = {"partial": partial, "residual": residual, "residual_out": residual_out, "out": out, "bias": bias,
                  "weight": weight, "norm_bias": norm_bias}
         for name, t in named.items():
-            if t is None:
+            if t is None or (quant and name == "out"):
                 continue
             if not t.is_cuda or t.dtype != partial.dtype or not t.is_contiguous():
                 raise ValueError(f"allreduce_residual_norm: {name} must be a contiguous CUDA tensor of {partial.dtype}, "
@@ -251,12 +289,12 @@ class CudaContext:
         ptr = lambda t: 0 if t is None else t.data_ptr()  # noqa: E731
         _cu.allreduce_residual_norm(self.pc, ptr(partial), ptr(residual), ptr(residual_out), ptr(out), ptr(bias),
                                     ptr(weight), ptr(norm_bias), partial.numel() // max(H, 1), H, int(dt), kinds[norm],
-                                    float(eps), _algo(algo), _stream(stream))
+                                    float(eps), _algo(algo), _stream(stream), ptr(out_scales))
         return residual_out if norm is None else (residual_out, out)
 
     def reduce_scatter_residual_norm(self, partial, residual, weight=None, norm_bias=None, *,
                                      norm: Optional[str] = "rms", eps: float = 1e-6, bias=None, residual_out=None,
-                                     out=None, gather_out: bool = True, stream=None):
+                                     out=None, gather_out: bool = True, stream=None, out_scales=None):
         """The row-parallel output step of sequence parallelism in ONE kernel launch: reduce-scatter
         of the partial sums over token shards, ``+ bias``, ``+ residual`` and the next norm, whose
         output is optionally allgathered.
@@ -270,6 +308,10 @@ class CudaContext:
         rows ``q * Ts``) and ``residual``'s shape without. ``bias``, ``weight`` and ``norm_bias`` must
         be the same on every rank. ``residual_out`` defaults to ``residual`` (in place); ``out`` is
         allocated when not given. Invalid arguments raise ``ValueError`` before anything is launched.
+
+        ``out_scales``: the FP8 form of :meth:`allreduce_residual_norm`, with ``out``'s rows (with
+        ``gather_out`` every shard's codes and scales, shard q at rows ``q * Ts``); the gathered rows
+        travel as H code bytes and one scale each.
 
         Returns ``(residual_out, out)``, or ``residual_out`` when ``norm`` is None."""
         import torch
@@ -290,12 +332,14 @@ class CudaContext:
         shard = (T // self.size, *partial.shape[1:])
         if residual_out is None:
             residual_out = residual
+        quant, out = self._norm_fp8_out(name, partial, norm, out, out_scales,
+                                        tuple(partial.shape) if gather_out else shard)
         if norm is not None and out is None:
             out = torch.empty(tuple(partial.shape) if gather_out else shard, dtype=partial.dtype, device=partial.device)
         named = {"partial": partial, "residual": residual, "residual_out": residual_out, "out": out, "bias": bias,
                  "weight": weight, "norm_bias": norm_bias}
         for key, t in named.items():
-            if t is None:
+            if t is None or (quant and key == "out"):
                 continue
             if not t.is_cuda or t.dtype != partial.dtype or not t.is_contiguous():
                 raise ValueError(f"{name}: {key} must be a contiguous CUDA tensor of {partial.dtype}, "
@@ -312,7 +356,7 @@ class CudaContext:
         ptr = lambda t: 0 if t is None else t.data_ptr()  # noqa: E731
         _cu.reduce_scatter_residual_norm(self.pc, ptr(partial), ptr(residual), ptr(residual_out), ptr(out), ptr(bias),
                                          ptr(weight), ptr(norm_bias), partial.numel() // max(H, 1), H, int(dt),
-                                         kinds[norm], float(eps), bool(gather_out), _stream(stream))
+                                         kinds[norm], float(eps), bool(gather_out), _stream(stream), ptr(out_scales))
         return residual_out if norm is None else (residual_out, out)
 
     def reduce_scatter_residual_norm_backward(self, grad_out, residual_out, grad_residual_out=None, weight=None, *,

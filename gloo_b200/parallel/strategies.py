@@ -51,6 +51,29 @@ def _norm_fusable(cc, partial, residual, residual_shape, norm_module, kind, vect
     return True
 
 
+def fp8_rows(o):
+    """Row-wise FP8 quantisation of ``o`` in torch, the bytes the fused FP8 ``out`` has: ``(codes,
+    scales)``, float8_e4m3fn codes of ``o``'s shape and float32 scales ``o.shape[:-1] + (1,)``, with
+    ``amax = max(max |o|, 1e-4)`` per row, ``codes = e4m3(o * (448 / amax))`` and ``scales = amax /
+    448``. The scale divides by a tensor: on CUDA, torch divides by a Python scalar by multiplying
+    with its rounded reciprocal, which is not ``amax / 448`` correctly rounded."""
+    import torch
+
+    a = o.float().abs().amax(-1, keepdim=True).clamp_min(1e-4)
+    return (o.float() * (448.0 / a)).to(torch.float8_e4m3fn), a / torch.full_like(a, 448.0)
+
+
+def _check_fp8_call(name, norm_module, tensors):
+    """The FP8 form is forward-only and needs a norm."""
+    import torch
+
+    if norm_module is None:
+        raise ValueError(f"{name}: fp8 needs a norm_module")
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors):
+        raise ValueError(f"{name}: fp8 is forward-only; run it under torch.no_grad() or on tensors that do not "
+                         "require grad")
+
+
 def _aligned_like(s, *grads) -> bool:
     """Whether the gradients (None: absent) have ``s``'s dtype and device and, made contiguous,
     the 16-byte alignment the fused backward needs."""
@@ -459,7 +482,8 @@ class TensorParallel(_Base):
 
         return _G.apply(x)
 
-    def reduce_residual_norm(self, partial, residual, norm_module=None, bias=None, copy_out: bool = False):
+    def reduce_residual_norm(self, partial, residual, norm_module=None, bias=None, copy_out: bool = False,
+                             fp8: bool = False):
         """g fused with what follows a row-parallel matmul: ``s = allreduce(partial) + bias +
         residual`` and the next norm. Returns ``(s, norm_module(s))``, or ``s`` when
         ``norm_module`` is None. ``norm_module`` is an ``nn.LayerNorm``, an ``nn.RMSNorm`` or None.
@@ -477,12 +501,32 @@ class TensorParallel(_Base):
         allreduces. After a fused forward that is one fused kernel
         (``CudaContext.allreduce_residual_norm_backward``), which gives every rank the same bytes of
         every gradient and computes only the vector gradients autograd needs; a gradient it cannot
-        take (dtype, alignment) is allreduced and the norm recomputed with torch."""
+        take (dtype, alignment) is allreduced and the norm recomputed with torch.
+
+        ``fp8``: returns ``(s, (codes, scales))``, the norm's output as float8_e4m3fn codes and
+        float32 per-row scales ``(..., 1)`` (``fp8_rows`` of it, byte for byte), for a row-wise scaled
+        FP8 GEMM. The fused kernel quantises in the same launch
+        (``CudaContext.allreduce_residual_norm(out_scales=)``); where it cannot run (as above, or H
+        not a multiple of 16) the composition above runs, then ``fp8_rows``. Forward-only: with
+        grad mode on, an input or norm parameter that requires grad raises ``ValueError``."""
         import torch
 
         if copy_out and norm_module is None:
             raise ValueError("reduce_residual_norm: copy_out needs a norm_module")
         kind, weight, norm_bias, eps = _norm_parts(norm_module, partial.dtype)
+        if fp8:
+            if copy_out:
+                raise ValueError("reduce_residual_norm: fp8 is forward-only and takes no copy_out")
+            _check_fp8_call("reduce_residual_norm", norm_module, (partial, residual, bias, weight, norm_bias))
+            if not self._fusable(partial, residual, norm_module, kind, (bias, weight, norm_bias)) or \
+                    partial.shape[-1] % 16:
+                s, out = self.reduce_residual_norm(partial, residual, norm_module, bias)
+                return s, fp8_rows(out)
+            s = torch.empty_like(residual, memory_format=torch.contiguous_format)
+            scales = torch.empty((*partial.shape[:-1], 1), dtype=torch.float32, device=partial.device)
+            _, codes = self.cc.allreduce_residual_norm(partial.contiguous(), residual.contiguous(), weight, norm_bias,
+                                                       norm=kind, eps=eps, bias=bias, residual_out=s, out_scales=scales)
+            return s, (codes, scales)
         if not self._fusable(partial, residual, norm_module, kind, (bias, weight, norm_bias)):
             y = self.reduce_from_region(partial)
             if bias is not None:
@@ -673,7 +717,7 @@ class SequenceParallel(_Base):
         return _Scatter.apply(x)
 
     def reduce_scatter_residual_norm(self, partial, residual_shard, norm_module=None, bias=None,
-                                     gather_out: bool = True):
+                                     gather_out: bool = True, fp8: bool = False):
         """``reduce_scatter_to_sequence`` fused with what follows a row-parallel matmul: ``s =
         reduce_scatter(partial) + bias + residual_shard`` on this rank's shard and the next norm,
         whose output is allgathered when ``gather_out``. Returns ``(s, out)``, or ``s`` when
@@ -688,22 +732,43 @@ class SequenceParallel(_Base):
         one fused kernel too (``CudaContext.reduce_scatter_residual_norm_backward``); otherwise it
         runs the collectives and a torch recompute of the norm. Anything else
         runs ``reduce_scatter_to_sequence``, ``+ bias``, ``+ residual_shard``, the module and
-        ``gather_from_sequence``."""
+        ``gather_from_sequence``.
+
+        ``fp8``: returns ``(s, (codes, scales))``, ``out`` as float8_e4m3fn codes and float32 per-row
+        scales ``(..., 1)`` (``fp8_rows`` of it, byte for byte); a gathered ``out`` travels as codes
+        and scales. Where the fused kernel cannot run (as above, or H not a multiple of 16) the
+        composition above runs, then ``fp8_rows``. Forward-only, as in
+        ``TensorParallel.reduce_residual_norm``."""
         import torch
 
         kind, weight, norm_bias, eps = _norm_parts(norm_module, partial.dtype)
+        if fp8:
+            _check_fp8_call("reduce_scatter_residual_norm", norm_module,
+                            (partial, residual_shard, bias, weight, norm_bias))
         fused = (partial.dim() > 0 and partial.shape[0] % self.size == 0 and
                  _norm_fusable(self.cc, partial, residual_shard, (partial.shape[0] // self.size, *partial.shape[1:]),
-                               norm_module, kind, (bias, weight, norm_bias)))
+                               norm_module, kind, (bias, weight, norm_bias)) and
+                 not (fp8 and partial.shape[-1] % 16))
         if fused:
             from ..types import _torch_map
 
             try:  # a row too wide for the staging pool is outside the limits too
                 _C.cuda.plan_reduce_scatter_norm(self.cc.pc, partial.numel() // partial.shape[-1], partial.shape[-1],
                                                  int(_torch_map()[partial.dtype]), {None: 0, "rms": 1, "layer": 2}[kind],
-                                                 gather_out)
+                                                 gather_out, fp8)
             except ValueError:
                 fused = False
+        if fp8 and not fused:
+            s, out = self.reduce_scatter_residual_norm(partial, residual_shard, norm_module, bias, gather_out)
+            return s, fp8_rows(out)
+        if fp8:
+            s = torch.empty_like(residual_shard, memory_format=torch.contiguous_format)
+            rows = partial.shape if gather_out else residual_shard.shape
+            scales = torch.empty((*rows[:-1], 1), dtype=torch.float32, device=partial.device)
+            _, codes = self.cc.reduce_scatter_residual_norm(partial.contiguous(), residual_shard.contiguous(), weight,
+                                                            norm_bias, norm=kind, eps=eps, bias=bias, residual_out=s,
+                                                            gather_out=gather_out, out_scales=scales)
+            return s, (codes, scales)
         if not fused:
             y = self.reduce_scatter_to_sequence(partial)
             if bias is not None:

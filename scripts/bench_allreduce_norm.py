@@ -23,6 +23,11 @@ against the composition TensorParallel's autograd runs without it: clone + `cc.a
 gradient, the norm recomputed under torch autograd, the add and the bias row sum. bf16, with weight
 and bias gradients (and the norm bias for layer); T on both sides of the one-shot / two-shot
 threshold. Before timing, each shape records how far the two gradients of `partial` lie apart.
+
+`--fp8` times the FP8 form (`allreduce_residual_norm(out_scales=)`: `out` as e4m3 codes with one
+fp32 scale per row, in the same launch) against the fused bf16 call followed by the torch
+quantisation of its `out` (`strategies.fp8_rows`), at decode T (1-128) and prefill T (4096), bf16,
+with the launches per call of each. Each shape first checks that the two give the same bytes.
 """
 import argparse
 import json
@@ -37,7 +42,7 @@ import torch.nn.functional as F  # noqa: E402
 
 import gloo_b200 as gb  # noqa: E402
 from gloo_b200.ops import cuda as gcu  # noqa: E402
-from gloo_b200.parallel.strategies import _norm_input_grad  # noqa: E402
+from gloo_b200.parallel.strategies import _norm_input_grad, fp8_rows  # noqa: E402
 
 DECODE_T = (1, 8, 32, 128)
 PREFILL_T = (4096,)
@@ -102,6 +107,52 @@ def bench_rank(ctx, device, args, world, profile_unfused=True):
                 row["fused_launches_per_call"] = launches_fused(cc, fused)
                 row["unfused_kernels_per_call"] = kernels_unfused(unfused, profile_unfused)
                 row["speedup"] = row["unfused_us"] / row["fused_us"]
+                rows.append(row)
+    return rows
+
+
+def bench_fp8_rank(ctx, device, args, world, profile_composed=True):
+    cc = gcu.CudaContext(ctx, device, stage_bytes=args.stage_mb << 20)
+    cc.set_timeout(600000)
+    stream = torch.cuda.current_stream()
+    dtype = torch.bfloat16
+    rows = []
+    for H in HIDDEN:
+        for T in DECODE_T + PREFILL_T:
+            g = torch.Generator(device="cpu").manual_seed(T * 131 + H)
+            partial = torch.randn(T, H, generator=g).to(dtype).cuda()
+            residual = torch.randn(T, H, generator=g).to(dtype).cuda()
+            bias = torch.randn(H, generator=g).to(dtype).cuda()
+            weight = (1 + 0.1 * torch.randn(H, generator=g)).to(dtype).cuda()
+            norm_bias = (0.1 * torch.randn(H, generator=g)).to(dtype).cuda()
+            res_out, out = torch.empty_like(residual), torch.empty_like(residual)
+            codes = torch.empty(T, H, dtype=torch.float8_e4m3fn, device="cuda")
+            scales = torch.empty(T, 1, dtype=torch.float32, device="cuda")
+            for norm in ("rms", "layer"):
+                nb = norm_bias if norm == "layer" else None
+
+                def fused_fp8():
+                    cc.allreduce_residual_norm(partial, residual, weight, nb, norm=norm, eps=1e-6, bias=bias,
+                                               residual_out=res_out, out=codes, out_scales=scales)
+
+                def composed():
+                    cc.allreduce_residual_norm(partial, residual, weight, nb, norm=norm, eps=1e-6, bias=bias,
+                                               residual_out=res_out, out=out)
+                    return fp8_rows(out)
+
+                want_c, want_s = composed()
+                fused_fp8()
+                torch.cuda.synchronize()
+                same = bool(torch.equal(codes.view(torch.uint8), want_c.view(torch.uint8)) and torch.equal(scales, want_s))
+                plan = gb._C.cuda.plan_residual_norm(cc.pc, T, H, int(gb.DataType.BFLOAT16), {"rms": 1, "layer": 2}[norm],
+                                                     0, True)
+                row = {"T": T, "H": H, "dtype": "bfloat16", "norm": norm, "variant": plan["variant"],
+                       "same_bytes": same}
+                row["fp8_fused_us"] = timed(ctx, cc, fused_fp8, stream, args, world)
+                row["bf16_fused_plus_torch_quant_us"] = timed(ctx, cc, composed, stream, args, world)
+                row["fp8_fused_launches_per_call"] = launches_fused(cc, fused_fp8)
+                row["composed_kernels_per_call"] = kernels_unfused(composed, profile_composed)
+                row["speedup"] = row["bf16_fused_plus_torch_quant_us"] / row["fp8_fused_us"]
                 rows.append(row)
     return rows
 
@@ -218,10 +269,14 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--stage-mb", type=int, default=128)
     ap.add_argument("--backward", action="store_true", help="time the fused backward against its composition")
+    ap.add_argument("--fp8", action="store_true", help="time the FP8 out against bf16 + torch quantisation")
     args = ap.parse_args()
+    kind = "_backward" if args.backward else "_fp8" if args.fp8 else ""
     if args.threads:
         world = args.threads
-        run = bench_backward_rank if args.backward else lambda ctx, dev, a, w: bench_rank(ctx, dev, a, w, False)
+        run = bench_backward_rank if args.backward else \
+            (lambda ctx, dev, a, w: bench_fp8_rank(ctx, dev, a, w, False)) if args.fp8 else \
+            (lambda ctx, dev, a, w: bench_rank(ctx, dev, a, w, False))
         rows = gb.spawn_threads(world, lambda ctx: run(ctx, 0, args, 1), cuda_device=0, timeout_ms=600000)[0]
         mode = f"{world} ranks as threads on one GPU: overhead only, not link numbers"
         info = gpu_info(0)
@@ -232,11 +287,12 @@ def main():
         torch.cuda.set_device(local)
         ctx = gb.init_context(rank, world, path=f"/tmp/glb_norm_{os.environ.get('MASTER_PORT', '0')}_{os.getppid()}",
                               timeout_ms=120000)
-        rows = (bench_backward_rank if args.backward else bench_rank)(ctx, local, args, world)
+        rows = (bench_backward_rank if args.backward else bench_fp8_rank if args.fp8 else bench_rank)(ctx, local, args,
+                                                                                                world)
         mode = f"{world} ranks, one per GPU"
         info = gpu_info(local)
     if rank == 0:
-        doc = {"benchmark": "allreduce_residual_norm" + ("_backward" if args.backward else ""), "mode": mode, "ranks": world, **info, "iters": args.iters,
+        doc = {"benchmark": "allreduce_residual_norm" + kind, "mode": mode, "ranks": world, **info, "iters": args.iters,
                "warmup": args.warmup, "reps": args.reps, "rows": rows}
         text = json.dumps(doc)
         print(text)

@@ -24,6 +24,12 @@ stream's gradient and the allgather, one kernel per chunk plus one that finishes
 against the composition SequenceParallel's autograd ran before it: `cc.reduce_scatter`, the norm
 recomputed under torch autograd, the add, the bias row sum and `cc.allgather`. Before timing, each
 shape records how far the two gradients of `partial` lie apart.
+
+`--fp8` times the FP8 form (`reduce_scatter_residual_norm(out_scales=)`: the gathered `out` as e4m3
+codes with one fp32 scale per row, in the same launch, so the allgather carries codes) against the
+fused bf16 call followed by the torch quantisation of its gathered `out` (`strategies.fp8_rows`),
+with the launches per call of each (torch's kernels counted by torch.profiler, one rank per process
+only). Each shape first checks that the two give the same bytes.
 """
 import argparse
 import json
@@ -37,9 +43,9 @@ import torch  # noqa: E402
 import torch.nn.functional as F  # noqa: E402
 
 import gloo_b200 as gb  # noqa: E402
-from bench_allreduce_norm import gpu_info, launches_fused, timed  # noqa: E402
+from bench_allreduce_norm import gpu_info, kernels_unfused, launches_fused, timed  # noqa: E402
 from gloo_b200.ops import cuda as gcu  # noqa: E402
-from gloo_b200.parallel.strategies import _norm_input_grad  # noqa: E402
+from gloo_b200.parallel.strategies import _norm_input_grad, fp8_rows  # noqa: E402
 
 DECODE_T = (8, 64, 256)
 PREFILL_T = (4096,)
@@ -95,6 +101,54 @@ def bench_rank(ctx, device, args, world):
                     row[f"{name}_us"] = timed(ctx, cc, fn, stream, args, world)
                 row["fused_launches_per_call"] = launches_fused(cc, fused)
                 row["speedup"] = row["unfused_us"] / row["fused_us"]
+                rows.append(row)
+    return rows
+
+
+def bench_fp8_rank(ctx, device, args, world, profile_composed=True):
+    cc = gcu.CudaContext(ctx, device, stage_bytes=args.stage_mb << 20)
+    cc.set_timeout(600000)
+    stream = torch.cuda.current_stream()
+    dtype, P, rank = torch.bfloat16, ctx.size, ctx.rank
+    rows = []
+    for H in HIDDEN:
+        for T in DECODE_T + PREFILL_T:
+            Ts = T // P
+            g = torch.Generator(device="cpu").manual_seed(T * 131 + H)
+            residual = torch.randn(T, H, generator=g).to(dtype)[rank * Ts:(rank + 1) * Ts].contiguous().cuda()
+            bias = torch.randn(H, generator=g).to(dtype).cuda()
+            weight = (1 + 0.1 * torch.randn(H, generator=g)).to(dtype).cuda()
+            norm_bias = (0.1 * torch.randn(H, generator=g)).to(dtype).cuda()
+            partial = torch.randn(T, H, generator=torch.Generator().manual_seed(T * 131 + H + 7 + rank)).to(dtype).cuda()
+            res_out, out = torch.empty_like(residual), torch.empty(T, H, dtype=dtype, device="cuda")
+            codes = torch.empty(T, H, dtype=torch.float8_e4m3fn, device="cuda")
+            scales = torch.empty(T, 1, dtype=torch.float32, device="cuda")
+            for norm in ("rms", "layer"):
+                nb = norm_bias if norm == "layer" else None
+
+                def fused_fp8():
+                    cc.reduce_scatter_residual_norm(partial, residual, weight, nb, norm=norm, eps=1e-6, bias=bias,
+                                                    residual_out=res_out, out=codes, out_scales=scales)
+
+                def composed():
+                    cc.reduce_scatter_residual_norm(partial, residual, weight, nb, norm=norm, eps=1e-6, bias=bias,
+                                                    residual_out=res_out, out=out)
+                    return fp8_rows(out)
+
+                want_c, want_s = composed()
+                fused_fp8()
+                torch.cuda.synchronize()
+                same = bool(torch.equal(codes.view(torch.uint8), want_c.view(torch.uint8)) and torch.equal(scales, want_s))
+                plans = [gb._C.cuda.plan_reduce_scatter_norm(cc.pc, T, H, int(gb.DataType.BFLOAT16),
+                                                             {"rms": 1, "layer": 2}[norm], True, fp8) for fp8 in (False, True)]
+                row = {"T": T, "H": H, "dtype": "bfloat16", "norm": norm, "shard_bytes": Ts * H * 2,
+                       "variant": plans[1]["variant"], "same_bytes": same, "bf16_chunk_rows": plans[0]["chunk_rows"],
+                       "fp8_chunk_rows": plans[1]["chunk_rows"]}
+                row["fp8_fused_us"] = timed(ctx, cc, fused_fp8, stream, args, world)
+                row["bf16_fused_plus_torch_quant_us"] = timed(ctx, cc, composed, stream, args, world)
+                row["fp8_fused_launches_per_call"] = launches_fused(cc, fused_fp8)
+                row["composed_kernels_per_call"] = kernels_unfused(composed, profile_composed)
+                row["speedup"] = row["bf16_fused_plus_torch_quant_us"] / row["fp8_fused_us"]
                 rows.append(row)
     return rows
 
@@ -165,11 +219,13 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--stage-mb", type=int, default=128)
     ap.add_argument("--backward", action="store_true", help="time the fused backward against its composition")
+    ap.add_argument("--fp8", action="store_true", help="time the FP8 out against bf16 + torch quantisation")
     args = ap.parse_args()
-    run = bench_backward_rank if args.backward else bench_rank
+    run = bench_backward_rank if args.backward else bench_fp8_rank if args.fp8 else bench_rank
     if args.threads:
         world = args.threads
-        rows = gb.spawn_threads(world, lambda ctx: run(ctx, 0, args, 1), cuda_device=0, timeout_ms=600000)[0]
+        thread_run = (lambda ctx, dev, a, w: bench_fp8_rank(ctx, dev, a, w, False)) if args.fp8 else run
+        rows = gb.spawn_threads(world, lambda ctx: thread_run(ctx, 0, args, 1), cuda_device=0, timeout_ms=600000)[0]
         mode = f"{world} ranks as threads on one GPU: overhead only, not link numbers"
         info, rank = gpu_info(0), 0
     else:
@@ -182,7 +238,7 @@ def main():
         mode = f"{world} ranks, one per GPU"
         info = gpu_info(local)
     if rank == 0:
-        name = "reduce_scatter_residual_norm" + ("_backward" if args.backward else "")
+        name = "reduce_scatter_residual_norm" + ("_backward" if args.backward else "_fp8" if args.fp8 else "")
         doc = {"benchmark": name, "mode": mode, "ranks": world, **info, "iters": args.iters,
                "warmup": args.warmup, "reps": args.reps, "rows": rows}
         text = json.dumps(doc)

@@ -53,8 +53,10 @@ KERNELS = [
     ("ll_combine_topk_bf16", r"moeLLCombineKernel<__nv_bfloat16>"),
     ("ll_combine_topk_f16", r"moeLLCombineKernel<__half>"),
     ("ll_combine_topk_f32", r"moeLLCombineKernel<float>"),
-    ("reduce_scatter_norm_bf16_rms", r"allreduceNormKernel<__nv_bfloat16, 1, 4>"),
-    ("reduce_scatter_norm_f32_layer", r"allreduceNormKernel<float, 2, 4>"),
+    ("reduce_scatter_norm_bf16_rms", r"allreduceNormKernel<__nv_bfloat16, 1, 4, false>"),
+    ("reduce_scatter_norm_f32_layer", r"allreduceNormKernel<float, 2, 4, false>"),
+    ("reduce_scatter_norm_fp8_bf16_rms", r"allreduceNormKernel<__nv_bfloat16, 1, 4, true>"),
+    ("allreduce_norm_fp8_bf16_layer_two_shot", r"allreduceNormKernel<__nv_bfloat16, 2, 2, true>"),
     ("reduce_scatter_norm_backward_bf16_rms", r"normBackwardKernel<__nv_bfloat16, 1, 4>"),
     ("allreduce_norm_backward_bf16_rms_one_shot", r"normBackwardKernel<__nv_bfloat16, 1, 1>"),
     ("allreduce_norm_backward_bf16_rms_two_shot", r"normBackwardKernel<__nv_bfloat16, 1, 2>"),
