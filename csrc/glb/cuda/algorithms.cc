@@ -174,6 +174,7 @@ CudaAllreduceCore::CudaAllreduceCore(std::shared_ptr<Context> ctx, std::vector<v
     chunkEvents_.resize(hostChunks_);
     for (auto& ev : chunkEvents_) GLB_CUDA_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
   }
+  if (!pc_) tiles_ = std::make_unique<TileCounter>(dev0);
 }
 
 CudaAllreduceCore::~CudaAllreduceCore() {
@@ -218,7 +219,7 @@ void CudaAllreduceCore::runHostWorkspace(CudaStream& s0) {
   s0.waitOn(*h2dStream_);
   if (scale_ != 1.0) {
     void* one[1] = {ptrs_[0]};
-    launchLocalAllreduceMany(one, 1, count_, dt_, op_, static_cast<float>(scale_), *s0);
+    launchLocalAllreduceMany(one, 1, count_, dt_, op_, static_cast<float>(scale_), tiles_->get(), *s0);
     noteLaunch();
   }
 }
@@ -257,7 +258,8 @@ void CudaAllreduceCore::run() {
 
   if (fuseLocal_ && ctx_->size == 1) {
     // The whole step in one pass: every buffer := scale * reduce(all buffers).
-    launchLocalAllreduceMany(ptrs_.data(), static_cast<int>(ptrs_.size()), count_, dt_, op_, static_cast<float>(scale_), *s0);
+    launchLocalAllreduceMany(ptrs_.data(), static_cast<int>(ptrs_.size()), count_, dt_, op_, static_cast<float>(scale_),
+                             tiles_->get(), *s0);
     noteLaunch();
   } else if (fuseLocal_) {
     // One launch: fold, exchange and fan-out inside the collective kernel.
@@ -295,7 +297,7 @@ void CudaAllreduceCore::run() {
       }
     } else if (scale_ != 1.0) {
       void* one[1] = {ptrs_[0]};
-      launchLocalAllreduceMany(one, 1, count_, dt_, op_, static_cast<float>(scale_), *s0);
+      launchLocalAllreduceMany(one, 1, count_, dt_, op_, static_cast<float>(scale_), tiles_->get(), *s0);
       noteLaunch();
     }
     // 3. replicate to the other local pointers
@@ -408,6 +410,7 @@ CudaAllreduceLocal<T>::CudaAllreduceLocal(const std::shared_ptr<Context>& contex
                                           const size_t count, const std::vector<cudaStream_t>& streams)
     : Algorithm(context), ptrs_(cuda::eraseType(ptrs)), count_(count), syncOutputs_(streams.empty()) {
   streams_ = cuda::makeStreamsFor(ptrs_, streams);
+  if (!streams_.empty()) tiles_ = std::make_unique<cuda::TileCounter>(streams_[0].getDeviceID());
 }
 
 template <typename T>
@@ -422,7 +425,7 @@ void CudaAllreduceLocal<T>::run() {
   // One pass: every buffer := sum of all buffers (peer buffers of other local GPUs are
   // read and written through peer access).
   cuda::launchLocalAllreduceMany(ptrs_.data(), static_cast<int>(ptrs_.size()), count_, DataTypeOf<T>::value, ReduceOp::SUM,
-                                 1.0f, *s0);
+                                 1.0f, tiles_->get(), *s0);
   cuda::noteLaunch();
   s0.record();
   for (size_t i = 1; i < streams_.size(); i++) streams_[i].waitOn(s0);

@@ -29,6 +29,7 @@
 
 #include "glb/algorithm.h"
 #include "glb/cuda/collectives.h"
+#include "glb/cuda/kernels.h"
 #include "glb/cuda/stream.h"
 
 namespace glb {
@@ -93,6 +94,7 @@ class CudaAllreduceCore {
   std::shared_ptr<PeerBuffer> reg_;
   size_t regOffset_ = 0;
   void* hostScratch_ = nullptr;  // pinned, host workspace only
+  std::unique_ptr<TileCounter> tiles_;  // the local fused step's: single rank or host workspace only
   struct Literal;
   std::unique_ptr<Literal> literal_;
 };
@@ -205,6 +207,7 @@ class CudaAllreduceLocal : public Algorithm {
   size_t count_;
   bool syncOutputs_;
   std::vector<cuda::CudaStream> streams_;
+  std::unique_ptr<cuda::TileCounter> tiles_;
 };
 
 template <typename T, typename W = CudaPeerWorkspace<T>>

@@ -295,8 +295,9 @@ void allreduce(PeerContext& pc, const PeerBuffer& buf, size_t byteOffset, size_t
     if (ep.extra.n > 0 || scale != 1.0f) {
       std::vector<void*> all{local};
       for (int k = 0; k < ep.extra.n; k++) all.push_back(ep.extra.p[k]);
-      launchLocalAllreduceMany(all.data(), static_cast<int>(all.size()), count, dt, op, scale, stream);
-      checkLaunch("allreduce(local)");
+      pc.orderStreams(stream);
+      launchLocalAllreduceMany(all.data(), static_cast<int>(all.size()), count, dt, op, scale, pc.localTileCounter(), stream);
+      finish(pc, stream, "allreduce(local)");
     }
     return;
   }
@@ -399,8 +400,9 @@ void allreduce(PeerContext& pc, const void* in, void* out, size_t count, DataTyp
       if (in != out) GLB_CUDA_CHECK(cudaMemcpyAsync(out, in, bytes, cudaMemcpyDeviceToDevice, stream));
       std::vector<void*> all{out};
       for (int k = 0; k < ep.extra.n; k++) all.push_back(ep.extra.p[k]);
-      launchLocalAllreduceMany(all.data(), static_cast<int>(all.size()), count, dt, op, scale, stream);
-      checkLaunch("allreduce(local)");
+      pc.orderStreams(stream);
+      launchLocalAllreduceMany(all.data(), static_cast<int>(all.size()), count, dt, op, scale, pc.localTileCounter(), stream);
+      finish(pc, stream, "allreduce(local)");
     } else if (in != out) {
       GLB_CUDA_CHECK(cudaMemcpyAsync(out, in, bytes, cudaMemcpyDeviceToDevice, stream));
     }

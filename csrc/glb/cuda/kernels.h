@@ -324,8 +324,23 @@ void launchLocalReduceMany(void* dst, const void* const* srcs, int nsrc, size_t 
                            cudaStream_t stream);
 void launchLocalBroadcast(void* const* dsts, int ndst, const void* src, size_t bytes, cudaStream_t stream);
 // Every buffer := scale * reduce(all buffers) in one pass (fused reduce + broadcast).
+// tileCounter: a device word on the launching device that is zero when the launch runs; the
+// bulk-copy kernel hands out its tiles through it and leaves it zero again. Launches that share
+// a counter must run one after the other on the device (one stream, or ordered by events).
 void launchLocalAllreduceMany(void* const* bufs, int n, size_t count, DataType dt, ReduceOp op, float scale,
-                              cudaStream_t stream);
+                              unsigned int* tileCounter, cudaStream_t stream);
+// Owns a zeroed tile counter for launchLocalAllreduceMany on `device`.
+class TileCounter {
+ public:
+  explicit TileCounter(int device);
+  ~TileCounter();
+  TileCounter(const TileCounter&) = delete;
+  TileCounter& operator=(const TileCounter&) = delete;
+  unsigned int* get() const { return p_; }
+
+ private:
+  unsigned int* p_ = nullptr;
+};
 // Whether launchLocalAllreduceMany runs the TMA bulk-copy kernel for these arguments (at least
 // 1 MB per buffer, every pointer 16-byte aligned, n small enough for its shared-memory stages)
 // rather than the LDG/STG kernel. An explicit setLocalAllreduceShape() overrides it.

@@ -225,6 +225,7 @@ PeerContext::PeerContext(std::shared_ptr<Context> context, int dev, PeerOptions 
   inputStatusDev_ = reinterpret_cast<InputStatus*>(reinterpret_cast<char*>(hostStatusDev_) + 16);
   setTimeout(std::chrono::duration_cast<std::chrono::milliseconds>(context->getTimeout()));
   GLB_CUDA_CHECK(cudaEventCreateWithFlags(&orderEvent_, cudaEventDisableTiming));
+  localTiles_ = std::make_unique<TileCounter>(device);
   hostBarrier();
   GLB_INFO(describe());
 }

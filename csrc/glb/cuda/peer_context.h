@@ -31,6 +31,7 @@
 #include "glb/context.h"
 #include "glb/cuda/cuda_util.h"
 #include "glb/cuda/comm_types.h"
+#include "glb/cuda/kernels.h"
 
 namespace glb {
 namespace cuda {
@@ -142,6 +143,9 @@ class PeerContext : public std::enable_shared_from_this<PeerContext> {
   void orderStreams(cudaStream_t stream);
   // Called right after a collective kernel has been launched on `stream`.
   void markLaunched(cudaStream_t stream);
+  // The tile counter of the single-rank fused step (launchLocalAllreduceMany); its calls are
+  // ordered by orderStreams / markLaunched like the collectives'.
+  unsigned int* localTileCounter() const { return localTiles_->get(); }
 
   // ---- collective calls: every rank, same order ------------------------------------
   std::shared_ptr<PeerBuffer> allocSymmetric(size_t bytes);
@@ -235,6 +239,7 @@ class PeerContext : public std::enable_shared_from_this<PeerContext> {
   cudaStream_t lastStream_ = nullptr;
   bool haveLastStream_ = false;
   cudaEvent_t orderEvent_ = nullptr;
+  std::unique_ptr<TileCounter> localTiles_;
   std::mutex occMu_;
   std::map<std::pair<const void*, size_t>, int> occupancy_;  // (kernel, dynamic smem) -> CTAs per SM
   // cudaIpc mappings are per (peer, allocation): cache them, opening twice is an error.

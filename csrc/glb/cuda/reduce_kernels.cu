@@ -17,6 +17,7 @@
 
 #include "glb/common/utils.h"
 #include "glb/cuda/bulk_copy.cuh"
+#include "glb/cuda/cuda_util.h"
 #include "glb/cuda/device_common.cuh"
 #include "glb/cuda/kernels.h"
 
@@ -114,44 +115,70 @@ localAllreduceManyKernel(DstPtrs bufs, int n, size_t count, DevOp op, float scal
 }
 
 // The same step as a TMA (cp.async.bulk) pipeline. The vector is cut into tiles of
-// kLocalBulkTile bytes, dealt round-robin to a persistent grid (the active window stays
-// contiguous, as with the grid-stride kernel). Each CTA keeps kLocalBulkStages stages of n
-// tiles (one per buffer) in dynamic shared memory: thread 0 loads tile k + stages - 1 of every
-// buffer against one mbarrier while the CTA reduces tile k in shared memory into the buffer-0
-// slot, which thread 0 then stores back to all n buffers as one bulk group. The arithmetic per 16-byte pack is
-// PackTraits<T>'s in the same order as localAllreduceManyKernel, and what is left after the
-// last whole tile goes through the same pack and scalar code, so both kernels give the same
-// bits. All pointers must be 16-byte aligned.
+// kLocalBulkTile bytes for a persistent grid of one CTA per SM. Each CTA keeps kLocalBulkStages
+// stages of n tiles (one per buffer) in dynamic shared memory: thread 0 loads the tile of stage
+// k + stages - 1 from every buffer against one mbarrier while the CTA reduces stage k in shared
+// memory into the buffer-0 slot, which thread 0 then stores back to all n buffers as one bulk
+// group. The arithmetic per 16-byte pack is PackTraits<T>'s in the same order as
+// localAllreduceManyKernel, and what is left after the last whole tile goes through the same
+// pack and scalar code, so both kernels give the same bits. All pointers must be 16-byte aligned.
+//
+// Tiles are dealt on demand, so an SM that runs slower than the others takes fewer of them
+// instead of ending the step last. A CTA's first stages - 1 tiles are blockIdx.x + j * gridDim.x,
+// so the pipeline fills with no atomic on its path; every later one is claimed from `tiles` by
+// thread 0, one stage ahead of its load. A CTA stops at its first claim past the end, so a launch
+// makes exactly (tiles past the static ones) + gridDim.x claims, and the last of them sets
+// *tiles back to zero for the next launch.
 template <typename T>
 __global__ void __launch_bounds__(kLocalThreads)
-localAllreduceManyBulkKernel(DstPtrs bufs, int n, size_t count, DevOp op, float scale) {
+localAllreduceManyBulkKernel(DstPtrs bufs, int n, size_t count, DevOp op, float scale, unsigned int* tiles) {
   using PT = PackTraits<T>;
   constexpr uint32_t tile = kLocalBulkTile;
   constexpr int stages = kLocalBulkStages;
   extern __shared__ __align__(128) char smem[];  // [stages][n][tile]
   __shared__ uint64_t full[stages];
+  __shared__ size_t slot[stages];  // the tile in each stage; ntiles or more: none, the CTA is done
   const size_t ntiles = count * sizeof(T) / tile;
-  const size_t mine = blockIdx.x < ntiles ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+  const size_t firstClaimed = static_cast<size_t>(stages - 1) * gridDim.x;
+  const size_t claims = (ntiles > firstClaimed ? ntiles - firstClaimed : 0) + gridDim.x;
   const size_t stageBytes = static_cast<size_t>(n) * tile;
   if (threadIdx.x == 0) {
     for (int s = 0; s < stages; s++) mbarInit(&full[s], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  auto load = [&](size_t k) {  // thread 0: tile k of this CTA, all n buffers
-    const int s = static_cast<int>(k % stages);
-    const size_t off = (blockIdx.x + k * gridDim.x) * tile;
-    mbarExpectTx(&full[s], static_cast<uint32_t>(stageBytes));
-    for (int b = 0; b < n; b++) bulkLoad(smem + s * stageBytes + b * tile, static_cast<const char*>(bufs.p[b]) + off, tile, &full[s]);
+  auto claimed = [&](unsigned int c) -> size_t {  // thread 0: the tile that ticket c (from atomicAdd) stands for
+    if (c + 1 == claims) *tiles = 0;  // every other claim of this launch has been made
+    return firstClaimed + c;
   };
+  auto load = [&](size_t k, size_t t) {  // thread 0: tile t into stage k % stages; false past the end
+    const int s = static_cast<int>(k % stages);
+    slot[s] = t;
+    if (t >= ntiles) {
+      mbarExpectTx(&full[s], 0);  // completes the phase with no bytes: the waiting threads read `slot` and stop
+      return false;
+    }
+    mbarExpectTx(&full[s], static_cast<uint32_t>(stageBytes));
+    for (int b = 0; b < n; b++) bulkLoad(smem + s * stageBytes + b * tile, static_cast<const char*>(bufs.p[b]) + t * tile, tile, &full[s]);
+    return true;
+  };
+  bool more = true;  // thread 0: no claim has come back past the end yet
   if (threadIdx.x == 0) {
-    for (size_t k = 0; k < mine && k < static_cast<size_t>(stages - 1); k++) load(k);
+    for (int k = 0; more && k < stages - 1; k++) {
+      const size_t t = blockIdx.x + static_cast<size_t>(k) * gridDim.x;
+      more = load(k, t < ntiles ? t : claimed(atomicAdd(tiles, 1u)));
+    }
   }
   const uint32_t packs = tile / 16;
-  for (size_t k = 0; k < mine; k++) {
+  for (size_t k = 0;; k++) {
     const int s = static_cast<int>(k % stages);
     char* st = smem + s * stageBytes;
+    // The ticket for stage k + stages - 1, taken now and first looked at by the refill below, so
+    // that warp 0 does not wait for the atomic: its latency hides behind this stage.
+    const unsigned int ticket = threadIdx.x == 0 && more ? atomicAdd(tiles, 1u) : 0u;
     mbarWait(&full[s], static_cast<uint32_t>(k / stages) & 1u);
+    const size_t t = slot[s];
+    if (t >= ntiles) break;
     for (uint32_t v = threadIdx.x; v < packs; v += blockDim.x) {
       typename PT::AccPack acc = PT::widen(*reinterpret_cast<const Pack16*>(st + v * 16));
       for (int b = 1; b < n; b++) PT::combine(acc, *reinterpret_cast<const Pack16*>(st + b * tile + v * 16), op);
@@ -161,13 +188,12 @@ localAllreduceManyBulkKernel(DstPtrs bufs, int n, size_t count, DevOp op, float 
     fenceProxyAsyncShared();
     __syncthreads();
     if (threadIdx.x == 0) {
-      const size_t off = (blockIdx.x + k * gridDim.x) * tile;
-      for (int b = 0; b < n; b++) bulkStore(static_cast<char*>(bufs.p[b]) + off, st, tile);
+      for (int b = 0; b < n; b++) bulkStore(static_cast<char*>(bufs.p[b]) + t * tile, st, tile);
       bulkCommit();
-      // Refill the stage of tile k - 1 once its stores have read it (tile k's may still run).
-      if (k + stages - 1 < mine) {
+      // Refill the stage of k - 1 once its stores have read it (stage k's may still run).
+      if (more) {
         bulkWaitRead<1>();
-        load(k + stages - 1);
+        more = load(k + stages - 1, claimed(ticket));
       }
     }
   }
@@ -254,10 +280,15 @@ __global__ void spinKernel(long long cycles) {
 //  * Per call with the L2 flushed (p50 of 50): the bulk kernel loses at 256 KB per buffer
 //    (64 K floats 8.4 us against 7.4; the mbarrier set-up and the pipeline fill) and wins from
 //    1 MB (256 K floats 9.2 against 10.6 us, 1 M 13.7 against 18.3, 10 M 64 against 70).
-// On an H100 80GB HBM3 at 700 W (same clock), scripts/bench_local.py: LDG/STG step 0.570 ms
-// (2.81 TB/s), bulk step 0.548 ms (2.92 TB/s), cudaMemcpyAsync D2D 0.536 ms (2.98 TB/s), in-place
-// copy 0.581 (LDG/STG) and 0.565 ms (bulk), read-only 2.86 TB/s, write-only 3.22 TB/s; bench.py's
-// N=1 step 0.547-0.548 ms against 0.569-0.571 ms before the bulk kernel (three runs each).
+// On an H100 80GB HBM3 at 700 W (same clock), scripts/bench_local.py: LDG/STG step 0.574 ms
+// (2.79 TB/s), bulk step 0.537 ms (2.98 TB/s), cudaMemcpyAsync D2D 0.537 ms (2.98 TB/s), in-place
+// copy 0.587 (LDG/STG) and 0.563 ms (bulk), read-only 2.87 TB/s, write-only 3.21 TB/s; bench.py's
+// N=1 step 0.535-0.537 ms (median 0.5355 of six runs).
+//  * Bulk tiles dealt round-robin (a fixed 184 or 185 per CTA) instead of on demand: median 0.549 ms
+//    of six runs alternated with the above (0.548-0.550, one run at 0.556).
+//    Per-CTA %globaltimer at exit, p50 over 100 launches: the slowest CTA ended 8.6 us after the
+//    median one (1.6 % of the step) and the first 110 us before the last; on demand, 1.6 us (0.3 %).
+//    Claiming a tile right before its load instead of a stage ahead was 0.4 % slower.
 struct LocalShape {
   int ctasPerSm = 4;
   int unroll = 1;
@@ -337,8 +368,19 @@ bool localAllreduceUsesBulk(void* const* bufs, int n, size_t count, DataType dt)
   return static_cast<size_t>(kLocalBulkStages) * n * kLocalBulkTile * kLocalBulkCtasPerSm <= static_cast<size_t>(smemOptin);
 }
 
+TileCounter::TileCounter(int device) {
+  DeviceGuard g(device);
+  GLB_CUDA_CHECK(cudaMalloc(&p_, sizeof(*p_)));
+  // Zeroed before the constructor returns: the launches that use it may come on any stream,
+  // including ones that do not synchronise with the legacy default stream.
+  GLB_CUDA_CHECK(cudaMemsetAsync(p_, 0, sizeof(*p_), 0));
+  GLB_CUDA_CHECK(cudaStreamSynchronize(0));
+}
+
+TileCounter::~TileCounter() { cudaFree(p_); }
+
 void launchLocalAllreduceMany(void* const* bufs, int n, size_t count, DataType dt, ReduceOp op, float scale,
-                              cudaStream_t stream) {
+                              unsigned int* tileCounter, cudaStream_t stream) {
   if (count == 0 || n == 0) return;
   DstPtrs bp;
   bool vectorOk = true;
@@ -354,7 +396,7 @@ void launchLocalAllreduceMany(void* const* bufs, int n, size_t count, DataType d
       const auto kernel = localAllreduceManyBulkKernel<T>;
       cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
       const int grid = gridFor(count * sizeof(T) / kLocalBulkTile * kLocalThreads, kLocalThreads, kLocalBulkCtasPerSm);
-      kernel<<<grid, kLocalThreads, smem, stream>>>(bp, n, count, static_cast<DevOp>(op), scale);
+      kernel<<<grid, kLocalThreads, smem, stream>>>(bp, n, count, static_cast<DevOp>(op), scale, tileCounter);
     });
     return;
   }

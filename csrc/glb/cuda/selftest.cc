@@ -1534,7 +1534,8 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
     launchFill(b.p, n, DataType::FLOAT32, 1.0, 3.0, stream);
     launchFill(c.p, n, DataType::FLOAT32, 2.0, 3.0, stream);
     void* all[3] = {a.p, b.p, c.p};
-    launchLocalAllreduceMany(all, 3, n, DataType::FLOAT32, ReduceOp::SUM, 1.0f, stream);
+    TileCounter tiles(pc.device);
+    launchLocalAllreduceMany(all, 3, n, DataType::FLOAT32, ReduceOp::SUM, 1.0f, tiles.get(), stream);
     noteLaunch();
     DevBuf res(16);
     unsigned long long init[2] = {0ull, ~0ull};
@@ -1552,7 +1553,8 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
     launchFill(b.p, m, DataType::FLOAT32, 1.0, 2.0, stream);
     void* all[2] = {a.p, b.p};
     if (!localAllreduceUsesBulk(all, 2, m, DataType::FLOAT32)) return "the size no longer selects the bulk kernel";
-    launchLocalAllreduceMany(all, 2, m, DataType::FLOAT32, ReduceOp::SUM, 0.5f, stream);
+    TileCounter tiles(pc.device);
+    launchLocalAllreduceMany(all, 2, m, DataType::FLOAT32, ReduceOp::SUM, 0.5f, tiles.get(), stream);
     noteLaunch();
     DevBuf res(16);
     unsigned long long init[2] = {0ull, ~0ull};

@@ -484,10 +484,16 @@ void registerCuda(py::module_& root) {
                                    uintptr_t stream) {
     std::vector<void*> ps;
     for (auto b : bufs) ps.push_back(P(b));
+    // A tile counter of this call's own, stream ordered: calls on different streams may overlap.
+    unsigned int* tiles = nullptr;
+    GLB_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&tiles), sizeof(*tiles), S(stream)));
+    GLB_CUDA_CHECK(cudaMemsetAsync(tiles, 0, sizeof(*tiles), S(stream)));
     launchLocalAllreduceMany(ps.data(), static_cast<int>(ps.size()), count, static_cast<DataType>(dtype),
-                             static_cast<ReduceOp>(op), static_cast<float>(scale), S(stream));
+                             static_cast<ReduceOp>(op), static_cast<float>(scale), tiles, S(stream));
     noteLaunch();
-    GLB_CUDA_CHECK(cudaGetLastError());
+    const cudaError_t launched = cudaGetLastError();
+    GLB_CUDA_CHECK(cudaFreeAsync(tiles, S(stream)));
+    GLB_CUDA_CHECK(launched);
   }, py::arg("bufs"), py::arg("count"), py::arg("dtype"), py::arg("op") = 1, py::arg("scale") = 1.0, py::arg("stream") = 0,
      "Every buffer := scale * reduce(all buffers), one kernel, one pass.");
   m.def("local_allreduce_many_uses_bulk", [](std::vector<uintptr_t> bufs, size_t count, int dtype) {

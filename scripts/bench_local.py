@@ -24,9 +24,12 @@ The buffers stay 2 x 400 MB whatever the dtype, so every rate compares directly 
 read_only and write_only run on a float32 view of the same bytes.
 
 On an H100 80GB HBM3 (SXM, power limit 700 W, max SM clock 1980 MHz), medians of 3 rounds:
-fused_ldg_stg 0.570 ms (2.81 TB/s), fused_bulk 0.548 ms (2.92 TB/s), copy_ldg_stg 0.581 ms,
-copy_bulk 0.565 ms, memcpy_d2d 0.536 ms (2.98 TB/s), read_only 2.86 TB/s, write_only 3.22 TB/s.
-The bulk step runs at 0.98 of the device-to-device copy and 1.04 of the LDG/STG step.
+fused_ldg_stg 0.574 ms (2.79 TB/s), fused_bulk 0.537 ms (2.98 TB/s), copy_ldg_stg 0.587 ms,
+copy_bulk 0.563 ms, memcpy_d2d 0.537 ms (2.98 TB/s), read_only 2.87 TB/s, write_only 3.21 TB/s.
+The bulk step runs at 0.999 of the device-to-device copy and 1.07 of the LDG/STG step. Its time
+here includes the stream-ordered allocation and zeroing of the tile counter that each
+local_allreduce_many call makes for itself (bench.py's step, whose counter lives with the
+algorithm object, takes 0.535-0.537 ms).
 """
 import argparse
 import json
