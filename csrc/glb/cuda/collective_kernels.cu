@@ -286,6 +286,54 @@ void launchGatherPush(const CommArgs& a, const void* in, const PeerPtrs& outs, v
                                                     va, onlyDst, vec);
 }
 
+// The cast allgather(v): my block is float32 at `in`; it is rounded to TO (round to nearest even,
+// overflow to +-inf, NaN stays NaN) as it is read, and only TO bytes are pushed. va counts TO
+// elements. `vec`: `in` and every output are 16-byte aligned.
+template <typename TO>
+__global__ void __launch_bounds__(kThreads, 2)
+castGatherPushKernel(CommArgs a, const float* __restrict__ in, PeerPtrs outs, VArgs va, bool vec) {
+  const uint32_t e = loadEpoch(a);
+  const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
+  const int P = a.nranks;
+  if (!blockBarrier<false>(a, e + 1)) {
+    retire(a, 2, 0);
+    return;
+  }
+  const size_t off = va.off[a.rank], len = va.len[a.rank];
+  const size_t nitems = vec && (off * sizeof(TO)) % 16 == 0 ? len / 8 : 0;
+  for (size_t it = tid; it < nitems; it += nthreads) {
+    float v[8];
+    Item8<float>::load(in + it * 8, v);
+    for (int i = 0; i < P; i++) Item8<TO>::store(static_cast<TO*>(outs.p[(a.rank + i) % P]) + off + it * 8, v);
+  }
+  for (size_t i = nitems * 8 + tid; i < len; i += nthreads) {
+    const TO c = Scalar<TO>::fromAcc(in[i]);
+    for (int r = 0; r < P; r++) static_cast<TO*>(outs.p[r])[off + i] = c;
+  }
+  blockBarrier(a, e + 2);
+  retire(a, 2, 0);
+}
+
+namespace {
+VArgs vargs(int nranks, const size_t* offs, const size_t* lens) {
+  VArgs va;
+  for (int i = 0; i < kMaxRanks; i++) {
+    va.off[i] = i < nranks ? offs[i] : 0;
+    va.len[i] = i < nranks ? lens[i] : 0;
+  }
+  return va;
+}
+}  // namespace
+
+void launchCastGatherPush(const CommArgs& a, const void* in, const PeerPtrs& outs, DataType outDt, const size_t* offs,
+                          const size_t* counts, bool vec, int blocks, cudaStream_t stream) {
+  dispatchHalfType(outDt, [&](auto tag) {
+    castGatherPushKernel<decltype(tag)><<<blocks, kThreads, 0, stream>>>(a, static_cast<const float*>(in), outs,
+                                                                          vargs(a.nranks, offs, counts), vec);
+  });
+}
+
 // ---- alltoall(v) / scatter: push chunk j of my input into slot (me) of rank j's output -------
 // sendOff/sendLen index my input per destination; recvOff[r] (same on all ranks by
 // symmetry of the exchange tables) is where MY chunk lands in rank r's output.
@@ -438,6 +486,115 @@ void launchReducePull(const CommArgs& a, const PeerPtrs& ins, void* mcIn, void* 
   });
 }
 
+// The cast reduce_scatter: 16-bit inputs, float32 `out`, SUM. Rank r's share is accumulated in
+// fp32 in peer order, scaled in fp32 and stored as fp32: it is never rounded to 16 bits. No
+// multimem form: multimem.ld_reduce on 16-bit data would return a 16-bit sum.
+template <typename TI, int NR, int UNROLL>
+__global__ void __launch_bounds__(kThreads)
+castReducePullKernel(CommArgs a, PeerPtrs ins, float* __restrict__ out, EArgs ea, float scale, bool vec) {
+  using PT = PackTraits<TI>;
+  const uint32_t e = loadEpoch(a);
+  const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
+  const int P = NR > 0 ? NR : a.nranks;
+  if (!blockBarrier<false>(a, e + 1)) {
+    retire(a, 2, 0);
+    return;
+  }
+  const size_t off = ea.off[a.rank], len = ea.len[a.rank];
+  const bool v16 = vec && (off * sizeof(TI)) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0;
+  const size_t nvec = v16 ? len / PT::kElems : 0;
+  const size_t byteOff = off * sizeof(TI);
+  constexpr int kSlots = NR > 0 ? NR : kMaxRanks;
+  const char* peer[kSlots];
+#pragma unroll
+  for (int i = 0; i < kSlots; i++) {
+    peer[i] = i < P ? static_cast<const char*>(ins.p[(a.rank + i) % P]) + byteOff : nullptr;
+  }
+  reducePeers<TI, kSlots, UNROLL, 0, false>(
+      P, tid, nvec, nthreads, DevOp::SUM, scale, [&](int i) { return peer[i]; },
+      [&](size_t v, const typename PT::AccPack& r) { Item8<float>::store(out + v * PT::kElems, r.v); });
+  for (size_t i = nvec * PT::kElems + tid; i < len; i += nthreads) {
+    float acc = Scalar<TI>::toAcc(static_cast<const TI*>(ins.p[0])[off + i]);
+    for (int r = 1; r < P; r++) acc += Scalar<TI>::toAcc(static_cast<const TI*>(ins.p[r])[off + i]);
+    if (scale != 1.0f) acc *= scale;
+    out[i] = acc;
+  }
+  blockBarrier(a, e + 2);
+  retire(a, 2, 0);
+}
+
+namespace {
+// The cast reduce-pull instantiation for (TI, P).
+template <typename TI>
+auto castReducePullFn(int nranks) {
+  if (nranks == 2) return castReducePullKernel<TI, 2, 4>;
+  if (nranks == 4) return castReducePullKernel<TI, 4, 2>;
+  if (nranks == 8) return castReducePullKernel<TI, 8, 2>;
+  return castReducePullKernel<TI, 0, 1>;
+}
+}  // namespace
+
+void launchCastReducePull(const CommArgs& a, const PeerPtrs& ins, float* out, const size_t* elemOff,
+                          const size_t* elemLen, DataType dt, float scale, bool vec, int blocks, cudaStream_t stream) {
+  EArgs ea;
+  for (int i = 0; i < kMaxRanks; i++) {
+    ea.off[i] = i < a.nranks ? elemOff[i] : 0;
+    ea.len[i] = i < a.nranks ? elemLen[i] : 0;
+  }
+  dispatchHalfType(dt, [&](auto tag) {
+    castReducePullFn<decltype(tag)>(a.nranks)<<<blocks, kThreads, 0, stream>>>(a, ins, out, ea, scale, vec);
+  });
+}
+
+// ---- one rank: out = TO(float(in) * scale) -----------------------------------------------------
+// The P = 1 form of the cast reduce_scatter (16-bit in, float32 out) and allgather (float32 in,
+// 16-bit out): the conversion and the scale of the collective, with nothing to exchange.
+template <typename TI, typename TO>
+__global__ void __launch_bounds__(kThreads)
+castScaleKernel(const TI* __restrict__ in, TO* __restrict__ out, size_t count, float scale, bool vec) {
+  const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
+  const size_t nitems = vec ? count / 8 : 0;
+  for (size_t it = tid; it < nitems; it += nthreads) {
+    float v[8];
+    Item8<TI>::load(in + it * 8, v);
+    if (scale != 1.0f) {
+#pragma unroll
+      for (int k = 0; k < 8; k++) v[k] *= scale;
+    }
+    Item8<TO>::store(out + it * 8, v);
+  }
+  for (size_t i = nitems * 8 + tid; i < count; i += nthreads) {
+    float x = Scalar<TI>::toAcc(in[i]);
+    if (scale != 1.0f) x *= scale;
+    out[i] = Scalar<TO>::fromAcc(x);
+  }
+}
+
+namespace {
+// Calls f(TI{}, TO{}) for the pairs of the cast reduce_scatter and allgather.
+template <typename F>
+void dispatchCastLocal(DataType in, DataType out, F&& f) {
+  if (in == DataType::FLOAT32) {
+    dispatchHalfType(out, [&](auto to) { f(float{}, to); });
+  } else if (out == DataType::FLOAT32) {
+    dispatchHalfType(in, [&](auto ti) { f(ti, float{}); });
+  }
+}
+}  // namespace
+
+void launchCastScale(const void* in, DataType inDt, void* out, DataType outDt, size_t count, float scale, int blocks,
+                     cudaStream_t stream) {
+  const bool vec = (reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) % 16 == 0;
+  dispatchCastLocal(inDt, outDt, [&](auto ti, auto to) {
+    using TI = decltype(ti);
+    using TO = decltype(to);
+    castScaleKernel<TI, TO><<<blocks, kThreads, 0, stream>>>(static_cast<const TI*>(in), static_cast<TO*>(out), count,
+                                                             scale, vec);
+  });
+}
+
 // ---- small allgather / alltoall without a barrier: flag-in-data lines -------------------------
 // Same protocol and pool region as llAllreduceKernel (every rank hears from every peer in a
 // launch, which is what makes two parity halves sufficient). Payload unit: 8 bytes.
@@ -523,6 +680,17 @@ const void* reducePullKernelPtr(DataType dt, int nranks) {
   return k;
 }
 
+const void* castReducePullKernelPtr(DataType dt, int nranks) {
+  const void* k = nullptr;
+  dispatchHalfType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(castReducePullFn<decltype(tag)>(nranks)); });
+  return k;
+}
+const void* castGatherPushKernelPtr(DataType outDt) {
+  const void* k = nullptr;
+  dispatchHalfType(outDt, [&](auto tag) { k = reinterpret_cast<const void*>(castGatherPushKernel<decltype(tag)>); });
+  return k;
+}
+
 void preloadCollectiveKernels() {
   touchKernel(broadcastKernel);
   touchKernel(gatherPushKernel);
@@ -531,6 +699,13 @@ void preloadCollectiveKernels() {
   for (DataType dt : kAllDataTypes) {
     dispatchType(dt, [&](auto tag) {
       for (int P : {0, 2, 4, 8}) touchKernel(reducePullFn<decltype(tag)>(P));
+    });
+    dispatchHalfType(dt, [&](auto tag) {
+      using T = decltype(tag);
+      for (int P : {0, 2, 4, 8}) touchKernel(castReducePullFn<T>(P));
+      touchKernel(castGatherPushKernel<T>);
+      touchKernel(castScaleKernel<T, float>);
+      touchKernel(castScaleKernel<float, T>);
     });
   }
   cudaGetLastError();

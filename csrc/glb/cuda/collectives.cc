@@ -2,6 +2,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <numeric>
 
 #include "glb/common/utils.h"
 #include "glb/cuda/kernels.h"
@@ -1848,6 +1849,180 @@ void reduce_scatter(PeerContext& pc, const void* in, void* out, const std::vecto
   auto st = stagedBulk(pc, off.back() * es, "reduce_scatter");
   if (off.back() > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(st.mine, in, off.back() * es, cudaMemcpyDeviceToDevice, stream));
   reducePullCommon(pc, st.ptrs, st.mc, true, out, counts, dt, op, scale, stream);
+}
+
+// ---- cast reduce_scatter / allgather(v) ---------------------------------------------------------
+
+namespace {
+bool isHalf(DataType t) { return t == DataType::FLOAT16 || t == DataType::BFLOAT16; }
+
+// What every cast call checks before it launches anything, on this rank's arguments: the dtype
+// pair (16-bit -> float32 for reduce_scatter, float32 -> 16-bit for allgather), SUM, one count per
+// rank, and disjoint input and output ranges (in place is impossible across dtypes). inBytes /
+// outBytes are the ranges the call reads and writes here.
+void checkCast(const PeerContext& pc, const char* what, bool reduce, DataType inDt, DataType outDt, ReduceOp op,
+               const std::vector<size_t>& counts, const void* in, size_t inBytes, const void* out, size_t outBytes) {
+  if (reduce ? !(isHalf(inDt) && outDt == DataType::FLOAT32) : !(inDt == DataType::FLOAT32 && isHalf(outDt))) {
+    GLB_THROW(InputException, what, ": the cast form takes ",
+              reduce ? "float16 / bfloat16 input and a float32 output" : "float32 input and a float16 / bfloat16 output",
+              ", got ", dataTypeName(inDt), " -> ", dataTypeName(outDt));
+  }
+  if (reduce && op != ReduceOp::SUM) GLB_THROW(InputException, what, ": the cast form reduces with SUM only");
+  if (static_cast<int>(counts.size()) != pc.size) {
+    GLB_THROW(InputException, what, ": ", counts.size(), " counts for ", pc.size, " ranks");
+  }
+  const uintptr_t i = reinterpret_cast<uintptr_t>(in), o = reinterpret_cast<uintptr_t>(out);
+  if (inBytes > 0 && outBytes > 0 && i < o + outBytes && o < i + inBytes) {
+    GLB_THROW(InputException, what, ": the input and output overlap; a cast cannot run in place");
+  }
+}
+
+size_t total(const std::vector<size_t>& counts) { return std::accumulate(counts.begin(), counts.end(), size_t(0)); }
+
+// One rank: the conversion and the scale, one local launch (none for an empty share).
+void castLocal(PeerContext& pc, const void* in, DataType inDt, void* out, DataType outDt, size_t count, float scale,
+               cudaStream_t stream, const char* what) {
+  if (count == 0) return;
+  pc.orderStreams(stream);
+  launchCastScale(in, inDt, out, outDt, count, scale, blocksFor(pc, ceilDiv(count, size_t(8)), 1, tuning().maxBlocks),
+                  stream);
+  finish(pc, stream, what);
+}
+
+void castReducePull(PeerContext& pc, const PeerPtrs& ins, bool vecIn, void* out, const std::vector<size_t>& counts,
+                    DataType dt, float scale, cudaStream_t stream) {
+  GLB_TRACE_RANGE("glb::cuda::reduce_scatter(cast)");
+  auto off = prefix(counts);
+  const size_t largest = *std::max_element(counts.begin(), counts.end());
+  const int blocks = std::min(blocksFor(pc, largest * elementSize(dt) / 16, 1, tuning().maxBlocks),
+                              pc.coResidentBlocks(castReducePullKernelPtr(dt, pc.size)));
+  prologue(pc, stream);
+  launchCastReducePull(pc.comm(), ins, static_cast<float*>(out), off.data(), counts.data(), dt, scale, vecIn, blocks,
+                       stream);
+  finish(pc, stream, "reduce_scatter(cast)");
+}
+
+void castGatherPush(PeerContext& pc, const void* in, const PeerPtrs& outs, bool vecOut, const std::vector<size_t>& counts,
+                    DataType outDt, cudaStream_t stream) {
+  GLB_TRACE_RANGE("glb::cuda::allgather(cast)");
+  auto off = prefix(counts);
+  const size_t largest = *std::max_element(counts.begin(), counts.end());
+  const bool vec = vecOut && reinterpret_cast<uintptr_t>(in) % 16 == 0;
+  prologue(pc, stream);
+  launchCastGatherPush(pc.comm(), in, outs, outDt, off.data(), counts.data(), vec,
+                       bwBlocks(pc, "allgather", castGatherPushKernelPtr(outDt), largest * elementSize(outDt)), stream);
+  finish(pc, stream, "allgather(cast)");
+}
+}  // namespace
+
+void reduce_scatter(PeerContext& pc, const PeerBuffer& in, size_t inOffset, void* out, const std::vector<size_t>& counts,
+                    DataType dt, DataType outDt, ReduceOp op, cudaStream_t stream, double scale) {
+  if (outDt == dt) {
+    reduce_scatter(pc, in, inOffset, out, counts, dt, op, stream, scale);
+    return;
+  }
+  DeviceGuard g(pc.device);
+  const char* src = static_cast<const char*>(in.local) + inOffset;
+  const size_t n = total(counts), mine = pc.rank < static_cast<int>(counts.size()) ? counts[pc.rank] : 0;
+  checkCast(pc, "reduce_scatter", true, dt, outDt, op, counts, src, n * elementSize(dt), out, mine * sizeof(float));
+  if (inOffset + n * elementSize(dt) > in.bytes) {
+    GLB_THROW(InputException, "reduce_scatter: the input range exceeds the registered buffer");
+  }
+  if (pc.size == 1) {
+    castLocal(pc, src, dt, out, outDt, mine, static_cast<float>(scale), stream, "reduce_scatter(cast, local)");
+    return;
+  }
+  castReducePull(pc, in.ptrsAt(inOffset), in.vectorOk && inOffset % 16 == 0, out, counts, dt, static_cast<float>(scale),
+                 stream);
+}
+
+void reduce_scatter(PeerContext& pc, const void* in, void* out, const std::vector<size_t>& counts, DataType dt,
+                    DataType outDt, ReduceOp op, cudaStream_t stream, double scale) {
+  if (outDt == dt) {
+    reduce_scatter(pc, in, out, counts, dt, op, stream, scale);
+    return;
+  }
+  DeviceGuard g(pc.device);
+  const size_t es = elementSize(dt);
+  const size_t n = total(counts), mine = pc.rank < static_cast<int>(counts.size()) ? counts[pc.rank] : 0;
+  checkCast(pc, "reduce_scatter", true, dt, outDt, op, counts, in, n * es, out, mine * sizeof(float));
+  const float s = static_cast<float>(scale);
+  if (pc.size == 1) {
+    castLocal(pc, in, dt, out, outDt, mine, s, stream, "reduce_scatter(cast, local)");
+    return;
+  }
+  if (exceedsBulk(pc, n * es)) {
+    GLB_TRACE_RANGE("glb::cuda::reduce_scatter(cast, pipelined)");
+    auto off = prefix(counts);
+    const size_t largest = *std::max_element(counts.begin(), counts.end());
+    const PipeShape sh = pipeShape(pc, castPipelinedReduceScatterKernelFor(dt, pc.size), 2, pc.size,
+                                   largest * es * pc.size, 0, 0, 0, "reduce_scatter");
+    prologue(pc, stream);
+    launchCastPipelinedReduceScatter(pc.comm(), in, static_cast<float*>(out), off.data(), counts.data(), dt, s,
+                                     pc.stagePtrs(layoutOf(pc).bulkOff), sh.tile, sh.xthreads, sh.blocks, stream);
+    finish(pc, stream, "reduce_scatter(cast, pipelined)");
+    return;
+  }
+  auto st = stagedBulk(pc, n * es, "reduce_scatter");
+  if (n > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(st.mine, in, n * es, cudaMemcpyDeviceToDevice, stream));
+  castReducePull(pc, st.ptrs, true, out, counts, dt, s, stream);
+}
+
+void allgatherv(PeerContext& pc, const void* in, DataType inDt, const PeerBuffer& out, size_t outOffset,
+                const std::vector<size_t>& counts, DataType outDt, cudaStream_t stream) {
+  const size_t es = elementSize(outDt);
+  if (inDt == outDt) {
+    std::vector<size_t> bytes(counts);
+    for (auto& b : bytes) b *= es;
+    allgatherv(pc, in, out, outOffset, bytes, stream);
+    return;
+  }
+  DeviceGuard g(pc.device);
+  char* dst = static_cast<char*>(out.local) + outOffset;
+  const size_t n = total(counts), mine = pc.rank < static_cast<int>(counts.size()) ? counts[pc.rank] : 0;
+  checkCast(pc, "allgather", false, inDt, outDt, ReduceOp::SUM, counts, in, mine * sizeof(float), dst, n * es);
+  if (outOffset + n * es > out.bytes) {
+    GLB_THROW(InputException, "allgather: the output range exceeds the registered buffer");
+  }
+  if (pc.size == 1) {
+    castLocal(pc, in, inDt, dst, outDt, mine, 1.0f, stream, "allgather(cast, local)");
+    return;
+  }
+  castGatherPush(pc, in, out.ptrsAt(outOffset), out.vectorOk && outOffset % 16 == 0, counts, outDt, stream);
+}
+
+void allgatherv(PeerContext& pc, const void* in, DataType inDt, void* out, const std::vector<size_t>& counts,
+                DataType outDt, cudaStream_t stream) {
+  const size_t es = elementSize(outDt);
+  if (inDt == outDt) {
+    std::vector<size_t> bytes(counts);
+    for (auto& b : bytes) b *= es;
+    allgatherv(pc, in, out, bytes, stream);
+    return;
+  }
+  DeviceGuard g(pc.device);
+  const size_t n = total(counts), mine = pc.rank < static_cast<int>(counts.size()) ? counts[pc.rank] : 0;
+  checkCast(pc, "allgather", false, inDt, outDt, ReduceOp::SUM, counts, in, mine * sizeof(float), out, n * es);
+  if (pc.size == 1) {
+    castLocal(pc, in, inDt, out, outDt, mine, 1.0f, stream, "allgather(cast, local)");
+    return;
+  }
+  if (exceedsBulk(pc, n * es)) {
+    GLB_TRACE_RANGE("glb::cuda::allgather(cast, pipelined)");
+    std::vector<size_t> bytes(counts);
+    for (auto& b : bytes) b *= es;
+    auto off = prefix(bytes);
+    const size_t largest = *std::max_element(bytes.begin(), bytes.end());
+    const PipeShape sh = pipeShape(pc, castPipelinedAllgatherKernelFor(outDt), 2, 1, largest, 0, 0, 0, "allgather");
+    prologue(pc, stream);
+    launchCastPipelinedAllgather(pc.comm(), in, out, outDt, off.data(), bytes.data(), pc.stagePtrs(layoutOf(pc).bulkOff),
+                                 sh.tile, sh.xthreads, sh.blocks, stream);
+    finish(pc, stream, "allgather(cast, pipelined)");
+    return;
+  }
+  auto st = stagedBulk(pc, n * es, "allgather");
+  castGatherPush(pc, in, st.ptrs, true, counts, outDt, stream);
+  if (n > 0) GLB_CUDA_CHECK(cudaMemcpyAsync(out, st.mine, n * es, cudaMemcpyDeviceToDevice, stream));
 }
 
 void reduce(PeerContext& pc, const PeerBuffer& in, size_t inOffset, const PeerBuffer& out, size_t outOffset,

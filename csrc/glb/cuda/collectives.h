@@ -229,6 +229,16 @@ void allgatherv(PeerContext& pc, const void* in, const PeerBuffer& out, size_t o
                 const std::vector<size_t>& bytesPerRank, cudaStream_t stream);
 void allgatherv(PeerContext& pc, const void* in, void* out, const std::vector<size_t>& bytesPerRank,
                 cudaStream_t stream);
+// The cast form (docs/cuda.md, "Cast reduce-scatter / allgather"): rank r's `in` holds counts[r]
+// float32 elements (inDt), and lands in every out as outDt (float16 / bfloat16), rounded once on
+// the sender (to nearest even; overflow to +-inf, NaN stays NaN), so only 16-bit bytes cross
+// NVLink. Counts are in elements; inDt == outDt is the byte form above. Another pair, an `in` that
+// overlaps the output or an output range beyond the registered buffer raises InputException
+// before any launch. Never LL; one launch per call at P > 1 (one local kernel at P = 1).
+void allgatherv(PeerContext& pc, const void* in, DataType inDt, const PeerBuffer& out, size_t outOffset,
+                const std::vector<size_t>& counts, DataType outDt, cudaStream_t stream);
+void allgatherv(PeerContext& pc, const void* in, DataType inDt, void* out, const std::vector<size_t>& counts,
+                DataType outDt, cudaStream_t stream);
 // Only `root` receives.
 void gatherv(PeerContext& pc, const void* in, const PeerBuffer& out, size_t outOffset,
              const std::vector<size_t>& bytesPerRank, int root, cudaStream_t stream);
@@ -365,6 +375,16 @@ void reduce_scatter(PeerContext& pc, const PeerBuffer& in, size_t inOffset, void
                     double scale = 1.0);
 void reduce_scatter(PeerContext& pc, const void* in, void* out, const std::vector<size_t>& counts, DataType dt,
                     ReduceOp op, cudaStream_t stream, double scale = 1.0);
+// The cast form (docs/cuda.md, "Cast reduce-scatter / allgather"): dt float16 / bfloat16, outDt
+// float32, op SUM. out[i] = fp32(sum over ranks of float(in_q[off_r + i])) * fp32(scale): the
+// sum is accumulated in fp32 and never rounded to 16 bits. outDt == dt is the call above. Every
+// path of that call runs (registered, staged, pipelined; one local kernel at P = 1), never LL or
+// NVLS; one launch per call at P > 1. Another pair, another op, an `out` that overlaps the input
+// or an input range beyond the registered buffer raises InputException before any launch.
+void reduce_scatter(PeerContext& pc, const PeerBuffer& in, size_t inOffset, void* out, const std::vector<size_t>& counts,
+                    DataType dt, DataType outDt, ReduceOp op, cudaStream_t stream, double scale = 1.0);
+void reduce_scatter(PeerContext& pc, const void* in, void* out, const std::vector<size_t>& counts, DataType dt,
+                    DataType outDt, ReduceOp op, cudaStream_t stream, double scale = 1.0);
 // Reduction of every rank's `in` delivered to root's `out` (both registered).
 void reduce(PeerContext& pc, const PeerBuffer& in, size_t inOffset, const PeerBuffer& out, size_t outOffset,
             size_t count, DataType dt, ReduceOp op, int root, cudaStream_t stream);

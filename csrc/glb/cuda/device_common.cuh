@@ -691,6 +691,20 @@ void dispatchType(DataType dt, F&& f) {
   }
 }
 
+// Calls f(T{}) when dt is a 16-bit floating type (float16, bfloat16); returns whether it is one.
+// The cast reduce-scatter and allgather take these on their 16-bit side.
+template <typename F>
+bool dispatchHalfType(DataType dt, F&& f) {
+  if (dt == DataType::FLOAT16) {
+    f(__half{});
+  } else if (dt == DataType::BFLOAT16) {
+    f(__nv_bfloat16{});
+  } else {
+    return false;
+  }
+  return true;
+}
+
 constexpr DataType kAllDataTypes[] = {DataType::INT8,    DataType::UINT8,       DataType::INT16,      DataType::INT32,
                                       DataType::UINT32,  DataType::INT64,       DataType::UINT64,     DataType::FLOAT32,
                                       DataType::FLOAT64, DataType::FLOAT16,     DataType::BFLOAT16,   DataType::FLOAT8_E4M3,

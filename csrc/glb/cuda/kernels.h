@@ -163,6 +163,18 @@ const void* pipelinedReduceScatterKernelFor(DataType dt, int nranks);
 void launchPipelinedReduceScatter(const CommArgs& a, const void* in, void* out, const size_t* elemOff,
                                   const size_t* elemLen, DataType dt, ReduceOp op, float scale, const PeerPtrs& stage,
                                   int tileVecs, int exchangeThreads, int blocks, cudaStream_t stream);
+// The cast forms of the two (docs/cuda.md, "Cast reduce-scatter / allgather"). reduce_scatter:
+// 16-bit `in` (dt float16 / bfloat16), float32 `out`, SUM, accumulated, scaled and stored in fp32.
+// allgather(v): float32 `in` rounded to outDt (float16 / bfloat16) in the copy-in stage; offs /
+// lens in outDt bytes, so the slots and the pulls move outDt bytes only.
+const void* castPipelinedReduceScatterKernelFor(DataType dt, int nranks);
+void launchCastPipelinedReduceScatter(const CommArgs& a, const void* in, float* out, const size_t* elemOff,
+                                      const size_t* elemLen, DataType dt, float scale, const PeerPtrs& stage,
+                                      int tileVecs, int exchangeThreads, int blocks, cudaStream_t stream);
+const void* castPipelinedAllgatherKernelFor(DataType outDt);
+void launchCastPipelinedAllgather(const CommArgs& a, const void* in, void* out, DataType outDt, const size_t* offs,
+                                  const size_t* lens, const PeerPtrs& stage, int tileVecs, int exchangeThreads,
+                                  int blocks, cudaStream_t stream);
 // reduce to `root` of plain pointers of any size: `count` elements cut into the shares of
 // reduce_scatter (elemOff / elemLen); only the root writes `out` (null elsewhere is fine).
 const void* pipelinedReduceKernelFor(DataType dt, int nranks);
@@ -189,6 +201,20 @@ void launchAlltoallPush(const CommArgs& a, const void* in, const PeerPtrs& outs,
 void launchReducePull(const CommArgs& a, const PeerPtrs& ins, void* mcIn, void* out, const size_t* elemOff,
                       const size_t* elemLen, DataType dt, ReduceOp op, float scale, bool vec, bool useMc, int blocks,
                       cudaStream_t stream);
+// The cast forms (docs/cuda.md, "Cast reduce-scatter / allgather"). Reduce-pull: 16-bit inputs
+// (dt float16 / bfloat16), SUM, rank r's share accumulated in fp32, scaled and stored as float32
+// to `out`. Gather push: float32 `in`, rounded once to outDt (float16 / bfloat16) on the source;
+// offs / counts in outDt elements; `vec`: `in` and the outputs are 16-byte aligned.
+void launchCastReducePull(const CommArgs& a, const PeerPtrs& ins, float* out, const size_t* elemOff,
+                          const size_t* elemLen, DataType dt, float scale, bool vec, int blocks, cudaStream_t stream);
+void launchCastGatherPush(const CommArgs& a, const void* in, const PeerPtrs& outs, DataType outDt, const size_t* offs,
+                          const size_t* counts, bool vec, int blocks, cudaStream_t stream);
+// One rank's form of both: out = outDt(float(in) * scale) for (float16 / bfloat16 -> float32) and
+// (float32 -> float16 / bfloat16).
+void launchCastScale(const void* in, DataType inDt, void* out, DataType outDt, size_t count, float scale, int blocks,
+                     cudaStream_t stream);
+const void* castReducePullKernelPtr(DataType dt, int nranks);
+const void* castGatherPushKernelPtr(DataType outDt);
 // Entry points, for occupancy queries (every CTA of a collective kernel must be resident).
 const void* broadcastKernelPtr();
 const void* gatherPushKernelPtr();

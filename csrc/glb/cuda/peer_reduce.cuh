@@ -8,13 +8,14 @@ namespace cuda {
 
 // Reduces packs [begin, end) with stride `stride` over P peers: pack o of rotated peer q is at
 // peer(q) + o * 16. Each result is widened to the PackTraits accumulator in peer order, scaled,
-// rounded once and handed to sink(o, pack).
+// rounded once and handed to sink(o, pack). With kNarrow false the scaled accumulator itself
+// (PackTraits<T>::AccPack, fp32 lanes for the 16-bit types) goes to the sink, unrounded.
 //
 // kSlots >= P is the number of peers the code is written for (kMaxRanks for any P). With
 // kBatch == 0 each thread keeps kSlots x U independent 128-bit loads in flight, as many as it can
 // afford (an NVLink round trip is ~2 us); with kBatch > 0 it reduces one pack at a time and loads
 // the peers' packs in batches of kBatch, in the same order, which bounds the registers at any P.
-template <typename T, int kSlots, int U, int kBatch, typename Peer, typename Sink>
+template <typename T, int kSlots, int U, int kBatch, bool kNarrow = true, typename Peer, typename Sink>
 __device__ __forceinline__ void reducePeers(int P, size_t begin, size_t end, size_t stride, DevOp op, float scale,
                                             Peer&& peer, Sink&& sink) {
   using PT = PackTraits<T>;
@@ -38,7 +39,11 @@ __device__ __forceinline__ void reducePeers(int P, size_t begin, size_t end, siz
         }
       }
       if (scale != 1.0f) PT::scale(acc, scale);
-      sink(o, PT::narrow(acc));
+      if constexpr (kNarrow) {
+        sink(o, PT::narrow(acc));
+      } else {
+        sink(o, acc);
+      }
     }
   } else {
     for (size_t o0 = begin; o0 < end; o0 += stride * U) {
@@ -63,7 +68,11 @@ __device__ __forceinline__ void reducePeers(int P, size_t begin, size_t end, siz
             if (q < P) PT::combine(acc, v[u][q], op);
           }
           if (scale != 1.0f) PT::scale(acc, scale);
-          sink(o, PT::narrow(acc));
+          if constexpr (kNarrow) {
+            sink(o, PT::narrow(acc));
+          } else {
+            sink(o, acc);
+          }
         }
       }
     }

@@ -354,12 +354,35 @@ __device__ __forceinline__ size_t largestOf(const PipeBlocks& pb, int P) {
 }
 }  // namespace
 
+// n float32 elements of src rounded to TO (nearest even, overflow to +-inf, NaN stays NaN) at dst
+// and, unless it is null, at dst2; by thread t of a team of nt.
+template <typename TO>
+__device__ __forceinline__ void castCopy(TO* dst, TO* dst2, const float* src, size_t n, int t, int nt) {
+  const uintptr_t all = reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst) |
+                        reinterpret_cast<uintptr_t>(dst2);
+  const size_t items = all % 16 == 0 ? n / 8 : 0;
+  for (size_t it = t; it < items; it += nt) {
+    float v[8];
+    Item8<float>::load(src + it * 8, v);
+    Item8<TO>::store(dst + it * 8, v);
+    if (dst2 != nullptr) Item8<TO>::store(dst2 + it * 8, v);
+  }
+  for (size_t i = items * 8 + t; i < n; i += nt) {
+    const TO c = Scalar<TO>::fromAcc(src[i]);
+    dst[i] = c;
+    if (dst2 != nullptr) dst2[i] = c;
+  }
+}
+
 // Slot: C bytes, my chunk. A(i): my chunk i -> my slot, and to out + off[me] unless `in` already
 // is that address (in place) or I receive nothing (gather, not the root). B(i-1): chunk i-1 of
 // every peer's slot -> out + off[q] (only the root for gather: a non-root never writes its out).
-__global__ void __launch_bounds__(kThreads)
-pipelinedAllgatherKernel(CommArgs a, const char* in, char* out, PipeBlocks pb, int onlyDst, PeerPtrs stage,
-                         int tileVecs, int exchangeThreads) {
+// TO = char copies bytes. TO = __half / __nv_bfloat16 is the cast allgather: `in` holds float32
+// elements, A(i) rounds them to TO as it reads them, and the blocks, the slots and the pulls are
+// in TO bytes, so only TO bytes cross NVLink.
+template <typename TO>
+__device__ __forceinline__ void allgatherPipe(CommArgs& a, const char* in, char* out, const PipeBlocks& pb, int onlyDst,
+                                              const PeerPtrs& stage, int tileVecs, int exchangeThreads) {
   const int P = a.nranks, me = a.rank;
   const size_t tileBytes = static_cast<size_t>(tileVecs) * 16;
   const size_t C = gridDim.x * tileBytes;
@@ -391,14 +414,34 @@ pipelinedAllgatherKernel(CommArgs a, const char* in, char* out, PipeBlocks pb, i
       // ---- A(i): my chunk i -> my slot (and my own block of the output) ----
       const size_t n = tilePart(pb.len[me], i, C, tileBytes);
       if (n > 0) {
-        const char* src = in + i * C + tileOff;
-        gridCopy(myStage + (i % 2) * C + tileOff, src, n, true, ct, cn);
-        if (copyOwn) gridCopy(out + pb.off[me] + i * C + tileOff, src, n, true, ct, cn);
+        if constexpr (std::is_same<TO, char>::value) {
+          const char* src = in + i * C + tileOff;
+          gridCopy(myStage + (i % 2) * C + tileOff, src, n, true, ct, cn);
+          if (copyOwn) gridCopy(out + pb.off[me] + i * C + tileOff, src, n, true, ct, cn);
+        } else {
+          const float* src = reinterpret_cast<const float*>(in) + (i * C + tileOff) / sizeof(TO);
+          castCopy(reinterpret_cast<TO*>(myStage + (i % 2) * C + tileOff),
+                   copyOwn ? reinterpret_cast<TO*>(out + pb.off[me] + i * C + tileOff) : nullptr, src, n / sizeof(TO),
+                   ct, cn);
+        }
       }
     }
     if (!blockBarrier(a, e + static_cast<uint32_t>(i) + 1)) break;
   }
   retire(a, static_cast<uint32_t>(nchunks + 1), 0);
+}
+
+__global__ void __launch_bounds__(kThreads)
+pipelinedAllgatherKernel(CommArgs a, const char* in, char* out, PipeBlocks pb, int onlyDst, PeerPtrs stage,
+                         int tileVecs, int exchangeThreads) {
+  allgatherPipe<char>(a, in, out, pb, onlyDst, stage, tileVecs, exchangeThreads);
+}
+
+template <typename TO>
+__global__ void __launch_bounds__(kThreads)
+castPipelinedAllgatherKernel(CommArgs a, const char* in, char* out, PipeBlocks pb, PeerPtrs stage, int tileVecs,
+                             int exchangeThreads) {
+  allgatherPipe<TO>(a, in, out, pb, -1, stage, tileVecs, exchangeThreads);
 }
 
 // A stage of reduce_scatter and reduce: chunk i of every share of `in` -> sub-slot q of `slot`
@@ -435,10 +478,12 @@ __device__ __forceinline__ void stageShares(const T* in, const PipeBlocks& pb, i
 // accumulator type of PackTraits (fp32 for the 16-bit and FP8 types), scaled, rounded once and
 // stored to out + (i-1)·C. Counts are in elements: a share of `in`, and `out`, may start at an
 // address that is not 16-byte aligned (element-wise loads / stores at their groups).
-template <typename T, int NR>
-__global__ void __launch_bounds__(kThreads)
-pipelinedReduceScatterKernel(CommArgs a, const T* in, T* out, PipeBlocks pb, DevOp op, float scale, PeerPtrs stage,
-                             int tileVecs, int exchangeThreads) {
+// TO = float with a 16-bit T is the cast reduce_scatter: the pool holds T, and the fp32
+// accumulator is stored as it is, never rounded to T.
+template <typename T, int NR, typename TO>
+__device__ __forceinline__ void reduceScatterPipe(CommArgs& a, const T* in, TO* out, const PipeBlocks& pb, DevOp op,
+                                                  float scale, const PeerPtrs& stage, int tileVecs,
+                                                  int exchangeThreads) {
   using PT = PackTraits<T>;
   const int P = NR > 0 ? NR : a.nranks;
   const int me = a.rank;
@@ -463,7 +508,7 @@ pipelinedReduceScatterKernel(CommArgs a, const T* in, T* out, PipeBlocks pb, Dev
       const size_t n = i >= 1 ? tilePart(pb.len[me], c, chunkElems, tileElems) : 0;
       if (n > 0) {
         const size_t ng = (n + PT::kElems - 1) / PT::kElems;
-        T* dst = out + c * chunkElems + blockIdx.x * tileElems;
+        TO* dst = out + c * chunkElems + blockIdx.x * tileElems;
         // Half the packs for 16-lane FP8, as in the allreduce pipeline. U is 6 rather than 8 at
         // P = 2, and any P loads in batches (of 4 for 8-byte lanes): the element-wise output path
         // needs the registers, and this keeps every instantiation free of spills (-Xptxas -v).
@@ -478,8 +523,24 @@ pipelinedReduceScatterKernel(CommArgs a, const T* in, T* out, PipeBlocks pb, Dev
           peer[q] = q < P ? static_cast<const char*>(stage.p[(me + q) % P]) + (c % 2) * slotBytes + me * C + tileOff
                           : nullptr;
         }
-        reducePeers<T, kSlots, U, kBatch>(P, xt, ng, xn, op, scale, [&](int q) { return peer[q]; },
-                                          [&](size_t o, const Pack16& r) { storeGroupP(dst, o, n, outAligned, r); });
+        if constexpr (std::is_same<T, TO>::value) {
+          reducePeers<T, kSlots, U, kBatch>(P, xt, ng, xn, op, scale, [&](int q) { return peer[q]; },
+                                            [&](size_t o, const Pack16& r) { storeGroupP(dst, o, n, outAligned, r); });
+        } else {
+          // group o of T is groups 2o and 2o + 1 of the float32 out
+          static_assert(PT::kElems == 8, "the cast form takes 16-bit inputs");
+          reducePeers<T, kSlots, U, kBatch, false>(
+              P, xt, ng, xn, op, scale, [&](int q) { return peer[q]; }, [&](size_t o, const typename PT::AccPack& r) {
+                Pack16 lo, hi;
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                  lo.w[k] = __float_as_uint(r.v[k]);
+                  hi.w[k] = __float_as_uint(r.v[4 + k]);
+                }
+                storeGroupP(dst, 2 * o, n, outAligned, lo);
+                storeGroupP(dst, 2 * o + 1, n, outAligned, hi);
+              });
+        }
       }
     } else if (i < nchunks) {
       // ---- A(i): chunk i of every share -> my slot (zero past a share's end) ----
@@ -488,6 +549,21 @@ pipelinedReduceScatterKernel(CommArgs a, const T* in, T* out, PipeBlocks pb, Dev
     if (!blockBarrier(a, e + static_cast<uint32_t>(i) + 1)) break;
   }
   retire(a, static_cast<uint32_t>(nchunks + 1), 0);
+}
+
+template <typename T, int NR>
+__global__ void __launch_bounds__(kThreads)
+pipelinedReduceScatterKernel(CommArgs a, const T* in, T* out, PipeBlocks pb, DevOp op, float scale, PeerPtrs stage,
+                             int tileVecs, int exchangeThreads) {
+  reduceScatterPipe<T, NR, T>(a, in, out, pb, op, scale, stage, tileVecs, exchangeThreads);
+}
+
+// The cast reduce_scatter (16-bit TI in, float32 out, SUM) of plain pointers of any size.
+template <typename TI, int NR>
+__global__ void __launch_bounds__(kThreads)
+castPipelinedReduceScatterKernel(CommArgs a, const TI* in, float* out, PipeBlocks pb, float scale, PeerPtrs stage,
+                                 int tileVecs, int exchangeThreads) {
+  reduceScatterPipe<TI, NR, float>(a, in, out, pb, DevOp::SUM, scale, stage, tileVecs, exchangeThreads);
 }
 
 // reduce to `root`: the shares are those of reduce_scatter, with three stages and two more pool
@@ -664,6 +740,15 @@ auto pipeRsFn(int nranks) {
   return pipelinedReduceScatterKernel<T, 0>;
 }
 
+// The cast pipelined reduce_scatter instantiation for (TI, P).
+template <typename TI>
+auto castPipeRsFn(int nranks) {
+  if (nranks == 2) return castPipelinedReduceScatterKernel<TI, 2>;
+  if (nranks == 4) return castPipelinedReduceScatterKernel<TI, 4>;
+  if (nranks == 8) return castPipelinedReduceScatterKernel<TI, 8>;
+  return castPipelinedReduceScatterKernel<TI, 0>;
+}
+
 // The pipelined reduce instantiation for (T, P).
 template <typename T>
 auto pipeReduceFn(int nranks) {
@@ -694,6 +779,18 @@ const void* pipelinedReduceScatterKernelFor(DataType dt, int nranks) {
   return k;
 }
 
+const void* castPipelinedReduceScatterKernelFor(DataType dt, int nranks) {
+  const void* k = nullptr;
+  dispatchHalfType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(castPipeRsFn<decltype(tag)>(nranks)); });
+  return k;
+}
+
+const void* castPipelinedAllgatherKernelFor(DataType outDt) {
+  const void* k = nullptr;
+  dispatchHalfType(outDt, [&](auto tag) { k = reinterpret_cast<const void*>(castPipelinedAllgatherKernel<decltype(tag)>); });
+  return k;
+}
+
 const void* pipelinedReduceKernelFor(DataType dt, int nranks) {
   const void* k = nullptr;
   dispatchType(dt, [&](auto tag) { k = reinterpret_cast<const void*>(pipeReduceFn<decltype(tag)>(nranks)); });
@@ -717,6 +814,27 @@ void launchPipelinedReduceScatter(const CommArgs& a, const void* in, void* out, 
                                                            pipeBlocks(a.nranks, elemOff, elemLen),
                                                            static_cast<DevOp>(op), scale, stage, tileVecs,
                                                            exchangeThreads);
+  });
+}
+
+void launchCastPipelinedAllgather(const CommArgs& a, const void* in, void* out, DataType outDt, const size_t* offs,
+                                  const size_t* lens, const PeerPtrs& stage, int tileVecs, int exchangeThreads,
+                                  int blocks, cudaStream_t stream) {
+  dispatchHalfType(outDt, [&](auto tag) {
+    castPipelinedAllgatherKernel<decltype(tag)><<<blocks, kThreads, 0, stream>>>(
+        a, static_cast<const char*>(in), static_cast<char*>(out), pipeBlocks(a.nranks, offs, lens), stage, tileVecs,
+        exchangeThreads);
+  });
+}
+
+void launchCastPipelinedReduceScatter(const CommArgs& a, const void* in, float* out, const size_t* elemOff,
+                                      const size_t* elemLen, DataType dt, float scale, const PeerPtrs& stage,
+                                      int tileVecs, int exchangeThreads, int blocks, cudaStream_t stream) {
+  dispatchHalfType(dt, [&](auto tag) {
+    using TI = decltype(tag);
+    castPipeRsFn<TI>(a.nranks)<<<blocks, kThreads, 0, stream>>>(a, static_cast<const TI*>(in), out,
+                                                                pipeBlocks(a.nranks, elemOff, elemLen), scale, stage,
+                                                                tileVecs, exchangeThreads);
   });
 }
 
@@ -750,6 +868,12 @@ void preloadPipelineKernels() {
         touchKernel(pipeRsFn<decltype(tag)>(nr));
         touchKernel(pipeReduceFn<decltype(tag)>(nr));
       }
+    });
+  }
+  for (DataType dt : kAllDataTypes) {
+    dispatchHalfType(dt, [](auto tag) {
+      for (int nr : {0, 2, 4, 8}) touchKernel(castPipeRsFn<decltype(tag)>(nr));
+      touchKernel(castPipelinedAllgatherKernel<decltype(tag)>);
     });
   }
   touchKernel(pipelinedAllgatherKernel);

@@ -66,6 +66,13 @@ float bf16ToFloat(uint16_t h) {
   return f;
 }
 
+// Round to nearest even (finite, non-NaN x).
+uint16_t floatToBf16(float x) {
+  uint32_t w;
+  std::memcpy(&w, &x, 4);
+  return static_cast<uint16_t>((w + 0x7fffu + ((w >> 16) & 1u)) >> 16);
+}
+
 // Fused allreduce + residual + norm in loopback: rank 0's partial row i, element j is 1 + i * H + j,
 // the residual 0.5 * (i * H + j), the bias j, gamma 1 + j / H and beta -j / H, all exact in fp32.
 // Every virtual peer's partial is rank 0's (their staging aliases mine), so row i reduces to
@@ -382,6 +389,28 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
       return "";
     });
 
+    // ---- cast reduce-scatter (16-bit in, f32 out): peer 0 holds 256, the others 1, so the share
+    // sums to 256 + P - 1, which fp32 holds and bf16 / f16 (P = 4: 259 needs 9 bits) would round.
+    R.run(strcat_all("castReducePullKernel<", P == 4 ? "f16," : "bf16,", P, ">"), [&]() -> std::string {
+      const DataType dt = P == 4 ? DataType::FLOAT16 : DataType::BFLOAT16;
+      for (int r = 0; r < P; r++) launchFill(pp.p[r], n, dt, r == 0 ? 256.0 : 1.0, 0.0, stream);
+      std::vector<size_t> off(P + 1, 0), len(P, 0);
+      for (int r = 0; r < P; r++) {
+        len[r] = n / P + (static_cast<size_t>(r) < n % P ? 1 : 0);
+        off[r + 1] = off[r] + len[r];
+      }
+      DevBuf out(len[0] * 4);
+      launchCastReducePull(ca, pp, static_cast<float*>(out.p), off.data(), len.data(), dt, 0.5f, true,
+                           std::min(pc.maxBlocks(), 16), stream);
+      noteLaunch();
+      auto h = download(out.p, len[0], stream);
+      const float want = 0.5f * static_cast<float>(256 + P - 1);
+      for (size_t i = 0; i < len[0]; i++) {
+        if (h[i] != want) return strcat_all("element ", i, ": got ", h[i], " want ", want);
+      }
+      return "";
+    });
+
     // ---- cast epilogue (f32 in, bf16 out) -----------------------------------------------------
     R.run(strcat_all("castAllreduceKernel<float,bf16> P=", P), [&]() -> std::string {
       for (int r = 0; r < P; r++) launchFill(pp.p[r], n, DataType::FLOAT32, r % 3, 0.0, stream);  // small exact values
@@ -544,6 +573,25 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
         if (!close(h[i], 7.0 + i)) return strcat_all("element ", i, ": got ", h[i]);
       }
       return h[per] == 0.0f ? "" : "wrote outside my block";
+    });
+    R.run(strcat_all("castGatherPushKernel<bf16> (allgather, f32 in) P=", P), [&]() -> std::string {
+      const size_t per = n / P;
+      std::vector<size_t> off(P), len(P, per);
+      for (int r = 0; r < P; r++) off[r] = r * per;
+      DevBuf in(per * 4);
+      launchFill(in.p, per, DataType::FLOAT32, 7.0, 1.0 / 3.0, stream);  // most need rounding
+      for (int r = 0; r < P; r++) GLB_CUDA_CHECK(cudaMemsetAsync(pp.p[r], 0, n * 2, stream));
+      launchCastGatherPush(ca, in.p, pp, DataType::BFLOAT16, off.data(), len.data(), true,
+                           std::min(2 * pc.maxBlocks(), 32), stream);
+      noteLaunch();
+      auto x = download(in.p, per, stream);
+      std::vector<uint16_t> h(n);
+      GLB_CUDA_CHECK(cudaMemcpyAsync(h.data(), pp.p[P - 1], n * 2, cudaMemcpyDeviceToHost, stream));
+      GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+      for (size_t i = 0; i < per; i++) {
+        if (h[i] != floatToBf16(x[i])) return strcat_all("element ", i, ": got ", bf16ToFloat(h[i]), " for ", x[i]);
+      }
+      return h[per] == 0 ? "" : "wrote outside my block";
     });
     R.run(strcat_all("alltoallPushKernel P=", P), [&]() -> std::string {
       const size_t per = n / P / 4 * 4;
@@ -1352,6 +1400,84 @@ std::vector<SelfTestResult> loopbackSelfTest(PeerContext& pc, cudaStream_t strea
       return "";
     });
   }
+  // The cast forms of the two. Allgather: f32 in, bf16 blocks rounded on the copy-in, every block
+  // rank 0's. Reduce-scatter: share 0 of the bf16 input is 0, 1, 2, ... (bf16-rounded), the fp32
+  // result P x 0.5 x that, exact in fp32 (P = 3 needs more than bf16's 8 bits above 256).
+  for (int P : {2, 8}) {
+    R.run(strcat_all("castPipelinedAllgatherKernel<bf16> P=", P), [&]() -> std::string {
+      const CommArgs ca = pc.loopbackComm(P);
+      const int blocks = std::min(pc.coResidentBlocks(castPipelinedAllgatherKernelFor(DataType::BFLOAT16)), 8), tile = 64;
+      const size_t C = static_cast<size_t>(blocks) * tile * 16;
+      GLB_ENFORCE_LE(2 * C, pc.stageBytes() - 2 * half, "pool too small for the pipelined self-test");
+      const size_t count = (5 * C + 36) / 2;  // five whole chunks and a part that is not a whole 16-byte group
+      std::vector<size_t> offs(P), lens(P, count * 2);
+      for (int r = 0; r < P; r++) offs[r] = r * count * 2;
+      DevBuf in(count * 4), out(P * count * 2);
+      launchFill(in.p, count, DataType::FLOAT32, 1.0, 1.0 / 3.0, stream);
+      GLB_CUDA_CHECK(cudaMemsetAsync(out.p, 0, out.bytes, stream));
+      launchCastPipelinedAllgather(ca, in.p, out.p, DataType::BFLOAT16, offs.data(), lens.data(), aliasedBulk(P), tile,
+                                   256, blocks, stream);
+      noteLaunch();
+      auto x = download(in.p, count, stream);
+      std::vector<uint16_t> h(P * count);
+      GLB_CUDA_CHECK(cudaMemcpyAsync(h.data(), out.p, out.bytes, cudaMemcpyDeviceToHost, stream));
+      GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+      for (int r = 0; r < P; r++) {
+        for (size_t i = 0; i < count; i++) {
+          if (h[r * count + i] != floatToBf16(x[i])) return strcat_all("block ", r, " element ", i, " differs");
+        }
+      }
+      return "";
+    });
+  }
+  for (int P : {2, 8, 3}) {
+    R.run(strcat_all("castPipelinedReduceScatterKernel<bf16,", P == 3 ? 0 : P, "> P=", P), [&]() -> std::string {
+      const CommArgs ca = pc.loopbackComm(P);
+      const void* k = castPipelinedReduceScatterKernelFor(DataType::BFLOAT16, P);
+      const int blocks = std::min(pc.coResidentBlocks(k), 8), tile = 32;
+      const size_t chunkElems = static_cast<size_t>(blocks) * tile * 8;
+      GLB_ENFORCE_LE(2 * P * chunkElems * 2, pc.stageBytes() - 2 * half, "pool too small for the pipelined self-test");
+      std::vector<size_t> counts(P), off(P + 1, 0);
+      for (int r = 0; r < P; r++) {
+        counts[r] = 3 * chunkElems + (P == 2 ? 0 : 7 + 5 * r);
+        off[r + 1] = off[r] + counts[r];
+      }
+      const size_t shift = P == 8 ? 1 : 0;
+      DevBuf in(off[P] * 2), out((counts[0] + shift) * 4);
+      launchFill(in.p, off[P], DataType::BFLOAT16, 0.0, 1.0, stream);
+      GLB_CUDA_CHECK(cudaMemsetAsync(out.p, 0, out.bytes, stream));
+      launchCastPipelinedReduceScatter(ca, in.p, static_cast<float*>(out.p) + shift, off.data(), counts.data(),
+                                       DataType::BFLOAT16, 0.5f, aliasedBulk(P), tile, 256, blocks, stream);
+      noteLaunch();
+      std::vector<uint16_t> x(counts[0]);
+      GLB_CUDA_CHECK(cudaMemcpyAsync(x.data(), in.p, counts[0] * 2, cudaMemcpyDeviceToHost, stream));
+      auto h = download(out.p, counts[0] + shift, stream);
+      for (size_t i = 0; i < counts[0]; i++) {
+        const double want = 0.5 * P * static_cast<double>(bf16ToFloat(x[i]));
+        if (h[i + shift] != want) return strcat_all("element ", i, ": got ", h[i + shift], " want ", want);
+      }
+      return "";
+    });
+  }
+  // One rank's form: f16 -> f32 scaled, and f32 -> bf16.
+  R.run("castScaleKernel<f16,float> / <float,bf16>", [&]() -> std::string {
+    const size_t count = 200 * 8 + 5;
+    DevBuf a(count * 2), b(count * 4), c(count * 2);
+    launchFill(a.p, count, DataType::FLOAT16, -100.0, 0.125, stream);  // exact in f16
+    launchCastScale(a.p, DataType::FLOAT16, b.p, DataType::FLOAT32, count, 3.0f, 16, stream);
+    launchCastScale(b.p, DataType::FLOAT32, c.p, DataType::BFLOAT16, count, 1.0f, 16, stream);
+    noteLaunch(2);
+    auto h = download(b.p, count, stream);
+    std::vector<uint16_t> hc(count);
+    GLB_CUDA_CHECK(cudaMemcpyAsync(hc.data(), c.p, count * 2, cudaMemcpyDeviceToHost, stream));
+    GLB_CUDA_CHECK(cudaStreamSynchronize(stream));
+    for (size_t i = 0; i < count; i++) {
+      const float want = 3.0f * static_cast<float>(-100.0 + 0.125 * static_cast<double>(i));
+      if (h[i] != want) return strcat_all("f32 element ", i, ": got ", h[i], " want ", want);
+      if (hc[i] != floatToBf16(want)) return strcat_all("bf16 element ", i, " differs");
+    }
+    return "";
+  });
   // reduce to root 0 with every virtual rank's slots aliasing mine: rank 0 stores P copies of share 0
   // of its input as its own share, and pulls every other share from "peer q's" result slot, which is
   // its own, which a root never writes: zero, as cleared here. The output starts filled with NaN.

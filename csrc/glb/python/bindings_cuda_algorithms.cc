@@ -160,6 +160,17 @@ void registerCudaAlgorithms(py::module_& m) {
     py::gil_scoped_release nogil;
     allgatherv(pc, P(in), P(out), bytesPerRank, S(st));
   });
+  // The cast form: counts in elements, float32 in, float16 / bfloat16 out.
+  m.def("allgatherv_cast_reg", [](PeerContext& pc, uintptr_t in, int inDtype, const PeerBuffer& out, size_t off,
+                                  std::vector<size_t> counts, int outDtype, uintptr_t st) {
+    py::gil_scoped_release nogil;
+    allgatherv(pc, P(in), static_cast<DataType>(inDtype), out, off, counts, static_cast<DataType>(outDtype), S(st));
+  });
+  m.def("allgatherv_cast", [](PeerContext& pc, uintptr_t in, int inDtype, uintptr_t out, std::vector<size_t> counts,
+                              int outDtype, uintptr_t st) {
+    py::gil_scoped_release nogil;
+    allgatherv(pc, P(in), static_cast<DataType>(inDtype), P(out), counts, static_cast<DataType>(outDtype), S(st));
+  });
   m.def("gatherv_reg", [](PeerContext& pc, uintptr_t in, const PeerBuffer& out, size_t off,
                           std::vector<size_t> bytesPerRank, int root, uintptr_t st) {
     py::gil_scoped_release nogil;
@@ -300,18 +311,21 @@ void registerCudaAlgorithms(py::module_& m) {
     py::gil_scoped_release nogil;
     scatter(pc, P(in), P(out), bytes, root, S(st));
   });
+  // out_dtype (-1: dtype) other than dtype: the cast form, float16 / bfloat16 in, float32 out
   m.def("reduce_scatter_reg", [](PeerContext& pc, const PeerBuffer& in, size_t off, uintptr_t out,
-                                 std::vector<size_t> counts, int dtype, int op, uintptr_t st, double scale) {
+                                 std::vector<size_t> counts, int dtype, int op, uintptr_t st, double scale, int outDtype) {
     py::gil_scoped_release nogil;
-    reduce_scatter(pc, in, off, P(out), counts, static_cast<DataType>(dtype), static_cast<ReduceOp>(op), S(st), scale);
+    reduce_scatter(pc, in, off, P(out), counts, static_cast<DataType>(dtype),
+                   static_cast<DataType>(outDtype < 0 ? dtype : outDtype), static_cast<ReduceOp>(op), S(st), scale);
   }, py::arg("pc"), py::arg("input"), py::arg("offset"), py::arg("output"), py::arg("counts"), py::arg("dtype"),
-     py::arg("op") = 1, py::arg("stream") = 0, py::arg("scale") = 1.0);
+     py::arg("op") = 1, py::arg("stream") = 0, py::arg("scale") = 1.0, py::arg("out_dtype") = -1);
   m.def("reduce_scatter", [](PeerContext& pc, uintptr_t in, uintptr_t out, std::vector<size_t> counts, int dtype,
-                             int op, uintptr_t st, double scale) {
+                             int op, uintptr_t st, double scale, int outDtype) {
     py::gil_scoped_release nogil;
-    reduce_scatter(pc, P(in), P(out), counts, static_cast<DataType>(dtype), static_cast<ReduceOp>(op), S(st), scale);
+    reduce_scatter(pc, P(in), P(out), counts, static_cast<DataType>(dtype),
+                   static_cast<DataType>(outDtype < 0 ? dtype : outDtype), static_cast<ReduceOp>(op), S(st), scale);
   }, py::arg("pc"), py::arg("input"), py::arg("output"), py::arg("counts"), py::arg("dtype"), py::arg("op") = 1,
-     py::arg("stream") = 0, py::arg("scale") = 1.0);
+     py::arg("stream") = 0, py::arg("scale") = 1.0, py::arg("out_dtype") = -1);
   m.def("reduce_reg", [](PeerContext& pc, const PeerBuffer& in, size_t inOff, const PeerBuffer& out, size_t outOff,
                          size_t count, int dtype, int op, int root, uintptr_t st) {
     py::gil_scoped_release nogil;

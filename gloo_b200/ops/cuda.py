@@ -580,15 +580,31 @@ class CudaContext:
     def allgather(self, output, input, stream=None):
         """Every rank's ``input`` (same size on all ranks), concatenated in rank order. Any size:
         a plain ``output`` larger than the staging pool streams through it in one kernel; ``input``
-        may be this rank's slice of ``output`` (in place)."""
+        may be this rank's slice of ``output`` (in place). A float32 ``input`` and a bfloat16 /
+        float16 ``output`` take the cast form (see :meth:`allgatherv`)."""
         return self.allgatherv(output, input, [input.numel()] * self.size, stream)
 
     def allgatherv(self, output, input, counts: Sequence[int], stream=None):
-        """Like :meth:`allgather` with ``counts[r]`` elements from rank r (zero allowed); any size."""
-        es = output.element_size()
-        sizes = [int(c) * es for c in counts]
+        """Like :meth:`allgather` with ``counts[r]`` elements from rank r (zero allowed); any size.
+
+        When ``output.dtype != input.dtype`` this is the cast form: a float32 ``input`` and a
+        bfloat16 / float16 ``output``. Each rank rounds its block once to the output dtype as it
+        reads it (round to nearest even, overflow to +-inf, NaN stays NaN: ``input.to(dtype)``),
+        so only 16-bit bytes cross NVLink and every rank gets the same bytes, one kernel launch.
+        ``input`` must not overlap ``output``. Other pairs raise ``ValueError``."""
         buf, off = self.lookup(output)
         iptr = input.data_ptr() if input is not None else 0
+        if input is not None and input.dtype != output.dtype:
+            _, _, idt, _ = describe(input)
+            _, _, odt, _ = describe(output)
+            counts = [int(c) for c in counts]
+            if buf is not None:
+                _cu.allgatherv_cast_reg(self.pc, iptr, int(idt), buf, off, counts, int(odt), _stream(stream))
+            else:
+                _cu.allgatherv_cast(self.pc, iptr, int(idt), output.data_ptr(), counts, int(odt), _stream(stream))
+            return output
+        es = output.element_size()
+        sizes = [int(c) * es for c in counts]
         if buf is not None:
             _cu.allgatherv_reg(self.pc, iptr, buf, off, sizes, _stream(stream))
         else:
@@ -1156,16 +1172,26 @@ class CudaContext:
         """``output`` := share ``rank`` of the reduction of every rank's ``input`` (``counts[r]``
         elements for rank r, an even split by default), times ``scale`` (floating types), with one
         rounding. Any size: a plain ``input`` larger than the staging pool streams through it in one
-        kernel; ``output`` may be this rank's share of ``input`` (in place)."""
+        kernel; ``output`` may be this rank's share of ``input`` (in place).
+
+        When ``output.dtype != input.dtype`` this is the cast form: a bfloat16 / float16 ``input``, a
+        float32 ``output`` and ``op`` SUM. ``output[i] = fp32(sum over ranks of float(input[off + i]))
+        * fp32(scale)``: the sum is accumulated in fp32 and never rounded to 16 bits, so ``output``
+        holds exactly what an fp32 reduction of the upcast inputs gives, while only 16-bit bytes
+        cross NVLink. One kernel launch; ``output`` must not overlap ``input``. Other pairs or ops
+        raise ``ValueError``."""
         ptr, n, dt, _ = describe(input)
+        odt = int(describe(output)[2]) if output.dtype != input.dtype else -1
         if counts is None:
             base, rem = divmod(n, self.size)
             counts = [base + (1 if r < rem else 0) for r in range(self.size)]
         buf, off = self.lookup(input)
         if buf is not None:
-            _cu.reduce_scatter_reg(self.pc, buf, off, output.data_ptr(), list(counts), int(dt), int(op), _stream(stream), scale)
+            _cu.reduce_scatter_reg(self.pc, buf, off, output.data_ptr(), list(counts), int(dt), int(op), _stream(stream), scale,
+                                   odt)
         else:
-            _cu.reduce_scatter(self.pc, ptr, output.data_ptr(), list(counts), int(dt), int(op), _stream(stream), scale)
+            _cu.reduce_scatter(self.pc, ptr, output.data_ptr(), list(counts), int(dt), int(op), _stream(stream), scale,
+                               odt)
         return output
 
     def reduce(self, output, input, root: int = 0, op: ReduceOp = ReduceOp.SUM, stream=None):

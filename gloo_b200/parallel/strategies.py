@@ -329,12 +329,20 @@ class ZeroShard(_Base):
         return start, counts[self.rank], counts
 
     def reduce_scatter_gradients(self, flat_grad, out_shard, average: bool = True):
+        """This rank's shard of the sum (or with ``average`` the mean) of every rank's ``flat_grad``.
+        A float32 ``out_shard`` of a bfloat16 / float16 ``flat_grad`` is the cast form: the sum is
+        accumulated in fp32 and the 1/P applied in fp32, never rounded to 16 bits."""
         _, _, counts = self.shard_range(flat_grad.numel())
         if _is_cuda(flat_grad):
             fused = average and flat_grad.is_floating_point()
             self.cc.reduce_scatter(out_shard, flat_grad, counts, scale=1.0 / self.size if fused else 1.0)
             if average and not fused:
                 out_shard.div_(self.size)
+        elif out_shard.dtype != flat_grad.dtype:
+            # the cast form on host tensors: an fp32 reduction of the upcast gradients, times fp32(1/P)
+            H.reduce_scatter(self.ctx, out_shard, flat_grad.to(out_shard.dtype), counts)
+            if average:
+                out_shard.mul_(1.0 / self.size)
         else:
             H.reduce_scatter(self.ctx, out_shard, flat_grad, counts)
             if average:
@@ -342,11 +350,13 @@ class ZeroShard(_Base):
         return out_shard
 
     def allgather_parameters(self, flat_param, shard):
+        """Every rank's ``shard`` into ``flat_param``. A float32 ``shard`` of a bfloat16 / float16
+        ``flat_param`` is rounded once to the parameter dtype on its own rank."""
         _, _, counts = self.shard_range(flat_param.numel())
         if _is_cuda(flat_param):
             self.cc.allgatherv(flat_param, shard, counts)
         else:
-            H.allgatherv(self.ctx, flat_param, counts, shard)
+            H.allgatherv(self.ctx, flat_param, counts, shard.to(flat_param.dtype))
         return flat_param
 
 
@@ -361,17 +371,30 @@ class ZeroOptimizer(_Base):
 
         zo = ZeroOptimizer(ctx, cuda_ctx, model.parameters(), torch.optim.AdamW, lr=1e-3)
         loss.backward(); zo.step(); zo.zero_grad()
+
+    ``master_dtype=torch.float32`` with bfloat16 / float16 parameters keeps fp32 master weights: the
+    optimizer owns an fp32 copy of this rank's shard (initialised from the parameters), the flat
+    buffers stay in the parameter dtype, and ``step()`` runs the cast reduce-scatter of the 16-bit
+    gradients into the fp32 shard gradient (fp32 accumulation, the 1/P fused, no 16-bit rounding),
+    the optimizer on the fp32 shard, and the cast allgather that rounds each master shard once to
+    the parameter dtype. Without it a 16-bit optimizer shard drops every update smaller than half a
+    16-bit step of the weight. With float32 parameters, or ``master_dtype=None``, nothing changes.
     """
 
-    def __init__(self, ctx, cuda_ctx, params: Iterable, optimizer_cls, average: bool = True, **optimizer_kwargs):
+    def __init__(self, ctx, cuda_ctx, params: Iterable, optimizer_cls, average: bool = True, master_dtype=None,
+                 **optimizer_kwargs):
         import torch
 
         super().__init__(ctx, cuda_ctx)
+        if master_dtype not in (None, torch.float32):
+            raise ValueError(f"ZeroOptimizer: master_dtype must be None or torch.float32, got {master_dtype}")
         self.average = average
         self.params = [p for p in params if p.requires_grad]
         assert self.params, "no trainable parameters"
         dtype, device = self.params[0].dtype, self.params[0].device
         assert all(p.dtype == dtype and p.device == device for p in self.params), "one dtype / device per ZeroOptimizer"
+        # fp32 master weights: only 16-bit parameters have anything to gain
+        self.master = master_dtype is not None and dtype in (torch.bfloat16, torch.float16)
         cuda = device.type == "cuda"
         align = max(1, 16 // self.params[0].element_size())
         offs, n = [], 0
@@ -394,8 +417,9 @@ class ZeroOptimizer(_Base):
         self.start = self.rank * (n // self.size)
         cnt = self.counts[self.rank]
         # the shard the optimizer owns: its own tensors (the collectives' inputs / outputs must not
-        # alias the flat buffers they gather into / scatter from)
-        self.shard = torch.nn.Parameter(self.flat_param[self.start:self.start + cnt].detach().clone())
+        # alias the flat buffers they gather into / scatter from); in master mode the fp32 upcast
+        mine = self.flat_param[self.start:self.start + cnt].detach()
+        self.shard = torch.nn.Parameter(mine.float() if self.master else mine.clone())
         self.shard.grad = torch.zeros_like(self.shard)
         self.optimizer = optimizer_cls([self.shard], **optimizer_kwargs)
 
@@ -421,11 +445,13 @@ class ZeroOptimizer(_Base):
                 p.grad = v
 
     def state_bytes(self) -> int:
-        """Bytes of optimizer state held by this rank (for the 1/P claim)."""
+        """Bytes of optimizer state held by this rank (for the 1/P claim), the fp32 master shard
+        included in master mode."""
         import torch
 
-        return sum(v.numel() * v.element_size() for st in self.optimizer.state.values() for v in st.values()
-                   if isinstance(v, torch.Tensor))
+        master = self.shard.numel() * self.shard.element_size() if self.master else 0
+        return master + sum(v.numel() * v.element_size() for st in self.optimizer.state.values() for v in st.values()
+                            if isinstance(v, torch.Tensor))
 
 
 class TensorParallel(_Base):
